@@ -11,7 +11,9 @@
 #include <stdint.h>
 #include <stdio.h>
 
+#include <algorithm>
 #include <map>
+#include <memory>
 #include <mutex>
 #include <string>
 #include <utility>
@@ -33,24 +35,106 @@ std::string &last_error_ref();
     }                                                                                                 \
   } while (0)
 
-// same, running `cleanup` (e.g. destroying a half-built handle) before returning
-#define B2S_CUDA_CHECK_CLEAN(cleanup, expr)                                                            \
-  do {                                                                                                \
-    cudaError_t _e = (expr);                                                                          \
-    if (_e != cudaSuccess) {                                                                          \
-      const std::string _why = std::string(#expr) + " failed: " + cudaGetErrorString(_e) + " (" +      \
-                               __FILE__ + ":" + std::to_string(__LINE__) + ")";                       \
-      cleanup;                                                                                        \
-      ::b2s::set_last_error(_why);                                                                    \
-      return B2S_ERR_CUDA;                                                                            \
-    }                                                                                                 \
-  } while (0)
-
 #define B2S_FAIL(code, msg)        \
   do {                             \
     ::b2s::set_last_error(msg);    \
     return (code);                 \
   } while (0)
+
+// ---- owners of the library's CUDA resources.  Every allocation, stream and event a handle or a call makes is held by
+// one of these, so error paths release what they made by returning.  Destructors ignore CUDA return codes and never
+// write the last-error text: the error already recorded is the one to report.
+
+// device memory (cudaMalloc), or pinned host memory (cudaHostAlloc) when HOST.  reserve(n) grows only: the contents are
+// discarded and at least one element is allocated.  With cudaHostAllocMapped, `dev` is the device alias of the memory.
+template <class T, bool HOST = false>
+struct Buf {
+  T *p = nullptr, *dev = nullptr;
+  size_t cap = 0;
+  Buf() = default;
+  Buf &operator=(Buf &&o) noexcept {  // a swap: the old memory goes with `o`
+    std::swap(p, o.p);
+    std::swap(dev, o.dev);
+    std::swap(cap, o.cap);
+    return *this;
+  }
+  ~Buf() { reset(); }
+  operator T *() const { return p; }
+  cudaError_t reset() {
+    T *q = p;
+    p = dev = nullptr;
+    cap = 0;
+    return !q ? cudaSuccess : HOST ? cudaFreeHost((void *)q) : cudaFree((void *)q);
+  }
+  cudaError_t reserve(size_t n, unsigned host_flags = cudaHostAllocDefault) {
+    n = std::max<size_t>(n, 1);
+    if (p && n <= cap) return cudaSuccess;
+    if (cudaError_t e = reset()) return e;
+    void *q = nullptr;
+    cudaError_t e = HOST ? cudaHostAlloc(&q, n * sizeof(T), host_flags) : cudaMalloc(&q, n * sizeof(T));
+    if (e != cudaSuccess) return e;
+    p = static_cast<T *>(q);
+    cap = n;
+    if (host_flags & cudaHostAllocMapped) {
+      void *d = nullptr;
+      if ((e = cudaHostGetDevicePointer(&d, q, 0)) != cudaSuccess) return e;
+      dev = static_cast<T *>(d);
+    }
+    return cudaSuccess;
+  }
+};
+template <class T>
+using HostBuf = Buf<T, true>;
+
+// stream-ordered memory of one call: cudaMallocAsync, and cudaFreeAsync on the same stream at scope exit
+template <class T>
+struct AsyncBuf {
+  T *p = nullptr;
+  cudaStream_t s;
+  explicit AsyncBuf(cudaStream_t stream) : s(stream) {}
+  AsyncBuf(const AsyncBuf &) = delete;
+  AsyncBuf &operator=(const AsyncBuf &) = delete;
+  ~AsyncBuf() {
+    if (p) cudaFreeAsync(p, s);
+  }
+  operator T *() const { return p; }
+  cudaError_t alloc(size_t n) { return cudaMallocAsync(reinterpret_cast<void **>(&p), n * sizeof(T), s); }
+};
+
+struct Event {
+  cudaEvent_t e = nullptr;
+  Event() = default;
+  Event(const Event &) = delete;
+  Event &operator=(const Event &) = delete;
+  ~Event() {
+    if (e) cudaEventDestroy(e);
+  }
+  operator cudaEvent_t() const { return e; }
+  cudaError_t create(unsigned flags = cudaEventDefault) { return cudaEventCreateWithFlags(&e, flags); }
+};
+
+// the caller's stream, borrowed; or, when the caller passes none, a non-blocking stream created and destroyed here.
+// Handles declare it first, so that it is destroyed after everything else they own.
+struct Stream {
+  cudaStream_t s = nullptr;
+  bool owned = false;
+  Stream() = default;
+  Stream(const Stream &) = delete;
+  Stream &operator=(const Stream &) = delete;
+  ~Stream() {
+    if (owned) cudaStreamDestroy(s);
+  }
+  operator cudaStream_t() const { return s; }
+  cudaError_t init(void *borrowed) {
+    if (borrowed) {
+      s = reinterpret_cast<cudaStream_t>(borrowed);
+      return cudaSuccess;
+    }
+    const cudaError_t e = cudaStreamCreateWithFlags(&s, cudaStreamNonBlocking);
+    owned = e == cudaSuccess;
+    return e;
+  }
+};
 
 constexpr double KT_PI = 3.14159265358979323846;   // Math.h:32
 constexpr double KT_2PI = 6.28318530717958647692;  // Math.h:33
@@ -148,11 +232,6 @@ __host__ __device__ inline void sensor_pose_of(const double robot[3], const doub
   out[2] = normalize_angle(offset[2] + th);
 }
 
-struct StreamRef {
-  cudaStream_t s = nullptr;
-  bool owned = false;
-};
-
 // cudaFuncAttributeMaxDynamicSharedMemorySize is one value per (kernel, device), shared by every handle of the process.
 // Handles of different sizes used from different threads must therefore never LOWER it between another thread's set
 // and launch: keep a process-wide running maximum per (kernel, device) and only ever raise the attribute.
@@ -186,6 +265,19 @@ inline void keep_pool_memory(int device) {
   }
   cudaGetLastError();
   done[device] = true;
+}
+
+inline b2s_status check_device(int device) {
+  if (b2s_device_count() <= device) B2S_FAIL(B2S_ERR_NO_DEVICE, "no usable CUDA device (the product path has no CPU fallback)");
+  return B2S_OK;
+}
+
+// prologue of every entry point that creates device state
+inline b2s_status open_device(int device) {
+  if (b2s_status st = check_device(device)) return st;
+  B2S_CUDA_CHECK(cudaSetDevice(device));
+  keep_pool_memory(device);
+  return B2S_OK;
 }
 
 // NVTX range around a host entry point (SURVEY.md §5 tracing): shows up as "b2s:<name>" in Nsight timelines; nvtx3 is

@@ -24,18 +24,16 @@
 using namespace b2s;
 
 struct b2s_gmap {
+  Stream stream;
   int device = 0;
-  cudaStream_t stream = nullptr;
-  bool own_stream = false;
   double cx = 0, cy = 0, delta = 0, xmin = 0, ymin = 0, xmax = 0, ymax = 0;
   int msx = 0, msy = 0, sx2 = 0, sy2 = 0;
-  int32_t *d_n = nullptr, *d_visits = nullptr;
-  float *d_accx = nullptr, *d_accy = nullptr;
-  int *d_flag = nullptr;
-  double *d_in = nullptr;   // [2][in_cap]: ranges, angles of the current scan
-  int in_cap = 0;
-  double *h_in = nullptr;   // pinned staging of the same
-  int *h_flag = nullptr;    // pinned
+  Buf<int32_t> d_n, d_visits;
+  Buf<float> d_accx, d_accy;
+  Buf<int> d_flag;
+  Buf<double> d_in;     // [2][capacity]: ranges, angles of the current scan
+  HostBuf<double> h_in;  // pinned staging of the same
+  HostBuf<int> h_flag;
 };
 
 namespace b2s {
@@ -137,10 +135,8 @@ b2s_status b2s_gmap_create(double center_x, double center_y, double xmin, double
                            double delta, int device, void *cuda_stream, b2s_gmap **out) {
   if (!out || !(delta > 0) || !(xmax > xmin) || !(ymax > ymin)) B2S_FAIL(B2S_ERR_BAD_PARAMS, "b2s_gmap_create: bad map bounds");
   *out = nullptr;
-  if (b2s_device_count() <= device) B2S_FAIL(B2S_ERR_NO_DEVICE, "no usable CUDA device (the product path has no CPU fallback)");
-  B2S_CUDA_CHECK(cudaSetDevice(device));
-  keep_pool_memory(device);
-  b2s_gmap *g = new (std::nothrow) b2s_gmap();
+  if (b2s_status st = open_device(device)) return st;
+  std::unique_ptr<b2s_gmap, decltype(&b2s_gmap_destroy)> g(new (std::nothrow) b2s_gmap(), b2s_gmap_destroy);
   if (!g) B2S_FAIL(B2S_ERR_CUDA, "out of host memory");
   g->device = device;
   g->cx = center_x; g->cy = center_y; g->delta = delta;
@@ -150,38 +146,25 @@ b2s_status b2s_gmap_create(double center_x, double center_y, double xmin, double
   g->msy = (ys >> 5) << 5;
   g->sx2 = (int)round((center_x - xmin) / delta);  // map.h:139-140
   g->sy2 = (int)round((center_y - ymin) / delta);
-  if (g->msx <= 0 || g->msy <= 0) {
-    delete g;
-    B2S_FAIL(B2S_ERR_BAD_PARAMS, "map smaller than one 32-cell patch");
-  }
-  if (cuda_stream) {
-    g->stream = reinterpret_cast<cudaStream_t>(cuda_stream);
-  } else {
-    B2S_CUDA_CHECK_CLEAN(b2s_gmap_destroy(g), cudaStreamCreateWithFlags(&g->stream, cudaStreamNonBlocking));
-    g->own_stream = true;
-  }
+  if (g->msx <= 0 || g->msy <= 0) B2S_FAIL(B2S_ERR_BAD_PARAMS, "map smaller than one 32-cell patch");
+  B2S_CUDA_CHECK(g->stream.init(cuda_stream));
   const size_t cells = (size_t)g->msx * g->msy;
-  B2S_CUDA_CHECK_CLEAN(b2s_gmap_destroy(g), cudaMalloc(reinterpret_cast<void **>(&g->d_n), cells * 4));
-  B2S_CUDA_CHECK_CLEAN(b2s_gmap_destroy(g), cudaMalloc(reinterpret_cast<void **>(&g->d_visits), cells * 4));
-  B2S_CUDA_CHECK_CLEAN(b2s_gmap_destroy(g), cudaMalloc(reinterpret_cast<void **>(&g->d_accx), cells * 4));
-  B2S_CUDA_CHECK_CLEAN(b2s_gmap_destroy(g), cudaMalloc(reinterpret_cast<void **>(&g->d_accy), cells * 4));
-  B2S_CUDA_CHECK_CLEAN(b2s_gmap_destroy(g), cudaMalloc(reinterpret_cast<void **>(&g->d_flag), sizeof(int)));
+  B2S_CUDA_CHECK(g->d_n.reserve(cells));
+  B2S_CUDA_CHECK(g->d_visits.reserve(cells));
+  B2S_CUDA_CHECK(g->d_accx.reserve(cells));
+  B2S_CUDA_CHECK(g->d_accy.reserve(cells));
+  B2S_CUDA_CHECK(g->d_flag.reserve(1));
   for (void *p : {(void *)g->d_n, (void *)g->d_visits, (void *)g->d_accx, (void *)g->d_accy})
-    B2S_CUDA_CHECK_CLEAN(b2s_gmap_destroy(g), cudaMemsetAsync(p, 0, cells * 4, g->stream));
-  B2S_CUDA_CHECK_CLEAN(b2s_gmap_destroy(g), cudaStreamSynchronize(g->stream));
-  *out = g;
+    B2S_CUDA_CHECK(cudaMemsetAsync(p, 0, cells * 4, g->stream));
+  B2S_CUDA_CHECK(cudaStreamSynchronize(g->stream));
+  *out = g.release();
   return B2S_OK;
 }
 
 void b2s_gmap_destroy(b2s_gmap *g) {
   if (!g) return;
   cudaSetDevice(g->device);
-  if (g->stream) cudaStreamSynchronize(g->stream);
-  for (void *p : {(void *)g->d_n, (void *)g->d_visits, (void *)g->d_accx, (void *)g->d_accy, (void *)g->d_flag, (void *)g->d_in})
-    if (p) cudaFree(p);
-  if (g->h_in) cudaFreeHost(g->h_in);
-  if (g->h_flag) cudaFreeHost(g->h_flag);
-  if (g->own_stream && g->stream) cudaStreamDestroy(g->stream);
+  cudaStreamSynchronize(g->stream);
   delete g;
 }
 
@@ -202,16 +185,10 @@ b2s_status b2s_gmap_compute_map(b2s_gmap *g, const double *ranges, const double 
   const double lx = laser_pose[0], ly = laser_pose[1];  // ComputeMap uses lp = (x, y, 0): beam angles are absolute
   const int p0x = cast_i32(round((lx - g->cx) / g->delta)) + g->sx2, p0y = cast_i32(round((ly - g->cy) / g->delta)) + g->sy2;
   if (p0x < 0 || p0y < 0 || p0x >= g->msx || p0y >= g->msy) B2S_FAIL(B2S_ERR_OUT_OF_RANGE, "laser position outside the map");
-  if (n > g->in_cap) {  // scan buffers live in the handle: no per-call allocation
-    if (g->d_in) B2S_CUDA_CHECK(cudaFree(g->d_in));
-    if (g->h_in) B2S_CUDA_CHECK(cudaFreeHost(g->h_in));
-    g->d_in = nullptr; g->h_in = nullptr; g->in_cap = 0;
-    const int cap = std::max(n, 2048);
-    B2S_CUDA_CHECK(cudaMalloc(reinterpret_cast<void **>(&g->d_in), sizeof(double) * 2 * (size_t)cap));
-    B2S_CUDA_CHECK(cudaMallocHost(reinterpret_cast<void **>(&g->h_in), sizeof(double) * 2 * (size_t)cap));
-    g->in_cap = cap;
-  }
-  if (!g->h_flag) B2S_CUDA_CHECK(cudaMallocHost(reinterpret_cast<void **>(&g->h_flag), sizeof(int)));
+  // scan buffers live in the handle: no per-call allocation
+  B2S_CUDA_CHECK(g->d_in.reserve(2 * (size_t)std::max(n, 2048)));
+  B2S_CUDA_CHECK(g->h_in.reserve(2 * (size_t)std::max(n, 2048)));
+  B2S_CUDA_CHECK(g->h_flag.reserve(1));
   std::memcpy(g->h_in, ranges, sizeof(double) * n);
   std::memcpy(g->h_in + n, angles, sizeof(double) * n);
   double *d_r = g->d_in, *d_a = g->d_in + n;
@@ -251,14 +228,13 @@ b2s_status b2s_gmap_copy_ros(b2s_gmap *g, int8_t *out) {
   // map_.info.width/height = (xmax - xmin) / resolution truncated to uint32 (gmapping.cc:70-71)
   const int width = (int)(uint32_t)((g->xmax - g->xmin) / g->delta), height = (int)(uint32_t)((g->ymax - g->ymin) / g->delta);
   if (width <= 0 || height <= 0) return B2S_OK;
-  int8_t *d = nullptr;
-  B2S_CUDA_CHECK(cudaMallocAsync(reinterpret_cast<void **>(&d), (size_t)width * height, g->stream));
+  AsyncBuf<int8_t> d(g->stream);
+  B2S_CUDA_CHECK(d.alloc((size_t)width * height));
   B2S_CUDA_CHECK(cudaMemsetAsync(d, 0, (size_t)width * height, g->stream));
   k_gm_ros<<<ceil_div((long long)g->msx * g->msy, 256), 256, 0, g->stream>>>(g->d_n, g->d_visits, g->msx, g->msy, 0.25,
                                                                             width, height, d);
   B2S_CUDA_CHECK(cudaGetLastError());
   B2S_CUDA_CHECK(cudaMemcpyAsync(out, d, (size_t)width * height, cudaMemcpyDeviceToHost, g->stream));
-  B2S_CUDA_CHECK(cudaFreeAsync(d, g->stream));
   B2S_CUDA_CHECK(cudaStreamSynchronize(g->stream));
   return B2S_OK;
 }

@@ -33,24 +33,22 @@
 using namespace b2s;
 
 struct b2s_hector_map {
+  Stream stream;
   int device = 0;
-  cudaStream_t stream = nullptr;
-  bool own_stream = false;
   int sx = 0, sy = 0;
   float cell_length = 0, scale_to_map = 0, off_x = 0, off_y = 0;
   float tw_lin = 0, tw_tx = 0, tw_ty = 0, wt_lin = 0, wt_tx = 0, wt_ty = 0;
   float lo_free = 0, lo_occ = 0;
   int curr_update_index = 0;
   unsigned int epoch = 0;
-  float *d_lo = nullptr;
-  int32_t *d_ui = nullptr;
-  unsigned long long *d_free = nullptr, *d_occ = nullptr;
-  float *d_pts = nullptr;
-  size_t pts_cap = 0;
-  float *d_out = nullptr;  // [3 pose + 9 H]
-  unsigned long long *d_visits = nullptr;
+  Buf<float> d_lo;
+  Buf<int32_t> d_ui;
+  Buf<unsigned long long> d_free, d_occ;
+  Buf<float> d_pts;
+  Buf<float> d_out;  // [3 pose + 9 H]
+  Buf<unsigned long long> d_visits;
   double last_ms[2] = {0, 0};
-  cudaEvent_t ev[4] = {nullptr, nullptr, nullptr, nullptr};  // update begin/end, match begin/end
+  Event ev[4];  // update begin/end, match begin/end
 };
 
 namespace b2s {
@@ -294,10 +292,8 @@ b2s_status b2s_hector_map_create(int size_x, int size_y, float resolution, float
                                  void *cuda_stream, b2s_hector_map **out) {
   if (!out || size_x <= 2 || size_y <= 2 || !(resolution > 0.0f)) B2S_FAIL(B2S_ERR_BAD_PARAMS, "b2s_hector_map_create: bad size/resolution");
   *out = nullptr;
-  if (b2s_device_count() <= device) B2S_FAIL(B2S_ERR_NO_DEVICE, "no usable CUDA device (the product path has no CPU fallback)");
-  B2S_CUDA_CHECK(cudaSetDevice(device));
-  keep_pool_memory(device);
-  b2s_hector_map *m = new (std::nothrow) b2s_hector_map();
+  if (b2s_status st = open_device(device)) return st;
+  std::unique_ptr<b2s_hector_map, decltype(&b2s_hector_map_destroy)> m(new (std::nothrow) b2s_hector_map(), b2s_hector_map_destroy);
   if (!m) B2S_FAIL(B2S_ERR_CUDA, "out of host memory");
   m->device = device;
   m->sx = size_x; m->sy = size_y;
@@ -318,40 +314,29 @@ b2s_status b2s_hector_map_create(int size_x, int size_y, float resolution, float
   m->wt_ty = -(i01 * m->tw_tx + m->wt_lin * m->tw_ty);
   m->lo_free = prob_to_log_odds(0.4f);  // GridMapLogOdds.h:98-102
   m->lo_occ = prob_to_log_odds(0.6f);
-  if (cuda_stream) {
-    m->stream = reinterpret_cast<cudaStream_t>(cuda_stream);
-  } else {
-    B2S_CUDA_CHECK_CLEAN(b2s_hector_map_destroy(m), cudaStreamCreateWithFlags(&m->stream, cudaStreamNonBlocking));
-    m->own_stream = true;
-  }
-  for (auto &e : m->ev) B2S_CUDA_CHECK_CLEAN(b2s_hector_map_destroy(m), cudaEventCreate(&e));
+  B2S_CUDA_CHECK(m->stream.init(cuda_stream));
+  for (auto &e : m->ev) B2S_CUDA_CHECK(e.create());
   const size_t cells = (size_t)size_x * size_y;
-  B2S_CUDA_CHECK_CLEAN(b2s_hector_map_destroy(m), cudaMalloc(reinterpret_cast<void **>(&m->d_lo), cells * 4));
-  B2S_CUDA_CHECK_CLEAN(b2s_hector_map_destroy(m), cudaMalloc(reinterpret_cast<void **>(&m->d_ui), cells * 4));
-  B2S_CUDA_CHECK_CLEAN(b2s_hector_map_destroy(m), cudaMalloc(reinterpret_cast<void **>(&m->d_free), cells * 8));
-  B2S_CUDA_CHECK_CLEAN(b2s_hector_map_destroy(m), cudaMalloc(reinterpret_cast<void **>(&m->d_occ), cells * 8));
-  B2S_CUDA_CHECK_CLEAN(b2s_hector_map_destroy(m), cudaMalloc(reinterpret_cast<void **>(&m->d_out), 12 * sizeof(float)));
-  B2S_CUDA_CHECK_CLEAN(b2s_hector_map_destroy(m), cudaMalloc(reinterpret_cast<void **>(&m->d_visits), sizeof(unsigned long long)));
-  B2S_CUDA_CHECK_CLEAN(b2s_hector_map_destroy(m), cudaMemsetAsync(m->d_lo, 0, cells * 4, m->stream));     // resetGridCell: logOdds 0
-  B2S_CUDA_CHECK_CLEAN(b2s_hector_map_destroy(m), cudaMemsetAsync(m->d_ui, 0xff, cells * 4, m->stream));  // updateIndex -1
-  B2S_CUDA_CHECK_CLEAN(b2s_hector_map_destroy(m), cudaMemsetAsync(m->d_free, 0, cells * 8, m->stream));
-  B2S_CUDA_CHECK_CLEAN(b2s_hector_map_destroy(m), cudaMemsetAsync(m->d_occ, 0, cells * 8, m->stream));
-  B2S_CUDA_CHECK_CLEAN(b2s_hector_map_destroy(m), cudaStreamSynchronize(m->stream));
+  B2S_CUDA_CHECK(m->d_lo.reserve(cells));
+  B2S_CUDA_CHECK(m->d_ui.reserve(cells));
+  B2S_CUDA_CHECK(m->d_free.reserve(cells));
+  B2S_CUDA_CHECK(m->d_occ.reserve(cells));
+  B2S_CUDA_CHECK(m->d_out.reserve(12));
+  B2S_CUDA_CHECK(m->d_visits.reserve(1));
+  B2S_CUDA_CHECK(cudaMemsetAsync(m->d_lo, 0, cells * 4, m->stream));     // resetGridCell: logOdds 0
+  B2S_CUDA_CHECK(cudaMemsetAsync(m->d_ui, 0xff, cells * 4, m->stream));  // updateIndex -1
+  B2S_CUDA_CHECK(cudaMemsetAsync(m->d_free, 0, cells * 8, m->stream));
+  B2S_CUDA_CHECK(cudaMemsetAsync(m->d_occ, 0, cells * 8, m->stream));
+  B2S_CUDA_CHECK(cudaStreamSynchronize(m->stream));
   m->epoch = 0;
-  *out = m;
+  *out = m.release();
   return B2S_OK;
 }
 
 void b2s_hector_map_destroy(b2s_hector_map *m) {
   if (!m) return;
   cudaSetDevice(m->device);
-  if (m->stream) cudaStreamSynchronize(m->stream);
-  for (void *p : {(void *)m->d_lo, (void *)m->d_ui, (void *)m->d_free, (void *)m->d_occ, (void *)m->d_pts, (void *)m->d_out,
-                  (void *)m->d_visits})
-    if (p) cudaFree(p);
-  for (auto &e : m->ev)
-    if (e) cudaEventDestroy(e);
-  if (m->own_stream && m->stream) cudaStreamDestroy(m->stream);
+  cudaStreamSynchronize(m->stream);
   delete m;
 }
 
@@ -363,12 +348,7 @@ b2s_status b2s_hector_map_set_factors(b2s_hector_map *m, float update_free, floa
 }
 
 static b2s_status hc_upload_points(b2s_hector_map *m, const float *points, int n) {
-  if ((size_t)n > m->pts_cap) {
-    if (m->d_pts) B2S_CUDA_CHECK(cudaFree(m->d_pts));
-    m->d_pts = nullptr;
-    B2S_CUDA_CHECK(cudaMalloc(reinterpret_cast<void **>(&m->d_pts), sizeof(float) * 2 * (size_t)n));
-    m->pts_cap = (size_t)n;
-  }
+  B2S_CUDA_CHECK(m->d_pts.reserve(2 * (size_t)n));
   B2S_CUDA_CHECK(cudaMemcpyAsync(m->d_pts, points, sizeof(float) * 2 * (size_t)n, cudaMemcpyHostToDevice, m->stream));
   return B2S_OK;
 }
@@ -463,12 +443,11 @@ b2s_status b2s_hector_map_copy_ros(b2s_hector_map *m, int8_t *out) {
   if (!m || !out) B2S_FAIL(B2S_ERR_BAD_PARAMS, "null argument");
   B2S_CUDA_CHECK(cudaSetDevice(m->device));
   const int n = m->sx * m->sy;
-  int8_t *d = nullptr;
-  B2S_CUDA_CHECK(cudaMallocAsync(reinterpret_cast<void **>(&d), (size_t)n, m->stream));
+  AsyncBuf<int8_t> d(m->stream);
+  B2S_CUDA_CHECK(d.alloc((size_t)n));
   k_hc_ros<<<ceil_div(n, 256), 256, 0, m->stream>>>(m->d_lo, n, d);
   B2S_CUDA_CHECK(cudaGetLastError());
   B2S_CUDA_CHECK(cudaMemcpyAsync(out, d, (size_t)n, cudaMemcpyDeviceToHost, m->stream));
-  B2S_CUDA_CHECK(cudaFreeAsync(d, m->stream));
   B2S_CUDA_CHECK(cudaStreamSynchronize(m->stream));
   return B2S_OK;
 }

@@ -1131,47 +1131,34 @@ static float hs_prob_to_log_odds(float prob) {  // GridMapLogOdds.h:153-157
 }  // namespace b2s
 
 struct b2s_hector_slam {
+  Stream stream;
   int device = 0;
-  cudaStream_t stream = nullptr;
-  bool own_stream = false;
   int levels = 0, batch = 1, cap = 0;
   int sx[HS_L] = {}, sy[HS_L] = {};
   float cell_length[HS_L] = {};
-  HsBatch P;
-  void *allocs[HS_L * 6 + 8] = {};
-  int n_allocs = 0;
-  HsState *d_state = nullptr;
-  float *d_out = nullptr;        // [batch][16] (per-scan / batch calls)
-  float *h_out = nullptr;        // pinned [batch][16]
-  float *h_pts = nullptr;        // host-mapped pinned staging of one scan (single-processor call)
-  float *h_pts_dev = nullptr;    // its device alias
-  volatile float *h_mail = nullptr;  // host-mapped mailbox [16]
-  float *h_mail_dev = nullptr;
-  float *h_hint = nullptr, *h_hint_dev = nullptr;  // host-mapped [3] pose hint of the per-scan call
+  HsBatch P;  // its level pointers view level_mem
+  struct {
+    Buf<float4> quad;
+    Buf<float> lo, pts;
+    Buf<int32_t> ui;
+    Buf<uint32_t> free_st, occ_st;
+  } level_mem[HS_L];
+  Buf<HsState> d_state;
+  Buf<float> d_out;                // [batch][16] (per-scan / batch calls)
+  HostBuf<float> h_out;            // pinned [batch][16]
+  HostBuf<float> h_pts;            // host-mapped pinned staging of one scan (single-processor call)
+  HostBuf<volatile float> h_mail;  // host-mapped mailbox [16]
+  HostBuf<float> h_hint;           // host-mapped [3] pose hint of the per-scan call
   unsigned int seq = 0;
-  unsigned int *d_barrier = nullptr;
+  Buf<unsigned int> d_barrier;
   unsigned long long host_updates = 0;  // upper bound of every level's device epoch
   int stream_ctas = HS_STREAM_CTAS;
   bool coop = true;
   unsigned int launch_tag = 0;  // id of the last stream launch (the kernel publishes per-scan verdicts under it)
   int cluster = 1;  // CTAs per thread-block cluster of the fast-mode stream kernel (1: no cluster launch)
-  cudaEvent_t ev_done = nullptr;
+  Event ev_done;
   bool launch_pending = false;  // a per-scan launch may still be running its update passes
 };
-
-static void hs_free_all(b2s_hector_slam *p) {
-  for (int i = 0; i < p->n_allocs; i++)
-    if (p->allocs[i]) cudaFree(p->allocs[i]);
-  p->n_allocs = 0;
-  if (p->d_state) cudaFree(p->d_state);
-  if (p->d_out) cudaFree(p->d_out);
-  if (p->d_barrier) cudaFree(p->d_barrier);
-  if (p->h_out) cudaFreeHost(p->h_out);
-  if (p->h_pts) cudaFreeHost(p->h_pts);
-  if (p->h_mail) cudaFreeHost(const_cast<float *>(p->h_mail));
-  if (p->h_hint) cudaFreeHost(p->h_hint);
-  if (p->ev_done) cudaEventDestroy(p->ev_done);
-}
 
 extern "C" void b2s_hector_slam_destroy(b2s_hector_slam *p);
 
@@ -1216,22 +1203,14 @@ static b2s_status hs_create(float map_resolution, int map_size_x, int map_size_y
     B2S_FAIL(B2S_ERR_BAD_PARAMS, "b2s_hector_slam_create: bad levels / size / resolution / batch");
   *out = nullptr;
   if (max_points > HS_MAX_PTS) B2S_FAIL(B2S_ERR_TOO_LARGE, "at most 4096 points per scan");
-  if (b2s_device_count() <= device) B2S_FAIL(B2S_ERR_NO_DEVICE, "no usable CUDA device (the product path has no CPU fallback)");
-  B2S_CUDA_CHECK(cudaSetDevice(device));
-  keep_pool_memory(device);
-  b2s_hector_slam *p = new (std::nothrow) b2s_hector_slam();
+  if (b2s_status st = open_device(device)) return st;
+  std::unique_ptr<b2s_hector_slam, decltype(&b2s_hector_slam_destroy)> p(new (std::nothrow) b2s_hector_slam(), b2s_hector_slam_destroy);
   if (!p) B2S_FAIL(B2S_ERR_CUDA, "out of host memory");
   p->device = device;
   p->levels = levels;
   p->batch = batch;
   p->cap = max_points;
-#define HS_CHECK(expr) B2S_CUDA_CHECK_CLEAN(b2s_hector_slam_destroy(p), expr)
-  if (cuda_stream) {
-    p->stream = reinterpret_cast<cudaStream_t>(cuda_stream);
-  } else {
-    HS_CHECK(cudaStreamCreateWithFlags(&p->stream, cudaStreamNonBlocking));
-    p->own_stream = true;
-  }
+  B2S_CUDA_CHECK(p->stream.init(cuda_stream));
   std::memset(&p->P, 0, sizeof(p->P));
   p->P.levels = levels; p->P.batch = batch; p->P.cap = max_points;
   p->P.lo_free = hs_prob_to_log_odds(0.4f);  // GridMapLogOdds.h:98-102
@@ -1261,46 +1240,38 @@ static b2s_status hs_create(float map_resolution, int map_size_x, int map_size_y
     m.wt_ty = -(i01 * m.tw_tx + m.wt_lin * m.tw_ty);
     m.iterations = 1 + (l == 0 ? 5 : 3);
     const size_t cells = (size_t)sx * sy * batch;
-    void **slots[4] = {(void **)&m.lo, (void **)&m.ui, (void **)&m.free_st, (void **)&m.occ_st};
-    for (void **s : slots) {
-      HS_CHECK(cudaMalloc(s, cells * 4));
-      p->allocs[p->n_allocs++] = *s;
-    }
-    HS_CHECK(cudaMalloc(reinterpret_cast<void **>(&m.quad), cells * 16));
-    p->allocs[p->n_allocs++] = m.quad;
-    HS_CHECK(cudaMalloc(reinterpret_cast<void **>(&m.pts), sizeof(float) * 2 * (size_t)max_points * batch));
-    p->allocs[p->n_allocs++] = m.pts;
+    auto &mem = p->level_mem[l];
+    B2S_CUDA_CHECK(mem.lo.reserve(cells));
+    B2S_CUDA_CHECK(mem.ui.reserve(cells));
+    B2S_CUDA_CHECK(mem.free_st.reserve(cells));
+    B2S_CUDA_CHECK(mem.occ_st.reserve(cells));
+    B2S_CUDA_CHECK(mem.quad.reserve(cells));
+    B2S_CUDA_CHECK(mem.pts.reserve(2 * (size_t)max_points * batch));
+    m.lo = mem.lo; m.ui = mem.ui; m.free_st = mem.free_st; m.occ_st = mem.occ_st; m.quad = mem.quad; m.pts = mem.pts;
     sx /= 2; sy /= 2;
     res *= 2.0f;
   }
-  HS_CHECK(cudaMalloc(reinterpret_cast<void **>(&p->d_state), sizeof(HsState) * (size_t)batch));
+  B2S_CUDA_CHECK(p->d_state.reserve(batch));
   p->P.state = p->d_state;
-  HS_CHECK(cudaMalloc(reinterpret_cast<void **>(&p->d_out), sizeof(float) * 16 * (size_t)batch));
-  HS_CHECK(cudaMalloc(reinterpret_cast<void **>(&p->d_barrier), sizeof(unsigned int)));
-  HS_CHECK(cudaMallocHost(reinterpret_cast<void **>(&p->h_out), sizeof(float) * 16 * (size_t)batch));
-  HS_CHECK(cudaHostAlloc(reinterpret_cast<void **>(&p->h_pts), sizeof(float) * 2 * (size_t)max_points, cudaHostAllocMapped));
-  HS_CHECK(cudaHostGetDevicePointer(reinterpret_cast<void **>(&p->h_pts_dev), p->h_pts, 0));
-  {
-    float *mail = nullptr;
-    HS_CHECK(cudaHostAlloc(reinterpret_cast<void **>(&mail), sizeof(float) * 16, cudaHostAllocMapped));
-    std::memset(mail, 0, sizeof(float) * 16);
-    p->h_mail = mail;
-    HS_CHECK(cudaHostGetDevicePointer(reinterpret_cast<void **>(&p->h_mail_dev), mail, 0));
-  }
-  HS_CHECK(cudaHostAlloc(reinterpret_cast<void **>(&p->h_hint), sizeof(float) * 4, cudaHostAllocMapped));
-  HS_CHECK(cudaHostGetDevicePointer(reinterpret_cast<void **>(&p->h_hint_dev), p->h_hint, 0));
-  HS_CHECK(cudaEventCreateWithFlags(&p->ev_done, cudaEventDisableTiming));
+  B2S_CUDA_CHECK(p->d_out.reserve(16 * (size_t)batch));
+  B2S_CUDA_CHECK(p->d_barrier.reserve(1));
+  B2S_CUDA_CHECK(p->h_out.reserve(16 * (size_t)batch));
+  B2S_CUDA_CHECK(p->h_pts.reserve(2 * (size_t)max_points, cudaHostAllocMapped));
+  B2S_CUDA_CHECK(p->h_mail.reserve(16, cudaHostAllocMapped));
+  std::memset((void *)p->h_mail.p, 0, sizeof(float) * 16);
+  B2S_CUDA_CHECK(p->h_hint.reserve(4, cudaHostAllocMapped));
+  B2S_CUDA_CHECK(p->ev_done.create(cudaEventDisableTiming));
   const size_t smem = hs_smem_bytes(max_points);
-  HS_CHECK(raise_dyn_smem(k_hs_match<true>, smem));
-  HS_CHECK(raise_dyn_smem(k_hs_match<false>, smem));
-  HS_CHECK(raise_dyn_smem(k_hs_stream<true, false>, smem));
-  HS_CHECK(raise_dyn_smem(k_hs_stream<false, false>, smem));
-  HS_CHECK(raise_dyn_smem(k_hs_stream<false, true>, smem));
+  B2S_CUDA_CHECK(raise_dyn_smem(k_hs_match<true>, smem));
+  B2S_CUDA_CHECK(raise_dyn_smem(k_hs_match<false>, smem));
+  B2S_CUDA_CHECK(raise_dyn_smem(k_hs_stream<true, false>, smem));
+  B2S_CUDA_CHECK(raise_dyn_smem(k_hs_stream<false, false>, smem));
+  B2S_CUDA_CHECK(raise_dyn_smem(k_hs_stream<false, true>, smem));
   {
     int coop = 0, sms = 0, per_sm = 0;
-    HS_CHECK(cudaDeviceGetAttribute(&coop, cudaDevAttrCooperativeLaunch, device));
-    HS_CHECK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device));
-    HS_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_hs_stream<true, false>, HS_THREADS, smem));
+    B2S_CUDA_CHECK(cudaDeviceGetAttribute(&coop, cudaDevAttrCooperativeLaunch, device));
+    B2S_CUDA_CHECK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device));
+    B2S_CUDA_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_hs_stream<true, false>, HS_THREADS, smem));
     p->coop = coop != 0;
     int want = HS_STREAM_CTAS;
     if (const char *ec = getenv("B2S_HS_STREAM_CTAS")) want = std::max(1, atoi(ec));  // tuning switch
@@ -1330,14 +1301,10 @@ static b2s_status hs_create(float map_resolution, int map_size_x, int map_size_y
     }
   }
   k_hs_state_init<<<ceil_div(batch, 128), 128, 0, p->stream>>>(p->d_state, batch, 2);
-  {
-    b2s_status st = hs_clear_maps(p);
-    if (st) { b2s_hector_slam_destroy(p); return st; }
-  }
-  HS_CHECK(cudaGetLastError());
-  HS_CHECK(cudaStreamSynchronize(p->stream));
-#undef HS_CHECK
-  *out = p;
+  if (b2s_status st = hs_clear_maps(p.get())) return st;
+  B2S_CUDA_CHECK(cudaGetLastError());
+  B2S_CUDA_CHECK(cudaStreamSynchronize(p->stream));
+  *out = p.release();
   return B2S_OK;
 }
 
@@ -1406,9 +1373,7 @@ b2s_status b2s_hector_slam_create_batch(int batch, int max_points, float map_res
 void b2s_hector_slam_destroy(b2s_hector_slam *p) {
   if (!p) return;
   cudaSetDevice(p->device);
-  if (p->stream) cudaStreamSynchronize(p->stream);
-  hs_free_all(p);
-  if (p->own_stream && p->stream) cudaStreamDestroy(p->stream);
+  cudaStreamSynchronize(p->stream);
   delete p;
 }
 
@@ -1461,20 +1426,20 @@ b2s_status b2s_hector_slam_update(b2s_hector_slam *p, const float *points, int n
   if (p->seq == 0) p->seq = 1;
   HsStream S;
   std::memset(&S, 0, sizeof(S));
-  S.pts = p->h_pts_dev;        // read over the host link by the matching CTA (8.6 KB for 1081 beams)
+  S.pts = p->h_pts.dev;        // read over the host link by the matching CTA (8.6 KB for 1081 beams)
   S.count0 = n_points;
   S.n_scans = 1;
-  S.first_hint = p->h_hint_dev;
+  S.first_hint = p->h_hint.dev;
   S.origo_x = origo[0]; S.origo_y = origo[1];
   S.map_without_matching = map_without_matching;
   S.out = p->d_out;
-  S.mailbox = p->h_mail_dev;
+  S.mailbox = p->h_mail.dev;
   S.seq = p->seq;
   if ((st = hs_launch_stream(p, S))) return st;
   B2S_CUDA_CHECK(cudaEventRecord(p->ev_done, p->stream));
   p->launch_pending = true;
   // the pose arrives through the mailbox as soon as the match is done; the update passes keep running
-  const volatile unsigned int *flag = reinterpret_cast<const volatile unsigned int *>(p->h_mail) + 15;
+  const volatile unsigned int *flag = reinterpret_cast<const volatile unsigned int *>(p->h_mail.p) + 15;
   for (unsigned long long spin = 0;; spin++) {
     if (*flag == p->seq) break;
     if ((spin & 0x3fff) == 0x3fff) {
@@ -1518,28 +1483,22 @@ b2s_status b2s_hector_slam_process_stream(b2s_hector_slam *p, int n_scans, const
     if (total > 0x7fffffffLL / 2) B2S_FAIL(B2S_ERR_TOO_LARGE, "stream too long for one call");
   }
   if ((st = hs_reserve_epochs(p, (unsigned long long)n_scans))) return st;
-  float *d_pts = nullptr, *d_hints = nullptr, *d_first = nullptr, *d_out = nullptr;
-  int *d_offs = nullptr, *d_cnt = nullptr;
-  auto release = [&]() {
-    for (void *q : {(void *)d_pts, (void *)d_hints, (void *)d_first, (void *)d_out, (void *)d_offs, (void *)d_cnt})
-      if (q) cudaFreeAsync(q, p->stream);
-    cudaStreamSynchronize(p->stream);
-  };
-#define HS_CHECK(expr) B2S_CUDA_CHECK_CLEAN(release(), expr)
-  HS_CHECK(cudaMallocAsync(reinterpret_cast<void **>(&d_pts), sizeof(float) * 2 * (size_t)std::max<long long>(total, 1), p->stream));
-  HS_CHECK(cudaMallocAsync(reinterpret_cast<void **>(&d_out), sizeof(float) * 16 * (size_t)n_scans, p->stream));
-  HS_CHECK(cudaMemsetAsync(d_out, 0, sizeof(float) * 16 * (size_t)n_scans, p->stream));  // no stale verdict tags
-  HS_CHECK(cudaMallocAsync(reinterpret_cast<void **>(&d_offs), sizeof(int) * (size_t)n_scans, p->stream));
-  HS_CHECK(cudaMallocAsync(reinterpret_cast<void **>(&d_cnt), sizeof(int) * (size_t)n_scans, p->stream));
-  if (total > 0) HS_CHECK(cudaMemcpyAsync(d_pts, points, sizeof(float) * 2 * (size_t)total, cudaMemcpyHostToDevice, p->stream));
-  HS_CHECK(cudaMemcpyAsync(d_offs, offs.data(), sizeof(int) * (size_t)n_scans, cudaMemcpyHostToDevice, p->stream));
-  HS_CHECK(cudaMemcpyAsync(d_cnt, n_points, sizeof(int) * (size_t)n_scans, cudaMemcpyHostToDevice, p->stream));
+  AsyncBuf<float> d_pts(p->stream), d_hints(p->stream), d_first(p->stream), d_out(p->stream);
+  AsyncBuf<int> d_offs(p->stream), d_cnt(p->stream);
+  B2S_CUDA_CHECK(d_pts.alloc(2 * (size_t)std::max<long long>(total, 1)));
+  B2S_CUDA_CHECK(d_out.alloc(16 * (size_t)n_scans));
+  B2S_CUDA_CHECK(cudaMemsetAsync(d_out, 0, sizeof(float) * 16 * (size_t)n_scans, p->stream));  // no stale verdict tags
+  B2S_CUDA_CHECK(d_offs.alloc(n_scans));
+  B2S_CUDA_CHECK(d_cnt.alloc(n_scans));
+  if (total > 0) B2S_CUDA_CHECK(cudaMemcpyAsync(d_pts, points, sizeof(float) * 2 * (size_t)total, cudaMemcpyHostToDevice, p->stream));
+  B2S_CUDA_CHECK(cudaMemcpyAsync(d_offs, offs.data(), sizeof(int) * (size_t)n_scans, cudaMemcpyHostToDevice, p->stream));
+  B2S_CUDA_CHECK(cudaMemcpyAsync(d_cnt, n_points, sizeof(int) * (size_t)n_scans, cudaMemcpyHostToDevice, p->stream));
   if (pose_hints) {
-    HS_CHECK(cudaMallocAsync(reinterpret_cast<void **>(&d_hints), sizeof(float) * 3 * (size_t)n_scans, p->stream));
-    HS_CHECK(cudaMemcpyAsync(d_hints, pose_hints, sizeof(float) * 3 * (size_t)n_scans, cudaMemcpyHostToDevice, p->stream));
+    B2S_CUDA_CHECK(d_hints.alloc(3 * (size_t)n_scans));
+    B2S_CUDA_CHECK(cudaMemcpyAsync(d_hints, pose_hints, sizeof(float) * 3 * (size_t)n_scans, cudaMemcpyHostToDevice, p->stream));
   } else if (first_pose_hint) {
-    HS_CHECK(cudaMallocAsync(reinterpret_cast<void **>(&d_first), sizeof(float) * 3, p->stream));
-    HS_CHECK(cudaMemcpyAsync(d_first, first_pose_hint, sizeof(float) * 3, cudaMemcpyHostToDevice, p->stream));
+    B2S_CUDA_CHECK(d_first.alloc(3));
+    B2S_CUDA_CHECK(cudaMemcpyAsync(d_first, first_pose_hint, sizeof(float) * 3, cudaMemcpyHostToDevice, p->stream));
   }
   HsStream S;
   std::memset(&S, 0, sizeof(S));
@@ -1548,12 +1507,10 @@ b2s_status b2s_hector_slam_process_stream(b2s_hector_slam *p, int n_scans, const
   S.origo_x = origo[0]; S.origo_y = origo[1];
   S.map_without_matching = map_without_matching;
   S.out = d_out;
-  if ((st = hs_launch_stream(p, S))) { release(); return st; }
+  if ((st = hs_launch_stream(p, S))) return st;
   std::vector<float> host((size_t)n_scans * 16);
-  HS_CHECK(cudaMemcpyAsync(host.data(), d_out, sizeof(float) * 16 * (size_t)n_scans, cudaMemcpyDeviceToHost, p->stream));
-  HS_CHECK(cudaStreamSynchronize(p->stream));
-#undef HS_CHECK
-  release();
+  B2S_CUDA_CHECK(cudaMemcpyAsync(host.data(), d_out, sizeof(float) * 16 * (size_t)n_scans, cudaMemcpyDeviceToHost, p->stream));
+  B2S_CUDA_CHECK(cudaStreamSynchronize(p->stream));
   for (int i = 0; i < n_scans; i++) {
     if (host[16 * (size_t)i + 14] != 0.0f) B2S_FAIL(B2S_ERR_CUDA, "b2s_hector_slam_process_stream: a cluster exchange of the match timed out");
     std::memcpy(out_poses + 3 * (size_t)i, host.data() + 16 * (size_t)i, 3 * sizeof(float));
@@ -1575,20 +1532,15 @@ b2s_status b2s_hector_slam_update_batch(b2s_hector_slam *p, const float *points,
   for (int b = 0; b < B; b++)
     if (n_points[b] < 0 || n_points[b] > p->cap) B2S_FAIL(B2S_ERR_TOO_LARGE, "a scan has more points than the handle's capacity");
   if ((st = hs_reserve_epochs(p, 1))) return st;
-  float *d_pts = nullptr, *d_hints = nullptr;
-  int *d_cnt = nullptr;
-  auto release = [&]() {
-    for (void *q : {(void *)d_pts, (void *)d_hints, (void *)d_cnt})
-      if (q) cudaFreeAsync(q, p->stream);
-  };
-#define HS_CHECK(expr) B2S_CUDA_CHECK_CLEAN((release(), cudaStreamSynchronize(p->stream)), expr)
-  HS_CHECK(cudaMallocAsync(reinterpret_cast<void **>(&d_pts), sizeof(float) * 2 * (size_t)p->cap * B, p->stream));
-  HS_CHECK(cudaMallocAsync(reinterpret_cast<void **>(&d_cnt), sizeof(int) * (size_t)B, p->stream));
-  HS_CHECK(cudaMemcpyAsync(d_pts, points, sizeof(float) * 2 * (size_t)p->cap * B, cudaMemcpyHostToDevice, p->stream));
-  HS_CHECK(cudaMemcpyAsync(d_cnt, n_points, sizeof(int) * (size_t)B, cudaMemcpyHostToDevice, p->stream));
+  AsyncBuf<float> d_pts(p->stream), d_hints(p->stream);
+  AsyncBuf<int> d_cnt(p->stream);
+  B2S_CUDA_CHECK(d_pts.alloc(2 * (size_t)p->cap * B));
+  B2S_CUDA_CHECK(d_cnt.alloc(B));
+  B2S_CUDA_CHECK(cudaMemcpyAsync(d_pts, points, sizeof(float) * 2 * (size_t)p->cap * B, cudaMemcpyHostToDevice, p->stream));
+  B2S_CUDA_CHECK(cudaMemcpyAsync(d_cnt, n_points, sizeof(int) * (size_t)B, cudaMemcpyHostToDevice, p->stream));
   if (pose_hints) {
-    HS_CHECK(cudaMallocAsync(reinterpret_cast<void **>(&d_hints), sizeof(float) * 3 * (size_t)B, p->stream));
-    HS_CHECK(cudaMemcpyAsync(d_hints, pose_hints, sizeof(float) * 3 * (size_t)B, cudaMemcpyHostToDevice, p->stream));
+    B2S_CUDA_CHECK(d_hints.alloc(3 * (size_t)B));
+    B2S_CUDA_CHECK(cudaMemcpyAsync(d_hints, pose_hints, sizeof(float) * 3 * (size_t)B, cudaMemcpyHostToDevice, p->stream));
   }
   HsCall C;
   std::memset(&C, 0, sizeof(C));
@@ -1606,11 +1558,9 @@ b2s_status b2s_hector_slam_update_batch(b2s_hector_slam *p, const float *points,
   const dim3 grid(std::max(1, std::min(ceil_div(std::max(max_n, 1) * p->levels, 8), sm_count(p->device) * 8 / std::max(1, std::min(B, 8)))), B);
   k_hs_mark<<<grid, 256, 0, p->stream>>>(p->P);
   k_hs_apply<<<grid, 256, 0, p->stream>>>(p->P);
-  HS_CHECK(cudaGetLastError());
-  HS_CHECK(cudaMemcpyAsync(p->h_out, p->d_out, sizeof(float) * 16 * (size_t)B, cudaMemcpyDeviceToHost, p->stream));
-  release();
-  HS_CHECK(cudaStreamSynchronize(p->stream));
-#undef HS_CHECK
+  B2S_CUDA_CHECK(cudaGetLastError());
+  B2S_CUDA_CHECK(cudaMemcpyAsync(p->h_out, p->d_out, sizeof(float) * 16 * (size_t)B, cudaMemcpyDeviceToHost, p->stream));
+  B2S_CUDA_CHECK(cudaStreamSynchronize(p->stream));
   for (int b = 0; b < B; b++) {
     std::memcpy(out_poses + 3 * (size_t)b, p->h_out + 16 * (size_t)b, 3 * sizeof(float));
     if (out_covs && !map_without_matching) std::memcpy(out_covs + 9 * (size_t)b, p->h_out + 16 * (size_t)b + 3, 9 * sizeof(float));
@@ -1685,14 +1635,12 @@ b2s_status b2s_hector_slam_copy_level_ros(b2s_hector_slam *p, int level, int8_t 
   B2S_CUDA_CHECK(cudaSetDevice(p->device));
   const HsLevel &m = p->P.l[level];
   const int n = m.sx * m.sy;
-  int8_t *d = nullptr;
-  B2S_CUDA_CHECK(cudaMallocAsync(reinterpret_cast<void **>(&d), (size_t)n, p->stream));
+  AsyncBuf<int8_t> d(p->stream);
+  B2S_CUDA_CHECK(d.alloc((size_t)n));
   k_hs_ros<<<ceil_div(n, 256), 256, 0, p->stream>>>(m.lo, n, d);
-  cudaError_t e = cudaGetLastError();
-  if (e == cudaSuccess) e = cudaMemcpyAsync(out, d, (size_t)n, cudaMemcpyDeviceToHost, p->stream);
-  cudaFreeAsync(d, p->stream);
-  if (e == cudaSuccess) e = cudaStreamSynchronize(p->stream);
-  B2S_CUDA_CHECK(e);
+  B2S_CUDA_CHECK(cudaGetLastError());
+  B2S_CUDA_CHECK(cudaMemcpyAsync(out, d, (size_t)n, cudaMemcpyDeviceToHost, p->stream));
+  B2S_CUDA_CHECK(cudaStreamSynchronize(p->stream));
   p->launch_pending = false;
   return B2S_OK;
 }

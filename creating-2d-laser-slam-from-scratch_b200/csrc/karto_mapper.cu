@@ -802,7 +802,7 @@ b2s_status b2s_mapper_create(const b2s_mapper_params *params, const b2s_laser *l
   *out = nullptr;
   b2s_status st = check_params(params, laser);
   if (st) return st;
-  if (b2s_device_count() <= device) B2S_FAIL(B2S_ERR_NO_DEVICE, "no usable CUDA device (the product path has no CPU fallback)");
+  if ((st = check_device(device))) return st;
   CudaBackend *c = new (std::nothrow) CudaBackend();
   if (!c) B2S_FAIL(B2S_ERR_CUDA, "out of host memory");
   c->device = device;

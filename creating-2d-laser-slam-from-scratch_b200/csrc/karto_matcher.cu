@@ -117,12 +117,11 @@ struct SweepDims {
 using namespace b2s;
 
 struct b2s_matcher {
+  Stream stream;
   b2s_matcher_params p;
   b2s_laser l;
   b2s_grid_info g;
   int device = 0;
-  cudaStream_t stream = nullptr;
-  bool own_stream = false;
   int max_batch = 0, max_base = 0;
   int batch = 0, n = 0, n_base = 0;
   bool scans_set = false, grids_set = false;
@@ -132,48 +131,42 @@ struct b2s_matcher {
   int num_sms = 1;  // the device's, set at create
   int smem_optin = 0;
 
-  uint8_t *d_kernel = nullptr;
-  double *d_ranges = nullptr, *d_poses = nullptr, *d_sensor = nullptr, *d_pts = nullptr, *d_local = nullptr;
-  uint8_t *d_grids = nullptr;
-  double *d_grid_off = nullptr;
-  double *d_base_ranges = nullptr, *d_base_poses = nullptr, *d_base_pts = nullptr;
-  size_t base_cap = 0;
-  double *d_pool = nullptr;        // scan pool: readings of scans that serve as base scans again and again
-  size_t pool_cap = 0, pool_count = 0;
-  int32_t *d_base_src = nullptr;   // [batch * n_base] pool rows of the current base sets
-  size_t base_src_cap = 0;
-  int32_t *d_lut = nullptr;
-  size_t lut_cap = 0;
-  int32_t *d_lists = nullptr, *d_counts = nullptr, *d_starts = nullptr;  // window kernel: per-(match, angle) grouped window origins
-  size_t lists_cap = 0, counts_cap = 0, starts_cap = 0;
-  double *d_part_best = nullptr, *d_glob_best = nullptr, *d_tie = nullptr;  // split-sweep phases: [B], [B], [B][5]
-  int32_t *d_status = nullptr;                                              // [B] statuses of a split sweep
-  cudaEvent_t ev_split[6] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};
+  Buf<uint8_t> d_kernel;
+  Buf<double> d_ranges, d_poses, d_sensor, d_pts, d_local;
+  Buf<uint8_t> d_grids;
+  Buf<double> d_grid_off;
+  Buf<double> d_base_ranges, d_base_poses, d_base_pts;
+  Buf<double> d_pool;              // scan pool: readings of scans that serve as base scans again and again
+  size_t pool_count = 0;
+  Buf<int32_t> d_base_src;         // [batch * n_base] pool rows of the current base sets
+  Buf<int32_t> d_lut;
+  Buf<int32_t> d_lists, d_counts, d_starts;  // window kernel: per-(match, angle) grouped window origins
+  Buf<double> d_part_best, d_glob_best, d_tie;  // split-sweep phases: [B], [B], [B][5]
+  Buf<int32_t> d_status;                        // [B] statuses of a split sweep
+  Event ev_split[6];
   double last_split_ms[4] = {0, 0, 0, 0};
   int last_k_first = 0;
-  uint16_t *d_sat = nullptr;  // [B][(sby+1)(sbx+1)] block summed-area tables of the grids
+  Buf<uint16_t> d_sat;  // [B][(sby+1)(sbx+1)] block summed-area tables of the grids
   int sbx = 0, sby = 0;
   bool sat_valid = false;
-  unsigned long long *d_stats = nullptr;  // [0] beam-angle pairs dropped as empty windows in the last sweep
-  unsigned long long *h_stats = nullptr;  // pinned copy, read back with the results
+  Buf<unsigned long long> d_stats;      // [0] beam-angle pairs dropped as empty windows in the last sweep
+  HostBuf<unsigned long long> h_stats;  // pinned copy, read back with the results
   bool pending = false;                   // a correlate_scan_begin awaits its _end
   int pending_batch = 0;                  // batch size that _begin enqueued
   double last_empty_frac = 0.0;
   bool grid_high_bytes = false;  // set_grids saw a byte > 127: the packed-byte window kernel is not applicable
-  int32_t *d_sums = nullptr;
-  size_t sums_cap = 0;
-  int32_t *d_bases = nullptr;  // [B][ny*nx] candidate base indices
-  size_t bases_cap = 0;
-  int32_t *d_flags = nullptr;  // [B] per-match: bit0 lattice regular stride-1, bits 8.. status
-  double *d_probs = nullptr;
-  double *d_centers = nullptr;
-  b2s_match_result *d_results = nullptr;
-  b2s_match_result *h_results = nullptr;  // pinned
-  int *d_work = nullptr;                   // persistent-CTA work counter
+  Buf<int32_t> d_sums;
+  Buf<int32_t> d_bases;  // [B][ny*nx] candidate base indices
+  Buf<int32_t> d_flags;  // [B] per-match: bit0 lattice regular stride-1, bits 8.. status
+  Buf<double> d_probs;
+  Buf<double> d_centers;
+  Buf<b2s_match_result> d_results;
+  HostBuf<b2s_match_result> h_results;  // pinned
+  Buf<int> d_work;                       // persistent-CTA work counter
   SweepDims last;
   b2s_search last_search;
   bool have_sweep = false;
-  cudaEvent_t ev[4] = {nullptr, nullptr, nullptr, nullptr};
+  Event ev[4];
   double last_ms[4] = {0, 0, 0, 0};
   int last_path = 0;
 };
@@ -1500,22 +1493,6 @@ static b2s_status layout_from_params(const b2s_matcher_params *p, b2s_grid_info 
   return B2S_OK;
 }
 
-template <class T>
-static b2s_status dev_alloc(T **p, size_t count) {
-  B2S_CUDA_CHECK(cudaMalloc(reinterpret_cast<void **>(p), std::max<size_t>(count, 1) * sizeof(T)));
-  return B2S_OK;
-}
-
-template <class T>
-static b2s_status ensure_cap(T **p, size_t *cap, size_t count) {
-  if (count <= *cap && *p) return B2S_OK;
-  if (*p) B2S_CUDA_CHECK(cudaFree(*p));
-  *p = nullptr;
-  B2S_CUDA_CHECK(cudaMalloc(reinterpret_cast<void **>(p), std::max<size_t>(count, 1) * sizeof(T)));
-  *cap = count;
-  return B2S_OK;
-}
-
 static b2s_status run_correlate(b2s_matcher *m, const b2s_search *s, bool centers_on_device, int k_first = 0,
                                 int na_override = -1, int mode = 0);
 
@@ -1552,20 +1529,14 @@ int b2s_device_count(void) {
 void b2s_matcher_destroy(b2s_matcher *m);
 static b2s_status matcher_create_impl(const b2s_matcher_params *params, const b2s_laser *laser, int device, int max_batch,
                                       int max_base_scans, void *cuda_stream, b2s_matcher *m, const b2s_grid_info &g) {
-  b2s_status st;
   m->p = *params; m->l = *laser; m->g = g; m->device = device;
   m->max_batch = max_batch; m->max_base = max_base_scans; m->n = laser->n_readings;
   cudaDeviceProp prop;
   B2S_CUDA_CHECK(cudaGetDeviceProperties(&prop, device));
   m->num_sms = prop.multiProcessorCount;
   m->smem_optin = (int)prop.sharedMemPerBlockOptin;
-  if (cuda_stream) {
-    m->stream = reinterpret_cast<cudaStream_t>(cuda_stream);
-  } else {
-    B2S_CUDA_CHECK(cudaStreamCreateWithFlags(&m->stream, cudaStreamNonBlocking));
-    m->own_stream = true;
-  }
-  for (auto &e : m->ev) B2S_CUDA_CHECK(cudaEventCreate(&e));
+  B2S_CUDA_CHECK(m->stream.init(cuda_stream));
+  for (auto &e : m->ev) B2S_CUDA_CHECK(e.create());
   // smear kernel on the host with glibc, exactly CorrelationGrid::CalculateKernel (Mapper.h:1032-1087)
   {
     int ks = g.kernel_size, half = ks / 2;
@@ -1579,34 +1550,34 @@ static b2s_status matcher_create_impl(const b2s_matcher_params *params, const b2
         K[(i + half) + ks * (j + half)] = (uint8_t)kv;
         if ((i != 0 || j != 0) && kv >= (uint32_t)GRID_OCCUPIED) m->smear_degenerate = true;
       }
-    if ((st = dev_alloc(&m->d_kernel, K.size()))) return st;
+    B2S_CUDA_CHECK(m->d_kernel.reserve(K.size()));
     B2S_CUDA_CHECK(cudaMemcpy(m->d_kernel, K.data(), K.size(), cudaMemcpyHostToDevice));
   }
   const size_t B = (size_t)max_batch, N = (size_t)std::max(m->n, 1);
   m->grid_pitch = (((size_t)g.data_size + 16) + 127) & ~(size_t)127;
   const int pstep = (g.search_side + 7) & ~7;
-  if ((st = dev_alloc(&m->d_ranges, B * N))) return st;
-  if ((st = dev_alloc(&m->d_poses, B * 3))) return st;
-  if ((st = dev_alloc(&m->d_sensor, B * 3))) return st;
-  if ((st = dev_alloc(&m->d_pts, B * N * 2))) return st;
-  if ((st = dev_alloc(&m->d_local, B * N * 2))) return st;
-  if ((st = dev_alloc(&m->d_grids, B * m->grid_pitch))) return st;
-  if ((st = dev_alloc(&m->d_grid_off, B * 2))) return st;
-  if ((st = dev_alloc(&m->d_flags, B))) return st;
-  if ((st = dev_alloc(&m->d_probs, B * (size_t)pstep * g.search_side))) return st;
-  if ((st = dev_alloc(&m->d_centers, B * 3))) return st;
-  if ((st = dev_alloc(&m->d_results, B))) return st;
-  if ((st = dev_alloc(&m->d_work, 1))) return st;
+  B2S_CUDA_CHECK(m->d_ranges.reserve(B * N));
+  B2S_CUDA_CHECK(m->d_poses.reserve(B * 3));
+  B2S_CUDA_CHECK(m->d_sensor.reserve(B * 3));
+  B2S_CUDA_CHECK(m->d_pts.reserve(B * N * 2));
+  B2S_CUDA_CHECK(m->d_local.reserve(B * N * 2));
+  B2S_CUDA_CHECK(m->d_grids.reserve(B * m->grid_pitch));
+  B2S_CUDA_CHECK(m->d_grid_off.reserve(B * 2));
+  B2S_CUDA_CHECK(m->d_flags.reserve(B));
+  B2S_CUDA_CHECK(m->d_probs.reserve(B * (size_t)pstep * g.search_side));
+  B2S_CUDA_CHECK(m->d_centers.reserve(B * 3));
+  B2S_CUDA_CHECK(m->d_results.reserve(B));
+  B2S_CUDA_CHECK(m->d_work.reserve(1));
   m->sbx = (g.width_step + 3) / 4;
   m->sby = (g.height + 3) / 4;
-  if ((st = dev_alloc(&m->d_sat, B * (size_t)((((m->sbx + 1) * (m->sby + 1)) + 7) & ~7)))) return st;  // per-match stride padded to 16 bytes
-  if ((st = dev_alloc(&m->d_stats, 1))) return st;
-  if ((st = dev_alloc(&m->d_part_best, B))) return st;
-  if ((st = dev_alloc(&m->d_glob_best, B))) return st;
-  if ((st = dev_alloc(&m->d_tie, B * 5))) return st;
-  if ((st = dev_alloc(&m->d_status, B))) return st;
-  B2S_CUDA_CHECK(cudaMallocHost(reinterpret_cast<void **>(&m->h_results), B * sizeof(b2s_match_result)));
-  B2S_CUDA_CHECK(cudaMallocHost(reinterpret_cast<void **>(&m->h_stats), sizeof(unsigned long long)));
+  B2S_CUDA_CHECK(m->d_sat.reserve(B * (size_t)((((m->sbx + 1) * (m->sby + 1)) + 7) & ~7)));  // per-match stride padded to 16 bytes
+  B2S_CUDA_CHECK(m->d_stats.reserve(1));
+  B2S_CUDA_CHECK(m->d_part_best.reserve(B));
+  B2S_CUDA_CHECK(m->d_glob_best.reserve(B));
+  B2S_CUDA_CHECK(m->d_tie.reserve(B * 5));
+  B2S_CUDA_CHECK(m->d_status.reserve(B));
+  B2S_CUDA_CHECK(m->h_results.reserve(B));
+  B2S_CUDA_CHECK(m->h_stats.reserve(1));
   *m->h_stats = 0;
   B2S_CUDA_CHECK(cudaMemsetAsync(m->d_grids, 0, B * m->grid_pitch, m->stream));
   B2S_CUDA_CHECK(cudaMemsetAsync(m->d_results, 0, B * sizeof(b2s_match_result), m->stream));
@@ -1622,38 +1593,18 @@ b2s_status b2s_matcher_create(const b2s_matcher_params *params, const b2s_laser 
   b2s_grid_info g;
   b2s_status st = layout_from_params(params, &g);
   if (st) return st;
-  if (b2s_device_count() <= device) B2S_FAIL(B2S_ERR_NO_DEVICE, "no usable CUDA device (the product path has no CPU fallback)");
-  B2S_CUDA_CHECK(cudaSetDevice(device));
-  keep_pool_memory(device);
-  b2s_matcher *m = new (std::nothrow) b2s_matcher();
+  if ((st = open_device(device))) return st;
+  std::unique_ptr<b2s_matcher, decltype(&b2s_matcher_destroy)> m(new (std::nothrow) b2s_matcher(), b2s_matcher_destroy);
   if (!m) B2S_FAIL(B2S_ERR_CUDA, "out of host memory");
-  st = matcher_create_impl(params, laser, device, max_batch, max_base_scans, cuda_stream, m, g);
-  if (st) {  // release whatever was allocated before the failure
-    const std::string why = b2s::last_error_ref();
-    b2s_matcher_destroy(m);
-    b2s::set_last_error(why);
-    return st;
-  }
-  *out = m;
+  if ((st = matcher_create_impl(params, laser, device, max_batch, max_base_scans, cuda_stream, m.get(), g))) return st;
+  *out = m.release();
   return B2S_OK;
 }
 
 void b2s_matcher_destroy(b2s_matcher *m) {
   if (!m) return;
   cudaSetDevice(m->device);
-  if (m->stream) cudaStreamSynchronize(m->stream);
-  void *ptrs[] = {m->d_kernel, m->d_ranges, m->d_poses, m->d_sensor, m->d_pts, m->d_local, m->d_grids,
-                  m->d_grid_off, m->d_base_ranges, m->d_base_poses, m->d_base_pts, m->d_pool, m->d_base_src, m->d_lut, m->d_lists, m->d_counts, m->d_starts, m->d_sat, m->d_stats, m->d_part_best, m->d_glob_best, m->d_tie, m->d_status, m->d_sums, m->d_bases,
-                  m->d_flags, m->d_probs, m->d_centers, m->d_results, m->d_work};
-  for (void *p : ptrs)
-    if (p) cudaFree(p);
-  if (m->h_results) cudaFreeHost(m->h_results);
-  if (m->h_stats) cudaFreeHost(m->h_stats);
-  for (auto &e : m->ev)
-    if (e) cudaEventDestroy(e);
-  for (auto &e : m->ev_split)
-    if (e) cudaEventDestroy(e);
-  if (m->own_stream && m->stream) cudaStreamDestroy(m->stream);
+  cudaStreamSynchronize(m->stream);
   delete m;
 }
 
@@ -1712,15 +1663,9 @@ static b2s_status add_scans_impl(b2s_matcher *m, int n_base, const double *base_
   m->n_base = n_base;
   if (n_base > 0 && n > 0) {
     const size_t need = (size_t)B * n_base;
-    if (need > m->base_cap) {
-      for (double **p : {&m->d_base_ranges, &m->d_base_poses, &m->d_base_pts})
-        if (*p) { B2S_CUDA_CHECK(cudaFree(*p)); *p = nullptr; }
-      b2s_status st;
-      if ((st = dev_alloc(&m->d_base_ranges, need * n))) return st;
-      if ((st = dev_alloc(&m->d_base_poses, need * 3))) return st;
-      if ((st = dev_alloc(&m->d_base_pts, need * n * 2))) return st;
-      m->base_cap = need;
-    }
+    B2S_CUDA_CHECK(m->d_base_ranges.reserve(need * n));
+    B2S_CUDA_CHECK(m->d_base_poses.reserve(need * 3));
+    B2S_CUDA_CHECK(m->d_base_pts.reserve(need * n * 2));
     B2S_CUDA_CHECK(cudaMemcpyAsync(m->d_base_poses, base_poses, sizeof(double) * need * 3, cudaMemcpyHostToDevice, m->stream));
     if (base_ranges) {
       B2S_CUDA_CHECK(cudaMemcpyAsync(m->d_base_ranges, base_ranges, sizeof(double) * need * n, cudaMemcpyHostToDevice, m->stream));
@@ -1728,11 +1673,7 @@ static b2s_status add_scans_impl(b2s_matcher *m, int n_base, const double *base_
     } else {
       for (size_t i = 0; i < need; i++)
         if (pool_rows[i] < 0 || (size_t)pool_rows[i] >= m->pool_count) B2S_FAIL(B2S_ERR_OUT_OF_RANGE, "scan pool row out of range");
-      if (need > m->base_src_cap) {
-        if (m->d_base_src) { B2S_CUDA_CHECK(cudaFree(m->d_base_src)); m->d_base_src = nullptr; }
-        B2S_CUDA_CHECK(cudaMalloc(reinterpret_cast<void **>(&m->d_base_src), sizeof(int32_t) * need));
-        m->base_src_cap = need;
-      }
+      B2S_CUDA_CHECK(m->d_base_src.reserve(need));
       B2S_CUDA_CHECK(cudaMemcpyAsync(m->d_base_src, pool_rows, sizeof(int32_t) * need, cudaMemcpyHostToDevice, m->stream));
       k_scan_points<<<(unsigned)need, 256, 0, m->stream>>>(m->d_pool, m->d_base_poses, m->l, nullptr, m->d_base_pts, nullptr, m->d_base_src);
     }
@@ -1743,12 +1684,11 @@ static b2s_status add_scans_impl(b2s_matcher *m, int n_base, const double *base_
       k_add_scan<<<(unsigned)need, 256, smem, m->stream>>>(m->d_base_pts, m->d_sensor, m->d_grid_off, m->d_grids,
                                                            m->grid_pitch, m->d_kernel, m->g, scale, (int)n, n_base);
     } else {
-      uint8_t *scratch = nullptr;
-      B2S_CUDA_CHECK(cudaMallocAsync(reinterpret_cast<void **>(&scratch), (size_t)B * n, m->stream));
+      AsyncBuf<uint8_t> scratch(m->stream);
+      B2S_CUDA_CHECK(scratch.alloc((size_t)B * n));
       k_add_scans_seq<<<ceil_div(B, 32), 32, 0, m->stream>>>(m->d_base_pts, m->d_sensor, m->d_grid_off, m->d_grids,
                                                              m->grid_pitch, m->d_kernel, m->g, scale, (int)n, n_base,
                                                              B, scratch);
-      B2S_CUDA_CHECK(cudaFreeAsync(scratch, m->stream));
     }
     B2S_CUDA_CHECK(cudaGetLastError());
   }
@@ -1770,17 +1710,13 @@ b2s_status b2s_matcher_pool_append(b2s_matcher *m, const double *ranges, int32_t
   if (!m || !ranges) B2S_FAIL(B2S_ERR_BAD_PARAMS, "null argument");
   B2S_CUDA_CHECK(cudaSetDevice(m->device));
   const size_t n = (size_t)std::max(m->l.n_readings, 1);
-  if (m->pool_count == m->pool_cap) {
-    const size_t cap = std::max<size_t>(256, m->pool_cap * 2);
-    double *fresh = nullptr;
-    b2s_status st = dev_alloc(&fresh, cap * n);
-    if (st) return st;
+  if ((m->pool_count + 1) * n > m->d_pool.cap) {  // full: twice the rows (256 at first)
+    Buf<double> fresh;
+    B2S_CUDA_CHECK(fresh.reserve(std::max<size_t>(256, 2 * m->pool_count) * n));
     if (m->pool_count)
       B2S_CUDA_CHECK(cudaMemcpyAsync(fresh, m->d_pool, sizeof(double) * m->pool_count * n, cudaMemcpyDeviceToDevice, m->stream));
     B2S_CUDA_CHECK(cudaStreamSynchronize(m->stream));
-    if (m->d_pool) B2S_CUDA_CHECK(cudaFree(m->d_pool));
-    m->d_pool = fresh;
-    m->pool_cap = cap;
+    m->d_pool = std::move(fresh);  // the old pool is freed with `fresh`
   }
   B2S_CUDA_CHECK(cudaMemcpyAsync(m->d_pool + m->pool_count * n, ranges, sizeof(double) * n, cudaMemcpyHostToDevice, m->stream));
   if (out_row) *out_row = (int32_t)m->pool_count;
@@ -1842,17 +1778,15 @@ b2s_status b2s_matcher_compute_offsets(b2s_matcher *m, int b, double angle_cente
   B2S_CUDA_CHECK(cudaSetDevice(m->device));
   const int na = n_steps(angle_offset, angle_res);
   const size_t n = (size_t)m->n;
-  int32_t *tmp = nullptr;
-  B2S_CUDA_CHECK(cudaMalloc(reinterpret_cast<void **>(&tmp), sizeof(int32_t) * std::max<size_t>(na * n, 1)));
+  Buf<int32_t> tmp;
+  B2S_CUDA_CHECK(tmp.reserve(na * n));
   // one-match launch on the slices of match b
   k_offsets<<<na, 256, 0, m->stream>>>(m->d_ranges + (size_t)b * n, m->d_local + (size_t)b * n * 2,
                                        m->d_grid_off + 2 * b, nullptr, 0, angle_center, 1, angle_offset, angle_res, na,
                                        (int)n, m->g.width_step, 1.0 / m->p.resolution, tmp, 0);
-  cudaError_t e = cudaGetLastError();
-  if (e == cudaSuccess) e = cudaMemcpyAsync(out, tmp, sizeof(int32_t) * na * n, cudaMemcpyDeviceToHost, m->stream);
-  if (e == cudaSuccess) e = cudaStreamSynchronize(m->stream);
-  cudaFree(tmp);
-  B2S_CUDA_CHECK(e);
+  B2S_CUDA_CHECK(cudaGetLastError());
+  B2S_CUDA_CHECK(cudaMemcpyAsync(out, tmp, sizeof(int32_t) * na * n, cudaMemcpyDeviceToHost, m->stream));
+  B2S_CUDA_CHECK(cudaStreamSynchronize(m->stream));
   if (out_n_angles) *out_n_angles = na;
   return B2S_OK;
 }
@@ -1947,7 +1881,7 @@ b2s_status b2s_matcher_match_scan(b2s_matcher *m, int do_penalize, int do_refine
   if (m->p.use_response_expansion) {  // Mapper.cpp:242-272 — applied to the matches whose response is ~0
     B2S_CUDA_CHECK(cudaMemcpyAsync(m->h_results, m->d_results, sizeof(b2s_match_result) * B, cudaMemcpyDeviceToHost, m->stream));
     B2S_CUDA_CHECK(cudaStreamSynchronize(m->stream));
-    std::vector<b2s_match_result> keep(m->h_results, m->h_results + B);
+    std::vector<b2s_match_result> keep(m->h_results.p, m->h_results.p + B);
     std::vector<char> pending(B, 0);
     bool any = false;
     for (int b = 0; b < B; b++)
@@ -2097,7 +2031,7 @@ b2s_status b2s_matcher_correlate_scan_split(b2s_matcher *m, void *nccl_comm, int
   if (!nc.ok) B2S_FAIL(B2S_ERR_BAD_STATE, "libnccl.so.2 could not be loaded (dlopen)");
   B2S_CUDA_CHECK(cudaSetDevice(m->device));
   for (auto &e : m->ev_split)
-    if (!e) B2S_CUDA_CHECK(cudaEventCreate(&e));
+    if (!e) B2S_CUDA_CHECK(e.create());
   const int B = m->batch;
   const size_t plen = (size_t)((m->g.search_side + 7) & ~7) * m->g.search_side;
   const int na_full = n_steps(search->angle_offset, search->angle_res);
@@ -2205,8 +2139,8 @@ static b2s_status run_correlate(b2s_matcher *m, const b2s_search *s, bool /*cent
   const double scale = 1.0 / m->p.resolution;
   const int ncell = nx * ny;
   b2s_status st;
-  if ((st = ensure_cap(&m->d_sums, &m->sums_cap, (size_t)B * na * ncell))) return st;
-  if ((st = ensure_cap(&m->d_bases, &m->bases_cap, (size_t)B * ncell))) return st;
+  B2S_CUDA_CHECK(m->d_sums.reserve((size_t)B * na * ncell));
+  B2S_CUDA_CHECK(m->d_bases.reserve((size_t)B * ncell));
 
   // ---- which sweep kernel ----
   // The window kernel needs a stride-1 lattice and a band of the grid in shared memory: the whole grid when it fits
@@ -2253,7 +2187,7 @@ static b2s_status run_correlate(b2s_matcher *m, const b2s_search *s, bool /*cent
     B2S_FAIL(B2S_ERR_TOO_LARGE, "window kernel forced but not applicable to this lattice / grid / beam count");
   if (m->force_kernel >= 2) use_window = true;
   const bool need_plain_lut = !use_window || s->fine;  // generic sweep and the angular covariance read the plain table
-  if (need_plain_lut && (st = ensure_cap(&m->d_lut, &m->lut_cap, (size_t)B * na * std::max(n, 1)))) return st;
+  if (need_plain_lut) B2S_CUDA_CHECK(m->d_lut.reserve((size_t)B * na * std::max(n, 1)));
 
   B2S_CUDA_CHECK(cudaEventRecord(m->ev[0], m->stream));
   k_bases<<<B, 256, 0, m->stream>>>(m->d_centers, m->d_grid_off, *s, m->g, scale, nx, ny, m->d_bases, m->d_flags,
@@ -2263,9 +2197,9 @@ static b2s_status run_correlate(b2s_matcher *m, const b2s_search *s, bool /*cent
                                              s->angle_offset, s->angle_res, na, n, m->g.width_step, scale, m->d_lut, k_first);
   const dim3 ggrid((unsigned)ceil_div(ncell, 8), (unsigned)B);
   if (use_window && na > 0) {
-    if ((st = ensure_cap(&m->d_lists, &m->lists_cap, (size_t)B * na * (n + LIST_PAD * nbands)))) return st;
-    if ((st = ensure_cap(&m->d_counts, &m->counts_cap, (size_t)B * na * 8 * nbands))) return st;
-    if ((st = ensure_cap(&m->d_starts, &m->starts_cap, (size_t)B * na * 8 * nbands))) return st;
+    B2S_CUDA_CHECK(m->d_lists.reserve((size_t)B * na * (n + LIST_PAD * nbands)));
+    B2S_CUDA_CHECK(m->d_counts.reserve((size_t)B * na * 8 * nbands));
+    B2S_CUDA_CHECK(m->d_starts.reserve((size_t)B * na * 8 * nbands));
     bool skip_empty = m->sat_valid && m->force_kernel != 3;
     if ((((size_t)n * OFF_SMEM_PER_BEAM + 15) & ~(size_t)15) + sizeof(uint16_t) * (size_t)((((m->sbx + 1) * (m->sby + 1)) + 7) & ~7) + 64 > 200 * 1024) skip_empty = false;
     const size_t sat_bytes = skip_empty ? sizeof(uint16_t) * (size_t)((((m->sbx + 1) * (m->sby + 1)) + 7) & ~7) : 0;
@@ -2276,7 +2210,7 @@ static b2s_status run_correlate(b2s_matcher *m, const b2s_search *s, bool /*cent
     k_offsets_sorted<<<B * ((na + OFF_CHUNK - 1) / OFF_CHUNK), 256, osm, m->stream>>>(
         m->d_ranges, m->d_local, m->d_grid_off, m->d_centers, m->d_bases, m->d_flags, s->angle_offset, s->angle_res, na, n,
         ncell, m->g.width_step, m->g.data_size, scale, rows_total, tiles_x_w * 32, m->d_lists, m->d_counts,
-        skip_empty ? m->d_sat : nullptr, m->sbx, m->sby, m->g.height, nx, ny, m->d_stats, band_rows, nbands, m->d_starts,
+        skip_empty ? m->d_sat.p : nullptr, m->sbx, m->sby, m->g.height, nx, ny, m->d_stats, band_rows, nbands, m->d_starts,
         stride, k_first, neg_bands);
   }
   B2S_CUDA_CHECK(cudaGetLastError());

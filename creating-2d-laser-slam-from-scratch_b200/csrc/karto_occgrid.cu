@@ -28,12 +28,11 @@
 using namespace b2s;
 
 struct b2s_occ_grid {
+  Stream stream;
   b2s_occ_grid_info info;
   int device = 0;
-  cudaStream_t stream = nullptr;
-  bool own_stream = false;
-  uint32_t *d_pass = nullptr, *d_hit = nullptr;
-  uint8_t *d_cells = nullptr;
+  Buf<uint32_t> d_pass, d_hit;
+  Buf<uint8_t> d_cells;
   double last_ms[2] = {0, 0};
 };
 
@@ -202,33 +201,26 @@ static b2s_status occ_create_impl(const b2s_laser *laser, int n_scans, const dou
     return B2S_OK;
   }
   if (double_equal(resolution, 0.0)) B2S_FAIL(B2S_ERR_BAD_PARAMS, "Resolution cannot be 0");  // Karto.h:5627-5630
-  if (b2s_device_count() <= device) B2S_FAIL(B2S_ERR_NO_DEVICE, "no usable CUDA device (the product path has no CPU fallback)");
-  B2S_CUDA_CHECK(cudaSetDevice(device));
-  keep_pool_memory(device);
-  b2s_occ_grid *g = new (std::nothrow) b2s_occ_grid();
+  if (b2s_status st = open_device(device)) return st;
+  std::unique_ptr<b2s_occ_grid, decltype(&b2s_occ_grid_destroy)> g(new (std::nothrow) b2s_occ_grid(), b2s_occ_grid_destroy);
   if (!g) B2S_FAIL(B2S_ERR_CUDA, "out of host memory");
   g->device = device;
-  if (cuda_stream) {
-    g->stream = reinterpret_cast<cudaStream_t>(cuda_stream);
-  } else {
-    B2S_CUDA_CHECK_CLEAN(b2s_occ_grid_destroy(g), cudaStreamCreateWithFlags(&g->stream, cudaStreamNonBlocking));
-    g->own_stream = true;
-  }
+  B2S_CUDA_CHECK(g->stream.init(cuda_stream));
   cudaStream_t st = g->stream;
   const size_t n = (size_t)std::max(laser->n_readings, 0), M = (size_t)n_scans;
-  double *d_ranges = nullptr, *d_poses = nullptr, *d_sensor = nullptr, *d_pts = nullptr, *d_bbox = nullptr;
-  unsigned long long *d_visits = nullptr;
-  cudaEvent_t ev[3];
-  for (auto &e : ev) B2S_CUDA_CHECK_CLEAN(b2s_occ_grid_destroy(g), cudaEventCreate(&e));
-  B2S_CUDA_CHECK_CLEAN(b2s_occ_grid_destroy(g), cudaMallocAsync(reinterpret_cast<void **>(&d_ranges), sizeof(double) * std::max<size_t>(M * n, 1), st));
-  B2S_CUDA_CHECK_CLEAN(b2s_occ_grid_destroy(g), cudaMallocAsync(reinterpret_cast<void **>(&d_poses), sizeof(double) * std::max<size_t>(M * 3, 1), st));
-  B2S_CUDA_CHECK_CLEAN(b2s_occ_grid_destroy(g), cudaMallocAsync(reinterpret_cast<void **>(&d_sensor), sizeof(double) * std::max<size_t>(M * 3, 1), st));
-  B2S_CUDA_CHECK_CLEAN(b2s_occ_grid_destroy(g), cudaMallocAsync(reinterpret_cast<void **>(&d_pts), sizeof(double) * std::max<size_t>(M * n * 2, 1), st));
-  B2S_CUDA_CHECK_CLEAN(b2s_occ_grid_destroy(g), cudaMallocAsync(reinterpret_cast<void **>(&d_bbox), sizeof(double) * (M + 1) * 4, st));
-  B2S_CUDA_CHECK_CLEAN(b2s_occ_grid_destroy(g), cudaMallocAsync(reinterpret_cast<void **>(&d_visits), sizeof(unsigned long long), st));
-  if (n && M) B2S_CUDA_CHECK_CLEAN(b2s_occ_grid_destroy(g), cudaMemcpyAsync(d_ranges, ranges, sizeof(double) * M * n, cudaMemcpyHostToDevice, st));
-  if (M) B2S_CUDA_CHECK_CLEAN(b2s_occ_grid_destroy(g), cudaMemcpyAsync(d_poses, poses, sizeof(double) * M * 3, cudaMemcpyHostToDevice, st));
-  B2S_CUDA_CHECK_CLEAN(b2s_occ_grid_destroy(g), cudaMemsetAsync(d_visits, 0, sizeof(unsigned long long), st));
+  Event ev[3];
+  for (auto &e : ev) B2S_CUDA_CHECK(e.create());
+  AsyncBuf<double> d_ranges(st), d_poses(st), d_sensor(st), d_pts(st), d_bbox(st);
+  AsyncBuf<unsigned long long> d_visits(st);
+  B2S_CUDA_CHECK(d_ranges.alloc(std::max<size_t>(M * n, 1)));
+  B2S_CUDA_CHECK(d_poses.alloc(std::max<size_t>(M * 3, 1)));
+  B2S_CUDA_CHECK(d_sensor.alloc(std::max<size_t>(M * 3, 1)));
+  B2S_CUDA_CHECK(d_pts.alloc(std::max<size_t>(M * n * 2, 1)));
+  B2S_CUDA_CHECK(d_bbox.alloc((M + 1) * 4));
+  B2S_CUDA_CHECK(d_visits.alloc(1));
+  if (n && M) B2S_CUDA_CHECK(cudaMemcpyAsync(d_ranges, ranges, sizeof(double) * M * n, cudaMemcpyHostToDevice, st));
+  if (M) B2S_CUDA_CHECK(cudaMemcpyAsync(d_poses, poses, sizeof(double) * M * 3, cudaMemcpyHostToDevice, st));
+  B2S_CUDA_CHECK(cudaMemsetAsync(d_visits, 0, sizeof(unsigned long long), st));
   double bb[4];
   if (M) k_scan_points<<<(unsigned)M, 256, 0, st>>>(d_ranges, d_poses, *laser, d_sensor, d_pts, nullptr, nullptr);
   if (given_bbox) {
@@ -236,16 +228,12 @@ static b2s_status occ_create_impl(const b2s_laser *laser, int n_scans, const dou
   } else {
     k_scan_bbox<<<(unsigned)M, 256, 0, st>>>(d_ranges, d_sensor, d_pts, *laser, d_bbox);
     k_bbox_union<<<1, 256, 0, st>>>(d_bbox, n_scans, d_bbox + 4 * M);
-    B2S_CUDA_CHECK_CLEAN(b2s_occ_grid_destroy(g), cudaGetLastError());
-    B2S_CUDA_CHECK_CLEAN(b2s_occ_grid_destroy(g), cudaMemcpyAsync(bb, d_bbox + 4 * M, sizeof(bb), cudaMemcpyDeviceToHost, st));
-    B2S_CUDA_CHECK_CLEAN(b2s_occ_grid_destroy(g), cudaStreamSynchronize(st));
+    B2S_CUDA_CHECK(cudaGetLastError());
+    B2S_CUDA_CHECK(cudaMemcpyAsync(bb, d_bbox + 4 * M, sizeof(bb), cudaMemcpyDeviceToHost, st));
+    B2S_CUDA_CHECK(cudaStreamSynchronize(st));
   }
   if (bbox_out) {
     for (int i = 0; i < 4; i++) bbox_out[i] = bb[i];
-    for (void *p : {(void *)d_ranges, (void *)d_poses, (void *)d_sensor, (void *)d_pts, (void *)d_bbox, (void *)d_visits})
-      cudaFreeAsync(p, st);
-    for (auto &e : ev) cudaEventDestroy(e);
-    b2s_occ_grid_destroy(g);
     return B2S_OK;
   }
   // OccupancyGrid::ComputeDimensions (Karto.h:5816-5821)
@@ -253,10 +241,8 @@ static b2s_status occ_create_impl(const b2s_laser *laser, int n_scans, const dou
   b2s_occ_grid_info &I = g->info;
   I.width = cast_i32(kround((bb[2] - bb[0]) * scale));
   I.height = cast_i32(kround((bb[3] - bb[1]) * scale));
-  if (I.width < 0 || I.height < 0 || (long long)I.width * I.height > (1ll << 31)) {
-    b2s_occ_grid_destroy(g);
+  if (I.width < 0 || I.height < 0 || (long long)I.width * I.height > (1ll << 31))
     B2S_FAIL(B2S_ERR_TOO_LARGE, "occupancy grid dimensions out of range");
-  }
   I.width_step = (I.width + 7) & ~7;
   I.data_size = I.width_step * I.height;
   I.offset[0] = bb[0];
@@ -264,12 +250,12 @@ static b2s_status occ_create_impl(const b2s_laser *laser, int n_scans, const dou
   I.resolution = resolution;
   I.cell_visits = 0;
   const size_t cells = (size_t)std::max(I.data_size, 1);
-  B2S_CUDA_CHECK_CLEAN(b2s_occ_grid_destroy(g), cudaMalloc(reinterpret_cast<void **>(&g->d_pass), sizeof(uint32_t) * cells));
-  B2S_CUDA_CHECK_CLEAN(b2s_occ_grid_destroy(g), cudaMalloc(reinterpret_cast<void **>(&g->d_hit), sizeof(uint32_t) * cells));
-  B2S_CUDA_CHECK_CLEAN(b2s_occ_grid_destroy(g), cudaMalloc(reinterpret_cast<void **>(&g->d_cells), cells));
-  B2S_CUDA_CHECK_CLEAN(b2s_occ_grid_destroy(g), cudaMemsetAsync(g->d_pass, 0, sizeof(uint32_t) * cells, st));
-  B2S_CUDA_CHECK_CLEAN(b2s_occ_grid_destroy(g), cudaMemsetAsync(g->d_hit, 0, sizeof(uint32_t) * cells, st));
-  B2S_CUDA_CHECK_CLEAN(b2s_occ_grid_destroy(g), cudaEventRecord(ev[0], st));
+  B2S_CUDA_CHECK(g->d_pass.reserve(cells));
+  B2S_CUDA_CHECK(g->d_hit.reserve(cells));
+  B2S_CUDA_CHECK(g->d_cells.reserve(cells));
+  B2S_CUDA_CHECK(cudaMemsetAsync(g->d_pass, 0, sizeof(uint32_t) * cells, st));
+  B2S_CUDA_CHECK(cudaMemsetAsync(g->d_hit, 0, sizeof(uint32_t) * cells, st));
+  B2S_CUDA_CHECK(cudaEventRecord(ev[0], st));
   if (n && M && I.data_size > 0) {
     const long long n_beams = (long long)M * (long long)n;
     const int sms = sm_count(device);
@@ -280,21 +266,18 @@ static b2s_status occ_create_impl(const b2s_laser *laser, int n_scans, const dou
     k_raytrace<<<blocks, 256, 0, st>>>(d_ranges, d_sensor, d_pts, *laser, n_beams, I.width, I.height, I.width_step,
                                        I.offset[0], I.offset[1], scale, g->d_pass, g->d_hit, d_visits);
   }
-  B2S_CUDA_CHECK_CLEAN(b2s_occ_grid_destroy(g), cudaEventRecord(ev[1], st));
+  B2S_CUDA_CHECK(cudaEventRecord(ev[1], st));
   if (I.data_size > 0) k_occ_threshold<<<ceil_div(I.data_size, 256), 256, 0, st>>>(g->d_pass, g->d_hit, I.data_size, g->d_cells);
-  B2S_CUDA_CHECK_CLEAN(b2s_occ_grid_destroy(g), cudaEventRecord(ev[2], st));
-  B2S_CUDA_CHECK_CLEAN(b2s_occ_grid_destroy(g), cudaGetLastError());
+  B2S_CUDA_CHECK(cudaEventRecord(ev[2], st));
+  B2S_CUDA_CHECK(cudaGetLastError());
   unsigned long long visits = 0;
-  B2S_CUDA_CHECK_CLEAN(b2s_occ_grid_destroy(g), cudaMemcpyAsync(&visits, d_visits, sizeof(visits), cudaMemcpyDeviceToHost, st));
-  for (void *p : {(void *)d_ranges, (void *)d_poses, (void *)d_sensor, (void *)d_pts, (void *)d_bbox, (void *)d_visits})
-    B2S_CUDA_CHECK_CLEAN(b2s_occ_grid_destroy(g), cudaFreeAsync(p, st));
-  B2S_CUDA_CHECK_CLEAN(b2s_occ_grid_destroy(g), cudaStreamSynchronize(st));
+  B2S_CUDA_CHECK(cudaMemcpyAsync(&visits, d_visits, sizeof(visits), cudaMemcpyDeviceToHost, st));
+  B2S_CUDA_CHECK(cudaStreamSynchronize(st));
   I.cell_visits = visits;
   float ms = 0;
   if (cudaEventElapsedTime(&ms, ev[0], ev[1]) == cudaSuccess) g->last_ms[0] = ms;
   if (cudaEventElapsedTime(&ms, ev[1], ev[2]) == cudaSuccess) g->last_ms[1] = ms;
-  for (auto &e : ev) cudaEventDestroy(e);
-  *out = g;
+  *out = g.release();
   return B2S_OK;
 }
 
@@ -336,7 +319,7 @@ b2s_status b2s_occ_grid_allreduce_counters(b2s_occ_grid *g, void *nccl_comm) {
   B2S_CUDA_CHECK(cudaSetDevice(g->device));
   const size_t cells = (size_t)std::max(g->info.data_size, 0);
   if (cells == 0) return B2S_OK;
-  for (uint32_t *buf : {g->d_pass, g->d_hit}) {
+  for (uint32_t *buf : {g->d_pass.p, g->d_hit.p}) {
     const int rc = nc.all_reduce(buf, buf, cells, NCCL_UINT32, NCCL_SUM, nccl_comm, g->stream);
     if (rc != 0) B2S_FAIL(B2S_ERR_CUDA, std::string("ncclAllReduce(counters) failed: ") + (nc.error_string ? nc.error_string(rc) : "NCCL error"));
   }
@@ -388,12 +371,11 @@ b2s_status b2s_occ_grid_copy_ros(b2s_occ_grid *g, int8_t *out) {
   B2S_CUDA_CHECK(cudaSetDevice(g->device));
   const int w = g->info.width, h = g->info.height;
   if (w * h == 0) return B2S_OK;
-  int8_t *d = nullptr;
-  B2S_CUDA_CHECK(cudaMallocAsync(reinterpret_cast<void **>(&d), (size_t)w * h, g->stream));
+  AsyncBuf<int8_t> d(g->stream);
+  B2S_CUDA_CHECK(d.alloc((size_t)w * h));
   k_occ_ros<<<ceil_div((long long)w * h, 256), 256, 0, g->stream>>>(g->d_cells, w, h, g->info.width_step, d);
   B2S_CUDA_CHECK(cudaGetLastError());
   B2S_CUDA_CHECK(cudaMemcpyAsync(out, d, (size_t)w * h, cudaMemcpyDeviceToHost, g->stream));
-  B2S_CUDA_CHECK(cudaFreeAsync(d, g->stream));
   B2S_CUDA_CHECK(cudaStreamSynchronize(g->stream));
   return B2S_OK;
 }
@@ -408,11 +390,7 @@ b2s_status b2s_occ_grid_last_timing(b2s_occ_grid *g, double out[2]) {
 void b2s_occ_grid_destroy(b2s_occ_grid *g) {
   if (!g) return;
   cudaSetDevice(g->device);
-  if (g->stream) cudaStreamSynchronize(g->stream);
-  if (g->d_pass) cudaFree(g->d_pass);
-  if (g->d_hit) cudaFree(g->d_hit);
-  if (g->d_cells) cudaFree(g->d_cells);
-  if (g->own_stream && g->stream) cudaStreamDestroy(g->stream);
+  cudaStreamSynchronize(g->stream);
   delete g;
 }
 

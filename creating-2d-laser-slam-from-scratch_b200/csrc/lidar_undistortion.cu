@@ -197,38 +197,28 @@ b2s_status b2s_lidar_undistort(int batch, int n_beams, const float *ranges, doub
     if (scans[b].use_odom && !(scans[b].odom_end_time != scans[b].odom_start_time))
       B2S_FAIL(B2S_ERR_BAD_PARAMS, "b2s_lidar_undistort: odometry interval of zero length");
   }
-  if (b2s_device_count() <= device) B2S_FAIL(B2S_ERR_NO_DEVICE, "no usable CUDA device (the product path has no CPU fallback)");
-  B2S_CUDA_CHECK(cudaSetDevice(device));
-  keep_pool_memory(device);
+  if (b2s_status st = open_device(device)) return st;
   cudaStream_t st = reinterpret_cast<cudaStream_t>(cuda_stream);
   const size_t nr = (size_t)batch * n_beams, ni = (size_t)batch * imu_stride;
-  float *d_r = nullptr, *d_o = nullptr;
-  double *d_imu = nullptr;
-  b2s_deskew_scan *d_s = nullptr;
-  auto release = [&]() {
-    for (void *q : {(void *)d_r, (void *)d_o, (void *)d_imu, (void *)d_s})
-      if (q) cudaFreeAsync(q, st);
-    cudaStreamSynchronize(st);
-  };
-#define DSK_CHECK(expr) B2S_CUDA_CHECK_CLEAN(release(), expr)
-  DSK_CHECK(cudaMallocAsync(reinterpret_cast<void **>(&d_r), nr * sizeof(float), st));
-  DSK_CHECK(cudaMallocAsync(reinterpret_cast<void **>(&d_o), nr * 3 * sizeof(float), st));
-  DSK_CHECK(cudaMallocAsync(reinterpret_cast<void **>(&d_imu), ni * 4 * sizeof(double), st));
-  DSK_CHECK(cudaMallocAsync(reinterpret_cast<void **>(&d_s), (size_t)batch * sizeof(b2s_deskew_scan), st));
-  DSK_CHECK(cudaMemcpyAsync(d_r, ranges, nr * sizeof(float), cudaMemcpyHostToDevice, st));
-  DSK_CHECK(cudaMemcpyAsync(d_imu, imu_time, ni * sizeof(double), cudaMemcpyHostToDevice, st));
-  DSK_CHECK(cudaMemcpyAsync(d_imu + ni, imu_rot_x, ni * sizeof(double), cudaMemcpyHostToDevice, st));
-  DSK_CHECK(cudaMemcpyAsync(d_imu + 2 * ni, imu_rot_y, ni * sizeof(double), cudaMemcpyHostToDevice, st));
-  DSK_CHECK(cudaMemcpyAsync(d_imu + 3 * ni, imu_rot_z, ni * sizeof(double), cudaMemcpyHostToDevice, st));
-  DSK_CHECK(cudaMemcpyAsync(d_s, scans, (size_t)batch * sizeof(b2s_deskew_scan), cudaMemcpyHostToDevice, st));
+  AsyncBuf<float> d_r(st), d_o(st);
+  AsyncBuf<double> d_imu(st);
+  AsyncBuf<b2s_deskew_scan> d_s(st);
+  B2S_CUDA_CHECK(d_r.alloc(nr));
+  B2S_CUDA_CHECK(d_o.alloc(nr * 3));
+  B2S_CUDA_CHECK(d_imu.alloc(ni * 4));
+  B2S_CUDA_CHECK(d_s.alloc(batch));
+  B2S_CUDA_CHECK(cudaMemcpyAsync(d_r, ranges, nr * sizeof(float), cudaMemcpyHostToDevice, st));
+  B2S_CUDA_CHECK(cudaMemcpyAsync(d_imu, imu_time, ni * sizeof(double), cudaMemcpyHostToDevice, st));
+  B2S_CUDA_CHECK(cudaMemcpyAsync(d_imu + ni, imu_rot_x, ni * sizeof(double), cudaMemcpyHostToDevice, st));
+  B2S_CUDA_CHECK(cudaMemcpyAsync(d_imu + 2 * ni, imu_rot_y, ni * sizeof(double), cudaMemcpyHostToDevice, st));
+  B2S_CUDA_CHECK(cudaMemcpyAsync(d_imu + 3 * ni, imu_rot_z, ni * sizeof(double), cudaMemcpyHostToDevice, st));
+  B2S_CUDA_CHECK(cudaMemcpyAsync(d_s, scans, (size_t)batch * sizeof(b2s_deskew_scan), cudaMemcpyHostToDevice, st));
   const dim3 grid(ceil_div(n_beams, DSK_THREADS), batch);
   k_deskew<<<grid, DSK_THREADS, 0, st>>>(d_r, n_beams, angle_min, angle_increment, d_s, d_imu, d_imu + ni, d_imu + 2 * ni,
                                          d_imu + 3 * ni, imu_stride, d_o);
-  DSK_CHECK(cudaGetLastError());
-  DSK_CHECK(cudaMemcpyAsync(out_xyz, d_o, nr * 3 * sizeof(float), cudaMemcpyDeviceToHost, st));
-  DSK_CHECK(cudaStreamSynchronize(st));
-#undef DSK_CHECK
-  release();
+  B2S_CUDA_CHECK(cudaGetLastError());
+  B2S_CUDA_CHECK(cudaMemcpyAsync(out_xyz, d_o, nr * 3 * sizeof(float), cudaMemcpyDeviceToHost, st));
+  B2S_CUDA_CHECK(cudaStreamSynchronize(st));
   return B2S_OK;
 }
 

@@ -302,9 +302,7 @@ extern "C" b2s_status b2s_plicp_match(const b2s_icp_params *params, int batch, i
   if (!params || !ref_ranges || !sens_ranges || !theta || !first_guess || !results || batch <= 0 || n < 3 ||
       params->max_iterations < 1)
     B2S_FAIL(B2S_ERR_BAD_PARAMS, "b2s_plicp_match: null/invalid argument");
-  if (b2s_device_count() <= device) B2S_FAIL(B2S_ERR_NO_DEVICE, "no usable CUDA device (the product path has no CPU fallback)");
-  B2S_CUDA_CHECK(cudaSetDevice(device));
-  keep_pool_memory(device);
+  if (b2s_status st = open_device(device)) return st;
   // shared memory: the kernel's static arrays + the per-beam dynamic part must fit the opt-in limit of the device
   cudaFuncAttributes fa;
   B2S_CUDA_CHECK(cudaFuncGetAttributes(&fa, k_plicp));
@@ -314,36 +312,23 @@ extern "C" b2s_status b2s_plicp_match(const b2s_icp_params *params, int batch, i
   if (smem + fa.sharedSizeBytes > (size_t)optin) B2S_FAIL(B2S_ERR_TOO_LARGE, "too many beams for the shared-memory PL-ICP kernel");
   // always opt in: static + dynamic crosses the 48 KB default long before the dynamic part alone does
   B2S_CUDA_CHECK(cudaFuncSetAttribute(k_plicp, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)((size_t)optin - fa.sharedSizeBytes)));
-  cudaStream_t st = reinterpret_cast<cudaStream_t>(cuda_stream);
-  bool own = false;
-  if (!st) {
-    B2S_CUDA_CHECK(cudaStreamCreateWithFlags(&st, cudaStreamNonBlocking));
-    own = true;
-  }
-  double *d_ref = nullptr, *d_sens = nullptr, *d_theta = nullptr, *d_guess = nullptr;
-  b2s_icp_result *d_res = nullptr;
+  Stream st;  // declared before the buffers freed on it
+  B2S_CUDA_CHECK(st.init(cuda_stream));
   const size_t bn = (size_t)batch * n;
-  auto release = [&]() {  // error paths too: nothing allocated here outlives the call
-    for (void *p : {(void *)d_ref, (void *)d_sens, (void *)d_theta, (void *)d_guess, (void *)d_res})
-      if (p) cudaFreeAsync(p, st);
-    cudaStreamSynchronize(st);
-    if (own) cudaStreamDestroy(st);
-  };
-#define ICP_CHECK(expr) B2S_CUDA_CHECK_CLEAN(release(), expr)
-  ICP_CHECK(cudaMallocAsync(reinterpret_cast<void **>(&d_ref), sizeof(double) * bn, st));
-  ICP_CHECK(cudaMallocAsync(reinterpret_cast<void **>(&d_sens), sizeof(double) * bn, st));
-  ICP_CHECK(cudaMallocAsync(reinterpret_cast<void **>(&d_theta), sizeof(double) * n, st));
-  ICP_CHECK(cudaMallocAsync(reinterpret_cast<void **>(&d_guess), sizeof(double) * 3 * batch, st));
-  ICP_CHECK(cudaMallocAsync(reinterpret_cast<void **>(&d_res), sizeof(b2s_icp_result) * batch, st));
-  ICP_CHECK(cudaMemcpyAsync(d_ref, ref_ranges, sizeof(double) * bn, cudaMemcpyHostToDevice, st));
-  ICP_CHECK(cudaMemcpyAsync(d_sens, sens_ranges, sizeof(double) * bn, cudaMemcpyHostToDevice, st));
-  ICP_CHECK(cudaMemcpyAsync(d_theta, theta, sizeof(double) * n, cudaMemcpyHostToDevice, st));
-  ICP_CHECK(cudaMemcpyAsync(d_guess, first_guess, sizeof(double) * 3 * batch, cudaMemcpyHostToDevice, st));
+  AsyncBuf<double> d_ref(st), d_sens(st), d_theta(st), d_guess(st);
+  AsyncBuf<b2s_icp_result> d_res(st);
+  B2S_CUDA_CHECK(d_ref.alloc(bn));
+  B2S_CUDA_CHECK(d_sens.alloc(bn));
+  B2S_CUDA_CHECK(d_theta.alloc(n));
+  B2S_CUDA_CHECK(d_guess.alloc(3 * (size_t)batch));
+  B2S_CUDA_CHECK(d_res.alloc(batch));
+  B2S_CUDA_CHECK(cudaMemcpyAsync(d_ref, ref_ranges, sizeof(double) * bn, cudaMemcpyHostToDevice, st));
+  B2S_CUDA_CHECK(cudaMemcpyAsync(d_sens, sens_ranges, sizeof(double) * bn, cudaMemcpyHostToDevice, st));
+  B2S_CUDA_CHECK(cudaMemcpyAsync(d_theta, theta, sizeof(double) * n, cudaMemcpyHostToDevice, st));
+  B2S_CUDA_CHECK(cudaMemcpyAsync(d_guess, first_guess, sizeof(double) * 3 * batch, cudaMemcpyHostToDevice, st));
   k_plicp<<<batch, ICP_THREADS, smem, st>>>(*params, n, d_ref, d_sens, d_theta, range_min, range_max, d_guess, d_res);
-  ICP_CHECK(cudaGetLastError());
-  ICP_CHECK(cudaMemcpyAsync(results, d_res, sizeof(b2s_icp_result) * batch, cudaMemcpyDeviceToHost, st));
-  ICP_CHECK(cudaStreamSynchronize(st));
-#undef ICP_CHECK
-  release();
+  B2S_CUDA_CHECK(cudaGetLastError());
+  B2S_CUDA_CHECK(cudaMemcpyAsync(results, d_res, sizeof(b2s_icp_result) * batch, cudaMemcpyDeviceToHost, st));
+  B2S_CUDA_CHECK(cudaStreamSynchronize(st));
   return B2S_OK;
 }
