@@ -872,8 +872,8 @@ struct ReduceArgs {
 };
 
 
-template <int STRIDE, bool GEN, int THREADS>
-__global__ void __launch_bounds__(THREADS, 1)
+template <int STRIDE, bool GEN>
+__global__ void __launch_bounds__(WIN_THREADS, 1)
     k_sweep_window(const uint8_t *__restrict__ grids, size_t grid_pitch, int data_size, int copy_bytes,
                    const int32_t *__restrict__ lists, const int32_t *__restrict__ counts,
                    const int32_t *__restrict__ starts, const int32_t *__restrict__ flags, int batch, int n, int na,
@@ -887,7 +887,7 @@ __global__ void __launch_bounds__(THREADS, 1)
   uint8_t *sgrid = smem;  // [WIN_GUARD zeros][band image][WIN_GUARD zeros]
   __shared__ uint64_t bar;
   __shared__ int s_unit, s_item;
-  __shared__ __align__(16) int32_t s_offsets[THREADS / 32][32];  // per-warp staging of 32 window origins
+  __shared__ __align__(16) int32_t s_offsets[WIN_THREADS / 32][32];  // per-warp staging of 32 window origins
 
   const int lane = threadIdx.x & 31;
   int32_t *s_off = s_offsets[threadIdx.x >> 5];
@@ -1493,8 +1493,7 @@ static b2s_status layout_from_params(const b2s_matcher_params *p, b2s_grid_info 
   return B2S_OK;
 }
 
-static b2s_status run_correlate(b2s_matcher *m, const b2s_search *s, bool centers_on_device, int k_first = 0,
-                                int na_override = -1, int mode = 0);
+static b2s_status run_correlate(b2s_matcher *m, const b2s_search *s, int k_first = 0, int na_override = -1, int mode = 0);
 
 // (re)build the per-match block summed-area tables after the grids changed
 static b2s_status build_sat(b2s_matcher *m) {
@@ -1807,7 +1806,7 @@ b2s_status b2s_matcher_correlate_scan_begin(b2s_matcher *m, const double *center
     for (int b = 0; b < B; b++) m->h_results[b] = cov_in[b];
     B2S_CUDA_CHECK(cudaMemcpyAsync(m->d_results, m->h_results, sizeof(b2s_match_result) * B, cudaMemcpyHostToDevice, m->stream));
   }
-  b2s_status st = run_correlate(m, search, true);
+  b2s_status st = run_correlate(m, search);
   if (st) return st;
   B2S_CUDA_CHECK(cudaMemcpyAsync(m->h_results, m->d_results, sizeof(b2s_match_result) * B, cudaMemcpyDeviceToHost, m->stream));
   B2S_CUDA_CHECK(cudaMemcpyAsync(m->h_stats, m->d_stats, sizeof(unsigned long long), cudaMemcpyDeviceToHost, m->stream));
@@ -1876,7 +1875,7 @@ b2s_status b2s_matcher_match_scan(b2s_matcher *m, int do_penalize, int do_refine
   coarse.fine = 0;
   // search centre = scan (sensor) pose (Mapper.cpp:237)
   B2S_CUDA_CHECK(cudaMemcpyAsync(m->d_centers, m->d_sensor, sizeof(double) * 3 * B, cudaMemcpyDeviceToDevice, m->stream));
-  b2s_status st = run_correlate(m, &coarse, true);
+  b2s_status st = run_correlate(m, &coarse);
   if (st) return st;
   if (m->p.use_response_expansion) {  // Mapper.cpp:242-272 — applied to the matches whose response is ~0
     B2S_CUDA_CHECK(cudaMemcpyAsync(m->h_results, m->d_results, sizeof(b2s_match_result) * B, cudaMemcpyDeviceToHost, m->stream));
@@ -1892,7 +1891,7 @@ b2s_status b2s_matcher_match_scan(b2s_matcher *m, int do_penalize, int do_refine
       b2s_search ex = coarse;
       ex.angle_offset = new_off;
       B2S_CUDA_CHECK(cudaMemcpyAsync(m->d_centers, m->d_sensor, sizeof(double) * 3 * B, cudaMemcpyDeviceToDevice, m->stream));
-      st = run_correlate(m, &ex, true);
+      st = run_correlate(m, &ex);
       if (st) return st;
       B2S_CUDA_CHECK(cudaMemcpyAsync(m->h_results, m->d_results, sizeof(b2s_match_result) * B, cudaMemcpyDeviceToHost, m->stream));
       B2S_CUDA_CHECK(cudaStreamSynchronize(m->stream));
@@ -1918,7 +1917,7 @@ b2s_status b2s_matcher_match_scan(b2s_matcher *m, int do_penalize, int do_refine
     fine.do_penalize = do_penalize;
     fine.fine = 1;
     k_results_to_centers<<<ceil_div(B, 128), 128, 0, m->stream>>>(m->d_results, m->d_centers, B);
-    st = run_correlate(m, &fine, true);
+    st = run_correlate(m, &fine);
     if (st) return st;
   }
   B2S_CUDA_CHECK(cudaMemcpyAsync(m->h_results, m->d_results, sizeof(b2s_match_result) * B, cudaMemcpyDeviceToHost, m->stream));
@@ -1953,7 +1952,7 @@ b2s_status b2s_matcher_correlate_split_begin(b2s_matcher *m, const double *cente
   const int B = m->batch;
   const size_t plen = (size_t)((m->g.search_side + 7) & ~7) * m->g.search_side;
   B2S_CUDA_CHECK(cudaMemcpyAsync(m->d_centers, centers, sizeof(double) * 3 * B, cudaMemcpyHostToDevice, m->stream));
-  b2s_status st = run_correlate(m, search, true, k_first, k_count, 1);
+  b2s_status st = run_correlate(m, search, k_first, k_count, 1);
   if (st) return st;
   B2S_CUDA_CHECK(cudaMemcpyAsync(best, m->d_part_best, sizeof(double) * B, cudaMemcpyDeviceToHost, m->stream));
   B2S_CUDA_CHECK(cudaMemcpyAsync(probs, m->d_probs, sizeof(double) * plen * B, cudaMemcpyDeviceToHost, m->stream));
@@ -2038,7 +2037,7 @@ b2s_status b2s_matcher_correlate_scan_split(b2s_matcher *m, void *nccl_comm, int
   const int base = na_full / world, extra = na_full % world;  // contiguous, balanced (parallel.shard_bounds)
   const int k_first = rank * base + std::min(rank, extra), k_count = base + (rank < extra ? 1 : 0);
   B2S_CUDA_CHECK(cudaMemcpyAsync(m->d_centers, centers, sizeof(double) * 3 * B, cudaMemcpyHostToDevice, m->stream));
-  b2s_status st = run_correlate(m, search, true, k_first, k_count, 1);
+  b2s_status st = run_correlate(m, search, k_first, k_count, 1);
   if (st) return st;
   k_status_pack<<<ceil_div(B, 128), 128, 0, m->stream>>>(m->d_results, m->d_status, B);
   auto check_nccl = [&](int rc, const char *what) -> b2s_status {
@@ -2124,8 +2123,7 @@ b2s_status b2s_matcher_last_timing(b2s_matcher *m, double out[4]) {
 namespace b2s {
 
 // One CorrelateScan over the batch with centres already in d_centers.  Results stay in d_results.
-static b2s_status run_correlate(b2s_matcher *m, const b2s_search *s, bool /*centers_on_device*/, int k_first, int na_override,
-                                int mode) {
+static b2s_status run_correlate(b2s_matcher *m, const b2s_search *s, int k_first, int na_override, int mode) {
   B2S_NVTX("K1 correlate (lists + sweep + tail)");
   if (s->angle_res == 0.0 || s->res_x == 0.0 || s->res_y == 0.0)
     B2S_FAIL(B2S_ERR_BAD_PARAMS, "search resolutions must be non-zero");  // assert at Mapper.cpp:319
@@ -2159,7 +2157,7 @@ static b2s_status run_correlate(b2s_matcher *m, const b2s_search *s, bool /*cent
   static size_t win_static = 0;
   if (!win_static) {
     cudaFuncAttributes fa;
-    B2S_CUDA_CHECK(cudaFuncGetAttributes(&fa, k_sweep_window<1, false, WIN_THREADS>));
+    B2S_CUDA_CHECK(cudaFuncGetAttributes(&fa, k_sweep_window<1, false>));
     win_static = fa.sharedSizeBytes;
   }
   const long long smem_limit = (long long)m->smem_optin - (long long)win_static - 512;
@@ -2231,23 +2229,16 @@ static b2s_status run_correlate(b2s_matcher *m, const b2s_search *s, bool /*cent
     // the GEN = false instantiation assumes exactly two lanes per row-start bank (see win_load)
     const int bank_step = ((m->g.width_step >> 2) * std::max(stride, 1)) & 31;
     const bool gen = (bank_step & 3) != 2;
-    // tuning switch: B2S_WIN_THREADS=384 runs the sweep with 12 warps per SM (leaves registers for co-resident kernels)
-    static const int win_threads = [] { const char *e = getenv("B2S_WIN_THREADS"); return (e && atoi(e) == 384) ? 384 : WIN_THREADS; }();
-    auto launch = [&](auto kern, int threads) -> b2s_status {
+    auto launch = [&](auto kern) -> b2s_status {
       B2S_CUDA_CHECK(raise_dyn_smem(kern, win_smem));
-      kern<<<ctas, threads, win_smem, m->stream>>>(m->d_grids, m->grid_pitch, m->g.data_size, copy_bytes, m->d_lists,
-                                                   m->d_counts, m->d_starts, m->d_flags, B, n, na, nx, ny,
-                                                   m->g.width_step, m->d_sums, m->d_work, band_rows, nbands,
-                                                   band_bytes, neg_bands);
+      kern<<<ctas, WIN_THREADS, win_smem, m->stream>>>(m->d_grids, m->grid_pitch, m->g.data_size, copy_bytes, m->d_lists,
+                                                       m->d_counts, m->d_starts, m->d_flags, B, n, na, nx, ny,
+                                                       m->g.width_step, m->d_sums, m->d_work, band_rows, nbands,
+                                                       band_bytes, neg_bands);
       return B2S_OK;
     };
-    if (win_threads == 384) {
-      if (stride == 2) st = gen ? launch(k_sweep_window<2, true, 384>, 384) : launch(k_sweep_window<2, false, 384>, 384);
-      else st = gen ? launch(k_sweep_window<1, true, 384>, 384) : launch(k_sweep_window<1, false, 384>, 384);
-    } else {
-      if (stride == 2) st = gen ? launch(k_sweep_window<2, true, WIN_THREADS>, WIN_THREADS) : launch(k_sweep_window<2, false, WIN_THREADS>, WIN_THREADS);
-      else st = gen ? launch(k_sweep_window<1, true, WIN_THREADS>, WIN_THREADS) : launch(k_sweep_window<1, false, WIN_THREADS>, WIN_THREADS);
-    }
+    if (stride == 2) st = gen ? launch(k_sweep_window<2, true>) : launch(k_sweep_window<2, false>);
+    else st = gen ? launch(k_sweep_window<1, true>) : launch(k_sweep_window<1, false>);
     if (st) return st;
     // matches whose lattice is not the regular raster (a centre exactly on a rounding tie) fall through;
     // they compute their lookup values on the fly (no table was materialised for them)
