@@ -290,6 +290,31 @@ struct NvtxRange {
 };
 #define B2S_NVTX(name) ::b2s::NvtxRange _b2s_nvtx_range("b2s:" name)
 
+// ---- mbarrier (shared-memory transaction barrier) wrappers: the Karto window sweep waits on its TMA copies with them,
+// the Hector cluster match on the partial sums its peers send ----
+__device__ __forceinline__ uint32_t smem_u32(const void *p) { return (uint32_t)__cvta_generic_to_shared(p); }
+__device__ __forceinline__ void mbar_init(uint64_t *bar, int count) {
+  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count));
+}
+__device__ __forceinline__ void fence_mbar_init() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
+__device__ __forceinline__ void mbar_expect_tx(uint64_t *bar, uint32_t bytes) {
+  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
+}
+// true once the phase of `parity` has completed; the instruction itself suspends the thread for a while before it says no
+__device__ __forceinline__ bool mbar_try_wait(uint64_t *bar, uint32_t parity) {
+  uint32_t done;
+  asm volatile(
+      "{\n\t"
+      ".reg .pred p;\n\t"
+      "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
+      "selp.u32 %0, 1, 0, p;\n\t"
+      "}\n"
+      : "=r"(done)
+      : "r"(smem_u32(bar)), "r"(parity)
+      : "memory");
+  return done != 0;
+}
+
 inline int ceil_div(long long a, long long b) { return (int)((a + b - 1) / b); }
 
 // SMs of `device` (132 on an H100 SXM): grid-stride kernels size their grids as a multiple of it.

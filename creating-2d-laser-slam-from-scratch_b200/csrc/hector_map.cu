@@ -22,6 +22,11 @@
 // parallel, then thread 0 accumulates H and dTr in point order (the reference's float32 summation order).
 //
 // HBM layout per cell: logOdds f32, updateIndex i32 (the reference's LogOddsCell, split SoA), + two u64 stamps.
+//
+// Shared with the processor (hector_slam.cu) through hector_grid.cuh: the map transform, the begin / end cells, the
+// Bresenham set-up and step, the bilinear bounds test and finish, the 3x3 solve, normalize_angle and the ROS map.
+// This handle's own: 64-bit stamps and a per-beam apply pass, the begin cell on the host, the updateByScanJustOnce end
+// cell, probabilities through the float expf and log-odds factors through logf.
 #include <algorithm>
 #include <cmath>
 #include <cstring>
@@ -29,6 +34,7 @@
 #include <vector>
 
 #include "common.cuh"
+#include "hector_grid.cuh"
 
 using namespace b2s;
 
@@ -36,8 +42,7 @@ struct b2s_hector_map {
   Stream stream;
   int device = 0;
   int sx = 0, sy = 0;
-  float cell_length = 0, scale_to_map = 0, off_x = 0, off_y = 0;
-  float tw_lin = 0, tw_tx = 0, tw_ty = 0, wt_lin = 0, wt_tx = 0, wt_ty = 0;
+  MapTransform tf = {};
   float lo_free = 0, lo_occ = 0;
   int curr_update_index = 0;
   unsigned int epoch = 0;
@@ -53,76 +58,35 @@ struct b2s_hector_map {
 
 namespace b2s {
 
-static float prob_to_log_odds(float prob) {  // GridMapLogOdds.h:153-157
-  float odds = prob / (1.0f - prob);
-  return logf(odds);
-}
-
-struct HcTransform {
-  float c, s, mx, my;  // poseTransform = Translation2f(mx, my) * Rotation2Df(theta)
-  int just_once;       // updateByScanJustOnce: end = begin + (int)round(p / 0.05) (OccGridMapBase.h:202-203)
-};
-
-__device__ __forceinline__ void hc_apply(const HcTransform &t, float px, float py, float &ox, float &oy) {
-  ox = __fadd_rn(__fadd_rn(__fmul_rn(t.c, px), __fmul_rn(-t.s, py)), t.mx);
-  oy = __fadd_rn(__fadd_rn(__fmul_rn(t.s, px), __fmul_rn(t.c, py)), t.my);
-}
-
-struct HcLine {
-  bool ok;
-  int x0, y0, x1, y1;
-  unsigned int da, db;
-  int err0, off_a, off_b;
-};
-
-// endpoints (OccGridMapBase.h:127-154) + updateLineBresenhami set-up (:220-258)
-__device__ __forceinline__ HcLine hc_line(const HcTransform &t, int bx, int by, float px, float py, int sx, int sy) {
-  HcLine L;
-  float ex, ey;
-  hc_apply(t, px, py, ex, ey);
-  ex = __fadd_rn(ex, 0.5f);
-  ey = __fadd_rn(ey, 0.5f);
-  L.x0 = bx; L.y0 = by;
-  L.x1 = (int)ex; L.y1 = (int)ey;  // Vector2f::cast<int>(): truncation
-  if (t.just_once) {  // points in metres; float / double literal -> double, ::round, (int)
-    L.x1 = bx + cast_i32(round((double)px / 0.05));
-    L.y1 = by + cast_i32(round((double)py / 0.05));
-  }
-  L.ok = !(L.x0 == L.x1 && L.y0 == L.y1);
-  if ((L.x0 < 0) || (L.x0 >= sx) || (L.y0 < 0) || (L.y0 >= sy)) L.ok = false;
-  if ((L.x1 < 0) || (L.x1 >= sx) || (L.y1 < 0) || (L.y1 >= sy)) L.ok = false;
-  const int dx = L.x1 - L.x0, dy = L.y1 - L.y0;
-  const unsigned int adx = (unsigned int)abs(dx), ady = (unsigned int)abs(dy);
-  const int odx = dx > 0 ? 1 : -1, ody = (dy > 0 ? 1 : -1) * sx;  // util::sign: sign(0) = -1
-  if (adx >= ady) { L.da = adx; L.db = ady; L.err0 = (int)(adx / 2); L.off_a = odx; L.off_b = ody; }
-  else { L.da = ady; L.db = adx; L.err0 = (int)(ady / 2); L.off_a = ody; L.off_b = odx; }
-  return L;
+// end cell + updateLineBresenhami set-up.  updateByScanJustOnce (OccGridMapBase.h:182-203) takes its end cell as
+// begin + (int)round(p / 0.05) on the raw points in metres: float / double literal -> double, ::round, (int).
+__device__ __forceinline__ BresenhamLine hc_line(float c, float s, float mx, float my, bool just_once, int bx, int by,
+                                                 float px, float py, int sx, int sy) {
+  const int2 end = just_once ? make_int2(bx + cast_i32(round((double)px / 0.05)), by + cast_i32(round((double)py / 0.05)))
+                             : end_cell(c, s, mx, my, px, py);
+  return bresenham_line(bx, by, end, sx, sy);
 }
 
 // pass 1: record, per traversed cell, the lowest beam index that frees it / ends on it
 __global__ void __launch_bounds__(256)
-    k_hc_mark(const float *__restrict__ pts, int n, HcTransform t, int bx, int by, int sx, int sy,
+    k_hc_mark(const float *__restrict__ pts, int n, float c, float s, float mx, float my, bool just_once, int bx, int by, int sx, int sy,
               unsigned long long epoch_hi, unsigned long long *__restrict__ free_st,
               unsigned long long *__restrict__ occ_st) {
   const int lane = threadIdx.x & 31;
   const int warp0 = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, nwarps = (gridDim.x * blockDim.x) >> 5;
   for (int i = warp0; i < n; i += nwarps) {
-    const HcLine L = hc_line(t, bx, by, pts[2 * i], pts[2 * i + 1], sx, sy);
+    const BresenhamLine L = hc_line(c, s, mx, my, just_once, bx, by, pts[2 * i], pts[2 * i + 1], sx, sy);
     if (!L.ok) continue;
     const unsigned long long stamp = epoch_hi | (unsigned long long)(0xffffffffu - (unsigned int)i);
     const int start = L.y0 * sx + L.x0;
-    for (unsigned int k = lane; k < L.da; k += 32) {  // bresenham2D: da cells from the start, end excluded
-      const unsigned int inc = (unsigned int)(((unsigned long long)L.err0 + (unsigned long long)k * L.db) / L.da);
-      const int off = start + (int)k * L.off_a + (int)inc * L.off_b;
-      atomicMax(free_st + off, stamp);
-    }
+    for (unsigned int k = lane; k < L.da; k += 32) atomicMax(free_st + bresenham_offset(L, start, k), stamp);
     if (lane == 0) atomicMax(occ_st + (L.y1 * sx + L.x1), stamp);
   }
 }
 
 // pass 2: the winner beam of each cell applies the reference's update exactly once
 __global__ void __launch_bounds__(256)
-    k_hc_apply(const float *__restrict__ pts, int n, HcTransform t, int bx, int by, int sx, int sy,
+    k_hc_apply(const float *__restrict__ pts, int n, float c, float s, float mx, float my, bool just_once, int bx, int by, int sx, int sy,
                unsigned long long epoch_hi, const unsigned long long *__restrict__ free_st,
                const unsigned long long *__restrict__ occ_st, float lo_free, float lo_occ, int mark_free, int mark_occ,
                float *__restrict__ lo, int32_t *__restrict__ ui, unsigned long long *__restrict__ visits) {
@@ -130,13 +94,12 @@ __global__ void __launch_bounds__(256)
   const int warp0 = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, nwarps = (gridDim.x * blockDim.x) >> 5;
   unsigned long long my_visits = 0;
   for (int i = warp0; i < n; i += nwarps) {
-    const HcLine L = hc_line(t, bx, by, pts[2 * i], pts[2 * i + 1], sx, sy);
+    const BresenhamLine L = hc_line(c, s, mx, my, just_once, bx, by, pts[2 * i], pts[2 * i + 1], sx, sy);
     if (!L.ok) continue;
     const unsigned long long stamp = epoch_hi | (unsigned long long)(0xffffffffu - (unsigned int)i);
     const int start = L.y0 * sx + L.x0;
     for (unsigned int k = lane; k < L.da; k += 32) {
-      const unsigned int inc = (unsigned int)(((unsigned long long)L.err0 + (unsigned long long)k * L.db) / L.da);
-      const int off = start + (int)k * L.off_a + (int)inc * L.off_b;
+      const int off = bresenham_offset(L, start, k);
       my_visits++;
       if (free_st[off] == stamp && (occ_st[off] >> 32) != (epoch_hi >> 32)) {
         // freed this scan, never an end point: bresenhamCellFree (OccGridMapBase.h:302-312)
@@ -167,39 +130,20 @@ __global__ void __launch_bounds__(256)
 
 // ---- K3: Gauss-Newton scan-to-map alignment (one grid level), whole iteration loop in one launch ----
 
-__device__ __forceinline__ float hc_prob(const float *__restrict__ lo, int index) {  // GridMapLogOdds.h:136-140
+// getGridProbability (GridMapLogOdds.h:136-140) with the device's float expf, where the reference rounds the C library's
+// double exp to float (as the processor's hs_prob_of does): the values can differ in the last bits, which is why
+// b2s_hector_map_match_data is held to 1e-4 of the reference rather than bit for bit.
+__device__ __forceinline__ float hc_prob(const float *__restrict__ lo, int index) {
   const float odds = expf(lo[index]);
   return odds / (odds + 1.0f);
 }
 
 __device__ __forceinline__ void hc_interp(const float *__restrict__ lo, int sx, int sy, float x, float y, float out[3]) {
-  const float lim_x = (float)sx - 2.0f, lim_y = (float)sy - 2.0f;  // setMapCellDims: dims - 2
-  if (x < 0.0f || x > lim_x || y < 0.0f || y > lim_y) { out[0] = out[1] = out[2] = 0.0f; return; }
+  if (!interp_inside(sx, sy, x, y)) { out[0] = out[1] = out[2] = 0.0f; return; }
   const int ix = (int)x, iy = (int)y;
-  const float fx = x - (float)ix, fy = y - (float)iy;
   const int index = iy * sx + ix;
-  const float i0 = hc_prob(lo, index), i1 = hc_prob(lo, index + 1);
-  const float i2 = hc_prob(lo, index + sx), i3 = hc_prob(lo, index + sx + 1);
-  const float dx1 = i0 - i1, dx2 = i2 - i3, dy1 = i0 - i2, dy2 = i1 - i3;
-  const float xfi = 1.0f - fx, yfi = 1.0f - fy;
-  out[0] = ((i0 * xfi + i1 * fx) * yfi) + ((i2 * xfi + i3 * fx) * fy);
-  out[1] = -((dx1 * yfi) + (dx2 * fy));
-  out[2] = -((dy1 * xfi) + (dy2 * fx));
-}
-
-__device__ inline void hc_inv3_mul(const float m[9], const float v[3], float out[3]) {  // Matrix3f::inverse() * v
-  const float c00 = m[4] * m[8] - m[5] * m[7], c10 = m[5] * m[6] - m[3] * m[8], c20 = m[3] * m[7] - m[4] * m[6];
-  const float det = c00 * m[0] + (c10 * m[1] + c20 * m[2]);  /* Eigen's unrolled 3-term redux: a0 + (a1 + a2) */
-  const float invdet = 1.0f / det;
-  float inv[9];
-  inv[0] = c00 * invdet; inv[3] = c10 * invdet; inv[6] = c20 * invdet;
-  inv[1] = (m[2] * m[7] - m[1] * m[8]) * invdet;
-  inv[4] = (m[0] * m[8] - m[2] * m[6]) * invdet;
-  inv[7] = (m[1] * m[6] - m[0] * m[7]) * invdet;
-  inv[2] = (m[1] * m[5] - m[2] * m[4]) * invdet;
-  inv[5] = (m[2] * m[3] - m[0] * m[5]) * invdet;
-  inv[8] = (m[0] * m[4] - m[1] * m[3]) * invdet;
-  for (int r = 0; r < 3; r++) out[r] = inv[3 * r] * v[0] + (inv[3 * r + 1] * v[1] + inv[3 * r + 2] * v[2]);
+  interp_finish(hc_prob(lo, index), hc_prob(lo, index + 1), hc_prob(lo, index + sx), hc_prob(lo, index + sx + 1),
+                x - (float)ix, y - (float)iy, out);
 }
 
 constexpr int GN_THREADS = 512;
@@ -207,7 +151,7 @@ constexpr int GN_CHUNK = 1024;  // points staged per pass
 
 __global__ void __launch_bounds__(GN_THREADS)
     k_hc_match(const float *__restrict__ lo, int sx, int sy, const float *__restrict__ pts, int n, float e0, float e1,
-               float e2, int iterations, float wt_lin, float wt_tx, float wt_ty, float *__restrict__ out) {
+               float e2, int iterations, MapTransform tf, float *__restrict__ out) {
   __shared__ float terms[GN_CHUNK][4];  // t1, t2, rotDeriv, funVal per point
   __shared__ float est[3];
   __shared__ float H[9], dTr[3];
@@ -253,7 +197,7 @@ __global__ void __launch_bounds__(GN_THREADS)
       H[3] = H[1]; H[6] = H[2]; H[7] = H[5];
       if (H[0] != 0.0f && H[4] != 0.0f) {  // estimateTransformationLogLh (ScanMatcher.h:107-141)
         float dir[3];
-        hc_inv3_mul(H, dTr, dir);
+        inv3_mul(H, dTr, dir);
         if (dir[2] > 0.2f) dir[2] = 0.2f;
         else if (dir[2] < -0.2f) dir[2] = -0.2f;
         est[0] += dir[0]; est[1] += dir[1]; est[2] += dir[2];
@@ -262,26 +206,11 @@ __global__ void __launch_bounds__(GN_THREADS)
     __syncthreads();
   }
   if (threadIdx.x == 0) {
-    // util::normalize_angle (UtilFunctions.h:36-48): double fmod, float result
-    const double two_pi = 2.0f * 3.14159265358979323846;
-    float a = (float)fmod(fmod((double)est[2], two_pi) + two_pi, two_pi);
-    if (a > 3.14159265358979323846) a = (float)((double)a - two_pi);  // `a -= 2.0f*M_PI` promotes to double
-    // getWorldCoordsPose (GridMapBase.h:229-233)
-    out[0] = (wt_lin * est[0] + (-0.0f) * est[1]) + wt_tx;
-    out[1] = ((-0.0f) * est[0] + wt_lin * est[1]) + wt_ty;
-    out[2] = a;
+    get_world_coords(tf, est[0], est[1], out[0], out[1]);
+    out[2] = util_normalize_angle(est[2]);
     for (int q = 0; q < 9; q++) out[3 + q] = H[q];
   }
 }
-
-// HectorMappingRos::publishMap (hector_slam.cc:254-317): free -> 0, occupied -> 100, else -1
-__global__ void k_hc_ros(const float *__restrict__ lo, int n, int8_t *__restrict__ out) {
-  int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= n) return;
-  const float v = lo[i];
-  out[i] = v < 0.0f ? 0 : (v > 0.0f ? 100 : -1);
-}
-
 
 }  // namespace b2s
 
@@ -297,23 +226,11 @@ b2s_status b2s_hector_map_create(int size_x, int size_y, float resolution, float
   if (!m) B2S_FAIL(B2S_ERR_CUDA, "out of host memory");
   m->device = device;
   m->sx = size_x; m->sy = size_y;
-  // MapRepMultiMap ctor (MapRepMultiMap.h:63-67) + GridMapBase::setMapTransformation (GridMapBase.h:270-286)
+  // MapRepMultiMap ctor (MapRepMultiMap.h:63-67): the map's offset
   const float total_x = resolution * (float)size_x, total_y = resolution * (float)size_y;
-  m->off_x = total_x * start_x;
-  m->off_y = total_y * start_y;
-  m->cell_length = resolution;
-  m->scale_to_map = 1.0f / resolution;
-  m->tw_lin = m->scale_to_map;  // AlignedScaling2f(s,s) * Translation2f(off): linear diag(s,s), translation s*off
-  m->tw_tx = m->scale_to_map * m->off_x;
-  m->tw_ty = m->scale_to_map * m->off_y;
-  const float det = m->tw_lin * m->tw_lin - 0.0f * 0.0f;  // Affine inverse, cofactor form
-  const float invdet = 1.0f / det;
-  m->wt_lin = m->tw_lin * invdet;
-  const float i01 = -0.0f * invdet;
-  m->wt_tx = -(m->wt_lin * m->tw_tx + i01 * m->tw_ty);
-  m->wt_ty = -(i01 * m->tw_tx + m->wt_lin * m->tw_ty);
-  m->lo_free = prob_to_log_odds(0.4f);  // GridMapLogOdds.h:98-102
-  m->lo_occ = prob_to_log_odds(0.6f);
+  m->tf = map_transform(resolution, total_x * start_x, total_y * start_y);
+  m->lo_free = prob_to_log_odds_logf(0.4f);
+  m->lo_occ = prob_to_log_odds_logf(0.6f);
   B2S_CUDA_CHECK(m->stream.init(cuda_stream));
   for (auto &e : m->ev) B2S_CUDA_CHECK(e.create());
   const size_t cells = (size_t)size_x * size_y;
@@ -342,8 +259,8 @@ void b2s_hector_map_destroy(b2s_hector_map *m) {
 
 b2s_status b2s_hector_map_set_factors(b2s_hector_map *m, float update_free, float update_occupied) {
   if (!m) B2S_FAIL(B2S_ERR_BAD_PARAMS, "null handle");
-  m->lo_free = prob_to_log_odds(update_free);
-  m->lo_occ = prob_to_log_odds(update_occupied);
+  m->lo_free = prob_to_log_odds_logf(update_free);
+  m->lo_occ = prob_to_log_odds_logf(update_occupied);
   return B2S_OK;
 }
 
@@ -359,18 +276,12 @@ static b2s_status hc_update(b2s_hector_map *m, const float *points, int n_points
   if (!m || !origo || !world_pose || n_points < 0 || (n_points > 0 && !points)) B2S_FAIL(B2S_ERR_BAD_PARAMS, "null argument");
   B2S_CUDA_CHECK(cudaSetDevice(m->device));
   const int mark_free = m->curr_update_index + 1, mark_occ = m->curr_update_index + 2;  // OccGridMapBase.h:120-121
-  // getMapCoordsPose (GridMapBase.h:238-242)
-  float mx = (m->tw_lin * world_pose[0] + 0.0f * world_pose[1]) + m->tw_tx;
-  float my = (0.0f * world_pose[0] + m->tw_lin * world_pose[1]) + m->tw_ty;
+  float mx, my;
+  get_map_coords(m->tf, world_pose[0], world_pose[1], mx, my);
   float heading = world_pose[2];
   if (just_once) { mx = 800.0f; my = 800.0f; heading = 0.0f; }  // Eigen::Vector3f mapPose(800, 800, 0) (OccGridMapBase.h:182)
-  HcTransform t;
-  t.c = cosf(heading);  // Rotation2Df: std::cos / std::sin on float, taken on the host (glibc)
-  t.s = sinf(heading);
-  t.just_once = just_once ? 1 : 0;
-  t.mx = mx; t.my = my;
-  const float bxf = (t.c * origo[0] + (-t.s) * origo[1]) + mx, byf = (t.s * origo[0] + t.c * origo[1]) + my;
-  const int bx = (int)(bxf + 0.5f), by = (int)(byf + 0.5f);  // Vector2i(float, float): truncation
+  const float c = cosf(heading), s = sinf(heading);  // Rotation2Df: std::cos / std::sin on float, taken on the host (glibc)
+  const int2 b0 = begin_cell(c, s, mx, my, origo[0], origo[1]);
   m->epoch++;
   const unsigned long long epoch_hi = (unsigned long long)m->epoch << 32;
   if (n_points > 0) {
@@ -379,8 +290,10 @@ static b2s_status hc_update(b2s_hector_map *m, const float *points, int n_points
     B2S_CUDA_CHECK(cudaMemsetAsync(m->d_visits, 0, sizeof(unsigned long long), m->stream));
     const int blocks = std::min(ceil_div(n_points, 8), sm_count(m->device) * 8);
     B2S_CUDA_CHECK(cudaEventRecord(m->ev[0], m->stream));
-    k_hc_mark<<<blocks, 256, 0, m->stream>>>(m->d_pts, n_points, t, bx, by, m->sx, m->sy, epoch_hi, m->d_free, m->d_occ);
-    k_hc_apply<<<blocks, 256, 0, m->stream>>>(m->d_pts, n_points, t, bx, by, m->sx, m->sy, epoch_hi, m->d_free, m->d_occ,
+    k_hc_mark<<<blocks, 256, 0, m->stream>>>(m->d_pts, n_points, c, s, mx, my, just_once, b0.x, b0.y, m->sx, m->sy, epoch_hi,
+                                             m->d_free, m->d_occ);
+    k_hc_apply<<<blocks, 256, 0, m->stream>>>(m->d_pts, n_points, c, s, mx, my, just_once, b0.x, b0.y, m->sx, m->sy, epoch_hi,
+                                              m->d_free, m->d_occ,
                                               m->lo_free, m->lo_occ, mark_free, mark_occ, m->d_lo, m->d_ui, m->d_visits);
     B2S_CUDA_CHECK(cudaEventRecord(m->ev[1], m->stream));
     B2S_CUDA_CHECK(cudaGetLastError());
@@ -412,11 +325,11 @@ b2s_status b2s_hector_map_match_data(b2s_hector_map *m, const float *points, int
   B2S_CUDA_CHECK(cudaSetDevice(m->device));
   b2s_status st = hc_upload_points(m, points, n_points);
   if (st) return st;
-  const float e0 = (m->tw_lin * begin_world_pose[0] + 0.0f * begin_world_pose[1]) + m->tw_tx;
-  const float e1 = (0.0f * begin_world_pose[0] + m->tw_lin * begin_world_pose[1]) + m->tw_ty;
+  float e0, e1;
+  get_map_coords(m->tf, begin_world_pose[0], begin_world_pose[1], e0, e1);
   B2S_CUDA_CHECK(cudaEventRecord(m->ev[2], m->stream));
   k_hc_match<<<1, GN_THREADS, 0, m->stream>>>(m->d_lo, m->sx, m->sy, m->d_pts, n_points, e0, e1, begin_world_pose[2],
-                                              1 + max_iterations, m->wt_lin, m->wt_tx, m->wt_ty, m->d_out);
+                                              1 + max_iterations, m->tf, m->d_out);
   B2S_CUDA_CHECK(cudaEventRecord(m->ev[3], m->stream));
   B2S_CUDA_CHECK(cudaGetLastError());
   float host[12];
@@ -445,7 +358,7 @@ b2s_status b2s_hector_map_copy_ros(b2s_hector_map *m, int8_t *out) {
   const int n = m->sx * m->sy;
   AsyncBuf<int8_t> d(m->stream);
   B2S_CUDA_CHECK(d.alloc((size_t)n));
-  k_hc_ros<<<ceil_div(n, 256), 256, 0, m->stream>>>(m->d_lo, n, d);
+  k_hector_ros<<<ceil_div(n, 256), 256, 0, m->stream>>>(m->d_lo, n, d);
   B2S_CUDA_CHECK(cudaGetLastError());
   B2S_CUDA_CHECK(cudaMemcpyAsync(out, d, (size_t)n, cudaMemcpyDeviceToHost, m->stream));
   B2S_CUDA_CHECK(cudaStreamSynchronize(m->stream));

@@ -27,6 +27,11 @@
 // ~1e-16 relative of a float rounding boundary: ~5e-9 per evaluation).  FAST mode differs in ONE thing: the nine sums are
 // tree-reduced (warp shuffles) instead of accumulated in point order, so its Hessians / poses differ in the last float bits
 // (~1e-6 m per scan, inside the 1e-4 contract) and a cell can move when a pose lands an ulp away.
+//
+// The grid arithmetic it shares with the single-map handle (hector_map.cu) is in hector_grid.cuh: map transform, begin /
+// end cells, Bresenham set-up and step, bilinear bounds test and finish, 3x3 solve, normalize_angle, ROS map, log-odds
+// factors.  Its own: the pyramid, the probability quads (double exp), 32-bit stamps with the bounding-box apply sweep,
+// the begin cell on the device, and the match's two-halves fetch.
 #include <algorithm>
 #include <atomic>
 #include <cmath>
@@ -39,6 +44,7 @@
 
 #include "common.cuh"
 #include "glibc_math.cuh"
+#include "hector_grid.cuh"
 
 using namespace b2s;
 
@@ -61,7 +67,7 @@ struct HsLevel {  // one MapRepMultiMap level, all B processors ([b][cells] plan
   uint32_t *free_st, *occ_st;  // per-scan stamps: (epoch << 12) | (4095 - beam)
   float *pts;                  // [b][cap][2] data container of this level (level 0: the current scan)
   int sx, sy;
-  float tw_lin, tw_tx, tw_ty, wt_lin, wt_tx, wt_ty;
+  MapTransform tf;
   int iterations;  // 1 + maxIterations of MapRepMultiMap::matchData (:144-166): 1+5 on level 0, 1+3 above
 };
 
@@ -120,11 +126,10 @@ __device__ __forceinline__ unsigned long long hs_now_ns() {
 constexpr int HS_CLUSTER = 4;
 constexpr int HS_POSE_WORDS = 7;  // e0, e1, cos, sin, sinRot, cosRot, spare
 struct __align__(16) HsXchg {
-  unsigned long long bar_pose, bar_part;  // mbarriers: pose arrived (helpers) / all partial sums arrived (master)
+  uint64_t bar_pose, bar_part;  // mbarriers: pose arrived (helpers) / all partial sums arrived (master)
   float pose[8];
   float part[HS_CLUSTER][12];             // [rank][sum]
 };
-__device__ __forceinline__ uint32_t hs_smem_u32(const void *p) { return (uint32_t)__cvta_generic_to_shared(p); }
 __device__ __forceinline__ uint32_t hs_cluster_rank() { uint32_t r; asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r)); return r; }
 __device__ __forceinline__ uint32_t hs_cluster_size() { uint32_t r; asm volatile("mov.u32 %0, %%cluster_nctarank;" : "=r"(r)); return r; }
 __device__ __forceinline__ uint32_t hs_mapa(uint32_t addr, uint32_t rank) {
@@ -137,30 +142,12 @@ __device__ __forceinline__ void hs_st_async(uint32_t remote_addr, float v, uint3
                "r"(__float_as_uint(v)), "r"(remote_bar)
                : "memory");
 }
-__device__ __forceinline__ void hs_mbar_init(unsigned long long *bar, int count) {
-  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(hs_smem_u32(bar)), "r"(count));
-}
-__device__ __forceinline__ void hs_mbar_expect_tx(unsigned long long *bar, uint32_t bytes) {
-  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(hs_smem_u32(bar)), "r"(bytes) : "memory");
-}
 // bounded: a lost exchange must not hang the device (the host reports B2S_ERR_CUDA when the flag is set)
-__device__ __forceinline__ bool hs_mbar_wait(unsigned long long *bar, uint32_t parity) {
-  const uint32_t addr = hs_smem_u32(bar);
+__device__ __forceinline__ bool mbar_wait_bounded(uint64_t *bar, uint32_t parity) {
   const long long t0 = clock64();
-  while (true) {
-    uint32_t done;
-    asm volatile(
-        "{\n\t"
-        ".reg .pred p;\n\t"
-        "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
-        "selp.u32 %0, 1, 0, p;\n\t"
-        "}\n"
-        : "=r"(done)
-        : "r"(addr), "r"(parity)
-        : "memory");
-    if (done) return true;
+  while (!mbar_try_wait(bar, parity))
     if (clock64() - t0 > (1ll << 25)) return false;  // ~17 ms; a legitimate wait is microseconds
-  }
+  return true;
 }
 __device__ __forceinline__ void hs_cluster_sync() {
   asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
@@ -181,8 +168,7 @@ struct HsFetch {
 };
 __device__ __forceinline__ HsFetch hs_fetch(const float4 *__restrict__ quad, int sx, int sy, float x, float y) {
   HsFetch f;
-  const float lim_x = (float)sx - 2.0f, lim_y = (float)sy - 2.0f;  // setMapCellDims: dims - 2
-  f.inside = !(x < 0.0f || x > lim_x || y < 0.0f || y > lim_y);
+  f.inside = interp_inside(sx, sy, x, y);
   f.i0 = f.i1 = f.i2 = f.i3 = 0.0f; f.fx = f.fy = 0.0f;
   if (f.inside) {
     const int ix = (int)x, iy = (int)y;
@@ -194,26 +180,7 @@ __device__ __forceinline__ HsFetch hs_fetch(const float4 *__restrict__ quad, int
 }
 __device__ __forceinline__ void hs_finish(const HsFetch &f, float out[3]) {
   if (!f.inside) { out[0] = out[1] = out[2] = 0.0f; return; }
-  const float dx1 = f.i0 - f.i1, dx2 = f.i2 - f.i3, dy1 = f.i0 - f.i2, dy2 = f.i1 - f.i3;
-  const float xfi = 1.0f - f.fx, yfi = 1.0f - f.fy;
-  out[0] = ((f.i0 * xfi + f.i1 * f.fx) * yfi) + ((f.i2 * xfi + f.i3 * f.fx) * f.fy);
-  out[1] = -((dx1 * yfi) + (dx2 * f.fy));
-  out[2] = -((dy1 * xfi) + (dy2 * f.fx));
-}
-
-__device__ __forceinline__ void hs_inv3_mul(const float m[9], const float v[3], float out[3]) {  // Matrix3f::inverse() * v
-  const float c00 = m[4] * m[8] - m[5] * m[7], c10 = m[5] * m[6] - m[3] * m[8], c20 = m[3] * m[7] - m[4] * m[6];
-  const float det = c00 * m[0] + (c10 * m[1] + c20 * m[2]);  /* Eigen's unrolled 3-term redux: a0 + (a1 + a2) */
-  const float invdet = 1.0f / det;
-  float inv[9];
-  inv[0] = c00 * invdet; inv[3] = c10 * invdet; inv[6] = c20 * invdet;
-  inv[1] = (m[2] * m[7] - m[1] * m[8]) * invdet;
-  inv[4] = (m[0] * m[8] - m[2] * m[6]) * invdet;
-  inv[7] = (m[1] * m[6] - m[0] * m[7]) * invdet;
-  inv[2] = (m[1] * m[5] - m[2] * m[4]) * invdet;
-  inv[5] = (m[2] * m[3] - m[0] * m[5]) * invdet;
-  inv[8] = (m[0] * m[4] - m[1] * m[3]) * invdet;
-  for (int r = 0; r < 3; r++) out[r] = inv[3 * r] * v[0] + (inv[3 * r + 1] * v[1] + inv[3 * r + 2] * v[2]);
+  interp_finish(f.i0, f.i1, f.i2, f.i3, f.fx, f.fy, out);
 }
 
 // util::poseDifferenceLargerThan (UtilFunctions.h:72-90).  Only <cmath> is included there, so the unqualified
@@ -246,24 +213,6 @@ __device__ __forceinline__ void hs_point_terms(const HsFetch &f, float2 p, float
   a[6] = t[1] * t[2]; a[7] = t[1] * rot; a[8] = t[2] * rot;  // H01 H02 H12
 }
 
-// util::normalize_angle (UtilFunctions.h:36-48): double fmod, float result
-__device__ __noinline__ float hs_normalize_angle(float e2) {
-  const double two_pi = 2.0f * 3.14159265358979323846;
-  const double d = (double)e2;
-  double r;
-  if (fabs(d) < two_pi) {
-    // fmod(d, 2pi) = d here, and for x = d + 2pi in (0, 4pi): fmod(x, 2pi) = x - 2pi when x >= 2pi (exact: Sterbenz), else x.
-    // Bit for bit the reference's two fmod calls, without the two software remainder loops.
-    const double x = d + two_pi;
-    r = x >= two_pi ? x - two_pi : x;
-  } else {
-    r = fmod(fmod(d, two_pi) + two_pi, two_pi);
-  }
-  float a = (float)r;
-  if ((double)a > 3.14159265358979323846) a = (float)((double)a - two_pi);  // `a -= 2.0f*M_PI` promotes to double
-  return a;
-}
-
 struct HsTrig {
   float c, s;              // Rotation2Df(angle): std::cos / std::sin(float) = glibc cosf / sinf
   float sin_rot, cos_rot;  // OccGridMapUtil.h:87-88: the C library's double sin / cos, rounded to float
@@ -287,34 +236,6 @@ __device__ __noinline__ HsTrig hs_trig(float angle, bool exact, bool use_fma) {
     t.cos_rot = t.c;
   }
   return t;
-}
-
-struct HsLine {
-  bool ok;
-  int x0, y0, x1, y1;
-  unsigned int da, db;
-  int err0, off_a, off_b;
-};
-
-// endpoints (OccGridMapBase.h:127-154) + updateLineBresenhami set-up (:220-258)
-__device__ __forceinline__ HsLine hs_line(float c, float s, float mx, float my, int bx, int by, float px, float py, int sx,
-                                          int sy) {
-  HsLine L;
-  float ex = __fadd_rn(__fadd_rn(__fmul_rn(c, px), __fmul_rn(-s, py)), mx);
-  float ey = __fadd_rn(__fadd_rn(__fmul_rn(s, px), __fmul_rn(c, py)), my);
-  ex = __fadd_rn(ex, 0.5f);
-  ey = __fadd_rn(ey, 0.5f);
-  L.x0 = bx; L.y0 = by;
-  L.x1 = (int)ex; L.y1 = (int)ey;  // Vector2f::cast<int>(): truncation
-  L.ok = !(L.x0 == L.x1 && L.y0 == L.y1);
-  if ((L.x0 < 0) || (L.x0 >= sx) || (L.y0 < 0) || (L.y0 >= sy)) L.ok = false;
-  if ((L.x1 < 0) || (L.x1 >= sx) || (L.y1 < 0) || (L.y1 >= sy)) L.ok = false;
-  const int dx = L.x1 - L.x0, dy = L.y1 - L.y0;
-  const unsigned int adx = (unsigned int)abs(dx), ady = (unsigned int)abs(dy);
-  const int odx = dx > 0 ? 1 : -1, ody = (dy > 0 ? 1 : -1) * sx;  // util::sign: sign(0) = -1
-  if (adx >= ady) { L.da = adx; L.db = ady; L.err0 = (int)(adx / 2); L.off_a = odx; L.off_b = ody; }
-  else { L.da = ady; L.db = adx; L.err0 = (int)(ady / 2); L.off_a = ody; L.off_b = odx; }
-  return L;
 }
 
 // Fast mode, cluster variant: the per-point phase of this CTA's share (points [0, cnt) of `pts`) and the CTA's nine sums.
@@ -391,7 +312,7 @@ __device__ bool hs_match_cta(const HsBatch &P, const HsCall &C, int b, unsigned 
   // of warp 0 (the solving thread publishes nothing itself: 21 serial remote stores would sit on its critical path)
   auto publish = [&]() {
     if constexpr (CLUSTER) {
-      const uint32_t a_pose = hs_smem_u32(xc->pose), a_bar = hs_smem_u32(&xc->bar_pose);
+      const uint32_t a_pose = smem_u32(xc->pose), a_bar = smem_u32(&xc->bar_pose);
 #pragma unroll 1
       for (uint32_t l = (uint32_t)lane; l + HS_POSE_WORDS < HS_POSE_WORDS * csize; l += 32) {
         const uint32_t r = 1 + l / HS_POSE_WORDS, q = l % HS_POSE_WORDS;
@@ -432,10 +353,9 @@ __device__ bool hs_match_cta(const HsBatch &P, const HsCall &C, int b, unsigned 
       if (lv > 0)  // dataContainers[lv-1].setFrom(dataContainer, 2^-lv) (DataPointContainer.h:46-59): exact scaling
         for (int i = tid; i < n; i += HS_THREADS)
           reinterpret_cast<float2 *>(m.pts)[(size_t)b * P.cap + i] = make_float2(__fmul_rn(spts[i].x, factor), __fmul_rn(spts[i].y, factor));
-      // getMapCoordsPose (GridMapBase.h:238-242)
       if (tid == 0) {
-        const float e0 = (m.tw_lin * world0 + 0.0f * world1) + m.tw_tx;
-        const float e1 = (0.0f * world0 + m.tw_lin * world1) + m.tw_ty;
+        float e0, e1;
+        get_map_coords(m.tf, world0, world1, e0, e1);
         const HsTrig tr = hs_trig(world2, exact, use_fma);
         bc[0] = e0; bc[1] = e1; bc[2] = world2; bc[3] = tr.c; bc[4] = tr.s; bc[5] = tr.sin_rot; bc[6] = tr.cos_rot;
       }
@@ -450,8 +370,8 @@ __device__ bool hs_match_cta(const HsBatch &P, const HsCall &C, int b, unsigned 
           float v = hs_share_sums(prob, m.sx, m.sy, spts, my1, factor, e0, e1, c, s, sin_rot, cos_rot, terms, pitch, tid, lane, warp);
           if (warp < 9) {
             if (csize > 1) {  // + the helpers' partial sums, in rank order
-              if (tid == 0) hs_mbar_expect_tx(&xc->bar_part, 36u * (csize - 1));
-              if (!hs_mbar_wait(&xc->bar_part, part_parity)) s_lost = 1;  // every reading thread observes the phase itself
+              if (tid == 0) mbar_expect_tx(&xc->bar_part, 36u * (csize - 1));
+              if (!mbar_wait_bounded(&xc->bar_part, part_parity)) s_lost = 1;  // every reading thread observes the phase itself
 #pragma unroll 1
               for (uint32_t r = 1; r < csize; r++) v += xc->part[r][warp];
             }
@@ -547,7 +467,7 @@ __device__ bool hs_match_cta(const HsBatch &P, const HsCall &C, int b, unsigned 
           float n0 = bc[0], n1 = bc[1], n2 = bc[2];
           if (Hm[0] != 0.0f && Hm[4] != 0.0f) {
             float dir[3];
-            hs_inv3_mul(Hm, dTr, dir);
+            inv3_mul(Hm, dTr, dir);
             if (dir[2] > 0.2f) dir[2] = 0.2f;
             else if (dir[2] < -0.2f) dir[2] = -0.2f;
             n0 += dir[0]; n1 += dir[1]; n2 += dir[2];
@@ -566,9 +486,8 @@ __device__ bool hs_match_cta(const HsBatch &P, const HsCall &C, int b, unsigned 
       }
       {
         const float e0 = bc[0], e1 = bc[1], e2 = bc[2];
-        const float a = hs_normalize_angle(e2);
-        world0 = (m.wt_lin * e0 + (-0.0f) * e1) + m.wt_tx;  // getWorldCoordsPose (GridMapBase.h:229-233)
-        world1 = ((-0.0f) * e0 + m.wt_lin * e1) + m.wt_ty;
+        const float a = util_normalize_angle(e2);
+        get_world_coords(m.tf, e0, e1, world0, world1);
         world2 = a;
         any = true;
       }
@@ -610,12 +529,11 @@ __device__ bool hs_match_cta(const HsBatch &P, const HsCall &C, int b, unsigned 
       glibc_sincosf(est[2], use_fma, &us, &uc);
       for (int l = 0; l < P.levels; l++) {
         const HsLevel &m = P.l[l];
-        const float mx = (m.tw_lin * est[0] + 0.0f * est[1]) + m.tw_tx;  // getMapCoordsPose (GridMapBase.h:238-242)
-        const float my = (0.0f * est[0] + m.tw_lin * est[1]) + m.tw_ty;
+        float mx, my;
+        get_map_coords(m.tf, est[0], est[1], mx, my);
         st->uc[l] = uc; st->us[l] = us; st->umx[l] = mx; st->umy[l] = my;
-        const float bxf = (uc * st->origo[l][0] + (-us) * st->origo[l][1]) + mx;
-        const float byf = (us * st->origo[l][0] + uc * st->origo[l][1]) + my;
-        st->bx[l] = (int)(bxf + 0.5f); st->by[l] = (int)(byf + 0.5f);  // Vector2i(float, float): truncation
+        const int2 b0 = begin_cell(uc, us, mx, my, st->origo[l][0], st->origo[l][1]);
+        st->bx[l] = b0.x; st->by[l] = b0.y;
         st->epoch[l] += 1;
         st->epoch_hi[l] = st->epoch[l] << 12;
         st->mark_free[l] = st->curr_update_index[l] + 1;  // OccGridMapBase.h:120-121
@@ -653,7 +571,7 @@ __device__ bool hs_match_cta(const HsBatch &P, const HsCall &C, int b, unsigned 
       int lo_x = 2147483647, lo_y = 2147483647, hi_x = -2147483647, hi_y = -2147483647;
       for (int i = tid; i < nl; i += HS_THREADS) {
         const float2 pt = pp[i];
-        const HsLine ln = hs_line(c, s, mx, my, bx, by, pt.x, pt.y, m.sx, m.sy);
+        const BresenhamLine ln = bresenham_line(bx, by, end_cell(c, s, mx, my, pt.x, pt.y), m.sx, m.sy);
         if (!ln.ok) continue;
         lo_x = min(lo_x, min(ln.x0, ln.x1)); hi_x = max(hi_x, max(ln.x0, ln.x1));
         lo_y = min(lo_y, min(ln.y0, ln.y1)); hi_y = max(hi_y, max(ln.y0, ln.y1));
@@ -718,15 +636,15 @@ __device__ void hs_match_helper(const HsBatch &P, const HsCall &C, unsigned char
   for (int i = tid; i < cnt; i += HS_THREADS) spts[i] = gp[p0 + i];
   __syncthreads();
   const int pitch = hs_pitch(P.cap);
-  const uint32_t r_part = hs_mapa(hs_smem_u32(&xc->part[rank][0]), 0), r_bar = hs_mapa(hs_smem_u32(&xc->bar_part), 0);
+  const uint32_t r_part = hs_mapa(smem_u32(&xc->part[rank][0]), 0), r_bar = hs_mapa(smem_u32(&xc->bar_part), 0);
   float factor = 1.0f;
   for (int l = 1; l < P.levels; l++) factor *= 0.5f;
   for (int lv = P.levels - 1; lv >= 0; lv--, factor *= 2.0f) {
     const HsLevel &m = P.l[lv];
     const float4 *prob = m.quad;
     for (int it = 0; it < m.iterations; it++) {
-      if (tid == 0) hs_mbar_expect_tx(&xc->bar_pose, 4u * HS_POSE_WORDS);
-      hs_mbar_wait(&xc->bar_pose, pose_parity);  // every thread observes the phase itself (a time-out is reported by the master)
+      if (tid == 0) mbar_expect_tx(&xc->bar_pose, 4u * HS_POSE_WORDS);
+      mbar_wait_bounded(&xc->bar_pose, pose_parity);  // every thread observes the phase itself (a time-out is reported by the master)
       pose_parity ^= 1u;
       // Not needed for ordering — the master sends this pose only after it holds all nine sums of the previous iteration,
       // which are sent after the column reads — but that chain runs through another CTA, which compute-sanitizer's
@@ -786,14 +704,11 @@ __device__ unsigned long long hs_mark_pass(const HsBatch &P, int b, int w, int n
     const size_t cells = (size_t)m.sx * m.sy;
     uint32_t *fs = m.free_st + (size_t)b * cells, *os = m.occ_st + (size_t)b * cells;
     const float2 pt = __ldcg(reinterpret_cast<const float2 *>(m.pts) + (size_t)b * P.cap + i);
-    const HsLine ln = hs_line(u.c, u.s, u.mx, u.my, u.bx, u.by, pt.x, pt.y, m.sx, m.sy);
+    const BresenhamLine ln = bresenham_line(u.bx, u.by, end_cell(u.c, u.s, u.mx, u.my, pt.x, pt.y), m.sx, m.sy);
     if (!ln.ok) continue;
     const uint32_t stamp = u.ehi | (uint32_t)(4095 - i);
     const int start = ln.y0 * m.sx + ln.x0;
-    for (unsigned int k = lane; k < ln.da; k += 32) {  // bresenham2D: da cells from the start, end excluded
-      const unsigned int inc = (unsigned int)(((unsigned long long)ln.err0 + (unsigned long long)k * ln.db) / ln.da);
-      atomicMax(fs + (start + (int)k * ln.off_a + (int)inc * ln.off_b), stamp);
-    }
+    for (unsigned int k = lane; k < ln.da; k += 32) atomicMax(fs + bresenham_offset(ln, start, k), stamp);
     if (lane == 0) {
       atomicMax(os + (ln.y1 * m.sx + ln.x1), stamp);
       my_visits += (unsigned long long)ln.da + 1;
@@ -945,9 +860,9 @@ __global__ void __launch_bounds__(HS_THREADS, 1) k_hs_stream(HsBatch P, HsStream
     crank = hs_cluster_rank();
     csize = hs_cluster_size();
     if (threadIdx.x == 0) {
-      hs_mbar_init(&xc.bar_pose, 1);
-      hs_mbar_init(&xc.bar_part, 1);
-      asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+      mbar_init(&xc.bar_pose, 1);
+      mbar_init(&xc.bar_part, 1);
+      fence_mbar_init();
     }
     hs_cluster_sync();  // no peer signals a barrier that is not initialised yet (once per launch)
   }
@@ -1025,18 +940,6 @@ __global__ void k_hs_epoch_reset(HsState *st, int batch) {
   const int b = blockIdx.x * blockDim.x + threadIdx.x;
   if (b >= batch) return;
   for (int l = 0; l < HS_L; l++) st[b].epoch[l] = 0;
-}
-
-__global__ void k_hs_ros(const float *__restrict__ lo, int n, int8_t *__restrict__ out) {
-  int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= n) return;
-  const float v = lo[i];
-  out[i] = v < 0.0f ? 0 : (v > 0.0f ? 100 : -1);  // HectorMappingRos::publishMap (hector_slam.cc:254-317)
-}
-
-static float hs_prob_to_log_odds(float prob) {  // GridMapLogOdds.h:153-157
-  float odds = prob / (1.0f - prob);
-  return (float)log((double)odds);
 }
 
 }  // namespace b2s
@@ -1124,8 +1027,8 @@ static b2s_status hs_create(float map_resolution, int map_size_x, int map_size_y
   B2S_CUDA_CHECK(p->stream.init(cuda_stream));
   std::memset(&p->P, 0, sizeof(p->P));
   p->P.levels = levels; p->P.batch = batch; p->P.cap = max_points;
-  p->P.lo_free = hs_prob_to_log_odds(0.4f);  // GridMapLogOdds.h:98-102
-  p->P.lo_occ = hs_prob_to_log_odds(0.6f);
+  p->P.lo_free = prob_to_log_odds(0.4f);  // GridMapLogOdds.h:98-102
+  p->P.lo_occ = prob_to_log_odds(0.6f);
   p->P.min_dist = 0.4f; p->P.min_angle = 0.13f;  // HectorSlamProcessor.h:63-64
   p->P.exact = 1;
   const int variant = glibc_sincosf_variant_of_host();
@@ -1139,14 +1042,7 @@ static b2s_status hs_create(float map_resolution, int map_size_x, int map_size_y
     HsLevel &m = p->P.l[l];
     m.sx = sx; m.sy = sy;
     p->sx[l] = sx; p->sy[l] = sy; p->cell_length[l] = res;
-    // GridMapBase::setMapTransformation (GridMapBase.h:270-286): AlignedScaling2f(s,s) * Translation2f(off)
-    const float scale_to_map = 1.0f / res;
-    m.tw_lin = scale_to_map;
-    m.tw_tx = scale_to_map * off_x; m.tw_ty = scale_to_map * off_y;
-    const float det = m.tw_lin * m.tw_lin - 0.0f * 0.0f, invdet = 1.0f / det, i01 = -0.0f * invdet;  // Affine inverse, cofactor form
-    m.wt_lin = m.tw_lin * invdet;
-    m.wt_tx = -(m.wt_lin * m.tw_tx + i01 * m.tw_ty);
-    m.wt_ty = -(i01 * m.tw_tx + m.wt_lin * m.tw_ty);
+    m.tf = map_transform(res, off_x, off_y);
     m.iterations = 1 + (l == 0 ? 5 : 3);
     const size_t cells = (size_t)sx * sy * batch;
     auto &mem = p->level_mem[l];
@@ -1285,8 +1181,8 @@ void b2s_hector_slam_destroy(b2s_hector_slam *p) {
 
 b2s_status b2s_hector_slam_set_update_factors(b2s_hector_slam *p, float update_free, float update_occupied) {
   if (!p) B2S_FAIL(B2S_ERR_BAD_PARAMS, "null handle");
-  p->P.lo_free = hs_prob_to_log_odds(update_free);
-  p->P.lo_occ = hs_prob_to_log_odds(update_occupied);
+  p->P.lo_free = prob_to_log_odds(update_free);
+  p->P.lo_occ = prob_to_log_odds(update_occupied);
   return B2S_OK;
 }
 
@@ -1543,7 +1439,7 @@ b2s_status b2s_hector_slam_copy_level_ros(b2s_hector_slam *p, int level, int8_t 
   const int n = m.sx * m.sy;
   AsyncBuf<int8_t> d(p->stream);
   B2S_CUDA_CHECK(d.alloc((size_t)n));
-  k_hs_ros<<<ceil_div(n, 256), 256, 0, p->stream>>>(m.lo, n, d);
+  k_hector_ros<<<ceil_div(n, 256), 256, 0, p->stream>>>(m.lo, n, d);
   B2S_CUDA_CHECK(cudaGetLastError());
   B2S_CUDA_CHECK(cudaMemcpyAsync(out, d, (size_t)n, cudaMemcpyDeviceToHost, p->stream));
   B2S_CUDA_CHECK(cudaStreamSynchronize(p->stream));

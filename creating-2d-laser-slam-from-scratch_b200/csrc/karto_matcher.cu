@@ -48,27 +48,8 @@ std::string &last_error_ref() { return g_last_error; }
 // device helpers
 // ----------------------------------------------------------------------------------------------
 
-__device__ __forceinline__ uint32_t smem_u32(const void *p) { return (uint32_t)__cvta_generic_to_shared(p); }
-
-__device__ __forceinline__ void mbar_init(uint64_t *bar, int count) {
-  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count));
-}
-__device__ __forceinline__ void mbar_expect_tx(uint64_t *bar, uint32_t bytes) {
-  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
-}
 __device__ __forceinline__ void mbar_wait(uint64_t *bar, uint32_t parity) {
-  uint32_t done = 0;
-  const uint32_t addr = smem_u32(bar);
-  while (!done) {
-    asm volatile(
-        "{\n\t"
-        ".reg .pred p;\n\t"
-        "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
-        "selp.u32 %0, 1, 0, p;\n\t"
-        "}\n"
-        : "=r"(done)
-        : "r"(addr), "r"(parity)
-        : "memory");
+  while (!mbar_try_wait(bar, parity)) {
   }
 }
 // TMA 1-D bulk copy global -> shared, completion signalled on an mbarrier (SASS: UBLKCP)
@@ -79,7 +60,6 @@ __device__ __forceinline__ void bulk_g2s(void *dst_smem, const void *src_gmem, u
                : "memory");
 }
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-__device__ __forceinline__ void fence_mbar_init() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
 
 // PRMT, default mode: selector nibble bit 3 replicates the sign bit of the selected byte.  Grid bytes are
 // <= 100 < 128, so a "sign-replicated" byte is 0x00: one PRMT extracts two bytes into packed u16 lanes.

@@ -1,4 +1,4 @@
-/* util::normalize_angle (lesson4 UtilFunctions.h:36-48) is fmod(fmod(a, 2pi) + 2pi, 2pi) in double.  hector_slam.cu takes
+/* util::normalize_angle (lesson4 UtilFunctions.h:36-48) is fmod(fmod(a, 2pi) + 2pi, 2pi) in double.  hector_grid.cuh takes
  * a shortcut for |a| < 2pi (no remainder loop); this program checks the shortcut against the C library's fmod, bit for
  * bit, on pseudo-random floats of every magnitude below 50 and on the edge cases.  argv[1] = number of samples. */
 #include <math.h>

@@ -22,7 +22,7 @@ def test_restated_sincosf_equals_host_libm(tmp_path):
 
 
 def test_normalize_angle_shortcut_equals_fmod(tmp_path):
-    """hs_normalize_angle's |a| < 2 pi path (one add, one compare, one subtract in double) against the two fmod calls of
+    """util_normalize_angle's |a| < 2 pi path (one add, one compare, one subtract in double) against the two fmod calls of
     util::normalize_angle on this machine's C library: identical bits."""
     exe = str(tmp_path / "normalize_angle_check")
     subprocess.check_call(["gcc", "-O2", "-ffp-contract=off", os.path.join(HERE, "normalize_angle_check.c"), "-o", exe, "-lm"])
