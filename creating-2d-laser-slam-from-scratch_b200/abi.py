@@ -90,6 +90,28 @@ class IcpResult(C.Structure):
                 ("nvalid", C.c_int32), ("reserved", C.c_int32)]
 
 
+class PclIcpParams(C.Structure):
+    """b2s_pcl_icp_params; defaults = a default-constructed pcl::IterativeClosestPoint (lesson2 scan_match_icp.h:49)."""
+    _fields_ = [("max_iterations", C.c_int32), ("drop_invalid_points", C.c_int32),
+                ("max_correspondence_distance", C.c_double), ("transformation_epsilon", C.c_double),
+                ("euclidean_fitness_epsilon", C.c_double)]
+
+
+def pcl_icp_params(**kw) -> PclIcpParams:
+    import sys
+    p = PclIcpParams(10, 0, sys.float_info.max ** 0.5, 0.0, -sys.float_info.max)
+    for k, v in kw.items():
+        if not hasattr(p, k):
+            raise AttributeError(k)
+        setattr(p, k, v)
+    return p
+
+
+class PclIcpResult(C.Structure):
+    _fields_ = [("x", C.c_float * 3), ("converged", C.c_int32), ("iterations", C.c_int32),
+                ("n_correspondences", C.c_int32), ("fitness_score", C.c_double)]
+
+
 def karto_round(v: float) -> float:
     """math::Round (Math.h:87-90)."""
     import math

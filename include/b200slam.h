@@ -573,6 +573,49 @@ b2s_status b2s_plicp_match(const b2s_icp_params *params, int batch, int n, const
                            const double *sens_ranges, const double *theta, double range_min, double range_max,
                            const double *first_guess, int device, void *cuda_stream, b2s_icp_result *results);
 
+/* ---------------------------------------------------------------- lesson2: PCL ICP scan matching
+ * ScanMatchICP (lesson2/src/scan_match_icp.cc): every LaserScan becomes a pcl::PointCloud<PointXYZ>
+ * (ConvertScan2PointCloud, :89-130) and the previous cloud is aligned to the current one by a default-constructed
+ * pcl::IterativeClosestPoint<PointXYZ, PointXYZ> (ScanMatchWithICP, :135-164).  align() gets no initial guess, so the
+ * pairs of a recording are independent and a whole recording is one batch.  PARITY UNPINNED: PCL is third-party code
+ * absent from the reference tree; its published behaviour (PCL 1.8) is restated, see DESIGN.md §2 and §4. */
+/* The node default-constructs its ICP (scan_match_icp.h:49) and sets nothing on it (scan_match_icp.cc:137-143), so
+ * every default below is PCL's own (parity unpinned). */
+typedef struct b2s_pcl_icp_params {
+  int32_t max_iterations;             /* max_iterations_, node default 10 (scan_match_icp.cc:143; parity unpinned).
+                                         Reaching it counts as converged (failure_after_max_iter_ = false) */
+  int32_t drop_invalid_points;        /* 0 = the node (scan_match_icp.cc:96-123; parity unpinned): a non-finite reading
+                                         or one outside (range_min, range_max) stays in the cloud as a point at
+                                         (0, 0, 0) and takes part in ICP.  1 = leave such readings out of both clouds */
+  double max_correspondence_distance; /* corr_dist_threshold_, node default sqrt(DBL_MAX) = unlimited
+                                         (scan_match_icp.cc:143; parity unpinned) */
+  double transformation_epsilon;      /* transformation_epsilon_, node default 0 (scan_match_icp.cc:143; parity
+                                         unpinned).  The rotation threshold is 1 - transformation_epsilon on cos(angle) */
+  double euclidean_fitness_epsilon;   /* euclidean_fitness_epsilon_, node default -DBL_MAX = off
+                                         (scan_match_icp.cc:143; parity unpinned) */
+} b2s_pcl_icp_params;
+
+typedef struct b2s_pcl_icp_result {
+  float x[3];                /* getFinalTransformation() as (x, y, yaw), yaw = atan2(R10, R00)
+                                (pcl::getTranslationAndEulerAngles, scan_match_icp.cc:156-161; parity unpinned).  It maps
+                                the source (previous) scan into the target (current) scan's frame */
+  int32_t converged;         /* hasConverged() (scan_match_icp.cc:148; parity unpinned) */
+  int32_t iterations;        /* iterations run, nr_iterations_ (scan_match_icp.cc:143; parity unpinned) */
+  int32_t n_correspondences; /* correspondences of the last iteration (scan_match_icp.cc:143; parity unpinned) */
+  double fitness_score;      /* getFitnessScore() (scan_match_icp.cc:145; parity unpinned): mean squared nearest-target
+                                distance of the aligned source, DBL_MAX when no point has a target */
+} b2s_pcl_icp_result;
+
+/* ConvertScan2PointCloud + ScanMatchWithICP for `n_pairs` scan pairs on the device.  ranges [n_scans][n] (host) share
+ * the LaserScan fields angle_min, angle_increment, range_min, range_max (beam angle angle_min + i * angle_increment in
+ * float, :112).  pairs [n_pairs][2] = (source, target) scan indices; NULL = the node's loop, (i - 1, i) for every i >= 1,
+ * with n_pairs = n_scans - 1.  guesses [n_pairs][3] = (x, y, yaw) initial transforms, NULL = identity as the node
+ * calls align().  Each scan is converted once, however many pairs use it.  B2S_ERR_TOO_LARGE when the beam count
+ * does not fit the kernel's shared memory (32 bytes per beam). */
+b2s_status b2s_pcl_icp_align(const b2s_pcl_icp_params *params, int n_scans, int n, const float *ranges, float angle_min,
+                             float angle_increment, float range_min, float range_max, int n_pairs, const int32_t *pairs,
+                             const float *guesses, int device, void *cuda_stream, b2s_pcl_icp_result *results);
+
 /* ---------------------------------------------------------------- lesson5: motion de-skew pre-stage (SURVEY.md §8(f).4)
  * LidarUndistortion (lesson5/src/lidar_undistortion.cc): every reading of a LaserScan is moved into the sensor frame
  * of the scan's first valid reading, using IMU angles integrated over the scan and the odometry increment across it.
