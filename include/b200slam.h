@@ -557,11 +557,14 @@ typedef struct b2s_icp_params {
 } b2s_icp_params;
 
 typedef struct b2s_icp_result {
-  double x[3];        /* sm_result.x: pose of the current scan in the reference scan's frame (plicp_odometry.cc:399-403) */
+  double x[3];        /* sm_result.x: pose of the current scan in the reference scan's frame (plicp_odometry.cc:399-403).
+                         When valid = 0 it is the last accepted estimate, or first_guess if no iteration succeeded —
+                         never the output of the iteration that failed (too few correspondences, or a solve without a
+                         finite solution) */
   double error;       /* sum of point-to-segment distances of the kept correspondences */
   int32_t valid;      /* sm_result.valid */
-  int32_t iterations;
-  int32_t nvalid;     /* correspondences kept in the last iteration */
+  int32_t iterations; /* iterations that succeeded; the one that failed is not counted */
+  int32_t nvalid;     /* correspondences kept in the last iteration, the failed one included */
   int32_t reserved;
 } b2s_icp_result;
 

@@ -19,7 +19,9 @@
  *   5. closed-form point-to-line solution (GPC: quadratic cost in (t, cos, sin), unit-norm constraint by a Lagrange
  *      multiplier = largest real root of a quartic),
  *   6. stop when the increment is below (epsilon_xy, epsilon_theta) or after max_iterations.
- * Acceptance is self-consistency only: recover a known synthetic transform (tests/test_oracle_plicp.py).
+ * Acceptance: every iteration agrees with an independent float64 statement of the algorithm
+ * (tests/plicp_reference.py) wherever no decision is within rounding of flipping, and known synthetic transforms are
+ * recovered (tests/test_plicp.py).
  */
 #include <math.h>
 #include <stdint.h>
@@ -229,7 +231,10 @@ int orc_plicp_match(const b2s_icp_params *P, int n, const double *ref_r, const d
         for (int col = 0; col < 4; col++) M[4 * r + col] += Mk[r] * CM[col] + Mk[4 + r] * CM[4 + col];
       for (int r = 0; r < 4; r++) g[r] += -2.0 * (qx * CM[r] + qy * CM[4 + r]);
     }
-    if (!gpc_solve(M, g, x_new)) { ok = 0; break; }
+    /* a failed solve leaves x_new at the last accepted estimate (the first guess if there is none) */
+    double x_gpc[3];
+    if (!gpc_solve(M, g, x_gpc)) { ok = 0; break; }
+    x_new[0] = x_gpc[0]; x_new[1] = x_gpc[1]; x_new[2] = x_gpc[2];
     /* pose_diff(x_new, x_old): x_new expressed relative to x_old */
     const double ddx = x_new[0] - x_old[0], ddy = x_new[1] - x_old[1];
     const double co = cos(x_old[2]), so = sin(x_old[2]);
