@@ -15,15 +15,27 @@
 //
 // Kernels:
 //   k_scan_points      point readings + scan-local points                              (fp64, O(B*N))
+//   k_grid_offsets     grid offset that centres the ROI on the scan's sensor position
 //   k_add_scan         FindValidPoints state machine + rasterise + max-smear           (byte atomics, O(B*S*N))
+//   k_add_scans_seq    the same, sequential, when an off-centre smear value reaches 100 (order-dependent)
+//   k_grid_sat         per-match summed-area table of the grid's non-empty 4x4 blocks
+//   k_bases            candidate lattice -> flat base indices; flags irregular and out-of-grid lattices
 //   k_offsets          per-angle lookup tables                                         (fp64 -> i32)
-//   k_sweep_window     THE HOT KERNEL: whole grid staged into shared memory by TMA bulk copy; one warp per
-//                      angle, one lane per candidate row; each 32-bit shared-memory word feeds 4 adjacent-x
-//                      candidates (byte-permute into packed u16 accumulators)           (int, smem-gather bound)
+//   k_offsets_sorted   window kernel's lists: window origins grouped by row band, byte alignment and interior /
+//                      edge, empty windows dropped through the summed-area table
+//   k_sweep_window     THE HOT KERNEL: grid (or a row band of it) staged into shared memory by TMA bulk copy;
+//                      one warp per (angle, 32x32 candidate tile), one lane per candidate row; each 32-bit
+//                      shared-memory word feeds 4 adjacent-x candidates (byte-permute into packed u16
+//                      accumulators)                                                    (int, smem-gather bound)
 //   k_sweep_generic    any lattice / any grid size: one warp per (x,y) candidate, lanes over beams,
 //                      gathers from global memory through L1/L2
-//   k_reduce           penalties, best response, tie-averaged pose, positional covariance (fp64, one CTA per match)
+//   k_reduce           penalties, best response, tie-averaged pose, positional covariance (fp64, one CTA per match);
+//                      the whole tail or one phase of an angle-split sweep
 //   k_angular_cov      fine-stage angular covariance (re-evaluates GetResponse at the best cell)
+//   k_results_to_centers, k_status_pack, k_status_apply: small copies between the stages
+//
+// Which sweep kernel runs, with which band geometry and shared-memory sizes, is decided by plan_sweep
+// (karto_sweep_plan.cuh) before anything is enqueued.
 #include <algorithm>
 #include <cmath>
 #include <cstdlib>
@@ -35,14 +47,11 @@
 #include <math_constants.h>
 
 #include "common.cuh"
+#include "karto_sweep_plan.cuh"
 #include "nccl_dl.cuh"
 #include "scan_kernels.cuh"
 
 namespace b2s {
-
-static thread_local std::string g_last_error;
-void set_last_error(const std::string &s) { g_last_error = s; }
-std::string &last_error_ref() { return g_last_error; }
 
 // ----------------------------------------------------------------------------------------------
 // device helpers
@@ -110,6 +119,7 @@ struct b2s_matcher {
   int force_kernel = 0;
   int num_sms = 1;  // the device's, set at create
   int smem_optin = 0;
+  size_t win_static_smem = 0;  // k_sweep_window's static shared memory: comes out of the opt-in budget of its image
 
   Buf<uint8_t> d_kernel;
   Buf<double> d_ranges, d_poses, d_sensor, d_pts, d_local;
@@ -479,12 +489,9 @@ __global__ void __launch_bounds__(256) k_sweep_generic(const uint8_t *__restrict
 // are entirely outside).  Lanes 16..31 fetch their 9 words rotated by one so that the two half-warps hit odd /
 // even banks (width_step/4 is even, so rows r and r+16 would otherwise always collide).
 // ----------------------------------------------------------------------------------------------
-constexpr int WIN_THREADS = 512;
-constexpr int WIN_GUARD = 128;          // zero bytes before and after the grid image in shared memory
+// (WIN_THREADS, WIN_GUARD, WIN_MAX_BANDS, LIST_PAD: karto_sweep_plan.cuh)
 constexpr int WIN_FLUSH_BEAMS = 512;    // beams accumulated in u16 lanes between flushes (512 * 127 < 65536)
 constexpr int32_t WIN_SKIP = -(1 << 29);
-constexpr int WIN_MAX_BANDS = 32;      // row bands a grid larger than shared memory is swept in
-constexpr int LIST_PAD = 16;            // per-(match, angle) list capacity = n + LIST_PAD * nbands
 
 // ----------------------------------------------------------------------------------------------
 // k_grid_sat: per match, a summed-area table over 4x4-cell blocks of "block holds a non-zero cell".  A beam whose
@@ -530,10 +537,8 @@ __global__ void __launch_bounds__(256)
 // The scan's readings and local points are staged in shared memory once per block and reused for every angle of
 // the chunk (16x less L2 traffic than one block per angle).  A non-finite reading (INVALID_SCAN, Karto.h:6478) always
 // yields a non-finite local point (inf/NaN propagate through the inverse transform), so only the points are staged.
-constexpr int OFF_CHUNK = 16;
-constexpr int OFF_Q = 2;                              // angles classified per pass
+// (OFF_CHUNK, OFF_Q, OFF_SMEM_PER_BEAM: karto_sweep_plan.cuh)
 constexpr int OFF_GS = 8 * WIN_MAX_BANDS;             // group slots per angle
-constexpr int OFF_SMEM_PER_BEAM = 16 + 5 * OFF_Q;     // two doubles + OFF_Q x (origin int32 + class byte)
 __global__ void __launch_bounds__(256)
     k_offsets_sorted(const double *__restrict__ ranges, const double *__restrict__ local,
                      const double *__restrict__ grid_off, const double *__restrict__ centers,
@@ -833,6 +838,15 @@ __device__ __forceinline__ void win_class_pair(const uint8_t *__restrict__ sgrid
   win_flush<SH, STRIDE, GEN>(lo, hi, acc, hi_half);
 }
 
+// What one k_reduce launch does: the whole tail of a CorrelateScan, or one phase of a sweep whose angles are split over
+// several GPUs (b2s_matcher_correlate_split_*).  The phases are ordered: the first two compute the best response.
+enum ReducePhase : int {
+  REDUCE_WHOLE = 0,
+  REDUCE_SPLIT_BEST = 1,    // this angle subset's best response and per-cell maxima
+  REDUCE_SPLIT_TIES = 2,    // tie sums {x, y, cos, sin, count} against the global best
+  REDUCE_SPLIT_FINISH = 3,  // mean pose and covariance from the global best, tie sums and maxima plane
+};
+
 struct ReduceArgs {
   const int32_t *sums;
   const double *centers;
@@ -844,7 +858,8 @@ struct ReduceArgs {
   int n, nx, ny, na;
   double *probs_all;
   b2s_match_result *results;
-  int k_first, mode;
+  int k_first;
+  ReducePhase phase;
   double *part_best;
   const double *glob_best;
   double *tie_out;
@@ -996,7 +1011,7 @@ __global__ void __launch_bounds__(WIN_THREADS, 1)
 // at most RED_MAX_TIES of them (bit-identical to the reference), otherwise by a fixed-order tree.
 // ----------------------------------------------------------------------------------------------
 constexpr int RED_THREADS = 512;
-// (stand-alone k_reduce: 60 registers, two CTAs per SM, so one match's serial tail overlaps another's streaming pass)
+// (two CTAs per SM, so one match's serial tail overlaps another's streaming pass)
 constexpr int RED_MAX_TIES = 512;
 constexpr int RED_UNROLL = 8;
 
@@ -1024,8 +1039,9 @@ __device__ __forceinline__ float red_fscore(int32_t isum, float apf_k, float dpf
   return (float)isum * apf_k * dpf;
 }
 
-__device__ __forceinline__ void reduce_match_body(const int b, const ReduceArgs &A) {
-  const int32_t *sums = A.sums;  // no __restrict__ / no read-only path: the fused sweep wrote them in this very launch
+__global__ void __launch_bounds__(RED_THREADS, 2) k_reduce(ReduceArgs A) {
+  const int b = blockIdx.x;
+  const int32_t *sums = A.sums;
   const double *__restrict__ centers = A.centers;
   const int32_t *__restrict__ flags = A.flags;
   const b2s_matcher_params &p = A.p;
@@ -1035,7 +1051,8 @@ __device__ __forceinline__ void reduce_match_body(const int b, const ReduceArgs 
   const int n = A.n, nx = A.nx, ny = A.ny, na = A.na;
   double *__restrict__ probs_all = A.probs_all;
   b2s_match_result *__restrict__ results = A.results;
-  const int k_first = A.k_first, mode = A.mode;
+  const int k_first = A.k_first;
+  const ReducePhase phase = A.phase;
   double *__restrict__ part_best = A.part_best;
   const double *__restrict__ glob_best = A.glob_best;
   double *__restrict__ tie_out = A.tie_out;
@@ -1064,7 +1081,7 @@ __device__ __forceinline__ void reduce_match_body(const int b, const ReduceArgs 
   __shared__ double s_best;
   __shared__ double s_mean[3];
   if (tid == 0) { s_err = 0; s_count = 0; }
-  if (!s.fine && mode <= 1)
+  if (!s.fine && phase <= REDUCE_SPLIT_BEST)
     for (int i = tid; i < pstep * g.search_side; i += RED_THREADS) probs[i] = 0.0;  // Clear (Mapper.cpp:329)
 
   // Float pre-filter.  The exact fp64 response (reference operation order, candidate_response) is only needed for
@@ -1093,7 +1110,7 @@ __device__ __forceinline__ void reduce_match_body(const int b, const ReduceArgs 
   double best = -1.0;
   float fmax0 = 0.0f, fmax1 = 0.0f;  // float maxima of this thread's first two cells, kept for pass 2
   bool known0 = false, known1 = false;
-  for (int c = tid; c < ncell && mode <= 1; c += RED_THREADS) {
+  for (int c = tid; c < ncell && phase <= REDUCE_SPLIT_BEST; c += RED_THREADS) {
     const int iy = c / nx, ix = c % nx;
     const double y = start_y + (double)(uint32_t)iy * s.res_y, x = start_x + (double)(uint32_t)ix * s.res_x;
     const double sq = x * x + y * y;
@@ -1171,14 +1188,14 @@ __device__ __forceinline__ void reduce_match_body(const int b, const ReduceArgs 
     if (tid < d) cov_terms[0][tid] = dmax(cov_terms[0][tid], cov_terms[0][tid + d]);
     __syncthreads();
   }
-  if (tid == 0) s_best = mode <= 1 ? cov_terms[0][0] : glob_best[b];
+  if (tid == 0) s_best = phase <= REDUCE_SPLIT_BEST ? cov_terms[0][0] : glob_best[b];
   __syncthreads();
   best = s_best;
   if (s_err) {
     if (tid == 0) res->status = B2S_ERR_OUT_OF_RANGE;
     return;
   }
-  if (mode == 1) {  // split sweep, phase 1: this angle subset's best (the per-cell maxima are in `probs`)
+  if (phase == REDUCE_SPLIT_BEST) {  // split sweep, phase 1: this angle subset's best (the per-cell maxima are in `probs`)
     if (tid == 0) { part_best[b] = best; res->status = B2S_OK; }
     return;
   }
@@ -1186,7 +1203,7 @@ __device__ __forceinline__ void reduce_match_body(const int b, const ReduceArgs 
   // ---- pass 2: poses tied with the best (Mapper.cpp:455-487) ----
   double ax = 0, ay = 0, tx = 0, ty = 0;
   const float tie_thr = (float)((best - KT_TOLERANCE) * (1.0 - 1.0e-6)) - 1.0e-9f;
-  for (int c = tid; c < ncell && mode != 3; c += RED_THREADS) {
+  for (int c = tid; c < ncell && phase != REDUCE_SPLIT_FINISH; c += RED_THREADS) {
     if (c == tid && known0 && fmax0 < tie_thr) continue;  // no candidate of this cell can tie (pass 1's maximum)
     if (c == tid + RED_THREADS && known1 && fmax1 < tie_thr) continue;
     const int iy = c / nx, ix = c % nx;
@@ -1218,17 +1235,17 @@ __device__ __forceinline__ void reduce_match_body(const int b, const ReduceArgs 
     }
   }
   __syncthreads();
-  if (mode == 3 && tid == 0) s_count = (int)tie_in[5 * b + 4];
+  if (phase == REDUCE_SPLIT_FINISH && tid == 0) s_count = (int)tie_in[5 * b + 4];
   __syncthreads();
   const int total = s_count;
-  if (total == 0 && mode != 2) {
+  if (total == 0 && phase != REDUCE_SPLIT_TIES) {
     if (tid == 0) res->status = B2S_ERR_NO_BEST_POSE;  // Mapper.cpp:484-487
     return;
   }
-  if (mode == 3) {
+  if (phase == REDUCE_SPLIT_FINISH) {
     if (tid == 0) { red[0] = tie_in[5 * b]; red[1] = tie_in[5 * b + 1]; red[2] = tie_in[5 * b + 2]; red[3] = tie_in[5 * b + 3]; }
     __syncthreads();
-  } else if (total <= RED_MAX_TIES && mode == 0) {
+  } else if (total <= RED_MAX_TIES && phase == REDUCE_WHOLE) {
     // rank-sort the tie list by reference linear index, then one thread sums in that exact order
     for (int i = tid; i < total; i += RED_THREADS) {
       int v = tie_idx[i], rank = 0;
@@ -1261,7 +1278,7 @@ __device__ __forceinline__ void reduce_match_body(const int b, const ReduceArgs 
     if (tid == 0) { red[0] = cov_terms[0][0]; red[1] = cov_terms[1][0]; red[2] = cov_terms[2][0]; red[3] = cov_terms[3][0]; }
     __syncthreads();
   }
-  if (mode == 2) {  // split sweep, phase 2: this subset's tie sums {x, y, cos, sin, count}
+  if (phase == REDUCE_SPLIT_TIES) {  // split sweep, phase 2: this subset's tie sums {x, y, cos, sin, count}
     if (tid == 0) {
       tie_out[5 * b] = red[0]; tie_out[5 * b + 1] = red[1]; tie_out[5 * b + 2] = red[2]; tie_out[5 * b + 3] = red[3];
       tie_out[5 * b + 4] = (double)total;
@@ -1349,10 +1366,6 @@ __device__ __forceinline__ void reduce_match_body(const int b, const ReduceArgs 
   res->response = s.fine ? best : (best > 1.0 ? 1.0 : best);  // Mapper.cpp:514-517
   res->status = B2S_OK;
   res->tie_count = total;
-}
-
-__global__ void __launch_bounds__(RED_THREADS, 2) k_reduce(ReduceArgs A) {
-  reduce_match_body(blockIdx.x, A);
 }
 
 // ----------------------------------------------------------------------------------------------
@@ -1450,22 +1463,9 @@ __global__ void k_status_apply(b2s_match_result *__restrict__ results, const int
 // ----------------------------------------------------------------------------------------------
 
 static b2s_status layout_from_params(const b2s_matcher_params *p, b2s_grid_info *g) {
-  // ScanMatcher::Create (Mapper.cpp:126-172) + CorrelationGrid ctor (Mapper.h:920-1027) + Grid::Resize (Karto.h:4438)
   if (p->resolution <= 0 || p->search_size <= 0 || p->smear_deviation < 0 || p->range_threshold <= 0)
     B2S_FAIL(B2S_ERR_BAD_PARAMS, "ScanMatcher::Create: invalid parameters");
-  uint32_t side = cast_u32(kround(p->search_size / p->resolution) + 1);
-  uint32_t margin = cast_u32(ceil(p->range_threshold / p->resolution));
-  int32_t grid_size = (int32_t)(side + 2 * margin);
-  int32_t half_kernel = cast_i32(kround(2.0 * p->smear_deviation / p->resolution));
-  uint32_t border = (uint32_t)(half_kernel + 1);
-  g->width = grid_size + 2 * (int32_t)border;
-  g->height = grid_size + 2 * (int32_t)border;
-  g->width_step = (int32_t)(((size_t)g->width + 7) & ~(size_t)7);
-  g->data_size = g->width_step * g->height;
-  g->roi_x = g->roi_y = (int32_t)border;
-  g->roi_w = g->roi_h = grid_size;
-  g->kernel_size = 2 * half_kernel + 1;
-  g->search_side = (int32_t)side;
+  *g = grid_layout(*p);
   double resolution = 1.0 / (1.0 / p->resolution);
   double min_dev = 0.5 * resolution, max_dev = 10 * resolution;  // Mapper.h:1041-1053 throws
   if (!(p->smear_deviation >= min_dev && p->smear_deviation <= max_dev))
@@ -1473,13 +1473,32 @@ static b2s_status layout_from_params(const b2s_matcher_params *p, b2s_grid_info 
   return B2S_OK;
 }
 
-static b2s_status run_correlate(b2s_matcher *m, const b2s_search *s, int k_first = 0, int na_override = -1, int mode = 0);
+// Between a b2s_matcher_correlate_scan_begin and its _end the handle's state must not change.
+static b2s_status refuse_if_pending(const b2s_matcher *m) {
+  if (m && m->pending) B2S_FAIL(B2S_ERR_BAD_STATE, "a b2s_matcher_correlate_scan_begin awaits its _end: the handle cannot change state in between");
+  return B2S_OK;
+}
+static b2s_status require_scans_and_grids(const b2s_matcher *m) {
+  if (!m->scans_set || !m->grids_set) B2S_FAIL(B2S_ERR_BAD_STATE, "scans and grids must be set first");
+  return B2S_OK;
+}
+
+// last_ms from the events of the last sweep: lists, sweep, fp64 tail (a span whose events are not complete keeps its value)
+static void read_sweep_ms(b2s_matcher *m) {
+  for (int i = 0; i < 3; i++) {
+    float ms = 0;
+    if (cudaEventElapsedTime(&ms, m->ev[i], m->ev[i + 1]) == cudaSuccess) m->last_ms[i] = ms;
+  }
+}
+
+static b2s_status run_correlate(b2s_matcher *m, const b2s_search *s, int k_first = 0, int na_override = -1,
+                                ReducePhase phase = REDUCE_WHOLE);
 
 // (re)build the per-match block summed-area tables after the grids changed
 static b2s_status build_sat(b2s_matcher *m) {
   const size_t sm = sizeof(uint32_t) * (size_t)(m->sbx + 1) * (m->sby + 1);
   m->sat_valid = false;
-  if (sm > 200 * 1024 || (m->g.width_step % 4) != 0 || (long long)m->sbx * m->sby >= 65535) return B2S_OK;  // no skipping
+  if (sm > LIST_SMEM_MAX || (m->g.width_step % 4) != 0 || (long long)m->sbx * m->sby >= 65535) return B2S_OK;  // no skipping
   if (sm > 16 * 1024) B2S_CUDA_CHECK(raise_dyn_smem(k_grid_sat, sm));
   k_grid_sat<<<m->batch, 256, sm, m->stream>>>(m->d_grids, m->grid_pitch, m->g.width_step, m->g.height, m->sbx, m->sby, m->d_sat);
   B2S_CUDA_CHECK(cudaGetLastError());
@@ -1494,17 +1513,6 @@ static b2s_status build_sat(b2s_matcher *m) {
 // ================================================================================================
 extern "C" {
 
-int b2s_abi_version(void) { return B2S_ABI_VERSION; }
-const char *b2s_last_error(void) { return b2s::last_error_ref().c_str(); }
-int b2s_device_count(void) {
-  int n = 0;
-  if (cudaGetDeviceCount(&n) != cudaSuccess) {
-    cudaGetLastError();
-    return 0;
-  }
-  return n;
-}
-
 void b2s_matcher_destroy(b2s_matcher *m);
 static b2s_status matcher_create_impl(const b2s_matcher_params *params, const b2s_laser *laser, int device, int max_batch,
                                       int max_base_scans, void *cuda_stream, b2s_matcher *m, const b2s_grid_info &g) {
@@ -1514,6 +1522,9 @@ static b2s_status matcher_create_impl(const b2s_matcher_params *params, const b2
   B2S_CUDA_CHECK(cudaGetDeviceProperties(&prop, device));
   m->num_sms = prop.multiProcessorCount;
   m->smem_optin = (int)prop.sharedMemPerBlockOptin;
+  cudaFuncAttributes fa;
+  B2S_CUDA_CHECK(cudaFuncGetAttributes(&fa, k_sweep_window<1, false>));
+  m->win_static_smem = fa.sharedSizeBytes;
   B2S_CUDA_CHECK(m->stream.init(cuda_stream));
   for (auto &e : m->ev) B2S_CUDA_CHECK(e.create());
   // smear kernel on the host with glibc, exactly CorrelationGrid::CalculateKernel (Mapper.h:1032-1087)
@@ -1534,7 +1545,6 @@ static b2s_status matcher_create_impl(const b2s_matcher_params *params, const b2
   }
   const size_t B = (size_t)max_batch, N = (size_t)std::max(m->n, 1);
   m->grid_pitch = (((size_t)g.data_size + 16) + 127) & ~(size_t)127;
-  const int pstep = (g.search_side + 7) & ~7;
   B2S_CUDA_CHECK(m->d_ranges.reserve(B * N));
   B2S_CUDA_CHECK(m->d_poses.reserve(B * 3));
   B2S_CUDA_CHECK(m->d_sensor.reserve(B * 3));
@@ -1543,13 +1553,13 @@ static b2s_status matcher_create_impl(const b2s_matcher_params *params, const b2
   B2S_CUDA_CHECK(m->d_grids.reserve(B * m->grid_pitch));
   B2S_CUDA_CHECK(m->d_grid_off.reserve(B * 2));
   B2S_CUDA_CHECK(m->d_flags.reserve(B));
-  B2S_CUDA_CHECK(m->d_probs.reserve(B * (size_t)pstep * g.search_side));
+  B2S_CUDA_CHECK(m->d_probs.reserve(B * probs_len(g.search_side)));
   B2S_CUDA_CHECK(m->d_centers.reserve(B * 3));
   B2S_CUDA_CHECK(m->d_results.reserve(B));
   B2S_CUDA_CHECK(m->d_work.reserve(1));
   m->sbx = (g.width_step + 3) / 4;
   m->sby = (g.height + 3) / 4;
-  B2S_CUDA_CHECK(m->d_sat.reserve(B * (size_t)((((m->sbx + 1) * (m->sby + 1)) + 7) & ~7)));  // per-match stride padded to 16 bytes
+  B2S_CUDA_CHECK(m->d_sat.reserve(B * sat_stride(m->sbx, m->sby)));
   B2S_CUDA_CHECK(m->d_stats.reserve(1));
   B2S_CUDA_CHECK(m->d_part_best.reserve(B));
   B2S_CUDA_CHECK(m->d_glob_best.reserve(B));
@@ -1606,7 +1616,7 @@ b2s_status b2s_matcher_sync(b2s_matcher *m) {
 }
 
 b2s_status b2s_matcher_set_scans(b2s_matcher *m, int batch, const double *ranges, const double *poses) {
-  if (m && m->pending) B2S_FAIL(B2S_ERR_BAD_STATE, "a b2s_matcher_correlate_scan_begin awaits its _end: the handle cannot change state in between");
+  if (b2s_status st = refuse_if_pending(m)) return st;
   if (!m || !ranges || !poses) B2S_FAIL(B2S_ERR_BAD_PARAMS, "null argument");
   if (batch <= 0 || batch > m->max_batch) B2S_FAIL(B2S_ERR_TOO_LARGE, "batch exceeds the handle's max_batch");
   B2S_CUDA_CHECK(cudaSetDevice(m->device));
@@ -1627,7 +1637,7 @@ b2s_status b2s_matcher_set_scans(b2s_matcher *m, int batch, const double *ranges
 static b2s_status add_scans_impl(b2s_matcher *m, int n_base, const double *base_ranges, const int32_t *pool_rows,
                                  const double *base_poses) {
   B2S_NVTX("K1 add_scans (rasterise + smear)");
-  if (m && m->pending) B2S_FAIL(B2S_ERR_BAD_STATE, "a b2s_matcher_correlate_scan_begin awaits its _end: the handle cannot change state in between");
+  if (b2s_status st = refuse_if_pending(m)) return st;
   if (!m || n_base < 0 || (n_base > 0 && ((!base_ranges && !pool_rows) || !base_poses))) B2S_FAIL(B2S_ERR_BAD_PARAMS, "null argument");
   if (!m->scans_set) B2S_FAIL(B2S_ERR_BAD_STATE, "b2s_matcher_set_scans must precede b2s_matcher_add_scans");
   if (n_base > m->max_base) B2S_FAIL(B2S_ERR_TOO_LARGE, "n_base exceeds the handle's max_base_scans");
@@ -1685,7 +1695,7 @@ b2s_status b2s_matcher_add_scans(b2s_matcher *m, int n_base, const double *base_
 // ---- scan pool: readings that serve as base scans of many matches (a mapper's running window, near chains, loop
 // candidates) are uploaded once and referenced by row afterwards
 b2s_status b2s_matcher_pool_append(b2s_matcher *m, const double *ranges, int32_t *out_row) {
-  if (m && m->pending) B2S_FAIL(B2S_ERR_BAD_STATE, "a b2s_matcher_correlate_scan_begin awaits its _end: the handle cannot change state in between");
+  if (b2s_status st = refuse_if_pending(m)) return st;
   if (!m || !ranges) B2S_FAIL(B2S_ERR_BAD_PARAMS, "null argument");
   B2S_CUDA_CHECK(cudaSetDevice(m->device));
   const size_t n = (size_t)std::max(m->l.n_readings, 1);
@@ -1711,7 +1721,7 @@ b2s_status b2s_matcher_add_scans_pool(b2s_matcher *m, int n_base, const int32_t 
 }
 
 b2s_status b2s_matcher_set_grids(b2s_matcher *m, const uint8_t *grids, const double *offsets) {
-  if (m && m->pending) B2S_FAIL(B2S_ERR_BAD_STATE, "a b2s_matcher_correlate_scan_begin awaits its _end: the handle cannot change state in between");
+  if (b2s_status st = refuse_if_pending(m)) return st;
   if (!m || !grids || !offsets) B2S_FAIL(B2S_ERR_BAD_PARAMS, "null argument");
   if (!m->scans_set) B2S_FAIL(B2S_ERR_BAD_STATE, "b2s_matcher_set_scans must precede b2s_matcher_set_grids");
   B2S_CUDA_CHECK(cudaSetDevice(m->device));
@@ -1752,7 +1762,7 @@ b2s_status b2s_matcher_get_point_readings(b2s_matcher *m, int b, double *out_xy)
 b2s_status b2s_matcher_compute_offsets(b2s_matcher *m, int b, double angle_center, double angle_offset,
                                        double angle_res, int32_t *out, int32_t *out_n_angles) {
   if (!m || !out || b < 0 || b >= m->batch) B2S_FAIL(B2S_ERR_BAD_PARAMS, "bad argument");
-  if (!m->scans_set || !m->grids_set) B2S_FAIL(B2S_ERR_BAD_STATE, "scans and grids must be set first");
+  if (b2s_status st = require_scans_and_grids(m)) return st;
   if (angle_res == 0.0) B2S_FAIL(B2S_ERR_BAD_PARAMS, "angle resolution must be non-zero");
   B2S_CUDA_CHECK(cudaSetDevice(m->device));
   const int na = n_steps(angle_offset, angle_res);
@@ -1776,7 +1786,7 @@ b2s_status b2s_matcher_compute_offsets(b2s_matcher *m, int b, double angle_cente
 b2s_status b2s_matcher_correlate_scan_begin(b2s_matcher *m, const double *centers, const b2s_search *search,
                                             const b2s_match_result *cov_in) {
   if (!m || !centers || !search) B2S_FAIL(B2S_ERR_BAD_PARAMS, "null argument");
-  if (!m->scans_set || !m->grids_set) B2S_FAIL(B2S_ERR_BAD_STATE, "scans and grids must be set first");
+  if (b2s_status st = require_scans_and_grids(m)) return st;
   if (search->fine && !cov_in) B2S_FAIL(B2S_ERR_BAD_PARAMS, "the fine stage needs the incoming covariances (rCovariance is IN/OUT)");
   if (m->pending) B2S_FAIL(B2S_ERR_BAD_STATE, "b2s_matcher_correlate_scan_begin while an earlier one awaits its _end");
   B2S_CUDA_CHECK(cudaSetDevice(m->device));
@@ -1805,14 +1815,7 @@ b2s_status b2s_matcher_correlate_scan_end(b2s_matcher *m, b2s_match_result *resu
   std::memcpy(results, m->h_results, sizeof(b2s_match_result) * B);
   if (m->last_path == 2 && m->last.na > 0 && m->n > 0) m->last_empty_frac = (double)*m->h_stats / ((double)B * m->last.na * m->n);
   else m->last_empty_frac = 0.0;
-  for (int i = 1; i < 3; i++) {
-    float ms = 0;
-    if (cudaEventElapsedTime(&ms, m->ev[i - 1], m->ev[i]) == cudaSuccess) m->last_ms[i - 1] = ms;
-  }
-  {
-    float ms = 0;
-    if (cudaEventElapsedTime(&ms, m->ev[2], m->ev[3]) == cudaSuccess) m->last_ms[2] = ms;
-  }
+  read_sweep_ms(m);
   return B2S_OK;
 }
 
@@ -1826,9 +1829,9 @@ b2s_status b2s_matcher_correlate_scan(b2s_matcher *m, const double *centers, con
 
 b2s_status b2s_matcher_match_scan(b2s_matcher *m, int do_penalize, int do_refine, b2s_match_result *results) {
   B2S_NVTX("K1 MatchScan (coarse + fine)");
-  if (m && m->pending) B2S_FAIL(B2S_ERR_BAD_STATE, "a b2s_matcher_correlate_scan_begin awaits its _end: the handle cannot change state in between");
+  if (b2s_status st = refuse_if_pending(m)) return st;
   if (!m || !results) B2S_FAIL(B2S_ERR_BAD_PARAMS, "null argument");
-  if (!m->scans_set || !m->grids_set) B2S_FAIL(B2S_ERR_BAD_STATE, "scans and grids must be set first");
+  if (b2s_status st = require_scans_and_grids(m)) return st;
   B2S_CUDA_CHECK(cudaSetDevice(m->device));
   const int B = m->batch;
   if (m->n == 0) {  // Mapper.cpp:199-209: no readings -> pose passthrough, maximum covariance
@@ -1924,15 +1927,15 @@ b2s_status b2s_matcher_match_scan_host(b2s_matcher *m, int batch, const double *
  *   finish: in global best / tie sums / plane; out the same results as b2s_matcher_correlate_scan (coarse stage). */
 b2s_status b2s_matcher_correlate_split_begin(b2s_matcher *m, const double *centers, const b2s_search *search, int k_first,
                                              int k_count, double *best, double *probs, int32_t *status) {
-  if (m && m->pending) B2S_FAIL(B2S_ERR_BAD_STATE, "a b2s_matcher_correlate_scan_begin awaits its _end: the handle cannot change state in between");
+  if (b2s_status st = refuse_if_pending(m)) return st;
   if (!m || !centers || !search || !best || !probs || !status || k_count < 0) B2S_FAIL(B2S_ERR_BAD_PARAMS, "null argument");
   if (search->fine) B2S_FAIL(B2S_ERR_BAD_PARAMS, "only the coarse stage (doingFineMatch = false) can be split");
-  if (!m->scans_set || !m->grids_set) B2S_FAIL(B2S_ERR_BAD_STATE, "scans and grids must be set first");
+  if (b2s_status st = require_scans_and_grids(m)) return st;
   B2S_CUDA_CHECK(cudaSetDevice(m->device));
   const int B = m->batch;
-  const size_t plen = (size_t)((m->g.search_side + 7) & ~7) * m->g.search_side;
+  const size_t plen = probs_len(m->g.search_side);
   B2S_CUDA_CHECK(cudaMemcpyAsync(m->d_centers, centers, sizeof(double) * 3 * B, cudaMemcpyHostToDevice, m->stream));
-  b2s_status st = run_correlate(m, search, k_first, k_count, 1);
+  b2s_status st = run_correlate(m, search, k_first, k_count, REDUCE_SPLIT_BEST);
   if (st) return st;
   B2S_CUDA_CHECK(cudaMemcpyAsync(best, m->d_part_best, sizeof(double) * B, cudaMemcpyDeviceToHost, m->stream));
   B2S_CUDA_CHECK(cudaMemcpyAsync(probs, m->d_probs, sizeof(double) * plen * B, cudaMemcpyDeviceToHost, m->stream));
@@ -1942,32 +1945,32 @@ b2s_status b2s_matcher_correlate_split_begin(b2s_matcher *m, const double *cente
   return B2S_OK;
 }
 
-static ReduceArgs reduce_args(b2s_matcher *m, const b2s_search &s, int nx, int ny, int na, int k_first, int mode) {
+static ReduceArgs reduce_args(b2s_matcher *m, const b2s_search &s, int nx, int ny, int na, int k_first, ReducePhase phase) {
   ReduceArgs A;
   A.sums = m->d_sums; A.centers = m->d_centers; A.flags = m->d_flags;
   A.p = m->p; A.s = s; A.g = m->g; A.scale = 1.0 / m->p.resolution;
   A.n = m->n; A.nx = nx; A.ny = ny; A.na = na;
   A.probs_all = m->d_probs; A.results = m->d_results;
-  A.k_first = k_first; A.mode = mode;
+  A.k_first = k_first; A.phase = phase;
   A.part_best = m->d_part_best; A.glob_best = m->d_glob_best; A.tie_out = m->d_tie; A.tie_in = m->d_tie;
   return A;
 }
 
-static b2s_status split_phase(b2s_matcher *m, int mode) {
-  k_reduce<<<m->batch, RED_THREADS, 0, m->stream>>>(reduce_args(m, m->last_search, m->last.nx, m->last.ny, m->last.na, m->last_k_first, mode));
+static b2s_status split_phase(b2s_matcher *m, ReducePhase phase) {
+  k_reduce<<<m->batch, RED_THREADS, 0, m->stream>>>(reduce_args(m, m->last_search, m->last.nx, m->last.ny, m->last.na, m->last_k_first, phase));
   B2S_CUDA_CHECK(cudaGetLastError());
   return B2S_OK;
 }
 
 b2s_status b2s_matcher_correlate_split_ties(b2s_matcher *m, const double *global_best, double *tie_sums) {
-  if (m && m->pending) B2S_FAIL(B2S_ERR_BAD_STATE, "a b2s_matcher_correlate_scan_begin awaits its _end: the handle cannot change state in between");
+  if (b2s_status st = refuse_if_pending(m)) return st;
   if (!m || !global_best || !tie_sums) B2S_FAIL(B2S_ERR_BAD_PARAMS, "null argument");
   if (!m->have_sweep) B2S_FAIL(B2S_ERR_BAD_STATE, "b2s_matcher_correlate_split_begin must come first");
   B2S_CUDA_CHECK(cudaSetDevice(m->device));
   const int B = m->batch;
   B2S_CUDA_CHECK(cudaMemcpyAsync(m->d_glob_best, global_best, sizeof(double) * B, cudaMemcpyHostToDevice, m->stream));
   B2S_CUDA_CHECK(cudaMemsetAsync(m->d_tie, 0, sizeof(double) * 5 * B, m->stream));
-  b2s_status st = split_phase(m, 2);
+  b2s_status st = split_phase(m, REDUCE_SPLIT_TIES);
   if (st) return st;
   B2S_CUDA_CHECK(cudaMemcpyAsync(tie_sums, m->d_tie, sizeof(double) * 5 * B, cudaMemcpyDeviceToHost, m->stream));
   B2S_CUDA_CHECK(cudaStreamSynchronize(m->stream));
@@ -1976,16 +1979,16 @@ b2s_status b2s_matcher_correlate_split_ties(b2s_matcher *m, const double *global
 
 b2s_status b2s_matcher_correlate_split_finish(b2s_matcher *m, const double *global_best, const double *tie_sums,
                                               const double *probs, b2s_match_result *results) {
-  if (m && m->pending) B2S_FAIL(B2S_ERR_BAD_STATE, "a b2s_matcher_correlate_scan_begin awaits its _end: the handle cannot change state in between");
+  if (b2s_status st = refuse_if_pending(m)) return st;
   if (!m || !global_best || !tie_sums || !probs || !results) B2S_FAIL(B2S_ERR_BAD_PARAMS, "null argument");
   if (!m->have_sweep) B2S_FAIL(B2S_ERR_BAD_STATE, "b2s_matcher_correlate_split_begin must come first");
   B2S_CUDA_CHECK(cudaSetDevice(m->device));
   const int B = m->batch;
-  const size_t plen = (size_t)((m->g.search_side + 7) & ~7) * m->g.search_side;
+  const size_t plen = probs_len(m->g.search_side);
   B2S_CUDA_CHECK(cudaMemcpyAsync(m->d_glob_best, global_best, sizeof(double) * B, cudaMemcpyHostToDevice, m->stream));
   B2S_CUDA_CHECK(cudaMemcpyAsync(m->d_tie, tie_sums, sizeof(double) * 5 * B, cudaMemcpyHostToDevice, m->stream));
   B2S_CUDA_CHECK(cudaMemcpyAsync(m->d_probs, probs, sizeof(double) * plen * B, cudaMemcpyHostToDevice, m->stream));
-  b2s_status st = split_phase(m, 3);
+  b2s_status st = split_phase(m, REDUCE_SPLIT_FINISH);
   if (st) return st;
   B2S_CUDA_CHECK(cudaMemcpyAsync(m->h_results, m->d_results, sizeof(b2s_match_result) * B, cudaMemcpyDeviceToHost, m->stream));
   B2S_CUDA_CHECK(cudaStreamSynchronize(m->stream));
@@ -2005,19 +2008,19 @@ b2s_status b2s_matcher_correlate_scan_split(b2s_matcher *m, void *nccl_comm, int
     B2S_FAIL(B2S_ERR_BAD_PARAMS, "null / bad argument");
   if (m->pending) B2S_FAIL(B2S_ERR_BAD_STATE, "a b2s_matcher_correlate_scan_begin awaits its _end");
   if (search->fine) B2S_FAIL(B2S_ERR_BAD_PARAMS, "only the coarse stage (doingFineMatch = false) can be split");
-  if (!m->scans_set || !m->grids_set) B2S_FAIL(B2S_ERR_BAD_STATE, "scans and grids must be set first");
+  if (b2s_status st = require_scans_and_grids(m)) return st;
   const NcclApi &nc = nccl_api();
   if (!nc.ok) B2S_FAIL(B2S_ERR_BAD_STATE, "libnccl.so.2 could not be loaded (dlopen)");
   B2S_CUDA_CHECK(cudaSetDevice(m->device));
   for (auto &e : m->ev_split)
     if (!e) B2S_CUDA_CHECK(e.create());
   const int B = m->batch;
-  const size_t plen = (size_t)((m->g.search_side + 7) & ~7) * m->g.search_side;
+  const size_t plen = probs_len(m->g.search_side);
   const int na_full = n_steps(search->angle_offset, search->angle_res);
   const int base = na_full / world, extra = na_full % world;  // contiguous, balanced (parallel.shard_bounds)
   const int k_first = rank * base + std::min(rank, extra), k_count = base + (rank < extra ? 1 : 0);
   B2S_CUDA_CHECK(cudaMemcpyAsync(m->d_centers, centers, sizeof(double) * 3 * B, cudaMemcpyHostToDevice, m->stream));
-  b2s_status st = run_correlate(m, search, k_first, k_count, 1);
+  b2s_status st = run_correlate(m, search, k_first, k_count, REDUCE_SPLIT_BEST);
   if (st) return st;
   k_status_pack<<<ceil_div(B, 128), 128, 0, m->stream>>>(m->d_results, m->d_status, B);
   auto check_nccl = [&](int rc, const char *what) -> b2s_status {
@@ -2032,11 +2035,11 @@ b2s_status b2s_matcher_correlate_scan_split(b2s_matcher *m, void *nccl_comm, int
   if ((st = check_nccl(nc.all_reduce(m->d_status, m->d_status, (size_t)B, NCCL_INT32, NCCL_MAX, nccl_comm, m->stream), "ncclAllReduce(status)"))) return st;
   B2S_CUDA_CHECK(cudaEventRecord(m->ev_split[2], m->stream));
   B2S_CUDA_CHECK(cudaMemsetAsync(m->d_tie, 0, sizeof(double) * 5 * B, m->stream));
-  if ((st = split_phase(m, 2))) return st;
+  if ((st = split_phase(m, REDUCE_SPLIT_TIES))) return st;
   B2S_CUDA_CHECK(cudaEventRecord(m->ev_split[3], m->stream));
   if ((st = check_nccl(nc.all_reduce(m->d_tie, m->d_tie, (size_t)5 * B, NCCL_FLOAT64, NCCL_SUM, nccl_comm, m->stream), "ncclAllReduce(ties)"))) return st;
   B2S_CUDA_CHECK(cudaEventRecord(m->ev_split[4], m->stream));
-  if ((st = split_phase(m, 3))) return st;
+  if ((st = split_phase(m, REDUCE_SPLIT_FINISH))) return st;
   k_status_apply<<<ceil_div(B, 128), 128, 0, m->stream>>>(m->d_results, m->d_status, B);
   B2S_CUDA_CHECK(cudaGetLastError());
   B2S_CUDA_CHECK(cudaEventRecord(m->ev_split[5], m->stream));
@@ -2088,10 +2091,7 @@ b2s_status b2s_matcher_last_timing(b2s_matcher *m, double out[4]) {
   if (!m || !out) B2S_FAIL(B2S_ERR_BAD_PARAMS, "null argument");
   if (m->have_sweep && !m->pending && cudaSetDevice(m->device) == cudaSuccess && cudaStreamSynchronize(m->stream) == cudaSuccess) {
     // the events of the LAST sweep (whichever entry point ran it: correlate_scan, match_scan's last stage, a split phase)
-    for (int i = 0; i < 3; i++) {
-      float ms = 0;
-      if (cudaEventElapsedTime(&ms, m->ev[i], m->ev[i + 1]) == cudaSuccess) m->last_ms[i] = ms;
-    }
+    read_sweep_ms(m);
     cudaGetLastError();
   }
   out[0] = m->last_ms[0]; out[1] = m->last_ms[1]; out[2] = m->last_ms[2]; out[3] = (double)m->last_path;
@@ -2103,122 +2103,65 @@ b2s_status b2s_matcher_last_timing(b2s_matcher *m, double out[4]) {
 namespace b2s {
 
 // One CorrelateScan over the batch with centres already in d_centers.  Results stay in d_results.
-static b2s_status run_correlate(b2s_matcher *m, const b2s_search *s, int k_first, int na_override, int mode) {
+static b2s_status run_correlate(b2s_matcher *m, const b2s_search *s, int k_first, int na_override, ReducePhase phase) {
   B2S_NVTX("K1 correlate (lists + sweep + tail)");
-  if (s->angle_res == 0.0 || s->res_x == 0.0 || s->res_y == 0.0)
-    B2S_FAIL(B2S_ERR_BAD_PARAMS, "search resolutions must be non-zero");  // assert at Mapper.cpp:319
-  const int B = m->batch, n = m->n;
-  const int nx = n_steps(s->offset_x, s->res_x), ny = n_steps(s->offset_y, s->res_y);
-  const int na_full = n_steps(s->angle_offset, s->angle_res);
-  const int na = na_override >= 0 ? na_override : na_full;  // angles swept by THIS call (a subset when the sweep is split)
-  if (k_first < 0 || k_first + na > na_full) B2S_FAIL(B2S_ERR_BAD_PARAMS, "angle subset outside the search");
-  if (nx <= 0 || ny <= 0 || na_full <= 0 || (long long)nx * ny * std::max(na, 1) > (1ll << 28))
-    B2S_FAIL(B2S_ERR_TOO_LARGE, "search volume too large");
+  const SweepPlan pl = plan_sweep(m->p, m->g, *s, m->n, m->batch, k_first, na_override, m->force_kernel, m->sat_valid,
+                                  m->grid_high_bytes, m->sbx, m->sby, m->num_sms, m->smem_optin, m->win_static_smem);
+  if (pl.status) B2S_FAIL(pl.status, pl.error);
+  const int B = m->batch, n = m->n, nx = pl.nx, ny = pl.ny, na = pl.na, ncell = nx * ny;
   const double scale = 1.0 / m->p.resolution;
-  const int ncell = nx * ny;
-  b2s_status st;
+  const bool lists = pl.use_window && na > 0;
   B2S_CUDA_CHECK(m->d_sums.reserve((size_t)B * na * ncell));
   B2S_CUDA_CHECK(m->d_bases.reserve((size_t)B * ncell));
-
-  // ---- which sweep kernel ----
-  // The window kernel needs a stride-1 lattice and a band of the grid in shared memory: the whole grid when it fits
-  // (nbands = 1), otherwise nbands row bands of band_rows origin rows + (window rows + 1) halo rows each.
-  const int copy_bytes = (m->g.data_size + 15) & ~15;
-  // candidate stride in grid cells: 1 (search resolution == grid resolution) or 2 (the coarse stage of MatchScan,
-  // Mapper.cpp:233-234); anything else goes to the generic kernel
-  const double gres = 1.0 / (1.0 / m->p.resolution);
-  auto stride_of = [&](double r) { return (r == gres || r == m->p.resolution) ? 1 : ((r == 2 * gres || r == 2 * m->p.resolution) ? 2 : 0); };
-  const int stride = (stride_of(s->res_x) == stride_of(s->res_y)) ? stride_of(s->res_x) : 0;
-  const int cpt = stride == 2 ? 16 : 32;  // candidates per 32-byte tile row
-  const int tiles_x_w = (nx + cpt - 1) / cpt, tiles_y_w = (ny + 31) / 32;
-  const int rows_total = tiles_y_w * 32;
-  const int halo_rows = std::max(stride, 1) * 31 + 2;  // rows below the first row of a 32-row candidate tile that a lane may touch
-  // static shared memory of the sweep kernel (its own + the fused tail's scratch) comes out of the opt-in budget
-  static size_t win_static = 0;
-  if (!win_static) {
-    cudaFuncAttributes fa;
-    B2S_CUDA_CHECK(cudaFuncGetAttributes(&fa, k_sweep_window<1, false>));
-    win_static = fa.sharedSizeBytes;
+  if (pl.need_plain_lut) B2S_CUDA_CHECK(m->d_lut.reserve((size_t)B * na * std::max(n, 1)));
+  if (lists) {
+    B2S_CUDA_CHECK(m->d_lists.reserve((size_t)B * na * (n + LIST_PAD * pl.nbands)));
+    B2S_CUDA_CHECK(m->d_counts.reserve((size_t)B * na * 8 * pl.nbands));
+    B2S_CUDA_CHECK(m->d_starts.reserve((size_t)B * na * 8 * pl.nbands));
   }
-  const long long smem_limit = (long long)m->smem_optin - (long long)win_static - 512;
-  int band_rows = std::max(m->g.height, 1), nbands = 1, band_bytes = copy_bytes, neg_bands = 0;
-  bool bands_ok = true;
-  if ((long long)copy_bytes + 2 * WIN_GUARD > smem_limit) {
-    const long long rows_fit = (smem_limit - 2 * WIN_GUARD) / m->g.width_step;
-    band_rows = (int)((rows_fit - halo_rows) & ~1LL);  // even: band starts stay 16-byte aligned (width_step % 8 == 0)
-    if (band_rows < 8) {
-      bands_ok = false;
-    } else {
-      // origins up to (window rows) below the grid still reach it from their upper row tiles: bands of their own
-      neg_bands = tiles_y_w > 1 ? (std::max(stride, 1) * (rows_total - 1) + 1 + band_rows - 1) / band_rows : 0;
-      nbands = (m->g.height + band_rows - 1) / band_rows + neg_bands;
-      band_bytes = (int)((long long)(band_rows + halo_rows) * m->g.width_step);
-      if (nbands > WIN_MAX_BANDS) bands_ok = false;
-    }
-  }
-  const size_t win_smem = (size_t)((band_bytes + 15) & ~15) + 2 * WIN_GUARD;
-  const bool win_fits = bands_ok && stride != 0 && (m->g.width_step % 8) == 0 && n > 0 &&
-                        (size_t)n * OFF_SMEM_PER_BEAM + 64 <= 200 * 1024 && !m->grid_high_bytes;
-  bool use_window = win_fits;
-  if (m->force_kernel == 1) use_window = false;
-  if (m->force_kernel >= 2 && !win_fits)
-    B2S_FAIL(B2S_ERR_TOO_LARGE, "window kernel forced but not applicable to this lattice / grid / beam count");
-  if (m->force_kernel >= 2) use_window = true;
-  const bool need_plain_lut = !use_window || s->fine;  // generic sweep and the angular covariance read the plain table
-  if (need_plain_lut) B2S_CUDA_CHECK(m->d_lut.reserve((size_t)B * na * std::max(n, 1)));
 
+  // ---- candidate bases, lookup tables, window lists ----
   B2S_CUDA_CHECK(cudaEventRecord(m->ev[0], m->stream));
   k_bases<<<B, 256, 0, m->stream>>>(m->d_centers, m->d_grid_off, *s, m->g, scale, nx, ny, m->d_bases, m->d_flags,
-                                    std::max(stride, 1));
-  if (need_plain_lut && na > 0)
+                                    std::max(pl.stride, 1));
+  if (pl.need_plain_lut && na > 0)
     k_offsets<<<B * na, 256, 0, m->stream>>>(m->d_ranges, m->d_local, m->d_grid_off, m->d_centers, 3, 0.0, 0,
                                              s->angle_offset, s->angle_res, na, n, m->g.width_step, scale, m->d_lut, k_first);
-  const dim3 ggrid((unsigned)ceil_div(ncell, 8), (unsigned)B);
-  if (use_window && na > 0) {
-    B2S_CUDA_CHECK(m->d_lists.reserve((size_t)B * na * (n + LIST_PAD * nbands)));
-    B2S_CUDA_CHECK(m->d_counts.reserve((size_t)B * na * 8 * nbands));
-    B2S_CUDA_CHECK(m->d_starts.reserve((size_t)B * na * 8 * nbands));
-    bool skip_empty = m->sat_valid && m->force_kernel != 3;
-    if ((((size_t)n * OFF_SMEM_PER_BEAM + 15) & ~(size_t)15) + sizeof(uint16_t) * (size_t)((((m->sbx + 1) * (m->sby + 1)) + 7) & ~7) + 64 > 200 * 1024) skip_empty = false;
-    const size_t sat_bytes = skip_empty ? sizeof(uint16_t) * (size_t)((((m->sbx + 1) * (m->sby + 1)) + 7) & ~7) : 0;
-    const size_t osm = (((size_t)n * OFF_SMEM_PER_BEAM + 15) & ~(size_t)15) + sat_bytes + 64;
+  if (lists) {
     B2S_CUDA_CHECK(cudaMemsetAsync(m->d_stats, 0, sizeof(unsigned long long), m->stream));
-    if (osm > 16 * 1024)  // static + dynamic shared memory together must stay under the 48 KB default: opt in early
-      B2S_CUDA_CHECK(raise_dyn_smem(k_offsets_sorted, osm));
-    k_offsets_sorted<<<B * ((na + OFF_CHUNK - 1) / OFF_CHUNK), 256, osm, m->stream>>>(
+    if (pl.osm > 16 * 1024)  // static + dynamic shared memory together must stay under the 48 KB default: opt in early
+      B2S_CUDA_CHECK(raise_dyn_smem(k_offsets_sorted, pl.osm));
+    k_offsets_sorted<<<B * ((na + OFF_CHUNK - 1) / OFF_CHUNK), 256, pl.osm, m->stream>>>(
         m->d_ranges, m->d_local, m->d_grid_off, m->d_centers, m->d_bases, m->d_flags, s->angle_offset, s->angle_res, na, n,
-        ncell, m->g.width_step, m->g.data_size, scale, rows_total, tiles_x_w * 32, m->d_lists, m->d_counts,
-        skip_empty ? m->d_sat.p : nullptr, m->sbx, m->sby, m->g.height, nx, ny, m->d_stats, band_rows, nbands, m->d_starts,
-        stride, k_first, neg_bands);
+        ncell, m->g.width_step, m->g.data_size, scale, pl.rows_total, pl.tiles_x * 32, m->d_lists, m->d_counts,
+        pl.skip_empty ? m->d_sat.p : nullptr, m->sbx, m->sby, m->g.height, nx, ny, m->d_stats, pl.band_rows, pl.nbands,
+        m->d_starts, pl.stride, k_first, pl.neg_bands);
   }
   B2S_CUDA_CHECK(cudaGetLastError());
   B2S_CUDA_CHECK(cudaEventRecord(m->ev[1], m->stream));
 
   // ---- response sweep ----
   if (na == 0) {
-    m->last_path = use_window ? 2 : 1;  // empty angle subset of a split sweep: nothing to sweep
-  } else if (use_window) {
+    m->last_path = pl.use_window ? 2 : 1;  // empty angle subset of a split sweep: nothing to sweep
+  } else if (pl.use_window) {
     B2S_CUDA_CHECK(cudaMemsetAsync(m->d_work, 0, sizeof(int), m->stream));
-    if (nbands > 1)  // bands accumulate with RED.ADD
+    if (pl.nbands > 1)  // bands accumulate with RED.ADD
       B2S_CUDA_CHECK(cudaMemsetAsync(m->d_sums, 0, sizeof(int32_t) * (size_t)B * na * ncell, m->stream));
-    const int ctas = (int)std::min<long long>((long long)B * nbands * (nbands > 1 ? tiles_y_w : 1), m->num_sms);
     // (A variant that ran each match's fp64 tail inside the sweep CTA right after its last tile — volume read back from
     // L2, no k_reduce pass — was built, parity-tested and measured SLOWER on cfg 2 (not re-measured on the H100): the
     // sweep kernel owns its SM, so the tail's serial stretches are no longer hidden by a second resident CTA as they are
     // in the stand-alone k_reduce.  Removed again; DESIGN.md §4.)
-    // the GEN = false instantiation assumes exactly two lanes per row-start bank (see win_load)
-    const int bank_step = ((m->g.width_step >> 2) * std::max(stride, 1)) & 31;
-    const bool gen = (bank_step & 3) != 2;
     auto launch = [&](auto kern) -> b2s_status {
-      B2S_CUDA_CHECK(raise_dyn_smem(kern, win_smem));
-      kern<<<ctas, WIN_THREADS, win_smem, m->stream>>>(m->d_grids, m->grid_pitch, m->g.data_size, copy_bytes, m->d_lists,
-                                                       m->d_counts, m->d_starts, m->d_flags, B, n, na, nx, ny,
-                                                       m->g.width_step, m->d_sums, m->d_work, band_rows, nbands,
-                                                       band_bytes, neg_bands);
+      B2S_CUDA_CHECK(raise_dyn_smem(kern, pl.win_smem));
+      kern<<<pl.ctas, WIN_THREADS, pl.win_smem, m->stream>>>(m->d_grids, m->grid_pitch, m->g.data_size, pl.copy_bytes,
+                                                             m->d_lists, m->d_counts, m->d_starts, m->d_flags, B, n, na,
+                                                             nx, ny, m->g.width_step, m->d_sums, m->d_work, pl.band_rows,
+                                                             pl.nbands, pl.band_bytes, pl.neg_bands);
       return B2S_OK;
     };
-    if (stride == 2) st = gen ? launch(k_sweep_window<2, true>) : launch(k_sweep_window<2, false>);
-    else st = gen ? launch(k_sweep_window<1, true>) : launch(k_sweep_window<1, false>);
+    b2s_status st;
+    if (pl.stride == 2) st = pl.gen ? launch(k_sweep_window<2, true>) : launch(k_sweep_window<2, false>);
+    else st = pl.gen ? launch(k_sweep_window<1, true>) : launch(k_sweep_window<1, false>);
     if (st) return st;
     // matches whose lattice is not the regular raster (a centre exactly on a rounding tie) fall through;
     // they compute their lookup values on the fly (no table was materialised for them)
@@ -2229,23 +2172,21 @@ static b2s_status run_correlate(b2s_matcher *m, const b2s_search *s, int k_first
                                                   m->g.width_step, scale, k_first);
     m->last_path = 2;
   } else {
-    k_sweep_generic<<<ggrid, 256, 0, m->stream>>>(m->d_grids, m->grid_pitch, m->g.data_size, m->d_lut, m->d_bases,
-                                                  m->d_flags, 0, n, na, ncell, m->d_sums, m->d_ranges, m->d_local,
-                                                  m->d_grid_off, m->d_centers, s->angle_offset, s->angle_res,
-                                                  m->g.width_step, scale, k_first);
+    k_sweep_generic<<<dim3((unsigned)ceil_div(ncell, 8), (unsigned)B), 256, 0, m->stream>>>(
+        m->d_grids, m->grid_pitch, m->g.data_size, m->d_lut, m->d_bases, m->d_flags, 0, n, na, ncell, m->d_sums,
+        m->d_ranges, m->d_local, m->d_grid_off, m->d_centers, s->angle_offset, s->angle_res, m->g.width_step, scale,
+        k_first);
     m->last_path = 1;
   }
   B2S_CUDA_CHECK(cudaGetLastError());
   B2S_CUDA_CHECK(cudaEventRecord(m->ev[2], m->stream));
 
   // ---- fp64 tail ----
-  k_reduce<<<B, RED_THREADS, 0, m->stream>>>(reduce_args(m, *s, nx, ny, na, k_first, mode));
-  if (s->fine) {
-    size_t sm = sizeof(double) * (size_t)na;
-    if (sm > 48 * 1024) B2S_FAIL(B2S_ERR_TOO_LARGE, "too many angles for the angular-covariance kernel");
-    k_angular_cov<<<B, 256, sm, m->stream>>>(m->d_grids, m->grid_pitch, m->g, m->d_grid_off, m->d_lut, m->d_centers, *s,
-                                             scale, n, na, m->d_results);
-  }
+  k_reduce<<<B, RED_THREADS, 0, m->stream>>>(reduce_args(m, *s, nx, ny, na, k_first, phase));
+  if (s->fine)  // plan_sweep refused angle counts whose responses do not fit in 48 KB
+    k_angular_cov<<<B, 256, sizeof(double) * (size_t)na, m->stream>>>(m->d_grids, m->grid_pitch, m->g, m->d_grid_off,
+                                                                      m->d_lut, m->d_centers, *s, scale, n, na,
+                                                                      m->d_results);
   B2S_CUDA_CHECK(cudaGetLastError());
   B2S_CUDA_CHECK(cudaEventRecord(m->ev[3], m->stream));
   m->last.nx = nx; m->last.ny = ny; m->last.na = na;

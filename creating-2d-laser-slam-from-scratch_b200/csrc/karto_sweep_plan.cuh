@@ -1,0 +1,140 @@
+// The host-side plan of one Karto correlative sweep (karto_matcher.cu, run_correlate): which sweep kernel runs, the
+// candidate stride, the row-band geometry of the window kernel and the shared-memory sizes of the list and sweep stages,
+// or the refusal of the search.  Pure arithmetic on the handle's geometry with no CUDA call, so that it can be checked
+// on a machine without a GPU (tests/sweep_plan_check.cu).
+//
+// The kernels are correct only if these numbers are: the bands must cover every window origin row, and the staged image
+// must hold every row a lane touches.  The constants below are the ones the kernels and the plan must agree on.
+#pragma once
+
+#include "common.cuh"
+
+namespace b2s {
+
+constexpr int WIN_THREADS = 512;
+constexpr int WIN_GUARD = 128;          // zero bytes before and after the grid image in shared memory
+constexpr int WIN_MAX_BANDS = 32;       // row bands a grid larger than shared memory is swept in
+constexpr int LIST_PAD = 16;            // per-(match, angle) list capacity = n + LIST_PAD * nbands
+constexpr int OFF_CHUNK = 16;           // angles per k_offsets_sorted block
+constexpr int OFF_Q = 2;                              // angles classified per pass
+constexpr int OFF_SMEM_PER_BEAM = 16 + 5 * OFF_Q;     // two doubles + OFF_Q x (origin int32 + class byte)
+constexpr size_t LIST_SMEM_MAX = 200 * 1024;  // dynamic shared memory of the list stage and of the SAT build
+
+// u16 entries per match of the block summed-area tables (k_grid_sat), padded to 16 bytes
+inline size_t sat_stride(int sbx, int sby) { return (size_t)((((sbx + 1) * (sby + 1)) + 7) & ~7); }
+// doubles per match of the per-cell maxima plane (m_pSearchSpaceProbs), rows padded to 8
+inline size_t probs_len(int search_side) { return (size_t)((search_side + 7) & ~7) * search_side; }
+
+// ScanMatcher::Create (Mapper.cpp:126-172) + CorrelationGrid ctor (Mapper.h:920-1027) + Grid::Resize (Karto.h:4438)
+inline b2s_grid_info grid_layout(const b2s_matcher_params &p) {
+  b2s_grid_info g;
+  uint32_t side = cast_u32(kround(p.search_size / p.resolution) + 1);
+  uint32_t margin = cast_u32(ceil(p.range_threshold / p.resolution));
+  int32_t grid_size = (int32_t)(side + 2 * margin);
+  int32_t half_kernel = cast_i32(kround(2.0 * p.smear_deviation / p.resolution));
+  uint32_t border = (uint32_t)(half_kernel + 1);
+  g.width = grid_size + 2 * (int32_t)border;
+  g.height = grid_size + 2 * (int32_t)border;
+  g.width_step = (int32_t)(((size_t)g.width + 7) & ~(size_t)7);
+  g.data_size = g.width_step * g.height;
+  g.roi_x = g.roi_y = (int32_t)border;
+  g.roi_w = g.roi_h = grid_size;
+  g.kernel_size = 2 * half_kernel + 1;
+  g.search_side = (int32_t)side;
+  return g;
+}
+
+struct SweepPlan {
+  b2s_status status = B2S_OK;  // not B2S_OK: the search is refused for the reason in `error`, before any launch
+  const char *error = nullptr;
+  int nx = 0, ny = 0, na = 0;  // candidate lattice; na = the angles THIS call sweeps (a subset when the sweep is split)
+  int stride = 0;              // candidate stride in grid cells: 1, 2, or 0 (neither: generic kernel only)
+  bool use_window = false;     // k_sweep_window (+ k_offsets_sorted); otherwise k_sweep_generic
+  bool need_plain_lut = false; // the generic sweep and the angular covariance read the plain [nA][N] table
+  // window kernel: tiles of 32 candidate rows; a grid larger than shared memory is swept in nbands row bands of
+  // band_rows origin rows + halo_rows rows each, the first neg_bands of them for origins before row 0
+  int copy_bytes = 0, tiles_x = 0, tiles_y = 0, rows_total = 0, halo_rows = 0;
+  int band_rows = 0, nbands = 1, band_bytes = 0, neg_bands = 0;
+  size_t win_smem = 0;  // dynamic shared memory of the sweep: band image + guards
+  bool gen = false;     // k_sweep_window<., true>: the lanes' row starts are not two per bank
+  int ctas = 0;         // persistent sweep CTAs
+  // list stage (k_offsets_sorted)
+  bool skip_empty = false;  // drop empty windows through the block summed-area table
+  size_t osm = 0;           // its dynamic shared memory
+};
+
+// p, g: the handle's parameters and grid; n: beams; k_first / na_override: the angle subset of a split sweep
+// (na_override < 0: every angle); force_kernel: b2s_matcher_set_kernel; sat_valid / grid_high_bytes / sbx / sby: the
+// state of the grids; num_sms, smem_optin: the device's; win_static: the sweep kernel's static shared memory.
+inline SweepPlan plan_sweep(const b2s_matcher_params &p, const b2s_grid_info &g, const b2s_search &s, int n, int batch,
+                            int k_first, int na_override, int force_kernel, bool sat_valid, bool grid_high_bytes,
+                            int sbx, int sby, int num_sms, int smem_optin, size_t win_static) {
+  SweepPlan pl;
+  auto refuse = [&pl](b2s_status st, const char *why) {
+    pl.status = st;
+    pl.error = why;
+    return pl;
+  };
+  if (s.angle_res == 0.0 || s.res_x == 0.0 || s.res_y == 0.0)
+    return refuse(B2S_ERR_BAD_PARAMS, "search resolutions must be non-zero");  // assert at Mapper.cpp:319
+  pl.nx = n_steps(s.offset_x, s.res_x);
+  pl.ny = n_steps(s.offset_y, s.res_y);
+  const int na_full = n_steps(s.angle_offset, s.angle_res);
+  pl.na = na_override >= 0 ? na_override : na_full;
+  if (k_first < 0 || k_first + pl.na > na_full) return refuse(B2S_ERR_BAD_PARAMS, "angle subset outside the search");
+  if (pl.nx <= 0 || pl.ny <= 0 || na_full <= 0 || (long long)pl.nx * pl.ny * std::max(pl.na, 1) > (1ll << 28))
+    return refuse(B2S_ERR_TOO_LARGE, "search volume too large");
+
+  // The window kernel needs a stride-1 or stride-2 lattice and a band of the grid in shared memory: the whole grid when
+  // it fits (nbands = 1), otherwise nbands row bands.
+  pl.copy_bytes = (g.data_size + 15) & ~15;
+  // candidate stride in grid cells: 1 (search resolution == grid resolution) or 2 (the coarse stage of MatchScan,
+  // Mapper.cpp:233-234); anything else goes to the generic kernel
+  const double gres = 1.0 / (1.0 / p.resolution);
+  auto stride_of = [&](double r) { return (r == gres || r == p.resolution) ? 1 : ((r == 2 * gres || r == 2 * p.resolution) ? 2 : 0); };
+  pl.stride = (stride_of(s.res_x) == stride_of(s.res_y)) ? stride_of(s.res_x) : 0;
+  const int stride1 = std::max(pl.stride, 1);
+  const int cpt = pl.stride == 2 ? 16 : 32;  // candidates per 32-byte tile row
+  pl.tiles_x = (pl.nx + cpt - 1) / cpt;
+  pl.tiles_y = (pl.ny + 31) / 32;
+  pl.rows_total = pl.tiles_y * 32;
+  pl.halo_rows = stride1 * 31 + 2;  // rows below the first row of a 32-row candidate tile that a lane may touch
+  const long long smem_limit = (long long)smem_optin - (long long)win_static - 512;
+  pl.band_rows = std::max(g.height, 1);
+  pl.band_bytes = pl.copy_bytes;
+  bool bands_ok = true;
+  if ((long long)pl.copy_bytes + 2 * WIN_GUARD > smem_limit) {
+    const long long rows_fit = (smem_limit - 2 * WIN_GUARD) / g.width_step;
+    pl.band_rows = (int)((rows_fit - pl.halo_rows) & ~1LL);  // even: band starts stay 16-byte aligned (width_step % 8 == 0)
+    if (pl.band_rows < 8) {
+      bands_ok = false;
+    } else {
+      // origins up to (window rows) below the grid still reach it from their upper row tiles: bands of their own
+      pl.neg_bands = pl.tiles_y > 1 ? (stride1 * (pl.rows_total - 1) + 1 + pl.band_rows - 1) / pl.band_rows : 0;
+      pl.nbands = (g.height + pl.band_rows - 1) / pl.band_rows + pl.neg_bands;
+      pl.band_bytes = (int)((long long)(pl.band_rows + pl.halo_rows) * g.width_step);
+      if (pl.nbands > WIN_MAX_BANDS) bands_ok = false;
+    }
+  }
+  pl.win_smem = (size_t)((pl.band_bytes + 15) & ~15) + 2 * WIN_GUARD;
+  const bool win_fits = bands_ok && pl.stride != 0 && (g.width_step % 8) == 0 && n > 0 &&
+                        (size_t)n * OFF_SMEM_PER_BEAM + 64 <= LIST_SMEM_MAX && !grid_high_bytes;
+  if (force_kernel >= 2 && !win_fits)
+    return refuse(B2S_ERR_TOO_LARGE, "window kernel forced but not applicable to this lattice / grid / beam count");
+  pl.use_window = force_kernel >= 2 || (win_fits && force_kernel != 1);
+  pl.need_plain_lut = !pl.use_window || s.fine;
+  if (s.fine && sizeof(double) * (size_t)pl.na > 48 * 1024)
+    return refuse(B2S_ERR_TOO_LARGE, "too many angles for the angular-covariance kernel");
+
+  const size_t beams_bytes = ((size_t)n * OFF_SMEM_PER_BEAM + 15) & ~(size_t)15;
+  const size_t sat_bytes = sizeof(uint16_t) * sat_stride(sbx, sby);
+  pl.skip_empty = sat_valid && force_kernel != 3 && beams_bytes + sat_bytes + 64 <= LIST_SMEM_MAX;
+  pl.osm = beams_bytes + (pl.skip_empty ? sat_bytes : 0) + 64;
+  pl.ctas = (int)std::min<long long>((long long)batch * pl.nbands * (pl.nbands > 1 ? pl.tiles_y : 1), num_sms);
+  // the GEN = false instantiation assumes exactly two lanes per row-start bank (see win_load)
+  const int bank_step = ((g.width_step >> 2) * stride1) & 31;
+  pl.gen = (bank_step & 3) != 2;
+  return pl;
+}
+
+}  // namespace b2s
