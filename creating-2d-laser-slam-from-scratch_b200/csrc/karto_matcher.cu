@@ -17,7 +17,8 @@
 //   k_scan_points      point readings + scan-local points                              (fp64, O(B*N))
 //   k_grid_offsets     grid offset that centres the ROI on the scan's sensor position
 //   k_add_scan         FindValidPoints state machine + rasterise + max-smear           (byte atomics, O(B*S*N))
-//   k_add_scans_seq    the same, sequential, when an off-centre smear value reaches 100 (order-dependent)
+//   k_add_scans_seq    the same, sequential, when an off-centre smear value reaches 100 (order-dependent) or a base
+//                      scan does not fit in k_add_scan's shared memory
 //   k_grid_sat         per-match summed-area table of the grid's non-empty 4x4 blocks
 //   k_bases            candidate lattice -> flat base indices; flags irregular and out-of-grid lattices
 //   k_offsets          per-angle lookup tables                                         (fp64 -> i32)
@@ -120,6 +121,7 @@ struct b2s_matcher {
   int num_sms = 1;  // the device's, set at create
   int smem_optin = 0;
   size_t win_static_smem = 0;  // k_sweep_window's static shared memory: comes out of the opt-in budget of its image
+  size_t add_static_smem = 0;  // k_add_scan's, likewise for the base scan it stages
 
   Buf<uint8_t> d_kernel;
   Buf<double> d_ranges, d_poses, d_sensor, d_pts, d_local;
@@ -1525,6 +1527,8 @@ static b2s_status matcher_create_impl(const b2s_matcher_params *params, const b2
   cudaFuncAttributes fa;
   B2S_CUDA_CHECK(cudaFuncGetAttributes(&fa, k_sweep_window<1, false>));
   m->win_static_smem = fa.sharedSizeBytes;
+  B2S_CUDA_CHECK(cudaFuncGetAttributes(&fa, k_add_scan));
+  m->add_static_smem = fa.sharedSizeBytes;
   B2S_CUDA_CHECK(m->stream.init(cuda_stream));
   for (auto &e : m->ev) B2S_CUDA_CHECK(e.create());
   // smear kernel on the host with glibc, exactly CorrelationGrid::CalculateKernel (Mapper.h:1032-1087)
@@ -1666,10 +1670,12 @@ static b2s_status add_scans_impl(b2s_matcher *m, int n_base, const double *base_
       B2S_CUDA_CHECK(cudaMemcpyAsync(m->d_base_src, pool_rows, sizeof(int32_t) * need, cudaMemcpyHostToDevice, m->stream));
       k_scan_points<<<(unsigned)need, 256, 0, m->stream>>>(m->d_pool, m->d_base_poses, m->l, nullptr, m->d_base_pts, nullptr, m->d_base_src);
     }
-    if (!m->smear_degenerate) {
-      size_t smem = n * (2 * sizeof(double) + 2 * sizeof(int) + 1) + sizeof(int) + 16;
-      if (smem > 16 * 1024)
-        B2S_CUDA_CHECK(raise_dyn_smem(k_add_scan, smem));
+    // k_add_scan stages a whole base scan in shared memory (25 bytes per beam).  Beyond the device's opt-in limit
+    // (about 9 300 beams on an H100) the sequential kernel, exact for any beam count, builds the grids instead.
+    const size_t smem = n * (2 * sizeof(double) + 2 * sizeof(int) + 1) + sizeof(int) + 16;
+    const bool staged = !m->smear_degenerate && smem + m->add_static_smem <= (size_t)m->smem_optin;
+    if (staged && smem > 16 * 1024) B2S_CUDA_CHECK(raise_dyn_smem(k_add_scan, smem));
+    if (staged) {
       k_add_scan<<<(unsigned)need, 256, smem, m->stream>>>(m->d_base_pts, m->d_sensor, m->d_grid_off, m->d_grids,
                                                            m->grid_pitch, m->d_kernel, m->g, scale, (int)n, n_base);
     } else {
@@ -2183,10 +2189,13 @@ static b2s_status run_correlate(b2s_matcher *m, const b2s_search *s, int k_first
 
   // ---- fp64 tail ----
   k_reduce<<<B, RED_THREADS, 0, m->stream>>>(reduce_args(m, *s, nx, ny, na, k_first, phase));
-  if (s->fine)  // plan_sweep refused angle counts whose responses do not fit in 48 KB
+  if (s->fine) {  // plan_sweep refused angle counts whose responses do not fit in 48 KB
+    // the kernel's own static shared memory comes on top: 48 KB of responses (6 144 angles) needs the opt-in
+    if (sizeof(double) * (size_t)na > 16 * 1024) B2S_CUDA_CHECK(raise_dyn_smem(k_angular_cov, sizeof(double) * (size_t)na));
     k_angular_cov<<<B, 256, sizeof(double) * (size_t)na, m->stream>>>(m->d_grids, m->grid_pitch, m->g, m->d_grid_off,
                                                                       m->d_lut, m->d_centers, *s, scale, n, na,
                                                                       m->d_results);
+  }
   B2S_CUDA_CHECK(cudaGetLastError());
   B2S_CUDA_CHECK(cudaEventRecord(m->ev[3], m->stream));
   m->last.nx = nx; m->last.ny = ny; m->last.na = na;

@@ -130,7 +130,8 @@ b2s_status b2s_matcher_set_scans(b2s_matcher *m, int batch, const double *ranges
 
 /* MatchScan steps 1-4 + AddScans (Mapper.cpp:195-225, 699-811; Mapper.h:971-1005): centre grid b on scan
  * b's sensor pose and rasterise + smear its `n_base` base scans.  base_ranges: [batch][n_base][n_readings],
- * base_poses: [batch][n_base][3]. */
+ * base_poses: [batch][n_base][3].  Any beam count is accepted: scans too long for the parallel kernel's shared memory
+ * (more than about 9 300 beams on an H100) are rasterised by the sequential kernel, with the same grid bytes. */
 b2s_status b2s_matcher_add_scans(b2s_matcher *m, int n_base, const double *base_ranges, const double *base_poses);
 
 /* Scan pool: readings that serve as base scans of many matches (a mapper's running window, near chains, loop-closure
