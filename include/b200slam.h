@@ -653,6 +653,25 @@ b2s_status b2s_lidar_undistort(int batch, int n_beams, const float *ranges, doub
                                const double *imu_rot_y, const double *imu_rot_z, int imu_stride, float *out_xyz, int device,
                                void *cuda_stream);
 
+/* ---------------------------------------------------------------- lesson1: corner-feature extraction
+ * LaserScan::ScanCallback (lesson1/src/feature_detection.cc:77-179): the finite readings of a scan, a curvature
+ * c = d * d from an 11-reading stencil (:112-124), and in each of six sectors the first 20 entries above edge_threshold
+ * walked down a std::sort-ed range (:139-171).  Bit-identical to the node, ties included: where the 20th pick is tied
+ * the device sorts that sector with a restatement of libstdc++'s introsort.  Every call is stateless. */
+#define B2S_FEATURE_MAX_BEAMS 1500 /* max_scan_count (feature_detection.cc:23) */
+
+/* ranges [batch][n] (host) -> out_ranges [batch][n] (host): the first n entries of the published corner_scan.ranges,
+ * a picked beam's range and 0 elsewhere (the node's entries n .. 1499 are always 0; a picked range of 0 is invisible).
+ * out_count [batch] (may be NULL): the number of picks, or -1 for a scan with a NaN curvature (finite ranges of
+ * magnitude around 1e37 overflow the stencil both ways; the node's std::sort is undefined on it), whose out_ranges row
+ * is all 0.  out_curvature [batch][n] (may be NULL): c at the beam of each reading the stencil covers, NaN at every
+ * other beam; every NaN in it is the quiet NaN 0x7fc00000.  edge_threshold is the node's edge_threshold_ (1.0, :69).  B2S_ERR_BAD_PARAMS for a NULL ranges or
+ * out_ranges, batch < 0, n < 0, or a negative or NaN edge_threshold (which would pick the node's {0, 0} placeholders);
+ * B2S_ERR_TOO_LARGE for n > B2S_FEATURE_MAX_BEAMS, where the node overflows its buffer.  batch == 0 or n == 0 does
+ * nothing, but still requires a device.  Returns when the results are on the host. */
+b2s_status b2s_feature_detect(int batch, int n, const float *ranges, float edge_threshold, float *out_ranges,
+                              int32_t *out_count, float *out_curvature, int device, void *cuda_stream);
+
 #ifdef __cplusplus
 }
 #endif
