@@ -211,7 +211,10 @@ void orc_hector_grid_probabilities(const float *log_odds, int n, float *out) {
 static void interp(const orc_hmap *m, float x, float y, float out[3]) {
   float lim_x = (float)m->size_x - 2.0f, lim_y = (float)m->size_y - 2.0f; /* setMapCellDims: dims - 2 */
   if (x < 0.0f || x > lim_x || y < 0.0f || y > lim_y) { out[0] = out[1] = out[2] = 0.0f; return; }
-  int ix = (int)x, iy = (int)y;
+  /* A NaN coordinate (a pose that went through a singular Hessian) passes the test above.  The reference's (int) of
+   * NaN is undefined (x86 gives INT_MIN and reads far outside the map); here it is 0, as the device's conversion
+   * (cvt.rzi.s32.f32) gives, so the read stays inside and the NaN reaches the outputs through fx / fy. */
+  int ix = x == x ? (int)x : 0, iy = y == y ? (int)y : 0;
   float fx = x - (float)ix, fy = y - (float)iy;
   int index = iy * m->size_x + ix;
   float i0 = grid_prob(m, index), i1 = grid_prob(m, index + 1);
@@ -309,6 +312,7 @@ typedef struct {
   float origo[ORC_HPROC_MAX_LEVELS][2];
   float last_map_update_pose[3], last_scan_match_pose[3], last_cov[9];
   float min_dist, min_angle;
+  int map_updated; /* the last update()'s gate decision (the device handle reports it per scan) */
 } orc_hproc;
 
 orc_hproc *orc_hproc_create(float resolution, int size_x, int size_y, float start_x, float start_y, int levels) {
@@ -390,7 +394,8 @@ void orc_hproc_update(orc_hproc *p, const float *points, int n, const float orig
     memcpy(est, pose_hint, sizeof(est));
   }
   memcpy(p->last_scan_match_pose, est, sizeof(est));
-  if (pose_difference_larger_than(est, p->last_map_update_pose, p->min_dist, p->min_angle) || map_without_matching) {
+  p->map_updated = pose_difference_larger_than(est, p->last_map_update_pose, p->min_dist, p->min_angle) || map_without_matching;
+  if (p->map_updated) {
     /* MapRepMultiMap::updateByScan (:174-191): the coarse levels use dataContainers filled by the LAST matchData —
      * with map_without_matching they are stale (empty before the first match); reproduced as is */
     for (int l = 0; l < p->levels; l++) {
@@ -402,6 +407,8 @@ void orc_hproc_update(orc_hproc *p, const float *points, int n, const float orig
   memcpy(out_pose, est, sizeof(est));
   if (out_cov && !map_without_matching) memcpy(out_cov, p->last_cov, sizeof(p->last_cov));
 }
+
+int orc_hproc_map_updated(const orc_hproc *p) { return p->map_updated; }
 
 int orc_hproc_level_dims(const orc_hproc *p, int level, int dims[2]) {
   if (level < 0 || level >= p->levels) return -1;

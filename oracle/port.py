@@ -297,6 +297,7 @@ class PortHectorProcessor:
         pose, cov = np.zeros(3, np.float32), np.zeros(9, np.float32)
         self.L.orc_hproc_update(self.h, _p(p, C.c_float), len(p), _p(o, C.c_float), _p(w, C.c_float),
                                 int(map_without_matching), _p(pose, C.c_float), _p(cov, C.c_float))
+        self.map_updated = bool(self.L.orc_hproc_map_updated(self.h))  # the gate's decision, as HectorSlam reports it
         return pose, cov.reshape(3, 3)
 
     def level(self, i):
