@@ -113,16 +113,20 @@ __global__ void __launch_bounds__(256)
   }
 }
 
-// GMapping::PublishMap thresholding (gmapping.cc:141-159) into width x height (MAP_IDX = width*y + x)
+// GMapping::PublishMap thresholding (gmapping.cc:141-159) into width x height (MAP_IDX = width*y + x).  One thread per
+// published byte.  Storage cells (x + k*width, y - k) all land on byte (x, y); the reference loops x outer, y inner,
+// so the one with the largest x is written last and wins.  msx <= width + 1, so only storage cell (width, y - 1) can
+// shadow (0, y).  A byte no storage cell maps to keeps the caller's 0.
 __global__ void k_gm_ros(const int32_t *__restrict__ n, const int32_t *__restrict__ visits, int msx, int msy,
                          double occ_thresh, int width, int height, int8_t *__restrict__ out) {
-  int c = blockIdx.x * blockDim.x + threadIdx.x;
-  if (c >= msx * msy) return;
-  const int x = c % msx, y = c / msx;
+  const long long o = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (o >= (long long)width * height) return;
+  int x = (int)(o % width), y = (int)(o / width);
+  if (x == 0 && y > 0 && width < msx && y - 1 < msy) { x = width; y -= 1; }
+  if (x >= msx || y >= msy) return;
+  const size_t c = (size_t)x + (size_t)y * msx;
   const int v = visits[c];
   const double occ = v ? (double)n[c] * 1 / (double)v : -1;
-  const size_t o = (size_t)width * y + x;
-  if (o >= (size_t)width * height) return;
   out[o] = occ < 0 ? -1 : (occ > occ_thresh ? 100 : 0);
 }
 
@@ -231,8 +235,8 @@ b2s_status b2s_gmap_copy_ros(b2s_gmap *g, int8_t *out) {
   AsyncBuf<int8_t> d(g->stream);
   B2S_CUDA_CHECK(d.alloc((size_t)width * height));
   B2S_CUDA_CHECK(cudaMemsetAsync(d, 0, (size_t)width * height, g->stream));
-  k_gm_ros<<<ceil_div((long long)g->msx * g->msy, 256), 256, 0, g->stream>>>(g->d_n, g->d_visits, g->msx, g->msy, 0.25,
-                                                                            width, height, d);
+  k_gm_ros<<<ceil_div((long long)width * height, 256), 256, 0, g->stream>>>(g->d_n, g->d_visits, g->msx, g->msy, 0.25,
+                                                                          width, height, d);
   B2S_CUDA_CHECK(cudaGetLastError());
   B2S_CUDA_CHECK(cudaMemcpyAsync(out, d, (size_t)width * height, cudaMemcpyDeviceToHost, g->stream));
   B2S_CUDA_CHECK(cudaStreamSynchronize(g->stream));

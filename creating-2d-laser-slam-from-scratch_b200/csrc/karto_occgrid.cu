@@ -241,7 +241,8 @@ static b2s_status occ_create_impl(const b2s_laser *laser, int n_scans, const dou
   b2s_occ_grid_info &I = g->info;
   I.width = cast_i32(kround((bb[2] - bb[0]) * scale));
   I.height = cast_i32(kround((bb[3] - bb[1]) * scale));
-  if (I.width < 0 || I.height < 0 || (long long)I.width * I.height > (1ll << 31))
+  // the counters hold width_step * height cells (rows padded to 8), indexed and sized in int32
+  if (I.width < 0 || I.height < 0 || I.width > INT32_MAX - 7 || ((long long)I.width + 7) / 8 * 8 * I.height > INT32_MAX)
     B2S_FAIL(B2S_ERR_TOO_LARGE, "occupancy grid dimensions out of range");
   I.width_step = (I.width + 7) & ~7;
   I.data_size = I.width_step * I.height;
