@@ -17,7 +17,9 @@
 // no host round trip between scans (b2s_hector_slam_process_stream: ONE cooperative kernel walks the whole stream;
 // b2s_hector_slam_update: one launch per scan, the pose comes back through a host-mapped mailbox as soon as the match
 // is done while the map update still runs).  A handle holds B independent processors (independent robots / maps,
-// SURVEY.md §8(e): "shard over independent maps"); B = 1 is the reference's single processor.
+// SURVEY.md §8(e): "shard over independent maps"); B = 1 is the reference's single processor.  They step together one
+// scan each (b2s_hector_slam_update_batch: three launches per step), or each walks its own recording in ONE launch, one
+// CTA per processor (b2s_hector_slam_process_stream_batch).
 //
 // Arithmetic: float32 in the reference's operation order, no FMA (-fmad=false).  EXACT mode (default) reproduces the
 // reference bit for bit: the nine sums of getCompleteHessianDerivs are accumulated sequentially in point order (one lane
@@ -108,6 +110,8 @@ struct HsCall {  // one scan per processor
   unsigned int seq;
   unsigned int tag;     // != 0: published (release, gpu scope) in out[b][15] once the scan's state is complete
   float *carry;         // shared-memory [3] or NULL: receives the scan-match pose (the next scan's hint in a stream)
+  int own_row = 0;      // 0: row b of hints / out / n0 is processor b's; != 0: they already point at this CTA's scan
+                        // (row 0), whatever b is — a processor walking its own stream (k_hs_stream_batch)
 };
 
 __device__ __forceinline__ unsigned long long hs_now_ns() {
@@ -291,7 +295,8 @@ __device__ bool hs_match_cta(const HsBatch &P, const HsCall &C, int b, unsigned 
   HsState *st = P.state + b;
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   constexpr int NW = HS_THREADS / 32;
-  const int n = C.n0 ? C.n0[b] : C.n0_uniform;
+  const int row = C.own_row ? 0 : b;  // row of C.hints / C.out / C.n0
+  const int n = C.n0 ? C.n0[row] : C.n0_uniform;
   constexpr bool exact = EXACT;  // compile-time: each mode's kernel carries only its own code
   const bool use_fma = P.use_fma != 0;
   float2 *spts = reinterpret_cast<float2 *>(smem);
@@ -338,7 +343,7 @@ __device__ bool hs_match_cta(const HsBatch &P, const HsCall &C, int b, unsigned 
     reinterpret_cast<float2 *>(P.l[0].pts)[(size_t)b * P.cap + i] = p;  // level-0 container for the update passes
   }
   if (tid == 0) {
-    const float *h = C.hints ? C.hints + 3 * b : st->last_match_pose;
+    const float *h = C.hints ? C.hints + 3 * row : st->last_match_pose;
     s_world[0] = h[0]; s_world[1] = h[1]; s_world[2] = h[2];
   }
   __syncthreads();
@@ -543,7 +548,7 @@ __device__ bool hs_match_cta(const HsBatch &P, const HsCall &C, int b, unsigned 
       st->last_update_pose[0] = est[0]; st->last_update_pose[1] = est[1]; st->last_update_pose[2] = est[2];
       st->n_updated += 1;
     }
-    float *o = C.out + 16 * (size_t)b;
+    float *o = C.out + 16 * (size_t)row;
     o[0] = est[0]; o[1] = est[1]; o[2] = est[2];
     for (int q = 0; q < 9; q++) o[3 + q] = lcov[q];
     o[12] = do_update ? 1.0f : 0.0f;
@@ -598,7 +603,7 @@ __device__ bool hs_match_cta(const HsBatch &P, const HsCall &C, int b, unsigned 
   if (C.tag) {
     __syncthreads();  // the bounding boxes (other threads' stores) are ordered before the release below
     if (tid == 0)
-      asm volatile("st.release.gpu.global.u32 [%0], %1;" ::"l"(C.out + 16 * (size_t)b + 15), "r"(C.tag) : "memory");
+      asm volatile("st.release.gpu.global.u32 [%0], %1;" ::"l"(C.out + 16 * (size_t)row + 15), "r"(C.tag) : "memory");
   }
   return verdict;
 }
@@ -914,6 +919,61 @@ __global__ void __launch_bounds__(HS_THREADS, 1) k_hs_stream(HsBatch P, HsStream
   }
 }
 
+// ---- batched streams: ONE launch, one CTA per processor, each walking its own recording ----
+struct HsFleet {
+  const float *pts;          // every scan's points, processor-major ([sum n_points][2])
+  const long long *offsets;  // [total scans] first point of each scan (64-bit: a fleet's recordings exceed 2^31 floats)
+  const int *counts;         // [total scans]
+  const long long *first;    // [B + 1] first scan of processor b (scans first[b] ... first[b + 1] - 1)
+  const float *hints;        // [total scans][3] or NULL (chain through the processor's last scan-match pose)
+  const float *first_hints;  // [B][3] or NULL: hint of each processor's first scan when chaining
+  float origo_x, origo_y;
+  int map_without_matching;
+  float *out;                // [total scans][16]
+};
+
+// The node's loop of processor b = blockIdx.x over its scans: match (hs_match_cta), then, if the gate opens, the mark
+// and apply passes on this CTA's 18 warps.  Nothing crosses CTAs: no grid barrier, no verdict tags, and B may exceed the
+// resident CTAs (later processors start as earlier ones finish).  The match reads the probability quads with plain
+// (L1-allocating, coherent) loads that the SAME CTA rewrote in its previous apply pass; the __syncthreads after the
+// apply orders those stores before the loads (CTA scope), so no L1 drop is needed as in k_hs_stream.
+template <bool EXACT>
+__global__ void __launch_bounds__(HS_THREADS, 1) k_hs_stream_batch(HsBatch P, HsFleet F) {
+  extern __shared__ __align__(16) unsigned char hs_smem[];
+  __shared__ float s_last[3];  // the previous scan's match pose: the next scan's hint without a global round trip
+  const int b = blockIdx.x;
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  constexpr int NW = HS_THREADS / 32;
+  HsState *st = P.state + b;
+  const long long s0 = F.first[b], s1 = F.first[b + 1];
+  unsigned long long visits = 0;
+  for (long long i = s0; i < s1; i++) {
+    HsCall C;
+    C.pts0 = F.pts + 2 * F.offsets[i];
+    C.n0 = nullptr;
+    C.n0_uniform = F.counts[i];
+    C.pts_stride = 0;
+    C.hints = F.hints ? F.hints + 3 * i : (i > s0 ? s_last : (F.first_hints ? F.first_hints + 3 * (size_t)b : nullptr));
+    C.origo_x = F.origo_x; C.origo_y = F.origo_y;
+    C.map_without_matching = F.map_without_matching;
+    C.out = F.out + 16 * i;
+    C.mailbox = nullptr;
+    C.seq = 0;
+    C.tag = 0;
+    C.carry = s_last;
+    C.own_row = 1;
+    if (hs_match_cta<EXACT, false>(P, C, b, hs_smem)) {
+      const unsigned long long t0 = hs_now_ns();
+      visits += hs_mark_pass(P, b, warp, NW, lane);  // (lane 0 carries the warp's count)
+      __syncthreads();
+      hs_apply_pass(P, b, warp, NW, lane);
+      __syncthreads();  // the next match reads the refreshed quads; the next gate rewrites the update parameters
+      if (threadIdx.x == 0) st->t_update_ns = hs_now_ns() - t0;
+    }
+  }
+  if (lane == 0 && visits) atomicAdd(&st->visits, visits);
+}
+
 __global__ void k_hs_fill(float *__restrict__ p, size_t n, float v) {
   const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i < n) p[i] = v;
@@ -1072,6 +1132,8 @@ static b2s_status hs_create(float map_resolution, int map_size_x, int map_size_y
   B2S_CUDA_CHECK(raise_dyn_smem(k_hs_stream<true, false>, smem));
   B2S_CUDA_CHECK(raise_dyn_smem(k_hs_stream<false, false>, smem));
   B2S_CUDA_CHECK(raise_dyn_smem(k_hs_stream<false, true>, smem));
+  B2S_CUDA_CHECK(raise_dyn_smem(k_hs_stream_batch<true>, smem));
+  B2S_CUDA_CHECK(raise_dyn_smem(k_hs_stream_batch<false>, smem));
   {
     int coop = 0, sms = 0, per_sm = 0;
     B2S_CUDA_CHECK(cudaDeviceGetAttribute(&coop, cudaDevAttrCooperativeLaunch, device));
@@ -1322,6 +1384,84 @@ b2s_status b2s_hector_slam_process_stream(b2s_hector_slam *p, int n_scans, const
   return B2S_OK;
 }
 
+b2s_status b2s_hector_slam_process_stream_batch(b2s_hector_slam *p, const int32_t *n_scans, const float *points,
+                                                const int32_t *n_points, const float origo[2],
+                                                const float *first_pose_hints, const float *pose_hints,
+                                                int map_without_matching, float *out_poses, int32_t *out_map_updated,
+                                                float *out_last_covs) {
+  B2S_NVTX("Hector batched streams");
+  if (!p || !n_scans || !origo || !out_poses) B2S_FAIL(B2S_ERR_BAD_PARAMS, "null argument");
+  if (map_without_matching && !pose_hints) B2S_FAIL(B2S_ERR_BAD_PARAMS, "map_without_matching needs a pose per scan (pose_hints)");
+  const int B = p->batch;
+  // every count is checked before anything is enqueued: a refused call changes nothing
+  std::vector<long long> first((size_t)B + 1);
+  long long total = 0;
+  int longest = 0;
+  for (int b = 0; b < B; b++) {
+    if (n_scans[b] < 0) B2S_FAIL(B2S_ERR_BAD_PARAMS, "negative scan count");
+    first[b] = total;
+    total += n_scans[b];
+    longest = std::max(longest, (int)n_scans[b]);
+  }
+  first[B] = total;
+  if (total > 0 && (!points || !n_points)) B2S_FAIL(B2S_ERR_BAD_PARAMS, "null argument");
+  if ((unsigned)longest >= HS_EPOCH_MAX) B2S_FAIL(B2S_ERR_TOO_LARGE, "too many scans of one processor in one call (stamp epochs are 20 bits)");
+  std::vector<long long> offs((size_t)total);
+  long long n_pts = 0;
+  for (long long i = 0; i < total; i++) {
+    if (n_points[i] < 0) B2S_FAIL(B2S_ERR_BAD_PARAMS, "negative point count");
+    if (n_points[i] > p->cap) B2S_FAIL(B2S_ERR_TOO_LARGE, "a scan has more points than the handle's capacity");
+    offs[(size_t)i] = n_pts;
+    n_pts += n_points[i];
+  }
+  if (total == 0) return B2S_OK;
+  B2S_CUDA_CHECK(cudaSetDevice(p->device));
+  b2s_status st = hs_wait_launch(p);
+  if (st) return st;
+  if ((st = hs_reserve_epochs(p, (unsigned long long)longest))) return st;  // a processor's epochs advance once per scan at most
+  AsyncBuf<float> d_pts(p->stream), d_hints(p->stream), d_first_hints(p->stream), d_out(p->stream);
+  AsyncBuf<long long> d_offs(p->stream), d_first(p->stream);
+  AsyncBuf<int> d_cnt(p->stream);
+  const size_t T = (size_t)total;
+  B2S_CUDA_CHECK(d_pts.alloc(2 * (size_t)std::max<long long>(n_pts, 1)));
+  B2S_CUDA_CHECK(d_offs.alloc(T));
+  B2S_CUDA_CHECK(d_cnt.alloc(T));
+  B2S_CUDA_CHECK(d_first.alloc((size_t)B + 1));
+  B2S_CUDA_CHECK(d_out.alloc(16 * T));
+  if (n_pts > 0) B2S_CUDA_CHECK(cudaMemcpyAsync(d_pts, points, sizeof(float) * 2 * (size_t)n_pts, cudaMemcpyHostToDevice, p->stream));
+  B2S_CUDA_CHECK(cudaMemcpyAsync(d_offs, offs.data(), sizeof(long long) * T, cudaMemcpyHostToDevice, p->stream));
+  B2S_CUDA_CHECK(cudaMemcpyAsync(d_cnt, n_points, sizeof(int) * T, cudaMemcpyHostToDevice, p->stream));
+  B2S_CUDA_CHECK(cudaMemcpyAsync(d_first, first.data(), sizeof(long long) * ((size_t)B + 1), cudaMemcpyHostToDevice, p->stream));
+  if (pose_hints) {
+    B2S_CUDA_CHECK(d_hints.alloc(3 * T));
+    B2S_CUDA_CHECK(cudaMemcpyAsync(d_hints, pose_hints, sizeof(float) * 3 * T, cudaMemcpyHostToDevice, p->stream));
+  } else if (first_pose_hints) {
+    B2S_CUDA_CHECK(d_first_hints.alloc(3 * (size_t)B));
+    B2S_CUDA_CHECK(cudaMemcpyAsync(d_first_hints, first_pose_hints, sizeof(float) * 3 * (size_t)B, cudaMemcpyHostToDevice, p->stream));
+  }
+  HsFleet F;
+  F.pts = d_pts; F.offsets = d_offs; F.counts = d_cnt; F.first = d_first;
+  F.hints = d_hints; F.first_hints = d_first_hints;
+  F.origo_x = origo[0]; F.origo_y = origo[1];
+  F.map_without_matching = map_without_matching;
+  F.out = d_out;
+  const size_t smem = hs_smem_bytes(p->cap);
+  if (p->P.exact) k_hs_stream_batch<true><<<B, HS_THREADS, smem, p->stream>>>(p->P, F);
+  else k_hs_stream_batch<false><<<B, HS_THREADS, smem, p->stream>>>(p->P, F);
+  B2S_CUDA_CHECK(cudaGetLastError());
+  std::vector<float> host(16 * T);
+  B2S_CUDA_CHECK(cudaMemcpyAsync(host.data(), d_out, sizeof(float) * 16 * T, cudaMemcpyDeviceToHost, p->stream));
+  B2S_CUDA_CHECK(cudaStreamSynchronize(p->stream));
+  for (size_t i = 0; i < T; i++) {
+    std::memcpy(out_poses + 3 * i, host.data() + 16 * i, 3 * sizeof(float));
+    if (out_map_updated) out_map_updated[i] = host[16 * i + 12] != 0.0f ? 1 : 0;
+  }
+  if (out_last_covs && !map_without_matching)
+    for (int b = 0; b < B; b++)
+      if (n_scans[b] > 0) std::memcpy(out_last_covs + 9 * (size_t)b, host.data() + 16 * (size_t)(first[b + 1] - 1) + 3, 9 * sizeof(float));
+  return B2S_OK;
+}
+
 b2s_status b2s_hector_slam_update_batch(b2s_hector_slam *p, const float *points, const int32_t *n_points, const float origo[2],
                                         const float *pose_hints, int map_without_matching, float *out_poses, float *out_covs,
                                         int32_t *out_map_updated) {
@@ -1432,19 +1572,23 @@ b2s_status b2s_hector_slam_copy_level(b2s_hector_slam *p, int level, float *log_
   return b2s_hector_slam_copy_level_of(p, 0, level, log_odds, update_index);
 }
 
-b2s_status b2s_hector_slam_copy_level_ros(b2s_hector_slam *p, int level, int8_t *out) {
-  if (!p || !out || level < 0 || level >= p->levels) B2S_FAIL(B2S_ERR_BAD_PARAMS, "bad level");
+b2s_status b2s_hector_slam_copy_level_ros_of(b2s_hector_slam *p, int b, int level, int8_t *out) {
+  if (!p || !out || level < 0 || level >= p->levels || b < 0 || b >= p->batch) B2S_FAIL(B2S_ERR_BAD_PARAMS, "bad level / processor");
   B2S_CUDA_CHECK(cudaSetDevice(p->device));
   const HsLevel &m = p->P.l[level];
   const int n = m.sx * m.sy;
   AsyncBuf<int8_t> d(p->stream);
   B2S_CUDA_CHECK(d.alloc((size_t)n));
-  k_hector_ros<<<ceil_div(n, 256), 256, 0, p->stream>>>(m.lo, n, d);
+  k_hector_ros<<<ceil_div(n, 256), 256, 0, p->stream>>>(m.lo + (size_t)b * n, n, d);
   B2S_CUDA_CHECK(cudaGetLastError());
   B2S_CUDA_CHECK(cudaMemcpyAsync(out, d, (size_t)n, cudaMemcpyDeviceToHost, p->stream));
   B2S_CUDA_CHECK(cudaStreamSynchronize(p->stream));
   p->launch_pending = false;
   return B2S_OK;
+}
+
+b2s_status b2s_hector_slam_copy_level_ros(b2s_hector_slam *p, int level, int8_t *out) {
+  return b2s_hector_slam_copy_level_ros_of(p, 0, level, out);
 }
 
 b2s_status b2s_hector_slam_stats(b2s_hector_slam *p, double out[5]) {

@@ -42,6 +42,8 @@ def _bind():
                                                C.c_int, vp, C.POINTER(vp)]
     L.b2s_hector_slam_set_exact.argtypes = [vp, C.c_int]
     L.b2s_hector_slam_process_stream.argtypes = [vp, C.c_int, fp, ip, fp, fp, fp, C.c_int, fp, ip, fp]
+    L.b2s_hector_slam_process_stream_batch.argtypes = [vp, ip, fp, ip, fp, fp, fp, C.c_int, fp, ip, fp]
+    L.b2s_hector_slam_copy_level_ros_of.argtypes = [vp, C.c_int, C.c_int, C.POINTER(C.c_int8)]
     L.b2s_hector_slam_update_batch.argtypes = [vp, fp, ip, fp, fp, C.c_int, fp, fp, ip]
     L.b2s_hector_slam_update_batch_device.argtypes = [vp, vp, vp, C.c_int, fp, vp, C.c_int]
     L.b2s_hector_slam_sync.argtypes = [vp]
@@ -165,6 +167,33 @@ class HectorSlam:
                                                     _f(poses), upd.ctypes.data_as(C.POINTER(C.c_int32)), _f(cov)))
         return poses, upd.astype(bool), cov.reshape(3, 3)
 
+    def process_stream_batch(self, streams, origo, first_hints=None, pose_hints=None, map_without_matching=False):
+        """Every processor of the handle over its own recording in one call.  streams: B lists of [n, 2] scans (an
+        empty list leaves that processor untouched); first_hints [B, 3]; pose_hints: B arrays [n_b, 3].  Returns
+        [(poses [n_b, 3], updated flags [n_b])] per processor and the last covariances [B, 3, 3] (zero where a processor
+        had no scans or with map_without_matching)."""
+        B = self.batch or 1
+        if len(streams) != B:
+            raise ValueError(f"{len(streams)} streams for a handle of {B} processors")
+        ns = np.array([len(s) for s in streams], np.int32)
+        scans = [f32(sc).reshape(-1, 2) for s in streams for sc in s]
+        cnt = np.array([len(sc) for sc in scans], np.int32)
+        cat = f32(np.concatenate(scans, 0)) if scans else np.zeros((0, 2), np.float32)
+        total = int(ns.sum())
+        poses, upd, covs = np.zeros((total, 3), np.float32), np.zeros(total, np.int32), np.zeros((B, 9), np.float32)
+        fh = f32(first_hints).reshape(B, 3) if first_hints is not None else None
+        ph = None
+        if pose_hints is not None:
+            ph = f32(np.concatenate([f32(h).reshape(-1, 3) for h in pose_hints], 0)) if total else np.zeros((0, 3), np.float32)
+        ip = C.POINTER(C.c_int32)
+        check(self.L.b2s_hector_slam_process_stream_batch(self.h, ns.ctypes.data_as(ip), _f(cat), cnt.ctypes.data_as(ip),
+                                                          _f(f32(origo)), _f(fh) if fh is not None else None,
+                                                          _f(ph) if ph is not None else None, int(map_without_matching),
+                                                          _f(poses), upd.ctypes.data_as(ip), _f(covs)))
+        edges = np.concatenate([[0], np.cumsum(ns)])
+        out = [(poses[edges[b]:edges[b + 1]], upd[edges[b]:edges[b + 1]].astype(bool)) for b in range(B)]
+        return out, covs.reshape(B, 3, 3)
+
     def update_batch(self, scans, origo, pose_hints, map_without_matching=False):
         """One scan per processor of a batched handle.  scans: list of B [n_b, 2] arrays."""
         B = self.batch
@@ -229,6 +258,13 @@ class HectorSlam:
         sx, sy, _ = self.level_dims(i)
         out = np.zeros((sy, sx), np.int8)
         check(self.L.b2s_hector_slam_copy_level_ros(self.h, i, out.ctypes.data_as(C.POINTER(C.c_int8))))
+        return out
+
+    def ros_map_of(self, b, level=0):
+        """nav_msgs/OccupancyGrid payload of processor b's level."""
+        sx, sy, _ = self.level_dims(level)
+        out = np.zeros((sy, sx), np.int8)
+        check(self.L.b2s_hector_slam_copy_level_ros_of(self.h, b, level, out.ctypes.data_as(C.POINTER(C.c_int8))))
         return out
 
     def stats(self):

@@ -487,6 +487,25 @@ b2s_status b2s_hector_slam_update_batch_device(b2s_hector_slam *p, const float *
 b2s_status b2s_hector_slam_sync(b2s_hector_slam *p);
 b2s_status b2s_hector_slam_copy_level_of(b2s_hector_slam *p, int processor, int level, float *log_odds,
                                          int32_t *update_index);
+/* nav_msgs/OccupancyGrid payload of one processor's level (b2s_hector_slam_copy_level_ros is processor 0's) */
+b2s_status b2s_hector_slam_copy_level_ros_of(b2s_hector_slam *p, int processor, int level, int8_t *out);
+/* b2s_hector_slam_process_stream for EVERY processor of the handle in one call, each over its own recording (any
+ * handle, B = 1 included).  n_scans [B] (0: the processor is left untouched); scans are processor-major: processor b's
+ * scans follow processor b-1's, n_points [sum n_scans] and the points ([sum n_points][2], level-0 map-cell units) in the
+ * same order.  Hint of a processor's scan i = its pose of scan i-1 (first_pose_hints[b] for its first scan; NULL = its
+ * current last scan-match pose), or pose_hints [sum n_scans][3] when given (required with map_without_matching).
+ * out_poses [sum n_scans][3]; out_map_updated [sum n_scans] and out_last_covs [B][9] (the level-0 Hessian of the
+ * processor's last scan; its row is untouched when it has no scans or with map_without_matching) may be NULL.
+ * Processor b's poses, gate decisions, Hessian, last poses and cells are those of b2s_hector_slam_process_stream over
+ * its scans on a single-processor handle with the same settings; two calls over consecutive parts of every recording
+ * equal one.  ONE launch, one CTA per processor (nothing shared between them: B may exceed the resident CTAs).
+ * Refused before anything is enqueued: B2S_ERR_BAD_PARAMS for NULL arrays or negative counts, B2S_ERR_TOO_LARGE for a
+ * scan above the handle's max_points or a processor with 2^20 - 1 or more scans. */
+b2s_status b2s_hector_slam_process_stream_batch(b2s_hector_slam *p, const int32_t *n_scans, const float *points,
+                                                const int32_t *n_points, const float origo[2],
+                                                const float *first_pose_hints, const float *pose_hints,
+                                                int map_without_matching, float *out_poses, int32_t *out_map_updated,
+                                                float *out_last_covs);
 /* getLastScanMatchPose / getLastMapUpdatePose (HectorSlamProcessor.h:118-119) of one processor; either may be NULL */
 b2s_status b2s_hector_slam_last_poses(b2s_hector_slam *p, int processor, float last_scan_match_pose[3],
                                       float last_map_update_pose[3]);
