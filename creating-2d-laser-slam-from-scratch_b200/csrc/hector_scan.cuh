@@ -1,0 +1,89 @@
+// lesson4's LaserScan -> DataContainer conversion, per beam, shared by the host adapters (ros_io.cu: b2s_ros_hector_points,
+// b2s_ros_hector_scans) and the ingest stage of the batched stream kernel (hector_slam.cu: k_hs_stream_batch<_, true>).
+// HectorMappingRos::scanCallback (lesson4/src/hector_mapping/hector_slam.cc:186-205) does two things to a scan:
+//   projector_.projectLaser(scan, cloud, 30.0)     laser_geometry's LaserProjection (not in the reference tree, see
+//                                                  DESIGN §7: restated from the package's published behaviour)
+//   rosPointCloudToDataContainer                    hector_slam.cc:320-362 (pinned by tests/test_ros_io.py)
+// Only IEEE multiply / add / compare / convert here: the transcendental values (the beams' unit vectors, the laser yaw's
+// cosine and sine) are the host C library's, computed by the caller and passed in, so the device and the host adapter
+// produce the same points bit for bit under the library's -fmad=false.
+#pragma once
+#include <cmath>
+
+#include "common.cuh"
+
+namespace b2s {
+
+// The node's settings of rosPointCloudToDataContainer, prepared once per call (hector_scan_filter).
+struct HectorScanFilter {
+  float sqr_min, sqr_max;      // min_dist^2, max_dist^2 in float (hector_slam.cc:151-155)
+  double use_max_scan_range;
+  double lx, ly, lz, c, s;     // tf::Transform of the laser in base_link (tfScalar = double): translation, cos / sin of yaw
+  float z_min, z_max;
+  float scale_to_map;
+};
+
+// laser_in_base = (x, y, z, yaw) as float; cos / sin of the yaw are taken in double by the host C library
+inline HectorScanFilter hector_scan_filter(const float laser_in_base[4], float scale_to_map, float min_dist, float max_dist,
+                                           double use_max_scan_range, float z_min, float z_max) {
+  HectorScanFilter f;
+  f.sqr_min = min_dist * min_dist;
+  f.sqr_max = max_dist * max_dist;
+  f.use_max_scan_range = use_max_scan_range;
+  f.lx = laser_in_base[0]; f.ly = laser_in_base[1]; f.lz = laser_in_base[2];
+  f.c = cos((double)laser_in_base[3]);
+  f.s = sin((double)laser_in_base[3]);
+  f.z_min = z_min; f.z_max = z_max;
+  f.scale_to_map = scale_to_map;
+  return f;
+}
+
+// rosPointCloudToDataContainer on one laser-frame point: true if the node keeps it, with its DataContainer entry
+// (base_link position in map-cell units) in (ox, oy)
+__host__ __device__ __forceinline__ bool hector_filter_point(const HectorScanFilter &f, float x, float y, float z, float &ox,
+                                                             float &oy) {
+  const float dist_sqr = x * x + y * y;
+  if (!((dist_sqr > f.sqr_min) && (dist_sqr < f.sqr_max))) return false;
+  if ((x < 0.0f) && (dist_sqr < 0.50f)) return false;  // behind the robot
+  if ((double)dist_sqr > f.use_max_scan_range * f.use_max_scan_range) return false;
+  const double bx = f.c * (double)x - f.s * (double)y + f.lx, by = f.s * (double)x + f.c * (double)y + f.ly;
+  const double bz = (double)z + f.lz;
+  const float z_laser = (float)(bz - f.lz);
+  if (!(z_laser > f.z_min && z_laser < f.z_max)) return false;
+  ox = (float)bx * f.scale_to_map;
+  oy = (float)by * f.scale_to_map;
+  return true;
+}
+
+// LaserProjection::projectLaser (sensor_msgs::PointCloud form) on beam i: kept iff range < cutoff (double) and
+// range >= range_min (float); NaN and +-inf drop out.  Point32 x / y = (float)(range * unit vector), z = 0.
+__host__ __device__ __forceinline__ bool hector_project_beam(float range, double ux, double uy, double cutoff, float range_min,
+                                                             float &x, float &y) {
+  if (!(((double)range < cutoff) && (range >= range_min))) return false;
+  x = (float)((double)range * ux);
+  y = (float)((double)range * uy);
+  return true;
+}
+
+// Both stages on one beam
+__host__ __device__ __forceinline__ bool hector_scan_beam(const HectorScanFilter &f, float range, double ux, double uy,
+                                                          double cutoff, float range_min, float &ox, float &oy) {
+  float x, y;
+  if (!hector_project_beam(range, ux, uy, cutoff, range_min, x, y)) return false;
+  return hector_filter_point(f, x, y, 0.0f, ox, oy);
+}
+
+// getUnitVectors_: cos / sin(angle_min + (double)i * angle_increment) in double by the host C library, the float32 message
+// fields widened; interleaved [n][2].  angle_max only names laser_geometry's cache.
+inline void hector_unit_vectors(float angle_min, float angle_increment, int n, double *out) {
+  for (int i = 0; i < n; i++) {
+    const double a = (double)angle_min + (double)i * (double)angle_increment;
+    out[2 * i] = cos(a);
+    out[2 * i + 1] = sin(a);
+  }
+}
+
+// projectLaser's cutoff: a negative range_cutoff means the message's range_max
+inline double hector_range_cutoff(double range_cutoff, float range_max) { return range_cutoff < 0.0 ? (double)range_max : range_cutoff; }
+
+}  // namespace b2s

@@ -19,7 +19,8 @@
 // is done while the map update still runs).  A handle holds B independent processors (independent robots / maps,
 // SURVEY.md §8(e): "shard over independent maps"); B = 1 is the reference's single processor.  They step together one
 // scan each (b2s_hector_slam_update_batch: three launches per step), or each walks its own recording in ONE launch, one
-// CTA per processor (b2s_hector_slam_process_stream_batch).
+// CTA per processor (b2s_hector_slam_process_stream_batch; b2s_hector_slam_process_scans_batch takes the raw LaserScan
+// ranges and converts each scan inside that launch).
 //
 // Arithmetic: float32 in the reference's operation order, no FMA (-fmad=false).  EXACT mode (default) reproduces the
 // reference bit for bit: the nine sums of getCompleteHessianDerivs are accumulated sequentially in point order (one lane
@@ -47,6 +48,7 @@
 #include "common.cuh"
 #include "glibc_math.cuh"
 #include "hector_grid.cuh"
+#include "hector_scan.cuh"
 
 using namespace b2s;
 
@@ -930,6 +932,18 @@ struct HsFleet {
   float origo_x, origo_y;
   int map_without_matching;
   float *out;                // [total scans][16]
+  const struct HsIngest *ingest;  // device: the ingest variant's input (k_hs_stream_batch<_, true>), else NULL
+};
+
+// Scans as raw LaserScan ranges (k_hs_stream_batch<_, true>): F.pts / offsets / counts are unused.  In device memory
+// behind one pointer: a larger kernel parameter block costs the existing instantiations registers.
+struct HsIngest {
+  const float *ranges;       // [total scans][n_ranges] float32
+  const double2 *units;      // [n_ranges] the beams' unit vectors (host C library cos / sin)
+  int n_ranges;
+  float range_min;
+  double range_cutoff;       // projectLaser's cutoff (a negative one already replaced by range_max)
+  HectorScanFilter filter;
 };
 
 // The node's loop of processor b = blockIdx.x over its scans: match (hs_match_cta), then, if the gate opens, the mark
@@ -937,7 +951,13 @@ struct HsFleet {
 // resident CTAs (later processors start as earlier ones finish).  The match reads the probability quads with plain
 // (L1-allocating, coherent) loads that the SAME CTA rewrote in its previous apply pass; the __syncthreads after the
 // apply orders those stores before the loads (CTA scope), so no L1 drop is needed as in k_hs_stream.
-template <bool EXACT>
+//
+// INGEST: each scan arrives as n_ranges float32 ranges.  Before its match the CTA converts it (hector_scan.cuh: the
+// node's projectLaser + rosPointCloudToDataContainer, per beam) and compacts the kept beams in beam order into its level-0
+// container row, HS_THREADS beams per round: ballot / popc inside a warp, warp offsets through shared memory, a running
+// base across rounds.  hs_match_cta then reads that row as its input and copies it onto itself: each element is read and
+// written back unchanged by the same thread, which is benign.
+template <bool EXACT, bool INGEST>
 __global__ void __launch_bounds__(HS_THREADS, 1) k_hs_stream_batch(HsBatch P, HsFleet F) {
   extern __shared__ __align__(16) unsigned char hs_smem[];
   __shared__ float s_last[3];  // the previous scan's match pose: the next scan's hint without a global round trip
@@ -949,9 +969,44 @@ __global__ void __launch_bounds__(HS_THREADS, 1) k_hs_stream_batch(HsBatch P, Hs
   unsigned long long visits = 0;
   for (long long i = s0; i < s1; i++) {
     HsCall C;
-    C.pts0 = F.pts + 2 * F.offsets[i];
-    C.n0 = nullptr;
-    C.n0_uniform = F.counts[i];
+    if constexpr (INGEST) {
+      __shared__ int s_warp_kept[NW];
+      const HsIngest &I = *F.ingest;
+      float2 *row = reinterpret_cast<float2 *>(P.l[0].pts) + (size_t)b * P.cap;
+      const int nr = I.n_ranges;
+      const float *r = I.ranges + (size_t)i * nr;
+      int base = 0;
+      for (int c0 = 0; c0 < nr; c0 += HS_THREADS) {
+        const int j = c0 + (int)threadIdx.x;
+        float2 q = make_float2(0.0f, 0.0f);
+        bool keep = false;
+        if (j < nr) {
+          const double2 u = I.units[j];
+          keep = hector_scan_beam(I.filter, r[j], u.x, u.y, I.range_cutoff, I.range_min, q.x, q.y);
+        }
+        const unsigned m = __ballot_sync(0xffffffffu, keep);
+        if (lane == 0) s_warp_kept[warp] = __popc(m);
+        __syncthreads();
+        int off = base, round = 0;
+#pragma unroll
+        for (int w = 0; w < NW; w++) {
+          const int k = s_warp_kept[w];
+          off += w < warp ? k : 0;
+          round += k;
+        }
+        if (keep) row[off + __popc(m & ((1u << lane) - 1u))] = q;
+        base += round;
+        __syncthreads();  // s_warp_kept is rewritten by the next round; the row is read by the match
+      }
+      if (threadIdx.x == 0) F.out[16 * i + 15] = __int_as_float(base);  // the scan's kept-beam count for the host
+      C.pts0 = P.l[0].pts + 2 * (size_t)b * P.cap;
+      C.n0 = nullptr;
+      C.n0_uniform = base;
+    } else {
+      C.pts0 = F.pts + 2 * F.offsets[i];
+      C.n0 = nullptr;
+      C.n0_uniform = F.counts[i];
+    }
     C.pts_stride = 0;
     C.hints = F.hints ? F.hints + 3 * i : (i > s0 ? s_last : (F.first_hints ? F.first_hints + 3 * (size_t)b : nullptr));
     C.origo_x = F.origo_x; C.origo_y = F.origo_y;
@@ -1132,8 +1187,10 @@ static b2s_status hs_create(float map_resolution, int map_size_x, int map_size_y
   B2S_CUDA_CHECK(raise_dyn_smem(k_hs_stream<true, false>, smem));
   B2S_CUDA_CHECK(raise_dyn_smem(k_hs_stream<false, false>, smem));
   B2S_CUDA_CHECK(raise_dyn_smem(k_hs_stream<false, true>, smem));
-  B2S_CUDA_CHECK(raise_dyn_smem(k_hs_stream_batch<true>, smem));
-  B2S_CUDA_CHECK(raise_dyn_smem(k_hs_stream_batch<false>, smem));
+  B2S_CUDA_CHECK(raise_dyn_smem(k_hs_stream_batch<true, false>, smem));
+  B2S_CUDA_CHECK(raise_dyn_smem(k_hs_stream_batch<false, false>, smem));
+  B2S_CUDA_CHECK(raise_dyn_smem(k_hs_stream_batch<true, true>, smem));
+  B2S_CUDA_CHECK(raise_dyn_smem(k_hs_stream_batch<false, true>, smem));
   {
     int coop = 0, sms = 0, per_sm = 0;
     B2S_CUDA_CHECK(cudaDeviceGetAttribute(&coop, cudaDevAttrCooperativeLaunch, device));
@@ -1218,6 +1275,79 @@ static b2s_status hs_launch_stream(b2s_hector_slam *p, const HsStream &S) {
     else k_hs_stream<false, false><<<1, HS_THREADS, smem, p->stream>>>(P, Sv);
     B2S_CUDA_CHECK(cudaGetLastError());
   }
+  return B2S_OK;
+}
+
+// Processor b's scans of a batched call are first[b] ... first[b + 1] - 1 (first has B + 1 entries).  Refuses negative
+// counts; `longest` is the most scans of one processor.
+static b2s_status hs_fleet_counts(const b2s_hector_slam *p, const int32_t *n_scans, std::vector<long long> &first, int &longest) {
+  const int B = p->batch;
+  first.assign((size_t)B + 1, 0);
+  long long total = 0;
+  longest = 0;
+  for (int b = 0; b < B; b++) {
+    if (n_scans[b] < 0) B2S_FAIL(B2S_ERR_BAD_PARAMS, "negative scan count");
+    first[b] = total;
+    total += n_scans[b];
+    longest = std::max(longest, (int)n_scans[b]);
+  }
+  first[B] = total;
+  return B2S_OK;
+}
+
+// The body the batched stream calls share, once the caller has checked its inputs: hint uploads, ONE k_hs_stream_batch
+// launch and the read-back.  `upload(F)` enqueues the scans (points, or raw ranges for INGEST) and fills F's input fields.
+template <class Upload>
+static b2s_status hs_fleet_run(b2s_hector_slam *p, const int32_t *n_scans, const std::vector<long long> &first, int longest,
+                               bool ingest, const float *first_pose_hints, const float *pose_hints, int map_without_matching,
+                               float *out_poses, int32_t *out_map_updated, float *out_last_covs, int32_t *out_n_points,
+                               Upload &upload) {
+  const int B = p->batch;
+  const size_t T = (size_t)first[(size_t)B];
+  if (T == 0) return B2S_OK;
+  B2S_CUDA_CHECK(cudaSetDevice(p->device));
+  b2s_status st = hs_wait_launch(p);
+  if (st) return st;
+  if ((st = hs_reserve_epochs(p, (unsigned long long)longest))) return st;  // a processor's epochs advance once per scan at most
+  HsFleet F;
+  std::memset(&F, 0, sizeof(F));
+  if ((st = upload(F))) return st;
+  AsyncBuf<float> d_hints(p->stream), d_first_hints(p->stream), d_out(p->stream);
+  AsyncBuf<long long> d_first(p->stream);
+  B2S_CUDA_CHECK(d_first.alloc((size_t)B + 1));
+  B2S_CUDA_CHECK(d_out.alloc(16 * T));
+  B2S_CUDA_CHECK(cudaMemcpyAsync(d_first, first.data(), sizeof(long long) * ((size_t)B + 1), cudaMemcpyHostToDevice, p->stream));
+  if (pose_hints) {
+    B2S_CUDA_CHECK(d_hints.alloc(3 * T));
+    B2S_CUDA_CHECK(cudaMemcpyAsync(d_hints, pose_hints, sizeof(float) * 3 * T, cudaMemcpyHostToDevice, p->stream));
+  } else if (first_pose_hints) {
+    B2S_CUDA_CHECK(d_first_hints.alloc(3 * (size_t)B));
+    B2S_CUDA_CHECK(cudaMemcpyAsync(d_first_hints, first_pose_hints, sizeof(float) * 3 * (size_t)B, cudaMemcpyHostToDevice, p->stream));
+  }
+  F.first = d_first;
+  F.hints = d_hints; F.first_hints = d_first_hints;
+  F.map_without_matching = map_without_matching;
+  F.out = d_out;
+  const size_t smem = hs_smem_bytes(p->cap);
+  if (ingest) {
+    if (p->P.exact) k_hs_stream_batch<true, true><<<B, HS_THREADS, smem, p->stream>>>(p->P, F);
+    else k_hs_stream_batch<false, true><<<B, HS_THREADS, smem, p->stream>>>(p->P, F);
+  } else {
+    if (p->P.exact) k_hs_stream_batch<true, false><<<B, HS_THREADS, smem, p->stream>>>(p->P, F);
+    else k_hs_stream_batch<false, false><<<B, HS_THREADS, smem, p->stream>>>(p->P, F);
+  }
+  B2S_CUDA_CHECK(cudaGetLastError());
+  std::vector<float> host(16 * T);
+  B2S_CUDA_CHECK(cudaMemcpyAsync(host.data(), d_out, sizeof(float) * 16 * T, cudaMemcpyDeviceToHost, p->stream));
+  B2S_CUDA_CHECK(cudaStreamSynchronize(p->stream));
+  for (size_t i = 0; i < T; i++) {
+    std::memcpy(out_poses + 3 * i, host.data() + 16 * i, 3 * sizeof(float));
+    if (out_map_updated) out_map_updated[i] = host[16 * i + 12] != 0.0f ? 1 : 0;
+    if (out_n_points) std::memcpy(out_n_points + i, host.data() + 16 * i + 15, sizeof(int32_t));  // (ingest) kept beams
+  }
+  if (out_last_covs && !map_without_matching)
+    for (int b = 0; b < B; b++)
+      if (n_scans[b] > 0) std::memcpy(out_last_covs + 9 * (size_t)b, host.data() + 16 * (size_t)(first[b + 1] - 1) + 3, 9 * sizeof(float));
   return B2S_OK;
 }
 
@@ -1392,18 +1522,12 @@ b2s_status b2s_hector_slam_process_stream_batch(b2s_hector_slam *p, const int32_
   B2S_NVTX("Hector batched streams");
   if (!p || !n_scans || !origo || !out_poses) B2S_FAIL(B2S_ERR_BAD_PARAMS, "null argument");
   if (map_without_matching && !pose_hints) B2S_FAIL(B2S_ERR_BAD_PARAMS, "map_without_matching needs a pose per scan (pose_hints)");
-  const int B = p->batch;
   // every count is checked before anything is enqueued: a refused call changes nothing
-  std::vector<long long> first((size_t)B + 1);
-  long long total = 0;
+  std::vector<long long> first;
   int longest = 0;
-  for (int b = 0; b < B; b++) {
-    if (n_scans[b] < 0) B2S_FAIL(B2S_ERR_BAD_PARAMS, "negative scan count");
-    first[b] = total;
-    total += n_scans[b];
-    longest = std::max(longest, (int)n_scans[b]);
-  }
-  first[B] = total;
+  b2s_status st = hs_fleet_counts(p, n_scans, first, longest);
+  if (st) return st;
+  const long long total = first[(size_t)p->batch];
   if (total > 0 && (!points || !n_points)) B2S_FAIL(B2S_ERR_BAD_PARAMS, "null argument");
   if ((unsigned)longest >= HS_EPOCH_MAX) B2S_FAIL(B2S_ERR_TOO_LARGE, "too many scans of one processor in one call (stamp epochs are 20 bits)");
   std::vector<long long> offs((size_t)total);
@@ -1414,52 +1538,74 @@ b2s_status b2s_hector_slam_process_stream_batch(b2s_hector_slam *p, const int32_
     offs[(size_t)i] = n_pts;
     n_pts += n_points[i];
   }
-  if (total == 0) return B2S_OK;
-  B2S_CUDA_CHECK(cudaSetDevice(p->device));
-  b2s_status st = hs_wait_launch(p);
-  if (st) return st;
-  if ((st = hs_reserve_epochs(p, (unsigned long long)longest))) return st;  // a processor's epochs advance once per scan at most
-  AsyncBuf<float> d_pts(p->stream), d_hints(p->stream), d_first_hints(p->stream), d_out(p->stream);
-  AsyncBuf<long long> d_offs(p->stream), d_first(p->stream);
+  AsyncBuf<float> d_pts(p->stream);
+  AsyncBuf<long long> d_offs(p->stream);
   AsyncBuf<int> d_cnt(p->stream);
-  const size_t T = (size_t)total;
-  B2S_CUDA_CHECK(d_pts.alloc(2 * (size_t)std::max<long long>(n_pts, 1)));
-  B2S_CUDA_CHECK(d_offs.alloc(T));
-  B2S_CUDA_CHECK(d_cnt.alloc(T));
-  B2S_CUDA_CHECK(d_first.alloc((size_t)B + 1));
-  B2S_CUDA_CHECK(d_out.alloc(16 * T));
-  if (n_pts > 0) B2S_CUDA_CHECK(cudaMemcpyAsync(d_pts, points, sizeof(float) * 2 * (size_t)n_pts, cudaMemcpyHostToDevice, p->stream));
-  B2S_CUDA_CHECK(cudaMemcpyAsync(d_offs, offs.data(), sizeof(long long) * T, cudaMemcpyHostToDevice, p->stream));
-  B2S_CUDA_CHECK(cudaMemcpyAsync(d_cnt, n_points, sizeof(int) * T, cudaMemcpyHostToDevice, p->stream));
-  B2S_CUDA_CHECK(cudaMemcpyAsync(d_first, first.data(), sizeof(long long) * ((size_t)B + 1), cudaMemcpyHostToDevice, p->stream));
-  if (pose_hints) {
-    B2S_CUDA_CHECK(d_hints.alloc(3 * T));
-    B2S_CUDA_CHECK(cudaMemcpyAsync(d_hints, pose_hints, sizeof(float) * 3 * T, cudaMemcpyHostToDevice, p->stream));
-  } else if (first_pose_hints) {
-    B2S_CUDA_CHECK(d_first_hints.alloc(3 * (size_t)B));
-    B2S_CUDA_CHECK(cudaMemcpyAsync(d_first_hints, first_pose_hints, sizeof(float) * 3 * (size_t)B, cudaMemcpyHostToDevice, p->stream));
-  }
-  HsFleet F;
-  F.pts = d_pts; F.offsets = d_offs; F.counts = d_cnt; F.first = d_first;
-  F.hints = d_hints; F.first_hints = d_first_hints;
-  F.origo_x = origo[0]; F.origo_y = origo[1];
-  F.map_without_matching = map_without_matching;
-  F.out = d_out;
-  const size_t smem = hs_smem_bytes(p->cap);
-  if (p->P.exact) k_hs_stream_batch<true><<<B, HS_THREADS, smem, p->stream>>>(p->P, F);
-  else k_hs_stream_batch<false><<<B, HS_THREADS, smem, p->stream>>>(p->P, F);
-  B2S_CUDA_CHECK(cudaGetLastError());
-  std::vector<float> host(16 * T);
-  B2S_CUDA_CHECK(cudaMemcpyAsync(host.data(), d_out, sizeof(float) * 16 * T, cudaMemcpyDeviceToHost, p->stream));
-  B2S_CUDA_CHECK(cudaStreamSynchronize(p->stream));
-  for (size_t i = 0; i < T; i++) {
-    std::memcpy(out_poses + 3 * i, host.data() + 16 * i, 3 * sizeof(float));
-    if (out_map_updated) out_map_updated[i] = host[16 * i + 12] != 0.0f ? 1 : 0;
-  }
-  if (out_last_covs && !map_without_matching)
-    for (int b = 0; b < B; b++)
-      if (n_scans[b] > 0) std::memcpy(out_last_covs + 9 * (size_t)b, host.data() + 16 * (size_t)(first[b + 1] - 1) + 3, 9 * sizeof(float));
-  return B2S_OK;
+  auto upload = [&](HsFleet &F) -> b2s_status {
+    const size_t T = (size_t)total;
+    B2S_CUDA_CHECK(d_pts.alloc(2 * (size_t)std::max<long long>(n_pts, 1)));
+    B2S_CUDA_CHECK(d_offs.alloc(T));
+    B2S_CUDA_CHECK(d_cnt.alloc(T));
+    if (n_pts > 0) B2S_CUDA_CHECK(cudaMemcpyAsync(d_pts, points, sizeof(float) * 2 * (size_t)n_pts, cudaMemcpyHostToDevice, p->stream));
+    B2S_CUDA_CHECK(cudaMemcpyAsync(d_offs, offs.data(), sizeof(long long) * T, cudaMemcpyHostToDevice, p->stream));
+    B2S_CUDA_CHECK(cudaMemcpyAsync(d_cnt, n_points, sizeof(int) * T, cudaMemcpyHostToDevice, p->stream));
+    F.pts = d_pts; F.offsets = d_offs; F.counts = d_cnt;
+    F.origo_x = origo[0]; F.origo_y = origo[1];
+    return B2S_OK;
+  };
+  return hs_fleet_run(p, n_scans, first, longest, false, first_pose_hints, pose_hints, map_without_matching, out_poses,
+                      out_map_updated, out_last_covs, nullptr, upload);
+}
+
+b2s_status b2s_hector_slam_process_scans_batch(b2s_hector_slam *p, const b2s_laser_scan_msg *geometry,
+                                               const b2s_hector_scan_filter *filter, const int32_t *n_scans,
+                                               const float *ranges, const float *first_pose_hints, const float *pose_hints,
+                                               int map_without_matching, float *out_poses, int32_t *out_map_updated,
+                                               float *out_last_covs, int32_t *out_n_points) {
+  B2S_NVTX("Hector batched LaserScan streams");
+  if (!p || !geometry || !filter || !n_scans || !out_poses || geometry->n_ranges < 0)
+    B2S_FAIL(B2S_ERR_BAD_PARAMS, "null argument or negative count");
+  if (map_without_matching && !pose_hints) B2S_FAIL(B2S_ERR_BAD_PARAMS, "map_without_matching needs a pose per scan (pose_hints)");
+  const int n = geometry->n_ranges;
+  if (n > p->cap) B2S_FAIL(B2S_ERR_TOO_LARGE, "more ranges per scan than the handle's capacity");
+  std::vector<long long> first;
+  int longest = 0;
+  b2s_status st = hs_fleet_counts(p, n_scans, first, longest);
+  if (st) return st;
+  const long long total = first[(size_t)p->batch];
+  if (total > 0 && n > 0 && !ranges) B2S_FAIL(B2S_ERR_BAD_PARAMS, "null argument");
+  if ((unsigned)longest >= HS_EPOCH_MAX) B2S_FAIL(B2S_ERR_TOO_LARGE, "too many scans of one processor in one call (stamp epochs are 20 bits)");
+  const float scale_to_map = p->P.l[0].tf.tw_lin;  // GridMapBase::getScaleToMap of level 0: 1 / cell length
+  const b2s_hector_scan_filter &q = *filter;
+  const HectorScanFilter f = hector_scan_filter(q.laser_in_base, scale_to_map, q.min_dist, q.max_dist, q.use_max_scan_range,
+                                                q.z_min, q.z_max);
+  std::vector<double> unit(2 * (size_t)std::max(n, 1));
+  hector_unit_vectors(geometry->angle_min, geometry->angle_increment, n, unit.data());
+  AsyncBuf<float> d_ranges(p->stream);
+  AsyncBuf<double> d_unit(p->stream);
+  AsyncBuf<HsIngest> d_ingest(p->stream);
+  HsIngest I;  // (pageable: the copy is staged before cudaMemcpyAsync returns)
+  auto upload = [&](HsFleet &F) -> b2s_status {
+    const size_t nr = (size_t)total * (size_t)n;
+    B2S_CUDA_CHECK(d_ranges.alloc(std::max<size_t>(nr, 1)));
+    B2S_CUDA_CHECK(d_unit.alloc(unit.size()));
+    B2S_CUDA_CHECK(d_ingest.alloc(1));
+    if (nr > 0) B2S_CUDA_CHECK(cudaMemcpyAsync(d_ranges, ranges, sizeof(float) * nr, cudaMemcpyHostToDevice, p->stream));
+    B2S_CUDA_CHECK(cudaMemcpyAsync(d_unit, unit.data(), sizeof(double) * unit.size(), cudaMemcpyHostToDevice, p->stream));
+    I.ranges = d_ranges;
+    I.units = reinterpret_cast<const double2 *>(static_cast<double *>(d_unit));
+    I.n_ranges = n;
+    I.range_min = geometry->range_min;
+    I.range_cutoff = hector_range_cutoff(q.range_cutoff, geometry->range_max);
+    I.filter = f;
+    B2S_CUDA_CHECK(cudaMemcpyAsync(d_ingest, &I, sizeof(HsIngest), cudaMemcpyHostToDevice, p->stream));
+    F.ingest = d_ingest;
+    F.origo_x = (float)f.lx * scale_to_map;  // as b2s_ros_hector_scans' out_origo
+    F.origo_y = (float)f.ly * scale_to_map;
+    return B2S_OK;
+  };
+  return hs_fleet_run(p, n_scans, first, longest, true, first_pose_hints, pose_hints, map_without_matching, out_poses,
+                      out_map_updated, out_last_covs, out_n_points, upload);
 }
 
 b2s_status b2s_hector_slam_update_batch(b2s_hector_slam *p, const float *points, const int32_t *n_points, const float origo[2],

@@ -3,9 +3,12 @@
 //   SlamKarto::getLaser / addScan                       lesson6/src/karto_slam.cc:323-395, 407-434
 //   LaserRangeFinder::SetRangeThreshold / Update        lesson6/lib/open_karto/include/open_karto/Karto.h:3778-3787, 4152-4161
 //   HectorMappingRos::rosPointCloudToDataContainer      lesson4/src/hector_mapping/hector_slam.cc:320-362
+//   HectorMappingRos::scanCallback (projectLaser + the above, per-beam arithmetic in hector_scan.cuh)   :186-205
 #include <cmath>
+#include <vector>
 
 #include "common.cuh"
+#include "hector_scan.cuh"
 
 using namespace b2s;
 
@@ -46,28 +49,49 @@ b2s_status b2s_ros_hector_points(const float *pts, int n, const float laser_in_b
                                  float max_dist, double use_max_scan_range, float z_min, float z_max, float *out_points,
                                  float out_origo[2], int32_t *out_n) {
   if (!laser_in_base || !out_origo || !out_n || n < 0 || (n > 0 && (!pts || !out_points))) B2S_FAIL(B2S_ERR_BAD_PARAMS, "null argument");
-  const float sqr_min = min_dist * min_dist, sqr_max = max_dist * max_dist;  // hector_slam.cc:151-155 (from doubles, cast to float)
-  // tf::Transform of the laser in base_link: rotation about z by yaw (tfScalar = double), translation (x, y, z)
-  const double lx = laser_in_base[0], ly = laser_in_base[1], lz = laser_in_base[2];
-  const double c = cos((double)laser_in_base[3]), s = sin((double)laser_in_base[3]);
-  out_origo[0] = (float)lx * scale_to_map;  // Eigen::Vector2f(laserPos.x(), laserPos.y()) * scaleToMap
-  out_origo[1] = (float)ly * scale_to_map;
+  const HectorScanFilter f = hector_scan_filter(laser_in_base, scale_to_map, min_dist, max_dist, use_max_scan_range, z_min, z_max);
+  out_origo[0] = (float)f.lx * scale_to_map;  // Eigen::Vector2f(laserPos.x(), laserPos.y()) * scaleToMap
+  out_origo[1] = (float)f.ly * scale_to_map;
   int k = 0;
   for (int i = 0; i < n; i++) {
-    const float x = pts[3 * i], y = pts[3 * i + 1], z = pts[3 * i + 2];
-    const float dist_sqr = x * x + y * y;
-    if (!((dist_sqr > sqr_min) && (dist_sqr < sqr_max))) continue;
-    if ((x < 0.0f) && (dist_sqr < 0.50f)) continue;
-    if ((double)dist_sqr > use_max_scan_range * use_max_scan_range) continue;
-    const double bx = c * (double)x - s * (double)y + lx, by = s * (double)x + c * (double)y + ly, bz = (double)z + lz;
-    const float z_laser = (float)(bz - lz);
-    if (z_laser > z_min && z_laser < z_max) {
-      out_points[2 * k] = (float)bx * scale_to_map;
-      out_points[2 * k + 1] = (float)by * scale_to_map;
-      k++;
-    }
+    float x, y;
+    if (!hector_filter_point(f, pts[3 * i], pts[3 * i + 1], pts[3 * i + 2], x, y)) continue;
+    out_points[2 * k] = x;
+    out_points[2 * k + 1] = y;
+    k++;
   }
   *out_n = k;
+  return B2S_OK;
+}
+
+b2s_status b2s_ros_hector_scans(const b2s_laser_scan_msg *geometry, const b2s_hector_scan_filter *filter, float scale_to_map,
+                                int n_scans, const float *ranges, float *out_points, int32_t *out_n_points,
+                                float out_origo[2]) {
+  if (!geometry || !filter || !out_origo || n_scans < 0 || geometry->n_ranges < 0 || (n_scans > 0 && !out_n_points))
+    B2S_FAIL(B2S_ERR_BAD_PARAMS, "null argument or negative count");
+  const int n = geometry->n_ranges;
+  if (n_scans > 0 && n > 0 && (!ranges || !out_points)) B2S_FAIL(B2S_ERR_BAD_PARAMS, "null argument");
+  const b2s_hector_scan_filter &q = *filter;
+  const HectorScanFilter f = hector_scan_filter(q.laser_in_base, scale_to_map, q.min_dist, q.max_dist, q.use_max_scan_range,
+                                                q.z_min, q.z_max);
+  const double cutoff = hector_range_cutoff(q.range_cutoff, geometry->range_max);
+  std::vector<double> unit(2 * (size_t)n);
+  hector_unit_vectors(geometry->angle_min, geometry->angle_increment, n, unit.data());
+  out_origo[0] = (float)f.lx * scale_to_map;
+  out_origo[1] = (float)f.ly * scale_to_map;
+  size_t k = 0;
+  for (int s = 0; s < n_scans; s++) {
+    const float *r = ranges + (size_t)s * n;
+    const size_t k0 = k;
+    for (int i = 0; i < n; i++) {
+      float x, y;
+      if (!hector_scan_beam(f, r[i], unit[2 * i], unit[2 * i + 1], cutoff, geometry->range_min, x, y)) continue;
+      out_points[2 * k] = x;
+      out_points[2 * k + 1] = y;
+      k++;
+    }
+    out_n_points[s] = (int32_t)(k - k0);
+  }
   return B2S_OK;
 }
 

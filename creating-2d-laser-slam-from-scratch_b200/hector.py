@@ -194,6 +194,41 @@ class HectorSlam:
         out = [(poses[edges[b]:edges[b + 1]], upd[edges[b]:edges[b + 1]].astype(bool)) for b in range(B)]
         return out, covs.reshape(B, 3, 3)
 
+    def process_scans_batch(self, geometry, ranges, filt=None, first_hints=None, pose_hints=None,
+                            map_without_matching=False):
+        """process_stream_batch on raw LaserScans of one laser, converted on the device (b2s_hector_slam_process_scans_batch).
+        geometry: a rosio.LaserScanMsg (its ranges ignored); ranges: B arrays [n_b, n_ranges] float32 (n_b = 0 leaves that
+        processor untouched); filt: a rosio.HectorScanFilter (node defaults when None).  Returns what process_stream_batch
+        returns, plus the kept-beam counts of every scan, per processor."""
+        from . import rosio
+        B = self.batch or 1
+        if len(ranges) != B:
+            raise ValueError(f"{len(ranges)} recordings for a handle of {B} processors")
+        nr = geometry.n_ranges
+        recs = [np.ascontiguousarray(r, np.float32).reshape(-1, nr) if nr else np.zeros((len(r), 0), np.float32) for r in ranges]
+        ns = np.array([len(r) for r in recs], np.int32)
+        cat = np.ascontiguousarray(np.concatenate(recs, 0), np.float32)
+        total = int(ns.sum())
+        filt = filt if filt is not None else rosio.hector_scan_filter()
+        poses, upd, covs = np.zeros((total, 3), np.float32), np.zeros(total, np.int32), np.zeros((B, 9), np.float32)
+        kept = np.zeros(total, np.int32)
+        fh = f32(first_hints).reshape(B, 3) if first_hints is not None else None
+        ph = None
+        if pose_hints is not None:
+            ph = f32(np.concatenate([f32(h).reshape(-1, 3) for h in pose_hints], 0)) if total else np.zeros((0, 3), np.float32)
+        ip = C.POINTER(C.c_int32)
+        self.L.b2s_hector_slam_process_scans_batch.argtypes = [C.c_void_p, C.POINTER(rosio.LaserScanMsg),
+                                                               C.POINTER(rosio.HectorScanFilter), ip, C.POINTER(C.c_float),
+                                                               C.POINTER(C.c_float), C.POINTER(C.c_float), C.c_int,
+                                                               C.POINTER(C.c_float), ip, C.POINTER(C.c_float), ip]
+        check(self.L.b2s_hector_slam_process_scans_batch(self.h, C.byref(geometry), C.byref(filt), ns.ctypes.data_as(ip),
+                                                         _f(cat), _f(fh) if fh is not None else None,
+                                                         _f(ph) if ph is not None else None, int(map_without_matching),
+                                                         _f(poses), upd.ctypes.data_as(ip), _f(covs), kept.ctypes.data_as(ip)))
+        edges = np.concatenate([[0], np.cumsum(ns)])
+        out = [(poses[edges[b]:edges[b + 1]], upd[edges[b]:edges[b + 1]].astype(bool)) for b in range(B)]
+        return out, covs.reshape(B, 3, 3), [kept[edges[b]:edges[b + 1]] for b in range(B)]
+
     def update_batch(self, scans, origo, pose_hints, map_without_matching=False):
         """One scan per processor of a batched handle.  scans: list of B [n_b, 2] arrays."""
         B = self.batch

@@ -539,6 +539,39 @@ b2s_status b2s_ros_karto_readings(const b2s_laser_scan_msg *scan, int inverted, 
 b2s_status b2s_ros_hector_points(const float *points_xyz, int n, const float laser_in_base[4], float scale_to_map,
                                  float min_dist, float max_dist, double use_max_scan_range, float z_min, float z_max,
                                  float *out_points, float out_origo[2], int32_t *out_n);
+/* The settings of HectorMappingRos::scanCallback (lesson4/src/hector_mapping/hector_slam.cc:186-205) for turning raw
+ * LaserScan ranges into a DataContainer: laser_geometry's projectLaser(scan, cloud, range_cutoff), then
+ * rosPointCloudToDataContainer with the node's parameters.  Node defaults (hector_slam.cc:129, 150-161) in brackets. */
+typedef struct b2s_hector_scan_filter {
+  float laser_in_base[4];     /* x, y, z, yaw of the laser in base_link */
+  double range_cutoff;        /* [30.0] projectLaser keeps range < range_cutoff && range >= range_min; < 0: range_max */
+  double use_max_scan_range;  /* [20.0] */
+  float min_dist, max_dist;   /* [0.2, 30.0] squared-distance window */
+  float z_min, z_max;         /* [-1, 1] height window (the projected z is 0) */
+} b2s_hector_scan_filter;
+/* HectorMappingRos::scanCallback's conversion of n_scans LaserScans of one laser: geometry gives angle_min,
+ * angle_increment, range_min, range_max and n_ranges (its ranges pointer is ignored); ranges [n_scans][n_ranges] float32.
+ * Beam i projects along (cos, sin)(angle_min + i * angle_increment) computed in double, x / y = (float)(range * unit),
+ * z = 0, then passes b2s_ros_hector_points' filters and transform.  out_points [sum out_n_points][2] are the kept
+ * beams of every scan, in beam order, packed scan after scan (capacity n_scans * n_ranges): the input of
+ * b2s_hector_slam_process_stream_batch, or with n_scans = 1 of b2s_hector_slam_update.  out_n_points [n_scans];
+ * out_origo[2] = laser position * scale_to_map (scale_to_map = 1 / level-0 cell length, GridMapBase::getScaleToMap). */
+b2s_status b2s_ros_hector_scans(const b2s_laser_scan_msg *geometry, const b2s_hector_scan_filter *filter, float scale_to_map,
+                                int n_scans, const float *ranges, float *out_points, int32_t *out_n_points,
+                                float out_origo[2]);
+/* b2s_hector_slam_process_stream_batch on raw ranges: every processor of the handle walks its own recording of
+ * LaserScans of ONE laser (geometry + filter as for b2s_ros_hector_scans, scale_to_map = the handle's level-0 1 / cell
+ * length, origo = laser position * scale_to_map), converted on the device inside the same launch.  n_scans [B]
+ * (processor-major recordings, 0 = untouched), ranges [sum n_scans][geometry->n_ranges] float32; hints, outputs and
+ * the per-processor results as for b2s_hector_slam_process_stream_batch fed b2s_ros_hector_scans' points, which they
+ * equal bit for bit.  out_n_points [sum n_scans] (may be NULL): the beams each scan kept.
+ * Refused before anything is enqueued: B2S_ERR_BAD_PARAMS for NULL arrays or negative counts, B2S_ERR_TOO_LARGE for
+ * n_ranges above the handle's max_points or a processor with 2^20 - 1 or more scans. */
+b2s_status b2s_hector_slam_process_scans_batch(b2s_hector_slam *p, const b2s_laser_scan_msg *geometry,
+                                               const b2s_hector_scan_filter *filter, const int32_t *n_scans,
+                                               const float *ranges, const float *first_pose_hints, const float *pose_hints,
+                                               int map_without_matching, float *out_poses, int32_t *out_map_updated,
+                                               float *out_last_covs, int32_t *out_n_points);
 
 /* ---------------------------------------------------------------- K2b: GMapping hit/visit map */
 
