@@ -27,7 +27,7 @@
 //   k_sweep_window     THE HOT KERNEL: grid (or a row band of it) staged into shared memory by TMA bulk copy;
 //                      one warp per (angle, 32x32 candidate tile), one lane per candidate row; each 32-bit
 //                      shared-memory word feeds 4 adjacent-x candidates (byte-permute into packed u16
-//                      accumulators)                                                    (int, smem-gather bound)
+//                      accumulators)                                                    (int, issue bound)
 //   k_sweep_generic    any lattice / any grid size: one warp per (x,y) candidate, lanes over beams,
 //                      gathers from global memory through L1/L2
 //   k_reduce           penalties, best response, tie-averaged pose, positional covariance (fp64, one CTA per match);
@@ -481,10 +481,11 @@ __global__ void __launch_bounds__(256) k_sweep_generic(const uint8_t *__restrict
 //
 // Inner loop, per PAIR of same-alignment beams and per lane: 2 x 9 aligned 32-bit shared-memory loads (the 36
 // bytes covering the lane's 32 candidate cells), 9 packed-byte adds of the two beams' words (cell values <= 100,
-// so two fit a byte), then each summed word is split into two packed-u16 halves (bytes 0,2 / bytes 1,3) and added
-// to 18 packed-u16 accumulators kept in WORD-ALIGNED coordinates — the alignment (a compile-time constant of the
-// class) is only applied when the u16 lanes are flushed into the 32 per-candidate 32-bit sums.  One shared-memory
-// word therefore feeds 4 adjacent-x candidates and costs ~2.3 integer instructions per beam.
+// so two fit a byte), then each summed word is added whole to one accumulator and its bytes 1,3 (one byte permute) to
+// a packed-u16 one; bytes 0,2 are recovered as the difference at the flush, so they need no mask per word.  The 18
+// accumulators are kept in WORD-ALIGNED coordinates — the alignment (a compile-time constant of the class) is only
+// applied when the u16 lanes are flushed into the 32 per-candidate 32-bit sums.  The sweep is bound by instruction
+// issue (DESIGN.md §4): one shared-memory word feeds 4 adjacent-x candidates for ~2 integer instructions per beam.
 //
 // Flat-index semantics of the reference are kept bit-exactly: rows wrap exactly as `base + offset` does, and
 // positions outside [0, data_size) read zeros (guard bands, zero padding of the HBM image, redirect of rows that
@@ -728,6 +729,10 @@ __device__ __forceinline__ void win_flush_rot(const uint32_t (&lo)[9], const uin
 // lanes 0..15 and 1 for lanes 16..31; GEN = true: any of 0..7.
 template <int SH, int STRIDE, bool GEN>
 __device__ __forceinline__ void win_flush(uint32_t (&lo)[9], uint32_t (&hi)[9], uint32_t (&acc)[32], int rot) {
+  // lo holds the plain 32-bit sum of the packed words (see win_accumulate2); taking away bytes 1 and 3, which hi
+  // holds as u16 lanes, leaves bytes 0 and 2 as u16 lanes.  Exact modulo 2^32 because every u16 lane is < 65536.
+#pragma unroll
+  for (int j = 0; j < 9; j++) lo[j] -= hi[j] << 8;
   if (!GEN) {
     if (!rot) win_flush_rot<SH, STRIDE, 0>(lo, hi, acc);
     else win_flush_rot<SH, STRIDE, 1>(lo, hi, acc);
@@ -779,7 +784,7 @@ __device__ __forceinline__ void win_accumulate2(const uint32_t (&v1)[9], const u
 #pragma unroll
   for (int q = 0; q < (W9 ? 9 : 8); q++) {
     const uint32_t w = v1[q] + v2[q];      // packed bytes, each <= 254
-    lo[q] += w & 0x00ff00ffu;              // bytes 0, 2 -> u16 lanes
+    lo[q] += w;                            // all four bytes, carries included: bytes 0, 2 recovered at the flush
     hi[q] += __byte_perm(w, 0u, 0x4341);   // bytes 1, 3 -> u16 lanes
   }
 }
