@@ -5,14 +5,18 @@
 // functions with the node's arithmetic: PruneImuDeque's angle integration (:196-238) and PruneOdomDeque's odometry
 // increment (:296-333).
 //
-// PARITY UNPINNED: pcl::getTransformation / Eigen::Affine3f inverse and product are third-party header code that is not
-// in the reference tree (PCL 1.8, Eigen 3.3); their published algorithms are restated here (float arithmetic in Eigen's
-// coefficient order, 3-term sums as a0 + (a1 + a2)).  The tests compare the device stage with an independent CPU
-// restatement of the same algorithms bit for bit — that restatement is what is unpinned against the node itself.
+// The beam angles are the node's angle cache (CreateAngleCache, :162-174), built on the host with its arithmetic: the
+// angle in float from the LaserScan's float fields, its cos / sin from the C library in double.
+//
+// Pinned to the node (tests/test_deskew_reference.py, tests/test_gpu_deskew_edges.py) except for pcl::getTransformation
+// and Eigen::Affine3f inverse and product: those are third-party header code that is not in the reference tree (PCL 1.8,
+// Eigen 3.3), so their published algorithms are restated here (float arithmetic in Eigen's coefficient order, 3-term
+// sums as a0 + (a1 + a2)), and the node's build uses stand-ins that restate them the same way.
 #include <cmath>
 #include <cstdint>
 #include <cstring>
 #include <new>
+#include <vector>
 
 #include "common.cuh"
 
@@ -102,14 +106,15 @@ __device__ inline Affine3f pose_at(const b2s_deskew_scan &s, const double *__res
   return get_transformation(posx, posy, posz, rotx, roty, rotz);
 }
 
-// One CTA per (scan, slab of beams).  The reference takes transStartInverse from the FIRST VALID reading of the scan
-// (first_point_flag): every CTA finds that beam with a block-wide minimum, thread 0 inverts its pose once.
+// One CTA per (scan, slab of beams): scans on x, whose limit is 2^31 - 1, so a whole recording is one launch; slabs on y.
+// The reference takes transStartInverse from the FIRST VALID reading of the scan (first_point_flag): every CTA finds
+// that beam with a block-wide minimum, thread 0 inverts its pose once.
 constexpr int DSK_THREADS = 256;
 __global__ void __launch_bounds__(DSK_THREADS)
-    k_deskew(const float *__restrict__ ranges, int n_beams, double angle_min, double angle_increment,
+    k_deskew(const float *__restrict__ ranges, int n_beams, const double2 *__restrict__ angle_cs,
              const b2s_deskew_scan *__restrict__ scans, const double *__restrict__ imu_time, const double *__restrict__ imu_rx,
              const double *__restrict__ imu_ry, const double *__restrict__ imu_rz, int imu_stride, float *__restrict__ out_xyz) {
-  const int b = blockIdx.y;
+  const int b = blockIdx.x;
   const b2s_deskew_scan s = scans[b];
   const float *r = ranges + (size_t)b * n_beams;
   const double *it = imu_time + (size_t)b * imu_stride, *rx = imu_rx + (size_t)b * imu_stride,
@@ -125,7 +130,7 @@ __global__ void __launch_bounds__(DSK_THREADS)
   __syncthreads();
   if (threadIdx.x == 0 && s_first < n_beams) s_inv = affine_inverse(pose_at(s, it, rx, ry, rz, s_first));
   __syncthreads();
-  const int i = blockIdx.x * DSK_THREADS + threadIdx.x;
+  const int i = blockIdx.y * DSK_THREADS + threadIdx.x;
   if (i >= n_beams) return;
   float *o = out_xyz + ((size_t)b * n_beams + i) * 3;
   const float range = r[i];
@@ -133,8 +138,8 @@ __global__ void __launch_bounds__(DSK_THREADS)
     o[0] = o[1] = o[2] = 0.0f;
     return;
   }
-  const double angle = angle_min + i * angle_increment;  // CreateAngleCache (:160-172)
-  const double px = range * cos(angle), py = range * sin(angle), pz = 1.0;
+  const double2 cs = angle_cs[i];  // a_cos_[i], a_sin_[i]
+  const double px = range * cs.x, py = range * cs.y, pz = 1.0;
   const Affine3f bt = affine_mul(s_inv, pose_at(s, it, rx, ry, rz, i));
   o[0] = (float)(bt.m[0][0] * px + bt.m[0][1] * py + bt.m[0][2] * pz + bt.t[0]);
   o[1] = (float)(bt.m[1][0] * px + bt.m[1][1] * py + bt.m[1][2] * pz + bt.t[1]);
@@ -191,31 +196,44 @@ b2s_status b2s_lidar_undistort(int batch, int n_beams, const float *ranges, doub
   if (batch < 0 || n_beams < 1 || imu_stride < 1 || !ranges || !scans || !imu_time || !imu_rot_x || !imu_rot_y || !imu_rot_z || !out_xyz)
     B2S_FAIL(B2S_ERR_BAD_PARAMS, "b2s_lidar_undistort: null argument or empty scan");
   if (batch == 0) return B2S_OK;
+  if (ceil_div(n_beams, DSK_THREADS) > 65535) B2S_FAIL(B2S_ERR_BAD_PARAMS, "b2s_lidar_undistort: more than 65535 * 256 beams");
   for (int b = 0; b < batch; b++) {
     if (scans[b].imu_last < 0 || scans[b].imu_last >= imu_stride)
       B2S_FAIL(B2S_ERR_BAD_PARAMS, "b2s_lidar_undistort: imu_last outside the IMU table");
     if (scans[b].use_odom && !(scans[b].odom_end_time != scans[b].odom_start_time))
       B2S_FAIL(B2S_ERR_BAD_PARAMS, "b2s_lidar_undistort: odometry interval of zero length");
   }
+  // CreateAngleCache (:162-174): angle_min and angle_increment are float fields of the LaserScan and i is unsigned, so
+  // the angle is summed in float and only widened for the double cos / sin
+  const float amin = (float)angle_min, ainc = (float)angle_increment;
+  std::vector<double> angle_cs(2 * (size_t)n_beams);
+  for (int i = 0; i < n_beams; i++) {
+    const float step = (float)(unsigned)i * ainc;
+    const double angle = amin + step;
+    angle_cs[2 * i] = cos(angle);
+    angle_cs[2 * i + 1] = sin(angle);
+  }
   if (b2s_status st = open_device(device)) return st;
   cudaStream_t st = reinterpret_cast<cudaStream_t>(cuda_stream);
   const size_t nr = (size_t)batch * n_beams, ni = (size_t)batch * imu_stride;
   AsyncBuf<float> d_r(st), d_o(st);
-  AsyncBuf<double> d_imu(st);
+  AsyncBuf<double> d_imu(st), d_ang(st);
   AsyncBuf<b2s_deskew_scan> d_s(st);
   B2S_CUDA_CHECK(d_r.alloc(nr));
   B2S_CUDA_CHECK(d_o.alloc(nr * 3));
   B2S_CUDA_CHECK(d_imu.alloc(ni * 4));
+  B2S_CUDA_CHECK(d_ang.alloc(angle_cs.size()));
   B2S_CUDA_CHECK(d_s.alloc(batch));
   B2S_CUDA_CHECK(cudaMemcpyAsync(d_r, ranges, nr * sizeof(float), cudaMemcpyHostToDevice, st));
+  B2S_CUDA_CHECK(cudaMemcpyAsync(d_ang, angle_cs.data(), angle_cs.size() * sizeof(double), cudaMemcpyHostToDevice, st));
   B2S_CUDA_CHECK(cudaMemcpyAsync(d_imu, imu_time, ni * sizeof(double), cudaMemcpyHostToDevice, st));
   B2S_CUDA_CHECK(cudaMemcpyAsync(d_imu + ni, imu_rot_x, ni * sizeof(double), cudaMemcpyHostToDevice, st));
   B2S_CUDA_CHECK(cudaMemcpyAsync(d_imu + 2 * ni, imu_rot_y, ni * sizeof(double), cudaMemcpyHostToDevice, st));
   B2S_CUDA_CHECK(cudaMemcpyAsync(d_imu + 3 * ni, imu_rot_z, ni * sizeof(double), cudaMemcpyHostToDevice, st));
   B2S_CUDA_CHECK(cudaMemcpyAsync(d_s, scans, (size_t)batch * sizeof(b2s_deskew_scan), cudaMemcpyHostToDevice, st));
-  const dim3 grid(ceil_div(n_beams, DSK_THREADS), batch);
-  k_deskew<<<grid, DSK_THREADS, 0, st>>>(d_r, n_beams, angle_min, angle_increment, d_s, d_imu, d_imu + ni, d_imu + 2 * ni,
-                                         d_imu + 3 * ni, imu_stride, d_o);
+  const dim3 grid(batch, ceil_div(n_beams, DSK_THREADS));
+  k_deskew<<<grid, DSK_THREADS, 0, st>>>(d_r, n_beams, reinterpret_cast<const double2 *>(static_cast<double *>(d_ang)), d_s,
+                                         d_imu, d_imu + ni, d_imu + 2 * ni, d_imu + 3 * ni, imu_stride, d_o);
   B2S_CUDA_CHECK(cudaGetLastError());
   B2S_CUDA_CHECK(cudaMemcpyAsync(out_xyz, d_o, nr * 3 * sizeof(float), cudaMemcpyDeviceToHost, st));
   B2S_CUDA_CHECK(cudaStreamSynchronize(st));

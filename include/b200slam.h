@@ -676,8 +676,9 @@ b2s_status b2s_pcl_icp_align(const b2s_pcl_icp_params *params, int n_scans, int 
  * LidarUndistortion (lesson5/src/lidar_undistortion.cc): every reading of a LaserScan is moved into the sensor frame
  * of the scan's first valid reading, using IMU angles integrated over the scan and the odometry increment across it.
  * The per-beam loop (CorrectLaserScan, :339-393) runs on the device for a batch of scans; the per-scan preparation is
- * host arithmetic.  PARITY UNPINNED: pcl::getTransformation and Eigen::Affine3f inverse / product are third-party
- * header code absent from the reference tree (PCL 1.8, Eigen 3.3); their published algorithms are restated. */
+ * host arithmetic.  Pinned to the unmodified node (tests/test_deskew_reference.py, tests/test_gpu_deskew_edges.py)
+ * except pcl::getTransformation and Eigen::Affine3f inverse / product: those are third-party header code absent from
+ * the reference tree (PCL 1.8, Eigen 3.3), and their published algorithms are restated. */
 typedef struct b2s_deskew_scan {
   double time_start, time_increment;   /* header.stamp (start of the sweep), LaserScan::time_increment */
   float range_min, range_max;          /* readings outside [range_min, range_max] or non-finite are skipped (:349-352) */
@@ -697,9 +698,11 @@ int32_t b2s_deskew_integrate_imu(int n_imu, const double *stamp, const double *a
 /* PruneOdomDeque's increment (:296-333): start / end pose as (x, y, z, roll, pitch, yaw) — the position of the
  * odometry message and tf::Matrix3x3(orientation).getRPY — gives odom_incre_x_/y_/z_. */
 void b2s_deskew_odom_increment(const double start_pose[6], const double end_pose[6], float out_increment[3]);
-/* CorrectLaserScan for `batch` scans: ranges [batch][n_beams] (host), beam angles angle_min + i * angle_increment
- * (CreateAngleCache, :160-172), per-scan parameters, IMU tables [batch][imu_stride]; out_xyz [batch][n_beams][3] (host):
- * the corrected point cloud, skipped readings as (0, 0, 0) (the cloud is cleared and resized per scan). */
+/* CorrectLaserScan for `batch` scans (any batch >= 1; n_beams <= 65535 * 256): ranges [batch][n_beams] (host),
+ * per-scan parameters, IMU tables [batch][imu_stride]; out_xyz [batch][n_beams][3] (host): the corrected point cloud,
+ * skipped readings as (0, 0, 0) (the cloud is cleared and resized per scan).  angle_min and angle_increment are the
+ * LaserScan's float32 fields: they are rounded to float and beam i's angle is summed in float, angle_min + i *
+ * angle_increment, as CreateAngleCache (:162-174) sums them, before its cos / sin are taken in double. */
 b2s_status b2s_lidar_undistort(int batch, int n_beams, const float *ranges, double angle_min, double angle_increment,
                                const b2s_deskew_scan *scans, const double *imu_time, const double *imu_rot_x,
                                const double *imu_rot_y, const double *imu_rot_z, int imu_stride, float *out_xyz, int device,

@@ -1,8 +1,10 @@
 /* TEST INFRASTRUCTURE — CPU restatement of lesson5's motion de-skew (LidarUndistortion, lesson5/src/lidar_undistortion.cc).
- * PARITY UNPINNED: the arithmetic inside CorrectLaserScan lives in third-party headers that are not in the reference
- * tree — pcl::getTransformation (PCL 1.8 common/impl/eigen.hpp) and Eigen 3.3 Affine3f inverse / product — so they are
- * restated here from their published algorithms; whether PCL's unqualified cos / sin resolve to the float or the double
- * C functions cannot be checked (the double ones, rounded to float, are used, as the lesson4 headers were found to do).
+ * Pinned bit for bit to the unmodified node (oracle/ref_lesson5.cpp, tests/test_deskew_reference.py) except for the
+ * arithmetic that lives in third-party headers not in the reference tree — pcl::getTransformation (PCL 1.8
+ * common/impl/eigen.hpp) and Eigen 3.3 Affine3f inverse / product — which is restated here from their published
+ * algorithms, and the same way in the node's stand-ins; whether PCL's unqualified cos / sin resolve to the float or the
+ * double C functions cannot be checked (the double ones, rounded to float, are used, as the lesson4 headers were found
+ * to do).
  *   orc_deskew_integrate_imu   PruneImuDeque's angle integration        (lidar_undistortion.cc:196-238)
  *   orc_deskew_odom_increment  PruneOdomDeque's odometry increment      (:296-333)
  *   orc_deskew_scan            CorrectLaserScan                          (:339-393) with ComputeRotation (:396-430) and
@@ -124,7 +126,9 @@ void orc_deskew_scan(int n_beams, const float *ranges, double angle_min, double 
     const float r = ranges[i];
     if (!isfinite(r) || r < s->range_min || r > s->range_max) continue;
     const double t = s->time_start + i * s->time_increment;
-    const double angle = angle_min + i * angle_increment;  /* CreateAngleCache (:160-172) */
+    /* CreateAngleCache (:162-174): float fields and an unsigned index, so the angle is summed in float */
+    const float step = (float)(unsigned)i * (float)angle_increment;
+    const double angle = (float)angle_min + step;
     const double px = r * cos(angle), py = r * sin(angle), pz = 1.0;
     float rotx = 0, roty = 0, rotz = 0, posx = 0, posy = 0, posz = 0;
     if (s->use_imu) compute_rotation(s, imu_time, rx, ry, rz, t, &rotx, &roty, &rotz);

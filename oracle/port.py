@@ -330,7 +330,7 @@ def plicp_match(params, ref_ranges, sens_ranges, theta, range_min, range_max, fi
     return res
 
 
-# ---------------------------------------------------------------- lesson5 de-skew (deskew_oracle.c) — PARITY UNPINNED
+# ---------------------------------------------------------------- lesson5 de-skew (deskew_oracle.c) — pinned except PCL / Eigen
 
 def deskew_integrate_imu(stamps, angular_velocity, scan_start, scan_end, capacity=2000):
     L = lib()

@@ -4,7 +4,8 @@
  * Eigen is absent from this image and cannot be fetched, and every lesson4 Hector header includes <Eigen/...>.
  * This is the smallest stand-in for the fixed-size types those headers use (Vector2f/3f/4f/2i, Matrix3f,
  * Matrix<float,3,7>, Affine2f/3f, Translation2f/3f, Rotation2Df, AlignedScaling2f/3f) so that the UNMODIFIED
- * reference headers compile where they lie under the reference checkout (oracle/ref_hector.cpp).  All the SLAM logic
+ * reference headers compile where they lie under the reference checkout (oracle/ref_hector.cpp); lesson5's
+ * lidar_undistortion.cc uses Affine3f as well (oracle/ref_lesson5.cpp).  All the SLAM logic
  * that runs is then the reference's own; only these linear-algebra primitives are ours.  They mirror Eigen 3.3's
  * fixed-size behaviour as follows (scalar float, no vectorisation for these sizes, no FMA contraction in a build
  * without -march):
@@ -15,6 +16,7 @@
  *   Translation * Rotation2D                        -> linear = [[c,-s],[s,c]] with c = cosf(a), s = sinf(a); translation = t
  *   AlignedScaling * Translation                    -> linear = diag(s); translation = diag(s)*t
  *   Transform::inverse() (Affine)                   -> L' = L.inverse(); t' = -(L' * t)
+ *   Affine3f * Affine3f                             -> L = L1 * L2; t = L1 * t2 + t1
  *   2x2 / 3x3 inverse                               -> cofactor / determinant forms, multiplied by 1/det
  * Re-verify against a real Eigen build whenever one is available.
  */
@@ -334,13 +336,22 @@ struct Transform {
   }
 };
 
-/* generic square inverse is only needed for the (unused) 3-D transform of GridMapBase::setMapTransformation */
+/* the 3-D transform of GridMapBase::setMapTransformation (unused there), and lesson5's Affine3f (oracle/ref_lesson5.cpp):
+ * coefficient (i, j) of the 4x4 matrix, and the product of two transforms as linear = L1 L2, translation = L1 t2 + t1,
+ * each coefficient a three-term redux p0 + (p1 + p2), as csrc/lidar_undistortion.cu restates Eigen's product */
 template <typename T, int Mode>
 struct Transform<T, 3, Mode> {
   Matrix<T, 3, 3> lin;
   Matrix<T, 3, 1> tr;
   Transform() {}
   Matrix<T, 3, 1> operator*(const Matrix<T, 3, 1> &p) const { return tr + lin * p; }
+  Transform operator*(const Transform &o) const {
+    Transform r;
+    r.lin = lin * o.lin;
+    r.tr = lin * o.tr + tr;
+    return r;
+  }
+  T operator()(int i, int j) const { return i == 3 ? T(j == 3 ? 1 : 0) : j == 3 ? tr[i] : lin(i, j); }
   Transform inverse() const {
     Transform r;
     r.lin = lin.inverse();

@@ -10,7 +10,10 @@
 namespace std_msgs {
 struct Header {
   uint32_t seq = 0;
-  struct { uint32_t sec = 0, nsec = 0; } stamp;
+  struct {
+    uint32_t sec = 0, nsec = 0;
+    double toSec() const { return (double)sec + 1e-9 * (double)nsec; }  // ros::Time::toSec
+  } stamp;
   std::string frame_id;
 };
 }  // namespace std_msgs

@@ -1,7 +1,7 @@
 """lesson5 motion de-skew (LidarUndistortion): the host preparation of the library against the C restatement (CPU), the
 restatement against closed-form motion, and the batched device stage against the restatement (GPU, bit-identical: the two
-share an operation order).  PARITY UNPINNED against the reference node itself — pcl::getTransformation and Eigen's
-Affine3f arithmetic are third-party code absent from the reference tree (see oracle/deskew_oracle.c)."""
+share an operation order).  The comparison with the unmodified node is tests/test_deskew_reference.py; pcl::getTransformation
+and Eigen's Affine3f arithmetic are third-party code absent from the reference tree (see oracle/deskew_oracle.c)."""
 import numpy as np
 import pytest
 
