@@ -90,6 +90,31 @@ class IcpResult(C.Structure):
                 ("nvalid", C.c_int32), ("reserved", C.c_int32)]
 
 
+class PlicpOdomParams(C.Structure):
+    """b2s_plicp_odom_params; defaults = lesson3/src/plicp_odometry.cc:64-67 and an identity laser mount."""
+    _fields_ = [("icp", IcpParams), ("kf_dist_linear", C.c_double), ("kf_dist_angular", C.c_double),
+                ("kf_scan_count", C.c_int32), ("reserved", C.c_int32), ("base_to_laser", C.c_double * 7)]
+
+
+def plicp_odom_params(icp=None, base_to_laser=(0, 0, 0, 0, 0, 0, 1), **kw) -> PlicpOdomParams:
+    import math
+    p = PlicpOdomParams(icp if icp is not None else icp_params(), 0.1, 5.0 * (math.pi / 180.0), 10, 0,
+                        (C.c_double * 7)(*base_to_laser))
+    for k, v in kw.items():
+        if not hasattr(p, k):
+            raise AttributeError(k)
+        setattr(p, k, v)
+    return p
+
+
+class PlicpOdomStep(C.Structure):
+    """b2s_plicp_odom_step."""
+    _fields_ = [("position", C.c_double * 3), ("orientation", C.c_double * 4), ("linear", C.c_double * 3),
+                ("angular", C.c_double * 3), ("first_guess", C.c_double * 3), ("icp", IcpResult),
+                ("published", C.c_int32), ("keyframe", C.c_int32), ("reference_scan", C.c_int32),
+                ("reserved", C.c_int32)]
+
+
 class PclIcpParams(C.Structure):
     """b2s_pcl_icp_params; defaults = a default-constructed pcl::IterativeClosestPoint (lesson2 scan_match_icp.h:49)."""
     _fields_ = [("max_iterations", C.c_int32), ("drop_invalid_points", C.c_int32),

@@ -629,6 +629,60 @@ b2s_status b2s_plicp_match(const b2s_icp_params *params, int batch, int n, const
                            const double *sens_ranges, const double *theta, double range_min, double range_max,
                            const double *first_guess, int device, void *cuda_stream, b2s_icp_result *results);
 
+/* ScanMatchPLICP (lesson3/src/plicp_odometry.cc:191-517), the node around sm_icp, for B independent recordings (robots)
+ * of one laser: key frame, constant-velocity prediction (GetPrediction, :442-456: only linear.x >= 1e-6 predicts; there
+ * is never an angular prediction), the prediction moved into the laser frame through the base-to-laser transform,
+ * sm_icp against the key frame (the matcher of b2s_plicp_match), the correction composed into base_in_odom_ and the
+ * key-frame rule (NewKeyframeNeeded, :498-517: |yaw| > kf_dist_angular, then ++count == kf_scan_count, which alone
+ * resets the count, then x^2 + y^2 > kf_dist_linear^2).  The state is the node's: tf2::Transform (3x3 basis and origin
+ * in double) for base_in_odom_ and base_in_odom_keyframe_, latest_velocity_, last_icp_time_, the scan count and the key
+ * frame's float32 ranges.  dt = (stamp - last stamp) as ros::Time arithmetic; equal stamps give dt = 0 and an inf / NaN
+ * velocity, kept as IEEE arithmetic gives it.  last_icp_time_ always advances; velocity and pose change only on a valid
+ * match.  One rule the node leaves undefined: after a failed match (icp.valid = 0) the node tests the key-frame rule on
+ * a default-constructed, uninitialised tf2::Transform; here it is the identity, so only the scan-count rule can
+ * promote such a scan (DESIGN.md §7).  Pinned to the unmodified node except sm_icp and tf2's LinearMath, whose
+ * published code is restated (PARITY UNPINNED for sm_icp; the device's sin / cos / atan2 may differ from glibc's in the
+ * last place). */
+typedef struct b2s_plicp_odom_params {
+  b2s_icp_params icp;              /* sm_params subset, node defaults (b2s_icp_params) */
+  double kf_dist_linear;           /* 0.1 m */
+  double kf_dist_angular;          /* 5 deg, in rad */
+  int32_t kf_scan_count, reserved; /* 10 */
+  double base_to_laser[7];         /* translation x, y, z + quaternion x, y, z, w: lookupTransform(base, laser) */
+} b2s_plicp_odom_params;
+
+typedef struct b2s_plicp_odom_step { /* one LaserScan's outcome */
+  double position[3], orientation[4]; /* odom_msg.pose.pose = toMsg(base_in_odom_) (orientation x, y, z, w) */
+  double linear[3], angular[3];       /* odom_msg.twist.twist = latest_velocity_ */
+  double first_guess[3];              /* input_.first_guess */
+  b2s_icp_result icp;                 /* output_ */
+  int32_t published;      /* 0 for a recording's first scan (initialisation only: nothing published, all fields 0
+                             except orientation w = 1, keyframe = 1, reference_scan = -1) */
+  int32_t keyframe;       /* this scan became the key frame */
+  int32_t reference_scan; /* index in the recording of the key frame it was matched against */
+  int32_t reserved;
+} b2s_plicp_odom_step;
+
+typedef struct b2s_plicp_odom b2s_plicp_odom; /* opaque: B ScanMatchPLICP nodes */
+
+/* One laser geometry for every recording: the LaserScan's float32 angle_min, angle_increment (beam angle angle_min +
+ * i * angle_increment summed in float, :308), range_min, range_max (valid iff range_min < r < range_max, :295).
+ * B2S_ERR_BAD_PARAMS for NULL pointers, batch < 1, n_beams < 3, icp.max_iterations < 1 or a zero / non-finite mount
+ * quaternion; B2S_ERR_NO_DEVICE without a device; B2S_ERR_TOO_LARGE above the pair kernel's beam limit (2408 on an
+ * H100, 82 bytes of shared memory per beam). */
+b2s_status b2s_plicp_odom_create(const b2s_plicp_odom_params *params, int batch, int n_beams, float angle_min,
+                                 float angle_increment, float range_min, float range_max, int device, void *cuda_stream,
+                                 b2s_plicp_odom **out);
+void b2s_plicp_odom_destroy(b2s_plicp_odom *h);
+/* ScanCallback on every recording's next n_scans[b] LaserScans (0: recording b is untouched), in ONE launch (one CTA per
+ * recording, no host round trip between scans).  Recordings are processor-major: ranges [sum n_scans][n_beams] float32,
+ * stamps [sum n_scans][2] (header.stamp sec, nsec), out [sum n_scans].  Two calls over consecutive parts of every
+ * recording equal one call.  B2S_ERR_BAD_PARAMS (nothing enqueued) for NULL arrays or a negative count. */
+b2s_status b2s_plicp_odom_process(b2s_plicp_odom *h, const int32_t *n_scans, const float *ranges, const uint32_t *stamps,
+                                  b2s_plicp_odom_step *out);
+/* a fresh node for one recording, or for all with recording = -1: its next scan initialises it */
+b2s_status b2s_plicp_odom_reset(b2s_plicp_odom *h, int recording);
+
 /* ---------------------------------------------------------------- lesson2: PCL ICP scan matching
  * ScanMatchICP (lesson2/src/scan_match_icp.cc): every LaserScan becomes a pcl::PointCloud<PointXYZ>
  * (ConvertScan2PointCloud, :89-130) and the previous cloud is aligned to the current one by a default-constructed

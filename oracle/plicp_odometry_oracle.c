@@ -1,0 +1,169 @@
+/*
+ * plicp_odometry_oracle.c — TEST INFRASTRUCTURE, NOT PRODUCT CODE.
+ *
+ * CPU restatement of lesson3's odometry node, ScanMatchPLICP (reference/lesson3/src/plicp_odometry.cc:191-517): the
+ * node's loop in C around the PL-ICP restatement orc_plicp_match (oracle/plicp_oracle.c).  Built with it into a library
+ * of its own (oracle/plicp_odometry_port.py), with the flags of oracle/Makefile.
+ */
+#include <math.h>
+#include <stdint.h>
+#include <stdlib.h>
+#include <string.h>
+
+#include "../include/b200slam.h"
+
+int orc_plicp_match(const b2s_icp_params *P, int n, const double *ref_r, const double *sens_r, const double *theta,
+                    double range_min, double range_max, const double first_guess[3], b2s_icp_result *out);
+
+/* The node's loop for ONE recording from a fresh node, in C around orc_plicp_match.  tf2's LinearMath (Transform product
+ * and inverse, Matrix3x3::setRotation / getRotation, Quaternion::setRPY) and tf2::getYaw are restated from geometry2,
+ * operation by operation, in double without FMA contraction.  After a failed match the node tests NewKeyframeNeeded on a
+ * default-constructed (uninitialised) tf2::Transform; here it is the identity (DESIGN.md §7).  The unmodified node,
+ * compiled against the stand-ins under oracle/shim/ (oracle/ref_lesson3.cpp), pins this restatement bit for bit. */
+typedef struct { double m[3][3], o[3]; } orc_tf;
+
+static void tf_identity(orc_tf *t) {
+  for (int i = 0; i < 3; i++) {
+    for (int j = 0; j < 3; j++) t->m[i][j] = i == j ? 1.0 : 0.0;
+    t->o[i] = 0.0;
+  }
+}
+static orc_tf tf_mul(const orc_tf *a, const orc_tf *b) {
+  orc_tf c;
+  for (int i = 0; i < 3; i++) {
+    for (int j = 0; j < 3; j++) c.m[i][j] = b->m[0][j] * a->m[i][0] + b->m[1][j] * a->m[i][1] + b->m[2][j] * a->m[i][2];
+    c.o[i] = (b->o[0] * a->m[i][0] + b->o[1] * a->m[i][1] + b->o[2] * a->m[i][2]) + a->o[i];
+  }
+  return c;
+}
+static orc_tf tf_inverse(const orc_tf *a) {
+  orc_tf c;
+  for (int i = 0; i < 3; i++)
+    for (int j = 0; j < 3; j++) c.m[i][j] = a->m[j][i];
+  const double no[3] = {-a->o[0], -a->o[1], -a->o[2]};
+  for (int i = 0; i < 3; i++) c.o[i] = c.m[i][0] * no[0] + c.m[i][1] * no[1] + c.m[i][2] * no[2];
+  return c;
+}
+static void tf_set_rotation(orc_tf *t, const double q[4]) {
+  const double d = q[0] * q[0] + q[1] * q[1] + q[2] * q[2] + q[3] * q[3], s = 2.0 / d;
+  const double xs = q[0] * s, ys = q[1] * s, zs = q[2] * s;
+  const double wx = q[3] * xs, wy = q[3] * ys, wz = q[3] * zs;
+  const double xx = q[0] * xs, xy = q[0] * ys, xz = q[0] * zs;
+  const double yy = q[1] * ys, yz = q[1] * zs, zz = q[2] * zs;
+  t->m[0][0] = 1.0 - (yy + zz); t->m[0][1] = xy - wz; t->m[0][2] = xz + wy;
+  t->m[1][0] = xy + wz; t->m[1][1] = 1.0 - (xx + zz); t->m[1][2] = yz - wx;
+  t->m[2][0] = xz - wy; t->m[2][1] = yz + wx; t->m[2][2] = 1.0 - (xx + yy);
+}
+static void tf_get_rotation(const orc_tf *t, double q[4]) {
+  const double trace = t->m[0][0] + t->m[1][1] + t->m[2][2];
+  if (trace > 0.0) {
+    double s = sqrt(trace + 1.0);
+    q[3] = s * 0.5;
+    s = 0.5 / s;
+    q[0] = (t->m[2][1] - t->m[1][2]) * s;
+    q[1] = (t->m[0][2] - t->m[2][0]) * s;
+    q[2] = (t->m[1][0] - t->m[0][1]) * s;
+  } else {
+    const int i = t->m[0][0] < t->m[1][1] ? (t->m[1][1] < t->m[2][2] ? 2 : 1) : (t->m[0][0] < t->m[2][2] ? 2 : 0);
+    const int j = (i + 1) % 3, k = (i + 2) % 3;
+    double s = sqrt(t->m[i][i] - t->m[j][j] - t->m[k][k] + 1.0);
+    q[i] = s * 0.5;
+    s = 0.5 / s;
+    q[3] = (t->m[k][j] - t->m[j][k]) * s;
+    q[j] = (t->m[j][i] + t->m[i][j]) * s;
+    q[k] = (t->m[k][i] + t->m[i][k]) * s;
+  }
+}
+static double tf_yaw_of(const orc_tf *t) {
+  double q[4];
+  tf_get_rotation(t, q);
+  const double x = q[0], y = q[1], z = q[2], w = q[3];
+  const double sqx = x * x, sqy = y * y, sqz = z * z, sqw = w * w;
+  const double sarg = -2 * (x * z - w * y) / (sqx + sqy + sqz + sqw);
+  if (sarg <= -0.99999) return -2 * atan2(y, x);
+  if (sarg >= 0.99999) return 2 * atan2(y, x);
+  return atan2(2 * (x * y + w * z), sqw + sqx - sqy - sqz);
+}
+static orc_tf tf_from_xyt(double x, double y, double theta) {
+  const double hy = theta * 0.5, hp = 0.0 * 0.5, hr = 0.0 * 0.5;
+  const double cy = cos(hy), sy = sin(hy), cp = cos(hp), sp = sin(hp), cr = cos(hr), sr = sin(hr);
+  const double q[4] = {sr * cp * cy - cr * sp * sy, cr * sp * cy + sr * cp * sy, cr * cp * sy - sr * sp * cy,
+                       cr * cp * cy + sr * sp * sy};
+  orc_tf t;
+  t.o[0] = x; t.o[1] = y; t.o[2] = 0.0;
+  tf_set_rotation(&t, q);
+  return t;
+}
+
+/* ranges [n_scans][n] float32, stamps [n_scans][2] (sec, nsec) -> out [n_scans] as b2s_plicp_odom_process fills it */
+void orc_plicp_odometry(const b2s_plicp_odom_params *P, int n, float angle_min, float angle_increment, float range_min,
+                        float range_max, int n_scans, const float *ranges, const uint32_t *stamps,
+                        b2s_plicp_odom_step *out) {
+  double *theta = malloc(sizeof(double) * n), *kf = malloc(sizeof(double) * n), *cur = malloc(sizeof(double) * n);
+  for (int i = 0; i < n; i++) theta[i] = (double)(angle_min + (float)i * angle_increment); /* :308 */
+  orc_tf b2l, l2b, bio, bio_kf;
+  b2l.o[0] = P->base_to_laser[0]; b2l.o[1] = P->base_to_laser[1]; b2l.o[2] = P->base_to_laser[2];
+  tf_set_rotation(&b2l, P->base_to_laser + 3);
+  l2b = tf_inverse(&b2l);
+  tf_identity(&bio);
+  tf_identity(&bio_kf);
+  double vx = 0.0, vaz = 0.0;
+  uint32_t last_sec = 0, last_nsec = 0;
+  int scan_count = 0, kf_scan = 0;
+  for (int s = 0; s < n_scans; s++) {
+    const float *r = ranges + (size_t)s * n;
+    b2s_plicp_odom_step *o = out + s;
+    memset(o, 0, sizeof *o);
+    if (s == 0) {
+      for (int i = 0; i < n; i++) kf[i] = r[i];
+      last_sec = stamps[0]; last_nsec = stamps[1];
+      o->orientation[3] = 1.0; o->keyframe = 1; o->reference_scan = -1;
+      continue;
+    }
+    for (int i = 0; i < n; i++) cur[i] = r[i];
+    /* ros::Time difference, ros::Duration normalisation, toSec() */
+    long long dsec = (long long)(int32_t)stamps[2 * s] - (int32_t)last_sec;
+    long long dnsec = (long long)(int32_t)stamps[2 * s + 1] - (int32_t)last_nsec;
+    long long nsec_part = dnsec % 1000000000LL, sec_part = dsec + dnsec / 1000000000LL;
+    if (nsec_part < 0) { nsec_part += 1000000000LL; --sec_part; }
+    const double dt = (double)(int32_t)sec_part + 1e-9 * (double)(int32_t)nsec_part;
+    const double pr_x = vx < 1e-6 ? 0.0 : dt * vx;
+    orc_tf pc = tf_from_xyt(pr_x, 0.0, 0.0);
+    orc_tf kfi = tf_inverse(&bio_kf), rel = tf_mul(&bio, &kfi);
+    pc = tf_mul(&pc, &rel);
+    orc_tf bioi = tf_inverse(&bio), t1 = tf_mul(&l2b, &bioi), t2 = tf_mul(&t1, &pc), t3 = tf_mul(&t2, &bio);
+    orc_tf pcl = tf_mul(&t3, &b2l);
+    const double guess[3] = {pcl.o[0], pcl.o[1], tf_yaw_of(&pcl)};
+    b2s_icp_result res;
+    orc_plicp_match(&P->icp, n, kf, cur, theta, (double)range_min, (double)range_max, guess, &res);
+    orc_tf corr;
+    tf_identity(&corr);
+    if (res.valid) {
+      orc_tf cl = tf_from_xyt(res.x[0], res.x[1], res.x[2]), u = tf_mul(&b2l, &cl);
+      corr = tf_mul(&u, &l2b);
+      bio = tf_mul(&bio_kf, &corr);
+      vx = corr.o[0] / dt;
+      vaz = tf_yaw_of(&corr) / dt;
+    }
+    for (int q = 0; q < 3; q++) { o->position[q] = bio.o[q]; o->first_guess[q] = guess[q]; }
+    tf_get_rotation(&bio, o->orientation);
+    o->linear[0] = vx;
+    o->angular[2] = vaz;
+    o->icp = res;
+    o->published = 1;
+    o->reference_scan = kf_scan;
+    int promote;
+    scan_count++;
+    if (fabs(tf_yaw_of(&corr)) > P->kf_dist_angular) promote = 1;
+    else if (scan_count == P->kf_scan_count) { scan_count = 0; promote = 1; }
+    else promote = corr.o[0] * corr.o[0] + corr.o[1] * corr.o[1] > P->kf_dist_linear * P->kf_dist_linear;
+    if (promote) {
+      memcpy(kf, cur, sizeof(double) * n);
+      bio_kf = bio;
+      kf_scan = s;
+    }
+    o->keyframe = promote;
+    last_sec = stamps[2 * s]; last_nsec = stamps[2 * s + 1];
+  }
+  free(theta); free(kf); free(cur);
+}

@@ -1,0 +1,98 @@
+"""TEST INFRASTRUCTURE — ctypes binding of oracle/_ref/liblesson3_ref.so: the UNMODIFIED lesson3 odometry node,
+reference/lesson3/src/plicp_odometry.cc, compiled where it lies against the ROS, tf2 and CSM stand-ins under oracle/shim/
+(with oracle/shim_lesson3/ros/ros.h in place of shim/ros/ros.h) by oracle/ref_lesson3.cpp, with sm_icp answered by
+oracle/plicp_oracle.c.  `build(ref)` makes the library from a
+checkout of the original project; where it is absent the tests replay its recorded answers (tests/reference_record.py).
+Only tests/ and __graft_entry__ may import this module.
+"""
+from __future__ import annotations
+
+import ctypes as C
+import os
+import subprocess
+import sys
+
+import numpy as np
+
+_HERE = os.path.dirname(os.path.abspath(__file__))
+_ROOT = os.path.dirname(_HERE)
+_PATH = os.path.join(_HERE, "_ref", "liblesson3_ref.so")
+# the flags of oracle/Makefile's builds: x86-64 baseline, no -march, no FMA contraction
+CXXFLAGS = ["-std=c++17", "-O2", "-fPIC", "-w", "-ffp-contract=off"]
+CFLAGS = ["-std=c11", "-O2", "-fPIC", "-w", "-ffp-contract=off"]
+_SHIM = ["../shim_lesson3/ros/ros.h", "sensor_msgs/LaserScan.h", "nav_msgs/Odometry.h", "geometry_msgs/messages.h",
+         "geometry_msgs/TransformStamped.h", "geometry_msgs/TwistStamped.h", "tf2/LinearMath/Transform.h", "tf2/utils.h",
+         "tf2_ros/transform_listener.h", "tf2_ros/transform_broadcaster.h", "tf2_geometry_msgs/tf2_geometry_msgs.h",
+         "csm/csm_all.h"]
+_lib = None
+
+
+def build(ref: str) -> str:
+    srcs = [os.path.join(ref, "lesson3", "src", "plicp_odometry.cc"),
+            os.path.join(ref, "lesson3", "include", "lesson3", "plicp_odometry.h")]
+    drv, orc = os.path.join(_HERE, "ref_lesson3.cpp"), os.path.join(_HERE, "plicp_oracle.c")
+    deps = srcs + [drv, orc, os.path.join(_ROOT, "include", "b200slam.h")] + [os.path.join(_HERE, "shim", h) for h in _SHIM]
+    if not os.path.exists(_PATH) or any(os.path.getmtime(d) > os.path.getmtime(_PATH) for d in deps):
+        os.makedirs(os.path.dirname(_PATH), exist_ok=True)
+        tmp = _PATH + f".{os.getpid()}.tmp"
+        obj = tmp + ".o"
+        subprocess.check_call([os.environ.get("CC", "gcc")] + CFLAGS + ["-c", orc, "-o", obj])
+        subprocess.check_call([os.environ.get("CXX", "g++")] + CXXFLAGS +
+                              ["-shared", "-I" + os.path.join(_HERE, "shim_lesson3"), "-I" + os.path.join(_HERE, "shim"),
+                               "-I" + os.path.abspath(ref),
+                               "-I" + os.path.join(os.path.abspath(ref), "lesson3", "include"), drv, obj, "-o", tmp,
+                               "-lm"])
+        os.remove(obj)
+        os.replace(tmp, _PATH)
+    return _PATH
+
+
+def available() -> bool:
+    return os.path.exists(_PATH)
+
+
+def lib():
+    global _lib
+    if _lib is None:
+        L = C.CDLL(_PATH)
+        dp, fp = C.POINTER(C.c_double), C.POINTER(C.c_float)
+        L.ref_plicp_clear_params.argtypes = []
+        L.ref_plicp_clear_params.restype = None
+        L.ref_plicp_param.argtypes = [C.c_char_p, C.c_double]
+        L.ref_plicp_param.restype = None
+        L.ref_plicp_new.argtypes = [dp]
+        L.ref_plicp_new.restype = None
+        L.ref_plicp_scan.argtypes = [C.c_uint32, C.c_uint32, fp, C.c_int, fp, C.c_void_p]
+        L.ref_plicp_scan.restype = C.c_int
+        _lib = L
+    return _lib
+
+
+def run(params: dict, mount, fields, ranges, stamps):
+    """A fresh node with the parameter-server values `params` (name -> number) and the laser mount (translation xyz +
+    quaternion xyzw) over one recording.  fields = (angle_min, angle_increment, range_min, range_max) float32,
+    ranges [S][n] float32, stamps [S][2].  -> structured array [S] of the package's plicp.STEP_DTYPE (reference_scan is
+    the index of the key frame each scan was matched against, tracked from the keyframe flags)."""
+    L = lib()
+    sys.path.insert(0, _ROOT) if _ROOT not in sys.path else None
+    import importlib
+    dtype = importlib.import_module("creating-2d-laser-slam-from-scratch_b200.plicp").STEP_DTYPE
+    L.ref_plicp_clear_params()
+    for k, v in params.items():
+        L.ref_plicp_param(k.encode(), float(v))
+    m = np.ascontiguousarray(mount, np.float64)
+    L.ref_plicp_new(m.ctypes.data_as(C.POINTER(C.c_double)))
+    f = np.ascontiguousarray(fields, np.float32)
+    r = np.ascontiguousarray(ranges, np.float32)
+    out = np.zeros(len(r), dtype)
+    kf = -1
+    for s in range(len(r)):
+        rc = L.ref_plicp_scan(int(stamps[s][0]), int(stamps[s][1]), f.ctypes.data_as(C.POINTER(C.c_float)), r.shape[1],
+                              r[s].ctypes.data_as(C.POINTER(C.c_float)), out[s:s + 1].ctypes.data)
+        if rc != 0:
+            raise RuntimeError("the lesson3 node threw (a CSM switch the stand-in refuses)")
+        if out[s]["published"]:
+            out[s]["reference_scan"] = kf
+        if out[s]["keyframe"]:
+            kf = s
+    return out
