@@ -20,6 +20,7 @@
 #include <vector>
 
 #include "common.cuh"
+#include "gmapping_grid.cuh"
 
 using namespace b2s;
 
@@ -38,38 +39,14 @@ struct b2s_gmap {
 
 namespace b2s {
 
-__device__ __forceinline__ int gm_world2map(double w, double c, double delta, int half) {  // map.h:171-174
-  return cast_i32(round((w - c) / delta)) + half;
-}
-
-struct GmRay {
-  bool valid, hit;
-  int p1x, p1y;
-  double hx, hy;
-};
-
-__device__ __forceinline__ GmRay gm_ray(double d, double angle, double lx, double ly, double cx, double cy,
-                                        double delta, int sx2, int sy2, double max_range, double max_use) {
-  GmRay r;
-  r.valid = !(d > max_range || d == 0.0 || !isfinite(d));  // gmapping.cc:193-195
-  r.hit = false; r.p1x = r.p1y = 0; r.hx = r.hy = 0;
-  if (!r.valid) return r;
-  if (d > max_use) d = max_use;
-  r.hx = __dadd_rn(lx, __dmul_rn(d, cos(angle)));
-  r.hy = __dadd_rn(ly, __dmul_rn(d, sin(angle)));
-  r.p1x = gm_world2map(r.hx, cx, delta, sx2);
-  r.p1y = gm_world2map(r.hy, cy, delta, sy2);
-  r.hit = d < max_use;  // gmapping.cc:218
-  return r;
-}
-
 // any ray leaving the map? (the reference asserts / indexes out of range there: map.h:186-191, harray2d.h:206-227)
 __global__ void k_gm_check(const double *__restrict__ ranges, const double *__restrict__ angles, int nb, double lx,
                            double ly, double cx, double cy, double delta, int sx2, int sy2, int msx, int msy,
                            double max_range, double max_use, int *__restrict__ flag) {
   int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= nb) return;
-  GmRay r = gm_ray(ranges[i], angles[i], lx, ly, cx, cy, delta, sx2, sy2, max_range, max_use);
+  const auto u = [&] { return make_double2(cos(angles[i]), sin(angles[i])); };
+  GmRay r = gm_ray(ranges[i], u, lx, ly, cx, cy, delta, sx2, sy2, max_range, max_use);
   if (r.valid && (r.p1x < 0 || r.p1y < 0 || r.p1x >= msx || r.p1y >= msy)) *flag = 1;
 }
 
@@ -83,25 +60,14 @@ __global__ void __launch_bounds__(256)
   const int warp0 = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, nwarps = (gridDim.x * blockDim.x) >> 5;
   const int p0x = gm_world2map(lx, cx, delta, sx2), p0y = gm_world2map(ly, cy, delta, sy2);
   for (int i = warp0; i < nb; i += nwarps) {
-    GmRay r = gm_ray(ranges[i], angles[i], lx, ly, cx, cy, delta, sx2, sy2, max_range, max_use);
+    const auto u = [&] { return make_double2(cos(angles[i]), sin(angles[i])); };
+    GmRay r = gm_ray(ranges[i], u, lx, ly, cx, cy, delta, sx2, sy2, max_range, max_use);
     if (!r.valid) continue;
-    const int dx = abs(r.p1x - p0x), dy = abs(r.p1y - p0y);
-    const bool xmajor = dy <= dx;  // gridlinetraversal.h:44
-    // canonical traversal starts at the endpoint with the smaller dominant coordinate (start wins ties)
-    const int s_maj = xmajor ? p0x : p0y, e_maj = xmajor ? r.p1x : r.p1y;
-    const int s_min = xmajor ? p0y : p0x, e_min = xmajor ? r.p1y : r.p1x;
-    const bool from_end = s_maj > e_maj;
-    const int b_maj = from_end ? e_maj : s_maj, b_min = from_end ? e_min : s_min;
-    const int o_min = from_end ? s_min : e_min;
-    const int step_min = (o_min > b_min) ? 1 : -1;
-    const long long dmaj = xmajor ? dx : dy, dmin = xmajor ? dy : dx;
-    const long long k_end = from_end ? 0 : dmaj;  // the step at which the traversal sits on p1
-    for (long long k = lane; k <= dmaj; k += 32) {
-      if (k == k_end) continue;  // all points but the last of the p0 -> p1 list are free (gmapping.cc:229-235)
-      const long long j = dmaj > 0 ? (2 * k * dmin + dmaj) / (2 * dmaj) : 0;
-      const int maj = b_maj + (int)k, mn = b_min + step_min * (int)j;
-      const int x = xmajor ? maj : mn, y = xmajor ? mn : maj;
-      atomicAdd(visits + x + (size_t)y * msx, 1);
+    const GmLine L = gm_line(p0x, p0y, r.p1x, r.p1y);
+    for (long long k = lane; k <= L.dmaj; k += 32) {
+      if (k == L.k_end) continue;  // all points but the last of the p0 -> p1 list are free (gmapping.cc:229-235)
+      const int2 c = gm_line_cell(L, k);
+      atomicAdd(visits + c.x + (size_t)c.y * msx, 1);
     }
     if (lane == 0 && r.hit) {  // gmapping.cc:237-241, map.h:37-48
       const size_t c = (size_t)r.p1x + (size_t)r.p1y * msx;
@@ -125,9 +91,7 @@ __global__ void k_gm_ros(const int32_t *__restrict__ n, const int32_t *__restric
   if (x == 0 && y > 0 && width < msx && y - 1 < msy) { x = width; y -= 1; }
   if (x >= msx || y >= msy) return;
   const size_t c = (size_t)x + (size_t)y * msx;
-  const int v = visits[c];
-  const double occ = v ? (double)n[c] * 1 / (double)v : -1;
-  out[o] = occ < 0 ? -1 : (occ > occ_thresh ? 100 : 0);
+  out[o] = gm_classify(n[c], visits[c], occ_thresh);
 }
 
 }  // namespace b2s

@@ -60,6 +60,12 @@ __device__ __forceinline__ int2 end_cell(float c, float s, float mx, float my, f
   return make_int2((int)__fadd_rn(ex, 0.5f), (int)__fadd_rn(ey, 0.5f));
 }
 
+// end cell of one beam in updateByScanJustOnce (:175-217), the lesson4 make-map variant: begin + (int)round(p / 0.05)
+// on the raw point in metres (float / double literal -> double, ::round, (int)), whatever the map's cell size
+__device__ __forceinline__ int2 just_once_end_cell(int bx, int by, float px, float py) {
+  return make_int2(bx + cast_i32(round((double)px / 0.05)), by + cast_i32(round((double)py / 0.05)));
+}
+
 // updateLineBresenhami's set-up (:220-258): the line is drawn iff begin != end and both cells are inside the map.
 // bresenham2D then visits da cells from the start (the end cell excluded), see bresenham_offset.
 struct BresenhamLine {

@@ -58,12 +58,10 @@ struct b2s_hector_map {
 
 namespace b2s {
 
-// end cell + updateLineBresenhami set-up.  updateByScanJustOnce (OccGridMapBase.h:182-203) takes its end cell as
-// begin + (int)round(p / 0.05) on the raw points in metres: float / double literal -> double, ::round, (int).
+// end cell + updateLineBresenhami set-up
 __device__ __forceinline__ BresenhamLine hc_line(float c, float s, float mx, float my, bool just_once, int bx, int by,
                                                  float px, float py, int sx, int sy) {
-  const int2 end = just_once ? make_int2(bx + cast_i32(round((double)px / 0.05)), by + cast_i32(round((double)py / 0.05)))
-                             : end_cell(c, s, mx, my, px, py);
+  const int2 end = just_once ? just_once_end_cell(bx, by, px, py) : end_cell(c, s, mx, my, px, py);
   return bresenham_line(bx, by, end, sx, sy);
 }
 

@@ -785,6 +785,63 @@ b2s_status b2s_lidar_undistort(int batch, int n_beams, const float *ranges, doub
 b2s_status b2s_feature_detect(int batch, int n, const float *ranges, float edge_threshold, float *out_ranges,
                               int32_t *out_count, float *out_curvature, int device, void *cuda_stream);
 
+/* ---------------------------------------------------------------- lesson4: the make-map nodes over whole recordings
+ * lesson4's GMapping node (src/gmapping/gmapping.cc) and Hector make-map node (src/hector_mapping/hector_mapping.cc)
+ * each build a fresh map from every LaserScan with the robot at the origin and publish it as a nav_msgs/OccupancyGrid.
+ * These calls return, for every scan of a recording, the `data` payload the node publishes, bit for bit
+ * (tests/test_lesson4_nodes_reference.py pins the restatement to the unmodified nodes, tests/test_gpu_lesson4_nodes.py
+ * the device to the restatement).  One laser per call: `geometry` stands in for the node's first scan (angle_min,
+ * angle_increment, range_min, range_max, n_ranges; its `ranges` pointer is not read).  ranges [n_scans][n_ranges]
+ * float32 (host); out_maps [n_scans][height][width] int8 (host; page-locked memory lets the copies overlap the
+ * compute), every byte defined.  out_dims = (width, height) as the node sizes its message; with out_maps NULL the call
+ * only fills out_dims and needs no device.  Scans are independent: calls over consecutive chunks of a recording equal
+ * one call.  n_scans == 0 does nothing.  Refused before anything is written: B2S_ERR_BAD_PARAMS for NULL arguments
+ * (ranges may be NULL only when out_maps is NULL or n_scans is 0), negative counts or unusable bounds;
+ * B2S_ERR_TOO_LARGE for n_ranges above B2S_NODE_MAPS_MAX_RANGES or a payload of 2^31 bytes or more.
+ * The beams' unit vectors are taken on the host with the C library; no transcendental function runs on the device.
+ * Returns when the maps are on the host. */
+#define B2S_NODE_MAPS_MAX_RANGES 16384
+
+typedef struct b2s_gmapping_node_params { /* GMapping::InitParams (gmapping.cc:44-84); node defaults in brackets */
+  double max_range;     /* maxRange [30 - 0.01]: beams longer than this, 0 or non-finite are skipped */
+  double max_use_range; /* maxUrange [25]: longer beams are clipped to it and mark no hit */
+  double xmin, ymin, xmax, ymax; /* map bounds [-40, -40, 40, 40] */
+  double delta;         /* cell size [0.05] */
+  double occ_thresh;    /* occupied above this hit fraction [0.25] */
+} b2s_gmapping_node_params;
+
+/* GMapping::ScanCallback on every scan.  width = (xmax - xmin) / (float)delta truncated, as the node divides by the
+ * message's float32 resolution (gmapping.cc:72-73): 1599 at the defaults, while the map's storage is 1600 x 1600
+ * (ceil((xmax - xmin) / delta) rounded down to 32-cell patches, map.h:133).  Storage cell (x, y) is published at
+ * MAP_IDX(width, x, y) = width * y + x, x outer and y inner, so a later cell overwrites an earlier one at the same byte
+ * (at the defaults storage column 1599 of row y lands on byte (0, y + 1)); writes at or past width * height, where the
+ * node overruns its own buffer (1 601 writes on 1 600 bytes at the defaults), are dropped; a byte no storage cell
+ * reaches is 0, as the node's resized vector leaves it.  The beam cache is CreateCache's (:112-124): angle_min +
+ * i * angle_increment summed in float, then the C library's double cos / sin.  B2S_ERR_OUT_OF_RANGE, with the first
+ * such scan named in b2s_last_error(), when a kept beam's end cell or the laser's cell lies outside the storage (the
+ * node's assert, map.h:186-191); nothing is written then.  B2S_ERR_BAD_PARAMS also when the storage is smaller than
+ * one 32-cell patch. */
+b2s_status b2s_gmapping_node_maps(const b2s_laser_scan_msg *geometry, const b2s_gmapping_node_params *params,
+                                  int n_scans, const float *ranges, int32_t out_dims[2], int8_t *out_maps, int device,
+                                  void *cuda_stream);
+
+typedef struct b2s_hector_mapping_node_params { /* HectorMapping::InitParams (hector_mapping.cc:44-79) */
+  double xmin, ymin, xmax, ymax; /* map bounds [-40, -40, 40, 40] */
+  float delta;                   /* resolution_, a float in the node [0.05] */
+  float reserved;                /* 0 */
+} b2s_hector_mapping_node_params;
+
+/* HectorMapping::ScanCallback on every scan.  width = (int)((xmax - xmin) / delta), height likewise (1599 x 1599 at
+ * the defaults).  A beam is kept iff range_min < r < range_max - 0.1f (:150-156); its point is (cos(a) * r,
+ * sin(a) * r) in double rounded to float, the angle a accumulated in float beam by beam (:144-163) and cos / sin the
+ * C library's double functions, as the node's unqualified call on a float resolves where <math.h> is not included
+ * (DESIGN §7).  updateByScanJustOnce (OccGridMapBase.h:175-217) draws every kept beam from cell (800, 800) to
+ * (800, 800) + (int)round(p / 0.05), whatever delta is, when the two differ and both lie inside the map.  Each byte
+ * is 100 where a drawn beam ends, else 0 where one passes, else -1 (PublishMap, :177-211). */
+b2s_status b2s_hector_mapping_node_maps(const b2s_laser_scan_msg *geometry, const b2s_hector_mapping_node_params *params,
+                                        int n_scans, const float *ranges, int32_t out_dims[2], int8_t *out_maps,
+                                        int device, void *cuda_stream);
+
 #ifdef __cplusplus
 }
 #endif
