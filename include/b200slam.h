@@ -766,6 +766,55 @@ b2s_status b2s_lidar_undistort(int batch, int n_beams, const float *ranges, doub
                                const double *imu_rot_y, const double *imu_rot_z, int imu_stride, float *out_xyz, int device,
                                void *cuda_stream);
 
+/* The whole node over one recording of one laser: LidarUndistortion's callbacks (:82-159) and queue pruning
+ * (PruneImuDeque :177-249, PruneOdomDeque :252-336) on the host, CorrectLaserScan for every published scan on the
+ * device.  The node's AsyncSpinner serves the three streams under separate locks, so what it saw at a scan's callback
+ * is the number of IMU and odometry messages delivered before it: imu_arrived / odom_arrived, non-decreasing over the
+ * scans.  Scan k is corrected at the callback of scan k + 1 with the messages delivered by then, so the last scan is
+ * never published; a scan whose queues do not cover it is dropped.  The angle cache and the beam count come from the
+ * first scan, as the node caches them; stamp, time_increment, range_min and range_max from each.  Stamps are
+ * (sec, nsec) and compared as ros::Time::toSec doubles.  tf's quaternionMsgToTF and Matrix3x3::getRPY are restated on the
+ * host (a zero quaternion, the default of a message the node never received, gives NaN angles). */
+typedef struct b2s_imu_msg {
+  uint32_t sec, nsec;
+  double angular_velocity[3];
+} b2s_imu_msg;
+typedef struct b2s_odom_msg {
+  uint32_t sec, nsec;
+  double position[3], orientation[4]; /* quaternion x, y, z, w */
+} b2s_odom_msg;
+typedef struct b2s_deskew_node_scan {
+  uint32_t sec, nsec;                   /* header.stamp */
+  float time_increment, range_min, range_max;
+  int32_t imu_arrived, odom_arrived;    /* messages of each log delivered before this scan's callback */
+  int32_t reserved;                     /* 0 */
+} b2s_deskew_node_scan;
+
+/* out_status values, per corrected scan */
+#define B2S_DESKEW_PUBLISHED 0  /* the node published the scan's cloud */
+#define B2S_DESKEW_HELD 1       /* the recording's last scan: still in the laser queue */
+#define B2S_DESKEW_WAIT_IMU 2   /* "Waiting for IMU data": the IMU queue is empty or does not cover the scan */
+#define B2S_DESKEW_IMU_EMPTY 3  /* the IMU queue was pruned empty */
+#define B2S_DESKEW_WAIT_ODOM 4  /* "Waiting for Odometry data" */
+#define B2S_DESKEW_ODOM_EMPTY 5 /* the odometry queue was pruned empty */
+#define B2S_DESKEW_UNDEFINED 6  /* the node's IMU integration reads imu_time_[-1] (the first message it integrates is
+                                   at or after the scan start) or passes its 2000-entry table */
+
+/* ranges [n_scans][n_beams] (host); imu [n_imu] and odom [n_odom] in delivery order (NULL allowed where the flag is off
+ * or the count is 0).  out_status [n_scans]: a B2S_DESKEW_* value per scan.  out_state [n_scans] (may be NULL): the
+ * b2s_deskew_scan a published row was computed from (imu_last -1 where an IMU gap covers the whole scan: the node then
+ * takes rotation 0 throughout), or an undefined row's with imu_last -2; other rows are zero bytes.  Fed with the IMU
+ * table b2s_deskew_integrate_imu returns over the pruned queue, it reproduces the row through b2s_lidar_undistort.
+ * out_xyz [n_scans][n_beams][3] (host): the published cloud, zero bytes in every other row.  Refused before anything is
+ * written: B2S_ERR_BAD_PARAMS for NULL arrays, negative counts, n_beams < 1, arrival counts that decrease or exceed
+ * their log, or a NULL log whose flag is on.  n_scans == 0 does nothing and needs no device; otherwise
+ * B2S_ERR_NO_DEVICE without one.  The odometry prune still runs after an undefined IMU integration, as the node goes
+ * on; an undefined row keeps that status whatever the odometry prune finds.  Returns when the clouds are on the host. */
+b2s_status b2s_lidar_undistortion_node(int use_imu, int use_odom, float angle_min, float angle_increment, int n_beams,
+                                       int n_scans, const b2s_deskew_node_scan *scans, const float *ranges, int n_imu,
+                                       const b2s_imu_msg *imu, int n_odom, const b2s_odom_msg *odom, int32_t *out_status,
+                                       b2s_deskew_scan *out_state, float *out_xyz, int device, void *cuda_stream);
+
 /* ---------------------------------------------------------------- lesson1: corner-feature extraction
  * LaserScan::ScanCallback (lesson1/src/feature_detection.cc:77-179): the finite readings of a scan, a curvature
  * c = d * d from an 11-reading stencil (:112-124), and in each of six sectors the first 20 entries above edge_threshold
