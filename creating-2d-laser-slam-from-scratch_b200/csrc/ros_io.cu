@@ -12,10 +12,11 @@
 
 using namespace b2s;
 
-extern "C" {
+namespace b2s {
 
-b2s_status b2s_ros_karto_laser(const b2s_laser_scan_msg *scan, const double laser_pose_in_base[3], double use_scan_range,
-                               b2s_laser *out) {
+// getLaser's setters without any reading-count check (b2s_karto_node_create uses it too)
+b2s_status karto_laser_from_msg(const b2s_laser_scan_msg *scan, const double laser_pose_in_base[3], double use_scan_range,
+                                b2s_laser *out) {
   if (!scan || !laser_pose_in_base || !out) B2S_FAIL(B2S_ERR_BAD_PARAMS, "null argument");
   // the setters take kt_double: the float32 message fields widen exactly
   const double min_angle = scan->angle_min, max_angle = scan->angle_max, res = scan->angle_increment;
@@ -32,9 +33,19 @@ b2s_status b2s_ros_karto_laser(const b2s_laser_scan_msg *scan, const double lase
   out->offset_pose[2] = laser_pose_in_base[2];
   out->n_readings = (int32_t)cast_u32(kround((max_angle - min_angle) / res));  // Update(): no + 1
   out->reserved = 0;
+  return B2S_OK;
+}
+
+}  // namespace b2s
+
+extern "C" {
+
+b2s_status b2s_ros_karto_laser(const b2s_laser_scan_msg *scan, const double laser_pose_in_base[3], double use_scan_range,
+                               b2s_laser *out) {
+  if (b2s_status st = karto_laser_from_msg(scan, laser_pose_in_base, use_scan_range, out)) return st;
   if (out->n_readings != scan->n_ranges)
     B2S_FAIL(B2S_ERR_BAD_PARAMS, "LaserScan carries a different number of ranges than Round((angle_max - angle_min) / angle_increment): "
-                                 "LaserRangeFinder::Validate rejects such scans");
+                                 "this function requires the two to be equal");
   return B2S_OK;
 }
 

@@ -525,12 +525,84 @@ typedef struct b2s_laser_scan_msg { /* the sensor_msgs/LaserScan fields the node
  * angles / ranges from the message, offset = laser pose in base_link (x, y, yaw), range threshold clipped into
  * [range_min, range_max] (Karto.h:3778-3787), n_readings = Round((max - min) / resolution) WITHOUT + 1
  * (LaserRangeFinder::Update, Karto.h:4152-4161).  Returns B2S_ERR_BAD_PARAMS if the message carries a different
- * number of ranges than that (LaserRangeFinder::Validate would reject every scan). */
+ * number of ranges than that.  That check is this function's own, stricter than the reference: its
+ * LaserRangeFinder::Validate(SensorData *) has the count comparison commented out (Karto.cpp:186-199) and accepts every
+ * scan, and LocalizedRangeScan::Update then uses the first n_readings readings.  b2s_karto_node_create follows the
+ * reference and accepts n_ranges >= n_readings. */
 b2s_status b2s_ros_karto_laser(const b2s_laser_scan_msg *scan, const double laser_pose_in_base[3], double use_scan_range,
                                b2s_laser *out);
 /* SlamKarto::addScan (karto_slam.cc:407-434): float32 ranges -> kt_double readings, in reverse order for a laser
  * mounted upside-down (lasers_inverted_) */
 b2s_status b2s_ros_karto_readings(const b2s_laser_scan_msg *scan, int inverted, double *out_readings);
+
+/* ---------------------------------------------------------------- lesson6: the Karto SLAM node over whole recordings
+ * SlamKarto (lesson6/src/karto_slam.cc) for one laser: its throttle, getLaser, getOdomPose, Mapper::Process (the device
+ * Mapper, b2s_mapper_*), the map -> odom transform and the map-update gate with updateMap (the device occupancy grid,
+ * b2s_occ_grid_*), over a recording handed in as arrays.  tests/test_karto_node_reference.py pins the restatement
+ * oracle/karto_node_port.py to the unmodified node; tests/test_gpu_karto_node.py pins this handle to the restatement.
+ * The tf arithmetic is tf's LinearMath in double, operation by operation (Transform product and inverse, Matrix3x3
+ * setRotation / getRotation, Quaternion setRPY, getYaw through getRPY); ros::Time / Duration are roscpp's integer
+ * arithmetic.  Neither tf nor roscpp is in the reference tree, so those lines are pinned to the stand-ins under
+ * oracle/shim_lesson6/ (DESIGN.md §7). */
+typedef struct b2s_karto_node_params {
+  int32_t throttle_scans;     /* [1] a scan is processed when the count of scans handed in so far divides by it */
+  int32_t reserved;           /* 0 */
+  double map_update_interval; /* [5.0] s, ros::Duration::fromSec: a map is due when the stamp difference is STRICTLY
+                                 greater */
+  double resolution;          /* [0.05] m, OccupancyGrid::CreateFromScans */
+  double use_scan_range;      /* [12.0] m, the laser's range threshold (clipped into [range_min, range_max]) */
+  b2s_mapper_params mapper;   /* values as the Mapper STORES them after SlamKarto::InitParams (three of its setParam*
+                                 calls square their argument); the matchers' range_threshold is replaced by the
+                                 laser's */
+} b2s_karto_node_params;
+
+/* out_state values, one per scan handed in */
+#define B2S_KARTO_THROTTLED 0    /* laser_count_ % throttle_scans != 0: the callback returned at once */
+#define B2S_KARTO_NO_ODOM 1      /* the odom <- base_link lookup failed (a NaN in the scan's odom row): skipped */
+#define B2S_KARTO_NOT_MOVED 2    /* Mapper::Process returned false (HasMovedEnough) */
+#define B2S_KARTO_PROCESSED 3    /* Mapper::Process returned true */
+
+/* One published map (the node's sst_.publish): info as b2s_occ_grid_info_get gives it (origin = offset, float32
+ * resolution in the message = (float)resolution), payload [height][width] int8 as b2s_occ_grid_copy_ros.  scan_index
+ * counts every scan handed to the handle, over all calls.  Both pointers are valid only during the call. */
+typedef void (*b2s_karto_map_fn)(void *user, int32_t scan_index, const b2s_occ_grid_info *info, const int8_t *payload);
+
+typedef struct b2s_karto_node b2s_karto_node; /* opaque: one SlamKarto */
+
+/* SlamKarto's constructor and getLaser.  geometry = the recording's LaserScan fields (angle_min, angle_max,
+ * angle_increment, range_min, range_max, n_ranges; its ranges pointer is not read).  The laser has m =
+ * Round((angle_max - angle_min) / angle_increment) readings (LaserRangeFinder::Update, no + 1); a scan's first m
+ * readings are used, after the reversal of an upside-down laser, and the rest are ignored, as the node does.  A standard
+ * ROS scan (angle_max = angle_min + (n - 1) * angle_increment) has m = n - 1: its last beam is dropped.
+ * laser_mount = base_link <- laser as translation xyz + quaternion xyzw: the laser's offset is its x, y and getYaw; it
+ * is upside-down when the mount sends base_link's point (0, 0, 1 + z) to z <= 0 in the laser frame.  solver: NULL =
+ * use_back_end false (the node's default), else the back end Mapper::SetScanSolver gets (copied; its user data must
+ * outlive the handle).  B2S_ERR_BAD_PARAMS for NULL pointers, throttle_scans <= 0 (the node divides by it),
+ * resolution not > 0, a map_update_interval that is not finite or outside ros::Duration's 32-bit range, a zero
+ * angle_increment, a zero / non-finite mount quaternion, m < 1, or n_ranges < m (the node reads past the message's
+ * ranges); whatever b2s_mapper_create refuses; B2S_ERR_NO_DEVICE without a device. */
+b2s_status b2s_karto_node_create(const b2s_karto_node_params *params, const b2s_laser_scan_msg *geometry,
+                                 const double laser_mount[7], const b2s_scan_solver *solver, int device,
+                                 b2s_karto_node **out);
+void b2s_karto_node_destroy(b2s_karto_node *node);
+/* The inner Mapper: b2s_mapper_get_poses / _get_edges / _stats / _scan_count read the node's graph.  Owned by the
+ * node; do not destroy it or process scans through it. */
+b2s_mapper *b2s_karto_node_mapper(b2s_karto_node *node);
+/* SlamKarto::laserCallback on the next n_scans LaserScans: ranges [n_scans][n_ranges] float32 (widened to double as the
+ * node does), stamps [n_scans][2] = header.stamp (sec, nsec), odom [n_scans][7] = the odom <- base_link transform the
+ * tf lookup answers at that stamp (translation xyz + quaternion xyzw; any NaN = the lookup fails).  Per scan:
+ * out_state (B2S_KARTO_*), out_pose [3] the corrected pose Mapper::Process left (0 unless processed), out_map_to_odom
+ * [7] map_to_odom_ after the scan (translation xyz + quaternion xyzw, from getRotation), out_map_published 1 when
+ * updateMap published; any output may be NULL.  A processed scan's scan time is 0 (the node never sets it), so
+ * minimum_time_interval never admits a scan.  A map is built when none was yet or the stamp minus the last map's stamp
+ * exceeds map_update_interval, from every processed scan at its corrected pose at that moment (they move after a loop
+ * closure when a solver is set), and handed to on_map (may be NULL) before the call goes on.  Two calls over
+ * consecutive parts of a recording equal one call.  B2S_ERR_BAD_PARAMS (nothing written) for NULL arrays with
+ * n_scans > 0 or n_scans < 0; B2S_ERR_BAD_STATE after a call failed inside the Mapper (its rows up to the failing scan
+ * are written then).  Returns when every map has been handed out. */
+b2s_status b2s_karto_node_process(b2s_karto_node *node, int n_scans, const float *ranges, const uint32_t *stamps,
+                                  const double *odom, int32_t *out_state, double *out_pose, double *out_map_to_odom,
+                                  int32_t *out_map_published, b2s_karto_map_fn on_map, void *user);
 /* HectorMappingRos::rosPointCloudToDataContainer (lesson4/src/hector_mapping/hector_slam.cc:320-362): laser-frame points
  * ([n][3] float x, y, z as laser_geometry projected them) -> DataContainer entries in map-cell units.  laser_in_base =
  * (x, y, z, yaw) of the laser in base_link.  Filters: squared distance in (min_dist^2, max_dist^2), not behind the robot

@@ -1,0 +1,3 @@
+// TEST INFRASTRUCTURE — see tf_core.h.
+#pragma once
+#include "tf/tf_core.h"
