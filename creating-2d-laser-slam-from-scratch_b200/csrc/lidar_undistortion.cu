@@ -21,6 +21,7 @@
 #include <vector>
 
 #include "common.cuh"
+#include "ros_math.cuh"
 
 using namespace b2s;
 
@@ -246,43 +247,15 @@ __global__ void __launch_bounds__(NODE_THREADS)
   }
 }
 
-double to_sec(uint32_t sec, uint32_t nsec) { return (double)sec + 1e-9 * (double)nsec; }  // ros::Time::toSec
-
 // (x, y, z, roll, pitch, yaw) of an odometry message as PruneOdomDeque takes it (:304-325): tf::quaternionMsgToTF, then
-// tf::Matrix3x3(q).getRPY, restated from tf's published LinearMath (setRotation, getEulerYPR solution 1)
+// tf::Matrix3x3(q).getRPY
 void odom_pose(const b2s_odom_msg &m, double out[6]) {
-  const double x = m.orientation[0], y = m.orientation[1], z = m.orientation[2], w = m.orientation[3];
-  const double d = x * x + y * y + z * z + w * w, s = 2.0 / d;
-  const double xs = x * s, ys = y * s, zs = z * s;
-  const double wx = w * xs, wy = w * ys, wz = w * zs;
-  const double xx = x * xs, xy = x * ys, xz = x * zs;
-  const double yy = y * ys, yz = y * zs, zz = z * zs;
-  const double m00 = 1.0 - (yy + zz), m01 = xy - wz, m02 = xz + wy;
-  const double m10 = xy + wz;  // getRPY does not read m[1][1] or m[1][2]
-  const double m20 = xz - wy, m21 = yz + wx, m22 = 1.0 - (xx + yy);
-  double roll, pitch, yaw;
-  if (std::fabs(m20) >= 1) {
-    yaw = 0;
-    const double delta = std::atan2(m01, m02);
-    if (m20 > 0) {
-      pitch = -M_PI / 2;
-      roll = -yaw + std::atan2(-m01, -m02);
-    } else {
-      pitch = M_PI / 2;
-      roll = yaw + delta;
-    }
-  } else {
-    pitch = -std::asin(m20);
-    const double c = std::cos(pitch);
-    roll = std::atan2(m21 / c, m22 / c);
-    yaw = std::atan2(m10 / c, m00 / c);
-  }
+  TfTransform t;
+  tf_set_rotation(t, m.orientation);
   out[0] = m.position[0];
   out[1] = m.position[1];
   out[2] = m.position[2];
-  out[3] = roll;
-  out[4] = pitch;
-  out[5] = yaw;
+  tf_get_rpy(t, out[3], out[4], out[5]);
 }
 
 }  // namespace
@@ -379,8 +352,8 @@ b2s_status b2s_lidar_undistortion_node(int use_imu, int use_odom, float angle_mi
 
   // ---- the callbacks, on the host: statuses, per-scan states and the IMU queue of every published scan
   std::vector<double> imu_t(use_imu ? n_imu : 0), odom_t(use_odom ? n_odom : 0);
-  for (size_t i = 0; i < imu_t.size(); i++) imu_t[i] = to_sec(imu[i].sec, imu[i].nsec);
-  for (size_t i = 0; i < odom_t.size(); i++) odom_t[i] = to_sec(odom[i].sec, odom[i].nsec);
+  for (size_t i = 0; i < imu_t.size(); i++) imu_t[i] = ros_time_to_sec(imu[i].sec, imu[i].nsec);
+  for (size_t i = 0; i < odom_t.size(); i++) odom_t[i] = ros_time_to_sec(odom[i].sec, odom[i].nsec);
   const double scan_count = (double)n_beams;  // scan_count_, a double member, from the first scan (:136)
   std::vector<NodeRow> rows;
   std::vector<b2s_deskew_scan> states;
@@ -398,7 +371,7 @@ b2s_status b2s_lidar_undistortion_node(int use_imu, int use_odom, float angle_mi
         return;
       }
       const b2s_deskew_node_scan &sc = scans[j], &next = scans[j + 1];
-      const double start = to_sec(sc.sec, sc.nsec), inc = sc.time_increment, end = start + inc * (scan_count - 1);
+      const double start = ros_time_to_sec(sc.sec, sc.nsec), inc = sc.time_increment, end = start + inc * (scan_count - 1);
       w.scan_end = end;
       s.time_start = start;
       s.time_increment = inc;

@@ -8,29 +8,23 @@
 // composes the correction into base_in_odom_ (:397-413), writes the published odometry (:472-492) and decides the key
 // frame (:498-517).  Promoting a scan swaps the two slots' pointers; nothing is copied in shared memory.
 //
-// tf2 LinearMath is followed operation by operation (Transform product and inverse, Matrix3x3::setRotation /
-// getRotation, Quaternion::setRPY, tf2::getYaw), in double with no FMA contraction (-fmad=false); only the device's
-// sin / cos / atan2 / sqrt may differ from glibc's in the last place.  The state between calls lives in device memory
+// tf2 LinearMath and ros::Duration are ros_math.cuh's, in double with no FMA contraction (-fmad=false); only the
+// device's sin / cos / atan2 / sqrt may differ from glibc's in the last place.  The state between calls lives in device memory
 // (PlicpOdomState, the key frame's float32 ranges), so calls over consecutive parts of a recording equal one call.
 #include <cmath>
 #include <vector>
 
 #include "common.cuh"
 #include "plicp_pair.cuh"
+#include "ros_math.cuh"
 
 using namespace b2s;
 
 namespace b2s {
 
-// tf2::Transform: 3x3 basis (rows) and origin
-struct Tf {
-  double m[3][3];
-  double o[3];
-};
-
 // per-recording state of the node between scans
 struct PlicpOdomState {
-  Tf base_in_odom, base_in_odom_keyframe;
+  TfTransform base_in_odom, base_in_odom_keyframe;
   double velocity_linear_x, velocity_angular_z;  // latest_velocity_ (the node sets no other field)
   uint32_t last_sec, last_nsec;                   // last_icp_time_
   int32_t scan_count;                             // scan_count_
@@ -39,92 +33,17 @@ struct PlicpOdomState {
   int32_t reserved;
 };
 
-__device__ inline void tf_identity(Tf &t) {
-  for (int i = 0; i < 3; i++) {
-    for (int j = 0; j < 3; j++) t.m[i][j] = i == j ? 1.0 : 0.0;
-    t.o[i] = 0.0;
-  }
-}
-
-// Transform::operator* : (basis1 * basis2, transform1(origin2)); Matrix3x3 product via tdotx/y/z, Vector3::dot3
-__device__ inline Tf tf_mul(const Tf &a, const Tf &b) {
-  Tf c;
-  for (int i = 0; i < 3; i++) {
-    for (int j = 0; j < 3; j++) c.m[i][j] = b.m[0][j] * a.m[i][0] + b.m[1][j] * a.m[i][1] + b.m[2][j] * a.m[i][2];
-    c.o[i] = (b.o[0] * a.m[i][0] + b.o[1] * a.m[i][1] + b.o[2] * a.m[i][2]) + a.o[i];
-  }
-  return c;
-}
-
-// Transform::inverse : (basis^T, basis^T * -origin)
-__device__ inline Tf tf_inverse(const Tf &a) {
-  Tf c;
-  for (int i = 0; i < 3; i++)
-    for (int j = 0; j < 3; j++) c.m[i][j] = a.m[j][i];
-  const double no[3] = {-a.o[0], -a.o[1], -a.o[2]};
-  for (int i = 0; i < 3; i++) c.o[i] = c.m[i][0] * no[0] + c.m[i][1] * no[1] + c.m[i][2] * no[2];
-  return c;
-}
-
-// Matrix3x3::setRotation(q), q = (x, y, z, w)
-__device__ inline void tf_set_rotation(Tf &t, const double q[4]) {
-  const double d = q[0] * q[0] + q[1] * q[1] + q[2] * q[2] + q[3] * q[3];
-  const double s = 2.0 / d;
-  const double xs = q[0] * s, ys = q[1] * s, zs = q[2] * s;
-  const double wx = q[3] * xs, wy = q[3] * ys, wz = q[3] * zs;
-  const double xx = q[0] * xs, xy = q[0] * ys, xz = q[0] * zs;
-  const double yy = q[1] * ys, yz = q[1] * zs, zz = q[2] * zs;
-  t.m[0][0] = 1.0 - (yy + zz); t.m[0][1] = xy - wz; t.m[0][2] = xz + wy;
-  t.m[1][0] = xy + wz; t.m[1][1] = 1.0 - (xx + zz); t.m[1][2] = yz - wx;
-  t.m[2][0] = xz - wy; t.m[2][1] = yz + wx; t.m[2][2] = 1.0 - (xx + yy);
-}
-
-// Matrix3x3::getRotation(q)
-__device__ inline void tf_get_rotation(const Tf &t, double q[4]) {
-  const double trace = t.m[0][0] + t.m[1][1] + t.m[2][2];
-  if (trace > 0.0) {
-    double s = sqrt(trace + 1.0);
-    q[3] = s * 0.5;
-    s = 0.5 / s;
-    q[0] = (t.m[2][1] - t.m[1][2]) * s;
-    q[1] = (t.m[0][2] - t.m[2][0]) * s;
-    q[2] = (t.m[1][0] - t.m[0][1]) * s;
-  } else {
-    const int i = t.m[0][0] < t.m[1][1] ? (t.m[1][1] < t.m[2][2] ? 2 : 1) : (t.m[0][0] < t.m[2][2] ? 2 : 0);
-    const int j = (i + 1) % 3, k = (i + 2) % 3;
-    double s = sqrt(t.m[i][i] - t.m[j][j] - t.m[k][k] + 1.0);
-    q[i] = s * 0.5;
-    s = 0.5 / s;
-    q[3] = (t.m[k][j] - t.m[j][k]) * s;
-    q[j] = (t.m[j][i] + t.m[i][j]) * s;
-    q[k] = (t.m[k][i] + t.m[i][k]) * s;
-  }
-}
-
-// tf2::getYaw(q) = the yaw of tf2::getEulerYPR (tf2/utils.h)
-__device__ inline double tf_get_yaw(const double q[4]) {
-  const double x = q[0], y = q[1], z = q[2], w = q[3];
-  const double sqx = x * x, sqy = y * y, sqz = z * z, sqw = w * w;
-  const double sarg = -2 * (x * z - w * y) / (sqx + sqy + sqz + sqw);
-  if (sarg <= -0.99999) return -2 * atan2(y, x);
-  if (sarg >= 0.99999) return 2 * atan2(y, x);
-  return atan2(2 * (x * y + w * z), sqw + sqx - sqy - sqz);
-}
-
-__device__ inline double tf_yaw_of(const Tf &t) {
+__device__ inline double tf_yaw_of(const TfTransform &t) {
   double q[4];
   tf_get_rotation(t, q);
-  return tf_get_yaw(q);
+  return tf2_get_yaw(q);
 }
 
 // ScanMatchPLICP::CreateTfFromXYTheta (:461-467): origin (x, y, 0), rotation Quaternion::setRPY(0, 0, theta)
-__device__ inline Tf tf_from_xyt(double x, double y, double theta) {
-  const double roll = 0.0, pitch = 0.0;
-  const double hy = theta * 0.5, hp = pitch * 0.5, hr = roll * 0.5;
-  const double cy = cos(hy), sy = sin(hy), cp = cos(hp), sp = sin(hp), cr = cos(hr), sr = sin(hr);
-  const double q[4] = {sr * cp * cy - cr * sp * sy, cr * sp * cy + sr * cp * sy, cr * cp * sy - sr * sp * cy,
-                       cr * cp * cy + sr * sp * sy};
-  Tf t;
+__device__ inline TfTransform tf_from_xyt(double x, double y, double theta) {
+  double q[4];
+  quat_set_rpy(0.0, 0.0, theta, q);
+  TfTransform t;
   t.o[0] = x; t.o[1] = y; t.o[2] = 0.0;
   tf_set_rotation(t, q);
   return t;
@@ -168,7 +87,7 @@ __global__ void __launch_bounds__(ICP_THREADS) k_plicp_odometry(OdomLaunch A) {
   float *kf_store = A.keyframe_ranges + (size_t)b * n;
   int seen = A.state[b].scans_seen;  // every thread tracks it; only thread 0 touches the rest of the state
   PlicpOdomState st;
-  Tf base_to_laser, laser_to_base;
+  TfTransform base_to_laser, laser_to_base;
   if (tid == 0) {
     st = A.state[b];
     // GetBaseToLaserTf (:257-280): tf2::fromMsg(transform, base_to_laser_), laser_to_base_ = its inverse
@@ -212,18 +131,14 @@ __global__ void __launch_bounds__(ICP_THREADS) k_plicp_odometry(OdomLaunch A) {
       icp_load_point(r[i], beam_theta(A.angle_min, A.angle_increment, i), rmin, rmax, cx, cy, cv, i);
     double guess[3] = {0.0, 0.0, 0.0}, dt = 0.0;
     if (tid == 0) {
-      // dt = (time - last_icp_time_).toSec(): ros::Duration of the (sec, nsec) differences, normalised
-      long long dsec = (long long)(int32_t)stamp[0] - (int32_t)st.last_sec;
-      long long dnsec = (long long)(int32_t)stamp[1] - (int32_t)st.last_nsec;
-      long long nsec_part = dnsec % 1000000000LL, sec_part = dsec + dnsec / 1000000000LL;
-      if (nsec_part < 0) { nsec_part += 1000000000LL; --sec_part; }
-      dt = (double)(int32_t)sec_part + 1e-9 * (double)(int32_t)nsec_part;
+      // dt = (time - last_icp_time_).toSec()
+      dt = ros_duration_to_sec(ros_time_diff(stamp[0], stamp[1], st.last_sec, st.last_nsec));
       // GetPrediction (:442-456): only linear.x is ever set; linear.y and linear.z (the angle) are 0
       const double pr_x = st.velocity_linear_x < 1e-6 ? 0.0 : dt * st.velocity_linear_x;
       const double pr_y = 0.0, pr_a = 0.0;
-      Tf pc = tf_from_xyt(pr_x, pr_y, pr_a);
+      TfTransform pc = tf_from_xyt(pr_x, pr_y, pr_a);
       pc = tf_mul(pc, tf_mul(st.base_in_odom, tf_inverse(st.base_in_odom_keyframe)));
-      const Tf pcl = tf_mul(tf_mul(tf_mul(tf_mul(laser_to_base, tf_inverse(st.base_in_odom)), pc), st.base_in_odom),
+      const TfTransform pcl = tf_mul(tf_mul(tf_mul(tf_mul(laser_to_base, tf_inverse(st.base_in_odom)), pc), st.base_in_odom),
                             base_to_laser);
       guess[0] = pcl.o[0];
       guess[1] = pcl.o[1];
@@ -233,10 +148,10 @@ __global__ void __launch_bounds__(ICP_THREADS) k_plicp_odometry(OdomLaunch A) {
     S.rx = kx; S.ry = ky; S.rv = kv; S.sx = cx; S.sy = cy; S.sv = cv;
     icp_pair(A.P.icp, n, min_theta, max_theta, S, guess, &res);
     if (tid == 0) {
-      Tf corr;
+      TfTransform corr;
       tf_identity(corr);  // a failed match leaves corr_ch default-constructed: taken as the identity (DESIGN.md §7)
       if (res.valid) {
-        const Tf corr_l = tf_from_xyt(res.x[0], res.x[1], res.x[2]);
+        const TfTransform corr_l = tf_from_xyt(res.x[0], res.x[1], res.x[2]);
         corr = tf_mul(tf_mul(base_to_laser, corr_l), laser_to_base);
         st.base_in_odom = tf_mul(st.base_in_odom_keyframe, corr);
         st.velocity_linear_x = corr.o[0] / dt;

@@ -542,8 +542,8 @@ b2s_status b2s_ros_karto_readings(const b2s_laser_scan_msg *scan, int inverted, 
  * oracle/karto_node_port.py to the unmodified node; tests/test_gpu_karto_node.py pins this handle to the restatement.
  * The tf arithmetic is tf's LinearMath in double, operation by operation (Transform product and inverse, Matrix3x3
  * setRotation / getRotation, Quaternion setRPY, getYaw through getRPY); ros::Time / Duration are roscpp's integer
- * arithmetic.  Neither tf nor roscpp is in the reference tree, so those lines are pinned to the stand-ins under
- * oracle/shim_lesson6/ (DESIGN.md §7). */
+ * arithmetic.  Neither tf nor roscpp is in the reference tree; the library's one definition of them (csrc/ros_math.cuh)
+ * is held bit for bit to the node's stand-ins under oracle/shim/ by tests/test_ros_math.py (DESIGN.md §7). */
 typedef struct b2s_karto_node_params {
   int32_t throttle_scans;     /* [1] a scan is processed when the count of scans handed in so far divides by it */
   int32_t reserved;           /* 0 */

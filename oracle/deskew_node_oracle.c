@@ -3,8 +3,8 @@
  * CorrectLaserScan (:339-393) and ResetParameters (:60-79), with the node's members as state.  Built on the per-scan
  * restatements of deskew_oracle.c (orc_deskew_integrate_imu, orc_deskew_odom_increment, orc_deskew_scan), linked into a
  * library of its own (oracle/deskew_node_port.py).  Pinned to the unmodified node by tests/test_deskew_node_reference.py
- * except tf's quaternionMsgToTF and Matrix3x3::getRPY, which are restated here as the node's stand-in
- * (oracle/shim/tf/LinearMath/Matrix3x3.h) restates them: tf is not in the reference tree.
+ * except tf's quaternionMsgToTF and Matrix3x3::getRPY, which are linear_math.h's, as the node's stand-in
+ * (oracle/shim/tf2/LinearMath/Transform.h) restates them: tf is not in the reference tree.
  *
  * The node's AsyncSpinner runs the IMU, odometry and scan callbacks under separate locks, so what a scan callback sees
  * is the number of messages of each log delivered before it (imu_arrived / odom_arrived). */
@@ -12,6 +12,8 @@
 #include <stdint.h>
 #include <stdlib.h>
 #include <string.h>
+
+#include "linear_math.h"
 
 typedef struct {
   double time_start, time_increment;
@@ -40,41 +42,15 @@ void orc_deskew_scan(int n_beams, const float *ranges, double angle_min, double 
 enum { PUBLISHED = 0, HELD = 1, WAIT_IMU = 2, IMU_EMPTY = 3, WAIT_ODOM = 4, ODOM_EMPTY = 5, UNDEFINED = 6 };
 #define QUEUE_LENGTH 2000 /* queueLength (:20) */
 
-static double to_sec(uint32_t sec, uint32_t nsec) { return (double)sec + 1e-9 * (double)nsec; } /* ros::Time::toSec */
-
-/* tf::quaternionMsgToTF, then tf::Matrix3x3(q) (setRotation) and getRPY (getEulerYPR, solution 1) */
-static void get_rpy(const double q[4], double *roll, double *pitch, double *yaw) {
-  const double d = q[0] * q[0] + q[1] * q[1] + q[2] * q[2] + q[3] * q[3], s = 2.0 / d;
-  const double xs = q[0] * s, ys = q[1] * s, zs = q[2] * s;
-  const double wx = q[3] * xs, wy = q[3] * ys, wz = q[3] * zs;
-  const double xx = q[0] * xs, xy = q[0] * ys, xz = q[0] * zs;
-  const double yy = q[1] * ys, yz = q[1] * zs, zz = q[2] * zs;
-  const double m[3][3] = {{1.0 - (yy + zz), xy - wz, xz + wy}, {xy + wz, 1.0 - (xx + zz), yz - wx}, {xz - wy, yz + wx, 1.0 - (xx + yy)}};
-  if (fabs(m[2][0]) >= 1) {
-    *yaw = 0;
-    const double delta = atan2(m[0][1], m[0][2]);
-    if (m[2][0] > 0) {
-      *pitch = -M_PI / 2;
-      *roll = -*yaw + atan2(-m[0][1], -m[0][2]);
-    } else {
-      *pitch = M_PI / 2;
-      *roll = *yaw + delta;
-    }
-    return;
-  }
-  *pitch = -asin(m[2][0]);
-  const double c = cos(*pitch);
-  *roll = atan2(m[2][1] / c, m[2][2] / c);
-  *yaw = atan2(m[1][0] / c, m[0][0] / c);
-}
-
 static void pose_of(const orc_odom_msg *m, double out[6]) {
   static const orc_odom_msg none; /* nav_msgs::Odometry(): stamp 0, position 0, quaternion (0, 0, 0, 0) */
   if (!m) m = &none;
   out[0] = m->position[0];
   out[1] = m->position[1];
   out[2] = m->position[2];
-  get_rpy(m->orientation, &out[3], &out[4], &out[5]);
+  orc_tf t; /* tf::quaternionMsgToTF, then tf::Matrix3x3(q).getRPY */
+  tf_set_rotation(&t, m->orientation);
+  tf_get_rpy(&t, &out[3], &out[4], &out[5]);
 }
 
 /* One recording through the node.  Per scan j: out_status[j]; out_state[j] (zero unless published or undefined);
@@ -96,10 +72,10 @@ int orc_deskew_node(int use_imu, int use_odom, float angle_min, float angle_incr
   double *mt = tab, *mx = tab + QUEUE_LENGTH, *my = tab + 2 * QUEUE_LENGTH, *mz = tab + 3 * QUEUE_LENGTH;
   double *st = tab + 4 * QUEUE_LENGTH, *sx = st + QUEUE_LENGTH, *sy = st + 2 * QUEUE_LENGTH, *sz = st + 3 * QUEUE_LENGTH;
   for (int i = 0; i < n_imu; i++) {
-    imu_t[i] = to_sec(imu[i].sec, imu[i].nsec);
+    imu_t[i] = ros_time_to_sec(imu[i].sec, imu[i].nsec);
     memcpy(imu_w + 3 * i, imu[i].angular_velocity, sizeof(double) * 3);
   }
-  for (int i = 0; i < n_odom; i++) odom_t[i] = to_sec(odom[i].sec, odom[i].nsec);
+  for (int i = 0; i < n_odom; i++) odom_t[i] = ros_time_to_sec(odom[i].sec, odom[i].nsec);
   const double scan_count = (double)n_beams;
   int ilo = 0, olo = 0, start_msg = -1, end_msg = -1;
   memset(out_xyz, 0, sizeof(float) * 3 * (size_t)n_beams * (size_t)n_scans);
@@ -114,7 +90,7 @@ int orc_deskew_node(int use_imu, int use_odom, float angle_min, float angle_incr
       goto done;
     }
     const orc_node_scan *sc = &scans[j], *next = &scans[j + 1];
-    const double start = to_sec(sc->sec, sc->nsec), inc = sc->time_increment, end = start + inc * (scan_count - 1);
+    const double start = ros_time_to_sec(sc->sec, sc->nsec), inc = sc->time_increment, end = start + inc * (scan_count - 1);
     s.time_start = start;
     s.time_increment = inc;
     s.range_min = sc->range_min;

@@ -16,6 +16,7 @@ deskew = importlib.import_module("creating-2d-laser-slam-from-scratch_b200.deske
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 _SRC = [os.path.join(_HERE, f) for f in ("deskew_node_oracle.c", "deskew_oracle.c")]
+_HDR = os.path.join(_HERE, "linear_math.h")
 _LIB = os.path.join(_HERE, "libdeskew_node_oracle.so")
 # the flags of oracle/Makefile: x86-64 baseline, no FMA contraction
 CFLAGS = ["-O2", "-fPIC", "-std=c11", "-ffp-contract=off", "-Wall", "-Wextra", "-D_DEFAULT_SOURCE"]
@@ -24,7 +25,7 @@ _lib = None
 
 
 def build(force: bool = False) -> str:
-    deps = _SRC + [os.path.abspath(__file__)]
+    deps = _SRC + [_HDR, os.path.abspath(__file__)]
     if force or not os.path.exists(_LIB) or any(os.path.getmtime(d) > os.path.getmtime(_LIB) for d in deps):
         tmp = _LIB + f".{os.getpid()}.tmp"
         subprocess.check_call([os.environ.get("CC", "gcc")] + CFLAGS + ["-shared"] + _SRC + ["-o", tmp, "-lm"])

@@ -11,84 +11,24 @@
 #include <string.h>
 
 #include "../include/b200slam.h"
+#include "linear_math.h"
 
 int orc_plicp_match(const b2s_icp_params *P, int n, const double *ref_r, const double *sens_r, const double *theta,
                     double range_min, double range_max, const double first_guess[3], b2s_icp_result *out);
 
-/* The node's loop for ONE recording from a fresh node, in C around orc_plicp_match.  tf2's LinearMath (Transform product
- * and inverse, Matrix3x3::setRotation / getRotation, Quaternion::setRPY) and tf2::getYaw are restated from geometry2,
- * operation by operation, in double without FMA contraction.  After a failed match the node tests NewKeyframeNeeded on a
+/* The node's loop for ONE recording from a fresh node, in C around orc_plicp_match.  tf2's LinearMath and ros::Duration
+ * are linear_math.h's, in double without FMA contraction.  After a failed match the node tests NewKeyframeNeeded on a
  * default-constructed (uninitialised) tf2::Transform; here it is the identity (DESIGN.md §7).  The unmodified node,
  * compiled against the stand-ins under oracle/shim/ (oracle/ref_lesson3.cpp), pins this restatement bit for bit. */
-typedef struct { double m[3][3], o[3]; } orc_tf;
-
-static void tf_identity(orc_tf *t) {
-  for (int i = 0; i < 3; i++) {
-    for (int j = 0; j < 3; j++) t->m[i][j] = i == j ? 1.0 : 0.0;
-    t->o[i] = 0.0;
-  }
-}
-static orc_tf tf_mul(const orc_tf *a, const orc_tf *b) {
-  orc_tf c;
-  for (int i = 0; i < 3; i++) {
-    for (int j = 0; j < 3; j++) c.m[i][j] = b->m[0][j] * a->m[i][0] + b->m[1][j] * a->m[i][1] + b->m[2][j] * a->m[i][2];
-    c.o[i] = (b->o[0] * a->m[i][0] + b->o[1] * a->m[i][1] + b->o[2] * a->m[i][2]) + a->o[i];
-  }
-  return c;
-}
-static orc_tf tf_inverse(const orc_tf *a) {
-  orc_tf c;
-  for (int i = 0; i < 3; i++)
-    for (int j = 0; j < 3; j++) c.m[i][j] = a->m[j][i];
-  const double no[3] = {-a->o[0], -a->o[1], -a->o[2]};
-  for (int i = 0; i < 3; i++) c.o[i] = c.m[i][0] * no[0] + c.m[i][1] * no[1] + c.m[i][2] * no[2];
-  return c;
-}
-static void tf_set_rotation(orc_tf *t, const double q[4]) {
-  const double d = q[0] * q[0] + q[1] * q[1] + q[2] * q[2] + q[3] * q[3], s = 2.0 / d;
-  const double xs = q[0] * s, ys = q[1] * s, zs = q[2] * s;
-  const double wx = q[3] * xs, wy = q[3] * ys, wz = q[3] * zs;
-  const double xx = q[0] * xs, xy = q[0] * ys, xz = q[0] * zs;
-  const double yy = q[1] * ys, yz = q[1] * zs, zz = q[2] * zs;
-  t->m[0][0] = 1.0 - (yy + zz); t->m[0][1] = xy - wz; t->m[0][2] = xz + wy;
-  t->m[1][0] = xy + wz; t->m[1][1] = 1.0 - (xx + zz); t->m[1][2] = yz - wx;
-  t->m[2][0] = xz - wy; t->m[2][1] = yz + wx; t->m[2][2] = 1.0 - (xx + yy);
-}
-static void tf_get_rotation(const orc_tf *t, double q[4]) {
-  const double trace = t->m[0][0] + t->m[1][1] + t->m[2][2];
-  if (trace > 0.0) {
-    double s = sqrt(trace + 1.0);
-    q[3] = s * 0.5;
-    s = 0.5 / s;
-    q[0] = (t->m[2][1] - t->m[1][2]) * s;
-    q[1] = (t->m[0][2] - t->m[2][0]) * s;
-    q[2] = (t->m[1][0] - t->m[0][1]) * s;
-  } else {
-    const int i = t->m[0][0] < t->m[1][1] ? (t->m[1][1] < t->m[2][2] ? 2 : 1) : (t->m[0][0] < t->m[2][2] ? 2 : 0);
-    const int j = (i + 1) % 3, k = (i + 2) % 3;
-    double s = sqrt(t->m[i][i] - t->m[j][j] - t->m[k][k] + 1.0);
-    q[i] = s * 0.5;
-    s = 0.5 / s;
-    q[3] = (t->m[k][j] - t->m[j][k]) * s;
-    q[j] = (t->m[j][i] + t->m[i][j]) * s;
-    q[k] = (t->m[k][i] + t->m[i][k]) * s;
-  }
-}
 static double tf_yaw_of(const orc_tf *t) {
   double q[4];
   tf_get_rotation(t, q);
-  const double x = q[0], y = q[1], z = q[2], w = q[3];
-  const double sqx = x * x, sqy = y * y, sqz = z * z, sqw = w * w;
-  const double sarg = -2 * (x * z - w * y) / (sqx + sqy + sqz + sqw);
-  if (sarg <= -0.99999) return -2 * atan2(y, x);
-  if (sarg >= 0.99999) return 2 * atan2(y, x);
-  return atan2(2 * (x * y + w * z), sqw + sqx - sqy - sqz);
+  return tf2_get_yaw(q);
 }
+/* ScanMatchPLICP::CreateTfFromXYTheta: origin (x, y, 0), rotation Quaternion::setRPY(0, 0, theta) */
 static orc_tf tf_from_xyt(double x, double y, double theta) {
-  const double hy = theta * 0.5, hp = 0.0 * 0.5, hr = 0.0 * 0.5;
-  const double cy = cos(hy), sy = sin(hy), cp = cos(hp), sp = sin(hp), cr = cos(hr), sr = sin(hr);
-  const double q[4] = {sr * cp * cy - cr * sp * sy, cr * sp * cy + sr * cp * sy, cr * cp * sy - sr * sp * cy,
-                       cr * cp * cy + sr * sp * sy};
+  double q[4];
+  quat_set_rpy(0.0, 0.0, theta, q);
   orc_tf t;
   t.o[0] = x; t.o[1] = y; t.o[2] = 0.0;
   tf_set_rotation(&t, q);
@@ -121,12 +61,7 @@ void orc_plicp_odometry(const b2s_plicp_odom_params *P, int n, float angle_min, 
       continue;
     }
     for (int i = 0; i < n; i++) cur[i] = r[i];
-    /* ros::Time difference, ros::Duration normalisation, toSec() */
-    long long dsec = (long long)(int32_t)stamps[2 * s] - (int32_t)last_sec;
-    long long dnsec = (long long)(int32_t)stamps[2 * s + 1] - (int32_t)last_nsec;
-    long long nsec_part = dnsec % 1000000000LL, sec_part = dsec + dnsec / 1000000000LL;
-    if (nsec_part < 0) { nsec_part += 1000000000LL; --sec_part; }
-    const double dt = (double)(int32_t)sec_part + 1e-9 * (double)(int32_t)nsec_part;
+    const double dt = ros_duration_to_sec(ros_time_diff(stamps[2 * s], stamps[2 * s + 1], last_sec, last_nsec));
     const double pr_x = vx < 1e-6 ? 0.0 : dt * vx;
     orc_tf pc = tf_from_xyt(pr_x, 0.0, 0.0);
     orc_tf kfi = tf_inverse(&bio_kf), rel = tf_mul(&bio, &kfi);

@@ -25,7 +25,7 @@ _lib = None
 
 
 def build(force: bool = False) -> str:
-    deps = _SRC + [_HDR, os.path.abspath(__file__)]
+    deps = _SRC + [_HDR, os.path.join(_HERE, "linear_math.h"), os.path.abspath(__file__)]
     if force or not os.path.exists(_LIB) or any(os.path.getmtime(d) > os.path.getmtime(_LIB) for d in deps):
         tmp = _LIB + f".{os.getpid()}.tmp"
         subprocess.check_call([os.environ.get("CC", "gcc")] + CFLAGS + ["-shared"] + _SRC + ["-o", tmp, "-lm"])

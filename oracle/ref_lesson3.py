@@ -1,7 +1,6 @@
 """TEST INFRASTRUCTURE — ctypes binding of oracle/_ref/liblesson3_ref.so: the UNMODIFIED lesson3 odometry node,
 reference/lesson3/src/plicp_odometry.cc, compiled where it lies against the ROS, tf2 and CSM stand-ins under oracle/shim/
-(with oracle/shim_lesson3/ros/ros.h in place of shim/ros/ros.h) by oracle/ref_lesson3.cpp, with sm_icp answered by
-oracle/plicp_oracle.c.  `build(ref)` makes the library from a
+by oracle/ref_lesson3.cpp, with sm_icp answered by oracle/plicp_oracle.c.  `build(ref)` makes the library from a
 checkout of the original project; where it is absent the tests replay its recorded answers (tests/reference_record.py).
 Only tests/ and __graft_entry__ may import this module.
 """
@@ -20,7 +19,7 @@ _PATH = os.path.join(_HERE, "_ref", "liblesson3_ref.so")
 # the flags of oracle/Makefile's builds: x86-64 baseline, no -march, no FMA contraction
 CXXFLAGS = ["-std=c++17", "-O2", "-fPIC", "-w", "-ffp-contract=off"]
 CFLAGS = ["-std=c11", "-O2", "-fPIC", "-w", "-ffp-contract=off"]
-_SHIM = ["../shim_lesson3/ros/ros.h", "sensor_msgs/LaserScan.h", "nav_msgs/Odometry.h", "geometry_msgs/messages.h",
+_SHIM = ["ros/ros.h", "sensor_msgs/LaserScan.h", "nav_msgs/Odometry.h", "geometry_msgs/messages.h",
          "geometry_msgs/TransformStamped.h", "geometry_msgs/TwistStamped.h", "tf2/LinearMath/Transform.h", "tf2/utils.h",
          "tf2_ros/transform_listener.h", "tf2_ros/transform_broadcaster.h", "tf2_geometry_msgs/tf2_geometry_msgs.h",
          "csm/csm_all.h"]
@@ -38,7 +37,7 @@ def build(ref: str) -> str:
         obj = tmp + ".o"
         subprocess.check_call([os.environ.get("CC", "gcc")] + CFLAGS + ["-c", orc, "-o", obj])
         subprocess.check_call([os.environ.get("CXX", "g++")] + CXXFLAGS +
-                              ["-shared", "-I" + os.path.join(_HERE, "shim_lesson3"), "-I" + os.path.join(_HERE, "shim"),
+                              ["-shared", "-I" + os.path.join(_HERE, "shim"),
                                "-I" + os.path.abspath(ref),
                                "-I" + os.path.join(os.path.abspath(ref), "lesson3", "include"), drv, obj, "-o", tmp,
                                "-lm"])

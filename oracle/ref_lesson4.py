@@ -1,6 +1,6 @@
 """TEST INFRASTRUCTURE — ctypes binding of oracle/_ref/liblesson4_ref.so: lesson4's UNMODIFIED make-map nodes,
 reference/lesson4/src/gmapping/gmapping.cc and reference/lesson4/src/hector_mapping/hector_mapping.cc, compiled where
-they lie against the ROS stand-in under oracle/shim_lesson4/ and the message and Eigen stand-ins under oracle/shim/ by
+they lie against the ROS, message and Eigen stand-ins under oracle/shim/ by
 oracle/ref_lesson4_gmapping.cpp and oracle/ref_lesson4_hector.cpp (two translation units: see the latter).
 `build(ref)` makes the library from a checkout of the original project; where it is absent the tests replay its
 recorded answers (tests/reference_record.py).  Only tests/ and __graft_entry__ may import this module.
@@ -18,7 +18,7 @@ _PATH = os.path.join(_HERE, "_ref", "liblesson4_ref.so")
 # the flags of oracle/Makefile's reference builds: x86-64 baseline, no -march, no FMA contraction
 CXXFLAGS = ["-std=c++17", "-O2", "-fPIC", "-w", "-ffp-contract=off"]
 _DRIVERS = ["ref_lesson4_gmapping.cpp", "ref_lesson4_hector.cpp"]
-_SHIM = ["../shim_lesson4/ros/ros.h", "sensor_msgs/LaserScan.h", "nav_msgs/OccupancyGrid.h", "nav_msgs/MapMetaData.h",
+_SHIM = ["ros/ros.h", "sensor_msgs/LaserScan.h", "nav_msgs/OccupancyGrid.h", "nav_msgs/MapMetaData.h",
          "geometry_msgs/messages.h", "Eigen/mini_eigen.h"]
 SENTINEL = 0x55  # ref_lesson4_gmapping.cpp: a byte behind the map the node did not write
 _lib = None
@@ -31,7 +31,7 @@ def build(ref: str) -> str:
     if not os.path.exists(_PATH) or any(os.path.getmtime(d) > os.path.getmtime(_PATH) for d in deps):
         os.makedirs(os.path.dirname(_PATH), exist_ok=True)
         tmp = _PATH + f".{os.getpid()}.tmp"
-        inc = ["-I" + os.path.join(_HERE, "shim_lesson4"), "-I" + os.path.join(_HERE, "shim"), "-I" + os.path.abspath(ref),
+        inc = ["-I" + os.path.join(_HERE, "shim"), "-I" + os.path.abspath(ref),
                "-I" + os.path.join(l4, "include"), "-I" + os.path.join(l4, "include", "lesson4", "hector_mapping")]
         objs = []
         for d in _DRIVERS:

@@ -2,8 +2,7 @@
  * ref_lesson4_gmapping.cpp — TEST INFRASTRUCTURE, NOT PRODUCT CODE.
  * extern "C" driver around the UNMODIFIED lesson4 GMapping make-map node, reference/lesson4/src/gmapping/gmapping.cc,
  * #included where it lies (oracle/ref_lesson4.py builds it into _ref/liblesson4_ref.so).  ROS is absent; the stand-ins
- * under oracle/shim_lesson4/ (its ROS core, first on the include path) and oracle/shim/ (LaserScan, OccupancyGrid,
- * MapMetaData with a float32 resolution) provide the message types, the private node handle and its parameters.  The
+ * under oracle/shim/ (the ROS core, LaserScan, OccupancyGrid, MapMetaData with a float32 resolution) provide the message types, the private node handle and its parameters.  The
  * node's main() is renamed so the library has none; every line of ScanCallback that runs here is the reference's.
  *
  * At its defaults the node's PublishMap writes past the end of map_.data (MAP_IDX(1599, x, y) for x, y < 1600 on a

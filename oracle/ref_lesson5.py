@@ -18,7 +18,8 @@ _PATH = os.path.join(_HERE, "_ref", "liblesson5_ref.so")
 CXXFLAGS = ["-std=c++17", "-O2", "-fPIC", "-w", "-ffp-contract=off"]
 QUEUE_LENGTH = 2000  # the node's imu table length (lidar_undistortion.cc:20)
 _SHIM = ["ros/ros.h", "sensor_msgs/LaserScan.h", "sensor_msgs/Imu.h", "sensor_msgs/PointCloud2.h", "nav_msgs/Odometry.h",
-         "geometry_msgs/messages.h", "tf/LinearMath/Quaternion.h", "tf/LinearMath/Matrix3x3.h", "tf/transform_datatypes.h",
+         "geometry_msgs/messages.h", "tf2/LinearMath/Transform.h", "tf/LinearMath/Quaternion.h", "tf/LinearMath/Matrix3x3.h",
+         "tf/transform_datatypes.h",
          "pcl/point_types.h", "pcl/point_cloud.h", "pcl/common/common.h", "pcl/common/transforms.h",
          "pcl_ros/point_cloud.h", "pcl_conversions/pcl_conversions.h", "Eigen/mini_eigen.h"]
 _lib = None

@@ -19,10 +19,11 @@ _ROOT = os.path.dirname(_HERE)
 _PATH = os.path.join(_HERE, "_ref", "liblesson6_ref.so")
 # the flags of the other reference builds: x86-64 baseline, no -march, no FMA contraction
 CXXFLAGS = ["-std=c++17", "-O2", "-fPIC", "-w", "-ffp-contract=off"]
-_SHIM6 = ["ros/ros.h", "ros/console.h", "boost/thread.hpp", "message_filters/subscriber.h", "tf/tf_core.h",
+_SHIM6 = ["boost/thread.hpp", "message_filters/subscriber.h", "tf/tf_core.h",
           "tf/transform_listener.h", "tf/transform_broadcaster.h", "tf/message_filter.h", "visualization_msgs/MarkerArray.h",
           "nav_msgs/GetMap.h"]
-_SHIM = ["boost/thread.hpp", "tf2/LinearMath/Transform.h", "sensor_msgs/LaserScan.h", "nav_msgs/OccupancyGrid.h",
+_SHIM = ["ros/ros.h", "ros/console.h", "boost/thread.hpp", "tf2/LinearMath/Transform.h", "tf/LinearMath/Quaternion.h",
+         "tf/LinearMath/Matrix3x3.h", "sensor_msgs/LaserScan.h", "nav_msgs/OccupancyGrid.h",
          "nav_msgs/MapMetaData.h", "geometry_msgs/messages.h"]
 MAP_FN = C.CFUNCTYPE(None, C.c_void_p, C.c_int32, C.c_int32, C.c_float, C.c_double, C.c_double, C.POINTER(C.c_int8))
 _lib = None

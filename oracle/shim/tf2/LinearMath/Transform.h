@@ -1,8 +1,11 @@
 // TEST INFRASTRUCTURE — tf2's LinearMath (geometry2: tf2/LinearMath/{Vector3,Quaternion,Matrix3x3,Transform}.h) as far as
-// lesson3's plicp_odometry.cc uses it, for compiling the node unmodified (oracle/ref_lesson3.cpp).  Every operation is
-// restated from geometry2's code, operation by operation in double (the driver is built without FMA contraction):
-// Matrix3x3 product through tdotx / tdoty / tdotz, Transform product (basis product, origin through dot3 + origin),
-// inverse (transpose, transpose * -origin), setRotation / getRotation and Quaternion::setRPY.
+// the unmodified nodes use it: lesson3's plicp_odometry.cc (oracle/ref_lesson3.cpp), and through tf's names
+// (tf/LinearMath/*.h, tf/tf_core.h) lesson5's lidar_undistortion.cc and lesson6's karto_slam.cc; tf's LinearMath is the
+// same Bullet code.  Every operation is restated from geometry2's code, operation by operation in double (the drivers
+// are built without FMA contraction): Matrix3x3 product through tdotx / tdoty / tdotz, Transform product (basis
+// product, origin through dot3 + origin), inverse (transpose, transpose * -origin), setRotation / getRotation, getRPY
+// and Quaternion::setRPY.  The library states the same arithmetic in csrc/ros_math.cuh; tests/ros_math_check.cpp holds
+// the two equal.
 //
 // One deliberate difference: tf2 leaves a default-constructed Transform uninitialised, and the node reads one
 // (plicp_odometry.cc:397, 423: corr_ch after a failed match).  Here the default constructor builds the IDENTITY, the
@@ -60,6 +63,7 @@ struct Quaternion {
 struct Matrix3x3 {
   Vector3 el[3];
   Matrix3x3() = default;
+  explicit Matrix3x3(const Quaternion &q) { setRotation(q); }
   Matrix3x3(double xx, double xy, double xz, double yx, double yy, double yz, double zx, double zy, double zz)
       : el{Vector3(xx, xy, xz), Vector3(yx, yy, yz), Vector3(zx, zy, zz)} {}
   const Vector3 &operator[](int i) const { return el[i]; }
@@ -102,6 +106,26 @@ struct Matrix3x3 {
       temp[k] = (el[k][i] + el[i][k]) * s;
     }
     q.setValue(temp[0], temp[1], temp[2], temp[3]);
+  }
+  // getEulerYPR, solution 1: R = Rz(yaw) Ry(pitch) Rx(roll); at the pitch singularity yaw is 0 and roll takes the
+  // whole turn
+  void getRPY(double &roll, double &pitch, double &yaw) const {
+    if (std::fabs(el[2].x()) >= 1) {
+      yaw = 0;
+      const double delta = std::atan2(el[0].y(), el[0].z());
+      if (el[2].x() > 0) {
+        pitch = -M_PI / 2;
+        roll = -yaw + std::atan2(-el[0].y(), -el[0].z());
+      } else {
+        pitch = M_PI / 2;
+        roll = yaw + delta;
+      }
+      return;
+    }
+    pitch = -std::asin(el[2].x());
+    const double c = std::cos(pitch);
+    roll = std::atan2(el[2].y() / c, el[2].z() / c);
+    yaw = std::atan2(el[1].x() / c, el[0].x() / c);
   }
 };
 

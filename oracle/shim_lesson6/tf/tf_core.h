@@ -1,8 +1,9 @@
 // TEST INFRASTRUCTURE, NOT tf — the tf (ROS 1) types lesson6's karto_slam.cc uses, for compiling the node unmodified
 // (oracle/ref_lesson6.cpp).  tf is not in the reference tree; its LinearMath is the tf2 stand-in
-// (oracle/shim/tf2/LinearMath/Transform.h: tf's Transform, Matrix3x3 and Quaternion share that arithmetic, operation by
-// operation in double), with tf's names and the few members tf adds: Vector3::setValue, Transform(Quaternion, Vector3),
-// Stamped<T>, StampedTransform, createQuaternionFromRPY and getYaw (Matrix3x3::getRPY's yaw, solution 1 of getEulerYPR).
+// (oracle/shim/tf2/LinearMath/Transform.h, under tf's names in oracle/shim/tf/LinearMath/: tf's Transform, Matrix3x3 and
+// Quaternion share that arithmetic, operation by operation in double), with the few members tf adds:
+// Vector3::setValue, Transform(Quaternion, Vector3), Stamped<T>, StampedTransform, createQuaternionFromRPY and getYaw
+// (the yaw of Matrix3x3::getRPY).
 // The listener answers every lookup from what the driver set: base_link <- laser is the mount, odom <- base_link the
 // scan's odometry row (a row holding a NaN makes the lookup throw tf::TransformException).  Timing, interpolation and
 // the transform tree of real tf are not modelled; the library restates exactly this arithmetic (DESIGN.md §7).
@@ -13,13 +14,9 @@
 #include <string>
 
 #include "ros/ros.h"
-#include "tf2/LinearMath/Transform.h"
+#include "tf/LinearMath/Matrix3x3.h"
 
 namespace tf {
-
-typedef double tfScalar;
-typedef tf2::Quaternion Quaternion;
-typedef tf2::Matrix3x3 Matrix3x3;
 
 struct Vector3 : tf2::Vector3 {
   Vector3() = default;
@@ -68,12 +65,9 @@ inline Quaternion createQuaternionFromRPY(double roll, double pitch, double yaw)
 }
 
 inline double getYaw(const Quaternion &q) {
-  Matrix3x3 m;
-  m.setRotation(q);
-  if (std::fabs(m[2].x()) >= 1) return 0.0;
-  const double pitch = -std::asin(m[2].x());
-  const double c = std::cos(pitch);
-  return std::atan2(m[1].x() / c, m[0].x() / c);
+  double roll, pitch, yaw;
+  Matrix3x3(q).getRPY(roll, pitch, yaw);
+  return yaw;
 }
 
 struct TransformException : std::runtime_error {
