@@ -1,5 +1,6 @@
 // lesson4's LaserScan -> DataContainer conversion, per beam, shared by the host adapters (ros_io.cu: b2s_ros_hector_points,
-// b2s_ros_hector_scans) and the ingest stage of the batched stream kernel (hector_slam.cu: k_hs_stream_batch<_, true>).
+// b2s_ros_hector_scans) and the ingest stage of the batched stream kernel (hector_slam.cu: k_hs_stream_batch<_, true>),
+// and the node handle's form of it with the laser mount's full basis (hector_node.cu, k_hs_stream_node).
 // HectorMappingRos::scanCallback (lesson4/src/hector_mapping/hector_slam.cc:186-205) does two things to a scan:
 //   projector_.projectLaser(scan, cloud, 30.0)     laser_geometry's LaserProjection (not in the reference tree, see
 //                                                  DESIGN §7: restated from the package's published behaviour)
@@ -11,6 +12,7 @@
 #include <cmath>
 
 #include "common.cuh"
+#include "ros_math.cuh"
 
 namespace b2s {
 
@@ -63,6 +65,53 @@ __host__ __device__ __forceinline__ bool hector_project_beam(float range, double
   x = (float)((double)range * ux);
   y = (float)((double)range * uy);
   return true;
+}
+
+// The node's own settings of rosPointCloudToDataContainer (b2s_hector_node_*): the full tf::StampedTransform of the laser
+// mount (base_link <- laser, tfScalar = double) and the thresholds squared in double, then rounded to float, as
+// InitParams stores them (hector_slam.cc:150-155).
+struct HectorNodeFilter {
+  float sqr_min, sqr_max;
+  double use_max_scan_range;
+  TfTransform mount;  // basis rows from Matrix3x3::setRotation, origin = the mount's translation
+  float z_min, z_max;
+  float scale_to_map;
+};
+
+// The node handle's staging for its map publishes (hector_node.cu owns it, hs_node_run in hector_slam.cu fills it): a
+// copy stream, two level-0 payload slots on the device and page-locked on the host, and the per-scan record rows
+struct HsNodeIo {
+  Stream copy;
+  Buf<int8_t> d_map[2];
+  HostBuf<int8_t> h_map[2];
+  Event converted[2], copied[2];
+  HostBuf<float> h_rows;  // [scans of the call][16]: a scan's row is here once a later publish's `copied` has fired
+};
+
+// rosPointCloudToDataContainer (hector_slam.cc:331-358) on one laser-frame point with the full mount:
+// laserTransform * Vector3(x, y, z) row by row (tf::Transform::operator*), the z window on that z minus the mount's z
+__host__ __device__ __forceinline__ bool hector_node_filter_point(const HectorNodeFilter &f, float x, float y, float z,
+                                                                  float &ox, float &oy) {
+  const float dist_sqr = x * x + y * y;
+  if (!((dist_sqr > f.sqr_min) && (dist_sqr < f.sqr_max))) return false;
+  if ((x < 0.0f) && (dist_sqr < 0.50f)) return false;  // behind the robot
+  if ((double)dist_sqr > f.use_max_scan_range * f.use_max_scan_range) return false;
+  const double v[3] = {(double)x, (double)y, (double)z};
+  double b[3];
+  tf_apply(f.mount, v, b);
+  const float z_laser = (float)(b[2] - f.mount.o[2]);
+  if (!(z_laser > f.z_min && z_laser < f.z_max)) return false;
+  ox = (float)b[0] * f.scale_to_map;
+  oy = (float)b[1] * f.scale_to_map;
+  return true;
+}
+
+// projectLaser and the node's conversion on one beam
+__host__ __device__ __forceinline__ bool hector_node_beam(const HectorNodeFilter &f, float range, double ux, double uy,
+                                                          double cutoff, float range_min, float &ox, float &oy) {
+  float x, y;
+  if (!hector_project_beam(range, ux, uy, cutoff, range_min, x, y)) return false;
+  return hector_node_filter_point(f, x, y, 0.0f, ox, oy);
 }
 
 // Both stages on one beam

@@ -40,6 +40,7 @@
 #include <cmath>
 #include <cstdlib>
 #include <cstring>
+#include <functional>
 #include <new>
 #include <vector>
 
@@ -944,6 +945,7 @@ struct HsIngest {
   float range_min;
   double range_cutoff;       // projectLaser's cutoff (a negative one already replaced by range_max)
   HectorScanFilter filter;
+  HectorNodeFilter node;     // k_hs_stream_node's conversion (the full laser mount) instead of `filter`
 };
 
 // The node's loop of processor b = blockIdx.x over its scans: match (hs_match_cta), then, if the gate opens, the mark
@@ -957,9 +959,11 @@ struct HsIngest {
 // container row, HS_THREADS beams per round: ballot / popc inside a warp, warp offsets through shared memory, a running
 // base across rounds.  hs_match_cta then reads that row as its input and copies it onto itself: each element is read and
 // written back unchanged by the same thread, which is benign.
-template <bool EXACT, bool INGEST>
-__global__ void __launch_bounds__(HS_THREADS, 1) k_hs_stream_batch(HsBatch P, HsFleet F) {
-  extern __shared__ __align__(16) unsigned char hs_smem[];
+// INGEST selects the conversion: HS_INGEST_YAW (k_hs_stream_batch<_, true>: hector_scan_beam, the mount as x, y, z, yaw)
+// or HS_INGEST_NODE (k_hs_stream_node: hector_node_beam, the mount's full basis, for b2s_hector_node_*).
+enum { HS_INGEST_NONE = 0, HS_INGEST_YAW = 1, HS_INGEST_NODE = 2 };
+template <bool EXACT, int INGEST>
+__device__ __forceinline__ void hs_stream_batch_body(const HsBatch &P, const HsFleet &F, unsigned char *hs_smem) {
   __shared__ float s_last[3];  // the previous scan's match pose: the next scan's hint without a global round trip
   const int b = blockIdx.x;
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
@@ -969,7 +973,7 @@ __global__ void __launch_bounds__(HS_THREADS, 1) k_hs_stream_batch(HsBatch P, Hs
   unsigned long long visits = 0;
   for (long long i = s0; i < s1; i++) {
     HsCall C;
-    if constexpr (INGEST) {
+    if constexpr (INGEST != HS_INGEST_NONE) {
       __shared__ int s_warp_kept[NW];
       const HsIngest &I = *F.ingest;
       float2 *row = reinterpret_cast<float2 *>(P.l[0].pts) + (size_t)b * P.cap;
@@ -982,7 +986,10 @@ __global__ void __launch_bounds__(HS_THREADS, 1) k_hs_stream_batch(HsBatch P, Hs
         bool keep = false;
         if (j < nr) {
           const double2 u = I.units[j];
-          keep = hector_scan_beam(I.filter, r[j], u.x, u.y, I.range_cutoff, I.range_min, q.x, q.y);
+          if constexpr (INGEST == HS_INGEST_NODE)
+            keep = hector_node_beam(I.node, r[j], u.x, u.y, I.range_cutoff, I.range_min, q.x, q.y);
+          else
+            keep = hector_scan_beam(I.filter, r[j], u.x, u.y, I.range_cutoff, I.range_min, q.x, q.y);
         }
         const unsigned m = __ballot_sync(0xffffffffu, keep);
         if (lane == 0) s_warp_kept[warp] = __popc(m);
@@ -1027,6 +1034,19 @@ __global__ void __launch_bounds__(HS_THREADS, 1) k_hs_stream_batch(HsBatch P, Hs
     }
   }
   if (lane == 0 && visits) atomicAdd(&st->visits, visits);
+}
+
+template <bool EXACT, bool INGEST>
+__global__ void __launch_bounds__(HS_THREADS, 1) k_hs_stream_batch(HsBatch P, HsFleet F) {
+  extern __shared__ __align__(16) unsigned char hs_smem[];
+  hs_stream_batch_body<EXACT, INGEST ? HS_INGEST_YAW : HS_INGEST_NONE>(P, F, hs_smem);
+}
+
+// lesson4's HectorMappingRos (b2s_hector_node_*): k_hs_stream_batch's loop with the node's full-basis conversion, exact
+// mode, one processor (blockIdx.x = 0), over the scans F.first[0] ... F.first[1] - 1 of one part of a recording
+__global__ void __launch_bounds__(HS_THREADS, 1) k_hs_stream_node(HsBatch P, HsFleet F) {
+  extern __shared__ __align__(16) unsigned char hs_smem[];
+  hs_stream_batch_body<true, HS_INGEST_NODE>(P, F, hs_smem);
 }
 
 __global__ void k_hs_fill(float *__restrict__ p, size_t n, float v) {
@@ -1191,6 +1211,7 @@ static b2s_status hs_create(float map_resolution, int map_size_x, int map_size_y
   B2S_CUDA_CHECK(raise_dyn_smem(k_hs_stream_batch<false, false>, smem));
   B2S_CUDA_CHECK(raise_dyn_smem(k_hs_stream_batch<true, true>, smem));
   B2S_CUDA_CHECK(raise_dyn_smem(k_hs_stream_batch<false, true>, smem));
+  B2S_CUDA_CHECK(raise_dyn_smem(k_hs_stream_node, smem));
   {
     int coop = 0, sms = 0, per_sm = 0;
     B2S_CUDA_CHECK(cudaDeviceGetAttribute(&coop, cudaDevAttrCooperativeLaunch, device));
@@ -1350,6 +1371,128 @@ static b2s_status hs_fleet_run(b2s_hector_slam *p, const int32_t *n_scans, const
       if (n_scans[b] > 0) std::memcpy(out_last_covs + 9 * (size_t)b, host.data() + 16 * (size_t)(first[b + 1] - 1) + 3, 9 * sizeof(float));
   return B2S_OK;
 }
+
+namespace b2s {
+
+// HectorMappingRos::setMapInfo (hector_slam.cc:165-180) of level 0: getWorldCoords(0, 0) - cell length * 0.5f
+void hs_node_map_info(const b2s_hector_slam *p, float &origin_x, float &origin_y, float &cell_length, int &w, int &h) {
+  float wx, wy;
+  get_world_coords(p->P.l[0].tf, 0.0f, 0.0f, wx, wy);
+  cell_length = p->cell_length[0];
+  origin_x = wx - cell_length * 0.5f;
+  origin_y = wy - cell_length * 0.5f;
+  w = p->sx[0];
+  h = p->sy[0];
+}
+
+float hs_scale_to_map(const b2s_hector_slam *p) { return p->P.l[0].tf.tw_lin; }  // GridMapBase::getScaleToMap of level 0
+
+// ---- lesson4's HectorMappingRos (hector_node.cu) over one part of a recording ----
+// The scans run in k_hs_stream_node launches split at the publish points.  Before the scan a publish precedes, level 0
+// is converted to its ROS payload on the processor's stream (k_hector_ros); a second stream copies it, with the record
+// rows of the scans before it, into page-locked memory while the next part's launch runs.  Two payload slots: a slot is
+// handed to on_map (in publish order) before it is converted into again.
+b2s_status hs_node_run(b2s_hector_slam *p, HsNodeIo &io, const b2s_laser_scan_msg &geometry, const double *units,
+                       double range_cutoff, const HectorNodeFilter &filter, int n_scans, const float *ranges,
+                       const std::vector<int> &cuts, float *out_rows,
+                       const std::function<b2s_status(size_t, const int8_t *)> &on_map) {
+  const int nr = geometry.n_ranges;
+  const size_t cells = (size_t)p->sx[0] * p->sy[0];
+  B2S_CUDA_CHECK(cudaSetDevice(p->device));
+  b2s_status st = hs_wait_launch(p);
+  if (st) return st;
+  if ((st = hs_reserve_epochs(p, (unsigned long long)n_scans))) return st;
+  B2S_CUDA_CHECK(io.h_rows.reserve(16 * (size_t)std::max(n_scans, 1)));
+  for (int k = 0; k < 2; k++) {
+    B2S_CUDA_CHECK(io.d_map[k].reserve(cells));
+    B2S_CUDA_CHECK(io.h_map[k].reserve(cells));
+  }
+  // part boundaries: 0, every publish point, n_scans
+  std::vector<long long> bounds(1, 0);
+  for (int c : cuts)
+    if (c > bounds.back()) bounds.push_back(c);
+  if (n_scans > bounds.back()) bounds.push_back(n_scans);
+  AsyncBuf<float> d_ranges(p->stream), d_out(p->stream);
+  AsyncBuf<double> d_unit(p->stream);
+  AsyncBuf<HsIngest> d_ingest(p->stream);
+  AsyncBuf<long long> d_bounds(p->stream);
+  const size_t n_r = (size_t)n_scans * (size_t)nr;
+  B2S_CUDA_CHECK(d_ranges.alloc(std::max<size_t>(n_r, 1)));
+  B2S_CUDA_CHECK(d_unit.alloc(2 * (size_t)std::max(nr, 1)));
+  B2S_CUDA_CHECK(d_ingest.alloc(1));
+  B2S_CUDA_CHECK(d_bounds.alloc(bounds.size()));
+  B2S_CUDA_CHECK(d_out.alloc(16 * (size_t)std::max(n_scans, 1)));
+  if (n_r > 0) B2S_CUDA_CHECK(cudaMemcpyAsync(d_ranges, ranges, sizeof(float) * n_r, cudaMemcpyHostToDevice, p->stream));
+  if (nr > 0) B2S_CUDA_CHECK(cudaMemcpyAsync(d_unit, units, sizeof(double) * 2 * (size_t)nr, cudaMemcpyHostToDevice, p->stream));
+  B2S_CUDA_CHECK(cudaMemcpyAsync(d_bounds, bounds.data(), sizeof(long long) * bounds.size(), cudaMemcpyHostToDevice, p->stream));
+  HsIngest I;
+  std::memset(&I, 0, sizeof(I));
+  I.ranges = d_ranges;
+  I.units = reinterpret_cast<const double2 *>(static_cast<double *>(d_unit));
+  I.n_ranges = nr;
+  I.range_min = geometry.range_min;
+  I.range_cutoff = range_cutoff;
+  I.node = filter;
+  B2S_CUDA_CHECK(cudaMemcpyAsync(d_ingest, &I, sizeof(HsIngest), cudaMemcpyHostToDevice, p->stream));  // (staged: pageable)
+  // the copy stream reads d_out: on every way out it is drained before the stream-ordered frees above
+  struct DrainCopies {
+    cudaStream_t s;
+    ~DrainCopies() { cudaStreamSynchronize(s); }
+  } drain_copies{io.copy};
+  HsFleet F;
+  std::memset(&F, 0, sizeof(F));
+  F.ingest = d_ingest;
+  F.origo_x = (float)filter.mount.o[0] * filter.scale_to_map;  // dataContainer.setOrigo (hector_slam.cc:329)
+  F.origo_y = (float)filter.mount.o[1] * filter.scale_to_map;
+  F.out = d_out;
+  const size_t smem = hs_smem_bytes(p->cap);
+  struct Pending { size_t k; int slot; };
+  std::vector<Pending> pending;
+  size_t next_cut = 0, rows_copied = 0;
+  int slot = 0;
+  auto drain_one = [&]() -> b2s_status {
+    const Pending q = pending.front();
+    pending.erase(pending.begin());
+    B2S_CUDA_CHECK(cudaEventSynchronize(io.copied[q.slot]));
+    return on_map(q.k, io.h_map[q.slot]);
+  };
+  for (size_t c = 0; c + 1 < bounds.size(); c++) {  // every publish point lies in [0, n_scans): it starts a part
+    const long long a = bounds[c];
+    if (next_cut < cuts.size() && cuts[next_cut] == a) {  // the publish before scan a
+      if (pending.size() == 2) {
+        if ((st = drain_one())) return st;
+      }
+      k_hector_ros<<<ceil_div((long long)cells, 256), 256, 0, p->stream>>>(p->P.l[0].lo, (int)cells, io.d_map[slot]);
+      B2S_CUDA_CHECK(cudaGetLastError());
+      B2S_CUDA_CHECK(cudaEventRecord(io.converted[slot], p->stream));
+      B2S_CUDA_CHECK(cudaStreamWaitEvent(io.copy, io.converted[slot], 0));
+      B2S_CUDA_CHECK(cudaMemcpyAsync(io.h_map[slot], io.d_map[slot], cells, cudaMemcpyDeviceToHost, io.copy));
+      if ((size_t)a > rows_copied) {
+        B2S_CUDA_CHECK(cudaMemcpyAsync(io.h_rows + 16 * rows_copied, d_out + 16 * rows_copied,
+                                       sizeof(float) * 16 * ((size_t)a - rows_copied), cudaMemcpyDeviceToHost, io.copy));
+        rows_copied = (size_t)a;
+      }
+      B2S_CUDA_CHECK(cudaEventRecord(io.copied[slot], io.copy));
+      pending.push_back(Pending{next_cut, slot});
+      slot ^= 1;
+      next_cut++;
+    }
+    F.first = d_bounds + c;  // this part: scans bounds[c] ... bounds[c + 1] - 1
+    k_hs_stream_node<<<1, HS_THREADS, smem, p->stream>>>(p->P, F);
+    B2S_CUDA_CHECK(cudaGetLastError());
+  }
+  if ((size_t)n_scans > rows_copied)
+    B2S_CUDA_CHECK(cudaMemcpyAsync(io.h_rows + 16 * rows_copied, d_out + 16 * rows_copied,
+                                   sizeof(float) * 16 * ((size_t)n_scans - rows_copied), cudaMemcpyDeviceToHost, p->stream));
+  while (!pending.empty())
+    if ((st = drain_one())) return st;
+  B2S_CUDA_CHECK(cudaStreamSynchronize(io.copy));
+  B2S_CUDA_CHECK(cudaStreamSynchronize(p->stream));
+  std::memcpy(out_rows, io.h_rows, sizeof(float) * 16 * (size_t)n_scans);
+  return B2S_OK;
+}
+
+}  // namespace b2s
 
 extern "C" {
 

@@ -645,6 +645,91 @@ b2s_status b2s_hector_slam_process_scans_batch(b2s_hector_slam *p, const b2s_las
                                                int map_without_matching, float *out_poses, int32_t *out_map_updated,
                                                float *out_last_covs, int32_t *out_n_points);
 
+/* ---------------------------------------------------------------- lesson4: the Hector SLAM node over whole recordings
+ * HectorMappingRos (lesson4/src/hector_mapping/hector_slam.cc) for one laser: InitParams, the LaserScan conversion with
+ * the full laser mount, HectorSlamProcessor::update (the device processor, b2s_hector_slam_*), the pose-info message and
+ * tf (PoseInfoContainer.h) and publishMap of level 0 with its update-index gate, over a recording handed in as arrays.
+ * tests/test_gpu_hector_node.py pins this handle to the restatement oracle/hector_node_port.py.
+ *
+ * The publish schedule is the library's own (the node publishes from a thread every map_pub_period of wall time, so the
+ * reference's schedule depends on thread timing; DESIGN.md §7): tick 0 is the stamp of the first scan ever handed in,
+ * tick k = tick 0 + k * Duration::fromSec(map_pub_period) in roscpp's integer arithmetic.  Before scan i is processed,
+ * if its stamp >= the next tick, the map is published once, stamped with that tick, and the next tick becomes the first
+ * tick strictly after scan i's stamp (no catch-up over gaps).  So map 0 precedes scan 0 and is all -1, as the node's
+ * first publish at construction is. */
+typedef struct b2s_hector_node_params { /* HectorMappingRos::InitParams (hector_slam.cc:119-162), node defaults [] */
+  double map_resolution;             /* [0.05] m, cast to float for the processor */
+  int32_t map_size;                  /* [2048] cells, square */
+  int32_t map_multi_res_levels;      /* [3] */
+  double map_start_x, map_start_y;   /* [0.5, 0.5] cast to float */
+  double update_factor_free;         /* [0.4] (float setter) */
+  double update_factor_occupied;     /* [0.9] */
+  double map_update_distance_thresh; /* [0.4] */
+  double map_update_angle_thresh;    /* [0.9] */
+  double use_max_scan_range;         /* [20.0] m */
+  double laser_min_dist;             /* [0.2] m; the handle squares it in double, then rounds to float, as the node */
+  double laser_max_dist;             /* [30.0] m; likewise */
+  float laser_z_min_value;           /* [-1.0] */
+  float laser_z_max_value;           /* [1.0] */
+  double map_pub_period;             /* [2.0] s */
+} b2s_hector_node_params;
+
+/* nav_msgs/MapMetaData as setMapInfo fills it (hector_slam.cc:165-180): origin = getWorldCoords(0, 0) - cell length / 2
+ * (float, widened), orientation identity, resolution = the float cell length, width / height = level 0's size */
+typedef struct b2s_hector_node_map_info {
+  double origin_x, origin_y;
+  float resolution;
+  int32_t width, height;
+} b2s_hector_node_map_info;
+
+/* One published map: scan_index = the scans handed to the handle before it (over all calls), stamp (sec, nsec) = its
+ * tick (or the stamp given to b2s_hector_node_publish_map), payload [height][width] int8 (-1 / 0 / 100), rebuilt = 1
+ * when the grid's update index differed from the one at the previous publish (publishMap's gate; the payload is the
+ * same bytes either way).  Pointers are valid only during the call. */
+typedef void (*b2s_hector_node_map_fn)(void *user, int32_t scan_index, const uint32_t stamp[2],
+                                       const b2s_hector_node_map_info *info, const int8_t *payload, int32_t rebuilt);
+
+typedef struct b2s_hector_node b2s_hector_node; /* opaque: one HectorMappingRos */
+
+/* The node's constructor.  geometry = the recording's LaserScan fields (angle_min, angle_increment, range_min,
+ * range_max, n_ranges; its ranges pointer is not read); projectLaser's cutoff is 30 m as in the node.  laser_mount =
+ * base_link <- laser, translation xyz + quaternion xyzw (what the listener answers in the constructor); its basis is
+ * Matrix3x3::setRotation of the quaternion.  B2S_ERR_BAD_PARAMS for NULL pointers, a zero or non-finite mount, a
+ * non-positive resolution or map size, levels the processor refuses, a map_pub_period that is not positive and finite or
+ * whose ros::Duration is zero or outside its 32-bit range, and a zero angle_increment; B2S_ERR_TOO_LARGE for n_ranges
+ * above 4096; B2S_ERR_NO_DEVICE without a device. */
+b2s_status b2s_hector_node_create(const b2s_hector_node_params *params, const b2s_laser_scan_msg *geometry,
+                                  const double laser_mount[7], int device, b2s_hector_node **out);
+void b2s_hector_node_destroy(b2s_hector_node *node);
+/* The inner processor: b2s_hector_slam_level_dims / _copy_level / _copy_level_ros / _last_poses / _stats read the
+ * node's maps and poses.  Owned by the node; do not destroy it or process scans through it.  The node always runs in
+ * exact mode. */
+b2s_hector_slam *b2s_hector_node_processor(b2s_hector_node *node);
+/* HectorMappingRos::scanCallback on the next n_scans LaserScans: ranges [n_scans][n_ranges] float32, stamps
+ * [n_scans][2] = header.stamp (sec, nsec).  Per scan (any output may be NULL):
+ *   out_pose [3] float        getLastScanMatchPose after the scan
+ *   out_pose_msg [7] double   the PoseWithCovarianceStamped pose: x, y, 0, 0, 0, sin(yaw * 0.5f), cos(yaw * 0.5f)
+ *                             (the double sin / cos of the float half angle, as the node's unqualified calls bind
+ *                             under the stand-in headers; DESIGN.md §7).  odom_hector carries the same pose; the
+ *                             odom -> base_link tf is poseMsgToTF of it, and map -> odom stays the identity.
+ *   out_cov [36] double       lastScanMatchCov (the level-0 Hessian) spread as PoseInfoContainer::update does, every
+ *                             other entry 0.  A scan that keeps no beams leaves lastScanMatchCov as it was; before the
+ *                             first matched scan the node reads an uninitialised matrix, and the handle reports zeros.
+ *   out_map_updated           the gate's map-update decision
+ *   out_n_points              the beams the conversion kept
+ * Maps due by the schedule go to on_map (may be NULL) before the call returns, in order.  Two calls over consecutive
+ * parts of a recording equal one call.  B2S_ERR_BAD_PARAMS (nothing written, nothing changed) for NULL arrays with
+ * n_scans > 0 or n_scans < 0; B2S_ERR_TOO_LARGE for 2^20 - 1 or more scans in one call.  A call that fails after it
+ * started (a CUDA error) may already have handed out maps and moved the processor; the handle then answers every
+ * later process / publish_map call with B2S_ERR_BAD_STATE and must be destroyed. */
+b2s_status b2s_hector_node_process(b2s_hector_node *node, int n_scans, const float *ranges, const uint32_t *stamps,
+                                   float *out_pose, double *out_pose_msg, double *out_cov, int32_t *out_map_updated,
+                                   int32_t *out_n_points, b2s_hector_node_map_fn on_map, void *user);
+/* The node's publishMap of level 0 now, stamped `stamp` (sec, nsec): for a caller with its own clock and for the final
+ * map.  It shares the update-index gate with the scheduled publishes and does not move the schedule. */
+b2s_status b2s_hector_node_publish_map(b2s_hector_node *node, const uint32_t stamp[2], b2s_hector_node_map_fn on_map,
+                                       void *user);
+
 /* ---------------------------------------------------------------- K2b: GMapping hit/visit map */
 
 typedef struct b2s_gmap b2s_gmap; /* opaque: replaces GMapping::ScanMatcherMap (gmapping.cc:135) */
