@@ -165,12 +165,13 @@ inline float prob_to_log_odds_logf(float prob) {
 }
 
 // HectorMappingRos::publishMap (lesson4/src/hector_mapping/hector_slam.cc:254-317): free -> 0, occupied -> 100, else -1.
+__device__ __forceinline__ int8_t hector_ros_cell(float v) { return v < 0.0f ? 0 : (v > 0.0f ? 100 : -1); }
+
 // `static`: each translation unit gets its own copy, the library exports nothing from here.
 static __global__ void k_hector_ros(const float *__restrict__ lo, int n, int8_t *__restrict__ out) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
-  const float v = lo[i];
-  out[i] = v < 0.0f ? 0 : (v > 0.0f ? 100 : -1);
+  out[i] = hector_ros_cell(lo[i]);
 }
 
 }  // namespace b2s

@@ -1,5 +1,7 @@
-// lesson4's HectorMappingRos node (lesson4/src/hector_mapping/hector_slam.cc) over a whole recording of one laser: host
-// C++ around the device HectorSlamProcessor (hector_slam.cu), whose k_hs_stream_node converts and matches the scans.
+// lesson4's HectorMappingRos node (lesson4/src/hector_mapping/hector_slam.cc) over whole recordings, B nodes per handle:
+// host C++ around the device batched HectorSlamProcessor (hector_slam.cu), one processor per node, whose
+// k_hs_stream_node converts and matches every node's scans, one CTA per node.  The publish schedule and the launch
+// parts are hector_node_plan.cuh's; the single-node entry points are the batched ones with B = 1.
 //   HectorMappingRos::InitParams / constructor       hector_slam.cc:26-105, 119-162
 //   HectorMappingRos::setMapInfo                     :165-180
 //   HectorMappingRos::scanCallback                   :186-251  (projectLaser, rosPointCloudToDataContainer, update)
@@ -12,9 +14,11 @@
 #include <functional>
 #include <memory>
 #include <new>
+#include <string>
 #include <vector>
 
 #include "common.cuh"
+#include "hector_node_plan.cuh"
 #include "hector_scan.cuh"
 #include "ros_math.cuh"
 
@@ -23,9 +27,9 @@ namespace b2s {
 void hs_node_map_info(const b2s_hector_slam *p, float &origin_x, float &origin_y, float &cell_length, int &w, int &h);
 float hs_scale_to_map(const b2s_hector_slam *p);
 b2s_status hs_node_run(b2s_hector_slam *p, HsNodeIo &io, const b2s_laser_scan_msg &geometry, const double *units,
-                       double range_cutoff, const HectorNodeFilter &filter, int n_scans, const float *ranges,
-                       const std::vector<int> &cuts, float *out_rows,
-                       const std::function<b2s_status(size_t, const int8_t *)> &on_map);
+                       double range_cutoff, const HectorNodeFilter *filters, const HectorNodePlan &plan,
+                       const int32_t *n_scans, const float *ranges, float *out_rows,
+                       const std::function<b2s_status(int, int, const int8_t *, const float *, long long)> &on_map);
 }  // namespace b2s
 
 using namespace b2s;
@@ -33,81 +37,115 @@ using namespace b2s;
 namespace {
 constexpr int NODE_MAX_RANGES = 4096;      // the processor's per-scan capacity
 constexpr int NODE_MAX_SCANS = (1 << 20) - 1;  // stamp epochs of one call (hector_slam.cu)
+constexpr int NODE_MAX_BATCH = 65535;      // the publishes before one part are one launch's grid rows
 constexpr int64_t NS = 1000000000LL;
-
-int64_t stamp_ns(const uint32_t *s) { return (int64_t)s[0] * NS + (int64_t)s[1]; }
 }  // namespace
 
+// B nodes, one per processor of a batched HectorSlamProcessor; per-node state is indexed by node
 struct b2s_hector_node {
-  b2s_hector_node_params prm{};
+  int batch = 1;
   b2s_laser_scan_msg geom{};
   int device = 0;
   b2s_hector_slam *proc = nullptr;
-  HectorNodeFilter filter{};
+  std::vector<HectorNodeFilter> filters;
   double cutoff = 30.0;  // projector_.projectLaser(scan, laser_point_cloud_, 30.0)
   std::vector<double> units;
-  int64_t period_ns = 0;            // Duration::fromSec(map_pub_period)
-  bool started = false;             // tick 0 set (a scan was handed in)
-  int64_t next_tick_ns = 0;
-  int64_t scans = 0;                // scans handed in so far
-  int64_t updates = 0;              // map updates so far: level 0's getUpdateIndex() = updates - 1
-  int64_t last_get_map_update_index = -100;  // lastGetMapUpdateIndex
+  std::vector<int64_t> period_ns;       // Duration::fromSec(map_pub_period)
+  std::vector<HectorNodeClock> clock;   // the publish schedule (started, next tick)
+  std::vector<int64_t> scans;           // scans handed in so far
+  std::vector<int64_t> updates;         // map updates so far: level 0's getUpdateIndex() = updates - 1
+  std::vector<int64_t> last_get_map_update_index;  // lastGetMapUpdateIndex
   b2s_hector_node_map_info info{};
   HsNodeIo io;
   std::vector<float> rows;
-  std::vector<int8_t> payload;      // b2s_hector_node_publish_map's
+  std::vector<int8_t> payload;      // b2s_hector_node_publish_map_of's
   bool failed = false;              // a call failed partway: maps were handed out, the schedule was not committed
 };
 
 namespace {
 
-// publishMap's gate: rebuild when the grid's update index moved since the last publish
-int32_t map_gate(b2s_hector_node *n, int64_t updates) {
+// publishMap's gate: rebuild when node b's grid update index moved since its last publish
+int32_t map_gate(b2s_hector_node *n, int b, int64_t updates) {
   const int64_t index = updates - 1;
-  const bool rebuilt = index != n->last_get_map_update_index;
-  n->last_get_map_update_index = index;
+  const bool rebuilt = index != n->last_get_map_update_index[(size_t)b];
+  n->last_get_map_update_index[(size_t)b] = index;
   return rebuilt ? 1 : 0;
+}
+
+// the fields the batched processor holds once (HsBatch): equal in every node's parameters
+bool same_processor(const b2s_hector_node_params &a, const b2s_hector_node_params &b) {
+  return a.map_resolution == b.map_resolution && a.map_size == b.map_size &&
+         a.map_multi_res_levels == b.map_multi_res_levels && a.map_start_x == b.map_start_x &&
+         a.map_start_y == b.map_start_y && a.update_factor_free == b.update_factor_free &&
+         a.update_factor_occupied == b.update_factor_occupied &&
+         a.map_update_distance_thresh == b.map_update_distance_thresh &&
+         a.map_update_angle_thresh == b.map_update_angle_thresh;
+}
+
+// a single-node entry point's callback behind the batched one
+struct SingleMapFn {
+  b2s_hector_node_map_fn fn;
+  void *user;
+};
+void single_map(void *user, int32_t, int32_t scan_index, const uint32_t stamp[2], const b2s_hector_node_map_info *info,
+                const int8_t *payload, int32_t rebuilt) {
+  const SingleMapFn *s = static_cast<const SingleMapFn *>(user);
+  if (s->fn) s->fn(s->user, scan_index, stamp, info, payload, rebuilt);
 }
 
 }  // namespace
 
 extern "C" {
 
-b2s_status b2s_hector_node_create(const b2s_hector_node_params *params, const b2s_laser_scan_msg *geometry,
-                                  const double laser_mount[7], int device, b2s_hector_node **out) {
+b2s_status b2s_hector_node_create_batch(int batch, const b2s_hector_node_params *params,
+                                        const b2s_laser_scan_msg *geometry, const double *laser_mounts, int device,
+                                        b2s_hector_node **out) {
   if (!out) B2S_FAIL(B2S_ERR_BAD_PARAMS, "b2s_hector_node_create: null argument");
   *out = nullptr;
-  if (!params || !geometry || !laser_mount) B2S_FAIL(B2S_ERR_BAD_PARAMS, "b2s_hector_node_create: null argument");
-  const float res = static_cast<float>(params->map_resolution);
-  if (!(res > 0.0f) || !std::isfinite(res)) B2S_FAIL(B2S_ERR_BAD_PARAMS, "b2s_hector_node_create: map_resolution must be positive");
-  if (params->map_size <= 0) B2S_FAIL(B2S_ERR_BAD_PARAMS, "b2s_hector_node_create: map_size must be positive");
-  const double period = params->map_pub_period;
-  if (!(period > 0.0) || !std::isfinite(period) || std::floor(period) > 2147483647.0)
-    B2S_FAIL(B2S_ERR_BAD_PARAMS, "b2s_hector_node_create: map_pub_period must be positive, finite and inside ros::Duration's range");
-  const RosDuration d = ros_duration_from_sec(period);
-  const int64_t period_ns = (int64_t)d.sec * NS + (int64_t)d.nsec;
-  if (period_ns <= 0) B2S_FAIL(B2S_ERR_BAD_PARAMS, "b2s_hector_node_create: map_pub_period rounds to a zero ros::Duration");
+  if (!params || !geometry || !laser_mounts) B2S_FAIL(B2S_ERR_BAD_PARAMS, "b2s_hector_node_create: null argument");
+  if (batch < 1) B2S_FAIL(B2S_ERR_BAD_PARAMS, "b2s_hector_node_create_batch: batch must be positive");
+  if (batch > NODE_MAX_BATCH) B2S_FAIL(B2S_ERR_TOO_LARGE, "b2s_hector_node_create_batch: at most 65535 nodes");
+  std::vector<int64_t> period_ns((size_t)batch);
+  for (int b = 0; b < batch; b++) {
+    const b2s_hector_node_params &pb = params[b];
+    const double *mount = laser_mounts + 7 * (size_t)b;
+    const std::string who = batch > 1 ? "b2s_hector_node_create_batch: node " + std::to_string(b) + ": "
+                                      : std::string("b2s_hector_node_create: ");
+    if (!same_processor(pb, params[0]))
+      B2S_FAIL(B2S_ERR_BAD_PARAMS, who + "the processor's fields (map size, resolution, levels, start, update factors, "
+                                         "update thresholds) differ from node 0's");
+    const float res = static_cast<float>(pb.map_resolution);
+    if (!(res > 0.0f) || !std::isfinite(res)) B2S_FAIL(B2S_ERR_BAD_PARAMS, who + "map_resolution must be positive");
+    if (pb.map_size <= 0) B2S_FAIL(B2S_ERR_BAD_PARAMS, who + "map_size must be positive");
+    const double period = pb.map_pub_period;
+    if (!(period > 0.0) || !std::isfinite(period) || std::floor(period) > 2147483647.0)
+      B2S_FAIL(B2S_ERR_BAD_PARAMS, who + "map_pub_period must be positive, finite and inside ros::Duration's range");
+    const RosDuration d = ros_duration_from_sec(period);
+    period_ns[(size_t)b] = (int64_t)d.sec * NS + (int64_t)d.nsec;
+    if (period_ns[(size_t)b] <= 0) B2S_FAIL(B2S_ERR_BAD_PARAMS, who + "map_pub_period rounds to a zero ros::Duration");
+    double qn = 0.0;
+    for (int k = 0; k < 7; k++)
+      if (!std::isfinite(mount[k])) B2S_FAIL(B2S_ERR_BAD_PARAMS, who + "non-finite laser mount");
+    for (int k = 3; k < 7; k++) qn += mount[k] * mount[k];
+    if (!(qn > 0.0)) B2S_FAIL(B2S_ERR_BAD_PARAMS, who + "zero mount quaternion");
+  }
   if (geometry->angle_increment == 0.0f || geometry->n_ranges < 0)
     B2S_FAIL(B2S_ERR_BAD_PARAMS, "b2s_hector_node_create: zero angle_increment or negative n_ranges");
   if (geometry->n_ranges > NODE_MAX_RANGES) B2S_FAIL(B2S_ERR_TOO_LARGE, "b2s_hector_node_create: at most 4096 ranges per scan");
-  double qn = 0.0;
-  for (int k = 0; k < 7; k++)
-    if (!std::isfinite(laser_mount[k])) B2S_FAIL(B2S_ERR_BAD_PARAMS, "b2s_hector_node_create: non-finite laser mount");
-  for (int k = 3; k < 7; k++) qn += laser_mount[k] * laser_mount[k];
-  if (!(qn > 0.0)) B2S_FAIL(B2S_ERR_BAD_PARAMS, "b2s_hector_node_create: zero mount quaternion");
 
   // the constructor: HectorSlamProcessor(static_cast<float>(resolution), size, size, Vector2f(start), levels) + setters
+  const b2s_hector_node_params &p0 = params[0];
   b2s_hector_slam *proc = nullptr;
-  if (b2s_status st = b2s_hector_slam_create_batch(1, std::max(geometry->n_ranges, 1), res, params->map_size,
-                                                   params->map_size, static_cast<float>(params->map_start_x),
-                                                   static_cast<float>(params->map_start_y),
-                                                   params->map_multi_res_levels, device, nullptr, &proc))
+  if (b2s_status st = b2s_hector_slam_create_batch(batch, std::max(geometry->n_ranges, 1),
+                                                   static_cast<float>(p0.map_resolution), p0.map_size, p0.map_size,
+                                                   static_cast<float>(p0.map_start_x), static_cast<float>(p0.map_start_y),
+                                                   p0.map_multi_res_levels, device, nullptr, &proc))
     return st;
-  b2s_status st = b2s_hector_slam_set_update_factors(proc, static_cast<float>(params->update_factor_free),
-                                                      static_cast<float>(params->update_factor_occupied));
+  b2s_status st = b2s_hector_slam_set_update_factors(proc, static_cast<float>(p0.update_factor_free),
+                                                      static_cast<float>(p0.update_factor_occupied));
   if (!st)
-    st = b2s_hector_slam_set_map_update_min_diff(proc, static_cast<float>(params->map_update_distance_thresh),
-                                                 static_cast<float>(params->map_update_angle_thresh));
+    st = b2s_hector_slam_set_map_update_min_diff(proc, static_cast<float>(p0.map_update_distance_thresh),
+                                                 static_cast<float>(p0.map_update_angle_thresh));
   if (st) {
     b2s_hector_slam_destroy(proc);
     return st;
@@ -118,22 +156,31 @@ b2s_status b2s_hector_node_create(const b2s_hector_node_params *params, const b2
     B2S_FAIL(B2S_ERR_CUDA, "out of host memory");
   }
   std::unique_ptr<b2s_hector_node, decltype(&b2s_hector_node_destroy)> guard(n, b2s_hector_node_destroy);
-  n->prm = *params;
+  n->batch = batch;
   n->geom = *geometry;
   n->geom.ranges = nullptr;
   n->device = device;
   n->proc = proc;
   n->period_ns = period_ns;
+  n->clock.assign((size_t)batch, HectorNodeClock{});
+  n->scans.assign((size_t)batch, 0);
+  n->updates.assign((size_t)batch, 0);
+  n->last_get_map_update_index.assign((size_t)batch, -100);
   // rosPointCloudToDataContainer's settings: the thresholds as InitParams stores them, the mount's tf::Transform
-  HectorNodeFilter &f = n->filter;
-  f.sqr_min = static_cast<float>(params->laser_min_dist * params->laser_min_dist);
-  f.sqr_max = static_cast<float>(params->laser_max_dist * params->laser_max_dist);
-  f.use_max_scan_range = params->use_max_scan_range;
-  tf_set_rotation(f.mount, laser_mount + 3);
-  f.mount.o[0] = laser_mount[0]; f.mount.o[1] = laser_mount[1]; f.mount.o[2] = laser_mount[2];
-  f.z_min = params->laser_z_min_value;
-  f.z_max = params->laser_z_max_value;
-  f.scale_to_map = hs_scale_to_map(proc);
+  n->filters.resize((size_t)batch);
+  for (int b = 0; b < batch; b++) {
+    const b2s_hector_node_params &pb = params[b];
+    const double *mount = laser_mounts + 7 * (size_t)b;
+    HectorNodeFilter &f = n->filters[(size_t)b];
+    f.sqr_min = static_cast<float>(pb.laser_min_dist * pb.laser_min_dist);
+    f.sqr_max = static_cast<float>(pb.laser_max_dist * pb.laser_max_dist);
+    f.use_max_scan_range = pb.use_max_scan_range;
+    tf_set_rotation(f.mount, mount + 3);
+    f.mount.o[0] = mount[0]; f.mount.o[1] = mount[1]; f.mount.o[2] = mount[2];
+    f.z_min = pb.laser_z_min_value;
+    f.z_max = pb.laser_z_max_value;
+    f.scale_to_map = hs_scale_to_map(proc);
+  }
   n->units.resize(2 * (size_t)std::max(geometry->n_ranges, 1));
   hector_unit_vectors(geometry->angle_min, geometry->angle_increment, geometry->n_ranges, n->units.data());
   float ox, oy, cl;
@@ -152,6 +199,11 @@ b2s_status b2s_hector_node_create(const b2s_hector_node_params *params, const b2
   return B2S_OK;
 }
 
+b2s_status b2s_hector_node_create(const b2s_hector_node_params *params, const b2s_laser_scan_msg *geometry,
+                                  const double laser_mount[7], int device, b2s_hector_node **out) {
+  return b2s_hector_node_create_batch(1, params, geometry, laser_mount, device, out);
+}
+
 void b2s_hector_node_destroy(b2s_hector_node *n) {
   if (!n) return;
   if (n->proc) {
@@ -164,88 +216,103 @@ void b2s_hector_node_destroy(b2s_hector_node *n) {
 
 b2s_hector_slam *b2s_hector_node_processor(b2s_hector_node *n) { return n ? n->proc : nullptr; }
 
-b2s_status b2s_hector_node_process(b2s_hector_node *n, int n_scans, const float *ranges, const uint32_t *stamps,
-                                   float *out_pose, double *out_pose_msg, double *out_cov, int32_t *out_map_updated,
-                                   int32_t *out_n_points, b2s_hector_node_map_fn on_map, void *user) {
+b2s_status b2s_hector_node_process_batch(b2s_hector_node *n, const int32_t *n_scans, const float *ranges,
+                                         const uint32_t *stamps, float *out_pose, double *out_pose_msg, double *out_cov,
+                                         int32_t *out_map_updated, int32_t *out_n_points,
+                                         b2s_hector_node_batch_map_fn on_map, void *user) {
   B2S_NVTX("HectorMappingRos::scanCallback");
-  if (!n || n_scans < 0 || (n_scans > 0 && (!stamps || (!ranges && n->geom.n_ranges > 0))))
-    B2S_FAIL(B2S_ERR_BAD_PARAMS, "b2s_hector_node_process: null argument or negative count");
-  if (n->failed) B2S_FAIL(B2S_ERR_BAD_STATE, "b2s_hector_node_process: an earlier call failed partway; destroy the handle");
-  if (n_scans >= NODE_MAX_SCANS) B2S_FAIL(B2S_ERR_TOO_LARGE, "b2s_hector_node_process: too many scans in one call (split it)");
-  if (n_scans == 0) return B2S_OK;
-  // the schedule: the scans a publish precedes, and their ticks
-  std::vector<int> cuts;
-  std::vector<int64_t> ticks;
-  bool started = n->started;
-  int64_t next = n->next_tick_ns;
-  for (int i = 0; i < n_scans; i++) {
-    const int64_t s = stamp_ns(stamps + 2 * (size_t)i);
-    if (!started) {
-      started = true;
-      next = s;  // tick 0
-    }
-    if (s >= next) {
-      cuts.push_back(i);
-      ticks.push_back(next);
-      next += ((s - next) / n->period_ns + 1) * n->period_ns;  // the first tick strictly after s
-    }
+  if (!n || !n_scans) B2S_FAIL(B2S_ERR_BAD_PARAMS, "b2s_hector_node_process: null argument");
+  const int B = n->batch;
+  size_t T = 0;
+  bool too_many = false;
+  for (int b = 0; b < B; b++) {
+    if (n_scans[b] < 0) B2S_FAIL(B2S_ERR_BAD_PARAMS, "b2s_hector_node_process: negative scan count");
+    T += (size_t)n_scans[b];
+    too_many = too_many || n_scans[b] >= NODE_MAX_SCANS;
   }
-  n->rows.resize(16 * (size_t)n_scans);
-  int64_t counted = 0, updates = n->updates;  // flags of the call's scans [0, counted) are in `updates`
-  auto publish = [&](size_t k, const int8_t *payload) -> b2s_status {
-    const float *rows = n->io.h_rows;
-    for (; counted < cuts[k]; counted++) updates += rows[16 * (size_t)counted + 12] != 0.0f ? 1 : 0;
-    const int32_t rebuilt = map_gate(n, updates);
-    const uint32_t stamp[2] = {(uint32_t)(ticks[k] / NS), (uint32_t)(ticks[k] % NS)};
-    if (on_map) on_map(user, (int32_t)(n->scans + cuts[k]), stamp, &n->info, payload, rebuilt);
+  if (T > 0 && (!stamps || (!ranges && n->geom.n_ranges > 0)))
+    B2S_FAIL(B2S_ERR_BAD_PARAMS, "b2s_hector_node_process: null argument");
+  if (n->failed) B2S_FAIL(B2S_ERR_BAD_STATE, "b2s_hector_node_process: an earlier call failed partway; destroy the handle");
+  if (too_many) B2S_FAIL(B2S_ERR_TOO_LARGE, "b2s_hector_node_process: too many scans of one node in one call (split it)");
+  if (T == 0) return B2S_OK;
+  const HectorNodePlan plan = hector_node_plan(B, n_scans, stamps, n->clock.data(), n->period_ns.data());
+  n->rows.resize(16 * T);
+  std::vector<int64_t> updates = n->updates;  // node b's, through the rows handed to `publish` so far
+  auto publish = [&](int b, int k, const int8_t *payload, const float *rows, long long n_rows) -> b2s_status {
+    for (long long i = 0; i < n_rows; i++) updates[(size_t)b] += rows[16 * (size_t)i + 12] != 0.0f ? 1 : 0;
+    const int32_t rebuilt = map_gate(n, b, updates[(size_t)b]);
+    const int64_t tick = plan.ticks[(size_t)b][(size_t)k - 1];
+    const uint32_t stamp[2] = {(uint32_t)(tick / NS), (uint32_t)(tick % NS)};
+    if (on_map) on_map(user, b, (int32_t)(n->scans[(size_t)b] + plan.cuts[(size_t)b][(size_t)k - 1]), stamp, &n->info,
+                       payload, rebuilt);
     return B2S_OK;
   };
-  b2s_status st = hs_node_run(n->proc, n->io, n->geom, n->units.data(), n->cutoff, n->filter, n_scans, ranges, cuts,
-                              n->rows.data(), publish);
+  b2s_status st = hs_node_run(n->proc, n->io, n->geom, n->units.data(), n->cutoff, n->filters.data(), plan, n_scans,
+                              ranges, n->rows.data(), publish);
   if (st) {
-    // the processor, the maps handed out and the publish gate have moved, the schedule and the counters have not
+    // the processors, the maps handed out and the publish gates have moved, the schedules and the counters have not
     n->failed = true;
     return st;
   }
-  n->started = started;
-  n->next_tick_ns = next;
-  for (int i = 0; i < n_scans; i++) {
-    const float *r = n->rows.data() + 16 * (size_t)i;
-    const bool upd = r[12] != 0.0f;
-    n->updates += upd ? 1 : 0;
-    if (out_pose) std::memcpy(out_pose + 3 * (size_t)i, r, 3 * sizeof(float));
-    if (out_pose_msg) {
-      // PoseInfoContainer::update: position x / y, orientation w = cos(yaw * 0.5f), z = sin(yaw * 0.5f) (double calls)
-      double *m = out_pose_msg + 7 * (size_t)i;
-      const float half = r[2] * 0.5f;
-      m[0] = (double)r[0]; m[1] = (double)r[1]; m[2] = 0.0;
-      m[3] = 0.0; m[4] = 0.0; m[5] = sin((double)half); m[6] = cos((double)half);
+  n->clock = plan.after;
+  size_t i = 0;
+  for (int b = 0; b < B; b++) {
+    for (int j = 0; j < n_scans[b]; j++, i++) {
+      const float *r = n->rows.data() + 16 * i;
+      const bool upd = r[12] != 0.0f;
+      n->updates[(size_t)b] += upd ? 1 : 0;
+      if (out_pose) std::memcpy(out_pose + 3 * i, r, 3 * sizeof(float));
+      if (out_pose_msg) {
+        // PoseInfoContainer::update: position x / y, orientation w = cos(yaw * 0.5f), z = sin(yaw * 0.5f) (double calls)
+        double *m = out_pose_msg + 7 * i;
+        const float half = r[2] * 0.5f;
+        m[0] = (double)r[0]; m[1] = (double)r[1]; m[2] = 0.0;
+        m[3] = 0.0; m[4] = 0.0; m[5] = sin((double)half); m[6] = cos((double)half);
+      }
+      if (out_cov) {
+        const float *h = r + 3;  // row-major 3x3
+        double *c = out_cov + 36 * i;
+        for (int q = 0; q < 36; q++) c[q] = 0.0;
+        c[0] = (double)h[0]; c[7] = (double)h[4]; c[35] = (double)h[8];
+        c[1] = c[6] = (double)h[1];
+        c[5] = c[30] = (double)h[2];
+        c[11] = c[31] = (double)h[5];
+      }
+      if (out_map_updated) out_map_updated[i] = upd ? 1 : 0;
+      if (out_n_points) std::memcpy(out_n_points + i, r + 15, sizeof(int32_t));
     }
-    if (out_cov) {
-      const float *h = r + 3;  // row-major 3x3
-      double *c = out_cov + 36 * (size_t)i;
-      for (int q = 0; q < 36; q++) c[q] = 0.0;
-      c[0] = (double)h[0]; c[7] = (double)h[4]; c[35] = (double)h[8];
-      c[1] = c[6] = (double)h[1];
-      c[5] = c[30] = (double)h[2];
-      c[11] = c[31] = (double)h[5];
-    }
-    if (out_map_updated) out_map_updated[i] = upd ? 1 : 0;
-    if (out_n_points) std::memcpy(out_n_points + i, r + 15, sizeof(int32_t));
+    n->scans[(size_t)b] += n_scans[b];
   }
-  n->scans += n_scans;
+  return B2S_OK;
+}
+
+b2s_status b2s_hector_node_process(b2s_hector_node *n, int n_scans, const float *ranges, const uint32_t *stamps,
+                                   float *out_pose, double *out_pose_msg, double *out_cov, int32_t *out_map_updated,
+                                   int32_t *out_n_points, b2s_hector_node_map_fn on_map, void *user) {
+  if (n && n->batch != 1) B2S_FAIL(B2S_ERR_BAD_PARAMS, "b2s_hector_node_process: the handle has several nodes");
+  const int32_t count = n_scans;
+  SingleMapFn fn{on_map, user};
+  return b2s_hector_node_process_batch(n, &count, ranges, stamps, out_pose, out_pose_msg, out_cov, out_map_updated,
+                                       out_n_points, single_map, &fn);
+}
+
+b2s_status b2s_hector_node_publish_map_of(b2s_hector_node *n, int b, const uint32_t stamp[2],
+                                          b2s_hector_node_batch_map_fn on_map, void *user) {
+  if (!n || !stamp) B2S_FAIL(B2S_ERR_BAD_PARAMS, "b2s_hector_node_publish_map: null argument");
+  if (b < 0 || b >= n->batch) B2S_FAIL(B2S_ERR_BAD_PARAMS, "b2s_hector_node_publish_map_of: node index out of range");
+  if (n->failed) B2S_FAIL(B2S_ERR_BAD_STATE, "b2s_hector_node_publish_map: an earlier call failed partway; destroy the handle");
+  n->payload.resize((size_t)n->info.width * (size_t)n->info.height);
+  if (b2s_status st = b2s_hector_slam_copy_level_ros_of(n->proc, b, 0, n->payload.data())) return st;
+  const int32_t rebuilt = map_gate(n, b, n->updates[(size_t)b]);
+  if (on_map) on_map(user, b, (int32_t)n->scans[(size_t)b], stamp, &n->info, n->payload.data(), rebuilt);
   return B2S_OK;
 }
 
 b2s_status b2s_hector_node_publish_map(b2s_hector_node *n, const uint32_t stamp[2], b2s_hector_node_map_fn on_map,
                                        void *user) {
-  if (!n || !stamp) B2S_FAIL(B2S_ERR_BAD_PARAMS, "b2s_hector_node_publish_map: null argument");
-  if (n->failed) B2S_FAIL(B2S_ERR_BAD_STATE, "b2s_hector_node_publish_map: an earlier call failed partway; destroy the handle");
-  n->payload.resize((size_t)n->info.width * (size_t)n->info.height);
-  if (b2s_status st = b2s_hector_slam_copy_level_ros(n->proc, 0, n->payload.data())) return st;
-  const int32_t rebuilt = map_gate(n, n->updates);
-  if (on_map) on_map(user, (int32_t)n->scans, stamp, &n->info, n->payload.data(), rebuilt);
-  return B2S_OK;
+  if (n && n->batch != 1) B2S_FAIL(B2S_ERR_BAD_PARAMS, "b2s_hector_node_publish_map: the handle has several nodes");
+  SingleMapFn fn{on_map, user};
+  return b2s_hector_node_publish_map_of(n, 0, stamp, single_map, &fn);
 }
 
 }  // extern "C"

@@ -79,13 +79,14 @@ struct HectorNodeFilter {
 };
 
 // The node handle's staging for its map publishes (hector_node.cu owns it, hs_node_run in hector_slam.cu fills it): a
-// copy stream, two level-0 payload slots on the device and page-locked on the host, and the per-scan record rows
+// copy stream, two slots of level-0 payloads (one per node publishing before a part) on the device and page-locked on
+// the host, and the per-scan record rows
 struct HsNodeIo {
   Stream copy;
   Buf<int8_t> d_map[2];
   HostBuf<int8_t> h_map[2];
   Event converted[2], copied[2];
-  HostBuf<float> h_rows;  // [scans of the call][16]: a scan's row is here once a later publish's `copied` has fired
+  HostBuf<float> h_rows;  // [scans of the call][16], part-major: a part's rows are here once the next part's `copied` fired
 };
 
 // rosPointCloudToDataContainer (hector_slam.cc:331-358) on one laser-frame point with the full mount:

@@ -49,6 +49,7 @@
 #include "common.cuh"
 #include "glibc_math.cuh"
 #include "hector_grid.cuh"
+#include "hector_node_plan.cuh"
 #include "hector_scan.cuh"
 
 using namespace b2s;
@@ -291,7 +292,8 @@ __host__ __device__ inline size_t hs_smem_bytes(int cap) { return hs_terms_offse
 // MapRepMultiMap::matchData (:144-166) on every level, coarsest first, + the gate and the update parameters of
 // HectorSlamProcessor::update (:81-108), by ONE CTA for processor b.
 // Returns the gate's verdict (map update or not).
-template <bool EXACT, bool CLUSTER>
+// FIXED_ORIGO (k_hs_stream_node): the container's origo is the processor's own, already in st->origo[0], not C's.
+template <bool EXACT, bool CLUSTER, bool FIXED_ORIGO = false>
 __device__ bool hs_match_cta(const HsBatch &P, const HsCall &C, int b, unsigned char *smem, HsXchg *xc = nullptr,
                              uint32_t *xc_parity = nullptr) {
   static_assert(!(EXACT && CLUSTER), "the bit-exact sums are one sequential chain: nothing to split");
@@ -512,6 +514,7 @@ __device__ bool hs_match_cta(const HsBatch &P, const HsCall &C, int b, unsigned 
 #pragma unroll
       for (int q = 0; q < 9; q++) st->last_cov[q] = lcov[q];
     }
+    const float origo_x = FIXED_ORIGO ? st->origo[0][0] : C.origo_x, origo_y = FIXED_ORIGO ? st->origo[0][1] : C.origo_y;
     if (!C.map_without_matching) {
       st->n_matched = n_matched0 + 1;
       if (n > 0) {
@@ -519,14 +522,14 @@ __device__ bool hs_match_cta(const HsBatch &P, const HsCall &C, int b, unsigned 
         for (int l = 1; l < P.levels; l++) {
           factor *= 0.5f;
           st->n_pts[l] = n;
-          st->origo[l][0] = C.origo_x * factor; st->origo[l][1] = C.origo_y * factor;
+          st->origo[l][0] = origo_x * factor; st->origo[l][1] = origo_y * factor;
         }
       } else {
         for (int l = 1; l < P.levels; l++) st->n_pts[l] = 0;  // setFrom of an empty container
       }
     }
     st->n_pts[0] = n;
-    st->origo[0][0] = C.origo_x; st->origo[0][1] = C.origo_y;
+    st->origo[0][0] = origo_x; st->origo[0][1] = origo_y;
     st->last_match_pose[0] = est[0]; st->last_match_pose[1] = est[1]; st->last_match_pose[2] = est[2];
     if (C.carry) { C.carry[0] = est[0]; C.carry[1] = est[1]; C.carry[2] = est[2]; }
     const bool do_update = hs_pose_difference_larger_than(est, lup, P.min_dist, P.min_angle) ||
@@ -945,7 +948,7 @@ struct HsIngest {
   float range_min;
   double range_cutoff;       // projectLaser's cutoff (a negative one already replaced by range_max)
   HectorScanFilter filter;
-  HectorNodeFilter node;     // k_hs_stream_node's conversion (the full laser mount) instead of `filter`
+  const HectorNodeFilter *nodes;  // [B] device: k_hs_stream_node's conversion of each node (its full laser mount)
 };
 
 // The node's loop of processor b = blockIdx.x over its scans: match (hs_match_cta), then, if the gate opens, the mark
@@ -960,7 +963,9 @@ struct HsIngest {
 // base across rounds.  hs_match_cta then reads that row as its input and copies it onto itself: each element is read and
 // written back unchanged by the same thread, which is benign.
 // INGEST selects the conversion: HS_INGEST_YAW (k_hs_stream_batch<_, true>: hector_scan_beam, the mount as x, y, z, yaw)
-// or HS_INGEST_NODE (k_hs_stream_node: hector_node_beam, the mount's full basis, for b2s_hector_node_*).
+// or HS_INGEST_NODE (k_hs_stream_node: hector_node_beam with node b's filter I.nodes[b], the mount's full basis, and the
+// origo of that mount, for b2s_hector_node_*).  For HS_INGEST_NODE, F.first is one part of a node call: [B][2] =
+// (first scan, end scan) of node b, since a node's end inside a part is not the next node's begin.
 enum { HS_INGEST_NONE = 0, HS_INGEST_YAW = 1, HS_INGEST_NODE = 2 };
 template <bool EXACT, int INGEST>
 __device__ __forceinline__ void hs_stream_batch_body(const HsBatch &P, const HsFleet &F, unsigned char *hs_smem) {
@@ -969,7 +974,8 @@ __device__ __forceinline__ void hs_stream_batch_body(const HsBatch &P, const HsF
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   constexpr int NW = HS_THREADS / 32;
   HsState *st = P.state + b;
-  const long long s0 = F.first[b], s1 = F.first[b + 1];
+  constexpr bool NODE = INGEST == HS_INGEST_NODE;
+  const long long s0 = NODE ? F.first[2 * b] : F.first[b], s1 = NODE ? F.first[2 * b + 1] : F.first[b + 1];
   unsigned long long visits = 0;
   for (long long i = s0; i < s1; i++) {
     HsCall C;
@@ -987,7 +993,7 @@ __device__ __forceinline__ void hs_stream_batch_body(const HsBatch &P, const HsF
         if (j < nr) {
           const double2 u = I.units[j];
           if constexpr (INGEST == HS_INGEST_NODE)
-            keep = hector_node_beam(I.node, r[j], u.x, u.y, I.range_cutoff, I.range_min, q.x, q.y);
+            keep = hector_node_beam(I.nodes[b], r[j], u.x, u.y, I.range_cutoff, I.range_min, q.x, q.y);
           else
             keep = hector_scan_beam(I.filter, r[j], u.x, u.y, I.range_cutoff, I.range_min, q.x, q.y);
         }
@@ -1016,7 +1022,7 @@ __device__ __forceinline__ void hs_stream_batch_body(const HsBatch &P, const HsF
     }
     C.pts_stride = 0;
     C.hints = F.hints ? F.hints + 3 * i : (i > s0 ? s_last : (F.first_hints ? F.first_hints + 3 * (size_t)b : nullptr));
-    C.origo_x = F.origo_x; C.origo_y = F.origo_y;
+    C.origo_x = F.origo_x; C.origo_y = F.origo_y;  // (NODE: unused, hs_node_run set each processor's own)
     C.map_without_matching = F.map_without_matching;
     C.out = F.out + 16 * i;
     C.mailbox = nullptr;
@@ -1024,7 +1030,7 @@ __device__ __forceinline__ void hs_stream_batch_body(const HsBatch &P, const HsF
     C.tag = 0;
     C.carry = s_last;
     C.own_row = 1;
-    if (hs_match_cta<EXACT, false>(P, C, b, hs_smem)) {
+    if (hs_match_cta<EXACT, false, NODE>(P, C, b, hs_smem)) {
       const unsigned long long t0 = hs_now_ns();
       visits += hs_mark_pass(P, b, warp, NW, lane);  // (lane 0 carries the warp's count)
       __syncthreads();
@@ -1042,8 +1048,8 @@ __global__ void __launch_bounds__(HS_THREADS, 1) k_hs_stream_batch(HsBatch P, Hs
   hs_stream_batch_body<EXACT, INGEST ? HS_INGEST_YAW : HS_INGEST_NONE>(P, F, hs_smem);
 }
 
-// lesson4's HectorMappingRos (b2s_hector_node_*): k_hs_stream_batch's loop with the node's full-basis conversion, exact
-// mode, one processor (blockIdx.x = 0), over the scans F.first[0] ... F.first[1] - 1 of one part of a recording
+// lesson4's HectorMappingRos (b2s_hector_node_*): k_hs_stream_batch's loop with each node's full-basis conversion, exact
+// mode, one processor per CTA (node b = blockIdx.x), over node b's scans of one part of a node call
 __global__ void __launch_bounds__(HS_THREADS, 1) k_hs_stream_node(HsBatch P, HsFleet F) {
   extern __shared__ __align__(16) unsigned char hs_smem[];
   hs_stream_batch_body<true, HS_INGEST_NODE>(P, F, hs_smem);
@@ -1387,44 +1393,90 @@ void hs_node_map_info(const b2s_hector_slam *p, float &origin_x, float &origin_y
 
 float hs_scale_to_map(const b2s_hector_slam *p) { return p->P.l[0].tf.tw_lin; }  // GridMapBase::getScaleToMap of level 0
 
-// ---- lesson4's HectorMappingRos (hector_node.cu) over one part of a recording ----
-// The scans run in k_hs_stream_node launches split at the publish points.  Before the scan a publish precedes, level 0
-// is converted to its ROS payload on the processor's stream (k_hector_ros); a second stream copies it, with the record
-// rows of the scans before it, into page-locked memory while the next part's launch runs.  Two payload slots: a slot is
-// handed to on_map (in publish order) before it is converted into again.
+// ---- lesson4's HectorMappingRos (hector_node.cu): one node per processor, over one call ----
+// level 0 of the processors nodes[0 .. gridDim.y) -> their ROS payloads, back to back in `out`
+static __global__ void k_hector_ros_nodes(const float *__restrict__ lo, int cells, const int *__restrict__ nodes,
+                                          int8_t *__restrict__ out) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= cells) return;
+  out[(size_t)blockIdx.y * cells + i] = hector_ros_cell(lo[(size_t)nodes[blockIdx.y] * cells + i]);
+}
+
+// The call runs as the plan's parts (hector_node_plan.cuh), one k_hs_stream_node launch of B CTAs per part that has
+// scans, CTA b on node b's scans of the part.  Before part k >= 1, one k_hector_ros_nodes launch on the processor's
+// stream converts level 0 of every node publishing there into one slot of payloads; a second stream copies the slot,
+// with those nodes' record rows of part k - 1, into page-locked memory while part k's launch runs.  Two slots: a slot
+// is handed to on_map (part by part, nodes ascending inside a part) before it is converted into again.  on_map(b, k,
+// payload, rows, n) also gets node b's n record rows since its previous publish.  Rows are node-major throughout.
 b2s_status hs_node_run(b2s_hector_slam *p, HsNodeIo &io, const b2s_laser_scan_msg &geometry, const double *units,
-                       double range_cutoff, const HectorNodeFilter &filter, int n_scans, const float *ranges,
-                       const std::vector<int> &cuts, float *out_rows,
-                       const std::function<b2s_status(size_t, const int8_t *)> &on_map) {
-  const int nr = geometry.n_ranges;
+                       double range_cutoff, const HectorNodeFilter *filters, const HectorNodePlan &plan,
+                       const int32_t *n_scans, const float *ranges, float *out_rows,
+                       const std::function<b2s_status(int, int, const int8_t *, const float *, long long)> &on_map) {
+  const int nr = geometry.n_ranges, B = plan.batch, K = plan.n_parts;
   const size_t cells = (size_t)p->sx[0] * p->sy[0];
+  // parts [K][B] = node b's scans [first, end) of part k, node-major over the call
+  std::vector<long long> parts(2 * (size_t)K * B);
+  long long first = 0;
+  int longest = 0;
+  for (int b = 0; b < B; b++) {
+    for (int k = 0; k < K; k++) {
+      const size_t e = (size_t)k * B + b;
+      parts[2 * e] = first + plan.begin[e];
+      parts[2 * e + 1] = first + plan.end[e];
+    }
+    first += n_scans[b];
+    longest = std::max(longest, (int)n_scans[b]);
+  }
+  const size_t T = (size_t)first;
+  // the nodes publishing before part k: pub[pub0[k] .. pub0[k + 1]), those with k publishes or more, ascending
+  std::vector<int> pub;
+  std::vector<size_t> pub0((size_t)K + 1, 0);
+  size_t most = 0;
+  for (int k = 0; k < K; k++) {
+    for (int b = 0; k > 0 && b < B; b++)
+      if ((int)plan.cuts[(size_t)b].size() >= k) pub.push_back(b);
+    pub0[(size_t)k + 1] = pub.size();
+    most = std::max(most, pub0[(size_t)k + 1] - pub0[(size_t)k]);
+  }
   B2S_CUDA_CHECK(cudaSetDevice(p->device));
   b2s_status st = hs_wait_launch(p);
   if (st) return st;
-  if ((st = hs_reserve_epochs(p, (unsigned long long)n_scans))) return st;
-  B2S_CUDA_CHECK(io.h_rows.reserve(16 * (size_t)std::max(n_scans, 1)));
-  for (int k = 0; k < 2; k++) {
-    B2S_CUDA_CHECK(io.d_map[k].reserve(cells));
-    B2S_CUDA_CHECK(io.h_map[k].reserve(cells));
-  }
-  // part boundaries: 0, every publish point, n_scans
-  std::vector<long long> bounds(1, 0);
-  for (int c : cuts)
-    if (c > bounds.back()) bounds.push_back(c);
-  if (n_scans > bounds.back()) bounds.push_back(n_scans);
+  if ((st = hs_reserve_epochs(p, (unsigned long long)longest))) return st;  // per processor: its own scans
+  B2S_CUDA_CHECK(io.h_rows.reserve(16 * T));
+  if (most > 0)  // the first call that publishes allocates the slots; later calls reuse them
+    for (int s = 0; s < 2; s++) {
+      B2S_CUDA_CHECK(io.d_map[s].reserve(most * cells));
+      B2S_CUDA_CHECK(io.h_map[s].reserve(most * cells));
+    }
   AsyncBuf<float> d_ranges(p->stream), d_out(p->stream);
   AsyncBuf<double> d_unit(p->stream);
   AsyncBuf<HsIngest> d_ingest(p->stream);
-  AsyncBuf<long long> d_bounds(p->stream);
-  const size_t n_r = (size_t)n_scans * (size_t)nr;
+  AsyncBuf<HectorNodeFilter> d_filters(p->stream);
+  AsyncBuf<long long> d_parts(p->stream);
+  AsyncBuf<int> d_pub(p->stream);
+  const size_t n_r = T * (size_t)nr;
   B2S_CUDA_CHECK(d_ranges.alloc(std::max<size_t>(n_r, 1)));
   B2S_CUDA_CHECK(d_unit.alloc(2 * (size_t)std::max(nr, 1)));
   B2S_CUDA_CHECK(d_ingest.alloc(1));
-  B2S_CUDA_CHECK(d_bounds.alloc(bounds.size()));
-  B2S_CUDA_CHECK(d_out.alloc(16 * (size_t)std::max(n_scans, 1)));
+  B2S_CUDA_CHECK(d_filters.alloc((size_t)B));
+  B2S_CUDA_CHECK(d_parts.alloc(parts.size()));
+  B2S_CUDA_CHECK(d_pub.alloc(std::max<size_t>(pub.size(), 1)));
+  B2S_CUDA_CHECK(d_out.alloc(16 * std::max<size_t>(T, 1)));
   if (n_r > 0) B2S_CUDA_CHECK(cudaMemcpyAsync(d_ranges, ranges, sizeof(float) * n_r, cudaMemcpyHostToDevice, p->stream));
   if (nr > 0) B2S_CUDA_CHECK(cudaMemcpyAsync(d_unit, units, sizeof(double) * 2 * (size_t)nr, cudaMemcpyHostToDevice, p->stream));
-  B2S_CUDA_CHECK(cudaMemcpyAsync(d_bounds, bounds.data(), sizeof(long long) * bounds.size(), cudaMemcpyHostToDevice, p->stream));
+  // (pageable sources: staged before the calls return)
+  B2S_CUDA_CHECK(cudaMemcpyAsync(d_filters, filters, sizeof(HectorNodeFilter) * (size_t)B, cudaMemcpyHostToDevice, p->stream));
+  B2S_CUDA_CHECK(cudaMemcpyAsync(d_parts, parts.data(), sizeof(long long) * parts.size(), cudaMemcpyHostToDevice, p->stream));
+  if (!pub.empty()) B2S_CUDA_CHECK(cudaMemcpyAsync(d_pub, pub.data(), sizeof(int) * pub.size(), cudaMemcpyHostToDevice, p->stream));
+  // dataContainer.setOrigo (hector_slam.cc:329) of node b's mount, the same every scan: the processor's level-0 origo,
+  // which k_hs_stream_node's match reads (hs_match_cta<_, _, true>) instead of a per-CTA value held through the loop
+  std::vector<float> origo(2 * (size_t)B);
+  for (int b = 0; b < B; b++) {
+    origo[2 * (size_t)b] = (float)filters[b].mount.o[0] * filters[b].scale_to_map;
+    origo[2 * (size_t)b + 1] = (float)filters[b].mount.o[1] * filters[b].scale_to_map;
+  }
+  B2S_CUDA_CHECK(cudaMemcpy2DAsync(&p->d_state.p[0].origo[0][0], sizeof(HsState), origo.data(), 2 * sizeof(float),
+                                   2 * sizeof(float), (size_t)B, cudaMemcpyHostToDevice, p->stream));
   HsIngest I;
   std::memset(&I, 0, sizeof(I));
   I.ranges = d_ranges;
@@ -1432,8 +1484,8 @@ b2s_status hs_node_run(b2s_hector_slam *p, HsNodeIo &io, const b2s_laser_scan_ms
   I.n_ranges = nr;
   I.range_min = geometry.range_min;
   I.range_cutoff = range_cutoff;
-  I.node = filter;
-  B2S_CUDA_CHECK(cudaMemcpyAsync(d_ingest, &I, sizeof(HsIngest), cudaMemcpyHostToDevice, p->stream));  // (staged: pageable)
+  I.nodes = d_filters;
+  B2S_CUDA_CHECK(cudaMemcpyAsync(d_ingest, &I, sizeof(HsIngest), cudaMemcpyHostToDevice, p->stream));
   // the copy stream reads d_out: on every way out it is drained before the stream-ordered frees above
   struct DrainCopies {
     cudaStream_t s;
@@ -1442,53 +1494,58 @@ b2s_status hs_node_run(b2s_hector_slam *p, HsNodeIo &io, const b2s_laser_scan_ms
   HsFleet F;
   std::memset(&F, 0, sizeof(F));
   F.ingest = d_ingest;
-  F.origo_x = (float)filter.mount.o[0] * filter.scale_to_map;  // dataContainer.setOrigo (hector_slam.cc:329)
-  F.origo_y = (float)filter.mount.o[1] * filter.scale_to_map;
   F.out = d_out;
   const size_t smem = hs_smem_bytes(p->cap);
-  struct Pending { size_t k; int slot; };
+  struct Pending { int k, slot; };
   std::vector<Pending> pending;
-  size_t next_cut = 0, rows_copied = 0;
   int slot = 0;
   auto drain_one = [&]() -> b2s_status {
     const Pending q = pending.front();
     pending.erase(pending.begin());
     B2S_CUDA_CHECK(cudaEventSynchronize(io.copied[q.slot]));
-    return on_map(q.k, io.h_map[q.slot]);
+    for (size_t j = pub0[(size_t)q.k]; j < pub0[(size_t)q.k + 1]; j++) {
+      const long long *prev = parts.data() + 2 * ((size_t)(q.k - 1) * B + pub[j]);  // the rows before this publish
+      if (b2s_status s = on_map(pub[j], q.k, io.h_map[q.slot] + (j - pub0[(size_t)q.k]) * cells, io.h_rows + 16 * prev[0],
+                                prev[1] - prev[0]))
+        return s;
+    }
+    return B2S_OK;
   };
-  for (size_t c = 0; c + 1 < bounds.size(); c++) {  // every publish point lies in [0, n_scans): it starts a part
-    const long long a = bounds[c];
-    if (next_cut < cuts.size() && cuts[next_cut] == a) {  // the publish before scan a
+  for (int k = 0; k < K; k++) {
+    const size_t np = pub0[(size_t)k + 1] - pub0[(size_t)k];
+    if (np > 0) {  // the publishes before part k (k >= 1)
       if (pending.size() == 2) {
         if ((st = drain_one())) return st;
       }
-      k_hector_ros<<<ceil_div((long long)cells, 256), 256, 0, p->stream>>>(p->P.l[0].lo, (int)cells, io.d_map[slot]);
+      k_hector_ros_nodes<<<dim3((unsigned)ceil_div((long long)cells, 256), (unsigned)np), 256, 0, p->stream>>>(
+          p->P.l[0].lo, (int)cells, d_pub + pub0[(size_t)k], io.d_map[slot]);
       B2S_CUDA_CHECK(cudaGetLastError());
       B2S_CUDA_CHECK(cudaEventRecord(io.converted[slot], p->stream));
       B2S_CUDA_CHECK(cudaStreamWaitEvent(io.copy, io.converted[slot], 0));
-      B2S_CUDA_CHECK(cudaMemcpyAsync(io.h_map[slot], io.d_map[slot], cells, cudaMemcpyDeviceToHost, io.copy));
-      if ((size_t)a > rows_copied) {
-        B2S_CUDA_CHECK(cudaMemcpyAsync(io.h_rows + 16 * rows_copied, d_out + 16 * rows_copied,
-                                       sizeof(float) * 16 * ((size_t)a - rows_copied), cudaMemcpyDeviceToHost, io.copy));
-        rows_copied = (size_t)a;
+      B2S_CUDA_CHECK(cudaMemcpyAsync(io.h_map[slot], io.d_map[slot], np * cells, cudaMemcpyDeviceToHost, io.copy));
+      for (size_t j = pub0[(size_t)k]; j < pub0[(size_t)k + 1]; j++) {
+        const long long *prev = parts.data() + 2 * ((size_t)(k - 1) * B + pub[j]);
+        if (prev[1] > prev[0])
+          B2S_CUDA_CHECK(cudaMemcpyAsync(io.h_rows + 16 * prev[0], d_out + 16 * prev[0],
+                                         sizeof(float) * 16 * (size_t)(prev[1] - prev[0]), cudaMemcpyDeviceToHost, io.copy));
       }
       B2S_CUDA_CHECK(cudaEventRecord(io.copied[slot], io.copy));
-      pending.push_back(Pending{next_cut, slot});
+      pending.push_back(Pending{k, slot});
       slot ^= 1;
-      next_cut++;
     }
-    F.first = d_bounds + c;  // this part: scans bounds[c] ... bounds[c + 1] - 1
-    k_hs_stream_node<<<1, HS_THREADS, smem, p->stream>>>(p->P, F);
-    B2S_CUDA_CHECK(cudaGetLastError());
+    long long scans = 0;
+    for (int b = 0; b < B; b++) scans += parts[2 * ((size_t)k * B + b) + 1] - parts[2 * ((size_t)k * B + b)];
+    if (scans > 0) {
+      F.first = d_parts + 2 * (size_t)k * B;
+      k_hs_stream_node<<<B, HS_THREADS, smem, p->stream>>>(p->P, F);
+      B2S_CUDA_CHECK(cudaGetLastError());
+    }
   }
-  if ((size_t)n_scans > rows_copied)
-    B2S_CUDA_CHECK(cudaMemcpyAsync(io.h_rows + 16 * rows_copied, d_out + 16 * rows_copied,
-                                   sizeof(float) * 16 * ((size_t)n_scans - rows_copied), cudaMemcpyDeviceToHost, p->stream));
   while (!pending.empty())
     if ((st = drain_one())) return st;
+  B2S_CUDA_CHECK(cudaMemcpyAsync(out_rows, d_out, sizeof(float) * 16 * T, cudaMemcpyDeviceToHost, p->stream));
   B2S_CUDA_CHECK(cudaStreamSynchronize(io.copy));
   B2S_CUDA_CHECK(cudaStreamSynchronize(p->stream));
-  std::memcpy(out_rows, io.h_rows, sizeof(float) * 16 * (size_t)n_scans);
   return B2S_OK;
 }
 

@@ -29,6 +29,8 @@ class HectorNodeMapInfo(C.Structure):
 
 MAP_FN = C.CFUNCTYPE(None, C.c_void_p, C.c_int32, C.POINTER(C.c_uint32), C.POINTER(HectorNodeMapInfo),
                      C.POINTER(C.c_int8), C.c_int32)
+BATCH_MAP_FN = C.CFUNCTYPE(None, C.c_void_p, C.c_int32, C.c_int32, C.POINTER(C.c_uint32), C.POINTER(HectorNodeMapInfo),
+                           C.POINTER(C.c_int8), C.c_int32)
 
 # HectorMappingRos::InitParams (hector_slam.cc:119-162): ROS parameter -> (field, type, node default)
 _PARAMS = {
@@ -91,22 +93,41 @@ def _bind():
     L.b2s_hector_node_processor.restype = vp
     L.b2s_hector_node_process.argtypes = [vp, C.c_int, fp, C.POINTER(C.c_uint32), fp, dp, dp, ip, ip, MAP_FN, vp]
     L.b2s_hector_node_publish_map.argtypes = [vp, C.POINTER(C.c_uint32), MAP_FN, vp]
+    L.b2s_hector_node_create_batch.argtypes = [C.c_int, C.POINTER(HectorNodeParams), C.POINTER(LaserScanMsg), dp, C.c_int,
+                                               C.POINTER(vp)]
+    L.b2s_hector_node_process_batch.argtypes = [vp, ip, fp, C.POINTER(C.c_uint32), fp, dp, dp, ip, ip, BATCH_MAP_FN, vp]
+    L.b2s_hector_node_publish_map_of.argtypes = [vp, C.c_int, C.POINTER(C.c_uint32), BATCH_MAP_FN, vp]
     _bound = True
     return L
 
 
+def _map_dict(scan_index, stamp_p, info_p, payload_p, rebuilt):
+    i = info_p.contents
+    info = dict(origin_x=i.origin_x, origin_y=i.origin_y, resolution=i.resolution, width=i.width, height=i.height)
+    data = np.ctypeslib.as_array(payload_p, shape=(i.height * i.width,)).reshape(i.height, i.width).copy()
+    return dict(scan_index=int(scan_index), stamp=(int(stamp_p[0]), int(stamp_p[1])), info=info, payload=data,
+                rebuilt=bool(rebuilt))
+
+
 def _collector(maps, on_map):
     def cb(user, scan_index, stamp_p, info_p, payload_p, rebuilt):
-        i = info_p.contents
-        info = dict(origin_x=i.origin_x, origin_y=i.origin_y, resolution=i.resolution, width=i.width, height=i.height)
-        data = np.ctypeslib.as_array(payload_p, shape=(i.height * i.width,)).reshape(i.height, i.width).copy()
-        m = dict(scan_index=int(scan_index), stamp=(int(stamp_p[0]), int(stamp_p[1])), info=info, payload=data,
-                 rebuilt=bool(rebuilt))
+        m = _map_dict(scan_index, stamp_p, info_p, payload_p, rebuilt)
         if on_map is not None:
             on_map(m)
         else:
             maps.append(m)
     return MAP_FN(cb)
+
+
+def _batch_collector(maps, on_map):
+    """maps: one list per node; on_map(node, dict) instead when given"""
+    def cb(user, node, scan_index, stamp_p, info_p, payload_p, rebuilt):
+        m = _map_dict(scan_index, stamp_p, info_p, payload_p, rebuilt)
+        if on_map is not None:
+            on_map(int(node), m)
+        else:
+            maps[node].append(m)
+    return BATCH_MAP_FN(cb)
 
 
 class HectorNode:
@@ -166,3 +187,64 @@ class HectorNode:
             self.close()
         except Exception:
             pass
+
+
+class HectorNodeBatch:
+    """B HectorMappingRos nodes in one handle, one per recording or per setting (b2s_hector_node_create_batch): the
+    processor fields of every params set must be equal; mounts, range limits, z windows and periods may differ."""
+
+    def __init__(self, params_list, geometry: LaserScanMsg, mounts, device=0):
+        self.L = _bind()
+        self.h = C.c_void_p()
+        self.n_ranges = geometry.n_ranges
+        self.batch = len(params_list)
+        params = (HectorNodeParams * self.batch)(*params_list)
+        m = np.ascontiguousarray(mounts, np.float64)
+        assert m.shape == (self.batch, 7)
+        check(self.L.b2s_hector_node_create_batch(self.batch, params, C.byref(geometry),
+                                                  m.ctypes.data_as(C.POINTER(C.c_double)), device, C.byref(self.h)))
+        self.processor = C.c_void_p(self.L.b2s_hector_node_processor(self.h))
+
+    def process(self, ranges_list, stamps_list, on_map=None):
+        """ranges_list[b] [S_b][n] float32, stamps_list[b] [S_b][2] -> one dict per node, shaped as
+        HectorNode.process's.  Maps go to on_map(node, dict) in the call's order when given."""
+        counts = np.array([len(s) for s in stamps_list], np.int32)
+        assert len(counts) == self.batch and len(ranges_list) == self.batch
+        S = int(counts.sum())
+        r = np.zeros((S, self.n_ranges), np.float32)
+        s = np.zeros((S, 2), np.uint32)
+        at = np.concatenate([[0], np.cumsum(counts)])
+        for b in range(self.batch):
+            if counts[b]:
+                r[at[b]:at[b + 1]] = np.asarray(ranges_list[b], np.float32).reshape(counts[b], self.n_ranges)
+                s[at[b]:at[b + 1]] = np.asarray(stamps_list[b], np.uint32).reshape(counts[b], 2)
+        pose, msg, cov = np.zeros((S, 3), np.float32), np.zeros((S, 7)), np.zeros((S, 36))
+        upd, kept = np.zeros(S, np.int32), np.zeros(S, np.int32)
+        maps = [[] for _ in range(self.batch)]
+        fn = _batch_collector(maps, on_map)
+        ip, dp, fp = C.POINTER(C.c_int32), C.POINTER(C.c_double), C.POINTER(C.c_float)
+        check(self.L.b2s_hector_node_process_batch(self.h, counts.ctypes.data_as(ip), r.ctypes.data_as(fp),
+                                                   s.ctypes.data_as(C.POINTER(C.c_uint32)), pose.ctypes.data_as(fp),
+                                                   msg.ctypes.data_as(dp), cov.ctypes.data_as(dp),
+                                                   upd.ctypes.data_as(ip), kept.ctypes.data_as(ip), fn, None))
+        return [dict(pose=pose[at[b]:at[b + 1]], pose_msg=msg[at[b]:at[b + 1]], cov=cov[at[b]:at[b + 1]],
+                     map_updated=upd[at[b]:at[b + 1]].astype(bool), n_points=kept[at[b]:at[b + 1]], maps=maps[b])
+                for b in range(self.batch)]
+
+    def publish_map(self, b, stamp):
+        """node b's publishMap now, stamped (sec, nsec) -> the map dict"""
+        maps = [[] for _ in range(self.batch)]
+        st = (C.c_uint32 * 2)(*stamp)
+        check(self.L.b2s_hector_node_publish_map_of(self.h, b, st, _batch_collector(maps, None), None))
+        return maps[b][0]
+
+    def level_ros(self, b, level=0):
+        """Node b's processor level as a ROS payload (b2s_hector_slam_copy_level_ros_of)."""
+        dims, cl = (C.c_int * 2)(), C.c_float(0)
+        check(self.L.b2s_hector_slam_level_dims(self.processor, level, dims, C.byref(cl)))
+        out = np.zeros((dims[1], dims[0]), np.int8)
+        check(self.L.b2s_hector_slam_copy_level_ros_of(self.processor, b, level, out.ctypes.data_as(C.POINTER(C.c_int8))))
+        return out
+
+    close = HectorNode.close
+    __del__ = HectorNode.__del__

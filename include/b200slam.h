@@ -730,6 +730,42 @@ b2s_status b2s_hector_node_process(b2s_hector_node *node, int n_scans, const flo
 b2s_status b2s_hector_node_publish_map(b2s_hector_node *node, const uint32_t stamp[2], b2s_hector_node_map_fn on_map,
                                        void *user);
 
+/* Several nodes per handle, one per recording or per setting, run side by side on the device (one CTA per node).
+ * b2s_hector_node_create is this with batch = 1; on a handle with batch > 1, b2s_hector_node_process and
+ * b2s_hector_node_publish_map answer B2S_ERR_BAD_PARAMS.  b2s_hector_node_processor returns the batched processor:
+ * its _of getters read node b. */
+
+/* b2s_hector_node_map_fn with the node the map belongs to; scan_index counts that node's scans */
+typedef void (*b2s_hector_node_batch_map_fn)(void *user, int32_t node, int32_t scan_index, const uint32_t stamp[2],
+                                             const b2s_hector_node_map_info *info, const int8_t *payload,
+                                             int32_t rebuilt);
+
+/* params [batch], laser_mounts [batch][7]: one set per node, validated as b2s_hector_node_create validates its own
+ * (the refusal names the node).  The fields the processor holds once (map_resolution, map_size,
+ * map_multi_res_levels, map_start_x / _y, update_factor_free / _occupied, map_update_distance_thresh / _angle_thresh)
+ * must be equal in every set, else B2S_ERR_BAD_PARAMS; the mount, laser_min_dist / _max_dist, use_max_scan_range, the
+ * z window and map_pub_period may differ.  All nodes share one geometry.  B2S_ERR_TOO_LARGE for more than 65535 nodes. */
+b2s_status b2s_hector_node_create_batch(int batch, const b2s_hector_node_params *params,
+                                        const b2s_laser_scan_msg *geometry, const double *laser_mounts, int device,
+                                        b2s_hector_node **out);
+/* b2s_hector_node_process on every node at once: n_scans [batch] (0 leaves a node untouched, its schedule does not
+ * start), ranges / stamps / outputs node-major (node 0's scans first), as b2s_hector_slam_process_scans_batch.  Each
+ * node's maps reach on_map in its own publish order.  Across nodes the call runs in parts: part 0 holds every node's
+ * scans before its first publish in the call, part k >= 1 starts with the k-th publish of every node that has one; maps
+ * arrive part by part, and inside a part by ascending node.  Two calls over consecutive parts of every recording equal
+ * one call.  B2S_ERR_BAD_PARAMS (nothing written, nothing changed) for a NULL n_scans, a negative count, or NULL
+ * arrays with scans; B2S_ERR_TOO_LARGE for a node with 2^20 - 1 or more scans.  A failure after the call started marks
+ * the handle failed, as for b2s_hector_node_process.  The maps due before a part are converted on the device into one
+ * page-locked buffer per part, two parts in flight: 2 x (nodes publishing) x width x height bytes on each side,
+ * allocated by the first call that publishes and kept. */
+b2s_status b2s_hector_node_process_batch(b2s_hector_node *node, const int32_t *n_scans, const float *ranges,
+                                         const uint32_t *stamps, float *out_pose, double *out_pose_msg, double *out_cov,
+                                         int32_t *out_map_updated, int32_t *out_n_points,
+                                         b2s_hector_node_batch_map_fn on_map, void *user);
+/* b2s_hector_node_publish_map of node b (0 <= b < batch): shares node b's update-index gate, leaves the others' */
+b2s_status b2s_hector_node_publish_map_of(b2s_hector_node *node, int b, const uint32_t stamp[2],
+                                          b2s_hector_node_batch_map_fn on_map, void *user);
+
 /* ---------------------------------------------------------------- K2b: GMapping hit/visit map */
 
 typedef struct b2s_gmap b2s_gmap; /* opaque: replaces GMapping::ScanMatcherMap (gmapping.cc:135) */
