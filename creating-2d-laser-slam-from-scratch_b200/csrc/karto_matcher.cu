@@ -20,6 +20,7 @@
 //   k_add_scans_seq    the same, sequential, when an off-centre smear value reaches 100 (order-dependent) or a base
 //                      scan does not fit in k_add_scan's shared memory
 //   k_grid_sat         per-match summed-area table of the grid's non-empty 4x4 blocks
+//   k_grid_pool        per-match 4x4 max-pooled grid of the angle-pruning bound
 //   k_bases            candidate lattice -> flat base indices; flags irregular and out-of-grid lattices
 //   k_offsets          per-angle lookup tables                                         (fp64 -> i32)
 //   k_offsets_sorted   window kernel's lists: window origins grouped by row band, byte alignment and interior /
@@ -28,6 +29,9 @@
 //                      one warp per (angle, 32x32 candidate tile), one lane per candidate row; each 32-bit
 //                      shared-memory word feeds 4 adjacent-x candidates (byte-permute into packed u16
 //                      accumulators)                                                    (int, issue bound)
+//   k_sweep_bound, k_prune_probe, k_prune_select
+//                      angle pruning: an upper bound of every angle's responses from the pooled grid, an exact probe
+//                      of the most promising angles, then k_sweep_window on only the angles that can matter
 //   k_sweep_generic    any lattice / any grid size: one warp per (x,y) candidate, lanes over beams,
 //                      gathers from global memory through L1/L2
 //   k_reduce           penalties, best response, tie-averaged pose, positional covariance (fp64, one CTA per match);
@@ -141,8 +145,15 @@ struct b2s_matcher {
   Buf<uint16_t> d_sat;  // [B][(sby+1)(sbx+1)] block summed-area tables of the grids
   int sbx = 0, sby = 0;
   bool sat_valid = false;
-  Buf<unsigned long long> d_stats;      // [0] beam-angle pairs dropped as empty windows in the last sweep
+  Buf<unsigned long long> d_stats;      // [0] beam-angle pairs dropped as empty windows, [1] angles pruned, last sweep
   HostBuf<unsigned long long> h_stats;  // pinned copy, read back with the results
+  Buf<uint8_t> d_pools;                 // [B][pool_pitch] 4x4 max-pooled grids (k_grid_pool), when they fit (pool_fits)
+  Buf<double> d_ubr;                    // [B][nA] angle bounds of a pruned sweep
+  Buf<int32_t> d_angles, d_n_angles;    // [B][nA], [B]: the angle lists of a pruned sweep's two exact passes
+  Buf<uint8_t> d_keep;                  // [B][nA] angles a pruned sweep swept
+  SweepPlan last_plan;                  // of the last sweep
+  bool last_pruned = false;             // the last sweep skipped angles: get_response_sums sweeps them first
+  double last_pruned_frac = 0.0;
   bool pending = false;                   // a correlate_scan_begin awaits its _end
   int pending_batch = 0;                  // batch size that _begin enqueued
   double last_empty_frac = 0.0;
@@ -534,6 +545,34 @@ __global__ void __launch_bounds__(256)
   for (int i = threadIdx.x; i < (by + 1) * W; i += blockDim.x) out[i] = (uint16_t)s_sat[i];  // < 65536 blocks (checked by the host)
 }
 
+// ----------------------------------------------------------------------------------------------
+// k_grid_pool: per match, the 4x4 max-pooled grid of k_sweep_bound (layout: pool_lead / pool_pitch in
+// karto_sweep_plan.cuh).  The pooling is in FLAT index space, rows wrapping exactly as a candidate's `base + offset`
+// does, so the pooled byte at a block's corner is at least every byte a candidate of that block reads.  One thread
+// per 4 output bytes; grid bytes outside [0, data_size) count as 0.  grid(ceil(pool_pitch / 1024), B), 256 threads.
+// ----------------------------------------------------------------------------------------------
+__global__ void __launch_bounds__(256)
+    k_grid_pool(const uint8_t *__restrict__ grids, size_t grid_pitch, int data_size, int width_step,
+                int lead, uint8_t *__restrict__ pools, size_t pitch) {
+  const int b = blockIdx.y;
+  const int j4 = blockIdx.x * blockDim.x + threadIdx.x;
+  if ((size_t)j4 * 4 >= pitch) return;
+  const uint8_t *grid = grids + (size_t)b * grid_pitch;
+  const int f = 4 * j4 - lead;  // a multiple of 4, as are width_step and data_size
+  auto word = [&](int r) { return (r >= 0 && r < data_size) ? __ldg(reinterpret_cast<const uint32_t *>(grid + r)) : 0u; };
+  uint32_t m = 0;
+#pragma unroll
+  for (int dy = 0; dy < 4; dy++) {
+    const int r = f + dy * width_step;
+    const uint32_t w0 = word(r), w1 = word(r + 4);
+    // byte t of the result = max of bytes t..t+3 of the 8 bytes w1:w0
+    const uint32_t a = __vmaxu4(w0, __funnelshift_r(w0, w1, 8));
+    const uint32_t c = __vmaxu4(__funnelshift_r(w0, w1, 16), __funnelshift_r(w0, w1, 24));
+    m = __vmaxu4(m, __vmaxu4(a, c));
+  }
+  reinterpret_cast<uint32_t *>(pools + (size_t)b * pitch)[j4] = m;
+}
+
 // One block per (match, chunk of OFF_CHUNK angles): window origins grouped as [I0 I1 I2 I3 E0 E1 E2 E3] (I = interior,
 // E = edge, index = a & 3), every group a multiple of 4 long (an interior group donates its 0..3 surplus beams to its edge
 // group; edge groups are padded with far-negative sentinels of the same alignment).  counts[8] holds the group lengths.
@@ -871,6 +910,7 @@ struct ReduceArgs {
   const double *glob_best;
   double *tie_out;
   const double *tie_in;
+  const uint8_t *keep;  // [B][na] angles swept by a pruned sweep (nullptr: every angle); the others read as 0
 };
 
 
@@ -880,7 +920,9 @@ __global__ void __launch_bounds__(WIN_THREADS, 1)
                    const int32_t *__restrict__ lists, const int32_t *__restrict__ counts,
                    const int32_t *__restrict__ starts, const int32_t *__restrict__ flags, int batch, int n, int na,
                    int nx, int ny, int width_step, int32_t *__restrict__ sums, int *__restrict__ work_counter,
-                   int band_rows, int nbands, int band_bytes, int neg_bands) {
+                   int band_rows, int nbands, int band_bytes, int neg_bands, const int32_t *__restrict__ angles,
+                   const int32_t *__restrict__ n_angles) {
+  // angles != nullptr (a pruned sweep, nbands == 1): match b sweeps only the n_angles[b] angles angles[b * na + ...].
   // Grids larger than shared memory are swept in `nbands` row bands: a work unit is (match, band, 32-row candidate
   // tile); the image holds the rows that tile of a window whose ORIGIN lies in the band can touch (band_rows +
   // STRIDE * 31 + 2), k_offsets_sorted grouped the beams by the band of their origin (bands [0, neg_bands) hold origins
@@ -896,7 +938,6 @@ __global__ void __launch_bounds__(WIN_THREADS, 1)
   constexpr int CPT = 32 / STRIDE;  // candidates per tile row (a tile row is always 32 bytes)
   const int tiles_x = (nx + CPT - 1) / CPT, tiles_y = (ny + 31) >> 5;
   const int unit_tiles_y = nbands > 1 ? tiles_y : 1;        // banded: one row tile per unit
-  const int items = na * tiles_x * (nbands > 1 ? 1 : tiles_y);
   // word rotation of this lane (see win_load): lanes whose rows start in the same bank get different rotations
   int hi_half = lane >> 4;
   int loff[8];
@@ -928,10 +969,12 @@ __global__ void __launch_bounds__(WIN_THREADS, 1)
     if (unit >= batch * nbands * unit_tiles_y) break;
     const int b = unit / (nbands * unit_tiles_y), band = (unit / unit_tiles_y) % nbands, unit_ty = unit % unit_tiles_y;
     const int f = flags[b];
-    if ((f & 2) || !(f & 1)) {  // out-of-range lattice (error) or irregular lattice (generic kernel takes it)
+    const int na_b = angles ? n_angles[b] : na;
+    if ((f & 2) || !(f & 1) || na_b == 0) {  // out-of-range lattice (error), irregular lattice (generic kernel takes it)
       __syncthreads();
       continue;
     }
+    const int items = na_b * tiles_x * (nbands > 1 ? 1 : tiles_y);
     // first / one-past-last grid row of this unit's image (the whole grid when nbands == 1)
     const int row0 = (band - neg_bands) * band_rows + STRIDE * unit_ty * 32;
     const int lo_row = max(row0, 0);
@@ -971,6 +1014,7 @@ __global__ void __launch_bounds__(WIN_THREADS, 1)
         k = item / tiles_x; tx = item % tiles_x; ty = unit_ty;
       } else {
         k = item / (tiles_x * tiles_y);
+        if (angles) k = angles[(size_t)b * na + k];
         const int t = item % (tiles_x * tiles_y);
         ty = t / tiles_x; tx = t % tiles_x;
       }
@@ -1046,6 +1090,217 @@ __device__ __forceinline__ float red_fscore(int32_t isum, float apf_k, float dpf
   return (float)isum * apf_k * dpf;
 }
 
+// ----------------------------------------------------------------------------------------------
+// Angle pruning (SweepPlan::prune: one 32 x 32 stride-1 tile, the whole grid in shared memory, a whole search).
+//
+// CorrelateScan needs exact responses only for the best candidate, its DoubleEqual ties (1e-6) and the per-cell
+// maxima that reach best - 0.1 (the only cells ComputePositionalCovariance reads, Mapper.cpp:586).  A candidate whose
+// response is below best - 0.1 is none of these, and leaving it out cannot lower a cell maximum that reaches best - 0.1.
+// So an angle may be skipped when an upper bound of all its responses is below L - 0.1 for some lower bound L <= best:
+//   k_sweep_bound   UBr(k) = max over 8 x 8 blocks of 4 x 4 candidates of
+//                   (SUM_beams P[a_i + block corner]) / (N * 100) * (max distance penalty of the block * anglePenalty(k)),
+//                   P the 4x4 max-pooled grid (k_grid_pool), summed over the same beam lists the exact sweep uses
+//                   (beams dropped as empty windows add 0 everywhere).  Same fp64 operations as candidate_response, so
+//                   UBr(k) >= every response of angle k.
+//   k_prune_probe   the PRUNE_PROBE angles with the largest UBr are swept exactly (k_sweep_window on an angle list);
+//   k_prune_select  L = the largest exact response among them (a real candidate, so L <= best); every other angle is
+//                   swept iff UBr(k) >= L - 0.1 - 1e-9.  When L - 0.1 is near 0 (within the 1e-6 band in which a
+//                   response is not penalised, Mapper.cpp:399) every angle is swept.
+// k_reduce reads 0 for the angles never swept; the response volume is completed on request (get_response_sums).
+// ----------------------------------------------------------------------------------------------
+template <bool CHECK>
+__device__ __forceinline__ void bound_beams(const uint8_t *__restrict__ sp, const int32_t *__restrict__ list, int count,
+                                            int lane, int off_a, int off_b, uint32_t lead, uint32_t limit,
+                                            int32_t *__restrict__ s_off, uint32_t &ua, uint32_t &ub) {
+  for (int ib = 0; ib < count; ib += 32) {
+    const int cnt = min(32, count - ib);  // a multiple of 4
+    __syncwarp();
+    s_off[lane] = (lane < cnt) ? __ldg(list + ib + lane) : 0;
+    __syncwarp();
+    for (int j = 0; j < cnt; j += 4) {
+      const int4 a4 = *reinterpret_cast<const int4 *>(s_off + j);
+      const int32_t as[4] = {a4.x, a4.y, a4.z, a4.w};
+#pragma unroll
+      for (int q = 0; q < 4; q++) {
+        if (CHECK) {  // flat index a + corner, modulo 2^32 like the reference's base + offset; P is 0 outside
+          const uint32_t fa = (uint32_t)as[q] + (uint32_t)off_a, fb = (uint32_t)as[q] + (uint32_t)off_b;
+          ua += (fa + lead < limit) ? sp[(int32_t)fa] : 0u;
+          ub += (fb + lead < limit) ? sp[(int32_t)fb] : 0u;
+        } else {
+          ua += sp[as[q] + off_a];
+          ub += sp[as[q] + off_b];
+        }
+      }
+    }
+  }
+}
+
+// One persistent CTA per match at a time (like k_sweep_window): the pooled image is staged by TMA, warps take angles,
+// lane L owns blocks (L / 8, L % 8) and (L / 8 + 4, L % 8).  ubr[b][k] = UBr(k) (-1 for a match the window kernel
+// does not sweep).
+__global__ void __launch_bounds__(WIN_THREADS, 1)
+    k_sweep_bound(const uint8_t *__restrict__ pools, size_t pool_pitch_, int pool_bytes_, int lead,
+                  const int32_t *__restrict__ lists, const int32_t *__restrict__ counts,
+                  const int32_t *__restrict__ starts, const int32_t *__restrict__ flags,
+                  const double *__restrict__ centers, b2s_matcher_params p, b2s_search s, int batch, int n, int na,
+                  int nx, int ny, int width_step, int data_size, double *__restrict__ ubr, int *__restrict__ work_counter) {
+  extern __shared__ __align__(128) unsigned char smem[];  // [WIN_GUARD zeros][pooled image][WIN_GUARD zeros]
+  __shared__ uint64_t bar;
+  __shared__ int s_unit;
+  __shared__ __align__(16) int32_t s_offsets[WIN_THREADS / 32][32];
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  int32_t *s_off = s_offsets[warp];
+  const bool pen = s.do_penalize != 0;
+  // the largest distance penalty of the candidates of block (by, bx), as k_reduce computes sq and candidate_response
+  // the penalty (-1: the block holds no candidate)
+  auto block_dpen = [&](int by, int bx) {
+    double mx = -1.0;
+    for (int iy = 4 * by; iy < min(4 * by + 4, ny); iy++)
+      for (int ix = 4 * bx; ix < min(4 * bx + 4, nx); ix++) {
+        const double y = -s.offset_y + (double)(uint32_t)iy * s.res_y, x = -s.offset_x + (double)(uint32_t)ix * s.res_x;
+        const double sq = x * x + y * y;
+        mx = dmax(mx, pen ? dmax(1.0 - (DISTANCE_PENALTY_GAIN * sq / p.distance_variance_penalty), p.minimum_distance_penalty) : 1.0);
+      }
+    return mx;
+  };
+  const double dpen_a = block_dpen(lane >> 3, lane & 7), dpen_b = block_dpen((lane >> 3) + 4, lane & 7);
+  for (int i = threadIdx.x; i < WIN_GUARD / 4; i += blockDim.x) reinterpret_cast<uint32_t *>(smem)[i] = 0;
+  if (threadIdx.x == 0) {
+    mbar_init(&bar, 1);
+    fence_mbar_init();
+  }
+  __syncthreads();
+  const int off_a = 4 * (lane >> 3) * width_step + 4 * (lane & 7), off_b = off_a + 16 * width_step;
+  const double D = (double)((uint32_t)n * (uint32_t)GRID_OCCUPIED);
+  const int list_cap = n + LIST_PAD;
+  const uint8_t *sp = smem + WIN_GUARD + lead;  // grid flat index 0
+  uint32_t parity = 0;
+  while (true) {
+    if (threadIdx.x == 0) s_unit = atomicAdd(work_counter, 1);
+    __syncthreads();
+    const int b = s_unit;
+    if (b >= batch) break;
+    const int f = flags[b];
+    if ((f & 2) || !(f & 1)) {
+      for (int k = threadIdx.x; k < na; k += blockDim.x) ubr[(size_t)b * na + k] = -1.0;
+      __syncthreads();
+      continue;
+    }
+    if (threadIdx.x == 0) {
+      fence_proxy_async();
+      mbar_expect_tx(&bar, (uint32_t)pool_bytes_);
+      const uint8_t *src = pools + (size_t)b * pool_pitch_;
+      for (int off = 0; off < pool_bytes_; off += 32768)
+        bulk_g2s(smem + WIN_GUARD + off, src + off, (uint32_t)min(32768, pool_bytes_ - off), &bar);
+    }
+    if (threadIdx.x < WIN_GUARD / 4) reinterpret_cast<uint32_t *>(smem + WIN_GUARD + pool_bytes_)[threadIdx.x] = 0;
+    mbar_wait(&bar, parity);
+    parity ^= 1;
+    __syncthreads();
+    const double ch = centers[3 * b + 2];
+    for (int k = warp; k < na; k += WIN_THREADS / 32) {
+      const int32_t *list = lists + ((size_t)b * na + k) * list_cap;
+      const int32_t *cn = counts + ((size_t)b * na + k) * 8;
+      const int32_t *sg = starts + ((size_t)b * na + k) * 8;
+      // groups I0..I3 E0..E3 are contiguous: interior beams [0, sg[4]), edge beams after them.  Interior windows lie
+      // within WIN_GUARD - 16 bytes of the grid, so every corner they read is inside the staged image.
+      const int n_int = sg[4], n_edge = sg[7] + cn[7] - sg[4];
+      uint32_t ua = 0, ub = 0;
+      bound_beams<false>(sp, list, n_int, lane, off_a, off_b, lead, lead + data_size, s_off, ua, ub);
+      bound_beams<true>(sp, list + n_int, n_edge, lane, off_a, off_b, lead, lead + data_size, s_off, ua, ub);
+      // candidate_response's operations, with the block's largest sum and largest distance penalty
+      const double angle = (ch - s.angle_offset) + (double)(uint32_t)k * s.angle_res;
+      double apen = 1.0;
+      if (pen) {
+        const double sq_a = (angle - ch) * (angle - ch);
+        apen = dmax(1.0 - (ANGLE_PENALTY_GAIN * sq_a / p.angle_variance_penalty), p.minimum_angle_penalty);
+      }
+      double r = -1.0;
+      if (dpen_a >= 0.0) r = dmax(r, pen ? ((double)ua / D) * (dpen_a * apen) : (double)ua / D);
+      if (dpen_b >= 0.0) r = dmax(r, pen ? ((double)ub / D) * (dpen_b * apen) : (double)ub / D);
+#pragma unroll
+      for (int d = 16; d > 0; d >>= 1) r = dmax(r, __shfl_xor_sync(0xffffffffu, r, d));
+      if (lane == 0) ubr[(size_t)b * na + k] = r;
+    }
+    __syncthreads();  // everyone is done with the image before the next match's copy is issued
+  }
+}
+
+// The PRUNE_PROBE angles with the largest bounds (ties: lower index first) become match b's first angle list; keep[b][k]
+// marks the angles that will have been swept.  A match the window kernel does not sweep gets an empty list and an
+// all-ones mask (the generic kernel fills its whole volume).  One CTA per match.
+__global__ void __launch_bounds__(256)
+    k_prune_probe(const double *__restrict__ ubr, const int32_t *__restrict__ flags, int na,
+                  int32_t *__restrict__ angles, int32_t *__restrict__ n_angles, uint8_t *__restrict__ keep) {
+  const int b = blockIdx.x;
+  __shared__ double s_u[PRUNE_MAX_ANGLES];
+  const int f = flags[b];
+  const bool swept = !(f & 2) && (f & 1);
+  for (int k = threadIdx.x; k < na; k += blockDim.x) s_u[k] = ubr[(size_t)b * na + k];
+  __syncthreads();
+  const int T = min(PRUNE_PROBE, na);
+  for (int k = threadIdx.x; k < na; k += blockDim.x) {
+    const double u = s_u[k];
+    int rank = 0;
+    for (int j = 0; j < na; j++) rank += (s_u[j] > u) || (s_u[j] == u && j < k);
+    if (swept && rank < T) angles[(size_t)b * na + rank] = k;
+    keep[(size_t)b * na + k] = !swept || rank < T;
+  }
+  if (threadIdx.x == 0) n_angles[b] = swept ? T : 0;
+}
+
+// L from the probe's exact sums, then match b's second angle list: the angles not probed whose bound reaches
+// L - 0.1 - 1e-9.  pruned_total += the angles left out.  One CTA per match.
+__global__ void __launch_bounds__(256)
+    k_prune_select(const int32_t *__restrict__ sums, const double *__restrict__ ubr, const double *__restrict__ centers,
+                   const int32_t *__restrict__ flags, b2s_matcher_params p, b2s_search s, int n, int nx, int ny, int na,
+                   int32_t *__restrict__ angles, int32_t *__restrict__ n_angles, uint8_t *__restrict__ keep,
+                   unsigned long long *__restrict__ pruned_total) {
+  const int b = blockIdx.x;
+  const int f = flags[b];
+  if ((f & 2) || !(f & 1)) return;  // n_angles[b] is still 0, keep[b] all ones
+  __shared__ int32_t s_probe[PRUNE_PROBE];
+  __shared__ double s_red[256];
+  __shared__ int s_cnt;
+  const int T = n_angles[b], ncell = nx * ny;
+  if (threadIdx.x < T) s_probe[threadIdx.x] = angles[(size_t)b * na + threadIdx.x];
+  if (threadIdx.x == 0) s_cnt = 0;
+  __syncthreads();
+  const bool pen = s.do_penalize != 0;
+  const double ch = centers[3 * b + 2];
+  const double start_a = ch - s.angle_offset;
+  double L = -1.0;
+  for (int t = threadIdx.x; t < T * ncell; t += blockDim.x) {
+    const int k = s_probe[t / ncell], c = t % ncell;
+    const int iy = c / nx, ix = c % nx;
+    const double y = -s.offset_y + (double)(uint32_t)iy * s.res_y, x = -s.offset_x + (double)(uint32_t)ix * s.res_x;
+    const double angle = start_a + (double)(uint32_t)k * s.angle_res;
+    L = dmax(L, candidate_response(sums[((size_t)b * na + k) * ncell + c], n, pen, x * x + y * y, angle, ch, p));
+  }
+  s_red[threadIdx.x] = L;
+  __syncthreads();
+  for (int d = 128; d > 0; d >>= 1) {
+    if (threadIdx.x < d) s_red[threadIdx.x] = dmax(s_red[threadIdx.x], s_red[threadIdx.x + d]);
+    __syncthreads();
+  }
+  L = s_red[0];
+  const bool all = !(L - 0.1 > 1.0e-6);
+  const double cut = L - 0.1 - 1.0e-9;
+  int pruned = 0;
+  for (int k = threadIdx.x; k < na; k += blockDim.x) {
+    if (keep[(size_t)b * na + k]) continue;  // probed
+    if (all || ubr[(size_t)b * na + k] >= cut) {
+      angles[(size_t)b * na + atomicAdd(&s_cnt, 1)] = k;
+      keep[(size_t)b * na + k] = 1;
+    } else {
+      pruned++;
+    }
+  }
+  if (pruned) atomicAdd(pruned_total, (unsigned long long)pruned);
+  __syncthreads();
+  if (threadIdx.x == 0) n_angles[b] = s_cnt;
+}
+
 __global__ void __launch_bounds__(RED_THREADS, 2) k_reduce(ReduceArgs A) {
   const int b = blockIdx.x;
   const int32_t *sums = A.sums;
@@ -1087,6 +1342,13 @@ __global__ void __launch_bounds__(RED_THREADS, 2) k_reduce(ReduceArgs A) {
   __shared__ int sorted[RED_MAX_TIES];
   __shared__ double s_best;
   __shared__ double s_mean[3];
+  __shared__ uint8_t s_keep[PRUNE_MAX_ANGLES];
+  const bool masked = A.keep != nullptr;  // only with na <= PRUNE_MAX_ANGLES
+  for (int k = tid; k < na && masked; k += RED_THREADS) s_keep[k] = A.keep[(size_t)b * na + k];
+  // the sum of candidate c at angle k; an angle a pruned sweep skipped holds no candidate that can matter: 0
+  auto load_sum = [&](int k, int c) -> int32_t {
+    return (k < na && (!masked || s_keep[k])) ? __ldcg(bs + (size_t)k * ncell + c) : 0;
+  };
   if (tid == 0) { s_err = 0; s_count = 0; }
   if (!s.fine && phase <= REDUCE_SPLIT_BEST)
     for (int i = tid; i < pstep * g.search_side; i += RED_THREADS) probs[i] = 0.0;  // Clear (Mapper.cpp:329)
@@ -1131,7 +1393,7 @@ __global__ void __launch_bounds__(RED_THREADS, 2) k_reduce(ReduceArgs A) {
       for (int k0 = 0; k0 < na; k0 += RED_UNROLL) {
         int32_t v[RED_UNROLL];
 #pragma unroll
-        for (int u = 0; u < RED_UNROLL; u++) v[u] = (k0 + u < na) ? __ldcg(bs + (size_t)(k0 + u) * ncell + c) : 0;
+        for (int u = 0; u < RED_UNROLL; u++) v[u] = load_sum(k0 + u, c);
 #pragma unroll
         for (int u = 0; u < RED_UNROLL; u++) {
           if (k0 + u >= na) continue;
@@ -1158,7 +1420,7 @@ __global__ void __launch_bounds__(RED_THREADS, 2) k_reduce(ReduceArgs A) {
         for (int k0 = 0; k0 < na; k0 += RED_UNROLL) {
           int32_t v[RED_UNROLL];
 #pragma unroll
-          for (int u = 0; u < RED_UNROLL; u++) v[u] = (k0 + u < na) ? __ldcg(bs + (size_t)(k0 + u) * ncell + c) : 0;
+          for (int u = 0; u < RED_UNROLL; u++) v[u] = load_sum(k0 + u, c);
 #pragma unroll
           for (int u = 0; u < RED_UNROLL; u++) {
             if (k0 + u >= na) continue;
@@ -1174,7 +1436,7 @@ __global__ void __launch_bounds__(RED_THREADS, 2) k_reduce(ReduceArgs A) {
     } else {
       for (int k = 0; k < na; k++) {
         const double angle = start_a + (double)(uint32_t)(k_first + k) * s.angle_res;
-        cell_best = dmax(cell_best, candidate_response(__ldcg(bs + (size_t)k * ncell + c), n, pen, sq, angle, ch, p));
+        cell_best = dmax(cell_best, candidate_response(load_sum(k, c), n, pen, sq, angle, ch, p));
       }
     }
     best = dmax(best, cell_best);
@@ -1220,7 +1482,7 @@ __global__ void __launch_bounds__(RED_THREADS, 2) k_reduce(ReduceArgs A) {
     for (int k0 = 0; k0 < na; k0 += RED_UNROLL) {
       int32_t v[RED_UNROLL];
 #pragma unroll
-      for (int u = 0; u < RED_UNROLL; u++) v[u] = (k0 + u < na) ? __ldcg(bs + (size_t)(k0 + u) * ncell + c) : 0;
+      for (int u = 0; u < RED_UNROLL; u++) v[u] = load_sum(k0 + u, c);
 #pragma unroll
       for (int u = 0; u < RED_UNROLL; u++) {
         const int k = k0 + u;
@@ -1500,6 +1762,7 @@ static void read_sweep_ms(b2s_matcher *m) {
 
 static b2s_status run_correlate(b2s_matcher *m, const b2s_search *s, int k_first = 0, int na_override = -1,
                                 ReducePhase phase = REDUCE_WHOLE);
+static b2s_status launch_window(b2s_matcher *m, const SweepPlan &pl, const int32_t *angles);
 
 // (re)build the per-match block summed-area tables after the grids changed
 static b2s_status build_sat(b2s_matcher *m) {
@@ -1510,6 +1773,16 @@ static b2s_status build_sat(b2s_matcher *m) {
   k_grid_sat<<<m->batch, 256, sm, m->stream>>>(m->d_grids, m->grid_pitch, m->g.width_step, m->g.height, m->sbx, m->sby, m->d_sat);
   B2S_CUDA_CHECK(cudaGetLastError());
   m->sat_valid = true;
+  return B2S_OK;
+}
+
+// (re)build the per-match pooled grids of the angle-pruning bound after the grids changed (when they fit, see pool_fits)
+static b2s_status build_pool(b2s_matcher *m) {
+  if (!pool_fits(m->g, m->smem_optin, m->win_static_smem)) return B2S_OK;
+  const size_t pitch = pool_pitch(m->g);
+  k_grid_pool<<<dim3((unsigned)ceil_div((int)(pitch / 4), 256), (unsigned)m->batch), 256, 0, m->stream>>>(
+      m->d_grids, m->grid_pitch, m->g.data_size, m->g.width_step, pool_lead(m->g.width_step), m->d_pools, pitch);
+  B2S_CUDA_CHECK(cudaGetLastError());
   return B2S_OK;
 }
 
@@ -1569,14 +1842,15 @@ static b2s_status matcher_create_impl(const b2s_matcher_params *params, const b2
   m->sbx = (g.width_step + 3) / 4;
   m->sby = (g.height + 3) / 4;
   B2S_CUDA_CHECK(m->d_sat.reserve(B * sat_stride(m->sbx, m->sby)));
-  B2S_CUDA_CHECK(m->d_stats.reserve(1));
+  B2S_CUDA_CHECK(m->d_stats.reserve(2));
+  if (pool_fits(g, m->smem_optin, m->win_static_smem)) B2S_CUDA_CHECK(m->d_pools.reserve(B * pool_pitch(g)));
   B2S_CUDA_CHECK(m->d_part_best.reserve(B));
   B2S_CUDA_CHECK(m->d_glob_best.reserve(B));
   B2S_CUDA_CHECK(m->d_tie.reserve(B * 5));
   B2S_CUDA_CHECK(m->d_status.reserve(B));
   B2S_CUDA_CHECK(m->h_results.reserve(B));
-  B2S_CUDA_CHECK(m->h_stats.reserve(1));
-  *m->h_stats = 0;
+  B2S_CUDA_CHECK(m->h_stats.reserve(2));
+  m->h_stats[0] = m->h_stats[1] = 0;
   B2S_CUDA_CHECK(cudaMemsetAsync(m->d_grids, 0, B * m->grid_pitch, m->stream));
   B2S_CUDA_CHECK(cudaMemsetAsync(m->d_results, 0, B * sizeof(b2s_match_result), m->stream));
   B2S_CUDA_CHECK(cudaStreamSynchronize(m->stream));
@@ -1695,6 +1969,7 @@ static b2s_status add_scans_impl(b2s_matcher *m, int n_base, const double *base_
   m->grids_set = true;
   m->grid_high_bytes = false;
   m->have_sweep = false;
+  if (b2s_status st = build_pool(m)) return st;
   return build_sat(m);
 }
 
@@ -1746,6 +2021,7 @@ b2s_status b2s_matcher_set_grids(b2s_matcher *m, const uint8_t *grids, const dou
   B2S_CUDA_CHECK(cudaMemcpyAsync(m->d_grid_off, offsets, sizeof(double) * 2 * B, cudaMemcpyHostToDevice, m->stream));
   m->grids_set = true;
   m->have_sweep = false;
+  if (b2s_status st = build_pool(m)) return st;
   return build_sat(m);
 }
 
@@ -1810,7 +2086,7 @@ b2s_status b2s_matcher_correlate_scan_begin(b2s_matcher *m, const double *center
   b2s_status st = run_correlate(m, search);
   if (st) return st;
   B2S_CUDA_CHECK(cudaMemcpyAsync(m->h_results, m->d_results, sizeof(b2s_match_result) * B, cudaMemcpyDeviceToHost, m->stream));
-  B2S_CUDA_CHECK(cudaMemcpyAsync(m->h_stats, m->d_stats, sizeof(unsigned long long), cudaMemcpyDeviceToHost, m->stream));
+  B2S_CUDA_CHECK(cudaMemcpyAsync(m->h_stats, m->d_stats, 2 * sizeof(unsigned long long), cudaMemcpyDeviceToHost, m->stream));
   m->pending = true;
   m->pending_batch = B;
   return B2S_OK;
@@ -1826,6 +2102,7 @@ b2s_status b2s_matcher_correlate_scan_end(b2s_matcher *m, b2s_match_result *resu
   std::memcpy(results, m->h_results, sizeof(b2s_match_result) * B);
   if (m->last_path == 2 && m->last.na > 0 && m->n > 0) m->last_empty_frac = (double)*m->h_stats / ((double)B * m->last.na * m->n);
   else m->last_empty_frac = 0.0;
+  m->last_pruned_frac = m->last_pruned ? (double)m->h_stats[1] / ((double)B * m->last.na) : 0.0;
   read_sweep_ms(m);
   return B2S_OK;
 }
@@ -1964,6 +2241,7 @@ static ReduceArgs reduce_args(b2s_matcher *m, const b2s_search &s, int nx, int n
   A.probs_all = m->d_probs; A.results = m->d_results;
   A.k_first = k_first; A.phase = phase;
   A.part_best = m->d_part_best; A.glob_best = m->d_glob_best; A.tie_out = m->d_tie; A.tie_in = m->d_tie;
+  A.keep = nullptr;
   return A;
 }
 
@@ -2077,6 +2355,10 @@ b2s_status b2s_matcher_get_response_sums(b2s_matcher *m, int b, int32_t *out, in
   if (!m || !out || b < 0 || b >= m->batch) B2S_FAIL(B2S_ERR_BAD_PARAMS, "bad argument");
   if (!m->have_sweep) B2S_FAIL(B2S_ERR_BAD_STATE, "no sweep has been run");
   B2S_CUDA_CHECK(cudaSetDevice(m->device));
+  if (m->last_pruned) {  // sweep every angle of the last search (its lists, bases and grids are still resident)
+    if (b2s_status st = launch_window(m, m->last_plan, nullptr)) return st;
+    m->last_pruned = false;
+  }
   const int nx = m->last.nx, ny = m->last.ny, na = m->last.na;
   std::vector<int32_t> tmp((size_t)nx * ny * na);
   B2S_CUDA_CHECK(cudaMemcpyAsync(tmp.data(), m->d_sums + (size_t)b * nx * ny * na, sizeof(int32_t) * tmp.size(),
@@ -2098,6 +2380,12 @@ b2s_status b2s_matcher_last_stats(b2s_matcher *m, double out[4]) {
   return B2S_OK;
 }
 
+b2s_status b2s_matcher_last_pruned_frac(b2s_matcher *m, double *out) {
+  if (!m || !out) B2S_FAIL(B2S_ERR_BAD_PARAMS, "null argument");
+  *out = m->last_pruned_frac;
+  return B2S_OK;
+}
+
 b2s_status b2s_matcher_last_timing(b2s_matcher *m, double out[4]) {
   if (!m || !out) B2S_FAIL(B2S_ERR_BAD_PARAMS, "null argument");
   if (m->have_sweep && !m->pending && cudaSetDevice(m->device) == cudaSuccess && cudaStreamSynchronize(m->stream) == cudaSuccess) {
@@ -2112,6 +2400,24 @@ b2s_status b2s_matcher_last_timing(b2s_matcher *m, double out[4]) {
 }  // extern "C"
 
 namespace b2s {
+
+// The window sweep of plan pl over the handle's lists; angles != nullptr: only the angles of the per-match lists
+// d_angles / d_n_angles (a pruned sweep)
+static b2s_status launch_window(b2s_matcher *m, const SweepPlan &pl, const int32_t *angles) {
+  B2S_CUDA_CHECK(cudaMemsetAsync(m->d_work, 0, sizeof(int), m->stream));
+  auto launch = [&](auto kern) -> b2s_status {
+    B2S_CUDA_CHECK(raise_dyn_smem(kern, pl.win_smem));
+    kern<<<pl.ctas, WIN_THREADS, pl.win_smem, m->stream>>>(m->d_grids, m->grid_pitch, m->g.data_size, pl.copy_bytes,
+                                                           m->d_lists, m->d_counts, m->d_starts, m->d_flags, m->batch,
+                                                           m->n, pl.na, pl.nx, pl.ny, m->g.width_step, m->d_sums,
+                                                           m->d_work, pl.band_rows, pl.nbands, pl.band_bytes,
+                                                           pl.neg_bands, angles, angles ? m->d_n_angles.p : nullptr);
+    B2S_CUDA_CHECK(cudaGetLastError());
+    return B2S_OK;
+  };
+  if (pl.stride == 2) return pl.gen ? launch(k_sweep_window<2, true>) : launch(k_sweep_window<2, false>);
+  return pl.gen ? launch(k_sweep_window<1, true>) : launch(k_sweep_window<1, false>);
+}
 
 // One CorrelateScan over the batch with centres already in d_centers.  Results stay in d_results.
 static b2s_status run_correlate(b2s_matcher *m, const b2s_search *s, int k_first, int na_override, ReducePhase phase) {
@@ -2130,6 +2436,12 @@ static b2s_status run_correlate(b2s_matcher *m, const b2s_search *s, int k_first
     B2S_CUDA_CHECK(m->d_counts.reserve((size_t)B * na * 8 * pl.nbands));
     B2S_CUDA_CHECK(m->d_starts.reserve((size_t)B * na * 8 * pl.nbands));
   }
+  if (pl.prune) {
+    B2S_CUDA_CHECK(m->d_ubr.reserve((size_t)B * na));
+    B2S_CUDA_CHECK(m->d_angles.reserve((size_t)B * na));
+    B2S_CUDA_CHECK(m->d_n_angles.reserve((size_t)B));
+    B2S_CUDA_CHECK(m->d_keep.reserve((size_t)B * na));
+  }
 
   // ---- candidate bases, lookup tables, window lists ----
   B2S_CUDA_CHECK(cudaEventRecord(m->ev[0], m->stream));
@@ -2139,7 +2451,7 @@ static b2s_status run_correlate(b2s_matcher *m, const b2s_search *s, int k_first
     k_offsets<<<B * na, 256, 0, m->stream>>>(m->d_ranges, m->d_local, m->d_grid_off, m->d_centers, 3, 0.0, 0,
                                              s->angle_offset, s->angle_res, na, n, m->g.width_step, scale, m->d_lut, k_first);
   if (lists) {
-    B2S_CUDA_CHECK(cudaMemsetAsync(m->d_stats, 0, sizeof(unsigned long long), m->stream));
+    B2S_CUDA_CHECK(cudaMemsetAsync(m->d_stats, 0, 2 * sizeof(unsigned long long), m->stream));
     if (pl.osm > 16 * 1024)  // static + dynamic shared memory together must stay under the 48 KB default: opt in early
       B2S_CUDA_CHECK(raise_dyn_smem(k_offsets_sorted, pl.osm));
     k_offsets_sorted<<<B * ((na + OFF_CHUNK - 1) / OFF_CHUNK), 256, pl.osm, m->stream>>>(
@@ -2155,25 +2467,29 @@ static b2s_status run_correlate(b2s_matcher *m, const b2s_search *s, int k_first
   if (na == 0) {
     m->last_path = pl.use_window ? 2 : 1;  // empty angle subset of a split sweep: nothing to sweep
   } else if (pl.use_window) {
-    B2S_CUDA_CHECK(cudaMemsetAsync(m->d_work, 0, sizeof(int), m->stream));
-    if (pl.nbands > 1)  // bands accumulate with RED.ADD
-      B2S_CUDA_CHECK(cudaMemsetAsync(m->d_sums, 0, sizeof(int32_t) * (size_t)B * na * ncell, m->stream));
     // (A variant that ran each match's fp64 tail inside the sweep CTA right after its last tile — volume read back from
     // L2, no k_reduce pass — was built, parity-tested and measured SLOWER on cfg 2 (not re-measured on the H100): the
     // sweep kernel owns its SM, so the tail's serial stretches are no longer hidden by a second resident CTA as they are
     // in the stand-alone k_reduce.  Removed again; DESIGN.md §4.)
-    auto launch = [&](auto kern) -> b2s_status {
-      B2S_CUDA_CHECK(raise_dyn_smem(kern, pl.win_smem));
-      kern<<<pl.ctas, WIN_THREADS, pl.win_smem, m->stream>>>(m->d_grids, m->grid_pitch, m->g.data_size, pl.copy_bytes,
-                                                             m->d_lists, m->d_counts, m->d_starts, m->d_flags, B, n, na,
-                                                             nx, ny, m->g.width_step, m->d_sums, m->d_work, pl.band_rows,
-                                                             pl.nbands, pl.band_bytes, pl.neg_bands);
-      return B2S_OK;
-    };
-    b2s_status st;
-    if (pl.stride == 2) st = pl.gen ? launch(k_sweep_window<2, true>) : launch(k_sweep_window<2, false>);
-    else st = pl.gen ? launch(k_sweep_window<1, true>) : launch(k_sweep_window<1, false>);
-    if (st) return st;
+    if (pl.prune) {  // bound, probe, select, sweep the selected angles (see k_sweep_bound)
+      B2S_CUDA_CHECK(cudaMemsetAsync(m->d_work, 0, sizeof(int), m->stream));
+      B2S_CUDA_CHECK(raise_dyn_smem(k_sweep_bound, pl.bound_smem));
+      k_sweep_bound<<<pl.ctas, WIN_THREADS, pl.bound_smem, m->stream>>>(
+          m->d_pools, pool_pitch(m->g), pool_bytes(m->g), pool_lead(m->g.width_step), m->d_lists, m->d_counts,
+          m->d_starts, m->d_flags, m->d_centers, m->p, *s, B, n, na, nx, ny, m->g.width_step, m->g.data_size, m->d_ubr,
+          m->d_work);
+      k_prune_probe<<<B, 256, 0, m->stream>>>(m->d_ubr, m->d_flags, na, m->d_angles, m->d_n_angles, m->d_keep);
+      B2S_CUDA_CHECK(cudaGetLastError());
+      if (b2s_status st = launch_window(m, pl, m->d_angles)) return st;
+      k_prune_select<<<B, 256, 0, m->stream>>>(m->d_sums, m->d_ubr, m->d_centers, m->d_flags, m->p, *s, n, nx, ny, na,
+                                               m->d_angles, m->d_n_angles, m->d_keep, m->d_stats.p + 1);
+      B2S_CUDA_CHECK(cudaGetLastError());
+      if (b2s_status st = launch_window(m, pl, m->d_angles)) return st;
+    } else {
+      if (pl.nbands > 1)  // bands accumulate with RED.ADD
+        B2S_CUDA_CHECK(cudaMemsetAsync(m->d_sums, 0, sizeof(int32_t) * (size_t)B * na * ncell, m->stream));
+      if (b2s_status st = launch_window(m, pl, nullptr)) return st;
+    }
     // matches whose lattice is not the regular raster (a centre exactly on a rounding tie) fall through;
     // they compute their lookup values on the fly (no table was materialised for them)
     // (a few CTAs per match that exit at once unless the lattice is irregular: the kernel loops over the cells)
@@ -2193,7 +2509,9 @@ static b2s_status run_correlate(b2s_matcher *m, const b2s_search *s, int k_first
   B2S_CUDA_CHECK(cudaEventRecord(m->ev[2], m->stream));
 
   // ---- fp64 tail ----
-  k_reduce<<<B, RED_THREADS, 0, m->stream>>>(reduce_args(m, *s, nx, ny, na, k_first, phase));
+  ReduceArgs ra = reduce_args(m, *s, nx, ny, na, k_first, phase);
+  if (pl.prune) ra.keep = m->d_keep;
+  k_reduce<<<B, RED_THREADS, 0, m->stream>>>(ra);
   if (s->fine) {  // plan_sweep refused angle counts whose responses do not fit in 48 KB
     // the kernel's own static shared memory comes on top: 48 KB of responses (6 144 angles) needs the opt-in
     if (sizeof(double) * (size_t)na > 16 * 1024) B2S_CUDA_CHECK(raise_dyn_smem(k_angular_cov, sizeof(double) * (size_t)na));
@@ -2204,6 +2522,8 @@ static b2s_status run_correlate(b2s_matcher *m, const b2s_search *s, int k_first
   B2S_CUDA_CHECK(cudaGetLastError());
   B2S_CUDA_CHECK(cudaEventRecord(m->ev[3], m->stream));
   m->last.nx = nx; m->last.ny = ny; m->last.na = na;
+  m->last_plan = pl;
+  m->last_pruned = pl.prune && na > 0;
   m->last_search = *s;
   m->last_k_first = k_first;
   m->have_sweep = true;

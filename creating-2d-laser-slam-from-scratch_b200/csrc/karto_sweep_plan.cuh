@@ -19,9 +19,23 @@ constexpr int OFF_CHUNK = 16;           // angles per k_offsets_sorted block
 constexpr int OFF_Q = 2;                              // angles classified per pass
 constexpr int OFF_SMEM_PER_BEAM = 16 + 5 * OFF_Q;     // two doubles + OFF_Q x (origin int32 + class byte)
 constexpr size_t LIST_SMEM_MAX = 200 * 1024;  // dynamic shared memory of the list stage and of the SAT build
+constexpr int PRUNE_MIN_ANGLES = 32;    // fewer angles: the bound pass and the probe cost more than they save
+constexpr int PRUNE_MAX_ANGLES = 1024;  // the select kernels and k_reduce's angle mask hold one entry per angle
+constexpr int PRUNE_PROBE = 16;         // angles swept exactly to find the pruning threshold (one per sweep warp)
 
 // u16 entries per match of the block summed-area tables (k_grid_sat), padded to 16 bytes
 inline size_t sat_stride(int sbx, int sby) { return (size_t)((((sbx + 1) * (sby + 1)) + 7) & ~7); }
+// The 4x4 max-pooled grid (k_grid_pool) of one match: byte j holds P[j - pool_lead], P[f] = max over dy, dx in [0, 4)
+// of grid[f + dy * width_step + dx] (0 outside the grid).  It starts pool_lead bytes before grid byte 0 because a block
+// whose corner lies above the grid still reaches it; pool_bytes is what the bound pass stages, pool_pitch the stride.
+inline int pool_lead(int width_step) { return 4 * width_step; }
+inline int pool_bytes(const b2s_grid_info &g) { return (pool_lead(g.width_step) + g.data_size + 15) & ~15; }
+inline size_t pool_pitch(const b2s_grid_info &g) { return ((size_t)pool_bytes(g) + 127) & ~(size_t)127; }
+// the pooled image and its guards fit in k_sweep_bound's shared memory (k_sweep_bound's static shared memory is below
+// k_sweep_window's, so the window kernel's budget covers it)
+inline bool pool_fits(const b2s_grid_info &g, int smem_optin, size_t win_static) {
+  return (long long)pool_bytes(g) + 2 * WIN_GUARD <= (long long)smem_optin - (long long)win_static - 512;
+}
 // doubles per match of the per-cell maxima plane (m_pSearchSpaceProbs), rows padded to 8
 inline size_t probs_len(int search_side) { return (size_t)((search_side + 7) & ~7) * search_side; }
 
@@ -61,6 +75,10 @@ struct SweepPlan {
   // list stage (k_offsets_sorted)
   bool skip_empty = false;  // drop empty windows through the block summed-area table
   size_t osm = 0;           // its dynamic shared memory
+  // angle pruning (run_correlate): a bound pass over the max-pooled grid, an exact probe of the PRUNE_PROBE angles with
+  // the largest bounds, then an exact sweep of only the angles whose bound reaches the probe's best response - 0.1
+  bool prune = false;
+  size_t bound_smem = 0;  // dynamic shared memory of k_sweep_bound: pooled image + guards
 };
 
 // p, g: the handle's parameters and grid; n: beams; k_first / na_override: the angle subset of a split sweep
@@ -134,6 +152,13 @@ inline SweepPlan plan_sweep(const b2s_matcher_params &p, const b2s_grid_info &g,
   // the GEN = false instantiation assumes exactly two lanes per row-start bank (see win_load)
   const int bank_step = ((g.width_step >> 2) * stride1) & 31;
   pl.gen = (bank_step & 3) != 2;
+  // Pruning needs the whole grid and the whole pooled image in shared memory, one 32 x 32 stride-1 candidate tile (the
+  // bound's 8 x 8 blocks of 4 x 4 candidates), and the whole angle range of a search: an angle subset of a split sweep
+  // cannot know the global best.  Selector 3 sweeps every beam and every angle.
+  pl.bound_smem = (size_t)pool_bytes(g) + 2 * WIN_GUARD;
+  pl.prune = pl.use_window && pl.nbands == 1 && pl.stride == 1 && pl.tiles_x == 1 && pl.tiles_y == 1 &&
+             na_override < 0 && force_kernel != 3 && pl.na >= PRUNE_MIN_ANGLES && pl.na <= PRUNE_MAX_ANGLES &&
+             pool_fits(g, smem_optin, win_static);
   return pl;
 }
 

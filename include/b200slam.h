@@ -209,9 +209,12 @@ b2s_status b2s_matcher_last_timing(b2s_matcher *m, double out[4]);
  * because every cell of the nY x nX window lies in empty 4x4 blocks of the grid (they add 0 to every candidate, so
  * results are unchanged); out[1] = sweep path (1 generic, 2 window); out[2] = candidates per match; out[3] = beams. */
 b2s_status b2s_matcher_last_stats(b2s_matcher *m, double out[4]);
+/* Fraction of the (match, angle) pairs of the LAST correlate_scan call that the window kernel never swept because an
+ * upper bound of all their responses lies below best - 0.1 (results unchanged; 0 when the search was not pruned). */
+b2s_status b2s_matcher_last_pruned_frac(b2s_matcher *m, double *out);
 b2s_status b2s_matcher_sync(b2s_matcher *m);
 /* 0 = automatic, 1 = force the generic global-memory gather kernel, 2 = force the shared-memory window kernel,
- * 3 = window kernel without dropping empty windows (every beam is swept) */
+ * 3 = window kernel over every beam and every angle (no empty-window dropping, no angle pruning) */
 b2s_status b2s_matcher_set_kernel(b2s_matcher *m, int which);
 
 /* ---------------------------------------------------------------- lesson6 front end: karto::Mapper / MapperGraph
