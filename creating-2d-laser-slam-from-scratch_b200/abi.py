@@ -115,6 +115,39 @@ class PlicpOdomStep(C.Structure):
                 ("reserved", C.c_int32)]
 
 
+class PlicpScanMatchStep(C.Structure):
+    """b2s_plicp_scan_match_step."""
+    _fields_ = [("icp", IcpResult), ("theta_deg", C.c_double), ("matched", C.c_int32), ("reserved", C.c_int32)]
+
+
+# lesson3/src/scan_match_plicp.cc:38-157 (InitParams): the parameter-server names the node reads.  The first group maps
+# onto b2s_icp_params; the second only speeds up the correspondence search or matters under a switch of the third
+# group; the third selects CSM code paths the library does not build, so a non-zero value is refused.
+_SCAN_MATCH_ICP = ("max_angular_correction_deg", "max_linear_correction", "max_iterations", "epsilon_xy",
+                   "epsilon_theta", "max_correspondence_dist", "use_point_to_line_distance", "outliers_maxPerc",
+                   "outliers_adaptive_order", "outliers_adaptive_mult", "outliers_remove_doubles")
+_SCAN_MATCH_NO_EFFECT = ("sigma", "use_corr_tricks", "restart_threshold_mean_error", "restart_dt", "restart_dtheta",
+                         "clustering_threshold", "orientation_neighbourhood", "do_alpha_test_thresholdDeg")
+_SCAN_MATCH_REFUSED = ("restart", "do_alpha_test", "do_visibility_test", "do_compute_covariance", "debug_verify_tricks",
+                       "use_ml_weights", "use_sigma_weights")
+
+
+def plicp_scan_match_params(ros: dict | None = None) -> IcpParams:
+    """ScanMatchPLICP::InitParams over a ROS parameter dict: absent keys keep the node's defaults (the same as
+    icp_params()).  Switches of CSM code paths the library does not build (restart, do_alpha_test, ...) are refused
+    with ValueError when non-zero, and names the node never reads with KeyError."""
+    p = icp_params()
+    for k, v in dict(ros or {}).items():
+        if k in _SCAN_MATCH_ICP:
+            setattr(p, k, int(v) if isinstance(getattr(p, k), int) else float(v))
+        elif k in _SCAN_MATCH_REFUSED:
+            if int(v) != 0:
+                raise ValueError(f"{k} = {v}: this CSM switch is not built")
+        elif k not in _SCAN_MATCH_NO_EFFECT:
+            raise KeyError(f"{k} is not a parameter of the lesson3 scan-match node")
+    return p
+
+
 class PclIcpParams(C.Structure):
     """b2s_pcl_icp_params; defaults = a default-constructed pcl::IterativeClosestPoint (lesson2 scan_match_icp.h:49)."""
     _fields_ = [("max_iterations", C.c_int32), ("drop_invalid_points", C.c_int32),

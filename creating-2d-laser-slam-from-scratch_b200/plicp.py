@@ -1,5 +1,6 @@
-"""ctypes harness over the C ABI — K3 (lesson3): batched PL-ICP (sm_icp call site, plicp_odometry.cc:391) and the
-odometry node around it (ScanMatchPLICP, plicp_odometry.cc:191-517) for B recordings at once."""
+"""ctypes harness over the C ABI — K3 (lesson3): batched PL-ICP (sm_icp call site, plicp_odometry.cc:391), the
+odometry node around it (ScanMatchPLICP, plicp_odometry.cc:191-517) and the scan-to-scan node (ScanMatchPLICP,
+scan_match_plicp.cc:162-300), each for B recordings at once."""
 from __future__ import annotations
 
 import ctypes as C
@@ -26,6 +27,13 @@ def _bind():
         L.b2s_plicp_odom_process.argtypes = [C.c_void_p, C.POINTER(C.c_int32), C.POINTER(C.c_float),
                                              C.POINTER(C.c_uint32), C.POINTER(abi.PlicpOdomStep)]
         L.b2s_plicp_odom_reset.argtypes = [C.c_void_p, C.c_int]
+        ip, fp = C.POINTER(C.c_int32), C.POINTER(C.c_float)
+        L.b2s_plicp_scan_match_create.argtypes = [C.POINTER(abi.IcpParams), C.c_int, ip, fp, fp, C.c_int, C.c_void_p,
+                                                  C.POINTER(C.c_void_p)]
+        L.b2s_plicp_scan_match_destroy.argtypes = [C.c_void_p]
+        L.b2s_plicp_scan_match_destroy.restype = None
+        L.b2s_plicp_scan_match_process.argtypes = [C.c_void_p, ip, fp, fp, C.POINTER(abi.PlicpScanMatchStep)]
+        L.b2s_plicp_scan_match_reset.argtypes = [C.c_void_p, C.c_int]
         _bound = True
     return L
 
@@ -90,6 +98,70 @@ class Odometry:
     def close(self):
         if self._h:
             _bind().b2s_plicp_odom_destroy(self._h)
+            self._h = C.c_void_p()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+
+# one b2s_plicp_scan_match_step as a numpy record
+SCAN_MATCH_STEP_DTYPE = np.dtype([("x", "<f8", 3), ("error", "<f8"), ("valid", "<i4"), ("iterations", "<i4"),
+                                  ("nvalid", "<i4"), ("icp_reserved", "<i4"), ("theta_deg", "<f8"), ("matched", "<i4"),
+                                  ("reserved", "<i4")])
+
+
+class ScanMatch:
+    """B lesson3 scan-to-scan ScanMatchPLICP nodes on the device (b2s_plicp_scan_match_*), one laser per recording:
+    n_beams, angle_min and angle_increment are [B] (the LaserScans' float32 fields).  `params` is an abi.IcpParams,
+    e.g. abi.plicp_scan_match_params(ros_params)."""
+
+    def __init__(self, params: abi.IcpParams, n_beams, angle_min, angle_increment, device=0, stream=None):
+        L = _bind()
+        self._h = C.c_void_p()
+        self.n = np.ascontiguousarray(n_beams, np.int32).reshape(-1)
+        self.batch = len(self.n)
+        amin = np.ascontiguousarray(angle_min, np.float32).reshape(-1)
+        ainc = np.ascontiguousarray(angle_increment, np.float32).reshape(-1)
+        if len(amin) != self.batch or len(ainc) != self.batch:
+            raise ValueError("one beam count, angle_min and angle_increment per recording")
+        check(L.b2s_plicp_scan_match_create(C.byref(params), self.batch, self.n.ctypes.data_as(C.POINTER(C.c_int32)),
+                                            amin.ctypes.data_as(C.POINTER(C.c_float)),
+                                            ainc.ctypes.data_as(C.POINTER(C.c_float)), device,
+                                            C.c_void_p(stream) if stream else None, C.byref(self._h)))
+
+    def process(self, recordings, range_limits):
+        """recordings: B arrays [S_b][n_beams[b]] float32 ranges (S_b = 0 leaves recording b untouched);
+        range_limits: B arrays [S_b][2] float32 (range_min, range_max of each scan).  -> list of B structured arrays
+        of SCAN_MATCH_STEP_DTYPE, one row per scan."""
+        if len(recordings) != self.batch or len(range_limits) != self.batch:
+            raise ValueError("one recording and one range-limit array per recording of the handle")
+        rec = [np.asarray(r, np.float32) for r in recordings]
+        if any(r.size and (r.ndim != 2 or r.shape[1] != self.n[b]) for b, r in enumerate(rec)):
+            raise ValueError("recording b is [S_b][n_beams[b]]")
+        rec = [r.reshape(-1, self.n[b]) for b, r in enumerate(rec)]
+        lim = [np.asarray(l, np.float32).reshape(-1, 2) for l in range_limits]
+        counts = np.array([len(r) for r in rec], np.int32)
+        if any(len(l) != c for l, c in zip(lim, counts)):
+            raise ValueError("one (range_min, range_max) per scan")
+        total = int(counts.sum())
+        rng = np.ascontiguousarray(np.concatenate([r.reshape(-1) for r in rec]) if total else np.zeros(1, np.float32))
+        lm = np.ascontiguousarray(np.concatenate(lim) if total else np.zeros((1, 2), np.float32))
+        out = (abi.PlicpScanMatchStep * max(total, 1))()
+        check(_bind().b2s_plicp_scan_match_process(self._h, counts.ctypes.data_as(C.POINTER(C.c_int32)),
+                                                   rng.ctypes.data_as(C.POINTER(C.c_float)),
+                                                   lm.ctypes.data_as(C.POINTER(C.c_float)), out))
+        raw = np.frombuffer(out, dtype=SCAN_MATCH_STEP_DTYPE, count=total).copy()
+        return np.split(raw, np.cumsum(counts)[:-1])
+
+    def reset(self, recording=-1):
+        check(_bind().b2s_plicp_scan_match_reset(self._h, int(recording)))
+
+    def close(self):
+        if self._h:
+            _bind().b2s_plicp_scan_match_destroy(self._h)
             self._h = C.c_void_p()
 
     def __del__(self):

@@ -879,6 +879,41 @@ b2s_status b2s_plicp_odom_process(b2s_plicp_odom *h, const int32_t *n_scans, con
 /* a fresh node for one recording, or for all with recording = -1: its next scan initialises it */
 b2s_status b2s_plicp_odom_reset(b2s_plicp_odom *h, int recording);
 
+/* ScanMatchPLICP (lesson3/src/scan_match_plicp.cc:162-300), lesson3's scan-to-scan node, for B independent recordings,
+ * each of its own laser: every LaserScan is converted to an LDP (LaserScanToLDP, :220-261: valid iff range_min < r <
+ * range_max with the message's own float32 fields, so NaN and +-inf are invalid; beam angle angle_min + i *
+ * angle_increment summed in float) and matched by sm_icp (the matcher of b2s_plicp_match) against the scan before it
+ * from a zero first guess; the new scan then becomes the previous one.  The pairs of a recording are independent, so a
+ * call runs ONE launch with one CTA per scan pair across all recordings.  Pinned to the unmodified node except sm_icp
+ * (PARITY UNPINNED, DESIGN.md §7). */
+typedef struct b2s_plicp_scan_match_step { /* one LaserScan's outcome */
+  b2s_icp_result icp; /* output_ (all zero when matched = 0) */
+  double theta_deg;   /* output_.x[2] * 180 / M_PI in the node's operation order (what it prints, :289), valid or not */
+  int32_t matched;    /* 0 for the scan that initialises the node (nothing matched), else 1 */
+  int32_t reserved;
+} b2s_plicp_scan_match_step;
+
+typedef struct b2s_plicp_scan_match b2s_plicp_scan_match; /* opaque: B ScanMatchPLICP nodes */
+
+/* One laser per recording: n_beams[b], angle_min[b], angle_increment[b] (the LaserScans' float32 fields).
+ * B2S_ERR_BAD_PARAMS for NULL pointers, batch < 1, a beam count < 3 or icp.max_iterations < 1; B2S_ERR_NO_DEVICE
+ * without a device; B2S_ERR_TOO_LARGE when a beam count is above the pair kernel's limit (2408 on an H100, 82 bytes of
+ * shared memory per beam). */
+b2s_status b2s_plicp_scan_match_create(const b2s_icp_params *params, int batch, const int32_t *n_beams,
+                                       const float *angle_min, const float *angle_increment, int device,
+                                       void *cuda_stream, b2s_plicp_scan_match **out);
+void b2s_plicp_scan_match_destroy(b2s_plicp_scan_match *h);
+/* ScanCallback on every recording's next n_scans[b] LaserScans (0: recording b is untouched), in ONE launch.
+ * Recordings are processor-major and ragged: ranges holds n_scans[0] scans of n_beams[0] floats, then n_scans[1] scans
+ * of n_beams[1] floats, ...; range_limits [sum n_scans][2] = each scan's (range_min, range_max); out [sum n_scans].
+ * The handle keeps each recording's last scan and its range fields in device memory, so two calls over consecutive
+ * parts of every recording equal one call.  B2S_ERR_BAD_PARAMS (nothing enqueued, nothing written) for NULL arrays or
+ * a negative count. */
+b2s_status b2s_plicp_scan_match_process(b2s_plicp_scan_match *h, const int32_t *n_scans, const float *ranges,
+                                        const float *range_limits, b2s_plicp_scan_match_step *out);
+/* a fresh node for one recording, or for all with recording = -1: its next scan initialises it */
+b2s_status b2s_plicp_scan_match_reset(b2s_plicp_scan_match *h, int recording);
+
 /* ---------------------------------------------------------------- lesson2: PCL ICP scan matching
  * ScanMatchICP (lesson2/src/scan_match_icp.cc): every LaserScan becomes a pcl::PointCloud<PointXYZ>
  * (ConvertScan2PointCloud, :89-130) and the previous cloud is aligned to the current one by a default-constructed
