@@ -24,7 +24,8 @@
 //   k_bases            candidate lattice -> flat base indices; flags irregular and out-of-grid lattices
 //   k_offsets          per-angle lookup tables                                         (fp64 -> i32)
 //   k_offsets_sorted   window kernel's lists: window origins grouped by row band, byte alignment and interior /
-//                      edge, empty windows dropped through the summed-area table
+//                      edge, empty windows dropped through the summed-area table (a pruned sweep: only the angles it
+//                      sweeps)
 //   k_sweep_window     THE HOT KERNEL: grid (or a row band of it) staged into shared memory by TMA bulk copy;
 //                      one warp per (angle, 32x32 candidate tile), one lane per candidate row; each 32-bit
 //                      shared-memory word feeds 4 adjacent-x candidates (byte-permute into packed u16
@@ -573,14 +574,109 @@ __global__ void __launch_bounds__(256)
   reinterpret_cast<uint32_t *>(pools + (size_t)b * pitch)[j4] = m;
 }
 
+// ----------------------------------------------------------------------------------------------
+// A beam's window origin and class at one angle: the one definition that k_offsets_sorted (which lists the beams) and
+// k_sweep_bound (which bounds an angle from the same beams without lists) share, so that the two cannot disagree.
+// ----------------------------------------------------------------------------------------------
+// the angle k (counted from the search's first angle, k_first + index for an angle subset) of GridIndexLookup's table
+__device__ __forceinline__ double win_angle(double center, double angle_offset, double angle_res, int k) {
+  return (center - angle_offset) + (double)(uint32_t)k * angle_res;
+}
+
+// The geometry of one match's window lists (everything but the angle and the beam)
+struct WinGeom {
+  double gox, goy, scale;  // the grid offset of the match and 1 / resolution
+  int32_t base00;          // flat index of candidate (0, 0)
+  int32_t span32;          // last byte any lane may touch past a window origin, clamped to 2^29
+  int width_step, data_size, height;
+  int fx, fy;              // footprint of the candidate lattice in cells
+  float inv_step, inv_band;
+  int band_rows, nbands, neg_bands;
+};
+
+__device__ __forceinline__ WinGeom win_geom(double gox, double goy, double scale, int32_t base00, int stride,
+                                            int rows_total, int cols_total, int width_step, int data_size, int height,
+                                            int nx, int ny, int band_rows, int nbands, int neg_bands) {
+  WinGeom G;
+  G.gox = gox; G.goy = goy; G.scale = scale; G.base00 = base00;
+  const long long span = (long long)stride * (rows_total - 1) * width_step + cols_total + 8;  // last byte any lane may touch
+  G.span32 = (int32_t)min(span, (long long)(1 << 29));
+  G.width_step = width_step; G.data_size = data_size; G.height = height;
+  G.fx = stride * (nx - 1) + 1; G.fy = stride * (ny - 1) + 1;
+  G.inv_step = 1.0f / (float)width_step; G.inv_band = 1.0f / (float)band_rows;
+  G.band_rows = band_rows; G.nbands = nbands; G.neg_bands = neg_bands;
+  return G;
+}
+
+// Scan-local point (plx, ply) at the angle with the given cosine and sine: `a` = the window origin (base00 + the
+// GridIndexLookup value, flat index), returned = its group: 255 (dropped: the window lies wholly outside the grid, or
+// the point is not finite, or - when use_sat - every 4x4 block the window covers is empty, which sets `empty`), else
+// 8 * band + (a & 3) for an interior window, 8 * band + 4 + (a & 3) for an edge one.
+__device__ __forceinline__ int win_origin_class(double plx, double ply, double cosine, double sine, const WinGeom &G,
+                                                bool use_sat, const uint16_t *__restrict__ sat, int SW, int32_t &a,
+                                                bool &empty) {
+  // lut_value() inlined: a non-finite local point (INVALID_SCAN reading) makes ox/oy non-finite
+  const double ox = __dsub_rn(__dmul_rn(cosine, plx), __dmul_rn(sine, ply));
+  const double oy = __dadd_rn(__dmul_rn(sine, plx), __dmul_rn(cosine, ply));
+  int cls = 255;  // dropped
+  a = 0;
+  empty = false;
+  if (isfinite(ox) && isfinite(oy)) {
+    const int32_t gx = cast_i32(kround(__dmul_rn(__dsub_rn(__dadd_rn(ox, G.gox), G.gox), G.scale)));
+    const int32_t gy = cast_i32(kround(__dmul_rn(__dsub_rn(__dadd_rn(oy, G.goy), G.goy), G.scale)));
+    const int32_t o = (int32_t)((uint32_t)gx + (uint32_t)gy * (uint32_t)G.width_step);
+    a = (int32_t)((uint32_t)G.base00 + (uint32_t)o);
+    // window [a - 8, a + span] against [0, data_size): 32-bit arithmetic after clamping far-away origins
+    const int32_t ac = max(min(a, (int32_t)(1 << 29)), -(int32_t)(1 << 29));
+    const int32_t lo = ac - 8, hi = ac + G.span32;
+    if (hi < 0 || lo >= G.data_size) cls = 255;  // whole window outside: contributes 0
+    else if (lo >= -(WIN_GUARD - 16) && hi <= G.data_size + (WIN_GUARD - 16)) cls = a & 3;  // interior
+    else cls = 4 + (a & 3);                                                                  // edge
+    int y = 0, x = 0;
+    if ((use_sat || G.nbands > 1) && cls < 255 && (a >= 0 || G.neg_bands > 0)) {
+      // floor(a / width_step) by float reciprocal + fix-up (|a| < 2^24 is exact in float; larger values are
+      // corrected too); a < 0 only matters when origins below the grid get row bands of their own (neg_bands)
+      if (G.data_size <= (1 << 24) && ac == a) {
+        y = (int)((float)a * G.inv_step);
+        if (y * G.width_step > a) y--;
+        else if ((y + 1) * G.width_step <= a) y++;
+      } else {
+        y = a / G.width_step;
+        if (y * G.width_step > a) y--;
+      }
+      x = a - y * G.width_step;
+    }
+    if (G.nbands > 1 && cls < 8) {
+      int band = (int)((float)y * G.inv_band);
+      if (band * G.band_rows > y) band--;
+      else if ((band + 1) * G.band_rows <= y) band++;
+      cls += 8 * max(min(band + G.neg_bands, G.nbands - 1), 0);  // the row band that holds the window origin
+    }
+    if (use_sat && cls < 255 && a >= 0) {
+      // empty-window test on the 4x4-block summed-area table (only for windows that do not wrap a row end)
+      if (x + G.fx <= G.width_step && y + G.fy <= G.height) {
+        const int bx0 = x >> 2, bx1 = (x + G.fx - 1) >> 2, by0 = y >> 2, by1 = (y + G.fy - 1) >> 2;
+        const uint32_t c = (uint32_t)sat[(by1 + 1) * SW + bx1 + 1] - (uint32_t)sat[by0 * SW + bx1 + 1] -
+                           (uint32_t)sat[(by1 + 1) * SW + bx0] + (uint32_t)sat[by0 * SW + bx0];
+        if (c == 0) { cls = 255; empty = true; }
+      }
+    }
+  }
+  return cls;
+}
+
 // One block per (match, chunk of OFF_CHUNK angles): window origins grouped as [I0 I1 I2 I3 E0 E1 E2 E3] (I = interior,
 // E = edge, index = a & 3), every group a multiple of 4 long (an interior group donates its 0..3 surplus beams to its edge
 // group; edge groups are padded with far-negative sentinels of the same alignment).  counts[8] holds the group lengths.
 // The scan's readings and local points are staged in shared memory once per block and reused for every angle of
 // the chunk (16x less L2 traffic than one block per angle).  A non-finite reading (INVALID_SCAN, Karto.h:6478) always
 // yields a non-finite local point (inf/NaN propagate through the inverse transform), so only the points are staged.
+// LISTED (a pruned sweep): the block lists the angles at positions [k0, k0 + OFF_CHUNK) of match b's angle list
+// list_angles[b * n_angles ...] (list_n[b] long, list_chunks blocks per match), each at its own index k, so that
+// k_sweep_window reads them where it reads every angle's lists; the lists of the other angles are left as they were.
 // (OFF_CHUNK, OFF_Q, OFF_SMEM_PER_BEAM: karto_sweep_plan.cuh)
 constexpr int OFF_GS = 8 * WIN_MAX_BANDS;             // group slots per angle
+template <bool LISTED>
 __global__ void __launch_bounds__(256)
     k_offsets_sorted(const double *__restrict__ ranges, const double *__restrict__ local,
                      const double *__restrict__ grid_off, const double *__restrict__ centers,
@@ -589,7 +685,8 @@ __global__ void __launch_bounds__(256)
                      int rows_total, int cols_total, int32_t *__restrict__ lists, int32_t *__restrict__ counts,
                      const uint16_t *__restrict__ sat_all, int sbx, int sby, int height, int nx, int ny,
                      unsigned long long *__restrict__ stats, int band_rows, int nbands,
-                     int32_t *__restrict__ starts, int stride, int k_first, int neg_bands) {
+                     int32_t *__restrict__ starts, int stride, int k_first, int neg_bands,
+                     const int32_t *__restrict__ list_angles, const int32_t *__restrict__ list_n, int list_chunks) {
   extern __shared__ __align__(16) unsigned char s_raw[];
   double *s_lx = reinterpret_cast<double *>(s_raw), *s_ly = s_lx + n;  // [n] scan-local points
   int32_t *s_vals = reinterpret_cast<int32_t *>(s_ly + n);             // [OFF_Q][n] window origins
@@ -599,10 +696,11 @@ __global__ void __launch_bounds__(256)
   __shared__ int n_empty;
   const int ngroups = 8 * nbands;
   const int list_cap = n + LIST_PAD * nbands;
-  const int chunks = (n_angles + OFF_CHUNK - 1) / OFF_CHUNK;
+  const int chunks = LISTED ? list_chunks : (n_angles + OFF_CHUNK - 1) / OFF_CHUNK;
   const int b = blockIdx.x / chunks, k0 = (blockIdx.x % chunks) * OFF_CHUNK;
   const int f = flags[b];
   if ((f & 2) || !(f & 1)) return;  // error / irregular lattice: the generic kernel handles this match
+  if (LISTED && k0 >= list_n[b]) return;  // past the end of the match's angle list
   for (int i = threadIdx.x; i < n; i += blockDim.x) {
     s_lx[i] = local[((size_t)b * n + i) * 2];
     s_ly[i] = local[((size_t)b * n + i) * 2 + 1];
@@ -617,18 +715,17 @@ __global__ void __launch_bounds__(256)
   if (threadIdx.x == 0) n_empty = 0;
   const double center = centers[(size_t)b * 3 + 2];
   __shared__ double s_cos[OFF_CHUNK], s_sin[OFF_CHUNK];
-  if (threadIdx.x < OFF_CHUNK && k0 + threadIdx.x < n_angles) {  // one sincos per angle, not per thread
-    const double ang = (center - angle_offset) + (double)(uint32_t)(k_first + k0 + threadIdx.x) * angle_res;
+  __shared__ int s_k[LISTED ? OFF_CHUNK : 1];  // LISTED: the angle index of each list position of the chunk
+  if (threadIdx.x < OFF_CHUNK && k0 + threadIdx.x < (LISTED ? list_n[b] : n_angles)) {  // one sincos per angle, not per thread
+    int k = k0 + threadIdx.x;
+    if (LISTED) s_k[threadIdx.x] = k = list_angles[(size_t)b * n_angles + k];
+    const double ang = win_angle(center, angle_offset, angle_res, k_first + k);
     s_cos[threadIdx.x] = cos(ang);
     s_sin[threadIdx.x] = sin(ang);
   }
-  const double gox = grid_off[2 * b], goy = grid_off[2 * b + 1];
-  const int32_t base00 = bases[(size_t)b * ncell];
-  const long long span = (long long)stride * (rows_total - 1) * width_step + cols_total + 8;  // last byte any lane may touch
-  const int32_t span32 = (int32_t)min(span, (long long)(1 << 29));
-  const int fx = stride * (nx - 1) + 1, fy = stride * (ny - 1) + 1;  // footprint of the candidate lattice in cells
-  const float inv_step = 1.0f / (float)width_step, inv_band = 1.0f / (float)band_rows;
-  const int kend = min(k0 + OFF_CHUNK, n_angles);
+  const WinGeom G = win_geom(grid_off[2 * b], grid_off[2 * b + 1], scale, bases[(size_t)b * ncell], stride, rows_total,
+                             cols_total, width_step, data_size, height, nx, ny, band_rows, nbands, neg_bands);
+  const int kend = min(k0 + OFF_CHUNK, LISTED ? list_n[b] : n_angles);  // one past the chunk's last list position
   for (int kq = k0; kq < kend; kq += OFF_Q) {  // OFF_Q angles per pass: half the barriers, one read of the points
     const int nq = min(OFF_Q, kend - kq);
     __syncthreads();  // staging done / previous angles' smem fully consumed
@@ -640,53 +737,11 @@ __global__ void __launch_bounds__(256)
 #pragma unroll
       for (int q = 0; q < OFF_Q; q++) {
         if (q >= nq) break;
-        const double cosine = s_cos[kq - k0 + q], sine = s_sin[kq - k0 + q];
-        // lut_value() inlined: a non-finite local point (INVALID_SCAN reading) makes ox/oy non-finite
-        const double ox = __dsub_rn(__dmul_rn(cosine, plx), __dmul_rn(sine, ply));
-        const double oy = __dadd_rn(__dmul_rn(sine, plx), __dmul_rn(cosine, ply));
-        int cls = 255;  // dropped
-        int32_t a = 0;
-        if (isfinite(ox) && isfinite(oy)) {
-          const int32_t gx = cast_i32(kround(__dmul_rn(__dsub_rn(__dadd_rn(ox, gox), gox), scale)));
-          const int32_t gy = cast_i32(kround(__dmul_rn(__dsub_rn(__dadd_rn(oy, goy), goy), scale)));
-          const int32_t o = (int32_t)((uint32_t)gx + (uint32_t)gy * (uint32_t)width_step);
-          a = (int32_t)((uint32_t)base00 + (uint32_t)o);
-          // window [a - 8, a + span] against [0, data_size): 32-bit arithmetic after clamping far-away origins
-          const int32_t ac = max(min(a, (int32_t)(1 << 29)), -(int32_t)(1 << 29));
-          const int32_t lo = ac - 8, hi = ac + span32;
-          if (hi < 0 || lo >= data_size) cls = 255;  // whole window outside: contributes 0
-          else if (lo >= -(WIN_GUARD - 16) && hi <= data_size + (WIN_GUARD - 16)) cls = a & 3;  // interior
-          else cls = 4 + (a & 3);                                                                // edge
-          int y = 0, x = 0;
-          if ((sat_all || nbands > 1) && cls < 255 && (a >= 0 || neg_bands > 0)) {
-            // floor(a / width_step) by float reciprocal + fix-up (|a| < 2^24 is exact in float; larger values are
-            // corrected too); a < 0 only matters when origins below the grid get row bands of their own (neg_bands)
-            if (data_size <= (1 << 24) && ac == a) {
-              y = (int)((float)a * inv_step);
-              if (y * width_step > a) y--;
-              else if ((y + 1) * width_step <= a) y++;
-            } else {
-              y = a / width_step;
-              if (y * width_step > a) y--;
-            }
-            x = a - y * width_step;
-          }
-          if (nbands > 1 && cls < 8) {
-            int band = (int)((float)y * inv_band);
-            if (band * band_rows > y) band--;
-            else if ((band + 1) * band_rows <= y) band++;
-            cls += 8 * max(min(band + neg_bands, nbands - 1), 0);  // the row band that holds the window origin
-          }
-          if (sat_all && cls < 255 && a >= 0) {
-            // empty-window test on the 4x4-block summed-area table (only for windows that do not wrap a row end)
-            if (x + fx <= width_step && y + fy <= height) {
-              const int bx0 = x >> 2, bx1 = (x + fx - 1) >> 2, by0 = y >> 2, by1 = (y + fy - 1) >> 2;
-              const uint32_t c = (uint32_t)s_sat[(by1 + 1) * SW + bx1 + 1] - (uint32_t)s_sat[by0 * SW + bx1 + 1] -
-                                 (uint32_t)s_sat[(by1 + 1) * SW + bx0] + (uint32_t)s_sat[by0 * SW + bx0];
-              if (c == 0) { cls = 255; empty_here++; }
-            }
-          }
-        }
+        int32_t a;
+        bool empty;
+        const int cls = win_origin_class(plx, ply, s_cos[kq - k0 + q], s_sin[kq - k0 + q], G, sat_all != nullptr, s_sat,
+                                         SW, a, empty);
+        empty_here += empty;
         s_vals[q * n + i] = a;
         s_cls[q * n + i] = (uint8_t)cls;
         if (cls < 255) atomicAdd(&cnt[q * OFF_GS + cls], 1);
@@ -721,19 +776,21 @@ __global__ void __launch_bounds__(256)
           cls += 4;
           slot = atomicAdd(&fill[q * OFF_GS + cls], 1);
         }
-        lists[((size_t)b * n_angles + kq + q) * list_cap + seg[q * OFF_GS + cls] + slot] = s_vals[q * n + i];
+        const int k = LISTED ? s_k[kq - k0 + q] : kq + q;
+        lists[((size_t)b * n_angles + k) * list_cap + seg[q * OFF_GS + cls] + slot] = s_vals[q * n + i];
       }
     }
     __syncthreads();
     for (int t = threadIdx.x; t < nq * ngroups; t += blockDim.x) {
       const int q = t / ngroups, g = t % ngroups;
       const int cg = cnt[q * OFF_GS + g], sg_ = seg[q * OFF_GS + g];
-      int32_t *out = lists + ((size_t)b * n_angles + kq + q) * list_cap;
+      const int k = LISTED ? s_k[kq - k0 + q] : kq + q;
+      int32_t *out = lists + ((size_t)b * n_angles + k) * list_cap;
       if ((g & 7) >= 4)
         for (int r = cg; r < ((cg + 3) & ~3); r++)
           out[sg_ + r] = WIN_SKIP + (g & 3);  // pad: all-outside beams of the same alignment
-      counts[((size_t)b * n_angles + kq + q) * ngroups + g] = (cg + 3) & ~3;
-      starts[((size_t)b * n_angles + kq + q) * ngroups + g] = sg_;
+      counts[((size_t)b * n_angles + k) * ngroups + g] = (cg + 3) & ~3;
+      starts[((size_t)b * n_angles + k) * ngroups + g] = sg_;
     }
   }
   __syncthreads();
@@ -1099,37 +1156,34 @@ __device__ __forceinline__ float red_fscore(int32_t isum, float apf_k, float dpf
 // So an angle may be skipped when an upper bound of all its responses is below L - 0.1 for some lower bound L <= best:
 //   k_sweep_bound   UBr(k) = max over 8 x 8 blocks of 4 x 4 candidates of
 //                   (SUM_beams P[a_i + block corner]) / (N * 100) * (max distance penalty of the block * anglePenalty(k)),
-//                   P the 4x4 max-pooled grid (k_grid_pool), summed over the same beam lists the exact sweep uses
-//                   (beams dropped as empty windows add 0 everywhere).  Same fp64 operations as candidate_response, so
-//                   UBr(k) >= every response of angle k.
+//                   P the 4x4 max-pooled grid (k_grid_pool), summed over the beams the exact sweep's lists hold, placed
+//                   by the bound itself (beams dropped as empty windows add 0 everywhere).  Same fp64 operations as
+//                   candidate_response, so UBr(k) >= every response of angle k.  No window lists exist yet:
+//                   k_offsets_sorted lists only the angles of the two exact passes below.
 //   k_prune_probe   the PRUNE_PROBE angles with the largest UBr are swept exactly (k_sweep_window on an angle list);
 //   k_prune_select  L = the largest exact response among them (a real candidate, so L <= best); every other angle is
 //                   swept iff UBr(k) >= L - 0.1 - 1e-9.  When L - 0.1 is near 0 (within the 1e-6 band in which a
 //                   response is not penalised, Mapper.cpp:399) every angle is swept.
 // k_reduce reads 0 for the angles never swept; the response volume is completed on request (get_response_sums).
 // ----------------------------------------------------------------------------------------------
+// the window origins s_off[j0, j1) of this warp's staging row (j0, j1 multiples of 4), summed at the lane's two block
+// corners
 template <bool CHECK>
-__device__ __forceinline__ void bound_beams(const uint8_t *__restrict__ sp, const int32_t *__restrict__ list, int count,
-                                            int lane, int off_a, int off_b, uint32_t lead, uint32_t limit,
-                                            int32_t *__restrict__ s_off, uint32_t &ua, uint32_t &ub) {
-  for (int ib = 0; ib < count; ib += 32) {
-    const int cnt = min(32, count - ib);  // a multiple of 4
-    __syncwarp();
-    s_off[lane] = (lane < cnt) ? __ldg(list + ib + lane) : 0;
-    __syncwarp();
-    for (int j = 0; j < cnt; j += 4) {
-      const int4 a4 = *reinterpret_cast<const int4 *>(s_off + j);
-      const int32_t as[4] = {a4.x, a4.y, a4.z, a4.w};
+__device__ __forceinline__ void bound_beams(const uint8_t *__restrict__ sp, const int32_t *__restrict__ s_off, int j0,
+                                            int j1, int off_a, int off_b, uint32_t lead, uint32_t limit, uint32_t &ua,
+                                            uint32_t &ub) {
+  for (int j = j0; j < j1; j += 4) {
+    const int4 a4 = *reinterpret_cast<const int4 *>(s_off + j);  // one broadcast load: four window origins
+    const int32_t as[4] = {a4.x, a4.y, a4.z, a4.w};
 #pragma unroll
-      for (int q = 0; q < 4; q++) {
-        if (CHECK) {  // flat index a + corner, modulo 2^32 like the reference's base + offset; P is 0 outside
-          const uint32_t fa = (uint32_t)as[q] + (uint32_t)off_a, fb = (uint32_t)as[q] + (uint32_t)off_b;
-          ua += (fa + lead < limit) ? sp[(int32_t)fa] : 0u;
-          ub += (fb + lead < limit) ? sp[(int32_t)fb] : 0u;
-        } else {
-          ua += sp[as[q] + off_a];
-          ub += sp[as[q] + off_b];
-        }
+    for (int q = 0; q < 4; q++) {
+      if (CHECK) {  // flat index a + corner, modulo 2^32 like the reference's base + offset; P is 0 outside
+        const uint32_t fa = (uint32_t)as[q] + (uint32_t)off_a, fb = (uint32_t)as[q] + (uint32_t)off_b;
+        ua += (fa + lead < limit) ? sp[(int32_t)fa] : 0u;
+        ub += (fb + lead < limit) ? sp[(int32_t)fb] : 0u;
+      } else {
+        ua += sp[as[q] + off_a];
+        ub += sp[as[q] + off_b];
       }
     }
   }
@@ -1137,20 +1191,36 @@ __device__ __forceinline__ void bound_beams(const uint8_t *__restrict__ sp, cons
 
 // One persistent CTA per match at a time (like k_sweep_window): the pooled image is staged by TMA, warps take angles,
 // lane L owns blocks (L / 8, L % 8) and (L / 8 + 4, L % 8).  ubr[b][k] = UBr(k) (-1 for a match the window kernel
-// does not sweep).
+// does not sweep).  The bound reads no window lists: for each angle a warp places 32 beams at a time, one per lane,
+// with win_origin_class (the definition k_offsets_sorted lists them by), drops the ones the lists would drop, and
+// compacts the interior and the edge ones into its staging row.  Which beams add is the same set as in the lists and
+// integer sums commute, so UBr is the one the lists would give.  It also counts the empty windows of every (beam,
+// angle) pair into stats[0], as the lists of a sweep that is not pruned do.
+// STAGE (SweepPlan::bound_stage): the scan-local points and the summed-area table sit in shared memory after the
+// pooled image; otherwise they are read from global memory through L1.
+template <bool STAGE>
 __global__ void __launch_bounds__(WIN_THREADS, 1)
     k_sweep_bound(const uint8_t *__restrict__ pools, size_t pool_pitch_, int pool_bytes_, int lead,
-                  const int32_t *__restrict__ lists, const int32_t *__restrict__ counts,
-                  const int32_t *__restrict__ starts, const int32_t *__restrict__ flags,
+                  const double *__restrict__ local, const double *__restrict__ grid_off,
+                  const int32_t *__restrict__ bases, const uint16_t *__restrict__ sat_all, int sbx, int sby,
+                  int height, int rows_total, int cols_total, double scale, const int32_t *__restrict__ flags,
                   const double *__restrict__ centers, b2s_matcher_params p, b2s_search s, int batch, int n, int na,
-                  int nx, int ny, int width_step, int data_size, double *__restrict__ ubr, int *__restrict__ work_counter) {
-  extern __shared__ __align__(128) unsigned char smem[];  // [WIN_GUARD zeros][pooled image][WIN_GUARD zeros]
+                  int nx, int ny, int width_step, int data_size, double *__restrict__ ubr, int *__restrict__ work_counter,
+                  unsigned long long *__restrict__ stats) {
+  // [WIN_GUARD zeros][pooled image][WIN_GUARD zeros] (+ STAGE: [n] x, [n] y of the scan-local points, the SAT)
+  extern __shared__ __align__(128) unsigned char smem[];
   __shared__ uint64_t bar;
   __shared__ int s_unit;
   __shared__ __align__(16) int32_t s_offsets[WIN_THREADS / 32][32];
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   int32_t *s_off = s_offsets[warp];
   const bool pen = s.do_penalize != 0;
+  const int SW = sbx + 1;
+  const int sat_len = ((sby + 1) * SW + 7) & ~7;  // entries per match, padded to 16 bytes
+  double *s_lx = reinterpret_cast<double *>(smem + WIN_GUARD + pool_bytes_ + WIN_GUARD), *s_ly = s_lx + n;
+  uint16_t *s_sat = reinterpret_cast<uint16_t *>(s_ly + n);
+  const unsigned lanes_below = (1u << lane) - 1u;
+  unsigned long long empties = 0;
   // the largest distance penalty of the candidates of block (by, bx), as k_reduce computes sq and candidate_response
   // the penalty (-1: the block holds no candidate)
   auto block_dpen = [&](int by, int bx) {
@@ -1172,7 +1242,6 @@ __global__ void __launch_bounds__(WIN_THREADS, 1)
   __syncthreads();
   const int off_a = 4 * (lane >> 3) * width_step + 4 * (lane & 7), off_b = off_a + 16 * width_step;
   const double D = (double)((uint32_t)n * (uint32_t)GRID_OCCUPIED);
-  const int list_cap = n + LIST_PAD;
   const uint8_t *sp = smem + WIN_GUARD + lead;  // grid flat index 0
   uint32_t parity = 0;
   while (true) {
@@ -1194,22 +1263,51 @@ __global__ void __launch_bounds__(WIN_THREADS, 1)
         bulk_g2s(smem + WIN_GUARD + off, src + off, (uint32_t)min(32768, pool_bytes_ - off), &bar);
     }
     if (threadIdx.x < WIN_GUARD / 4) reinterpret_cast<uint32_t *>(smem + WIN_GUARD + pool_bytes_)[threadIdx.x] = 0;
+    const double *g_pts = local + (size_t)b * n * 2;
+    const uint16_t *g_sat = sat_all ? sat_all + (size_t)b * sat_len : nullptr;
+    if (STAGE) {
+      for (int i = threadIdx.x; i < n; i += blockDim.x) {
+        s_lx[i] = g_pts[2 * i];
+        s_ly[i] = g_pts[2 * i + 1];
+      }
+      if (sat_all)
+        for (int i = threadIdx.x; i < sat_len / 8; i += blockDim.x)
+          reinterpret_cast<uint4 *>(s_sat)[i] = reinterpret_cast<const uint4 *>(g_sat)[i];
+    }
+    const WinGeom G = win_geom(grid_off[2 * b], grid_off[2 * b + 1], scale, bases[(size_t)b * nx * ny], 1, rows_total,
+                               cols_total, width_step, data_size, height, nx, ny, 1, 1, 0);
     mbar_wait(&bar, parity);
     parity ^= 1;
     __syncthreads();
     const double ch = centers[3 * b + 2];
     for (int k = warp; k < na; k += WIN_THREADS / 32) {
-      const int32_t *list = lists + ((size_t)b * na + k) * list_cap;
-      const int32_t *cn = counts + ((size_t)b * na + k) * 8;
-      const int32_t *sg = starts + ((size_t)b * na + k) * 8;
-      // groups I0..I3 E0..E3 are contiguous: interior beams [0, sg[4]), edge beams after them.  Interior windows lie
-      // within WIN_GUARD - 16 bytes of the grid, so every corner they read is inside the staged image.
-      const int n_int = sg[4], n_edge = sg[7] + cn[7] - sg[4];
+      const double angle = win_angle(ch, s.angle_offset, s.angle_res, k);
+      const double cosine = cos(angle), sine = sin(angle);
       uint32_t ua = 0, ub = 0;
-      bound_beams<false>(sp, list, n_int, lane, off_a, off_b, lead, lead + data_size, s_off, ua, ub);
-      bound_beams<true>(sp, list + n_int, n_edge, lane, off_a, off_b, lead, lead + data_size, s_off, ua, ub);
+      for (int i0 = 0; i0 < n; i0 += 32) {
+        const int i = i0 + lane;
+        int cls = 255;
+        int32_t a = 0;
+        bool empty = false;
+        if (i < n) {
+          const double plx = STAGE ? s_lx[i] : __ldg(g_pts + 2 * i), ply = STAGE ? s_ly[i] : __ldg(g_pts + 2 * i + 1);
+          cls = win_origin_class(plx, ply, cosine, sine, G, sat_all != nullptr, STAGE ? s_sat : g_sat, SW, a, empty);
+        }
+        empties += empty;
+        // interior beams first, then the edge ones, padded to a multiple of 4 with an origin far outside the grid.
+        // Interior windows lie within WIN_GUARD - 16 bytes of the grid, so every corner they read is inside the staged
+        // image; the checked loop takes the last 0..3 of them with the edge beams (the value it reads is the same).
+        const unsigned m_int = __ballot_sync(0xffffffffu, cls < 4), m_edge = __ballot_sync(0xffffffffu, cls >= 4 && cls < 8);
+        const int n_int = __popc(m_int), n_all = n_int + __popc(m_edge);
+        __syncwarp();
+        if (cls < 4) s_off[__popc(m_int & lanes_below)] = a;
+        else if (cls < 8) s_off[n_int + __popc(m_edge & lanes_below)] = a;
+        if (lane >= n_all && lane < ((n_all + 3) & ~3)) s_off[lane] = WIN_SKIP;  // slots no beam was compacted into
+        __syncwarp();
+        bound_beams<false>(sp, s_off, 0, n_int & ~3, off_a, off_b, lead, lead + data_size, ua, ub);
+        bound_beams<true>(sp, s_off, n_int & ~3, (n_all + 3) & ~3, off_a, off_b, lead, lead + data_size, ua, ub);
+      }
       // candidate_response's operations, with the block's largest sum and largest distance penalty
-      const double angle = (ch - s.angle_offset) + (double)(uint32_t)k * s.angle_res;
       double apen = 1.0;
       if (pen) {
         const double sq_a = (angle - ch) * (angle - ch);
@@ -1224,6 +1322,9 @@ __global__ void __launch_bounds__(WIN_THREADS, 1)
     }
     __syncthreads();  // everyone is done with the image before the next match's copy is issued
   }
+#pragma unroll
+  for (int d = 16; d > 0; d >>= 1) empties += __shfl_xor_sync(0xffffffffu, empties, d);
+  if (lane == 0 && empties) atomicAdd(stats, empties);
 }
 
 // The PRUNE_PROBE angles with the largest bounds (ties: lower index first) become match b's first angle list; keep[b][k]
@@ -1763,6 +1864,8 @@ static void read_sweep_ms(b2s_matcher *m) {
 static b2s_status run_correlate(b2s_matcher *m, const b2s_search *s, int k_first = 0, int na_override = -1,
                                 ReducePhase phase = REDUCE_WHOLE);
 static b2s_status launch_window(b2s_matcher *m, const SweepPlan &pl, const int32_t *angles);
+static b2s_status launch_lists(b2s_matcher *m, const SweepPlan &pl, const b2s_search &s, int k_first, int listed_chunks,
+                               bool count_empty);
 
 // (re)build the per-match block summed-area tables after the grids changed
 static b2s_status build_sat(b2s_matcher *m) {
@@ -2355,7 +2458,9 @@ b2s_status b2s_matcher_get_response_sums(b2s_matcher *m, int b, int32_t *out, in
   if (!m || !out || b < 0 || b >= m->batch) B2S_FAIL(B2S_ERR_BAD_PARAMS, "bad argument");
   if (!m->have_sweep) B2S_FAIL(B2S_ERR_BAD_STATE, "no sweep has been run");
   B2S_CUDA_CHECK(cudaSetDevice(m->device));
-  if (m->last_pruned) {  // sweep every angle of the last search (its lists, bases and grids are still resident)
+  if (m->last_pruned) {  // list and sweep every angle of the last search (its bases and grids are still resident; the
+                         // lists of the angles it skipped were not built, or are an earlier search's)
+    if (b2s_status st = launch_lists(m, m->last_plan, m->last_search, m->last_k_first, 0, false)) return st;
     if (b2s_status st = launch_window(m, m->last_plan, nullptr)) return st;
     m->last_pruned = false;
   }
@@ -2419,6 +2524,28 @@ static b2s_status launch_window(b2s_matcher *m, const SweepPlan &pl, const int32
   return pl.gen ? launch(k_sweep_window<1, true>) : launch(k_sweep_window<1, false>);
 }
 
+// The window lists of plan pl for search s: every angle (listed_chunks == 0), or only the angles of the per-match
+// lists d_angles / d_n_angles of a pruned sweep, listed_chunks * OFF_CHUNK of them at most.  count_empty: add the
+// empty windows dropped to d_stats[0].
+static b2s_status launch_lists(b2s_matcher *m, const SweepPlan &pl, const b2s_search &s, int k_first, int listed_chunks,
+                               bool count_empty) {
+  const int na = pl.na, ncell = pl.nx * pl.ny;
+  auto launch = [&](auto kern, int chunks) -> b2s_status {
+    if (pl.osm > 16 * 1024)  // static + dynamic shared memory together must stay under the 48 KB default: opt in early
+      B2S_CUDA_CHECK(raise_dyn_smem(kern, pl.osm));
+    kern<<<m->batch * chunks, 256, pl.osm, m->stream>>>(
+        m->d_ranges, m->d_local, m->d_grid_off, m->d_centers, m->d_bases, m->d_flags, s.angle_offset, s.angle_res, na,
+        m->n, ncell, m->g.width_step, m->g.data_size, 1.0 / m->p.resolution, pl.rows_total, pl.tiles_x * 32,
+        m->d_lists, m->d_counts, pl.skip_empty ? m->d_sat.p : nullptr, m->sbx, m->sby, m->g.height, pl.nx, pl.ny,
+        count_empty ? m->d_stats.p : nullptr, pl.band_rows, pl.nbands, m->d_starts, pl.stride, k_first, pl.neg_bands,
+        listed_chunks ? m->d_angles.p : nullptr, listed_chunks ? m->d_n_angles.p : nullptr, chunks);
+    B2S_CUDA_CHECK(cudaGetLastError());
+    return B2S_OK;
+  };
+  if (listed_chunks) return launch(k_offsets_sorted<true>, listed_chunks);
+  return launch(k_offsets_sorted<false>, ceil_div(na, OFF_CHUNK));
+}
+
 // One CorrelateScan over the batch with centres already in d_centers.  Results stay in d_results.
 static b2s_status run_correlate(b2s_matcher *m, const b2s_search *s, int k_first, int na_override, ReducePhase phase) {
   B2S_NVTX("K1 correlate (lists + sweep + tail)");
@@ -2452,13 +2579,9 @@ static b2s_status run_correlate(b2s_matcher *m, const b2s_search *s, int k_first
                                              s->angle_offset, s->angle_res, na, n, m->g.width_step, scale, m->d_lut, k_first);
   if (lists) {
     B2S_CUDA_CHECK(cudaMemsetAsync(m->d_stats, 0, 2 * sizeof(unsigned long long), m->stream));
-    if (pl.osm > 16 * 1024)  // static + dynamic shared memory together must stay under the 48 KB default: opt in early
-      B2S_CUDA_CHECK(raise_dyn_smem(k_offsets_sorted, pl.osm));
-    k_offsets_sorted<<<B * ((na + OFF_CHUNK - 1) / OFF_CHUNK), 256, pl.osm, m->stream>>>(
-        m->d_ranges, m->d_local, m->d_grid_off, m->d_centers, m->d_bases, m->d_flags, s->angle_offset, s->angle_res, na, n,
-        ncell, m->g.width_step, m->g.data_size, scale, pl.rows_total, pl.tiles_x * 32, m->d_lists, m->d_counts,
-        pl.skip_empty ? m->d_sat.p : nullptr, m->sbx, m->sby, m->g.height, nx, ny, m->d_stats, pl.band_rows, pl.nbands,
-        m->d_starts, pl.stride, k_first, pl.neg_bands);
+    // a pruned sweep lists only the angles it sweeps, inside the sweep stage; k_sweep_bound counts the empty windows
+    if (!pl.prune)
+      if (b2s_status st = launch_lists(m, pl, *s, k_first, 0, true)) return st;
   }
   B2S_CUDA_CHECK(cudaGetLastError());
   B2S_CUDA_CHECK(cudaEventRecord(m->ev[1], m->stream));
@@ -2471,19 +2594,26 @@ static b2s_status run_correlate(b2s_matcher *m, const b2s_search *s, int k_first
     // L2, no k_reduce pass — was built, parity-tested and measured SLOWER on cfg 2 (not re-measured on the H100): the
     // sweep kernel owns its SM, so the tail's serial stretches are no longer hidden by a second resident CTA as they are
     // in the stand-alone k_reduce.  Removed again; DESIGN.md §4.)
-    if (pl.prune) {  // bound, probe, select, sweep the selected angles (see k_sweep_bound)
+    if (pl.prune) {  // bound, probe, select, sweep the selected angles (see k_sweep_bound); lists only for those
       B2S_CUDA_CHECK(cudaMemsetAsync(m->d_work, 0, sizeof(int), m->stream));
-      B2S_CUDA_CHECK(raise_dyn_smem(k_sweep_bound, pl.bound_smem));
-      k_sweep_bound<<<pl.ctas, WIN_THREADS, pl.bound_smem, m->stream>>>(
-          m->d_pools, pool_pitch(m->g), pool_bytes(m->g), pool_lead(m->g.width_step), m->d_lists, m->d_counts,
-          m->d_starts, m->d_flags, m->d_centers, m->p, *s, B, n, na, nx, ny, m->g.width_step, m->g.data_size, m->d_ubr,
-          m->d_work);
+      auto bound = [&](auto kern) -> b2s_status {
+        B2S_CUDA_CHECK(raise_dyn_smem(kern, pl.bound_smem));
+        kern<<<pl.ctas, WIN_THREADS, pl.bound_smem, m->stream>>>(
+            m->d_pools, pool_pitch(m->g), pool_bytes(m->g), pool_lead(m->g.width_step), m->d_local, m->d_grid_off,
+            m->d_bases, pl.skip_empty ? m->d_sat.p : nullptr, m->sbx, m->sby, m->g.height, pl.rows_total,
+            pl.tiles_x * 32, scale, m->d_flags, m->d_centers, m->p, *s, B, n, na, nx, ny, m->g.width_step,
+            m->g.data_size, m->d_ubr, m->d_work, m->d_stats.p);
+        return B2S_OK;
+      };
+      if (b2s_status st = pl.bound_stage ? bound(k_sweep_bound<true>) : bound(k_sweep_bound<false>)) return st;
       k_prune_probe<<<B, 256, 0, m->stream>>>(m->d_ubr, m->d_flags, na, m->d_angles, m->d_n_angles, m->d_keep);
       B2S_CUDA_CHECK(cudaGetLastError());
+      if (b2s_status st = launch_lists(m, pl, *s, k_first, ceil_div(PRUNE_PROBE, OFF_CHUNK), false)) return st;
       if (b2s_status st = launch_window(m, pl, m->d_angles)) return st;
       k_prune_select<<<B, 256, 0, m->stream>>>(m->d_sums, m->d_ubr, m->d_centers, m->d_flags, m->p, *s, n, nx, ny, na,
                                                m->d_angles, m->d_n_angles, m->d_keep, m->d_stats.p + 1);
       B2S_CUDA_CHECK(cudaGetLastError());
+      if (b2s_status st = launch_lists(m, pl, *s, k_first, ceil_div(na, OFF_CHUNK), false)) return st;
       if (b2s_status st = launch_window(m, pl, m->d_angles)) return st;
     } else {
       if (pl.nbands > 1)  // bands accumulate with RED.ADD

@@ -78,8 +78,16 @@ struct SweepPlan {
   // angle pruning (run_correlate): a bound pass over the max-pooled grid, an exact probe of the PRUNE_PROBE angles with
   // the largest bounds, then an exact sweep of only the angles whose bound reaches the probe's best response - 0.1
   bool prune = false;
-  size_t bound_smem = 0;  // dynamic shared memory of k_sweep_bound: pooled image + guards
+  // k_sweep_bound places every beam itself: it stages the scan-local points (and, with skip_empty, the summed-area
+  // table) in shared memory after the pooled image when they fit there, and reads them through L1 otherwise
+  bool bound_stage = false;
+  size_t bound_smem = 0;  // dynamic shared memory of k_sweep_bound: pooled image + guards (+ points + SAT when staged)
 };
+
+// shared memory k_sweep_bound stages after its pooled image (bound_stage): n scan-local points and the SAT when used
+inline size_t bound_stage_bytes(int n, bool skip_empty, int sbx, int sby) {
+  return (size_t)n * 2 * sizeof(double) + (skip_empty ? sizeof(uint16_t) * sat_stride(sbx, sby) : 0);
+}
 
 // p, g: the handle's parameters and grid; n: beams; k_first / na_override: the angle subset of a split sweep
 // (na_override < 0: every angle); force_kernel: b2s_matcher_set_kernel; sat_valid / grid_high_bytes / sbx / sby: the
@@ -159,6 +167,9 @@ inline SweepPlan plan_sweep(const b2s_matcher_params &p, const b2s_grid_info &g,
   pl.prune = pl.use_window && pl.nbands == 1 && pl.stride == 1 && pl.tiles_x == 1 && pl.tiles_y == 1 &&
              na_override < 0 && force_kernel != 3 && pl.na >= PRUNE_MIN_ANGLES && pl.na <= PRUNE_MAX_ANGLES &&
              pool_fits(g, smem_optin, win_static);
+  const size_t staged = bound_stage_bytes(n, pl.skip_empty, sbx, sby);
+  pl.bound_stage = pl.prune && (long long)(pl.bound_smem + staged) <= smem_limit;
+  if (pl.bound_stage) pl.bound_smem += staged;
   return pl;
 }
 
