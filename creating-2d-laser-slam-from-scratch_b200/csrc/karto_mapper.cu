@@ -26,6 +26,15 @@
 
 #include "common.cuh"
 
+namespace b2s {
+// A Mapper that belongs to a fleet of Karto nodes hands each batch of matches to the fleet, which runs it on matcher
+// handles shared by every node: base scans are named by their unique id in this Mapper, base_ids / base_poses
+// [batch][max_base] padded by repeating a match's last base scan.
+typedef b2s_status (*FleetMatchFn)(void *user, int which, int batch, const double *ranges, const double *poses,
+                                   int max_base, const int32_t *base_ids, const double *base_poses, int do_penalize,
+                                   int do_refine, b2s_match_result *results);
+}  // namespace b2s
+
 using namespace b2s;
 
 namespace {
@@ -178,6 +187,8 @@ struct b2s_mapper {
   b2s_match_scan_fn match = nullptr;
   void *match_user = nullptr;
   CudaBackend *cuda = nullptr;
+  b2s::FleetMatchFn fleet = nullptr;  // a Mapper of a Karto node fleet: its matches go to the fleet (karto_node.cu)
+  void *fleet_user = nullptr;
   b2s_scan_solver solver{};
   bool have_solver = false;
   std::deque<MScan> scans;  // MapperSensorManager::m_Scans (every sensor's scans by unique id); deque: stable addresses
@@ -283,6 +294,31 @@ b2s_status run_matches(b2s_mapper *m, int which, const std::vector<MatchJob> &jo
     m->n_match_calls += B;
     m->n_batches += 1;
     return cuda_match_ids(m, which, jobs, do_penalize, do_refine, out);
+  }
+  if (m->fleet) {  // as cuda_match_ids, with the base scans named by id for the fleet's shared pools
+    int max_base = 1;
+    for (const MatchJob &j : jobs) {
+      if (j.chain.empty()) B2S_FAIL(B2S_ERR_BAD_PARAMS, "mapper: MatchScan against an empty chain");
+      max_base = std::max(max_base, (int)j.chain.size());
+    }
+    std::vector<double> ranges((size_t)B * N), poses((size_t)B * 3), bp((size_t)B * max_base * 3);
+    std::vector<int32_t> ids((size_t)B * max_base);
+    for (int b = 0; b < B; b++) {
+      std::memcpy(&ranges[(size_t)b * N], jobs[b].ranges->data(), sizeof(double) * N);
+      poses[3 * b] = jobs[b].robot_pose.x; poses[3 * b + 1] = jobs[b].robot_pose.y; poses[3 * b + 2] = jobs[b].robot_pose.h;
+      const int nb = (int)jobs[b].chain.size();
+      for (int j = 0; j < max_base; j++) {
+        const int id = jobs[b].chain[std::min(j, nb - 1)];
+        const MScan &sc = m->scans[id];
+        const size_t k = (size_t)b * max_base + j;
+        ids[k] = id;
+        bp[3 * k] = sc.corrected.x; bp[3 * k + 1] = sc.corrected.y; bp[3 * k + 2] = sc.corrected.h;
+      }
+    }
+    m->n_match_calls += B;
+    m->n_batches += 1;
+    return m->fleet(m->fleet_user, which, B, ranges.data(), poses.data(), max_base, ids.data(), bp.data(),
+                    do_penalize ? 1 : 0, do_refine ? 1 : 0, out.data());
   }
   std::vector<double> ranges((size_t)B * N), poses((size_t)B * 3);
   std::vector<int32_t> first(B), count(B);
@@ -771,6 +807,32 @@ b2s_status b2s_mapper_create(const b2s_mapper_params *params, const b2s_laser *l
   (*out)->cuda = c;
   return B2S_OK;
 }
+
+}  // extern "C"
+
+namespace b2s {
+
+// a fleet Mapper (karto_node.cu): every match goes to `match`; the Mapper itself makes no CUDA call
+b2s_status mapper_create_fleet(const b2s_mapper_params *params, const b2s_laser *laser, FleetMatchFn match, void *user,
+                               b2s_mapper **out) {
+  *out = nullptr;
+  if (b2s_status st = check_params(params, laser)) return st;
+  b2s_mapper *m = new (std::nothrow) b2s_mapper();
+  if (!m) B2S_FAIL(B2S_ERR_CUDA, "out of host memory");
+  m->prm = *params;
+  m->laser = *laser;
+  m->fleet = match;
+  m->fleet_user = user;
+  *out = m;
+  return B2S_OK;
+}
+
+// readings [n_readings] of the Mapper's scan with unique id `id` (0 <= id < b2s_mapper_scan_count)
+const double *mapper_scan_ranges(const b2s_mapper *m, int id) { return m->scans[(size_t)id].ranges.data(); }
+
+}  // namespace b2s
+
+extern "C" {
 
 void b2s_mapper_destroy(b2s_mapper *m) {
   if (!m) return;

@@ -1,5 +1,8 @@
-// lesson6's SlamKarto node (lesson6/src/karto_slam.cc) over a whole recording of one laser: host C++ that drives the
-// device Mapper (karto_mapper.cu, every MatchScan on the device) and the device occupancy grid (karto_occgrid.cu).
+// lesson6's SlamKarto node (lesson6/src/karto_slam.cc) over whole recordings, B nodes per handle: host C++ that drives
+// one Mapper per node (karto_mapper.cu) and the device occupancy grid (karto_occgrid.cu).  Each node runs its per-scan
+// loop, unchanged, on a worker thread of its own; its device work (every MatchScan batch, every map build) becomes a
+// request to the dispatcher on the calling thread, which serves the requests of all nodes in rounds: the matches on
+// two matcher handles shared by every node, the maps in one batched build.  The single-node handle is the batch of one.
 //   SlamKarto::InitParams / constructor              karto_slam.cc:21-58, 81-252
 //   SlamKarto::laserCallback                         :286-325  (throttle, map-update gate)
 //   SlamKarto::getLaser                              :327-405  (offset, upside-down test)
@@ -7,8 +10,17 @@
 //   SlamKarto::getOdomPose                           :483-505
 //   SlamKarto::updateMap                             :507-581  (CreateFromScans over every processed scan)
 // tf's LinearMath and roscpp's Time / Duration are ros_math.cuh's (include/b200slam.h, DESIGN.md §7).
+#include <algorithm>
+#include <chrono>
 #include <cmath>
+#include <condition_variable>
+#include <cstddef>
 #include <cstring>
+#include <memory>
+#include <mutex>
+#include <new>
+#include <string>
+#include <thread>
 #include <vector>
 
 #include "common.cuh"
@@ -17,7 +29,22 @@
 namespace b2s {
 b2s_status karto_laser_from_msg(const b2s_laser_scan_msg *scan, const double laser_pose_in_base[3], double use_scan_range,
                                 b2s_laser *out);  // ros_io.cu
-}
+// karto_mapper.cu
+typedef b2s_status (*FleetMatchFn)(void *user, int which, int batch, const double *ranges, const double *poses,
+                                   int max_base, const int32_t *base_ids, const double *base_poses, int do_penalize,
+                                   int do_refine, b2s_match_result *results);
+b2s_status mapper_create_fleet(const b2s_mapper_params *params, const b2s_laser *laser, FleetMatchFn match, void *user,
+                               b2s_mapper **out);
+const double *mapper_scan_ranges(const b2s_mapper *m, int id);
+// karto_occgrid.cu
+struct OccBatch;
+b2s_status occ_batch_create(const b2s_laser &laser, int device, OccBatch **out);
+void occ_batch_destroy(OccBatch *b);
+double occ_batch_bytes_d2h(const OccBatch *b);
+b2s_status occ_batch_append(OccBatch *b, int count, const float *rows, int32_t *first);
+b2s_status occ_batch_build(OccBatch *b, int G, const int32_t *n_scans, const int32_t *rows, const double *poses,
+                           const double *resolution, b2s_occ_grid_info *info, int32_t *have, const int8_t **payload);
+}  // namespace b2s
 
 using namespace b2s;
 
@@ -45,49 +72,503 @@ double yaw_of(const TfTransform &t) {
 
 }  // namespace
 
-struct b2s_karto_node {
+namespace {
+
+constexpr int NODE_MAX_BATCH = 1024;  // nodes per handle
+constexpr int MATCH_MAX_BATCH = 256;  // matches per launch of the shared matchers; larger groups go out in parts
+
+// a node's device work, posted by its worker and served by the dispatcher
+struct Request {
+  bool map = false;
+  // a MatchScan batch (FleetMatchFn's arguments)
+  int which = 0, batch = 0, max_base = 0, do_penalize = 0, do_refine = 0;
+  const double *ranges = nullptr, *poses = nullptr, *base_poses = nullptr;
+  const int32_t *base_ids = nullptr;
+  b2s_match_result *results = nullptr;
+  // a map build: CreateFromScans over the node's first `count` scans at `map_poses`
+  int32_t scan_index = 0, count = 0;
+  const double *map_poses = nullptr;
+  int32_t published = 0;  // out: a map was built and handed to on_map
+  b2s_status status = B2S_OK;
+  bool done = false;
+};
+
+struct Failure {
+  long long round = -1;  // the round before which it happened
+  int node = -1;
+  b2s_status status = B2S_OK;
+  std::string message;
+  bool before(const Failure &o) const { return o.node < 0 || round < o.round || (round == o.round && node < o.node); }
+};
+
+// one call's rendezvous of the workers and the dispatcher: a round is served when every worker that has not finished
+// has posted its next request, so round k holds each live node's k-th request whatever the thread timing
+struct Lockstep {
+  std::mutex mu;
+  std::condition_variable to_dispatcher, to_workers;
+  int live = 0, waiting = 0;
+  long long round = 0;
+  std::vector<Request *> posted;  // [batch]
+  Failure first;
+  bool stop = false;              // a failure was recorded: every later request is refused
+  void fail(const Failure &f) {
+    if (f.before(first)) first = f;
+    stop = true;
+  }
+};
+
+}  // namespace
+
+// one SlamKarto of a handle
+struct KartoNodeState {
+  b2s_karto_node *owner = nullptr;
+  int index = 0;
   b2s_karto_node_params prm{};
-  b2s_laser laser{};
-  int n_msg = 0, device = 0;
-  bool inverted = false;
-  TfTransform base_laser;
   RosDuration interval{0, 0};
   b2s_mapper *mapper = nullptr;
   int64_t laser_count = 0;  // laser_count_ (every scan handed in)
   bool got_map = false;
   uint32_t last_map_sec = 0, last_map_nsec = 0;  // laserCallback's static last_map_update
   double map_to_odom[7] = {0, 0, 0, 0, 0, 0, 1};
+  std::vector<double> scan;                      // one scan's readings
+  std::vector<double> poses;                     // scratch for b2s_mapper_get_poses
+  std::vector<int32_t> match_row[2];             // row in each shared matcher's pool of each Mapper scan
+  std::vector<int32_t> map_row;                  // row in the map pool of each Mapper scan
+};
+
+struct b2s_karto_node {
+  int batch = 1;
+  b2s_laser laser{};
+  int n_msg = 0, device = 0;
+  bool inverted = false;
+  b2s_matcher_params matcher_params[2]{};
+  std::vector<KartoNodeState> nodes;
+  b2s_matcher *h[2] = {nullptr, nullptr};
+  int cap_batch = 8, cap_base[2] = {32, 32};
+  OccBatch *maps = nullptr;
+  Lockstep *lock = nullptr;  // the running call's
   bool failed = false;
-  std::vector<double> readings;  // [processed scans][m], appended once per processed scan
-  std::vector<double> poses;     // scratch for b2s_mapper_get_poses
-  std::vector<double> scan;      // one scan's readings
-  std::vector<int8_t> payload;   // scratch for b2s_occ_grid_copy_ros
+  double timing[8] = {0, 0, 0, 0, 0, 0, 0, 0};
+  // the dispatcher's scratch
+  std::vector<double> m_ranges, m_poses, m_base_poses;
+  std::vector<int32_t> m_rows;
+  std::vector<b2s_match_result> m_results;
+  std::vector<float> stage;
 };
 
 namespace {
 
-// SlamKarto::updateMap: CreateFromScans over every processed scan at its corrected pose now, then the ROS payload
-b2s_status update_map(b2s_karto_node *n, int32_t scan_index, b2s_karto_map_fn on_map, void *user, bool &published) {
-  published = false;
-  const int count = b2s_mapper_scan_count(n->mapper);
-  n->poses.resize(3 * (size_t)count);
-  if (count > 0)
-    if (b2s_status st = b2s_mapper_get_poses(n->mapper, n->poses.data())) return st;
-  b2s_occ_grid *g = nullptr;
-  if (b2s_status st = b2s_occ_grid_create_from_scans(&n->laser, count, n->readings.data(), n->poses.data(),
-                                                     n->prm.resolution, n->device, nullptr, &g))
-    return st;
-  if (!g) return B2S_OK;  // CreateFromScans returned NULL: no map, the gate stays open
-  b2s_occ_grid_info info;
-  b2s_status st = b2s_occ_grid_info_get(g, &info);
-  if (!st) {
-    n->payload.resize((size_t)info.width * (size_t)info.height);
-    st = b2s_occ_grid_copy_ros(g, n->payload.data());
+// set on a worker whose request was refused or failed on the device: the dispatcher has recorded the failure
+thread_local bool t_stopped = false;
+
+// a worker's request: posted, then the worker waits until the dispatcher served it
+b2s_status post(KartoNodeState &k, Request &r) {
+  Lockstep &L = *k.owner->lock;
+  std::unique_lock<std::mutex> g(L.mu);
+  if (!L.stop) {
+    L.posted[(size_t)k.index] = &r;
+    L.waiting++;
+    if (L.waiting == L.live) L.to_dispatcher.notify_one();
+    L.to_workers.wait(g, [&] { return r.done; });
+    if (!r.status) return B2S_OK;
   }
-  b2s_occ_grid_destroy(g);
-  if (st) return st;
-  if (on_map) on_map(user, scan_index, &info, n->payload.data());
-  published = true;
+  t_stopped = true;
+  B2S_FAIL(B2S_ERR_BAD_STATE, "stopped: a node of the handle failed");
+}
+
+// FleetMatchFn: the Mapper's match batch as a request
+b2s_status fleet_match(void *user, int which, int batch, const double *ranges, const double *poses, int max_base,
+                       const int32_t *base_ids, const double *base_poses, int do_penalize, int do_refine,
+                       b2s_match_result *results) {
+  KartoNodeState &k = *static_cast<KartoNodeState *>(user);
+  Request r;
+  r.which = which; r.batch = batch; r.max_base = max_base; r.do_penalize = do_penalize; r.do_refine = do_refine;
+  r.ranges = ranges; r.poses = poses; r.base_ids = base_ids; r.base_poses = base_poses; r.results = results;
+  return post(k, r);
+}
+
+// SlamKarto::updateMap as a request: CreateFromScans over every processed scan at its corrected pose now
+b2s_status update_map(KartoNodeState &k, int32_t scan_index, bool &published) {
+  published = false;
+  const int count = b2s_mapper_scan_count(k.mapper);
+  k.poses.resize(3 * (size_t)count);
+  if (count > 0)
+    if (b2s_status st = b2s_mapper_get_poses(k.mapper, k.poses.data())) return st;
+  Request r;
+  r.map = true;
+  r.scan_index = scan_index;
+  r.count = count;
+  r.map_poses = k.poses.data();
+  if (b2s_status st = post(k, r)) return st;
+  published = r.published != 0;  // CreateFromScans returned NULL: no map, the gate stays open
+  return B2S_OK;
+}
+
+struct CallRows {
+  const float *ranges;
+  const uint32_t *stamps;
+  const double *odom;
+  int32_t *out_state;
+  double *out_pose, *out_map_to_odom;
+  int32_t *out_map_published;
+};
+
+// SlamKarto::laserCallback on scan `i` of the call's rows (node-major), the body of the single node's loop
+b2s_status node_scan(b2s_karto_node *n, KartoNodeState &k, size_t i, const CallRows &a) {
+  const int m = n->laser.n_readings, nr = n->n_msg;
+  const int32_t scan_index = (int32_t)k.laser_count;
+  int32_t state = B2S_KARTO_THROTTLED, published = 0;
+  double pose[3] = {0, 0, 0};
+  k.laser_count++;
+  if (k.laser_count % k.prm.throttle_scans == 0) {
+    // getOdomPose: transformPose(odom_frame_, identity in base_frame_) at the scan's stamp
+    const double *row = a.odom + 7 * i;
+    bool ok = true;
+    for (int q = 0; q < 7; q++) ok = ok && !std::isnan(row[q]);
+    if (!ok) {
+      state = B2S_KARTO_NO_ODOM;
+    } else {
+      const TfTransform odom_base = tf_from_row(row);
+      double ident[7] = {0, 0, 0};  // tf::Transform(createQuaternionFromRPY(0, 0, 0), (0, 0, 0))
+      quat_set_rpy(0, 0, 0, ident + 3);
+      const TfTransform op = tf_mul(odom_base, tf_from_row(ident));
+      const double odom_pose[3] = {op.o[0], op.o[1], yaw_of(op)};
+      // addScan: float32 ranges widened, reversed for an upside-down laser; the laser's m readings are used
+      const float *r = a.ranges + i * (size_t)nr;
+      for (int q = 0; q < m; q++) k.scan[q] = (double)r[n->inverted ? nr - 1 - q : q];
+      int32_t processed = 0;
+      if (b2s_status st = b2s_mapper_process_sensor(k.mapper, "laser", k.scan.data(), odom_pose, 0.0, &processed, pose))
+        return st;
+      if (!processed) {
+        state = B2S_KARTO_NOT_MOVED;
+        pose[0] = pose[1] = pose[2] = 0;
+      } else {
+        state = B2S_KARTO_PROCESSED;
+        // map_to_odom_ = (odom <- base_link * T(corrected)^-1) rebuilt from its quaternion and origin, inverted
+        double corrected[7] = {pose[0], pose[1], 0.0}, odom_to_map[7];
+        quat_set_rpy(0, 0, pose[2], corrected + 3);
+        tf_to_row(tf_mul(odom_base, tf_inverse(tf_from_row(corrected))), odom_to_map);
+        tf_to_row(tf_inverse(tf_from_row(odom_to_map)), k.map_to_odom);
+        const uint32_t *s = a.stamps + 2 * i;
+        if (!k.got_map || ros_duration_gt(ros_time_diff(s[0], s[1], k.last_map_sec, k.last_map_nsec), k.interval)) {
+          bool done = false;
+          if (b2s_status st = update_map(k, scan_index, done)) return st;
+          if (done) {
+            k.last_map_sec = s[0];
+            k.last_map_nsec = s[1];
+            k.got_map = true;
+            published = 1;
+          }
+        }
+      }
+    }
+  }
+  if (a.out_state) a.out_state[i] = state;
+  if (a.out_pose) std::memcpy(a.out_pose + 3 * i, pose, sizeof pose);
+  if (a.out_map_to_odom) std::memcpy(a.out_map_to_odom + 7 * i, k.map_to_odom, sizeof k.map_to_odom);
+  if (a.out_map_published) a.out_map_published[i] = published;
+  return B2S_OK;
+}
+
+// a worker: node b's scans of the call, then it leaves the lockstep.  It makes no CUDA call and never calls on_map.
+void worker(b2s_karto_node *n, int b, size_t first, int count, const CallRows &a) {
+  KartoNodeState &k = n->nodes[(size_t)b];
+  Lockstep &L = *n->lock;
+  b2s_status st = B2S_OK;
+  for (int i = 0; i < count && !st; i++) st = node_scan(n, k, first + (size_t)i, a);
+  std::lock_guard<std::mutex> g(L.mu);
+  if (st && !t_stopped) {
+    Failure f;
+    f.round = L.round;
+    f.node = b;
+    f.status = st;
+    f.message = b2s_last_error();
+    L.fail(f);
+  }
+  L.live--;
+  if (L.waiting == L.live) L.to_dispatcher.notify_one();
+}
+
+// (re)creating a shared matcher drops its pool: every node's scans are appended again on their next match
+b2s_status ensure_matcher(b2s_karto_node *n, int which, int max_base) {
+  if (n->h[which] && max_base <= n->cap_base[which]) return B2S_OK;
+  const int cap = n->h[which] ? std::max(max_base, 2 * n->cap_base[which]) : std::max(max_base, n->cap_base[which]);
+  if (n->h[which]) b2s_matcher_destroy(n->h[which]);
+  n->h[which] = nullptr;
+  for (KartoNodeState &k : n->nodes) k.match_row[which].clear();
+  if (b2s_status st = b2s_matcher_create(&n->matcher_params[which], &n->laser, n->device, n->cap_batch, cap, nullptr,
+                                         &n->h[which]))
+    return st;
+  n->cap_base[which] = cap;
+  return B2S_OK;
+}
+
+// one group of match requests with the same (which, do_penalize, do_refine), node order
+b2s_status serve_matches(b2s_karto_node *n, const std::vector<std::pair<int, Request *>> &group) {
+  const Request &r0 = *group[0].second;
+  const int which = r0.which, N = n->laser.n_readings;
+  int max_base = 1, total = 0;
+  for (const auto &q : group) {
+    max_base = std::max(max_base, q.second->max_base);
+    total += q.second->batch;
+  }
+  if (b2s_status st = ensure_matcher(n, which, max_base)) return st;
+  b2s_matcher *h = n->h[which];
+  // the nodes' new scans into the shared pool, each once
+  for (const auto &q : group) {
+    KartoNodeState &k = n->nodes[(size_t)q.first];
+    std::vector<int32_t> &rows = k.match_row[which];
+    for (int id = (int)rows.size(), c = b2s_mapper_scan_count(k.mapper); id < c; id++) {
+      int32_t row = 0;
+      if (b2s_status st = b2s_matcher_pool_append(h, mapper_scan_ranges(k.mapper, id), &row)) return st;
+      rows.push_back(row);
+    }
+  }
+  n->m_ranges.resize((size_t)total * N);
+  n->m_poses.resize((size_t)total * 3);
+  n->m_rows.resize((size_t)total * max_base);
+  n->m_base_poses.resize((size_t)total * max_base * 3);
+  n->m_results.assign((size_t)total, b2s_match_result{});
+  size_t t = 0;
+  for (const auto &q : group) {
+    const Request &r = *q.second;
+    const std::vector<int32_t> &rows = n->nodes[(size_t)q.first].match_row[which];
+    std::memcpy(&n->m_ranges[t * N], r.ranges, sizeof(double) * N * r.batch);
+    std::memcpy(&n->m_poses[t * 3], r.poses, sizeof(double) * 3 * r.batch);
+    for (int b = 0; b < r.batch; b++, t++)
+      for (int j = 0; j < max_base; j++) {  // padded to the group's longest chain by repeating the last base scan
+        const size_t src = (size_t)b * r.max_base + std::min(j, r.max_base - 1), dst = t * max_base + j;
+        n->m_rows[dst] = rows[(size_t)r.base_ids[src]];
+        std::memcpy(&n->m_base_poses[3 * dst], r.base_poses + 3 * src, 3 * sizeof(double));
+      }
+  }
+  for (int at = 0; at < total; at += n->cap_batch) {
+    const int c = std::min(n->cap_batch, total - at);
+    b2s_status st = b2s_matcher_set_scans(h, c, &n->m_ranges[(size_t)at * N], &n->m_poses[(size_t)at * 3]);
+    if (!st) st = b2s_matcher_add_scans_pool(h, max_base, &n->m_rows[(size_t)at * max_base],
+                                             &n->m_base_poses[(size_t)at * max_base * 3]);
+    if (!st) st = b2s_matcher_match_scan(h, r0.do_penalize, r0.do_refine, &n->m_results[(size_t)at]);
+    if (st) return st;
+    n->timing[1] += 1;
+  }
+  n->timing[2] += total;
+  t = 0;
+  for (const auto &q : group) {
+    std::memcpy(q.second->results, &n->m_results[t], sizeof(b2s_match_result) * q.second->batch);
+    t += (size_t)q.second->batch;
+  }
+  return B2S_OK;
+}
+
+// every map request of a round in one batched build; maps to on_map in ascending node order
+b2s_status serve_maps(b2s_karto_node *n, const std::vector<std::pair<int, Request *>> &reqs, b2s_karto_node_batch_map_fn on_map,
+                      void *user) {
+  const int G = (int)reqs.size(), m = n->laser.n_readings;
+  // each node's scans not yet in the map pool, float32 (they are float32 ranges widened, so this is exact), one upload
+  size_t fresh = 0;
+  for (const auto &q : reqs) fresh += (size_t)q.second->count - std::min(n->nodes[(size_t)q.first].map_row.size(), (size_t)q.second->count);
+  n->stage.resize(fresh * (size_t)m);
+  size_t s = 0;
+  for (const auto &q : reqs) {
+    const KartoNodeState &k = n->nodes[(size_t)q.first];
+    for (int id = (int)k.map_row.size(); id < q.second->count; id++, s++) {
+      const double *r = mapper_scan_ranges(k.mapper, id);
+      for (int i = 0; i < m; i++) n->stage[s * m + i] = (float)r[i];
+    }
+  }
+  int32_t first = 0;
+  if (b2s_status st = occ_batch_append(n->maps, (int)fresh, n->stage.data(), &first)) return st;
+  std::vector<int32_t> n_scans((size_t)G), rows, have((size_t)G);
+  std::vector<double> poses, res((size_t)G);
+  for (int g = 0; g < G; g++) {
+    KartoNodeState &k = n->nodes[(size_t)reqs[(size_t)g].first];
+    const Request &r = *reqs[(size_t)g].second;
+    while ((int)k.map_row.size() < r.count) k.map_row.push_back(first++);
+    n_scans[(size_t)g] = r.count;
+    rows.insert(rows.end(), k.map_row.begin(), k.map_row.begin() + r.count);
+    poses.insert(poses.end(), r.map_poses, r.map_poses + 3 * (size_t)r.count);
+    res[(size_t)g] = k.prm.resolution;
+  }
+  std::vector<b2s_occ_grid_info> info((size_t)G);
+  std::vector<const int8_t *> payload((size_t)G);
+  if (b2s_status st = occ_batch_build(n->maps, G, n_scans.data(), rows.data(), poses.data(), res.data(), info.data(),
+                                      have.data(), payload.data()))
+    return st;
+  for (int g = 0; g < G; g++) {
+    Request &r = *reqs[(size_t)g].second;
+    if (!have[(size_t)g]) continue;
+    if (on_map) on_map(user, reqs[(size_t)g].first, r.scan_index, &info[(size_t)g], payload[(size_t)g]);
+    r.published = 1;
+    n->timing[3] += 1;
+  }
+  return B2S_OK;
+}
+
+double seconds_since(std::chrono::steady_clock::time_point t0) {
+  return std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count();
+}
+
+// one round: matches by group, then the maps; a failure stops every node at its next request
+void serve_round(b2s_karto_node *n, Lockstep &L, const std::vector<std::pair<int, Request *>> &reqs,
+                 b2s_karto_node_batch_map_fn on_map, void *user) {
+  if (L.stop) {  // a worker failed since the last round
+    for (const auto &q : reqs) q.second->status = B2S_ERR_BAD_STATE;
+    return;
+  }
+  std::vector<std::pair<int, Request *>> maps;
+  std::vector<std::vector<std::pair<int, Request *>>> groups;
+  std::vector<int> keys;
+  for (const auto &q : reqs) {
+    if (q.second->map) {
+      maps.push_back(q);
+      continue;
+    }
+    const int key = q.second->which * 4 + q.second->do_penalize * 2 + q.second->do_refine;
+    size_t gi = 0;
+    while (gi < keys.size() && keys[gi] != key) gi++;
+    if (gi == keys.size()) {
+      keys.push_back(key);
+      groups.emplace_back();
+    }
+    groups[gi].push_back(q);
+  }
+  auto fail = [&](const std::vector<std::pair<int, Request *>> &g, b2s_status st) {
+    Failure f;
+    f.round = L.round;
+    f.node = g[0].first;
+    f.status = st;
+    f.message = b2s_last_error();
+    std::lock_guard<std::mutex> lk(L.mu);
+    L.fail(f);
+  };
+  auto t0 = std::chrono::steady_clock::now();
+  for (const auto &g : groups) {
+    b2s_status st = L.stop ? B2S_ERR_BAD_STATE : serve_matches(n, g);
+    if (st && !L.stop) fail(g, st);
+    for (const auto &q : g) q.second->status = st;
+  }
+  n->timing[4] += seconds_since(t0);
+  if (!maps.empty()) {
+    t0 = std::chrono::steady_clock::now();
+    b2s_status st = L.stop ? B2S_ERR_BAD_STATE : serve_maps(n, maps, on_map, user);
+    if (st && !L.stop) fail(maps, st);
+    for (const auto &q : maps) q.second->status = st;
+    n->timing[5] += seconds_since(t0);
+  }
+}
+
+// the fields a node's getLaser derives, equal bit for bit
+bool same_bits(const void *a, const void *b, size_t n) { return std::memcmp(a, b, n) == 0; }
+bool same_laser(const b2s_laser &a, const b2s_laser &b) {
+  return a.n_readings == b.n_readings && same_bits(&a.min_angle, &b.min_angle, 8) &&
+         same_bits(&a.angular_resolution, &b.angular_resolution, 8) && same_bits(&a.min_range, &b.min_range, 8) &&
+         same_bits(&a.max_range, &b.max_range, 8) && same_bits(&a.range_threshold, &b.range_threshold, 8) &&
+         same_bits(a.offset_pose, b.offset_pose, sizeof a.offset_pose);
+}
+bool same_matcher(const b2s_matcher_params &a, const b2s_matcher_params &b) {
+  return same_bits(&a, &b, offsetof(b2s_matcher_params, use_response_expansion)) &&
+         a.use_response_expansion == b.use_response_expansion;
+}
+
+// a single-node entry point's callback behind the batched one
+struct SingleMapFn {
+  b2s_karto_map_fn fn;
+  void *user;
+};
+void single_map(void *user, int32_t, int32_t scan_index, const b2s_occ_grid_info *info, const int8_t *payload) {
+  const SingleMapFn *s = static_cast<const SingleMapFn *>(user);
+  if (s->fn) s->fn(s->user, scan_index, info, payload);
+}
+
+// the handle; `single`: b2s_karto_node_create's solver rule (any non-NULL solver is set), else a slot whose compute is
+// NULL means no back end
+b2s_status create_impl(int batch, const b2s_karto_node_params *params, const b2s_laser_scan_msg *geometry,
+                       const double *laser_mounts, const b2s_scan_solver *solvers, bool single, int device,
+                       b2s_karto_node **out) {
+  const char *fn = single ? "b2s_karto_node_create" : "b2s_karto_node_create_batch";
+  if (!out) B2S_FAIL(B2S_ERR_BAD_PARAMS, std::string(fn) + ": null argument");
+  *out = nullptr;
+  if (!params || !geometry || !laser_mounts) B2S_FAIL(B2S_ERR_BAD_PARAMS, std::string(fn) + ": null argument");
+  if (batch < 1) B2S_FAIL(B2S_ERR_BAD_PARAMS, std::string(fn) + ": batch must be positive");
+  if (batch > NODE_MAX_BATCH) B2S_FAIL(B2S_ERR_TOO_LARGE, std::string(fn) + ": at most 1024 nodes");
+  std::unique_ptr<b2s_karto_node, decltype(&b2s_karto_node_destroy)> n(new (std::nothrow) b2s_karto_node(),
+                                                                      b2s_karto_node_destroy);
+  if (!n) B2S_FAIL(B2S_ERR_CUDA, "out of host memory");
+  n->batch = batch;
+  n->device = device;
+  n->n_msg = geometry->n_ranges;
+  n->nodes.resize((size_t)batch);
+  for (int b = 0; b < batch; b++) {
+    const b2s_karto_node_params *p = params + b;
+    const double *laser_mount = laser_mounts + 7 * (size_t)b;
+    const std::string who = single ? std::string("b2s_karto_node_create: ")
+                                   : "b2s_karto_node_create_batch: node " + std::to_string(b) + ": ";
+    if (p->throttle_scans <= 0)
+      B2S_FAIL(B2S_ERR_BAD_PARAMS, who + "throttle_scans must be positive (the node divides by it)");
+    if (!(p->resolution > 0.0) || !std::isfinite(p->resolution))
+      B2S_FAIL(B2S_ERR_BAD_PARAMS, who + "resolution must be positive and finite");
+    const double iv = p->map_update_interval;
+    if (!std::isfinite(iv) || std::floor(iv) < -2147483648.0 || std::floor(iv) > 2147483647.0)
+      B2S_FAIL(B2S_ERR_BAD_PARAMS, who + "map_update_interval outside ros::Duration's range");
+    double qn = 0.0;
+    for (int k = 0; k < 7; k++)
+      if (!std::isfinite(laser_mount[k])) B2S_FAIL(B2S_ERR_BAD_PARAMS, who + "non-finite laser mount");
+    for (int k = 3; k < 7; k++) qn += laser_mount[k] * laser_mount[k];
+    if (!(qn > 0.0)) B2S_FAIL(B2S_ERR_BAD_PARAMS, who + "zero mount quaternion");
+
+    // getLaser: transformPose(base_frame_, identity in the laser frame), getYaw, and the upside-down test
+    const TfTransform base_laser = tf_from_row(laser_mount);
+    TfTransform identity;
+    tf_identity(identity);
+    const TfTransform laser_pose = tf_mul(base_laser, identity);
+    const double offset[3] = {laser_pose.o[0], laser_pose.o[1], yaw_of(laser_pose)};
+    const double up_in_laser[3] = {0, 0, 1 + laser_pose.o[2]};
+    double up[3];
+    tf_apply(tf_inverse(base_laser), up_in_laser, up);
+    b2s_laser laser;
+    if (b2s_status st = karto_laser_from_msg(geometry, offset, p->use_scan_range, &laser)) {
+      if (!single) set_last_error(who + b2s_last_error());
+      return st;
+    }
+    if (laser.n_readings < 1) B2S_FAIL(B2S_ERR_BAD_PARAMS, who + "the laser has no readings");
+    if (geometry->n_ranges < laser.n_readings)
+      B2S_FAIL(B2S_ERR_BAD_PARAMS, who + "the LaserScan carries fewer ranges than Round((angle_max - angle_min) / "
+                                         "angle_increment); the node would read past them");
+    b2s_mapper_params mp = p->mapper;
+    mp.sequential.range_threshold = laser.range_threshold;  // Mapper::Initialize takes the laser's (Mapper.cpp)
+    mp.loop.range_threshold = laser.range_threshold;
+    const bool inverted = up[2] <= 0;
+    if (b == 0) {
+      n->laser = laser;
+      n->inverted = inverted;
+      n->matcher_params[0] = mp.sequential;
+      n->matcher_params[1] = mp.loop;
+    } else {
+      // every node shares the two matchers and the map kernels' laser
+      if (!same_laser(laser, n->laser) || inverted != n->inverted)
+        B2S_FAIL(B2S_ERR_BAD_PARAMS, who + "its laser (offset, range threshold or upside-down flag) differs from node 0's");
+      if (!same_matcher(mp.sequential, n->matcher_params[0]) || !same_matcher(mp.loop, n->matcher_params[1]))
+        B2S_FAIL(B2S_ERR_BAD_PARAMS, who + "its matcher parameters (mapper.sequential / mapper.loop) differ from node 0's");
+    }
+    KartoNodeState &k = n->nodes[(size_t)b];
+    k.owner = n.get();
+    k.index = b;
+    k.prm = *p;
+    k.interval = ros_duration_from_sec(iv);
+    k.scan.resize((size_t)laser.n_readings);
+    if (b2s_status st = mapper_create_fleet(&mp, &laser, fleet_match, &k, &k.mapper)) {
+      if (!single) set_last_error(who + b2s_last_error());
+      return st;
+    }
+    const b2s_scan_solver *solver = solvers ? solvers + b : nullptr;
+    if (solver && (single || solver->compute))
+      if (b2s_status st = b2s_mapper_set_scan_solver(k.mapper, solver)) return st;
+    n->cap_base[0] = n->cap_base[1] = std::max(n->cap_base[0], std::max(32, p->mapper.scan_buffer_size + 1));
+  }
+  if (b2s_status st = check_device(device)) return st;
+  n->cap_batch = std::min(std::max(8, 2 * batch), MATCH_MAX_BATCH);
+  if (b2s_status st = occ_batch_create(n->laser, device, &n->maps)) return st;
+  *out = n.release();
   return B2S_OK;
 }
 
@@ -95,147 +576,133 @@ b2s_status update_map(b2s_karto_node *n, int32_t scan_index, b2s_karto_map_fn on
 
 extern "C" {
 
+b2s_status b2s_karto_node_create_batch(int batch, const b2s_karto_node_params *params, const b2s_laser_scan_msg *geometry,
+                                       const double *laser_mounts, const b2s_scan_solver *solvers, int device,
+                                       b2s_karto_node **out) {
+  return create_impl(batch, params, geometry, laser_mounts, solvers, false, device, out);
+}
+
 b2s_status b2s_karto_node_create(const b2s_karto_node_params *params, const b2s_laser_scan_msg *geometry,
                                  const double laser_mount[7], const b2s_scan_solver *solver, int device,
                                  b2s_karto_node **out) {
-  if (!out) B2S_FAIL(B2S_ERR_BAD_PARAMS, "b2s_karto_node_create: null argument");
-  *out = nullptr;
-  if (!params || !geometry || !laser_mount) B2S_FAIL(B2S_ERR_BAD_PARAMS, "b2s_karto_node_create: null argument");
-  if (params->throttle_scans <= 0)
-    B2S_FAIL(B2S_ERR_BAD_PARAMS, "b2s_karto_node_create: throttle_scans must be positive (the node divides by it)");
-  if (!(params->resolution > 0.0) || !std::isfinite(params->resolution))
-    B2S_FAIL(B2S_ERR_BAD_PARAMS, "b2s_karto_node_create: resolution must be positive and finite");
-  const double iv = params->map_update_interval;
-  if (!std::isfinite(iv) || std::floor(iv) < -2147483648.0 || std::floor(iv) > 2147483647.0)
-    B2S_FAIL(B2S_ERR_BAD_PARAMS, "b2s_karto_node_create: map_update_interval outside ros::Duration's range");
-  double qn = 0.0;
-  for (int k = 0; k < 7; k++)
-    if (!std::isfinite(laser_mount[k])) B2S_FAIL(B2S_ERR_BAD_PARAMS, "b2s_karto_node_create: non-finite laser mount");
-  for (int k = 3; k < 7; k++) qn += laser_mount[k] * laser_mount[k];
-  if (!(qn > 0.0)) B2S_FAIL(B2S_ERR_BAD_PARAMS, "b2s_karto_node_create: zero mount quaternion");
-
-  // getLaser: transformPose(base_frame_, identity in the laser frame), getYaw, and the upside-down test
-  const TfTransform base_laser = tf_from_row(laser_mount);
-  TfTransform identity;
-  tf_identity(identity);
-  const TfTransform laser_pose = tf_mul(base_laser, identity);
-  const double offset[3] = {laser_pose.o[0], laser_pose.o[1], yaw_of(laser_pose)};
-  const double up_in_laser[3] = {0, 0, 1 + laser_pose.o[2]};
-  double up[3];
-  tf_apply(tf_inverse(base_laser), up_in_laser, up);
-  b2s_laser laser;
-  if (b2s_status st = karto_laser_from_msg(geometry, offset, params->use_scan_range, &laser)) return st;
-  if (laser.n_readings < 1) B2S_FAIL(B2S_ERR_BAD_PARAMS, "b2s_karto_node_create: the laser has no readings");
-  if (geometry->n_ranges < laser.n_readings)
-    B2S_FAIL(B2S_ERR_BAD_PARAMS, "b2s_karto_node_create: the LaserScan carries fewer ranges than Round((angle_max - "
-                                 "angle_min) / angle_increment); the node would read past them");
-
-  b2s_mapper_params mp = params->mapper;
-  mp.sequential.range_threshold = laser.range_threshold;  // Mapper::Initialize takes the laser's (Mapper.cpp)
-  mp.loop.range_threshold = laser.range_threshold;
-  b2s_mapper *mapper = nullptr;
-  if (b2s_status st = b2s_mapper_create(&mp, &laser, device, &mapper)) return st;
-  if (solver) {
-    if (b2s_status st = b2s_mapper_set_scan_solver(mapper, solver)) {
-      b2s_mapper_destroy(mapper);
-      return st;
-    }
-  }
-  b2s_karto_node *n = new (std::nothrow) b2s_karto_node();
-  if (!n) {
-    b2s_mapper_destroy(mapper);
-    B2S_FAIL(B2S_ERR_CUDA, "out of host memory");
-  }
-  n->prm = *params;
-  n->laser = laser;
-  n->n_msg = geometry->n_ranges;
-  n->device = device;
-  n->inverted = up[2] <= 0;
-  n->base_laser = base_laser;
-  n->interval = ros_duration_from_sec(iv);
-  n->mapper = mapper;
-  n->scan.resize((size_t)laser.n_readings);
-  *out = n;
-  return B2S_OK;
+  return create_impl(1, params, geometry, laser_mount, solver, true, device, out);
 }
 
 void b2s_karto_node_destroy(b2s_karto_node *n) {
   if (!n) return;
-  b2s_mapper_destroy(n->mapper);
+  for (KartoNodeState &k : n->nodes) b2s_mapper_destroy(k.mapper);
+  for (b2s_matcher *h : n->h)
+    if (h) b2s_matcher_destroy(h);
+  occ_batch_destroy(n->maps);
   delete n;
 }
 
-b2s_mapper *b2s_karto_node_mapper(b2s_karto_node *n) { return n ? n->mapper : nullptr; }
+b2s_mapper *b2s_karto_node_mapper(b2s_karto_node *n) { return n && n->batch == 1 ? n->nodes[0].mapper : nullptr; }
+
+b2s_mapper *b2s_karto_node_mapper_of(b2s_karto_node *n, int b) {
+  return n && b >= 0 && b < n->batch ? n->nodes[(size_t)b].mapper : nullptr;
+}
+
+b2s_status b2s_karto_node_process_batch(b2s_karto_node *n, const int32_t *n_scans, const float *ranges,
+                                        const uint32_t *stamps, const double *odom, int32_t *out_state, double *out_pose,
+                                        double *out_map_to_odom, int32_t *out_map_published,
+                                        b2s_karto_node_batch_map_fn on_map, void *user) {
+  B2S_NVTX("SlamKarto::laserCallback");
+  if (!n || !n_scans) B2S_FAIL(B2S_ERR_BAD_PARAMS, "b2s_karto_node_process: null argument or negative count");
+  const int B = n->batch;
+  size_t T = 0;
+  for (int b = 0; b < B; b++) {
+    if (n_scans[b] < 0) B2S_FAIL(B2S_ERR_BAD_PARAMS, "b2s_karto_node_process: null argument or negative count");
+    T += (size_t)n_scans[b];
+  }
+  if (T > 0 && (!ranges || !stamps || !odom))
+    B2S_FAIL(B2S_ERR_BAD_PARAMS, "b2s_karto_node_process: null argument or negative count");
+  if (n->failed)
+    B2S_FAIL(B2S_ERR_BAD_STATE, "b2s_karto_node_process: an earlier call failed inside the Mapper; destroy the handle");
+  for (double &t : n->timing) t = 0;
+  if (T == 0) return B2S_OK;
+  const auto t0 = std::chrono::steady_clock::now();
+  const double bytes0 = occ_batch_bytes_d2h(n->maps);
+  B2S_CUDA_CHECK(cudaSetDevice(n->device));
+  const CallRows rows{ranges, stamps, odom, out_state, out_pose, out_map_to_odom, out_map_published};
+  Lockstep L;
+  L.posted.assign((size_t)B, nullptr);
+  n->lock = &L;
+  std::vector<std::thread> threads;
+  threads.reserve((size_t)B);
+  {
+    std::lock_guard<std::mutex> g(L.mu);  // no worker posts before every worker is counted
+    size_t first = 0;
+    for (int b = 0; b < B; b++) {
+      if (n_scans[b] > 0) {
+        try {
+          threads.emplace_back(worker, n, b, first, (int)n_scans[b], std::cref(rows));
+          L.live++;
+        } catch (...) {
+          Failure f;
+          f.round = 0;
+          f.node = b;
+          f.status = B2S_ERR_CUDA;
+          f.message = "could not start a worker thread";
+          L.fail(f);
+          break;
+        }
+      }
+      first += (size_t)n_scans[b];
+    }
+  }
+  // the dispatcher
+  std::vector<std::pair<int, Request *>> reqs;
+  for (;;) {
+    {
+      std::unique_lock<std::mutex> g(L.mu);
+      L.to_dispatcher.wait(g, [&] { return L.waiting == L.live; });
+      if (L.live == 0) break;
+      reqs.clear();
+      for (int b = 0; b < B; b++)
+        if (L.posted[(size_t)b]) reqs.emplace_back(b, L.posted[(size_t)b]);
+    }
+    serve_round(n, L, reqs, on_map, user);
+    n->timing[0] += 1;
+    {
+      std::lock_guard<std::mutex> g(L.mu);
+      for (auto &q : reqs) {
+        q.second->done = true;
+        L.posted[(size_t)q.first] = nullptr;
+      }
+      L.waiting = 0;
+      L.round++;
+    }
+    L.to_workers.notify_all();
+  }
+  for (std::thread &t : threads) t.join();
+  n->lock = nullptr;
+  n->timing[6] = occ_batch_bytes_d2h(n->maps) - bytes0;
+  n->timing[7] = seconds_since(t0);
+  if (L.first.node >= 0) {
+    // the Mappers, the maps handed out and the nodes' rows up to their stop have moved
+    n->failed = true;
+    set_last_error(B > 1 ? "b2s_karto_node_process_batch: node " + std::to_string(L.first.node) + ": " + L.first.message
+                         : L.first.message);
+    return L.first.status;
+  }
+  return B2S_OK;
+}
 
 b2s_status b2s_karto_node_process(b2s_karto_node *n, int n_scans, const float *ranges, const uint32_t *stamps,
                                   const double *odom, int32_t *out_state, double *out_pose, double *out_map_to_odom,
                                   int32_t *out_map_published, b2s_karto_map_fn on_map, void *user) {
-  B2S_NVTX("SlamKarto::laserCallback");
-  if (!n || n_scans < 0 || (n_scans > 0 && (!ranges || !stamps || !odom)))
-    B2S_FAIL(B2S_ERR_BAD_PARAMS, "b2s_karto_node_process: null argument or negative count");
-  if (n->failed)
-    B2S_FAIL(B2S_ERR_BAD_STATE, "b2s_karto_node_process: an earlier call failed inside the Mapper; destroy the handle");
-  const int m = n->laser.n_readings, nr = n->n_msg;
-  for (int i = 0; i < n_scans; i++) {
-    const int32_t scan_index = (int32_t)n->laser_count;
-    int32_t state = B2S_KARTO_THROTTLED, published = 0;
-    double pose[3] = {0, 0, 0};
-    n->laser_count++;
-    if (n->laser_count % n->prm.throttle_scans == 0) {
-      // getOdomPose: transformPose(odom_frame_, identity in base_frame_) at the scan's stamp
-      const double *row = odom + 7 * (size_t)i;
-      bool ok = true;
-      for (int k = 0; k < 7; k++) ok = ok && !std::isnan(row[k]);
-      if (!ok) {
-        state = B2S_KARTO_NO_ODOM;
-      } else {
-        const TfTransform odom_base = tf_from_row(row);
-        double ident[7] = {0, 0, 0};  // tf::Transform(createQuaternionFromRPY(0, 0, 0), (0, 0, 0))
-        quat_set_rpy(0, 0, 0, ident + 3);
-        const TfTransform op = tf_mul(odom_base, tf_from_row(ident));
-        const double odom_pose[3] = {op.o[0], op.o[1], yaw_of(op)};
-        // addScan: float32 ranges widened, reversed for an upside-down laser; the laser's m readings are used
-        const float *r = ranges + (size_t)i * nr;
-        for (int k = 0; k < m; k++) n->scan[k] = (double)r[n->inverted ? nr - 1 - k : k];
-        int32_t processed = 0;
-        b2s_status st = b2s_mapper_process_sensor(n->mapper, "laser", n->scan.data(), odom_pose, 0.0, &processed, pose);
-        if (st) {
-          n->failed = true;
-          return st;
-        }
-        if (!processed) {
-          state = B2S_KARTO_NOT_MOVED;
-          pose[0] = pose[1] = pose[2] = 0;
-        } else {
-          state = B2S_KARTO_PROCESSED;
-          n->readings.insert(n->readings.end(), n->scan.begin(), n->scan.end());
-          // map_to_odom_ = (odom <- base_link * T(corrected)^-1) rebuilt from its quaternion and origin, inverted
-          double corrected[7] = {pose[0], pose[1], 0.0}, odom_to_map[7];
-          quat_set_rpy(0, 0, pose[2], corrected + 3);
-          tf_to_row(tf_mul(odom_base, tf_inverse(tf_from_row(corrected))), odom_to_map);
-          tf_to_row(tf_inverse(tf_from_row(odom_to_map)), n->map_to_odom);
-          const uint32_t *s = stamps + 2 * (size_t)i;
-          if (!n->got_map || ros_duration_gt(ros_time_diff(s[0], s[1], n->last_map_sec, n->last_map_nsec), n->interval)) {
-            bool done = false;
-            if ((st = update_map(n, scan_index, on_map, user, done))) {
-              n->failed = true;
-              return st;
-            }
-            if (done) {
-              n->last_map_sec = s[0];
-              n->last_map_nsec = s[1];
-              n->got_map = true;
-              published = 1;
-            }
-          }
-        }
-      }
-    }
-    if (out_state) out_state[i] = state;
-    if (out_pose) std::memcpy(out_pose + 3 * (size_t)i, pose, sizeof pose);
-    if (out_map_to_odom) std::memcpy(out_map_to_odom + 7 * (size_t)i, n->map_to_odom, sizeof n->map_to_odom);
-    if (out_map_published) out_map_published[i] = published;
-  }
+  if (n && n->batch != 1) B2S_FAIL(B2S_ERR_BAD_PARAMS, "b2s_karto_node_process: the handle has several nodes");
+  if (n_scans < 0) B2S_FAIL(B2S_ERR_BAD_PARAMS, "b2s_karto_node_process: null argument or negative count");
+  const int32_t count = n_scans;
+  SingleMapFn fn{on_map, user};
+  return b2s_karto_node_process_batch(n, &count, ranges, stamps, odom, out_state, out_pose, out_map_to_odom,
+                                      out_map_published, single_map, &fn);
+}
+
+b2s_status b2s_karto_node_last_timing(const b2s_karto_node *n, double out[8]) {
+  if (!n || !out) B2S_FAIL(B2S_ERR_BAD_PARAMS, "null argument");
+  std::memcpy(out, n->timing, sizeof n->timing);
   return B2S_OK;
 }
 

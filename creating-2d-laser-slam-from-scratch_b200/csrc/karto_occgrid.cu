@@ -38,24 +38,28 @@ struct b2s_occ_grid {
 
 namespace b2s {
 
+// ---- per-beam / per-scan / per-cell device code, shared by the single-grid kernels and the batched build below
+
 // per-scan bounding box over the sensor position and the FILTERED point readings
-// (InRange(reading, minRange, rangeThreshold), Karto.h:5382,5400,5418-5424).  One block per scan.
-__global__ void k_scan_bbox(const double *__restrict__ ranges, const double *__restrict__ sensor,
-                            const double *__restrict__ pts, b2s_laser l, double *__restrict__ bbox) {
-  const int s = blockIdx.x, n = l.n_readings;
+// (InRange(reading, minRange, rangeThreshold), Karto.h:5382,5400,5418-5424).  One block of 256 threads per scan;
+// `ranges` and `pts` point at the scan's own row.
+template <class R>
+__device__ void scan_bbox_block(const R *__restrict__ ranges, const double *__restrict__ sensor,
+                                const double *__restrict__ pts, const b2s_laser &l, double *__restrict__ bbox) {
+  const int n = l.n_readings;
   const double big = 999999999999999999.99999;  // Karto.h:2765
   double mnx = big, mny = big, mxx = -big, mxy = -big;
   if (threadIdx.x == 0) {
-    double x = sensor[3 * s], y = sensor[3 * s + 1];
+    double x = sensor[0], y = sensor[1];
     if (x < mnx) mnx = x;
     if (y < mny) mny = y;
     if (x > mxx) mxx = x;
     if (y > mxy) mxy = y;
   }
   for (int i = threadIdx.x; i < n; i += blockDim.x) {
-    double r = ranges[(size_t)s * n + i];
+    double r = (double)ranges[i];
     if (!(r >= l.min_range && r <= l.range_threshold)) continue;
-    double x = pts[((size_t)s * n + i) * 2], y = pts[((size_t)s * n + i) * 2 + 1];
+    double x = pts[(size_t)i * 2], y = pts[(size_t)i * 2 + 1];
     if (x < mnx) mnx = x;
     if (y < mny) mny = y;
     if (x > mxx) mxx = x;
@@ -74,12 +78,12 @@ __global__ void k_scan_bbox(const double *__restrict__ ranges, const double *__r
     __syncthreads();
   }
   if (threadIdx.x == 0) {
-    bbox[4 * s] = sh[0][0]; bbox[4 * s + 1] = sh[1][0]; bbox[4 * s + 2] = sh[2][0]; bbox[4 * s + 3] = sh[3][0];
+    bbox[0] = sh[0][0]; bbox[1] = sh[1][0]; bbox[2] = sh[2][0]; bbox[3] = sh[3][0];
   }
 }
 
-// union of the per-scan boxes (OccupancyGrid::ComputeDimensions, Karto.h:5810-5814); single block
-__global__ void k_bbox_union(const double *__restrict__ bbox, int n_scans, double *__restrict__ out) {
+// union of n_scans per-scan boxes (OccupancyGrid::ComputeDimensions, Karto.h:5810-5814); one block of 256 threads
+__device__ void bbox_union_block(const double *__restrict__ bbox, int n_scans, double *__restrict__ out) {
   const double big = 999999999999999999.99999;
   double mnx = big, mny = big, mxx = -big, mxy = -big;
   for (int s = threadIdx.x; s < n_scans; s += blockDim.x) {
@@ -103,7 +107,76 @@ __global__ void k_bbox_union(const double *__restrict__ bbox, int n_scans, doubl
   if (threadIdx.x == 0) { out[0] = sh[0][0]; out[1] = sh[1][0]; out[2] = sh[2][0]; out[3] = sh[3][0]; }
 }
 
-// OccupancyGrid::AddScan + RayTrace + Grid::TraceLine (Karto.h:5852-5945, 4680-4745).  One warp per beam.
+// OccupancyGrid::AddScan + RayTrace + Grid::TraceLine (Karto.h:5852-5945, 4680-4745) for ONE beam, by one warp: the
+// lanes split the Bresenham steps.  Returns the cell visits this lane counted.
+__device__ __forceinline__ unsigned long long trace_beam(double rr, double sx, double sy, double px, double py,
+                                                         const b2s_laser &l, int w, int h, int step, double off_x,
+                                                         double off_y, double scale, int lane, uint32_t *__restrict__ pass,
+                                                         uint32_t *__restrict__ hit) {
+  if (rr <= l.min_range || rr >= l.max_range || isnan(rr)) return 0;  // Karto.h:5873-5878
+  unsigned long long visits = 0;
+  const bool end_valid = rr < (l.range_threshold - KT_TOLERANCE);     // Karto.h:5871
+  if (rr >= l.range_threshold) {  // Karto.h:5879-5887: clip to the range threshold, no hit
+    const double ratio = l.range_threshold / rr;
+    const double dx = px - sx, dy = py - sy;
+    px = __dadd_rn(sx, __dmul_rn(ratio, dx));
+    py = __dadd_rn(sy, __dmul_rn(ratio, dy));
+  }
+  int x0 = world_to_grid_1(sx, off_x, scale), y0 = world_to_grid_1(sy, off_y, scale);
+  int x1 = world_to_grid_1(px, off_x, scale), y1 = world_to_grid_1(py, off_y, scale);
+  const int tx = x1, ty = y1;
+  // TraceLine canonicalisation (Karto.h:4682-4692)
+  const bool steep = abs(y1 - y0) > abs(x1 - x0);
+  if (steep) { int t = x0; x0 = y0; y0 = t; t = x1; x1 = y1; y1 = t; }
+  if (x0 > x1) { int t = x0; x0 = x1; x1 = t; t = y0; y0 = y1; y1 = t; }
+  const long long dx = (long long)x1 - x0, dy = llabs((long long)y1 - y0);
+  const int ystep = (y0 < y1) ? 1 : -1;
+  for (long long k = lane; k <= dx; k += 32) {
+    // y before the update of step k: increments so far = floor((2*k*dy + dx) / (2*dx))  (0 when dx == 0)
+    const long long inc = dx > 0 ? (2 * k * dy + dx) / (2 * dx) : 0;
+    const int x = x0 + (int)k, y = y0 + ystep * (int)inc;
+    const int cx = steep ? y : x, cy = steep ? x : y;
+    if (cx >= 0 && cx < w && cy >= 0 && cy < h) {
+      atomicAdd(pass + cx + (size_t)cy * step, 1u);
+      visits++;
+    }
+  }
+  if (lane == 0 && end_valid && tx >= 0 && tx < w && ty >= 0 && ty < h) {  // Karto.h:5924-5942
+    atomicAdd(pass + tx + (size_t)ty * step, 1u);
+    atomicAdd(hit + tx + (size_t)ty * step, 1u);
+    visits += 2;
+  }
+  return visits;
+}
+
+// OccupancyGrid::UpdateCell (Karto.h:5970-5990): MinPassThrough = 2, OccupancyThreshold = 0.1
+__device__ __forceinline__ uint8_t occ_cell_value(uint32_t p, uint32_t h) {
+  uint8_t v = 0;
+  if (p > 2u) {
+    const double ratio = (double)h / (double)p;
+    v = ratio > 0.1 ? (uint8_t)GRID_OCCUPIED : (uint8_t)GRID_FREE;
+  }
+  return v;
+}
+
+// SlamKarto::updateMap payload (karto_slam.cc:546-569): unknown -> -1, occupied -> 100, free -> 0
+__device__ __forceinline__ int8_t occ_ros_value(uint8_t v) { return v == 0 ? -1 : (v == GRID_OCCUPIED ? 100 : 0); }
+
+// ---- the single-grid kernels (b2s_occ_grid_*)
+
+// One block per scan.
+__global__ void k_scan_bbox(const double *__restrict__ ranges, const double *__restrict__ sensor,
+                            const double *__restrict__ pts, b2s_laser l, double *__restrict__ bbox) {
+  const int s = blockIdx.x, n = l.n_readings;
+  scan_bbox_block(ranges + (size_t)s * n, sensor + 3 * s, pts + (size_t)s * n * 2, l, bbox + 4 * s);
+}
+
+// single block
+__global__ void k_bbox_union(const double *__restrict__ bbox, int n_scans, double *__restrict__ out) {
+  bbox_union_block(bbox, n_scans, out);
+}
+
+// One warp per beam.
 __global__ void __launch_bounds__(256)
     k_raytrace(const double *__restrict__ ranges, const double *__restrict__ sensor, const double *__restrict__ pts,
                b2s_laser l, long long n_beams, int w, int h, int step, double off_x, double off_y, double scale,
@@ -115,71 +188,110 @@ __global__ void __launch_bounds__(256)
   unsigned long long my_visits = 0;
   for (long long beam = warp0; beam < n_beams; beam += nwarps) {
     const int s = (int)(beam / n);
-    const double rr = ranges[beam];
-    if (rr <= l.min_range || rr >= l.max_range || isnan(rr)) continue;  // Karto.h:5873-5878
-    const bool end_valid = rr < (l.range_threshold - KT_TOLERANCE);     // Karto.h:5871
-    const double sx = sensor[3 * s], sy = sensor[3 * s + 1];
-    double px = pts[beam * 2], py = pts[beam * 2 + 1];
-    if (rr >= l.range_threshold) {  // Karto.h:5879-5887: clip to the range threshold, no hit
-      const double ratio = l.range_threshold / rr;
-      const double dx = px - sx, dy = py - sy;
-      px = __dadd_rn(sx, __dmul_rn(ratio, dx));
-      py = __dadd_rn(sy, __dmul_rn(ratio, dy));
-    }
-    int x0 = world_to_grid_1(sx, off_x, scale), y0 = world_to_grid_1(sy, off_y, scale);
-    int x1 = world_to_grid_1(px, off_x, scale), y1 = world_to_grid_1(py, off_y, scale);
-    const int tx = x1, ty = y1;
-    // TraceLine canonicalisation (Karto.h:4682-4692)
-    const bool steep = abs(y1 - y0) > abs(x1 - x0);
-    if (steep) { int t = x0; x0 = y0; y0 = t; t = x1; x1 = y1; y1 = t; }
-    if (x0 > x1) { int t = x0; x0 = x1; x1 = t; t = y0; y0 = y1; y1 = t; }
-    const long long dx = (long long)x1 - x0, dy = llabs((long long)y1 - y0);
-    const int ystep = (y0 < y1) ? 1 : -1;
-    for (long long k = lane; k <= dx; k += 32) {
-      // y before the update of step k: increments so far = floor((2*k*dy + dx) / (2*dx))  (0 when dx == 0)
-      const long long inc = dx > 0 ? (2 * k * dy + dx) / (2 * dx) : 0;
-      const int x = x0 + (int)k, y = y0 + ystep * (int)inc;
-      const int cx = steep ? y : x, cy = steep ? x : y;
-      if (cx >= 0 && cx < w && cy >= 0 && cy < h) {
-        atomicAdd(pass + cx + (size_t)cy * step, 1u);
-        my_visits++;
-      }
-    }
-    if (lane == 0 && end_valid && tx >= 0 && tx < w && ty >= 0 && ty < h) {  // Karto.h:5924-5942
-      atomicAdd(pass + tx + (size_t)ty * step, 1u);
-      atomicAdd(hit + tx + (size_t)ty * step, 1u);
-      my_visits += 2;
-    }
+    my_visits += trace_beam(ranges[beam], sensor[3 * s], sensor[3 * s + 1], pts[beam * 2], pts[beam * 2 + 1], l, w, h,
+                            step, off_x, off_y, scale, lane, pass, hit);
   }
 #pragma unroll
   for (int d = 16; d > 0; d >>= 1) my_visits += __shfl_xor_sync(0xffffffffu, my_visits, d);
   if (lane == 0 && my_visits) atomicAdd(visits, my_visits);
 }
 
-// OccupancyGrid::Update / UpdateCell (Karto.h:5953-5990): MinPassThrough = 2, OccupancyThreshold = 0.1
+// OccupancyGrid::Update (Karto.h:5953-5968)
 __global__ void k_occ_threshold(const uint32_t *__restrict__ pass, const uint32_t *__restrict__ hit, int n,
                                 uint8_t *__restrict__ cells) {
   int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
-  uint8_t v = 0;
-  const uint32_t p = pass[i];
-  if (p > 2u) {
-    const double ratio = (double)hit[i] / (double)p;
-    v = ratio > 0.1 ? (uint8_t)GRID_OCCUPIED : (uint8_t)GRID_FREE;
-  }
-  cells[i] = v;
+  cells[i] = occ_cell_value(pass[i], hit[i]);
 }
 
-// SlamKarto::updateMap payload (karto_slam.cc:546-569): unknown -> -1, occupied -> 100, free -> 0; row-major w x h
+// row-major w x h payload
 __global__ void k_occ_ros(const uint8_t *__restrict__ cells, int w, int h, int step, int8_t *__restrict__ out) {
   int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= w * h) return;
   const int x = i % w, y = i / w;
-  const uint8_t v = cells[x + (size_t)y * step];
-  out[i] = v == 0 ? -1 : (v == GRID_OCCUPIED ? 100 : 0);
+  out[i] = occ_ros_value(cells[x + (size_t)y * step]);
+}
+
+// ---- the batched build: G grids, each CreateFromScans over its own scans, every stage one launch for all grids.
+// Scans are numbered over all grids (grid 0's first); their readings are rows of a float32 pool.
+
+struct OccGridDev {     // one grid of a batched build, as its kernels read it
+  int w, h, step, scans;  // scans: the grid's scan count
+  double off_x, off_y, scale;
+  long long counters;   // first counter of the grid in the pass / hit arena
+  long long payload;    // first byte of its payload in the payload arena
+};
+
+// per-scan boxes; one block per scan, blockIdx.x = the scan's number over all grids
+__global__ void k_scan_bbox_rows(const float *__restrict__ pool, const int32_t *__restrict__ rows,
+                                 const double *__restrict__ sensor, const double *__restrict__ pts, b2s_laser l,
+                                 double *__restrict__ bbox) {
+  const int s = blockIdx.x, n = l.n_readings;
+  scan_bbox_block(pool + (size_t)rows[s] * n, sensor + 3 * s, pts + (size_t)s * n * 2, l, bbox + 4 * s);
+}
+
+// per-grid union; one block per grid, first[g] = the grid's first scan
+__global__ void k_bbox_union_grids(const double *__restrict__ bbox, const int32_t *__restrict__ first,
+                                   const int32_t *__restrict__ count, double *__restrict__ out) {
+  const int g = blockIdx.x;
+  bbox_union_block(bbox + 4 * (size_t)first[g], count[g], out + 4 * g);
+}
+
+// every beam of every scan of every grid, one warp per beam; scan_grid[s] = the grid scan s belongs to
+__global__ void __launch_bounds__(256)
+    k_raytrace_grids(const float *__restrict__ pool, const int32_t *__restrict__ rows,
+                     const int32_t *__restrict__ scan_grid, const double *__restrict__ sensor,
+                     const double *__restrict__ pts, b2s_laser l, long long n_beams,
+                     const OccGridDev *__restrict__ grids, uint32_t *__restrict__ pass, uint32_t *__restrict__ hit,
+                     unsigned long long *__restrict__ visits) {
+  const int lane = threadIdx.x & 31;
+  const long long warp0 = ((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+  const long long nwarps = ((long long)gridDim.x * blockDim.x) >> 5;
+  const int n = l.n_readings;
+  for (long long beam = warp0; beam < n_beams; beam += nwarps) {
+    const int s = (int)(beam / n), i = (int)(beam - (long long)s * n);
+    const int g = scan_grid[s];
+    const OccGridDev G = grids[g];
+    if (G.w <= 0 || G.h <= 0) continue;
+    unsigned long long v = trace_beam((double)pool[(size_t)rows[s] * n + i], sensor[3 * s], sensor[3 * s + 1],
+                                      pts[beam * 2], pts[beam * 2 + 1], l, G.w, G.h, G.step, G.off_x, G.off_y,
+                                      G.scale, lane, pass + G.counters, hit + G.counters);
+#pragma unroll
+    for (int d = 16; d > 0; d >>= 1) v += __shfl_xor_sync(0xffffffffu, v, d);
+    if (lane == 0 && v) atomicAdd(visits + g, v);
+  }
+}
+
+// thresholds and ROS payload of every grid: blockIdx.y = grid, x-blocks stride over its w x h cells
+__global__ void k_occ_ros_grids(const uint32_t *__restrict__ pass, const uint32_t *__restrict__ hit,
+                                const OccGridDev *__restrict__ grids, int8_t *__restrict__ out) {
+  const OccGridDev G = grids[blockIdx.y];
+  const long long cells = (long long)G.w * G.h;
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < cells; i += (long long)gridDim.x * blockDim.x) {
+    const int x = (int)(i % G.w), y = (int)(i / G.w);
+    const size_t c = (size_t)G.counters + x + (size_t)y * G.step;
+    out[G.payload + i] = occ_ros_value(occ_cell_value(pass[c], hit[c]));
+  }
 }
 
 }  // namespace b2s
+
+// OccupancyGrid::ComputeDimensions (Karto.h:5816-5821) from the scans' box {min x, min y, max x, max y}
+static b2s_status occ_dims(const double bb[4], double resolution, b2s_occ_grid_info &I) {
+  const double scale = 1.0 / resolution;
+  I.width = cast_i32(kround((bb[2] - bb[0]) * scale));
+  I.height = cast_i32(kround((bb[3] - bb[1]) * scale));
+  // the counters hold width_step * height cells (rows padded to 8), indexed and sized in int32
+  if (I.width < 0 || I.height < 0 || I.width > INT32_MAX - 7 || ((long long)I.width + 7) / 8 * 8 * I.height > INT32_MAX)
+    B2S_FAIL(B2S_ERR_TOO_LARGE, "occupancy grid dimensions out of range");
+  I.width_step = (I.width + 7) & ~7;
+  I.data_size = I.width_step * I.height;
+  I.offset[0] = bb[0];
+  I.offset[1] = bb[1];
+  I.resolution = resolution;
+  I.cell_visits = 0;
+  return B2S_OK;
+}
 
 extern "C" void b2s_occ_grid_destroy(b2s_occ_grid *g);
 extern "C" {
@@ -236,20 +348,9 @@ static b2s_status occ_create_impl(const b2s_laser *laser, int n_scans, const dou
     for (int i = 0; i < 4; i++) bbox_out[i] = bb[i];
     return B2S_OK;
   }
-  // OccupancyGrid::ComputeDimensions (Karto.h:5816-5821)
   const double scale = 1.0 / resolution;
   b2s_occ_grid_info &I = g->info;
-  I.width = cast_i32(kround((bb[2] - bb[0]) * scale));
-  I.height = cast_i32(kround((bb[3] - bb[1]) * scale));
-  // the counters hold width_step * height cells (rows padded to 8), indexed and sized in int32
-  if (I.width < 0 || I.height < 0 || I.width > INT32_MAX - 7 || ((long long)I.width + 7) / 8 * 8 * I.height > INT32_MAX)
-    B2S_FAIL(B2S_ERR_TOO_LARGE, "occupancy grid dimensions out of range");
-  I.width_step = (I.width + 7) & ~7;
-  I.data_size = I.width_step * I.height;
-  I.offset[0] = bb[0];
-  I.offset[1] = bb[1];
-  I.resolution = resolution;
-  I.cell_visits = 0;
+  if (b2s_status s = occ_dims(bb, resolution, I)) return s;
   const size_t cells = (size_t)std::max(I.data_size, 1);
   B2S_CUDA_CHECK(g->d_pass.reserve(cells));
   B2S_CUDA_CHECK(g->d_hit.reserve(cells));
@@ -396,3 +497,235 @@ void b2s_occ_grid_destroy(b2s_occ_grid *g) {
 }
 
 }  // extern "C"
+
+// ---- batched builds: CreateFromScans for many grids at once over a device-resident float32 pool of readings
+namespace b2s {
+
+struct OccBatch {
+  Stream stream;  // first: destroyed last
+  int device = 0;
+  b2s_laser laser{};
+  Buf<float> d_pool;                 // [pool_rows][n_readings] readings, each uploaded once
+  size_t pool_rows = 0;
+  HostBuf<float> h_stage;            // page-locked staging of appended rows
+  Buf<int32_t> d_rows, d_first, d_count, d_scan_grid;
+  Buf<double> d_poses, d_sensor, d_pts, d_bbox, d_union;
+  Buf<OccGridDev> d_grids;
+  Buf<uint32_t> d_pass, d_hit;       // one arena of counters for every grid of a build
+  Buf<unsigned long long> d_visits;
+  Buf<int8_t> d_payload;
+  HostBuf<int32_t> h_i32;            // rows, first, count, scan_grid of a build
+  HostBuf<double> h_f64;             // poses of a build; the unions read back
+  HostBuf<OccGridDev> h_grids;
+  HostBuf<unsigned long long> h_visits;
+  HostBuf<int8_t> h_payload;         // every payload of the last build
+  std::vector<OccGridDev> grids;
+  double bytes_d2h = 0;              // read back over the handle's life
+};
+
+b2s_status occ_batch_create(const b2s_laser &laser, int device, OccBatch **out) {
+  *out = nullptr;
+  if (b2s_status st = open_device(device)) return st;
+  std::unique_ptr<OccBatch> b(new (std::nothrow) OccBatch());
+  if (!b) B2S_FAIL(B2S_ERR_CUDA, "out of host memory");
+  b->device = device;
+  b->laser = laser;
+  B2S_CUDA_CHECK(b->stream.init(nullptr));
+  *out = b.release();
+  return B2S_OK;
+}
+
+void occ_batch_destroy(OccBatch *b) {
+  if (!b) return;
+  cudaSetDevice(b->device);
+  cudaStreamSynchronize(b->stream);
+  delete b;
+}
+
+double occ_batch_bytes_d2h(const OccBatch *b) { return b ? b->bytes_d2h : 0.0; }
+
+// rows [count][n_readings] (host) appended to the pool in one copy; *first = the first new row
+b2s_status occ_batch_append(OccBatch *b, int count, const float *rows, int32_t *first) {
+  const size_t n = (size_t)std::max(b->laser.n_readings, 1);
+  *first = (int32_t)b->pool_rows;
+  if (count <= 0) return B2S_OK;
+  if (b->pool_rows + (size_t)count > (size_t)INT32_MAX) B2S_FAIL(B2S_ERR_TOO_LARGE, "occupancy grid pool: too many scans");
+  B2S_CUDA_CHECK(cudaSetDevice(b->device));
+  cudaStream_t st = b->stream;
+  if ((b->pool_rows + count) * n > b->d_pool.cap) {  // full: twice the rows (256 at first)
+    Buf<float> fresh;
+    B2S_CUDA_CHECK(fresh.reserve(std::max<size_t>(std::max<size_t>(256, 2 * b->pool_rows), b->pool_rows + count) * n));
+    if (b->pool_rows)
+      B2S_CUDA_CHECK(cudaMemcpyAsync(fresh, b->d_pool, sizeof(float) * b->pool_rows * n, cudaMemcpyDeviceToDevice, st));
+    B2S_CUDA_CHECK(cudaStreamSynchronize(st));
+    b->d_pool = std::move(fresh);
+  }
+  B2S_CUDA_CHECK(cudaStreamSynchronize(st));  // the staging buffer is free again
+  B2S_CUDA_CHECK(b->h_stage.reserve((size_t)count * n));
+  std::memcpy(b->h_stage, rows, sizeof(float) * (size_t)count * (size_t)b->laser.n_readings);
+  B2S_CUDA_CHECK(cudaMemcpyAsync(b->d_pool + b->pool_rows * n, b->h_stage, sizeof(float) * count * n,
+                                 cudaMemcpyHostToDevice, st));
+  b->pool_rows += (size_t)count;
+  return B2S_OK;
+}
+
+// G grids, grid g = CreateFromScans over n_scans[g] scans: pool rows rows[], robot poses poses[][3] (grid 0's scans
+// first) at resolution[g].  have[g] = 0 when the grid has no scans (CreateFromScans returns NULL), else info[g] and
+// payload[g] (valid until the next build) are its map.
+b2s_status occ_batch_build(OccBatch *b, int G, const int32_t *n_scans, const int32_t *rows, const double *poses,
+                           const double *resolution, b2s_occ_grid_info *info, int32_t *have, const int8_t **payload) {
+  B2S_NVTX("K2c OccupancyGrid::CreateFromScans, batched");
+  const b2s_laser &l = b->laser;
+  const size_t n = (size_t)std::max(l.n_readings, 0);
+  size_t M = 0;
+  for (int g = 0; g < G; g++) {
+    have[g] = n_scans[g] > 0;
+    payload[g] = nullptr;
+    M += (size_t)std::max(n_scans[g], 0);
+    if (n_scans[g] > 0 && double_equal(resolution[g], 0.0)) B2S_FAIL(B2S_ERR_BAD_PARAMS, "Resolution cannot be 0");
+  }
+  if (M == 0) return B2S_OK;
+  B2S_CUDA_CHECK(cudaSetDevice(b->device));
+  cudaStream_t st = b->stream;
+  B2S_CUDA_CHECK(cudaStreamSynchronize(st));  // the page-locked buffers of the previous build are free
+  // the build's scans: pool rows, poses, and per grid its first scan and count (grids without scans are left out)
+  std::vector<int> live;
+  for (int g = 0; g < G; g++)
+    if (n_scans[g] > 0) live.push_back(g);
+  const int L = (int)live.size();
+  B2S_CUDA_CHECK(b->h_i32.reserve(2 * M + 2 * (size_t)L));
+  B2S_CUDA_CHECK(b->h_f64.reserve(std::max<size_t>(3 * M, 4 * (size_t)L)));
+  int32_t *h_rows = b->h_i32, *h_grid = h_rows + M, *h_first = h_grid + M, *h_count = h_first + L;
+  {
+    size_t s = 0;
+    for (int j = 0; j < L; j++) {
+      const int g = live[(size_t)j];
+      h_first[j] = (int32_t)s;
+      h_count[j] = n_scans[g];
+      for (int k = 0; k < n_scans[g]; k++) h_grid[s + k] = j;
+      s += (size_t)n_scans[g];
+    }
+  }
+  {
+    size_t s = 0;
+    for (int g = 0, src = 0; g < G; g++) {
+      const size_t c = (size_t)std::max(n_scans[g], 0);
+      if (c) {
+        std::memcpy(h_rows + s, rows + src, sizeof(int32_t) * c);
+        std::memcpy((double *)b->h_f64 + 3 * s, poses + 3 * (size_t)src, sizeof(double) * 3 * c);
+        s += c;
+      }
+      src += (int)c;
+    }
+  }
+  for (size_t s = 0; s < M; s++)
+    if (h_rows[s] < 0 || (size_t)h_rows[s] >= b->pool_rows) B2S_FAIL(B2S_ERR_OUT_OF_RANGE, "occupancy grid pool row out of range");
+  B2S_CUDA_CHECK(b->d_rows.reserve(M));
+  B2S_CUDA_CHECK(b->d_scan_grid.reserve(M));
+  B2S_CUDA_CHECK(b->d_first.reserve((size_t)L));
+  B2S_CUDA_CHECK(b->d_count.reserve((size_t)L));
+  B2S_CUDA_CHECK(b->d_poses.reserve(3 * M));
+  B2S_CUDA_CHECK(b->d_sensor.reserve(3 * M));
+  B2S_CUDA_CHECK(b->d_pts.reserve(M * std::max<size_t>(n, 1) * 2));
+  B2S_CUDA_CHECK(b->d_bbox.reserve(4 * M));
+  B2S_CUDA_CHECK(b->d_union.reserve(4 * (size_t)L));
+  B2S_CUDA_CHECK(cudaMemcpyAsync(b->d_rows, h_rows, sizeof(int32_t) * M, cudaMemcpyHostToDevice, st));
+  B2S_CUDA_CHECK(cudaMemcpyAsync(b->d_scan_grid, h_grid, sizeof(int32_t) * M, cudaMemcpyHostToDevice, st));
+  B2S_CUDA_CHECK(cudaMemcpyAsync(b->d_first, h_first, sizeof(int32_t) * L, cudaMemcpyHostToDevice, st));
+  B2S_CUDA_CHECK(cudaMemcpyAsync(b->d_count, h_count, sizeof(int32_t) * L, cudaMemcpyHostToDevice, st));
+  B2S_CUDA_CHECK(cudaMemcpyAsync(b->d_poses, b->h_f64, sizeof(double) * 3 * M, cudaMemcpyHostToDevice, st));
+  // points, per-scan boxes, per-grid unions, then the unions back to size the grids on the host
+  k_scan_points<<<(unsigned)M, 256, 0, st>>>((const float *)b->d_pool, (const double *)b->d_poses, l, b->d_sensor.p,
+                                             b->d_pts.p, nullptr, (const int32_t *)b->d_rows);
+  k_scan_bbox_rows<<<(unsigned)M, 256, 0, st>>>(b->d_pool, b->d_rows, b->d_sensor, b->d_pts, l, b->d_bbox);
+  k_bbox_union_grids<<<(unsigned)L, 256, 0, st>>>(b->d_bbox, b->d_first, b->d_count, b->d_union);
+  B2S_CUDA_CHECK(cudaGetLastError());
+  B2S_CUDA_CHECK(cudaMemcpyAsync(b->h_f64, b->d_union, sizeof(double) * 4 * L, cudaMemcpyDeviceToHost, st));
+  B2S_CUDA_CHECK(cudaStreamSynchronize(st));
+  b->bytes_d2h += sizeof(double) * 4.0 * L;
+  b->grids.resize((size_t)L);
+  long long counters = 0, bytes = 0;
+  for (int j = 0; j < L; j++) {
+    const int g = live[(size_t)j];
+    if (b2s_status s = occ_dims((const double *)b->h_f64 + 4 * j, resolution[g], info[g])) return s;
+    OccGridDev &D = b->grids[(size_t)j];
+    D.w = info[g].width; D.h = info[g].height; D.step = info[g].width_step; D.scans = n_scans[g];
+    D.off_x = info[g].offset[0]; D.off_y = info[g].offset[1]; D.scale = 1.0 / resolution[g];
+    D.counters = counters;
+    D.payload = bytes;
+    counters += info[g].data_size;
+    bytes += (long long)D.w * D.h;
+  }
+  B2S_CUDA_CHECK(b->d_pass.reserve((size_t)counters));
+  B2S_CUDA_CHECK(b->d_hit.reserve((size_t)counters));
+  B2S_CUDA_CHECK(b->d_visits.reserve((size_t)L));
+  B2S_CUDA_CHECK(b->d_grids.reserve((size_t)L));
+  B2S_CUDA_CHECK(b->h_grids.reserve((size_t)L));
+  B2S_CUDA_CHECK(b->d_payload.reserve((size_t)bytes));
+  B2S_CUDA_CHECK(b->h_payload.reserve((size_t)bytes));
+  B2S_CUDA_CHECK(b->h_visits.reserve((size_t)L));
+  std::memcpy(b->h_grids, b->grids.data(), sizeof(OccGridDev) * L);
+  B2S_CUDA_CHECK(cudaMemcpyAsync(b->d_grids, b->h_grids, sizeof(OccGridDev) * L, cudaMemcpyHostToDevice, st));
+  if (counters) {
+    B2S_CUDA_CHECK(cudaMemsetAsync(b->d_pass, 0, sizeof(uint32_t) * counters, st));
+    B2S_CUDA_CHECK(cudaMemsetAsync(b->d_hit, 0, sizeof(uint32_t) * counters, st));
+  }
+  B2S_CUDA_CHECK(cudaMemsetAsync(b->d_visits, 0, sizeof(unsigned long long) * L, st));
+  const long long n_beams = (long long)M * (long long)n;
+  if (n_beams && counters) {
+    const int blocks = (int)std::min<long long>((n_beams + 7) / 8, (long long)sm_count(b->device) * 16);
+    k_raytrace_grids<<<blocks, 256, 0, st>>>(b->d_pool, b->d_rows, b->d_scan_grid, b->d_sensor, b->d_pts, l, n_beams,
+                                             b->d_grids, b->d_pass, b->d_hit, b->d_visits);
+  }
+  if (bytes) {
+    long long most = 0;
+    for (const OccGridDev &D : b->grids) most = std::max(most, (long long)D.w * D.h);
+    const unsigned xb = (unsigned)std::min<long long>(ceil_div(most, 256), 1024);
+    k_occ_ros_grids<<<dim3(xb, (unsigned)L), 256, 0, st>>>(b->d_pass, b->d_hit, b->d_grids, b->d_payload);
+  }
+  B2S_CUDA_CHECK(cudaGetLastError());
+  if (bytes) B2S_CUDA_CHECK(cudaMemcpyAsync(b->h_payload, b->d_payload, (size_t)bytes, cudaMemcpyDeviceToHost, st));
+  B2S_CUDA_CHECK(cudaMemcpyAsync(b->h_visits, b->d_visits, sizeof(unsigned long long) * L, cudaMemcpyDeviceToHost, st));
+  B2S_CUDA_CHECK(cudaStreamSynchronize(st));
+  b->bytes_d2h += (double)bytes + sizeof(unsigned long long) * (double)L;
+  for (int j = 0; j < L; j++) {
+    const int g = live[(size_t)j];
+    info[g].cell_visits = b->h_visits[j];
+    payload[g] = (const int8_t *)b->h_payload + b->grids[(size_t)j].payload;
+  }
+  return B2S_OK;
+}
+
+}  // namespace b2s
+
+extern "C" b2s_status b2s_occ_grid_create_from_scans_batch(const b2s_laser *laser, int n_grids, const int32_t *n_scans,
+                                                           const float *ranges, const double *poses,
+                                                           const double *resolution, int device,
+                                                           b2s_occ_grid_batch_fn on_grid, void *user) {
+  if (!laser || n_grids < 0 || (n_grids > 0 && (!n_scans || !resolution)))
+    B2S_FAIL(B2S_ERR_BAD_PARAMS, "b2s_occ_grid_create_from_scans_batch: null argument or negative count");
+  size_t M = 0;
+  for (int g = 0; g < n_grids; g++) {
+    if (n_scans[g] < 0) B2S_FAIL(B2S_ERR_BAD_PARAMS, "b2s_occ_grid_create_from_scans_batch: negative scan count");
+    M += (size_t)n_scans[g];
+  }
+  if (M > (size_t)INT32_MAX) B2S_FAIL(B2S_ERR_TOO_LARGE, "b2s_occ_grid_create_from_scans_batch: too many scans");
+  if (M > 0 && (!ranges || !poses)) B2S_FAIL(B2S_ERR_BAD_PARAMS, "b2s_occ_grid_create_from_scans_batch: null argument");
+  if (M == 0) return B2S_OK;
+  OccBatch *raw = nullptr;
+  if (b2s_status st = occ_batch_create(*laser, device, &raw)) return st;
+  std::unique_ptr<OccBatch, decltype(&occ_batch_destroy)> b(raw, occ_batch_destroy);
+  int32_t first = 0;
+  if (b2s_status st = occ_batch_append(b.get(), (int)M, ranges, &first)) return st;
+  std::vector<int32_t> rows(M), have((size_t)n_grids);
+  for (size_t s = 0; s < M; s++) rows[s] = first + (int32_t)s;
+  std::vector<b2s_occ_grid_info> info((size_t)n_grids);
+  std::vector<const int8_t *> payload((size_t)n_grids);
+  if (b2s_status st = occ_batch_build(b.get(), n_grids, n_scans, rows.data(), poses, resolution, info.data(),
+                                      have.data(), payload.data()))
+    return st;
+  if (on_grid)
+    for (int g = 0; g < n_grids; g++)
+      if (have[(size_t)g]) on_grid(user, g, &info[(size_t)g], payload[(size_t)g]);
+  return B2S_OK;
+}

@@ -11,9 +11,12 @@ namespace b2s {
 // Karto.h:2894-2901).  One block per scan.
 // ----------------------------------------------------------------------------------------------
 // `src` (may be NULL): row of `ranges` scan b reads (a scan pool shared by many base sets); NULL = row b.
-static __global__ void k_scan_points(const double *__restrict__ ranges, const double *__restrict__ poses, b2s_laser l,
-                              double *__restrict__ sensor, double *__restrict__ pts, double *__restrict__ local,
-                              const int32_t *__restrict__ src) {
+// The float overload reads float32 readings widened to double (the Karto node's map pool), which is exact.
+template <class R>
+static __device__ __forceinline__ void scan_points_block(const R *__restrict__ ranges, const double *__restrict__ poses,
+                                                         const b2s_laser &l, double *__restrict__ sensor,
+                                                         double *__restrict__ pts, double *__restrict__ local,
+                                                         const int32_t *__restrict__ src) {
   const int b = blockIdx.x;
   const size_t row = src ? (size_t)src[b] : (size_t)b;
   const int n = l.n_readings;
@@ -44,7 +47,7 @@ static __global__ void k_scan_points(const double *__restrict__ ranges, const do
   __syncthreads();
   const double dh = normalize_angle(0.0 - tr[2]);
   for (int i = threadIdx.x; i < n; i += blockDim.x) {
-    double r = ranges[row * n + i];
+    double r = (double)ranges[row * n + i];
     double angle = sp[2] + l.min_angle + (double)(uint32_t)i * l.angular_resolution;
     double x = sp[0] + (r * cos(angle));
     double y = sp[1] + (r * sin(angle));
@@ -56,6 +59,16 @@ static __global__ void k_scan_points(const double *__restrict__ ranges, const do
       local[((size_t)b * n + i) * 2 + 1] = inv[3] * dx + inv[4] * dy + inv[5] * dh;
     }
   }
+}
+static __global__ void k_scan_points(const double *__restrict__ ranges, const double *__restrict__ poses, b2s_laser l,
+                                     double *__restrict__ sensor, double *__restrict__ pts, double *__restrict__ local,
+                                     const int32_t *__restrict__ src) {
+  scan_points_block(ranges, poses, l, sensor, pts, local, src);
+}
+static __global__ void k_scan_points(const float *__restrict__ ranges, const double *__restrict__ poses, b2s_laser l,
+                                     double *__restrict__ sensor, double *__restrict__ pts, double *__restrict__ local,
+                                     const int32_t *__restrict__ src) {
+  scan_points_block(ranges, poses, l, sensor, pts, local, src);
 }
 
 

@@ -20,6 +20,7 @@ class KartoNodeParams(C.Structure):
 
 
 MAP_FN = C.CFUNCTYPE(None, C.c_void_p, C.c_int32, C.POINTER(abi.OccGridInfo), C.POINTER(C.c_int8))
+BATCH_MAP_FN = C.CFUNCTYPE(None, C.c_void_p, C.c_int32, C.c_int32, C.POINTER(abi.OccGridInfo), C.POINTER(C.c_int8))
 
 # SlamKarto::InitParams (karto_slam.cc:81-252): ROS parameter -> (where the Mapper stores it, type, squared by setParam*).
 # minimum_time_interval is absent: the node never reads it.
@@ -103,6 +104,13 @@ def _bind():
     L.b2s_karto_node_mapper.restype = vp
     L.b2s_karto_node_process.argtypes = [vp, C.c_int, C.POINTER(C.c_float), C.POINTER(C.c_uint32), dp,
                                          C.POINTER(C.c_int32), dp, dp, C.POINTER(C.c_int32), MAP_FN, vp]
+    L.b2s_karto_node_create_batch.argtypes = [C.c_int, C.POINTER(KartoNodeParams), C.POINTER(LaserScanMsg), dp,
+                                              C.POINTER(ScanSolver), C.c_int, C.POINTER(vp)]
+    L.b2s_karto_node_mapper_of.argtypes = [vp, C.c_int]
+    L.b2s_karto_node_mapper_of.restype = vp
+    L.b2s_karto_node_process_batch.argtypes = [vp, C.POINTER(C.c_int32), C.POINTER(C.c_float), C.POINTER(C.c_uint32),
+                                               dp, C.POINTER(C.c_int32), dp, dp, C.POINTER(C.c_int32), BATCH_MAP_FN, vp]
+    L.b2s_karto_node_last_timing.argtypes = [vp, dp]
     _bound = True
     return L
 
@@ -115,6 +123,14 @@ class _InnerMapper(Mapper):
 
     def close(self):
         self.h = C.c_void_p()
+
+
+def _map_of(info_p, payload_p):
+    i = info_p.contents
+    info = dict(width=i.width, height=i.height, offset=np.array(i.offset[:]), resolution=i.resolution,
+                width_step=i.width_step, data_size=i.data_size, cell_visits=int(i.cell_visits))
+    data = np.ctypeslib.as_array(payload_p, shape=(i.height * i.width,)).reshape(i.height, i.width).copy()
+    return info, data
 
 
 class KartoNode:
@@ -150,9 +166,7 @@ class KartoNode:
         maps = []
 
         def cb(user, scan_index, info_p, payload_p):
-            i = info_p.contents
-            info = dict(width=i.width, height=i.height, offset=np.array(i.offset[:]), resolution=i.resolution)
-            data = np.ctypeslib.as_array(payload_p, shape=(i.height * i.width,)).reshape(i.height, i.width).copy()
+            info, data = _map_of(info_p, payload_p)
             maps.append((int(scan_index), info, data))
             if on_map is not None:
                 on_map(int(scan_index), info, data)
@@ -176,3 +190,84 @@ class KartoNode:
             self.close()
         except Exception:
             pass
+
+
+class KartoNodeBatch:
+    """B SlamKarto nodes in one handle, one per recording or per setting (b2s_karto_node_create_batch): their matches
+    share launches and their maps are built together.  Every node must derive the same laser (offset, range threshold,
+    upside-down flag) and the same matcher parameters; throttle, map interval, resolution, the Mapper's host-only
+    parameters and the back end may differ.  solvers: None, or one ScanSolver (or None) per node, each its own."""
+
+    def __init__(self, params_list, geometry: LaserScanMsg, mounts, solvers=None, device: int = 0):
+        self.L = _bind()
+        self.h = C.c_void_p()
+        self.n_ranges = geometry.n_ranges
+        self.batch = len(params_list)
+        params = (KartoNodeParams * self.batch)(*params_list)
+        m = np.ascontiguousarray(mounts, np.float64)
+        assert m.shape == (self.batch, 7)
+        slots = None
+        if solvers is not None:
+            assert len(solvers) == self.batch
+            slots = (ScanSolver * self.batch)(*[s if s is not None else ScanSolver() for s in solvers])
+        self._solvers = (solvers, slots)  # the vtables' owners must outlive the handle
+        check(self.L.b2s_karto_node_create_batch(self.batch, params, C.byref(geometry),
+                                                 m.ctypes.data_as(C.POINTER(C.c_double)), slots, device,
+                                                 C.byref(self.h)))
+        n = KartoNode._n_readings(params_list[0], geometry)
+        self._mappers = [_InnerMapper(self.L, self.L.b2s_karto_node_mapper_of(self.h, b), n) for b in range(self.batch)]
+
+    def mapper(self, b):
+        """node b's Mapper (graph getters of mapper.Mapper)"""
+        return self._mappers[b]
+
+    def process(self, ranges_list, stamps_list, odom_list, on_map=None):
+        """ranges_list[b] [S_b][n] float32, stamps_list[b] [S_b][2], odom_list[b] [S_b][7] -> one dict per node, shaped
+        as KartoNode.process's.  on_map(node, scan_index, info, payload) is called for each published map in the call's
+        order."""
+        counts = np.array([len(s) for s in stamps_list], np.int32)
+        assert len(counts) == self.batch and len(ranges_list) == self.batch and len(odom_list) == self.batch
+        S = int(counts.sum())
+        r = np.zeros((S, self.n_ranges), np.float32)
+        s = np.zeros((S, 2), np.uint32)
+        o = np.zeros((S, 7), np.float64)
+        at = np.concatenate([[0], np.cumsum(counts)]).astype(np.int64)
+        for b in range(self.batch):
+            if counts[b]:
+                r[at[b]:at[b + 1]] = np.asarray(ranges_list[b], np.float32).reshape(counts[b], self.n_ranges)
+                s[at[b]:at[b + 1]] = np.asarray(stamps_list[b], np.uint32).reshape(counts[b], 2)
+                o[at[b]:at[b + 1]] = np.asarray(odom_list[b], np.float64).reshape(counts[b], 7)
+        state, pub = np.zeros(S, np.int32), np.zeros(S, np.int32)
+        pose, m2o = np.zeros((S, 3)), np.zeros((S, 7))
+        maps = [[] for _ in range(self.batch)]
+
+        def cb(user, node, scan_index, info_p, payload_p):
+            info, data = _map_of(info_p, payload_p)
+            maps[node].append((int(scan_index), info, data))
+            if on_map is not None:
+                on_map(int(node), int(scan_index), info, data)
+
+        fn = BATCH_MAP_FN(cb)
+        i32, dp = C.POINTER(C.c_int32), C.POINTER(C.c_double)
+        check(self.L.b2s_karto_node_process_batch(self.h, counts.ctypes.data_as(i32), r.ctypes.data_as(C.POINTER(C.c_float)),
+                                                  s.ctypes.data_as(C.POINTER(C.c_uint32)), o.ctypes.data_as(dp),
+                                                  state.ctypes.data_as(i32), pose.ctypes.data_as(dp),
+                                                  m2o.ctypes.data_as(dp), pub.ctypes.data_as(i32), fn, None))
+        return [dict(state=state[at[b]:at[b + 1]], pose=pose[at[b]:at[b + 1]], map_to_odom=m2o[at[b]:at[b + 1]],
+                     map_published=pub[at[b]:at[b + 1]], maps=maps[b]) for b in range(self.batch)]
+
+    def last_timing(self):
+        """where the last process call went (b2s_karto_node_last_timing)"""
+        out = np.zeros(8)
+        check(self.L.b2s_karto_node_last_timing(self.h, out.ctypes.data_as(C.POINTER(C.c_double))))
+        keys = ("rounds", "match_launches", "matches", "maps", "match_s", "map_s", "map_bytes_d2h", "call_s")
+        return dict(zip(keys, out.tolist()))
+
+    def close(self):
+        if getattr(self, "h", None) and self.h.value:
+            for m in self._mappers:
+                m.close()
+            self.L.b2s_karto_node_destroy(self.h)
+            self.h = C.c_void_p()
+
+    __del__ = KartoNode.__del__

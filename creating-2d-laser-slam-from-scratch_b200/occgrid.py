@@ -136,3 +136,38 @@ class OccupancyGrid:
             self.close()
         except Exception:
             pass
+
+
+BATCH_GRID_FN = C.CFUNCTYPE(None, C.c_void_p, C.c_int32, C.POINTER(abi.OccGridInfo), C.POINTER(C.c_int8))
+
+
+def create_from_scans_batch(laser: abi.Laser, ranges_list, poses_list, resolutions, device: int = 0):
+    """b2s_occ_grid_create_from_scans_batch: grid g over ranges_list[g] [S_g][n] (float32) at poses_list[g] [S_g][3]
+    with resolutions[g], every grid in one batched build.  -> one (info dict, payload [h][w] int8) per grid, None for a
+    grid without scans."""
+    L = _bind()
+    L.b2s_occ_grid_create_from_scans_batch.argtypes = [C.POINTER(abi.Laser), C.c_int, C.POINTER(C.c_int32),
+                                                       C.POINTER(C.c_float), C.POINTER(C.c_double),
+                                                       C.POINTER(C.c_double), C.c_int, BATCH_GRID_FN, C.c_void_p]
+    G = len(ranges_list)
+    counts = np.array([len(r) for r in ranges_list], np.int32)
+    n = laser.n_readings
+    r = np.ascontiguousarray(np.concatenate([np.asarray(x, np.float32).reshape(-1, n) for x in ranges_list])
+                             if counts.sum() else np.zeros((0, n), np.float32))
+    p = np.ascontiguousarray(np.concatenate([np.asarray(x, np.float64).reshape(-1, 3) for x in poses_list])
+                             if counts.sum() else np.zeros((0, 3)))
+    res = np.ascontiguousarray(resolutions, np.float64)
+    out = [None] * G
+
+    def cb(user, g, info_p, payload_p):
+        i = info_p.contents
+        info = dict(width=i.width, height=i.height, width_step=i.width_step, data_size=i.data_size,
+                    offset=np.array(i.offset[:]), resolution=i.resolution, cell_visits=int(i.cell_visits))
+        out[g] = (info, np.ctypeslib.as_array(payload_p, shape=(i.height * i.width,)).reshape(i.height, i.width).copy()
+                  if i.height * i.width else np.zeros((i.height, i.width), np.int8))
+
+    fn = BATCH_GRID_FN(cb)
+    check(L.b2s_occ_grid_create_from_scans_batch(C.byref(laser), G, counts.ctypes.data_as(C.POINTER(C.c_int32)),
+                                                 r.ctypes.data_as(C.POINTER(C.c_float)), _d(p), _d(res), device, fn,
+                                                 None))
+    return out

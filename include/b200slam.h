@@ -346,6 +346,19 @@ typedef struct b2s_occ_grid b2s_occ_grid; /* opaque: replaces karto::OccupancyGr
 b2s_status b2s_occ_grid_create_from_scans(const b2s_laser *laser, int n_scans, const double *ranges,
                                           const double *poses, double resolution, int device,
                                           void *cuda_stream, b2s_occ_grid **out);
+/* Many grids at once: grid g = b2s_occ_grid_create_from_scans over its own n_scans[g] scans, ranges / poses grid-major
+ * (grid 0's scans first), at resolution[g].  The readings are float32 ([sum n_scans][n_readings]), widened to double on
+ * the device, so a grid equals b2s_occ_grid_create_from_scans over the same readings as doubles, bit for bit in info
+ * and payload.  Every stage is one launch for all grids (per-scan boxes, per-grid unions, one read-back of the unions
+ * to size the grids, one counter arena, one ray trace over every beam of every grid, one threshold + payload pass) and
+ * the payloads come back in one copy.  on_grid(user, g, info, payload [height][width] int8 as b2s_occ_grid_copy_ros)
+ * is called in ascending g for every grid with scans; a grid without scans has no map (CreateFromScans returns NULL)
+ * and is skipped.  Pointers are valid only during the callback.  B2S_ERR_BAD_PARAMS for NULL arrays, negative counts
+ * or a zero resolution of a grid with scans. */
+typedef void (*b2s_occ_grid_batch_fn)(void *user, int32_t grid, const b2s_occ_grid_info *info, const int8_t *payload);
+b2s_status b2s_occ_grid_create_from_scans_batch(const b2s_laser *laser, int n_grids, const int32_t *n_scans,
+                                                const float *ranges, const double *poses, const double *resolution,
+                                                int device, b2s_occ_grid_batch_fn on_grid, void *user);
 /* The same map built from a scan list SHARDED over several GPUs (SURVEY.md §8(e)(iii)): pass/hit counters are
  * commutative, so each rank ray-traces its shard into a grid sized by the GLOBAL bounding box and the counters are
  * summed (NCCL all-reduce, in place on the device pointers) before OccupancyGrid::Update thresholds them.
@@ -606,6 +619,51 @@ b2s_mapper *b2s_karto_node_mapper(b2s_karto_node *node);
 b2s_status b2s_karto_node_process(b2s_karto_node *node, int n_scans, const float *ranges, const uint32_t *stamps,
                                   const double *odom, int32_t *out_state, double *out_pose, double *out_map_to_odom,
                                   int32_t *out_map_published, b2s_karto_map_fn on_map, void *user);
+
+/* Several nodes per handle, one per recording or per setting.  Each node runs its own Mapper, unchanged, on a worker
+ * thread of its own for the length of a call; its device work (each MatchScan batch, each map build) is a request to
+ * the calling thread, which serves the requests of all nodes in rounds: round k holds the k-th request of every node
+ * still running, so the rounds follow from the data, not from thread timing.  A round's matches go out grouped by
+ * matcher and search kind on two matcher handles shared by all nodes (each node's scans in their device pools once),
+ * and its maps are built in one b2s_occ_grid_create_from_scans_batch over float32 readings the handle keeps on the
+ * device (each uploaded once).  Every node equals its own b2s_karto_node_create handle bit for bit: states, poses,
+ * map_to_odom, graph, b2s_mapper_stats and maps.  Threads are created by each call and joined before it returns.
+ * A node's solver callbacks run on its worker thread, concurrently with the other nodes' workers, so a solver instance
+ * must serve one node only.  b2s_karto_node_create is this with batch = 1; on a handle with batch > 1
+ * b2s_karto_node_process answers B2S_ERR_BAD_PARAMS and b2s_karto_node_mapper NULL. */
+
+/* b2s_karto_map_fn with the node the map belongs to; scan_index counts that node's scans */
+typedef void (*b2s_karto_node_batch_map_fn)(void *user, int32_t node, int32_t scan_index, const b2s_occ_grid_info *info,
+                                            const int8_t *payload);
+
+/* params [batch], laser_mounts [batch][7], solvers [batch] or NULL (no back end for any node; a slot whose compute is
+ * NULL: none for that node).  Each node is validated as b2s_karto_node_create validates its own, the refusal naming
+ * the node.  All nodes share one geometry, one laser and two matchers: the laser getLaser derives (offset, range
+ * threshold, upside-down flag) and mapper.sequential / mapper.loop after their range_threshold is replaced must be equal
+ * bit for bit in every node, else B2S_ERR_BAD_PARAMS (two mounts may differ where the laser does not, e.g. in z).
+ * throttle_scans, map_update_interval, resolution, the Mapper's host-only fields (travel gates, buffer size, link and
+ * loop thresholds, do_loop_closing, ...) and the solver may differ.  B2S_ERR_TOO_LARGE for more than 1024 nodes. */
+b2s_status b2s_karto_node_create_batch(int batch, const b2s_karto_node_params *params, const b2s_laser_scan_msg *geometry,
+                                       const double *laser_mounts, const b2s_scan_solver *solvers, int device,
+                                       b2s_karto_node **out);
+/* node b's Mapper (0 <= b < batch), for the getters as b2s_karto_node_mapper; NULL out of range */
+b2s_mapper *b2s_karto_node_mapper_of(b2s_karto_node *node, int b);
+/* b2s_karto_node_process on every node at once: n_scans [batch] (0 leaves a node untouched), ranges / stamps / odom
+ * and the outputs node-major (node 0's scans first).  Each node's maps reach on_map in its own order; across nodes
+ * they arrive round by round, inside a round by ascending node, the same for the same calls.  Two calls over
+ * consecutive parts of every recording, split anywhere per node, equal one call.  B2S_ERR_BAD_PARAMS (nothing written,
+ * nothing changed) for a NULL n_scans, a negative count or NULL arrays with scans; B2S_ERR_BAD_STATE after a failed
+ * call.  A device error or a Mapper failure in any node stops every node at its next request; the call returns the
+ * first failure (lowest round, then lowest node), named in b2s_last_error(), each node's rows up to its stop are
+ * written, and the handle refuses later calls with B2S_ERR_BAD_STATE. */
+b2s_status b2s_karto_node_process_batch(b2s_karto_node *node, const int32_t *n_scans, const float *ranges,
+                                        const uint32_t *stamps, const double *odom, int32_t *out_state, double *out_pose,
+                                        double *out_map_to_odom, int32_t *out_map_published,
+                                        b2s_karto_node_batch_map_fn on_map, void *user);
+/* Where the last process call went: out[0] rounds, out[1] matcher launches, out[2] matches, out[3] maps built,
+ * out[4] s serving matches, out[5] s building maps (both host wall time on the calling thread, device work included),
+ * out[6] bytes the map builds copied back from the device, out[7] s of the whole call */
+b2s_status b2s_karto_node_last_timing(const b2s_karto_node *node, double out[8]);
 /* HectorMappingRos::rosPointCloudToDataContainer (lesson4/src/hector_mapping/hector_slam.cc:320-362): laser-frame points
  * ([n][3] float x, y, z as laser_geometry projected them) -> DataContainer entries in map-cell units.  laser_in_base =
  * (x, y, z, yaw) of the laser in base_link.  Filters: squared distance in (min_dist^2, max_dist^2), not behind the robot
