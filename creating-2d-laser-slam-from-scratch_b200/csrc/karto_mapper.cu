@@ -1,7 +1,9 @@
 // lesson6 front end on top of K1 — the host driver of karto::Mapper / MapperGraph / MapperSensorManager (host C++).
 // Product code.  It decides WHAT to match (key frames, running window, near chains, loop-closure candidates) and keeps
 // the pose graph; every ScanMatcher::MatchScan runs on the device through the matcher ABI of this library, and the
-// independent matches of one Process call are sent as one batch.
+// independent matches of one Process call are sent as one batch.  The batch goes to a MatchPool: the Mapper's own
+// (b2s_mapper_create) or the one a Karto node batch shares (karto_node.cu).  b2s_mapper_create_with_matcher's plug-in
+// takes it instead where a host matcher stands in for the device.
 //
 // Reference behaviour (paths relative to reference/lesson6/lib/open_karto):
 //   Mapper::Process / HasMovedEnough / Initialize                          src/Mapper.cpp:1959-2125
@@ -27,12 +29,19 @@
 #include "common.cuh"
 
 namespace b2s {
-// A Mapper that belongs to a fleet of Karto nodes hands each batch of matches to the fleet, which runs it on matcher
-// handles shared by every node: base scans are named by their unique id in this Mapper, base_ids / base_poses
-// [batch][max_base] padded by repeating a match's last base scan.
-typedef b2s_status (*FleetMatchFn)(void *user, int which, int batch, const double *ranges, const double *poses,
-                                   int max_base, const int32_t *base_ids, const double *base_poses, int do_penalize,
-                                   int do_refine, b2s_match_result *results);
+// One batch of a Mapper's matches: base scans are named by their unique id in `mapper`, base_ids / base_poses
+// [batch][max_base] padded by repeating a match's last base scan.  karto_node.cu declares it too, identically.
+struct MatchRequest {
+  const b2s_mapper *mapper = nullptr;
+  int which = 0, batch = 0, max_base = 0, do_penalize = 0, do_refine = 0;
+  const double *ranges = nullptr, *poses = nullptr, *base_poses = nullptr;
+  const int32_t *base_ids = nullptr;
+  b2s_match_result *results = nullptr;
+};
+// A Mapper made by mapper_create_fleet hands each batch to `FleetMatchFn`, which runs it on a MatchPool: the Mapper's
+// own (b2s_mapper_create) or one shared by the nodes of a Karto node batch (karto_node.cu).
+typedef b2s_status (*FleetMatchFn)(void *user, const MatchRequest &r);
+struct MatchPool;
 }  // namespace b2s
 
 using namespace b2s;
@@ -162,33 +171,17 @@ struct SensorState {  // one ScanManager (Mapper.h:1265-1410): the scans, runnin
   int last_scan = -1;        // ScanManager::m_pLastScan
 };
 
-struct CudaBackend {  // the two ScanMatcher instances a Mapper owns, as b2s_matcher handles
-  int device = 0;
-  b2s_laser laser{};
-  b2s_matcher_params params[2]{};
-  b2s_matcher *h[2] = {nullptr, nullptr};
-  int cap_batch[2] = {0, 0}, cap_base[2] = {0, 0};
-  int min_base = 32;  // scan_buffer_size + 1: the sequential matcher's base set is the running window
-  std::vector<double> base_r, base_p;
-  std::vector<int32_t> base_rows;
-  size_t pool_n[2] = {0, 0};  // scans of the mapper already appended to each handle's device-resident pool
-  ~CudaBackend() {
-    for (auto *p : h)
-      if (p) b2s_matcher_destroy(p);
-  }
-};
-
 }  // namespace
 
 struct b2s_mapper {
   bool failed = false;  // a Process call failed after the scan entered the graph: the handle must be discarded
   b2s_mapper_params prm{};
   b2s_laser laser{};
-  b2s_match_scan_fn match = nullptr;
+  b2s_match_scan_fn match = nullptr;  // b2s_mapper_create_with_matcher's plug-in
   void *match_user = nullptr;
-  CudaBackend *cuda = nullptr;
-  b2s::FleetMatchFn fleet = nullptr;  // a Mapper of a Karto node fleet: its matches go to the fleet (karto_node.cu)
+  b2s::FleetMatchFn fleet = nullptr;  // else every match batch goes to `fleet`
   void *fleet_user = nullptr;
+  b2s::MatchPool *pool = nullptr;     // b2s_mapper_create's: the pool `fleet` serves from, owned
   b2s_scan_solver solver{};
   bool have_solver = false;
   std::deque<MScan> scans;  // MapperSensorManager::m_Scans (every sensor's scans by unique id); deque: stable addresses
@@ -244,45 +237,33 @@ struct MatchJob {
   std::vector<int> chain;        // base scans (indices into m->scans)
 };
 
-b2s_status cuda_ensure_handle(CudaBackend *c, int which, int batch, int max_base);
+// A batch of jobs laid out for a matcher: readings [B][N], robot poses [B][3], and job b's chain as base scan ids and
+// poses from first[b] on, in `width` slots per job (0: as many as the chain has), padded by repeating the chain's last
+// scan (rasterising a scan twice leaves the correlation grid unchanged).
+struct JobArrays {
+  std::vector<double> ranges, poses, base_poses;
+  std::vector<int32_t> first, ids;
+};
 
-// The CUDA path proper: base scans are referenced by their row in the handle's device-resident scan pool (every scan
-// of the mapper is uploaded once per handle), so a match uploads only the matched scans, the chain rows and the
-// chain poses.  Ragged chains are padded to the longest chain of the batch by repeating the last row.
-b2s_status cuda_match_ids(b2s_mapper *m, int which, const std::vector<MatchJob> &jobs, bool do_penalize, bool do_refine,
-                          std::vector<b2s_match_result> &out) {
-  CudaBackend *c = m->cuda;
-  const int B = (int)jobs.size(), N = m->laser.n_readings;
-  int max_base = 1;
-  for (const MatchJob &j : jobs) {
-    if (j.chain.empty()) B2S_FAIL(B2S_ERR_BAD_PARAMS, "mapper: MatchScan against an empty chain");
-    max_base = std::max(max_base, (int)j.chain.size());
-  }
-  b2s_status st = cuda_ensure_handle(c, which, B, max_base);
-  if (st) return st;
-  for (; c->pool_n[which] < m->scans.size(); c->pool_n[which]++) {  // new scans (all of them after a handle re-creation)
-    st = b2s_matcher_pool_append(c->h[which], m->scans[c->pool_n[which]].ranges.data(), nullptr);
-    if (st) return st;
-  }
-  std::vector<double> ranges((size_t)B * N), poses((size_t)B * 3);
-  c->base_rows.resize((size_t)B * max_base);
-  c->base_p.resize((size_t)B * max_base * 3);
-  for (int b = 0; b < B; b++) {
-    std::memcpy(&ranges[(size_t)b * N], jobs[b].ranges->data(), sizeof(double) * N);
-    poses[3 * b] = jobs[b].robot_pose.x; poses[3 * b + 1] = jobs[b].robot_pose.y; poses[3 * b + 2] = jobs[b].robot_pose.h;
-    const int nb = (int)jobs[b].chain.size();
-    for (int j = 0; j < max_base; j++) {
-      const int id = jobs[b].chain[std::min(j, nb - 1)];
-      const MScan &sc = m->scans[id];
-      const size_t k = (size_t)b * max_base + j;
-      c->base_rows[k] = id;
-      c->base_p[3 * k] = sc.corrected.x; c->base_p[3 * k + 1] = sc.corrected.y; c->base_p[3 * k + 2] = sc.corrected.h;
+JobArrays lay_out(const b2s_mapper *m, const std::vector<MatchJob> &jobs, int width) {
+  const size_t B = jobs.size(), N = (size_t)m->laser.n_readings;
+  JobArrays a;
+  a.ranges.resize(B * N);
+  a.poses.resize(B * 3);
+  for (size_t b = 0; b < B; b++) {
+    const MatchJob &j = jobs[b];
+    std::memcpy(&a.ranges[b * N], j.ranges->data(), sizeof(double) * N);
+    a.poses[3 * b] = j.robot_pose.x; a.poses[3 * b + 1] = j.robot_pose.y; a.poses[3 * b + 2] = j.robot_pose.h;
+    a.first.push_back((int32_t)a.ids.size());
+    const int nb = (int)j.chain.size();
+    for (int s = 0; s < (width ? width : nb); s++) {
+      const int id = j.chain[std::min(s, nb - 1)];
+      const P3 &p = m->scans[id].corrected;
+      a.ids.push_back(id);
+      a.base_poses.insert(a.base_poses.end(), {p.x, p.y, p.h});
     }
   }
-  st = b2s_matcher_set_scans(c->h[which], B, ranges.data(), poses.data());
-  if (!st) st = b2s_matcher_add_scans_pool(c->h[which], max_base, c->base_rows.data(), c->base_p.data());
-  if (!st) st = b2s_matcher_match_scan(c->h[which], do_penalize ? 1 : 0, do_refine ? 1 : 0, out.data());
-  return st;
+  return a;
 }
 
 b2s_status run_matches(b2s_mapper *m, int which, const std::vector<MatchJob> &jobs, bool do_penalize, bool do_refine,
@@ -290,100 +271,29 @@ b2s_status run_matches(b2s_mapper *m, int which, const std::vector<MatchJob> &jo
   const int B = (int)jobs.size(), N = m->laser.n_readings;
   out.assign(B, b2s_match_result{});
   if (B == 0) return B2S_OK;
-  if (m->cuda) {
-    m->n_match_calls += B;
-    m->n_batches += 1;
-    return cuda_match_ids(m, which, jobs, do_penalize, do_refine, out);
-  }
-  if (m->fleet) {  // as cuda_match_ids, with the base scans named by id for the fleet's shared pools
-    int max_base = 1;
+  int max_base = 0;  // FleetMatchFn takes every chain padded to the longest; the plug-in takes each as it is
+  if (m->fleet)
     for (const MatchJob &j : jobs) {
       if (j.chain.empty()) B2S_FAIL(B2S_ERR_BAD_PARAMS, "mapper: MatchScan against an empty chain");
       max_base = std::max(max_base, (int)j.chain.size());
     }
-    std::vector<double> ranges((size_t)B * N), poses((size_t)B * 3), bp((size_t)B * max_base * 3);
-    std::vector<int32_t> ids((size_t)B * max_base);
-    for (int b = 0; b < B; b++) {
-      std::memcpy(&ranges[(size_t)b * N], jobs[b].ranges->data(), sizeof(double) * N);
-      poses[3 * b] = jobs[b].robot_pose.x; poses[3 * b + 1] = jobs[b].robot_pose.y; poses[3 * b + 2] = jobs[b].robot_pose.h;
-      const int nb = (int)jobs[b].chain.size();
-      for (int j = 0; j < max_base; j++) {
-        const int id = jobs[b].chain[std::min(j, nb - 1)];
-        const MScan &sc = m->scans[id];
-        const size_t k = (size_t)b * max_base + j;
-        ids[k] = id;
-        bp[3 * k] = sc.corrected.x; bp[3 * k + 1] = sc.corrected.y; bp[3 * k + 2] = sc.corrected.h;
-      }
-    }
-    m->n_match_calls += B;
-    m->n_batches += 1;
-    return m->fleet(m->fleet_user, which, B, ranges.data(), poses.data(), max_base, ids.data(), bp.data(),
-                    do_penalize ? 1 : 0, do_refine ? 1 : 0, out.data());
-  }
-  std::vector<double> ranges((size_t)B * N), poses((size_t)B * 3);
-  std::vector<int32_t> first(B), count(B);
-  size_t total = 0;
-  for (int b = 0; b < B; b++) {
-    std::memcpy(&ranges[(size_t)b * N], jobs[b].ranges->data(), sizeof(double) * N);
-    poses[3 * b] = jobs[b].robot_pose.x; poses[3 * b + 1] = jobs[b].robot_pose.y; poses[3 * b + 2] = jobs[b].robot_pose.h;
-    first[b] = (int32_t)total;
-    count[b] = (int32_t)jobs[b].chain.size();
-    total += jobs[b].chain.size();
-  }
-  std::vector<double> br(total * N), bp(total * 3);
-  size_t k = 0;
-  for (int b = 0; b < B; b++)
-    for (int id : jobs[b].chain) {
-      const MScan &s = m->scans[id];
-      std::memcpy(&br[k * N], s.ranges.data(), sizeof(double) * N);
-      bp[3 * k] = s.corrected.x; bp[3 * k + 1] = s.corrected.y; bp[3 * k + 2] = s.corrected.h;
-      k++;
-    }
+  const JobArrays a = lay_out(m, jobs, max_base);
   m->n_match_calls += B;
   m->n_batches += 1;
-  return m->match(m->match_user, which, B, ranges.data(), poses.data(), first.data(), count.data(), br.data(), bp.data(),
-                  do_penalize ? 1 : 0, do_refine ? 1 : 0, out.data());
-}
-
-// (re)creating a handle costs tens of ms (device + pinned allocations): size it for the running window up front and
-// double on growth so that a stream re-creates it a handful of times at most
-b2s_status cuda_ensure_handle(CudaBackend *c, int which, int batch, int max_base) {
-  if (c->h[which] && batch <= c->cap_batch[which] && max_base <= c->cap_base[which]) return B2S_OK;
-  if (c->h[which]) b2s_matcher_destroy(c->h[which]);
-  c->h[which] = nullptr;
-  c->pool_n[which] = 0;
-  const int cb = std::max(std::max(batch, c->cap_batch[which] * 2), 8);
-  const int cs = std::max(std::max(max_base, c->cap_base[which] * 2), c->min_base);
-  b2s_status st = b2s_matcher_create(&c->params[which], &c->laser, c->device, cb, cs, nullptr, &c->h[which]);
-  if (st) return st;
-  c->cap_batch[which] = cb;
-  c->cap_base[which] = cs;
-  return B2S_OK;
-}
-
-// ---- the CUDA matcher behind the generic plug-in signature (host arrays in; the mapper itself takes the pooled path
-// above, this form serves callers that drive b2s_match_scan_fn directly): ragged chains are padded to the longest chain of the batch by repeating each
-// match's last base scan (rasterising a scan twice leaves the correlation grid unchanged)
-b2s_status cuda_match(void *user, int which, int batch, const double *ranges, const double *poses, const int32_t *base_first,
-                      const int32_t *n_base, const double *base_ranges, const double *base_poses, int do_penalize,
-                      int do_refine, b2s_match_result *results) {
-  CudaBackend *c = static_cast<CudaBackend *>(user);
-  const int N = c->laser.n_readings;
-  int max_base = 1;
-  for (int b = 0; b < batch; b++) max_base = std::max(max_base, (int)n_base[b]);
-  if (b2s_status st = cuda_ensure_handle(c, which, batch, max_base)) return st;
-  for (int b = 0; b < batch; b++)
-    if (n_base[b] <= 0) B2S_FAIL(B2S_ERR_BAD_PARAMS, "mapper: MatchScan against an empty chain");
-  c->base_r.resize((size_t)batch * max_base * N);
-  c->base_p.resize((size_t)batch * max_base * 3);
-  for (int b = 0; b < batch; b++)
-    for (int j = 0; j < max_base; j++) {
-      const size_t src = (size_t)base_first[b] + std::min(j, (int)n_base[b] - 1), dst = (size_t)b * max_base + j;
-      std::memcpy(&c->base_r[dst * N], base_ranges + src * N, sizeof(double) * N);
-      std::memcpy(&c->base_p[dst * 3], base_poses + src * 3, sizeof(double) * 3);
-    }
-  return b2s_matcher_match_scan_host(c->h[which], batch, ranges, poses, max_base, c->base_r.data(), c->base_p.data(),
-                                     do_penalize, do_refine, results);
+  if (m->fleet) {
+    MatchRequest r;
+    r.mapper = m;
+    r.which = which; r.batch = B; r.max_base = max_base; r.do_penalize = do_penalize; r.do_refine = do_refine;
+    r.ranges = a.ranges.data(); r.poses = a.poses.data(); r.base_ids = a.ids.data(); r.base_poses = a.base_poses.data();
+    r.results = out.data();
+    return m->fleet(m->fleet_user, r);
+  }
+  std::vector<int32_t> count(B);
+  for (int b = 0; b < B; b++) count[b] = (int32_t)jobs[b].chain.size();
+  std::vector<double> br(a.ids.size() * N);
+  for (size_t k = 0; k < a.ids.size(); k++) std::memcpy(&br[k * N], m->scans[a.ids[k]].ranges.data(), sizeof(double) * N);
+  return m->match(m->match_user, which, B, a.ranges.data(), a.poses.data(), a.first.data(), count.data(), br.data(),
+                  a.base_poses.data(), do_penalize ? 1 : 0, do_refine ? 1 : 0, out.data());
 }
 
 // ---- MapperGraph
@@ -786,33 +696,134 @@ b2s_status b2s_mapper_create_with_matcher(const b2s_mapper_params *params, const
   return B2S_OK;
 }
 
-b2s_status b2s_mapper_create(const b2s_mapper_params *params, const b2s_laser *laser, int device, b2s_mapper **out) {
-  if (!out) B2S_FAIL(B2S_ERR_BAD_PARAMS, "b2s_mapper_create: null argument");
-  *out = nullptr;
-  b2s_status st = check_params(params, laser);
-  if (st) return st;
-  if ((st = check_device(device))) return st;
-  CudaBackend *c = new (std::nothrow) CudaBackend();
-  if (!c) B2S_FAIL(B2S_ERR_CUDA, "out of host memory");
-  c->device = device;
-  c->laser = *laser;
-  c->params[0] = params->sequential;
-  c->params[1] = params->loop;
-  c->min_base = std::max(32, params->scan_buffer_size + 1);
-  st = b2s_mapper_create_with_matcher(params, laser, cuda_match, c, out);
-  if (st) {
-    delete c;
-    return st;
-  }
-  (*out)->cuda = c;
-  return B2S_OK;
-}
-
 }  // extern "C"
 
 namespace b2s {
 
-// a fleet Mapper (karto_node.cu): every match goes to `match`; the Mapper itself makes no CUDA call
+constexpr int MATCH_MAX_BATCH = 256;  // matches per launch; larger groups go out in parts
+
+// The two ScanMatcher instances (sequential, loop) as b2s_matcher handles serving the matches of one or more client
+// Mappers.  Base scans are referenced by their row in the handle's device-resident scan pool (each client scan is
+// uploaded once per handle), so a match uploads only the matched scan, the chain rows and the chain poses.
+struct MatchPool {
+  int device = 0;
+  b2s_laser laser{};
+  b2s_matcher_params params[2]{};
+  int first_batch = 8, first_base = 32;  // capacities of a handle's first creation
+  b2s_matcher *h[2] = {nullptr, nullptr};
+  int cap_batch[2] = {0, 0}, cap_base[2] = {0, 0};
+  std::vector<std::vector<int32_t>> rows[2];  // [which][client]: pool row of each of that client's scans
+  std::vector<double> ranges, poses, base_poses;
+  std::vector<int32_t> base_rows;
+  std::vector<b2s_match_result> results;
+  ~MatchPool() {
+    for (b2s_matcher *p : h)
+      if (p) b2s_matcher_destroy(p);
+  }
+
+  // (re)creating a handle costs tens of ms (device + pinned allocations) and drops its pool: it is sized for the
+  // clients and the running window up front and doubles on growth, so a stream re-creates it a handful of times at most
+  b2s_status ensure(int which, int batch, int max_base) {
+    batch = std::min(batch, MATCH_MAX_BATCH);
+    if (h[which] && batch <= cap_batch[which] && max_base <= cap_base[which]) return B2S_OK;
+    if (h[which]) b2s_matcher_destroy(h[which]);
+    h[which] = nullptr;
+    for (std::vector<int32_t> &r : rows[which]) r.clear();
+    const int cb = std::min(std::max({batch, 2 * cap_batch[which], first_batch}), MATCH_MAX_BATCH);
+    const int cs = std::max({max_base, 2 * cap_base[which], first_base});
+    if (b2s_status st = b2s_matcher_create(&params[which], &laser, device, cb, cs, nullptr, &h[which])) return st;
+    cap_batch[which] = cb;
+    cap_base[which] = cs;
+    return B2S_OK;
+  }
+};
+
+// `clients` Mappers, the longest running window scan_buffer_size; no handle is created before the first match
+b2s_status match_pool_create(const b2s_matcher_params params[2], const b2s_laser &laser, int device, int clients,
+                             int scan_buffer_size, MatchPool **out) {
+  *out = nullptr;
+  MatchPool *p = new (std::nothrow) MatchPool();
+  if (!p) B2S_FAIL(B2S_ERR_CUDA, "out of host memory");
+  p->device = device;
+  p->laser = laser;
+  p->params[0] = params[0];
+  p->params[1] = params[1];
+  p->first_batch = std::min(std::max(8, 2 * clients), MATCH_MAX_BATCH);
+  p->first_base = std::max(32, scan_buffer_size + 1);  // the sequential matcher's base set is the running window
+  p->rows[0].resize((size_t)clients);
+  p->rows[1].resize((size_t)clients);
+  *out = p;
+  return B2S_OK;
+}
+
+void match_pool_destroy(MatchPool *p) { delete p; }
+
+// One group of requests with the same (which, do_penalize, do_refine), each from the client Mapper numbered .first:
+// the clients' new scans enter the pool, chains are padded to the group's longest, and the group runs in launches of
+// at most the handle's batch capacity.  counts, if not null: += launches, += matches.
+b2s_status match_pool_serve(MatchPool *p, const std::vector<std::pair<int, const MatchRequest *>> &group, double *counts) {
+  const MatchRequest &r0 = *group[0].second;
+  const int which = r0.which, N = p->laser.n_readings;
+  int max_base = 1, total = 0;
+  for (const auto &q : group) {
+    max_base = std::max(max_base, q.second->max_base);
+    total += q.second->batch;
+  }
+  if (b2s_status st = p->ensure(which, total, max_base)) return st;
+  b2s_matcher *h = p->h[which];
+  for (const auto &q : group) {
+    const std::deque<MScan> &scans = q.second->mapper->scans;
+    std::vector<int32_t> &rows = p->rows[which][(size_t)q.first];
+    for (size_t id = rows.size(); id < scans.size(); id++) {
+      int32_t row = 0;
+      if (b2s_status st = b2s_matcher_pool_append(h, scans[id].ranges.data(), &row)) return st;
+      rows.push_back(row);
+    }
+  }
+  p->ranges.resize((size_t)total * N);
+  p->poses.resize((size_t)total * 3);
+  p->base_rows.resize((size_t)total * max_base);
+  p->base_poses.resize((size_t)total * max_base * 3);
+  p->results.assign((size_t)total, b2s_match_result{});
+  size_t t = 0;
+  for (const auto &q : group) {
+    const MatchRequest &r = *q.second;
+    const std::vector<int32_t> &rows = p->rows[which][(size_t)q.first];
+    std::memcpy(&p->ranges[t * N], r.ranges, sizeof(double) * N * r.batch);
+    std::memcpy(&p->poses[t * 3], r.poses, sizeof(double) * 3 * r.batch);
+    for (int b = 0; b < r.batch; b++, t++)
+      for (int j = 0; j < max_base; j++) {
+        const size_t src = (size_t)b * r.max_base + std::min(j, r.max_base - 1), dst = t * max_base + j;
+        p->base_rows[dst] = rows[(size_t)r.base_ids[src]];
+        std::memcpy(&p->base_poses[3 * dst], r.base_poses + 3 * src, 3 * sizeof(double));
+      }
+  }
+  for (int at = 0; at < total; at += p->cap_batch[which]) {
+    const int c = std::min(p->cap_batch[which], total - at);
+    b2s_status st = b2s_matcher_set_scans(h, c, &p->ranges[(size_t)at * N], &p->poses[(size_t)at * 3]);
+    if (!st) st = b2s_matcher_add_scans_pool(h, max_base, &p->base_rows[(size_t)at * max_base],
+                                             &p->base_poses[(size_t)at * max_base * 3]);
+    if (!st) st = b2s_matcher_match_scan(h, r0.do_penalize, r0.do_refine, &p->results[(size_t)at]);
+    if (st) return st;
+    if (counts) {
+      counts[0] += 1;
+      counts[1] += c;
+    }
+  }
+  t = 0;
+  for (const auto &q : group) {
+    std::memcpy(q.second->results, &p->results[t], sizeof(b2s_match_result) * q.second->batch);
+    t += (size_t)q.second->batch;
+  }
+  return B2S_OK;
+}
+
+// b2s_mapper_create's FleetMatchFn: the Mapper is its pool's one client, served at once on the calling thread
+b2s_status serve_own_pool(void *user, const MatchRequest &r) {
+  return match_pool_serve(static_cast<MatchPool *>(user), {{0, &r}}, nullptr);
+}
+
+// a Mapper whose every match batch goes to `match`; the Mapper itself makes no CUDA call
 b2s_status mapper_create_fleet(const b2s_mapper_params *params, const b2s_laser *laser, FleetMatchFn match, void *user,
                                b2s_mapper **out) {
   *out = nullptr;
@@ -834,9 +845,26 @@ const double *mapper_scan_ranges(const b2s_mapper *m, int id) { return m->scans[
 
 extern "C" {
 
+b2s_status b2s_mapper_create(const b2s_mapper_params *params, const b2s_laser *laser, int device, b2s_mapper **out) {
+  if (!out) B2S_FAIL(B2S_ERR_BAD_PARAMS, "b2s_mapper_create: null argument");
+  *out = nullptr;
+  b2s_status st = check_params(params, laser);
+  if (st) return st;
+  if ((st = check_device(device))) return st;
+  const b2s_matcher_params mp[2] = {params->sequential, params->loop};
+  MatchPool *pool = nullptr;
+  if ((st = match_pool_create(mp, *laser, device, 1, params->scan_buffer_size, &pool))) return st;
+  if ((st = mapper_create_fleet(params, laser, serve_own_pool, pool, out))) {
+    match_pool_destroy(pool);
+    return st;
+  }
+  (*out)->pool = pool;
+  return B2S_OK;
+}
+
 void b2s_mapper_destroy(b2s_mapper *m) {
   if (!m) return;
-  delete m->cuda;
+  match_pool_destroy(m->pool);
   delete m;
 }
 

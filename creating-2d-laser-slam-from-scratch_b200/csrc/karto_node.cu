@@ -2,7 +2,8 @@
 // one Mapper per node (karto_mapper.cu) and the device occupancy grid (karto_occgrid.cu).  Each node runs its per-scan
 // loop, unchanged, on a worker thread of its own; its device work (every MatchScan batch, every map build) becomes a
 // request to the dispatcher on the calling thread, which serves the requests of all nodes in rounds: the matches on
-// two matcher handles shared by every node, the maps in one batched build.  The single-node handle is the batch of one.
+// one MatchPool (karto_mapper.cu) whose every client is a node, the maps in one batched build.  The single-node handle
+// is the batch of one.
 //   SlamKarto::InitParams / constructor              karto_slam.cc:21-58, 81-252
 //   SlamKarto::laserCallback                         :286-325  (throttle, map-update gate)
 //   SlamKarto::getLaser                              :327-405  (offset, upside-down test)
@@ -30,12 +31,22 @@ namespace b2s {
 b2s_status karto_laser_from_msg(const b2s_laser_scan_msg *scan, const double laser_pose_in_base[3], double use_scan_range,
                                 b2s_laser *out);  // ros_io.cu
 // karto_mapper.cu
-typedef b2s_status (*FleetMatchFn)(void *user, int which, int batch, const double *ranges, const double *poses,
-                                   int max_base, const int32_t *base_ids, const double *base_poses, int do_penalize,
-                                   int do_refine, b2s_match_result *results);
+struct MatchRequest {
+  const b2s_mapper *mapper = nullptr;
+  int which = 0, batch = 0, max_base = 0, do_penalize = 0, do_refine = 0;
+  const double *ranges = nullptr, *poses = nullptr, *base_poses = nullptr;
+  const int32_t *base_ids = nullptr;
+  b2s_match_result *results = nullptr;
+};
+typedef b2s_status (*FleetMatchFn)(void *user, const MatchRequest &r);
 b2s_status mapper_create_fleet(const b2s_mapper_params *params, const b2s_laser *laser, FleetMatchFn match, void *user,
                                b2s_mapper **out);
 const double *mapper_scan_ranges(const b2s_mapper *m, int id);
+struct MatchPool;
+b2s_status match_pool_create(const b2s_matcher_params params[2], const b2s_laser &laser, int device, int clients,
+                             int scan_buffer_size, MatchPool **out);
+void match_pool_destroy(MatchPool *p);
+b2s_status match_pool_serve(MatchPool *p, const std::vector<std::pair<int, const MatchRequest *>> &group, double *counts);
 // karto_occgrid.cu
 struct OccBatch;
 b2s_status occ_batch_create(const b2s_laser &laser, int device, OccBatch **out);
@@ -75,16 +86,10 @@ double yaw_of(const TfTransform &t) {
 namespace {
 
 constexpr int NODE_MAX_BATCH = 1024;  // nodes per handle
-constexpr int MATCH_MAX_BATCH = 256;  // matches per launch of the shared matchers; larger groups go out in parts
 
 // a node's device work, posted by its worker and served by the dispatcher
 struct Request {
-  bool map = false;
-  // a MatchScan batch (FleetMatchFn's arguments)
-  int which = 0, batch = 0, max_base = 0, do_penalize = 0, do_refine = 0;
-  const double *ranges = nullptr, *poses = nullptr, *base_poses = nullptr;
-  const int32_t *base_ids = nullptr;
-  b2s_match_result *results = nullptr;
+  const MatchRequest *match = nullptr;  // a MatchScan batch, or else a map build
   // a map build: CreateFromScans over the node's first `count` scans at `map_poses`
   int32_t scan_index = 0, count = 0;
   const double *map_poses = nullptr;
@@ -132,7 +137,6 @@ struct KartoNodeState {
   double map_to_odom[7] = {0, 0, 0, 0, 0, 0, 1};
   std::vector<double> scan;                      // one scan's readings
   std::vector<double> poses;                     // scratch for b2s_mapper_get_poses
-  std::vector<int32_t> match_row[2];             // row in each shared matcher's pool of each Mapper scan
   std::vector<int32_t> map_row;                  // row in the map pool of each Mapper scan
 };
 
@@ -143,17 +147,12 @@ struct b2s_karto_node {
   bool inverted = false;
   b2s_matcher_params matcher_params[2]{};
   std::vector<KartoNodeState> nodes;
-  b2s_matcher *h[2] = {nullptr, nullptr};
-  int cap_batch = 8, cap_base[2] = {32, 32};
+  MatchPool *matches = nullptr;  // every node is a client, numbered by its index
   OccBatch *maps = nullptr;
   Lockstep *lock = nullptr;  // the running call's
   bool failed = false;
   double timing[8] = {0, 0, 0, 0, 0, 0, 0, 0};
-  // the dispatcher's scratch
-  std::vector<double> m_ranges, m_poses, m_base_poses;
-  std::vector<int32_t> m_rows;
-  std::vector<b2s_match_result> m_results;
-  std::vector<float> stage;
+  std::vector<float> stage;  // the dispatcher's scratch
 };
 
 namespace {
@@ -177,14 +176,10 @@ b2s_status post(KartoNodeState &k, Request &r) {
 }
 
 // FleetMatchFn: the Mapper's match batch as a request
-b2s_status fleet_match(void *user, int which, int batch, const double *ranges, const double *poses, int max_base,
-                       const int32_t *base_ids, const double *base_poses, int do_penalize, int do_refine,
-                       b2s_match_result *results) {
-  KartoNodeState &k = *static_cast<KartoNodeState *>(user);
+b2s_status fleet_match(void *user, const MatchRequest &m) {
   Request r;
-  r.which = which; r.batch = batch; r.max_base = max_base; r.do_penalize = do_penalize; r.do_refine = do_refine;
-  r.ranges = ranges; r.poses = poses; r.base_ids = base_ids; r.base_poses = base_poses; r.results = results;
-  return post(k, r);
+  r.match = &m;
+  return post(*static_cast<KartoNodeState *>(user), r);
 }
 
 // SlamKarto::updateMap as a request: CreateFromScans over every processed scan at its corrected pose now
@@ -195,7 +190,6 @@ b2s_status update_map(KartoNodeState &k, int32_t scan_index, bool &published) {
   if (count > 0)
     if (b2s_status st = b2s_mapper_get_poses(k.mapper, k.poses.data())) return st;
   Request r;
-  r.map = true;
   r.scan_index = scan_index;
   r.count = count;
   r.map_poses = k.poses.data();
@@ -289,75 +283,11 @@ void worker(b2s_karto_node *n, int b, size_t first, int count, const CallRows &a
   if (L.waiting == L.live) L.to_dispatcher.notify_one();
 }
 
-// (re)creating a shared matcher drops its pool: every node's scans are appended again on their next match
-b2s_status ensure_matcher(b2s_karto_node *n, int which, int max_base) {
-  if (n->h[which] && max_base <= n->cap_base[which]) return B2S_OK;
-  const int cap = n->h[which] ? std::max(max_base, 2 * n->cap_base[which]) : std::max(max_base, n->cap_base[which]);
-  if (n->h[which]) b2s_matcher_destroy(n->h[which]);
-  n->h[which] = nullptr;
-  for (KartoNodeState &k : n->nodes) k.match_row[which].clear();
-  if (b2s_status st = b2s_matcher_create(&n->matcher_params[which], &n->laser, n->device, n->cap_batch, cap, nullptr,
-                                         &n->h[which]))
-    return st;
-  n->cap_base[which] = cap;
-  return B2S_OK;
-}
-
-// one group of match requests with the same (which, do_penalize, do_refine), node order
+// one group of match requests with the same (which, do_penalize, do_refine), node order, on the nodes' shared pool
 b2s_status serve_matches(b2s_karto_node *n, const std::vector<std::pair<int, Request *>> &group) {
-  const Request &r0 = *group[0].second;
-  const int which = r0.which, N = n->laser.n_readings;
-  int max_base = 1, total = 0;
-  for (const auto &q : group) {
-    max_base = std::max(max_base, q.second->max_base);
-    total += q.second->batch;
-  }
-  if (b2s_status st = ensure_matcher(n, which, max_base)) return st;
-  b2s_matcher *h = n->h[which];
-  // the nodes' new scans into the shared pool, each once
-  for (const auto &q : group) {
-    KartoNodeState &k = n->nodes[(size_t)q.first];
-    std::vector<int32_t> &rows = k.match_row[which];
-    for (int id = (int)rows.size(), c = b2s_mapper_scan_count(k.mapper); id < c; id++) {
-      int32_t row = 0;
-      if (b2s_status st = b2s_matcher_pool_append(h, mapper_scan_ranges(k.mapper, id), &row)) return st;
-      rows.push_back(row);
-    }
-  }
-  n->m_ranges.resize((size_t)total * N);
-  n->m_poses.resize((size_t)total * 3);
-  n->m_rows.resize((size_t)total * max_base);
-  n->m_base_poses.resize((size_t)total * max_base * 3);
-  n->m_results.assign((size_t)total, b2s_match_result{});
-  size_t t = 0;
-  for (const auto &q : group) {
-    const Request &r = *q.second;
-    const std::vector<int32_t> &rows = n->nodes[(size_t)q.first].match_row[which];
-    std::memcpy(&n->m_ranges[t * N], r.ranges, sizeof(double) * N * r.batch);
-    std::memcpy(&n->m_poses[t * 3], r.poses, sizeof(double) * 3 * r.batch);
-    for (int b = 0; b < r.batch; b++, t++)
-      for (int j = 0; j < max_base; j++) {  // padded to the group's longest chain by repeating the last base scan
-        const size_t src = (size_t)b * r.max_base + std::min(j, r.max_base - 1), dst = t * max_base + j;
-        n->m_rows[dst] = rows[(size_t)r.base_ids[src]];
-        std::memcpy(&n->m_base_poses[3 * dst], r.base_poses + 3 * src, 3 * sizeof(double));
-      }
-  }
-  for (int at = 0; at < total; at += n->cap_batch) {
-    const int c = std::min(n->cap_batch, total - at);
-    b2s_status st = b2s_matcher_set_scans(h, c, &n->m_ranges[(size_t)at * N], &n->m_poses[(size_t)at * 3]);
-    if (!st) st = b2s_matcher_add_scans_pool(h, max_base, &n->m_rows[(size_t)at * max_base],
-                                             &n->m_base_poses[(size_t)at * max_base * 3]);
-    if (!st) st = b2s_matcher_match_scan(h, r0.do_penalize, r0.do_refine, &n->m_results[(size_t)at]);
-    if (st) return st;
-    n->timing[1] += 1;
-  }
-  n->timing[2] += total;
-  t = 0;
-  for (const auto &q : group) {
-    std::memcpy(q.second->results, &n->m_results[t], sizeof(b2s_match_result) * q.second->batch);
-    t += (size_t)q.second->batch;
-  }
-  return B2S_OK;
+  std::vector<std::pair<int, const MatchRequest *>> reqs;
+  for (const auto &q : group) reqs.emplace_back(q.first, q.second->match);
+  return match_pool_serve(n->matches, reqs, &n->timing[1]);  // timing[1], [2]: match launches, matches
 }
 
 // every map request of a round in one batched build; maps to on_map in ascending node order
@@ -419,11 +349,12 @@ void serve_round(b2s_karto_node *n, Lockstep &L, const std::vector<std::pair<int
   std::vector<std::vector<std::pair<int, Request *>>> groups;
   std::vector<int> keys;
   for (const auto &q : reqs) {
-    if (q.second->map) {
+    const MatchRequest *m = q.second->match;
+    if (!m) {
       maps.push_back(q);
       continue;
     }
-    const int key = q.second->which * 4 + q.second->do_penalize * 2 + q.second->do_refine;
+    const int key = m->which * 4 + m->do_penalize * 2 + m->do_refine;
     size_t gi = 0;
     while (gi < keys.size() && keys[gi] != key) gi++;
     if (gi == keys.size()) {
@@ -498,6 +429,7 @@ b2s_status create_impl(int batch, const b2s_karto_node_params *params, const b2s
   n->device = device;
   n->n_msg = geometry->n_ranges;
   n->nodes.resize((size_t)batch);
+  int window = 0;  // the longest running window of the nodes
   for (int b = 0; b < batch; b++) {
     const b2s_karto_node_params *p = params + b;
     const double *laser_mount = laser_mounts + 7 * (size_t)b;
@@ -563,10 +495,10 @@ b2s_status create_impl(int batch, const b2s_karto_node_params *params, const b2s
     const b2s_scan_solver *solver = solvers ? solvers + b : nullptr;
     if (solver && (single || solver->compute))
       if (b2s_status st = b2s_mapper_set_scan_solver(k.mapper, solver)) return st;
-    n->cap_base[0] = n->cap_base[1] = std::max(n->cap_base[0], std::max(32, p->mapper.scan_buffer_size + 1));
+    window = std::max(window, p->mapper.scan_buffer_size);
   }
   if (b2s_status st = check_device(device)) return st;
-  n->cap_batch = std::min(std::max(8, 2 * batch), MATCH_MAX_BATCH);
+  if (b2s_status st = match_pool_create(n->matcher_params, n->laser, device, batch, window, &n->matches)) return st;
   if (b2s_status st = occ_batch_create(n->laser, device, &n->maps)) return st;
   *out = n.release();
   return B2S_OK;
@@ -591,8 +523,7 @@ b2s_status b2s_karto_node_create(const b2s_karto_node_params *params, const b2s_
 void b2s_karto_node_destroy(b2s_karto_node *n) {
   if (!n) return;
   for (KartoNodeState &k : n->nodes) b2s_mapper_destroy(k.mapper);
-  for (b2s_matcher *h : n->h)
-    if (h) b2s_matcher_destroy(h);
+  match_pool_destroy(n->matches);
   occ_batch_destroy(n->maps);
   delete n;
 }
