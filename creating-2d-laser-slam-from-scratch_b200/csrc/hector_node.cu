@@ -1,7 +1,8 @@
 // lesson4's HectorMappingRos node (lesson4/src/hector_mapping/hector_slam.cc) over whole recordings, B nodes per handle:
-// host C++ around the device batched HectorSlamProcessor (hector_slam.cu), one processor per node, whose
-// k_hs_stream_node converts and matches every node's scans, one CTA per node.  The publish schedule and the launch
-// parts are hector_node_plan.cuh's; the single-node entry points are the batched ones with B = 1.
+// host C++ around the device batched HectorSlamProcessor (hector_slam.cu), one processor per node, whose ingest kernel
+// k_hs_stream_batch<true, true> converts (hector_scan.cuh, with each node's own filter) and matches every node's scans,
+// one CTA per node.  The publish schedule and the launch parts are hector_node_plan.cuh's; the single-node entry points
+// are the batched ones with B = 1.
 //   HectorMappingRos::InitParams / constructor       hector_slam.cc:26-105, 119-162
 //   HectorMappingRos::setMapInfo                     :165-180
 //   HectorMappingRos::scanCallback                   :186-251  (projectLaser, rosPointCloudToDataContainer, update)
@@ -27,7 +28,7 @@ namespace b2s {
 void hs_node_map_info(const b2s_hector_slam *p, float &origin_x, float &origin_y, float &cell_length, int &w, int &h);
 float hs_scale_to_map(const b2s_hector_slam *p);
 b2s_status hs_node_run(b2s_hector_slam *p, HsNodeIo &io, const b2s_laser_scan_msg &geometry, const double *units,
-                       double range_cutoff, const HectorNodeFilter *filters, const HectorNodePlan &plan,
+                       double range_cutoff, const HectorBeamFilter *filters, const HectorNodePlan &plan,
                        const int32_t *n_scans, const float *ranges, float *out_rows,
                        const std::function<b2s_status(int, int, const int8_t *, const float *, long long)> &on_map);
 }  // namespace b2s
@@ -47,7 +48,7 @@ struct b2s_hector_node {
   b2s_laser_scan_msg geom{};
   int device = 0;
   b2s_hector_slam *proc = nullptr;
-  std::vector<HectorNodeFilter> filters;
+  std::vector<HectorBeamFilter> filters;
   double cutoff = 30.0;  // projector_.projectLaser(scan, laser_point_cloud_, 30.0)
   std::vector<double> units;
   std::vector<int64_t> period_ns;       // Duration::fromSec(map_pub_period)
@@ -171,7 +172,7 @@ b2s_status b2s_hector_node_create_batch(int batch, const b2s_hector_node_params 
   for (int b = 0; b < batch; b++) {
     const b2s_hector_node_params &pb = params[b];
     const double *mount = laser_mounts + 7 * (size_t)b;
-    HectorNodeFilter &f = n->filters[(size_t)b];
+    HectorBeamFilter &f = n->filters[(size_t)b];
     f.sqr_min = static_cast<float>(pb.laser_min_dist * pb.laser_min_dist);
     f.sqr_max = static_cast<float>(pb.laser_max_dist * pb.laser_max_dist);
     f.use_max_scan_range = pb.use_max_scan_range;

@@ -1,12 +1,13 @@
-// lesson4's LaserScan -> DataContainer conversion, per beam, shared by the host adapters (ros_io.cu: b2s_ros_hector_points,
-// b2s_ros_hector_scans) and the ingest stage of the batched stream kernel (hector_slam.cu: k_hs_stream_batch<_, true>),
-// and the node handle's form of it with the laser mount's full basis (hector_node.cu, k_hs_stream_node).
+// lesson4's LaserScan -> DataContainer conversion, per beam, in one definition: the host adapters (ros_io.cu:
+// b2s_ros_hector_points, b2s_ros_hector_scans) and the ingest stage of the batched stream kernel (hector_slam.cu:
+// k_hs_stream_batch<_, true>, behind b2s_hector_slam_process_scans_batch and the node handle, hector_node.cu) all apply
+// it with a HectorBeamFilter, whose mount is a full tf::Transform.
 // HectorMappingRos::scanCallback (lesson4/src/hector_mapping/hector_slam.cc:186-205) does two things to a scan:
 //   projector_.projectLaser(scan, cloud, 30.0)     laser_geometry's LaserProjection (not in the reference tree, see
 //                                                  DESIGN §7: restated from the package's published behaviour)
 //   rosPointCloudToDataContainer                    hector_slam.cc:320-362 (pinned by tests/test_ros_io.py)
-// Only IEEE multiply / add / compare / convert here: the transcendental values (the beams' unit vectors, the laser yaw's
-// cosine and sine) are the host C library's, computed by the caller and passed in, so the device and the host adapter
+// Only IEEE multiply / add / compare / convert here: the transcendental values (the beams' unit vectors, the mount's
+// basis) are the host C library's, computed by the caller and passed in, so the device and the host adapter
 // produce the same points bit for bit under the library's -fmad=false.
 #pragma once
 #include <cmath>
@@ -15,47 +16,6 @@
 #include "ros_math.cuh"
 
 namespace b2s {
-
-// The node's settings of rosPointCloudToDataContainer, prepared once per call (hector_scan_filter).
-struct HectorScanFilter {
-  float sqr_min, sqr_max;      // min_dist^2, max_dist^2 in float (hector_slam.cc:151-155)
-  double use_max_scan_range;
-  double lx, ly, lz, c, s;     // tf::Transform of the laser in base_link (tfScalar = double): translation, cos / sin of yaw
-  float z_min, z_max;
-  float scale_to_map;
-};
-
-// laser_in_base = (x, y, z, yaw) as float; cos / sin of the yaw are taken in double by the host C library
-inline HectorScanFilter hector_scan_filter(const float laser_in_base[4], float scale_to_map, float min_dist, float max_dist,
-                                           double use_max_scan_range, float z_min, float z_max) {
-  HectorScanFilter f;
-  f.sqr_min = min_dist * min_dist;
-  f.sqr_max = max_dist * max_dist;
-  f.use_max_scan_range = use_max_scan_range;
-  f.lx = laser_in_base[0]; f.ly = laser_in_base[1]; f.lz = laser_in_base[2];
-  f.c = cos((double)laser_in_base[3]);
-  f.s = sin((double)laser_in_base[3]);
-  f.z_min = z_min; f.z_max = z_max;
-  f.scale_to_map = scale_to_map;
-  return f;
-}
-
-// rosPointCloudToDataContainer on one laser-frame point: true if the node keeps it, with its DataContainer entry
-// (base_link position in map-cell units) in (ox, oy)
-__host__ __device__ __forceinline__ bool hector_filter_point(const HectorScanFilter &f, float x, float y, float z, float &ox,
-                                                             float &oy) {
-  const float dist_sqr = x * x + y * y;
-  if (!((dist_sqr > f.sqr_min) && (dist_sqr < f.sqr_max))) return false;
-  if ((x < 0.0f) && (dist_sqr < 0.50f)) return false;  // behind the robot
-  if ((double)dist_sqr > f.use_max_scan_range * f.use_max_scan_range) return false;
-  const double bx = f.c * (double)x - f.s * (double)y + f.lx, by = f.s * (double)x + f.c * (double)y + f.ly;
-  const double bz = (double)z + f.lz;
-  const float z_laser = (float)(bz - f.lz);
-  if (!(z_laser > f.z_min && z_laser < f.z_max)) return false;
-  ox = (float)bx * f.scale_to_map;
-  oy = (float)by * f.scale_to_map;
-  return true;
-}
 
 // LaserProjection::projectLaser (sensor_msgs::PointCloud form) on beam i: kept iff range < cutoff (double) and
 // range >= range_min (float); NaN and +-inf drop out.  Point32 x / y = (float)(range * unit vector), z = 0.
@@ -67,16 +27,41 @@ __host__ __device__ __forceinline__ bool hector_project_beam(float range, double
   return true;
 }
 
-// The node's own settings of rosPointCloudToDataContainer (b2s_hector_node_*): the full tf::StampedTransform of the laser
-// mount (base_link <- laser, tfScalar = double) and the thresholds squared in double, then rounded to float, as
-// InitParams stores them (hector_slam.cc:150-155).
-struct HectorNodeFilter {
+// The settings of rosPointCloudToDataContainer: the tf::StampedTransform of the laser mount (base_link <- laser,
+// tfScalar = double) and the squared distance window.  The node handle (hector_node.cu) builds one per node from its
+// parameters; hector_scan_filter builds one from b2s_hector_scan_filter's.
+struct HectorBeamFilter {
   float sqr_min, sqr_max;
   double use_max_scan_range;
-  TfTransform mount;  // basis rows from Matrix3x3::setRotation, origin = the mount's translation
+  TfTransform mount;
   float z_min, z_max;
   float scale_to_map;
 };
+
+// b2s_hector_scan_filter's settings: the mount as (x, y, z, yaw) in float, the yaw's cosine and sine taken in double by
+// the host C library, the thresholds squared in float (the node handle squares them in double, as InitParams does).
+// The basis's third column is -0.0, a deliberate choice: Matrix3x3::setRotation of a yaw quaternion generally puts
+// +0.0 there, but tf_apply adds z * m[i][2] before the translation, and a projected beam has z = +0, so with -0.0 that
+// term is -0.0 and keeps the sign of an exactly-zero rotated sum.  Every beam then lands where c*x - s*y + lx and
+// s*x + c*y + ly put it, bit for bit, as b2s_hector_scan_filter's conversion always has; with +0.0, a rotated sum of -0
+// plus a -0.0 translation would come out +0.  Do not change it to match setRotation's basis.  Only a caller point with
+// z < 0 or z = -0.0 (b2s_ros_hector_points) sees the term as +0.0: there an exactly-zero coordinate may be +0 where
+// c*x - s*y + lx gives -0, which is tf's own arithmetic (Transform::operator*) on this basis.
+inline HectorBeamFilter hector_scan_filter(const float laser_in_base[4], float scale_to_map, float min_dist, float max_dist,
+                                           double use_max_scan_range, float z_min, float z_max) {
+  HectorBeamFilter f;
+  f.sqr_min = min_dist * min_dist;
+  f.sqr_max = max_dist * max_dist;
+  f.use_max_scan_range = use_max_scan_range;
+  const double c = cos((double)laser_in_base[3]), s = sin((double)laser_in_base[3]);
+  f.mount.m[0][0] = c; f.mount.m[0][1] = -s; f.mount.m[0][2] = -0.0;
+  f.mount.m[1][0] = s; f.mount.m[1][1] = c; f.mount.m[1][2] = -0.0;
+  f.mount.m[2][0] = 0.0; f.mount.m[2][1] = 0.0; f.mount.m[2][2] = 1.0;
+  f.mount.o[0] = laser_in_base[0]; f.mount.o[1] = laser_in_base[1]; f.mount.o[2] = laser_in_base[2];
+  f.z_min = z_min; f.z_max = z_max;
+  f.scale_to_map = scale_to_map;
+  return f;
+}
 
 // The node handle's staging for its map publishes (hector_node.cu owns it, hs_node_run in hector_slam.cu fills it): a
 // copy stream, two slots of level-0 payloads (one per node publishing before a part) on the device and page-locked on
@@ -89,9 +74,10 @@ struct HsNodeIo {
   HostBuf<float> h_rows;  // [scans of the call][16], part-major: a part's rows are here once the next part's `copied` fired
 };
 
-// rosPointCloudToDataContainer (hector_slam.cc:331-358) on one laser-frame point with the full mount:
-// laserTransform * Vector3(x, y, z) row by row (tf::Transform::operator*), the z window on that z minus the mount's z
-__host__ __device__ __forceinline__ bool hector_node_filter_point(const HectorNodeFilter &f, float x, float y, float z,
+// rosPointCloudToDataContainer (hector_slam.cc:331-358) on one laser-frame point: true if the node keeps it, with its
+// DataContainer entry (base_link position in map-cell units) in (ox, oy).  laserTransform * Vector3(x, y, z) row by row
+// (tf::Transform::operator*), the z window on that z minus the mount's z.
+__host__ __device__ __forceinline__ bool hector_node_filter_point(const HectorBeamFilter &f, float x, float y, float z,
                                                                   float &ox, float &oy) {
   const float dist_sqr = x * x + y * y;
   if (!((dist_sqr > f.sqr_min) && (dist_sqr < f.sqr_max))) return false;
@@ -108,19 +94,11 @@ __host__ __device__ __forceinline__ bool hector_node_filter_point(const HectorNo
 }
 
 // projectLaser and the node's conversion on one beam
-__host__ __device__ __forceinline__ bool hector_node_beam(const HectorNodeFilter &f, float range, double ux, double uy,
+__host__ __device__ __forceinline__ bool hector_node_beam(const HectorBeamFilter &f, float range, double ux, double uy,
                                                           double cutoff, float range_min, float &ox, float &oy) {
   float x, y;
   if (!hector_project_beam(range, ux, uy, cutoff, range_min, x, y)) return false;
   return hector_node_filter_point(f, x, y, 0.0f, ox, oy);
-}
-
-// Both stages on one beam
-__host__ __device__ __forceinline__ bool hector_scan_beam(const HectorScanFilter &f, float range, double ux, double uy,
-                                                          double cutoff, float range_min, float &ox, float &oy) {
-  float x, y;
-  if (!hector_project_beam(range, ux, uy, cutoff, range_min, x, y)) return false;
-  return hector_filter_point(f, x, y, 0.0f, ox, oy);
 }
 
 // getUnitVectors_: cos / sin(angle_min + (double)i * angle_increment) in double by the host C library, the float32 message

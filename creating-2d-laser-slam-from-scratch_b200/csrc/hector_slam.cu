@@ -292,8 +292,9 @@ __host__ __device__ inline size_t hs_smem_bytes(int cap) { return hs_terms_offse
 // MapRepMultiMap::matchData (:144-166) on every level, coarsest first, + the gate and the update parameters of
 // HectorSlamProcessor::update (:81-108), by ONE CTA for processor b.
 // Returns the gate's verdict (map update or not).
-// FIXED_ORIGO (k_hs_stream_node): the container's origo is the processor's own, already in st->origo[0], not C's.
-template <bool EXACT, bool CLUSTER, bool FIXED_ORIGO = false>
+// INGEST (k_hs_stream_batch<_, true>): the container's origo is the processor's own, which the host wrote into
+// st->origo[0] before the launch (hs_ingest_upload), not C's.
+template <bool EXACT, bool CLUSTER, bool INGEST = false>
 __device__ bool hs_match_cta(const HsBatch &P, const HsCall &C, int b, unsigned char *smem, HsXchg *xc = nullptr,
                              uint32_t *xc_parity = nullptr) {
   static_assert(!(EXACT && CLUSTER), "the bit-exact sums are one sequential chain: nothing to split");
@@ -514,7 +515,7 @@ __device__ bool hs_match_cta(const HsBatch &P, const HsCall &C, int b, unsigned 
 #pragma unroll
       for (int q = 0; q < 9; q++) st->last_cov[q] = lcov[q];
     }
-    const float origo_x = FIXED_ORIGO ? st->origo[0][0] : C.origo_x, origo_y = FIXED_ORIGO ? st->origo[0][1] : C.origo_y;
+    const float origo_x = INGEST ? st->origo[0][0] : C.origo_x, origo_y = INGEST ? st->origo[0][1] : C.origo_y;
     if (!C.map_without_matching) {
       st->n_matched = n_matched0 + 1;
       if (n > 0) {
@@ -930,56 +931,52 @@ struct HsFleet {
   const float *pts;          // every scan's points, processor-major ([sum n_points][2])
   const long long *offsets;  // [total scans] first point of each scan (64-bit: a fleet's recordings exceed 2^31 floats)
   const int *counts;         // [total scans]
-  const long long *first;    // [B + 1] first scan of processor b (scans first[b] ... first[b + 1] - 1)
+  const long long *first;    // [B][2] processor b's scans first[2b] ... first[2b + 1] - 1 (a node call's part ends a
+                             // processor's scans before the next one's begin)
   const float *hints;        // [total scans][3] or NULL (chain through the processor's last scan-match pose)
   const float *first_hints;  // [B][3] or NULL: hint of each processor's first scan when chaining
-  float origo_x, origo_y;
+  float origo_x, origo_y;    // (ingest: unused, each processor's own is in its state)
   int map_without_matching;
   float *out;                // [total scans][16]
-  const struct HsIngest *ingest;  // device: the ingest variant's input (k_hs_stream_batch<_, true>), else NULL
+  const struct HsIngest *ingest;  // device: the ingest kernel's input (k_hs_stream_batch<_, true>), else NULL
 };
 
 // Scans as raw LaserScan ranges (k_hs_stream_batch<_, true>): F.pts / offsets / counts are unused.  In device memory
-// behind one pointer: a larger kernel parameter block costs the existing instantiations registers.
+// behind one pointer: a larger kernel parameter block costs the point-stream instantiations registers.
 struct HsIngest {
   const float *ranges;       // [total scans][n_ranges] float32
   const double2 *units;      // [n_ranges] the beams' unit vectors (host C library cos / sin)
   int n_ranges;
   float range_min;
   double range_cutoff;       // projectLaser's cutoff (a negative one already replaced by range_max)
-  HectorScanFilter filter;
-  const HectorNodeFilter *nodes;  // [B] device: k_hs_stream_node's conversion of each node (its full laser mount)
+  const HectorBeamFilter *filters;  // [B] processor b's conversion
 };
 
-// The node's loop of processor b = blockIdx.x over its scans: match (hs_match_cta), then, if the gate opens, the mark
-// and apply passes on this CTA's 18 warps.  Nothing crosses CTAs: no grid barrier, no verdict tags, and B may exceed the
+// The loop of processor b = blockIdx.x over its scans: match (hs_match_cta), then, if the gate opens, the mark and
+// apply passes on this CTA's 18 warps.  Nothing crosses CTAs: no grid barrier, no verdict tags, and B may exceed the
 // resident CTAs (later processors start as earlier ones finish).  The match reads the probability quads with plain
 // (L1-allocating, coherent) loads that the SAME CTA rewrote in its previous apply pass; the __syncthreads after the
 // apply orders those stores before the loads (CTA scope), so no L1 drop is needed as in k_hs_stream.
 //
-// INGEST: each scan arrives as n_ranges float32 ranges.  Before its match the CTA converts it (hector_scan.cuh: the
-// node's projectLaser + rosPointCloudToDataContainer, per beam) and compacts the kept beams in beam order into its level-0
-// container row, HS_THREADS beams per round: ballot / popc inside a warp, warp offsets through shared memory, a running
-// base across rounds.  hs_match_cta then reads that row as its input and copies it onto itself: each element is read and
-// written back unchanged by the same thread, which is benign.
-// INGEST selects the conversion: HS_INGEST_YAW (k_hs_stream_batch<_, true>: hector_scan_beam, the mount as x, y, z, yaw)
-// or HS_INGEST_NODE (k_hs_stream_node: hector_node_beam with node b's filter I.nodes[b], the mount's full basis, and the
-// origo of that mount, for b2s_hector_node_*).  For HS_INGEST_NODE, F.first is one part of a node call: [B][2] =
-// (first scan, end scan) of node b, since a node's end inside a part is not the next node's begin.
-enum { HS_INGEST_NONE = 0, HS_INGEST_YAW = 1, HS_INGEST_NODE = 2 };
-template <bool EXACT, int INGEST>
-__device__ __forceinline__ void hs_stream_batch_body(const HsBatch &P, const HsFleet &F, unsigned char *hs_smem) {
+// INGEST: each scan arrives as n_ranges float32 ranges.  Before its match the CTA converts it with processor b's filter
+// (hector_scan.cuh: the node's projectLaser + rosPointCloudToDataContainer, per beam) and compacts the kept beams in
+// beam order into its level-0 container row, HS_THREADS beams per round: ballot / popc inside a warp, warp offsets
+// through shared memory, a running base across rounds.  hs_match_cta then reads that row as its input and copies it
+// onto itself: each element is read and written back unchanged by the same thread, which is benign.  The container's
+// origo is the processor's own (hs_match_cta<_, _, true>).
+template <bool EXACT, bool INGEST>
+__global__ void __launch_bounds__(HS_THREADS, 1) k_hs_stream_batch(HsBatch P, HsFleet F) {
+  extern __shared__ __align__(16) unsigned char hs_smem[];
   __shared__ float s_last[3];  // the previous scan's match pose: the next scan's hint without a global round trip
   const int b = blockIdx.x;
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   constexpr int NW = HS_THREADS / 32;
   HsState *st = P.state + b;
-  constexpr bool NODE = INGEST == HS_INGEST_NODE;
-  const long long s0 = NODE ? F.first[2 * b] : F.first[b], s1 = NODE ? F.first[2 * b + 1] : F.first[b + 1];
+  const long long s0 = F.first[2 * b], s1 = F.first[2 * b + 1];
   unsigned long long visits = 0;
   for (long long i = s0; i < s1; i++) {
     HsCall C;
-    if constexpr (INGEST != HS_INGEST_NONE) {
+    if constexpr (INGEST) {
       __shared__ int s_warp_kept[NW];
       const HsIngest &I = *F.ingest;
       float2 *row = reinterpret_cast<float2 *>(P.l[0].pts) + (size_t)b * P.cap;
@@ -992,10 +989,7 @@ __device__ __forceinline__ void hs_stream_batch_body(const HsBatch &P, const HsF
         bool keep = false;
         if (j < nr) {
           const double2 u = I.units[j];
-          if constexpr (INGEST == HS_INGEST_NODE)
-            keep = hector_node_beam(I.nodes[b], r[j], u.x, u.y, I.range_cutoff, I.range_min, q.x, q.y);
-          else
-            keep = hector_scan_beam(I.filter, r[j], u.x, u.y, I.range_cutoff, I.range_min, q.x, q.y);
+          keep = hector_node_beam(I.filters[b], r[j], u.x, u.y, I.range_cutoff, I.range_min, q.x, q.y);
         }
         const unsigned m = __ballot_sync(0xffffffffu, keep);
         if (lane == 0) s_warp_kept[warp] = __popc(m);
@@ -1022,7 +1016,7 @@ __device__ __forceinline__ void hs_stream_batch_body(const HsBatch &P, const HsF
     }
     C.pts_stride = 0;
     C.hints = F.hints ? F.hints + 3 * i : (i > s0 ? s_last : (F.first_hints ? F.first_hints + 3 * (size_t)b : nullptr));
-    C.origo_x = F.origo_x; C.origo_y = F.origo_y;  // (NODE: unused, hs_node_run set each processor's own)
+    C.origo_x = F.origo_x; C.origo_y = F.origo_y;
     C.map_without_matching = F.map_without_matching;
     C.out = F.out + 16 * i;
     C.mailbox = nullptr;
@@ -1030,7 +1024,7 @@ __device__ __forceinline__ void hs_stream_batch_body(const HsBatch &P, const HsF
     C.tag = 0;
     C.carry = s_last;
     C.own_row = 1;
-    if (hs_match_cta<EXACT, false, NODE>(P, C, b, hs_smem)) {
+    if (hs_match_cta<EXACT, false, INGEST>(P, C, b, hs_smem)) {
       const unsigned long long t0 = hs_now_ns();
       visits += hs_mark_pass(P, b, warp, NW, lane);  // (lane 0 carries the warp's count)
       __syncthreads();
@@ -1040,19 +1034,6 @@ __device__ __forceinline__ void hs_stream_batch_body(const HsBatch &P, const HsF
     }
   }
   if (lane == 0 && visits) atomicAdd(&st->visits, visits);
-}
-
-template <bool EXACT, bool INGEST>
-__global__ void __launch_bounds__(HS_THREADS, 1) k_hs_stream_batch(HsBatch P, HsFleet F) {
-  extern __shared__ __align__(16) unsigned char hs_smem[];
-  hs_stream_batch_body<EXACT, INGEST ? HS_INGEST_YAW : HS_INGEST_NONE>(P, F, hs_smem);
-}
-
-// lesson4's HectorMappingRos (b2s_hector_node_*): k_hs_stream_batch's loop with each node's full-basis conversion, exact
-// mode, one processor per CTA (node b = blockIdx.x), over node b's scans of one part of a node call
-__global__ void __launch_bounds__(HS_THREADS, 1) k_hs_stream_node(HsBatch P, HsFleet F) {
-  extern __shared__ __align__(16) unsigned char hs_smem[];
-  hs_stream_batch_body<true, HS_INGEST_NODE>(P, F, hs_smem);
 }
 
 __global__ void k_hs_fill(float *__restrict__ p, size_t n, float v) {
@@ -1217,7 +1198,6 @@ static b2s_status hs_create(float map_resolution, int map_size_x, int map_size_y
   B2S_CUDA_CHECK(raise_dyn_smem(k_hs_stream_batch<false, false>, smem));
   B2S_CUDA_CHECK(raise_dyn_smem(k_hs_stream_batch<true, true>, smem));
   B2S_CUDA_CHECK(raise_dyn_smem(k_hs_stream_batch<false, true>, smem));
-  B2S_CUDA_CHECK(raise_dyn_smem(k_hs_stream_node, smem));
   {
     int coop = 0, sms = 0, per_sm = 0;
     B2S_CUDA_CHECK(cudaDeviceGetAttribute(&coop, cudaDevAttrCooperativeLaunch, device));
@@ -1305,20 +1285,20 @@ static b2s_status hs_launch_stream(b2s_hector_slam *p, const HsStream &S) {
   return B2S_OK;
 }
 
-// Processor b's scans of a batched call are first[b] ... first[b + 1] - 1 (first has B + 1 entries).  Refuses negative
-// counts; `longest` is the most scans of one processor.
+// Processor b's scans of a batched call are first[2b] ... first[2b + 1] - 1 (HsFleet::first), in processor order, so
+// the call has first.back() scans.  Refuses negative counts; `longest` is the most scans of one processor.
 static b2s_status hs_fleet_counts(const b2s_hector_slam *p, const int32_t *n_scans, std::vector<long long> &first, int &longest) {
   const int B = p->batch;
-  first.assign((size_t)B + 1, 0);
+  first.assign(2 * (size_t)B, 0);
   long long total = 0;
   longest = 0;
   for (int b = 0; b < B; b++) {
     if (n_scans[b] < 0) B2S_FAIL(B2S_ERR_BAD_PARAMS, "negative scan count");
-    first[b] = total;
+    first[2 * (size_t)b] = total;
     total += n_scans[b];
+    first[2 * (size_t)b + 1] = total;
     longest = std::max(longest, (int)n_scans[b]);
   }
-  first[B] = total;
   return B2S_OK;
 }
 
@@ -1330,7 +1310,7 @@ static b2s_status hs_fleet_run(b2s_hector_slam *p, const int32_t *n_scans, const
                                float *out_poses, int32_t *out_map_updated, float *out_last_covs, int32_t *out_n_points,
                                Upload &upload) {
   const int B = p->batch;
-  const size_t T = (size_t)first[(size_t)B];
+  const size_t T = (size_t)first.back();
   if (T == 0) return B2S_OK;
   B2S_CUDA_CHECK(cudaSetDevice(p->device));
   b2s_status st = hs_wait_launch(p);
@@ -1341,9 +1321,9 @@ static b2s_status hs_fleet_run(b2s_hector_slam *p, const int32_t *n_scans, const
   if ((st = upload(F))) return st;
   AsyncBuf<float> d_hints(p->stream), d_first_hints(p->stream), d_out(p->stream);
   AsyncBuf<long long> d_first(p->stream);
-  B2S_CUDA_CHECK(d_first.alloc((size_t)B + 1));
+  B2S_CUDA_CHECK(d_first.alloc(first.size()));
   B2S_CUDA_CHECK(d_out.alloc(16 * T));
-  B2S_CUDA_CHECK(cudaMemcpyAsync(d_first, first.data(), sizeof(long long) * ((size_t)B + 1), cudaMemcpyHostToDevice, p->stream));
+  B2S_CUDA_CHECK(cudaMemcpyAsync(d_first, first.data(), sizeof(long long) * first.size(), cudaMemcpyHostToDevice, p->stream));
   if (pose_hints) {
     B2S_CUDA_CHECK(d_hints.alloc(3 * T));
     B2S_CUDA_CHECK(cudaMemcpyAsync(d_hints, pose_hints, sizeof(float) * 3 * T, cudaMemcpyHostToDevice, p->stream));
@@ -1374,7 +1354,86 @@ static b2s_status hs_fleet_run(b2s_hector_slam *p, const int32_t *n_scans, const
   }
   if (out_last_covs && !map_without_matching)
     for (int b = 0; b < B; b++)
-      if (n_scans[b] > 0) std::memcpy(out_last_covs + 9 * (size_t)b, host.data() + 16 * (size_t)(first[b + 1] - 1) + 3, 9 * sizeof(float));
+      if (n_scans[b] > 0) std::memcpy(out_last_covs + 9 * (size_t)b, host.data() + 16 * (size_t)(first[2 * (size_t)b + 1] - 1) + 3, 9 * sizeof(float));
+  return B2S_OK;
+}
+
+// One batched step on the processor's stream: k_hs_match of scan b = the d_n_points[b] points at d_points + 2 b cap,
+// then the grid-wide map update passes (k_hs_mark, k_hs_apply); max_n is the step's largest point count
+static b2s_status hs_launch_step(b2s_hector_slam *p, const float *d_points, const int32_t *d_n_points, int max_n,
+                                 const float origo[2], const float *d_pose_hints, int map_without_matching) {
+  const int B = p->batch;
+  HsCall C;
+  std::memset(&C, 0, sizeof(C));
+  C.pts0 = d_points; C.n0 = d_n_points; C.pts_stride = p->cap;
+  C.hints = d_pose_hints;
+  C.origo_x = origo[0]; C.origo_y = origo[1];
+  C.map_without_matching = map_without_matching;
+  C.out = p->d_out;
+  if (p->P.exact) k_hs_match<true><<<B, HS_THREADS, hs_smem_bytes(p->cap), p->stream>>>(p->P, C);
+  else k_hs_match<false><<<B, HS_THREADS, hs_smem_bytes(p->cap), p->stream>>>(p->P, C);
+  // data containers of the coarse levels may hold more points than this step's scans (map_without_matching): size the
+  // update grid by the capacity bound
+  const dim3 grid(std::max(1, std::min(ceil_div(std::max(max_n, 1) * p->levels, 8), sm_count(p->device) * 8 / std::max(1, std::min(B, 8)))), B);
+  k_hs_mark<<<grid, 256, 0, p->stream>>>(p->P);
+  k_hs_apply<<<grid, 256, 0, p->stream>>>(p->P);
+  B2S_CUDA_CHECK(cudaGetLastError());
+  return B2S_OK;
+}
+
+// k_hs_stream_batch<_, true>'s input in device memory, freed in stream order with the caller: the ranges, the unit
+// vectors, and one block holding the HsIngest (`ingest`), then the B filters, then the B level-0 origos
+struct HsIngestUpload {
+  AsyncBuf<float> ranges;
+  AsyncBuf<double> units;
+  AsyncBuf<unsigned char> block;
+  const HsIngest *ingest = nullptr;
+  explicit HsIngestUpload(cudaStream_t s) : ranges(s), units(s), block(s) {}
+};
+
+// Uploads the call's n_scans x nr ranges, the beams' unit vectors ([nr][2]) and processor b's filter filters[b], and
+// writes each processor's level-0 origo: dataContainer.setOrigo (hector_slam.cc:329) of its mount, the same on every
+// scan, which the ingest kernel's match reads there (hs_match_cta<_, _, true>) instead of a per-CTA value held through
+// the scan loop.  The origo of a processor without scans in the call is not read before it is written again: every
+// other match writes origo[0] before reading it, and every ingest launch follows this call's write.
+// The descriptor, the filters and the origos travel in ONE copy from pageable memory (each such copy is staged by the
+// host before it returns, several microseconds that a call per scan pays every scan); the origos then reach the
+// processors' states by a copy on the device.
+static b2s_status hs_ingest_upload(b2s_hector_slam *p, HsIngestUpload &d, size_t n_scans, int nr, const float *ranges,
+                                   const double *units, float range_min, double range_cutoff,
+                                   const HectorBeamFilter *filters) {
+  static_assert(sizeof(HsIngest) % alignof(HectorBeamFilter) == 0 && sizeof(HectorBeamFilter) % alignof(float2) == 0,
+                "the block's parts stay aligned");
+  const int B = p->batch;
+  const size_t n_r = n_scans * (size_t)nr;
+  const size_t at_filters = sizeof(HsIngest), at_origo = at_filters + sizeof(HectorBeamFilter) * (size_t)B;
+  const size_t bytes = at_origo + sizeof(float2) * (size_t)B;
+  B2S_CUDA_CHECK(d.ranges.alloc(std::max<size_t>(n_r, 1)));
+  B2S_CUDA_CHECK(d.units.alloc(2 * (size_t)std::max(nr, 1)));
+  B2S_CUDA_CHECK(d.block.alloc(bytes));
+  std::vector<unsigned char> h(bytes);
+  HsIngest I;
+  std::memset(&I, 0, sizeof(I));
+  I.ranges = d.ranges;
+  I.units = reinterpret_cast<const double2 *>(static_cast<double *>(d.units));
+  I.n_ranges = nr;
+  I.range_min = range_min;
+  I.range_cutoff = range_cutoff;
+  I.filters = reinterpret_cast<const HectorBeamFilter *>(d.block.p + at_filters);
+  std::memcpy(h.data(), &I, sizeof(I));
+  std::memcpy(h.data() + at_filters, filters, sizeof(HectorBeamFilter) * (size_t)B);
+  for (int b = 0; b < B; b++) {
+    const float2 o = make_float2((float)filters[b].mount.o[0] * filters[b].scale_to_map,
+                                 (float)filters[b].mount.o[1] * filters[b].scale_to_map);
+    std::memcpy(h.data() + at_origo + sizeof(float2) * (size_t)b, &o, sizeof(o));
+  }
+  // (pageable sources: staged before the calls return)
+  if (n_r > 0) B2S_CUDA_CHECK(cudaMemcpyAsync(d.ranges, ranges, sizeof(float) * n_r, cudaMemcpyHostToDevice, p->stream));
+  if (nr > 0) B2S_CUDA_CHECK(cudaMemcpyAsync(d.units, units, sizeof(double) * 2 * (size_t)nr, cudaMemcpyHostToDevice, p->stream));
+  B2S_CUDA_CHECK(cudaMemcpyAsync(d.block, h.data(), bytes, cudaMemcpyHostToDevice, p->stream));
+  B2S_CUDA_CHECK(cudaMemcpy2DAsync(&p->d_state.p[0].origo[0][0], sizeof(HsState), d.block.p + at_origo, sizeof(float2),
+                                   sizeof(float2), (size_t)B, cudaMemcpyDeviceToDevice, p->stream));
+  d.ingest = reinterpret_cast<const HsIngest *>(d.block.p);
   return B2S_OK;
 }
 
@@ -1402,14 +1461,15 @@ static __global__ void k_hector_ros_nodes(const float *__restrict__ lo, int cell
   out[(size_t)blockIdx.y * cells + i] = hector_ros_cell(lo[(size_t)nodes[blockIdx.y] * cells + i]);
 }
 
-// The call runs as the plan's parts (hector_node_plan.cuh), one k_hs_stream_node launch of B CTAs per part that has
-// scans, CTA b on node b's scans of the part.  Before part k >= 1, one k_hector_ros_nodes launch on the processor's
-// stream converts level 0 of every node publishing there into one slot of payloads; a second stream copies the slot,
-// with those nodes' record rows of part k - 1, into page-locked memory while part k's launch runs.  Two slots: a slot
-// is handed to on_map (part by part, nodes ascending inside a part) before it is converted into again.  on_map(b, k,
-// payload, rows, n) also gets node b's n record rows since its previous publish.  Rows are node-major throughout.
+// The call runs as the plan's parts (hector_node_plan.cuh), one k_hs_stream_batch<true, true> launch of B CTAs per
+// part that has scans, CTA b on node b's scans of the part.  Before part k >= 1, one k_hector_ros_nodes launch on the
+// processor's stream converts level 0 of every node publishing there into one slot of payloads; a second stream copies
+// the slot, with those nodes' record rows of part k - 1, into page-locked memory while part k's launch runs.  Two
+// slots: a slot is handed to on_map (part by part, nodes ascending inside a part) before it is converted into again.
+// on_map(b, k, payload, rows, n) also gets node b's n record rows since its previous publish.  Rows are node-major
+// throughout.
 b2s_status hs_node_run(b2s_hector_slam *p, HsNodeIo &io, const b2s_laser_scan_msg &geometry, const double *units,
-                       double range_cutoff, const HectorNodeFilter *filters, const HectorNodePlan &plan,
+                       double range_cutoff, const HectorBeamFilter *filters, const HectorNodePlan &plan,
                        const int32_t *n_scans, const float *ranges, float *out_rows,
                        const std::function<b2s_status(int, int, const int8_t *, const float *, long long)> &on_map) {
   const int nr = geometry.n_ranges, B = plan.batch, K = plan.n_parts;
@@ -1448,44 +1508,16 @@ b2s_status hs_node_run(b2s_hector_slam *p, HsNodeIo &io, const b2s_laser_scan_ms
       B2S_CUDA_CHECK(io.d_map[s].reserve(most * cells));
       B2S_CUDA_CHECK(io.h_map[s].reserve(most * cells));
     }
-  AsyncBuf<float> d_ranges(p->stream), d_out(p->stream);
-  AsyncBuf<double> d_unit(p->stream);
-  AsyncBuf<HsIngest> d_ingest(p->stream);
-  AsyncBuf<HectorNodeFilter> d_filters(p->stream);
+  HsIngestUpload d_in(p->stream);
+  AsyncBuf<float> d_out(p->stream);
   AsyncBuf<long long> d_parts(p->stream);
   AsyncBuf<int> d_pub(p->stream);
-  const size_t n_r = T * (size_t)nr;
-  B2S_CUDA_CHECK(d_ranges.alloc(std::max<size_t>(n_r, 1)));
-  B2S_CUDA_CHECK(d_unit.alloc(2 * (size_t)std::max(nr, 1)));
-  B2S_CUDA_CHECK(d_ingest.alloc(1));
-  B2S_CUDA_CHECK(d_filters.alloc((size_t)B));
   B2S_CUDA_CHECK(d_parts.alloc(parts.size()));
   B2S_CUDA_CHECK(d_pub.alloc(std::max<size_t>(pub.size(), 1)));
   B2S_CUDA_CHECK(d_out.alloc(16 * std::max<size_t>(T, 1)));
-  if (n_r > 0) B2S_CUDA_CHECK(cudaMemcpyAsync(d_ranges, ranges, sizeof(float) * n_r, cudaMemcpyHostToDevice, p->stream));
-  if (nr > 0) B2S_CUDA_CHECK(cudaMemcpyAsync(d_unit, units, sizeof(double) * 2 * (size_t)nr, cudaMemcpyHostToDevice, p->stream));
-  // (pageable sources: staged before the calls return)
-  B2S_CUDA_CHECK(cudaMemcpyAsync(d_filters, filters, sizeof(HectorNodeFilter) * (size_t)B, cudaMemcpyHostToDevice, p->stream));
+  if ((st = hs_ingest_upload(p, d_in, T, nr, ranges, units, geometry.range_min, range_cutoff, filters))) return st;
   B2S_CUDA_CHECK(cudaMemcpyAsync(d_parts, parts.data(), sizeof(long long) * parts.size(), cudaMemcpyHostToDevice, p->stream));
   if (!pub.empty()) B2S_CUDA_CHECK(cudaMemcpyAsync(d_pub, pub.data(), sizeof(int) * pub.size(), cudaMemcpyHostToDevice, p->stream));
-  // dataContainer.setOrigo (hector_slam.cc:329) of node b's mount, the same every scan: the processor's level-0 origo,
-  // which k_hs_stream_node's match reads (hs_match_cta<_, _, true>) instead of a per-CTA value held through the loop
-  std::vector<float> origo(2 * (size_t)B);
-  for (int b = 0; b < B; b++) {
-    origo[2 * (size_t)b] = (float)filters[b].mount.o[0] * filters[b].scale_to_map;
-    origo[2 * (size_t)b + 1] = (float)filters[b].mount.o[1] * filters[b].scale_to_map;
-  }
-  B2S_CUDA_CHECK(cudaMemcpy2DAsync(&p->d_state.p[0].origo[0][0], sizeof(HsState), origo.data(), 2 * sizeof(float),
-                                   2 * sizeof(float), (size_t)B, cudaMemcpyHostToDevice, p->stream));
-  HsIngest I;
-  std::memset(&I, 0, sizeof(I));
-  I.ranges = d_ranges;
-  I.units = reinterpret_cast<const double2 *>(static_cast<double *>(d_unit));
-  I.n_ranges = nr;
-  I.range_min = geometry.range_min;
-  I.range_cutoff = range_cutoff;
-  I.nodes = d_filters;
-  B2S_CUDA_CHECK(cudaMemcpyAsync(d_ingest, &I, sizeof(HsIngest), cudaMemcpyHostToDevice, p->stream));
   // the copy stream reads d_out: on every way out it is drained before the stream-ordered frees above
   struct DrainCopies {
     cudaStream_t s;
@@ -1493,7 +1525,7 @@ b2s_status hs_node_run(b2s_hector_slam *p, HsNodeIo &io, const b2s_laser_scan_ms
   } drain_copies{io.copy};
   HsFleet F;
   std::memset(&F, 0, sizeof(F));
-  F.ingest = d_ingest;
+  F.ingest = d_in.ingest;
   F.out = d_out;
   const size_t smem = hs_smem_bytes(p->cap);
   struct Pending { int k, slot; };
@@ -1537,7 +1569,7 @@ b2s_status hs_node_run(b2s_hector_slam *p, HsNodeIo &io, const b2s_laser_scan_ms
     for (int b = 0; b < B; b++) scans += parts[2 * ((size_t)k * B + b) + 1] - parts[2 * ((size_t)k * B + b)];
     if (scans > 0) {
       F.first = d_parts + 2 * (size_t)k * B;
-      k_hs_stream_node<<<B, HS_THREADS, smem, p->stream>>>(p->P, F);
+      k_hs_stream_batch<true, true><<<B, HS_THREADS, smem, p->stream>>>(p->P, F);
       B2S_CUDA_CHECK(cudaGetLastError());
     }
   }
@@ -1727,7 +1759,7 @@ b2s_status b2s_hector_slam_process_stream_batch(b2s_hector_slam *p, const int32_
   int longest = 0;
   b2s_status st = hs_fleet_counts(p, n_scans, first, longest);
   if (st) return st;
-  const long long total = first[(size_t)p->batch];
+  const long long total = first.back();
   if (total > 0 && (!points || !n_points)) B2S_FAIL(B2S_ERR_BAD_PARAMS, "null argument");
   if ((unsigned)longest >= HS_EPOCH_MAX) B2S_FAIL(B2S_ERR_TOO_LARGE, "too many scans of one processor in one call (stamp epochs are 20 bits)");
   std::vector<long long> offs((size_t)total);
@@ -1772,36 +1804,22 @@ b2s_status b2s_hector_slam_process_scans_batch(b2s_hector_slam *p, const b2s_las
   int longest = 0;
   b2s_status st = hs_fleet_counts(p, n_scans, first, longest);
   if (st) return st;
-  const long long total = first[(size_t)p->batch];
+  const long long total = first.back();
   if (total > 0 && n > 0 && !ranges) B2S_FAIL(B2S_ERR_BAD_PARAMS, "null argument");
   if ((unsigned)longest >= HS_EPOCH_MAX) B2S_FAIL(B2S_ERR_TOO_LARGE, "too many scans of one processor in one call (stamp epochs are 20 bits)");
   const float scale_to_map = p->P.l[0].tf.tw_lin;  // GridMapBase::getScaleToMap of level 0: 1 / cell length
   const b2s_hector_scan_filter &q = *filter;
-  const HectorScanFilter f = hector_scan_filter(q.laser_in_base, scale_to_map, q.min_dist, q.max_dist, q.use_max_scan_range,
+  const HectorBeamFilter f = hector_scan_filter(q.laser_in_base, scale_to_map, q.min_dist, q.max_dist, q.use_max_scan_range,
                                                 q.z_min, q.z_max);
-  std::vector<double> unit(2 * (size_t)std::max(n, 1));
+  const std::vector<HectorBeamFilter> filters((size_t)p->batch, f);  // one laser: every processor converts alike
+  std::vector<double> unit(2 * (size_t)n);
   hector_unit_vectors(geometry->angle_min, geometry->angle_increment, n, unit.data());
-  AsyncBuf<float> d_ranges(p->stream);
-  AsyncBuf<double> d_unit(p->stream);
-  AsyncBuf<HsIngest> d_ingest(p->stream);
-  HsIngest I;  // (pageable: the copy is staged before cudaMemcpyAsync returns)
+  HsIngestUpload d_in(p->stream);
   auto upload = [&](HsFleet &F) -> b2s_status {
-    const size_t nr = (size_t)total * (size_t)n;
-    B2S_CUDA_CHECK(d_ranges.alloc(std::max<size_t>(nr, 1)));
-    B2S_CUDA_CHECK(d_unit.alloc(unit.size()));
-    B2S_CUDA_CHECK(d_ingest.alloc(1));
-    if (nr > 0) B2S_CUDA_CHECK(cudaMemcpyAsync(d_ranges, ranges, sizeof(float) * nr, cudaMemcpyHostToDevice, p->stream));
-    B2S_CUDA_CHECK(cudaMemcpyAsync(d_unit, unit.data(), sizeof(double) * unit.size(), cudaMemcpyHostToDevice, p->stream));
-    I.ranges = d_ranges;
-    I.units = reinterpret_cast<const double2 *>(static_cast<double *>(d_unit));
-    I.n_ranges = n;
-    I.range_min = geometry->range_min;
-    I.range_cutoff = hector_range_cutoff(q.range_cutoff, geometry->range_max);
-    I.filter = f;
-    B2S_CUDA_CHECK(cudaMemcpyAsync(d_ingest, &I, sizeof(HsIngest), cudaMemcpyHostToDevice, p->stream));
-    F.ingest = d_ingest;
-    F.origo_x = (float)f.lx * scale_to_map;  // as b2s_ros_hector_scans' out_origo
-    F.origo_y = (float)f.ly * scale_to_map;
+    if (b2s_status s = hs_ingest_upload(p, d_in, (size_t)total, n, ranges, unit.data(), geometry->range_min,
+                                        hector_range_cutoff(q.range_cutoff, geometry->range_max), filters.data()))
+      return s;
+    F.ingest = d_in.ingest;
     return B2S_OK;
   };
   return hs_fleet_run(p, n_scans, first, longest, true, first_pose_hints, pose_hints, map_without_matching, out_poses,
@@ -1830,23 +1848,9 @@ b2s_status b2s_hector_slam_update_batch(b2s_hector_slam *p, const float *points,
     B2S_CUDA_CHECK(d_hints.alloc(3 * (size_t)B));
     B2S_CUDA_CHECK(cudaMemcpyAsync(d_hints, pose_hints, sizeof(float) * 3 * (size_t)B, cudaMemcpyHostToDevice, p->stream));
   }
-  HsCall C;
-  std::memset(&C, 0, sizeof(C));
-  C.pts0 = d_pts; C.n0 = d_cnt; C.pts_stride = p->cap;
-  C.hints = d_hints;
-  C.origo_x = origo[0]; C.origo_y = origo[1];
-  C.map_without_matching = map_without_matching;
-  C.out = p->d_out;
   int max_n = 0;
   for (int b = 0; b < B; b++) max_n = std::max(max_n, n_points[b]);
-  if (p->P.exact) k_hs_match<true><<<B, HS_THREADS, hs_smem_bytes(p->cap), p->stream>>>(p->P, C);
-  else k_hs_match<false><<<B, HS_THREADS, hs_smem_bytes(p->cap), p->stream>>>(p->P, C);
-  // data containers of the coarse levels may hold more points than this step's scans (map_without_matching): size the
-  // update grid by the capacity bound
-  const dim3 grid(std::max(1, std::min(ceil_div(std::max(max_n, 1) * p->levels, 8), sm_count(p->device) * 8 / std::max(1, std::min(B, 8)))), B);
-  k_hs_mark<<<grid, 256, 0, p->stream>>>(p->P);
-  k_hs_apply<<<grid, 256, 0, p->stream>>>(p->P);
-  B2S_CUDA_CHECK(cudaGetLastError());
+  if ((st = hs_launch_step(p, d_pts, d_cnt, max_n, origo, d_hints, map_without_matching))) return st;
   B2S_CUDA_CHECK(cudaMemcpyAsync(p->h_out, p->d_out, sizeof(float) * 16 * (size_t)B, cudaMemcpyDeviceToHost, p->stream));
   B2S_CUDA_CHECK(cudaStreamSynchronize(p->stream));
   for (int b = 0; b < B; b++) {
@@ -1869,21 +1873,7 @@ b2s_status b2s_hector_slam_update_batch_device(b2s_hector_slam *p, const float *
   b2s_status st = hs_wait_launch(p);
   if (st) return st;
   if ((st = hs_reserve_epochs(p, 1))) return st;
-  const int B = p->batch;
-  HsCall C;
-  std::memset(&C, 0, sizeof(C));
-  C.pts0 = d_points; C.n0 = d_n_points; C.pts_stride = p->cap;
-  C.hints = d_pose_hints;
-  C.origo_x = origo[0]; C.origo_y = origo[1];
-  C.map_without_matching = map_without_matching;
-  C.out = p->d_out;
-  if (p->P.exact) k_hs_match<true><<<B, HS_THREADS, hs_smem_bytes(p->cap), p->stream>>>(p->P, C);
-  else k_hs_match<false><<<B, HS_THREADS, hs_smem_bytes(p->cap), p->stream>>>(p->P, C);
-  const dim3 grid(std::max(1, std::min(ceil_div(std::max(max_n, 1) * p->levels, 8), sm_count(p->device) * 8 / std::max(1, std::min(B, 8)))), B);
-  k_hs_mark<<<grid, 256, 0, p->stream>>>(p->P);
-  k_hs_apply<<<grid, 256, 0, p->stream>>>(p->P);
-  B2S_CUDA_CHECK(cudaGetLastError());
-  return B2S_OK;
+  return hs_launch_step(p, d_points, d_n_points, max_n, origo, d_pose_hints, map_without_matching);
 }
 
 b2s_status b2s_hector_slam_sync(b2s_hector_slam *p) {

@@ -60,13 +60,13 @@ b2s_status b2s_ros_hector_points(const float *pts, int n, const float laser_in_b
                                  float max_dist, double use_max_scan_range, float z_min, float z_max, float *out_points,
                                  float out_origo[2], int32_t *out_n) {
   if (!laser_in_base || !out_origo || !out_n || n < 0 || (n > 0 && (!pts || !out_points))) B2S_FAIL(B2S_ERR_BAD_PARAMS, "null argument");
-  const HectorScanFilter f = hector_scan_filter(laser_in_base, scale_to_map, min_dist, max_dist, use_max_scan_range, z_min, z_max);
-  out_origo[0] = (float)f.lx * scale_to_map;  // Eigen::Vector2f(laserPos.x(), laserPos.y()) * scaleToMap
-  out_origo[1] = (float)f.ly * scale_to_map;
+  const HectorBeamFilter f = hector_scan_filter(laser_in_base, scale_to_map, min_dist, max_dist, use_max_scan_range, z_min, z_max);
+  out_origo[0] = (float)f.mount.o[0] * scale_to_map;  // Eigen::Vector2f(laserPos.x(), laserPos.y()) * scaleToMap
+  out_origo[1] = (float)f.mount.o[1] * scale_to_map;
   int k = 0;
   for (int i = 0; i < n; i++) {
     float x, y;
-    if (!hector_filter_point(f, pts[3 * i], pts[3 * i + 1], pts[3 * i + 2], x, y)) continue;
+    if (!hector_node_filter_point(f, pts[3 * i], pts[3 * i + 1], pts[3 * i + 2], x, y)) continue;
     out_points[2 * k] = x;
     out_points[2 * k + 1] = y;
     k++;
@@ -83,20 +83,20 @@ b2s_status b2s_ros_hector_scans(const b2s_laser_scan_msg *geometry, const b2s_he
   const int n = geometry->n_ranges;
   if (n_scans > 0 && n > 0 && (!ranges || !out_points)) B2S_FAIL(B2S_ERR_BAD_PARAMS, "null argument");
   const b2s_hector_scan_filter &q = *filter;
-  const HectorScanFilter f = hector_scan_filter(q.laser_in_base, scale_to_map, q.min_dist, q.max_dist, q.use_max_scan_range,
+  const HectorBeamFilter f = hector_scan_filter(q.laser_in_base, scale_to_map, q.min_dist, q.max_dist, q.use_max_scan_range,
                                                 q.z_min, q.z_max);
   const double cutoff = hector_range_cutoff(q.range_cutoff, geometry->range_max);
   std::vector<double> unit(2 * (size_t)n);
   hector_unit_vectors(geometry->angle_min, geometry->angle_increment, n, unit.data());
-  out_origo[0] = (float)f.lx * scale_to_map;
-  out_origo[1] = (float)f.ly * scale_to_map;
+  out_origo[0] = (float)f.mount.o[0] * scale_to_map;
+  out_origo[1] = (float)f.mount.o[1] * scale_to_map;
   size_t k = 0;
   for (int s = 0; s < n_scans; s++) {
     const float *r = ranges + (size_t)s * n;
     const size_t k0 = k;
     for (int i = 0; i < n; i++) {
       float x, y;
-      if (!hector_scan_beam(f, r[i], unit[2 * i], unit[2 * i + 1], cutoff, geometry->range_min, x, y)) continue;
+      if (!hector_node_beam(f, r[i], unit[2 * i], unit[2 * i + 1], cutoff, geometry->range_min, x, y)) continue;
       out_points[2 * k] = x;
       out_points[2 * k + 1] = y;
       k++;

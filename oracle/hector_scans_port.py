@@ -59,9 +59,12 @@ def to_data_container(pts_xyz, laser_in_base=(0, 0, 0, 0), scale_to_map=20.0, mi
                 continue
             if float(d) > use * use:
                 continue
-            bx = c * float(x) - s * float(y) + lx
-            by = s * float(x) + c * float(y) + ly
-            zl = f32((float(z) + lz) - lz)
+            # laserTransform * Vector3(x, y, z) in tf's order, on the basis rows (c, -s, -0.0), (s, c, -0.0), (0, 0, 1)
+            # that the library builds from the yaw: -0.0, not +0.0, in the third column
+            xd, yd, zd = float(x), float(y), float(z)
+            bx = (xd * c + yd * -s + zd * -0.0) + lx
+            by = (xd * s + yd * c + zd * -0.0) + ly
+            zl = f32(((xd * 0.0 + yd * 0.0 + zd * 1.0) + lz) - lz)
             if zl > zmin and zl < zmax:
                 out.append((f32(bx) * scale, f32(by) * scale))
         origo = np.array([f32(lx) * scale, f32(ly) * scale], np.float32)

@@ -148,6 +148,17 @@ def test_projection_then_existing_filter_equals_adapter(pkg):
         assert np.array_equal(got.view(np.int32), pts[k:k + cnt[s]].view(np.int32))
         assert np.array_equal(o.view(np.int32), origo.view(np.int32))
         k += cnt[s]
+    # caller points with z < 0 or z = -0.0 under a mount at x = y = -0.0: where the rotated sum is exactly -0, tf's
+    # z * -0.0 term of the basis makes the coordinate +0.0 (rows 0 and 1), and -0.0 for z > 0 (row 2)
+    corner = np.array([[-1.0, -0.0, -0.25], [-0.0, 1.0, -0.0], [-1.0, -0.0, 0.25], [-0.0, 1.0, 0.0]], np.float32)
+    for lb in ((-0.0, -0.0, 0.3, 0.0), (0.2, -0.1, 0.3, 0.4)):
+        got, o = R.hector_points(corner, laser_in_base=lb, scale_to_map=20.0)
+        want, wo = O.to_data_container(corner, lb, 20.0)
+        assert len(got) == 4
+        assert np.array_equal(got.view(np.int32), want.view(np.int32))
+        assert np.array_equal(o.view(np.int32), wo.view(np.int32))
+        if lb[0] == 0.0:
+            assert list(np.signbit([got[0, 1], got[1, 0], got[2, 1]])) == [False, False, True]
 
 
 def test_node_defaults_and_bad_arguments(pkg):

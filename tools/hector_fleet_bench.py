@@ -87,7 +87,7 @@ class Packed:
         return self.poses.reshape(self.B, self.n, 3).copy(), self.upd.reshape(self.B, self.n).astype(bool)
 
     def h2d_bytes(self):
-        return int(self.cat.nbytes + self.cnt.nbytes + 8 * len(self.cnt) + 8 * (self.B + 1) + self.firsts.nbytes)
+        return int(self.cat.nbytes + self.cnt.nbytes + 8 * len(self.cnt) + 16 * self.B + self.firsts.nbytes)
 
     def d2h_bytes(self):
         return 64 * len(self.cnt)

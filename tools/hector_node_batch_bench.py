@@ -96,7 +96,7 @@ def main():
                              sequential_s=round(seq, 3), sequential_scans_per_s=round(total / seq),
                              speedup=round(seq / s, 2)))
     print(json.dumps(dict(scans_per_node=a.scans, beams=laser.n_readings, map="2048x2048, 3 levels", runs=rows,
-                          kernel="k_hs_stream_node (one CTA per node, exact mode)", card=card())))
+                          kernel="k_hs_stream_batch<true, true> (one CTA per node, exact mode)", card=card())))
 
 
 if __name__ == "__main__":

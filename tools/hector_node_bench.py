@@ -130,7 +130,7 @@ def main():
         publish_share=round(1.0 - quiet / ms, 3), ms_one_publish=round(quiet, 1),
         route_parts_ms=round(route, 1), route_parts_scans_per_s=round(a.scans / route * 1e3), route_maps=len(cuts),
         route_per_scan_scans=k, route_per_scan_ms=round(per_scan, 1), route_per_scan_scans_per_s=round(k / per_scan * 1e3),
-        kernel="k_hs_stream_node (one CTA, exact mode)", card=card())))
+        kernel="k_hs_stream_batch<true, true> (one CTA, exact mode)", card=card())))
 
 
 if __name__ == "__main__":

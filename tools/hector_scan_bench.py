@@ -66,7 +66,8 @@ def recording(job):
 
 
 def kernel_ms(fn):
-    """device time of k_hs_stream_batch while fn runs, from torch.profiler (CUDA activities)"""
+    """device time of k_hs_stream_batch while fn runs, from torch.profiler (CUDA activities): each arm runs one of its
+    instantiations, <_, false> for (a) and <_, true> for (b)"""
     import torch
     from torch.profiler import ProfilerActivity, profile
     with profile(activities=[ProfilerActivity.CUDA, ProfilerActivity.CPU]) as prof:
@@ -144,11 +145,11 @@ class Fleet:
     def result(self):
         return self.poses.copy(), self.upd.copy(), self.covs.copy()
 
-    def h2d_host_arm(self):  # points, counts, 64-bit offsets, first[B + 1], first hints
-        return int(8 * int(self.cnt.sum()) + 4 * len(self.cnt) + 8 * len(self.cnt) + 8 * (self.B + 1) + self.firsts.nbytes)
+    def h2d_host_arm(self):  # points, counts, 64-bit offsets, first[B][2], first hints
+        return int(8 * int(self.cnt.sum()) + 4 * len(self.cnt) + 8 * len(self.cnt) + 16 * self.B + self.firsts.nbytes)
 
-    def h2d_device_arm(self):  # ranges, unit vectors, the ingest descriptor, first[B + 1], first hints
-        return int(self.ranges.nbytes + 16 * self.nr + 104 + 8 * (self.B + 1) + self.firsts.nbytes)
+    def h2d_device_arm(self):  # ranges, unit vectors, the ingest descriptor, B filters and origos, first[B][2], first hints
+        return int(self.ranges.nbytes + 16 * self.nr + 40 + (128 + 8) * self.B + 16 * self.B + self.firsts.nbytes)
 
 
 def run(H, R, ranges, firsts, exact, repeats):
