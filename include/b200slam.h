@@ -1104,6 +1104,60 @@ b2s_status b2s_lidar_undistortion_node(int use_imu, int use_odom, float angle_mi
                                        const b2s_imu_msg *imu, int n_odom, const b2s_odom_msg *odom, int32_t *out_status,
                                        b2s_deskew_scan *out_state, float *out_xyz, int device, void *cuda_stream);
 
+/* B LidarUndistortion nodes behind one handle, one laser per recording, fed in parts: each call hands every recording
+ * its next LaserScans and the IMU and odometry messages delivered with them, and the handle keeps each node's state
+ * across calls.  All recordings' published scans run in ONE launch (one CTA per scan, grid x up to 2^31 - 1).
+ * b2s_lidar_undistortion_node is this handle's path for one fresh recording, its rows shifted to the corrected scan. */
+#define B2S_DESKEW_CACHED 7     /* handle rows only: the callback of the node's first scan (ever or since reset) only
+                                   cached that scan */
+
+typedef struct b2s_deskew_node b2s_deskew_node; /* opaque: B LidarUndistortion nodes */
+typedef struct b2s_deskew_laser {               /* what the node takes from its first scan */
+  float angle_min, angle_increment;             /* CreateAngleCache's float fields */
+  int32_t n_beams;                              /* scan_count_ */
+  int32_t use_imu, use_odom;                    /* use_imu_ / use_odom_ */
+  int32_t reserved;                             /* 0 */
+} b2s_deskew_laser;
+
+/* lasers [batch].  B2S_ERR_BAD_PARAMS, before the device is touched, for batch < 1, n_beams < 1 or NULL pointers;
+ * B2S_ERR_NO_DEVICE without a device.  cuda_stream NULL: the handle makes its own. */
+b2s_status b2s_deskew_node_create(int batch, const b2s_deskew_laser *lasers, int device, void *cuda_stream,
+                                  b2s_deskew_node **out);
+void b2s_deskew_node_destroy(b2s_deskew_node *h);
+/* a fresh node for one recording, or for all with recording = -1: its next scan is cached as the first.
+ * B2S_ERR_BAD_PARAMS for a recording outside [-1, batch). */
+b2s_status b2s_deskew_node_reset(b2s_deskew_node *h, int recording);
+/* The callbacks of every recording's next n_scans[b] LaserScans (0 leaves recording b's scans as they are; its new
+ * messages still join its queues).
+ *
+ * Layout: arrays are recording-major and ragged.  scans, out_status and out_state have sum n_scans rows.  ranges holds
+ * n_scans[0] rows of n_beams[0] floats, then n_scans[1] rows of n_beams[1] floats, and so on; out_xyz has the same
+ * shape with 3 floats per beam.  imu has sum n_imu messages and odom sum n_odom, each recording's in delivery order.
+ *
+ * Arrival counts: a scan's imu_arrived / odom_arrived count its recording's messages OF THIS CALL delivered before its
+ * callback; they do not decrease and do not exceed that recording's count.  Messages after the last scan's count are
+ * delivered before the next call's first scan.  Messages of a recording whose flag is off are ignored.
+ *
+ * Rows are callback-indexed: row k of a recording in a call is what the callback of that call's k-th scan did.  It
+ * corrected the scan handed in just before it (for k = 0, the previous call's last scan), with the statuses, states
+ * and clouds of b2s_lidar_undistortion_node; or, for the node's first scan ever or since reset, it only cached the
+ * scan: B2S_DESKEW_CACHED, with zero state and cloud bytes.  B2S_DESKEW_HELD is never returned: the held scan stays in
+ * the handle.  Over a whole recording, rows 1 .. S - 1 therefore equal b2s_lidar_undistortion_node's rows 0 .. S - 2
+ * byte for byte, however the recording is cut into calls.  out_state may be NULL.
+ *
+ * State kept per recording: the first-scan flag; the held scan's stamp and float fields, its ranges on the device; the
+ * IMU and odometry queues, as copies of the messages not yet pruned (they grow as the node's deques do while a scan
+ * waits); start_odom_msg_ and end_odom_msg_.
+ *
+ * B2S_ERR_BAD_PARAMS, before anything is enqueued or written and with every recording's state unchanged, for NULL
+ * arrays where a count is non-zero (n_scans, n_imu and n_odom are always needed), negative counts, arrival counts that
+ * decrease or exceed their log, or a NULL log whose flag is on for some recording.  A device error marks the handle
+ * failed: later calls answer B2S_ERR_BAD_STATE.  Returns when the clouds are on the host. */
+b2s_status b2s_deskew_node_process(b2s_deskew_node *h, const int32_t *n_scans, const b2s_deskew_node_scan *scans,
+                                   const float *ranges, const int32_t *n_imu, const b2s_imu_msg *imu, const int32_t *n_odom,
+                                   const b2s_odom_msg *odom, int32_t *out_status, b2s_deskew_scan *out_state,
+                                   float *out_xyz);
+
 /* ---------------------------------------------------------------- lesson1: corner-feature extraction
  * LaserScan::ScanCallback (lesson1/src/feature_detection.cc:77-179): the finite readings of a scan, a curvature
  * c = d * d from an 11-reading stencil (:112-124), and in each of six sectors the first 20 entries above edge_threshold
