@@ -1,39 +1,23 @@
-"""TEST INFRASTRUCTURE — ctypes binding of oracle/libfeature_oracle.so, the C++ CPU restatement of lesson1's corner
-picker (feature_oracle.cpp, LaserScan::ScanCallback, feature_detection.cc:77-179).  It is a library of its own, built from
-one C++ file without FMA contraction, like the reference's catkin build.  Only tests/, __graft_entry__ and tools/ may
-import this module; the product never does.
+"""TEST INFRASTRUCTURE — ctypes binding of oracle/libfeature_oracle.so, the C++ CPU restatement of lesson1's corner picker
+(feature_oracle.cpp, LaserScan::ScanCallback, feature_detection.cc:77-179).  It is a library of its own, built from one
+C++ file by oracle/recipes.py.  Only tests/, __graft_entry__ and tools/ may import this module; the product never does.
 """
 from __future__ import annotations
 
 import ctypes as C
-import os
-import subprocess
 
 import numpy as np
 
-_HERE = os.path.dirname(os.path.abspath(__file__))
-_SRC = os.path.join(_HERE, "feature_oracle.cpp")
-_SORT = os.path.join(os.path.dirname(_HERE), "creating-2d-laser-slam-from-scratch_b200", "csrc", "introsort.cuh")
-_LIB = os.path.join(_HERE, "libfeature_oracle.so")
-CXXFLAGS = ["-std=c++17", "-O2", "-fPIC", "-ffp-contract=off", "-Wall", "-Wextra"]
+from oracle import recipes
+
 MAX_BEAMS = 1500
 _lib = None
-
-
-def build(force: bool = False) -> str:
-    deps = [_SRC, _SORT, os.path.abspath(__file__)]
-    if force or not os.path.exists(_LIB) or any(os.path.getmtime(d) > os.path.getmtime(_LIB) for d in deps):
-        tmp = _LIB + f".{os.getpid()}.tmp"
-        subprocess.check_call([os.environ.get("CXX", "g++")] + CXXFLAGS + ["-shared", _SRC, "-o", tmp])
-        os.replace(tmp, _LIB)  # atomic: a concurrent reader sees the old library or the new one
-    return _LIB
 
 
 def lib():
     global _lib
     if _lib is None:
-        build()
-        L = C.CDLL(_LIB)
+        L = C.CDLL(recipes.build("libfeature_oracle.so"))
         fp = C.POINTER(C.c_float)
         L.orc_feature_detect.argtypes = [C.c_int, fp, C.c_float, fp, fp, C.POINTER(C.c_int32)]
         L.orc_feature_detect.restype = C.c_int

@@ -7,7 +7,7 @@
  * It exists so the CUDA path can be checked on the GPU box, where the reference checkout is absent.
  *
  * PARITY PINNED: tests/test_oracle_vs_reference.py checks every function here against the
- * UNMODIFIED reference compiled by `make -C oracle ref` (oracle/_ref/libkarto_ref.so), bit-exact
+ * UNMODIFIED reference compiled by oracle/recipes.py (oracle/_ref/libkarto_ref.so), bit-exact
  * on grid bytes / lookup tables / integer response sums / counters and to 1e-12 on doubles, and
  * tests/golden/ holds vectors produced by that reference build (tests/golden/make_golden.py).
  *

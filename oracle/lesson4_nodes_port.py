@@ -1,43 +1,27 @@
-"""TEST INFRASTRUCTURE — ctypes binding of oracle/liblesson4_nodes_oracle.so: the plain-C CPU restatement of lesson4's
-two make-map nodes (lesson4_nodes_oracle.c) together with the GMapping and Hector map restatements it calls
-(gmapping_oracle.c, hector_oracle.c), a library of its own built with the flags of oracle/Makefile.  Only tests/,
-__graft_entry__ and tools/ may import this module; the product never does.
+"""TEST INFRASTRUCTURE — ctypes binding of oracle/liblesson4_nodes_oracle.so: the plain-C CPU restatement of lesson4's two
+make-map nodes (lesson4_nodes_oracle.c) together with the GMapping and Hector map restatements it calls
+(gmapping_oracle.c, hector_oracle.c), a library of its own built by oracle/recipes.py.  Only tests/, __graft_entry__ and
+tools/ may import this module; the product never does.
 """
 from __future__ import annotations
 
 import ctypes as C
 import importlib
-import os
-import subprocess
 
 import numpy as np
 
+from oracle import recipes
+
 node_maps = importlib.import_module("creating-2d-laser-slam-from-scratch_b200.node_maps")
 
-_HERE = os.path.dirname(os.path.abspath(__file__))
-_SRC = [os.path.join(_HERE, f) for f in ("lesson4_nodes_oracle.c", "gmapping_oracle.c", "hector_oracle.c")]
-_HDR = os.path.join(os.path.dirname(_HERE), "include", "b200slam.h")
-_LIB = os.path.join(_HERE, "liblesson4_nodes_oracle.so")
-# the flags of oracle/Makefile: x86-64 baseline, no FMA contraction
-CFLAGS = ["-O2", "-fPIC", "-std=c11", "-ffp-contract=off", "-Wall", "-Wextra"]
 SENTINEL = 0x55  # an overrun byte the node does not write
 _lib = None
-
-
-def build(force: bool = False) -> str:
-    deps = _SRC + [_HDR, os.path.abspath(__file__)]
-    if force or not os.path.exists(_LIB) or any(os.path.getmtime(d) > os.path.getmtime(_LIB) for d in deps):
-        tmp = _LIB + f".{os.getpid()}.tmp"
-        subprocess.check_call([os.environ.get("CC", "gcc")] + CFLAGS + ["-shared"] + _SRC + ["-o", tmp, "-lm"])
-        os.replace(tmp, _LIB)  # atomic: a concurrent reader sees the old library or the new one
-    return _LIB
 
 
 def lib():
     global _lib
     if _lib is None:
-        build()
-        L = C.CDLL(_LIB)
+        L = C.CDLL(recipes.build("liblesson4_nodes_oracle.so"))
         vp = C.c_void_p
         L.orc_gmapping_node_dims.argtypes = [vp, vp]
         L.orc_gmapping_node_maps.argtypes = [vp, vp, C.c_int, vp, vp, vp, C.c_int, vp]

@@ -1,42 +1,26 @@
 """TEST INFRASTRUCTURE — ctypes binding of oracle/libpcl_icp_oracle.so, the plain-C CPU restatement of lesson2's ICP
-scan matching (pcl_icp_oracle.c, PARITY UNPINNED).  It is a library of its own, built from one C file with the flags of
-oracle/Makefile, so that the restatement of lesson2 needs nothing from the other restatements.  Only tests/,
+scan matching (pcl_icp_oracle.c, PARITY UNPINNED).  It is a library of its own, built from one C file by
+oracle/recipes.py, so that the restatement of lesson2 needs nothing from the other restatements.  Only tests/,
 __graft_entry__ and tools/ may import this module; the product never does.
 """
 from __future__ import annotations
 
 import ctypes as C
 import importlib
-import os
-import subprocess
 
 import numpy as np
 
+from oracle import recipes
+
 abi = importlib.import_module("creating-2d-laser-slam-from-scratch_b200.abi")
 
-_HERE = os.path.dirname(os.path.abspath(__file__))
-_SRC = os.path.join(_HERE, "pcl_icp_oracle.c")
-_HDR = os.path.join(os.path.dirname(_HERE), "include", "b200slam.h")
-_LIB = os.path.join(_HERE, "libpcl_icp_oracle.so")
-# the flags of oracle/Makefile: x86-64 baseline, no FMA contraction
-CFLAGS = ["-O2", "-fPIC", "-std=c11", "-ffp-contract=off", "-Wall", "-Wextra"]
 _lib = None
-
-
-def build(force: bool = False) -> str:
-    deps = [_SRC, _HDR, os.path.abspath(__file__)]
-    if force or not os.path.exists(_LIB) or any(os.path.getmtime(d) > os.path.getmtime(_LIB) for d in deps):
-        tmp = _LIB + f".{os.getpid()}.tmp"
-        subprocess.check_call([os.environ.get("CC", "gcc")] + CFLAGS + ["-shared", _SRC, "-o", tmp, "-lm"])
-        os.replace(tmp, _LIB)  # atomic: a concurrent reader sees the old library or the new one
-    return _LIB
 
 
 def lib():
     global _lib
     if _lib is None:
-        build()
-        L = C.CDLL(_LIB)
+        L = C.CDLL(recipes.build("libpcl_icp_oracle.so"))
         fp = C.POINTER(C.c_float)
         L.orc_pcl_scan_to_cloud.argtypes = [C.c_int, fp, C.c_float, C.c_float, C.c_float, C.c_float, C.c_int, fp]
         L.orc_pcl_scan_to_cloud.restype = C.c_int

@@ -3,7 +3,7 @@
  *
  * CPU restatement of lesson3's odometry node, ScanMatchPLICP (reference/lesson3/src/plicp_odometry.cc:191-517): the
  * node's loop in C around the PL-ICP restatement orc_plicp_match (oracle/plicp_oracle.c).  Built with it into a library
- * of its own (oracle/plicp_odometry_port.py), with the flags of oracle/Makefile.
+ * of its own (oracle/plicp_odometry_port.py), built by oracle/recipes.py.
  */
 #include <math.h>
 #include <stdint.h>

@@ -1,43 +1,26 @@
 """TEST INFRASTRUCTURE — ctypes binding of oracle/libplicp_odometry_oracle.so: the plain-C CPU restatement of lesson3's
 odometry node (plicp_odometry_oracle.c) together with the PL-ICP restatement it calls (plicp_oracle.c), a library of its
-own built with the flags of oracle/Makefile.  Only tests/, __graft_entry__ and tools/ may import this module; the
-product never does.
+own built by oracle/recipes.py.  Only tests/, __graft_entry__ and tools/ may import this module; the product never does.
 """
 from __future__ import annotations
 
 import ctypes as C
 import importlib
-import os
-import subprocess
 
 import numpy as np
+
+from oracle import recipes
 
 abi = importlib.import_module("creating-2d-laser-slam-from-scratch_b200.abi")
 plicp = importlib.import_module("creating-2d-laser-slam-from-scratch_b200.plicp")
 
-_HERE = os.path.dirname(os.path.abspath(__file__))
-_SRC = [os.path.join(_HERE, "plicp_odometry_oracle.c"), os.path.join(_HERE, "plicp_oracle.c")]
-_HDR = os.path.join(os.path.dirname(_HERE), "include", "b200slam.h")
-_LIB = os.path.join(_HERE, "libplicp_odometry_oracle.so")
-# the flags of oracle/Makefile: x86-64 baseline, no FMA contraction
-CFLAGS = ["-O2", "-fPIC", "-std=c11", "-ffp-contract=off", "-Wall", "-Wextra"]
 _lib = None
-
-
-def build(force: bool = False) -> str:
-    deps = _SRC + [_HDR, os.path.join(_HERE, "linear_math.h"), os.path.abspath(__file__)]
-    if force or not os.path.exists(_LIB) or any(os.path.getmtime(d) > os.path.getmtime(_LIB) for d in deps):
-        tmp = _LIB + f".{os.getpid()}.tmp"
-        subprocess.check_call([os.environ.get("CC", "gcc")] + CFLAGS + ["-shared"] + _SRC + ["-o", tmp, "-lm"])
-        os.replace(tmp, _LIB)  # atomic: a concurrent reader sees the old library or the new one
-    return _LIB
 
 
 def lib():
     global _lib
     if _lib is None:
-        build()
-        L = C.CDLL(_LIB)
+        L = C.CDLL(recipes.build("libplicp_odometry_oracle.so"))
         L.orc_plicp_odometry.restype = None
         L.orc_plicp_odometry.argtypes = [C.POINTER(abi.PlicpOdomParams), C.c_int, C.c_float, C.c_float, C.c_float,
                                          C.c_float, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]

@@ -3,7 +3,7 @@
  *
  * CPU restatement of lesson3's scan-to-scan node, ScanMatchPLICP (reference/lesson3/src/scan_match_plicp.cc:162-300):
  * the node's loop in C around the PL-ICP restatement orc_plicp_match (oracle/plicp_oracle.c).  Built with it into a
- * library of its own (oracle/plicp_scan_match_port.py), with the flags of oracle/Makefile.  The unmodified node,
+ * library of its own (oracle/plicp_scan_match_port.py), built by oracle/recipes.py.  The unmodified node,
  * compiled against the stand-ins under oracle/shim/ (oracle/ref_lesson3_scan_match.cpp), pins it bit for bit.
  */
 #include <math.h>

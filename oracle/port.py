@@ -6,31 +6,20 @@ from __future__ import annotations
 
 import ctypes as C
 import importlib
-import os
-import subprocess
 
 import numpy as np
 
+from oracle import recipes
+
 abi = importlib.import_module("creating-2d-laser-slam-from-scratch_b200.abi")
 
-_HERE = os.path.dirname(os.path.abspath(__file__))
-_LIB = os.path.join(_HERE, "libslam_oracle.so")
 _lib = None
-
-
-def build(force: bool = False) -> str:
-    srcs = [os.path.join(_HERE, f) for f in ("karto_oracle.c", "gmapping_oracle.c", "hector_oracle.c", "plicp_oracle.c", "deskew_oracle.c",
-                                             "oracle_common.h", "Makefile")]
-    if force or not os.path.exists(_LIB) or any(os.path.getmtime(s) > os.path.getmtime(_LIB) for s in srcs):
-        subprocess.check_call(["make", "-C", _HERE, "-s", "-B", "libslam_oracle.so"])
-    return _LIB
 
 
 def lib():
     global _lib
     if _lib is None:
-        build()
-        L = C.CDLL(_LIB)
+        L = C.CDLL(recipes.build("libslam_oracle.so"))
         L.orc_round.restype = C.c_double
         L.orc_round.argtypes = [C.c_double]
         L.orc_normalize_angle.restype = C.c_double

@@ -1,15 +1,14 @@
 """TEST INFRASTRUCTURE — ctypes binding of oracle/_ref/libkarto_ref*.so (the UNMODIFIED reference
-open_karto compiled by oracle/Makefile `make ref`).  Only tests/, __graft_entry__.smoke() and
+open_karto compiled by oracle/recipes.py).  Only tests/, __graft_entry__.smoke() and
 bench.py's cpu_baseline / --impl reference legs may import this module.
 """
 from __future__ import annotations
 
 import ctypes as C
-import os
 
 import numpy as np
 
-_HERE = os.path.dirname(os.path.abspath(__file__))
+from oracle import recipes
 
 
 class MatcherParams(C.Structure):
@@ -45,12 +44,12 @@ def laser_params(laser) -> LaserParams:
                        laser.max_range, laser.range_threshold, (C.c_double * 3)(*laser.offset_pose))
 
 
-def lib_path(ndebug: bool = False) -> str:
-    return os.path.join(_HERE, "_ref", "libkarto_ref_ndebug.so" if ndebug else "libkarto_ref.so")
+def _name(ndebug: bool) -> str:
+    return "_ref/libkarto_ref_ndebug.so" if ndebug else "_ref/libkarto_ref.so"
 
 
 def available(ndebug: bool = False) -> bool:
-    return os.path.exists(lib_path(ndebug))
+    return recipes.available(_name(ndebug))
 
 
 _libs = {}
@@ -59,7 +58,7 @@ _libs = {}
 def _lib(ndebug: bool):
     if ndebug in _libs:
         return _libs[ndebug]
-    L = C.CDLL(lib_path(ndebug))
+    L = C.CDLL(recipes.path(_name(ndebug)))
     dp, ip, u8p, u32p = C.POINTER(C.c_double), C.POINTER(C.c_int32), C.POINTER(C.c_uint8), C.POINTER(C.c_uint32)
     L.ref_session_create.restype = C.c_void_p
     L.ref_session_create.argtypes = [C.POINTER(MatcherParams), C.POINTER(LaserParams)]

@@ -8,7 +8,7 @@
 // on synthetic inputs, dump its internal state (correlation grid bytes, lookup
 // tables, integer response sums, pass/hit counters) and time it.  Nothing here
 // restates the algorithm: every number comes out of the reference's own code.
-// Built by oracle/Makefile into oracle/_ref/libkarto_ref.so (git-ignored).
+// Built by oracle/recipes.py into oracle/_ref/libkarto_ref.so (git-ignored).
 //
 // Private members (ScanMatcher::AddScans / GetResponse / m_pGridLookup,
 // OccupancyGrid::m_pCellPassCnt ...) are reached with the usual

@@ -4,7 +4,7 @@
 // (dependency-free; gmapping.cc itself needs ROS).  GMapping::ComputeMap (src/gmapping/gmapping.cc:171-242) is
 // re-assembled here around those headers with the node's ROS message replaced by plain arrays: the Bresenham lines,
 // the PointAccumulator cells, the patch storage and world2map are all the reference's own code.
-// Built by oracle/Makefile into oracle/_ref/libgmapping_ref.so.
+// Built by oracle/recipes.py into oracle/_ref/libgmapping_ref.so.
 #include <cmath>
 #include <cstdint>
 #include <cstring>

@@ -1,23 +1,23 @@
 """TEST INFRASTRUCTURE — ctypes binding of oracle/_ref/libgmapping_ref.so (the reference's real GMapping grid
 headers, see oracle/ref_gmapping.cpp)."""
 import ctypes as C
-import os
 
 import numpy as np
 
-_HERE = os.path.dirname(os.path.abspath(__file__))
-_PATH = os.path.join(_HERE, "_ref", "libgmapping_ref.so")
+from oracle import recipes
+
+_NAME = "_ref/libgmapping_ref.so"
 _lib = None
 
 
 def available():
-    return os.path.exists(_PATH)
+    return recipes.available(_NAME)
 
 
 def lib():
     global _lib
     if _lib is None:
-        L = C.CDLL(_PATH)
+        L = C.CDLL(recipes.path(_NAME))
         L.refg_map_create.restype = C.c_void_p
         L.refg_map_create.argtypes = [C.c_double] * 7
         L.refg_map_destroy.argtypes = [C.c_void_p]

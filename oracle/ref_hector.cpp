@@ -1,7 +1,7 @@
 /*
  * ref_hector.cpp — TEST INFRASTRUCTURE, NOT PRODUCT CODE.
  * extern "C" driver around the UNMODIFIED lesson4 Hector headers, compiled where they lie under
- * reference/lesson4/include (oracle/Makefile target _ref/libhector_ref.so):
+ * reference/lesson4/include (oracle/recipes.py builds _ref/libhector_ref.so):
  *   hectorslam::GridMap  (map/GridMap.h -> OccGridMapBase.h:118-330, GridMapLogOdds.h:37-161, GridMapBase.h)
  *   HUtil (map/OccGridMapUtil.h:77-228)      ScanMatcher (matcher/ScanMatcher.h:60-141)
  *   HectorSlamProcessor  (slam_main/HectorSlamProcessor.h:81-108 -> MapRepMultiMap.h:144-191)

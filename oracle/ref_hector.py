@@ -1,28 +1,28 @@
 """TEST INFRASTRUCTURE — ctypes binding of oracle/_ref/libhector_ref.so: the UNMODIFIED lesson4 Hector headers
-(GridMap, OccGridMapUtil, ScanMatcher, HectorSlamProcessor) compiled by oracle/Makefile against the Eigen stand-in
+(GridMap, OccGridMapUtil, ScanMatcher, HectorSlamProcessor) compiled by oracle/recipes.py against the Eigen stand-in
 oracle/shim/Eigen/mini_eigen.h.  RefHectorMap has the interface of oracle.port.PortHectorMap.  Only tests/,
 __graft_entry__.smoke() and bench.py's cpu_baseline / --impl reference legs may import this module.
 """
 from __future__ import annotations
 
 import ctypes as C
-import os
 
 import numpy as np
 
-_HERE = os.path.dirname(os.path.abspath(__file__))
-_PATH = os.path.join(_HERE, "_ref", "libhector_ref.so")
+from oracle import recipes
+
+_NAME = "_ref/libhector_ref.so"
 _lib = None
 
 
 def available() -> bool:
-    return os.path.exists(_PATH)
+    return recipes.available(_NAME)
 
 
 def lib():
     global _lib
     if _lib is None:
-        L = C.CDLL(_PATH)
+        L = C.CDLL(recipes.path(_NAME))
         L.ref_hmap_create.restype = C.c_void_p
         L.ref_hmap_update_by_scan.restype = C.c_long
         L.ref_hmap_update_by_scan_just_once.restype = C.c_long

@@ -1,7 +1,7 @@
 /*
  * ref_lesson1.cpp — TEST INFRASTRUCTURE, NOT PRODUCT CODE.
  * extern "C" driver around the UNMODIFIED lesson1 node, reference/lesson1/src/feature_detection.cc, #included where it
- * lies (oracle/ref_lesson1.py builds _ref/liblesson1_ref.so).  ROS is absent; oracle/shim/ros/ros.h and
+ * lies (oracle/recipes.py builds _ref/liblesson1_ref.so).  ROS is absent; oracle/shim/ros/ros.h and
  * oracle/shim/sensor_msgs/LaserScan.h stand in for the message types and the node handle.  The node's main() is
  * renamed so the library has none; every line of LaserScan::ScanCallback (:77-179) that runs here is the reference's.
  */

@@ -1,7 +1,7 @@
 /*
  * ref_lesson3.cpp — TEST INFRASTRUCTURE, NOT PRODUCT CODE.
  * extern "C" driver around the UNMODIFIED lesson3 odometry node, reference/lesson3/src/plicp_odometry.cc, #included
- * where it lies (oracle/ref_lesson3.py builds _ref/liblesson3_ref.so).  ROS, tf2 and CSM are absent; the stand-ins under
+ * where it lies (oracle/recipes.py builds _ref/liblesson3_ref.so).  ROS, tf2 and CSM are absent; the stand-ins under
  * oracle/shim/ provide the message types, the node handle and its parameters, ros::Time, tf2's LinearMath, the tf2_ros
  * buffer (answering with the mount the driver sets) and CSM's types with sm_icp answered by orc_plicp_match
  * (oracle/plicp_oracle.c, linked in).  The node's main() is renamed so the library has none; every line of the node's

@@ -1,7 +1,7 @@
 /*
  * ref_lesson3_scan_match.cpp — TEST INFRASTRUCTURE, NOT PRODUCT CODE.
  * extern "C" driver around the UNMODIFIED lesson3 scan-to-scan node, reference/lesson3/src/scan_match_plicp.cc,
- * #included where it lies (oracle/ref_lesson3_scan_match.py builds _ref/liblesson3_scan_match_ref.so; the node's class
+ * #included where it lies (oracle/recipes.py builds _ref/liblesson3_scan_match_ref.so; the node's class
  * has the odometry node's name, so it gets a library of its own).  ROS and CSM are absent; the stand-ins under
  * oracle/shim/ provide the message types, the node handle and its parameters, ros::Time and CSM's types with sm_icp
  * answered by orc_plicp_match (oracle/plicp_oracle.c, linked in).  The node's main() is renamed so the library has

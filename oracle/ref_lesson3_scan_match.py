@@ -1,7 +1,7 @@
 """TEST INFRASTRUCTURE — ctypes binding of oracle/_ref/liblesson3_scan_match_ref.so: the UNMODIFIED lesson3 scan-to-scan
 node, reference/lesson3/src/scan_match_plicp.cc, compiled where it lies against the ROS and CSM stand-ins under
 oracle/shim/ by oracle/ref_lesson3_scan_match.cpp, with sm_icp answered by oracle/plicp_oracle.c.  Its class has the
-odometry node's name (oracle/ref_lesson3.py), so it is a library of its own.  `build(ref)` makes the library from a
+odometry node's name (oracle/ref_lesson3.py), so it is a library of its own, built by oracle/recipes.py from a
 checkout of the original project; where it is absent the tests replay its recorded answers (tests/reference_record.py).
 Only tests/ and __graft_entry__ may import this module.
 """
@@ -10,51 +10,26 @@ from __future__ import annotations
 import ctypes as C
 import importlib
 import os
-import subprocess
 import sys
 
 import numpy as np
 
+from oracle import recipes
+
 _HERE = os.path.dirname(os.path.abspath(__file__))
 _ROOT = os.path.dirname(_HERE)
-_PATH = os.path.join(_HERE, "_ref", "liblesson3_scan_match_ref.so")
-# the flags of oracle/Makefile's builds: x86-64 baseline, no -march, no FMA contraction
-CXXFLAGS = ["-std=c++17", "-O2", "-fPIC", "-w", "-ffp-contract=off"]
-CFLAGS = ["-std=c11", "-O2", "-fPIC", "-w", "-ffp-contract=off"]
-_SHIM = ["ros/ros.h", "sensor_msgs/LaserScan.h", "geometry_msgs/messages.h", "geometry_msgs/TwistStamped.h",
-         "tf2/LinearMath/Transform.h", "tf2/utils.h", "tf2_ros/transform_listener.h", "tf2_ros/transform_broadcaster.h",
-         "csm/csm_all.h"]
+_NAME = "_ref/liblesson3_scan_match_ref.so"
 _lib = None
 
 
-def build(ref: str) -> str:
-    srcs = [os.path.join(ref, "lesson3", "src", "scan_match_plicp.cc"),
-            os.path.join(ref, "lesson3", "include", "lesson3", "scan_match_plicp.h")]
-    drv, orc = os.path.join(_HERE, "ref_lesson3_scan_match.cpp"), os.path.join(_HERE, "plicp_oracle.c")
-    deps = srcs + [drv, orc, os.path.join(_ROOT, "include", "b200slam.h")] + [os.path.join(_HERE, "shim", h) for h in _SHIM]
-    if not os.path.exists(_PATH) or any(os.path.getmtime(d) > os.path.getmtime(_PATH) for d in deps):
-        os.makedirs(os.path.dirname(_PATH), exist_ok=True)
-        tmp = _PATH + f".{os.getpid()}.tmp"
-        obj = tmp + ".o"
-        subprocess.check_call([os.environ.get("CC", "gcc")] + CFLAGS + ["-c", orc, "-o", obj])
-        subprocess.check_call([os.environ.get("CXX", "g++")] + CXXFLAGS +
-                              ["-shared", "-I" + os.path.join(_HERE, "shim"),
-                               "-I" + os.path.abspath(ref),
-                               "-I" + os.path.join(os.path.abspath(ref), "lesson3", "include"), drv, obj, "-o", tmp,
-                               "-lm"])
-        os.remove(obj)
-        os.replace(tmp, _PATH)
-    return _PATH
-
-
 def available() -> bool:
-    return os.path.exists(_PATH)
+    return recipes.available(_NAME)
 
 
 def lib():
     global _lib
     if _lib is None:
-        L = C.CDLL(_PATH)
+        L = C.CDLL(recipes.path(_NAME))
         fp = C.POINTER(C.c_float)
         L.ref_sm_clear_params.argtypes = []
         L.ref_sm_clear_params.restype = None

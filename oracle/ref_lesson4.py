@@ -1,58 +1,31 @@
 """TEST INFRASTRUCTURE — ctypes binding of oracle/_ref/liblesson4_ref.so: lesson4's UNMODIFIED make-map nodes,
 reference/lesson4/src/gmapping/gmapping.cc and reference/lesson4/src/hector_mapping/hector_mapping.cc, compiled where
 they lie against the ROS, message and Eigen stand-ins under oracle/shim/ by
-oracle/ref_lesson4_gmapping.cpp and oracle/ref_lesson4_hector.cpp (two translation units: see the latter).
-`build(ref)` makes the library from a checkout of the original project; where it is absent the tests replay its
+oracle/ref_lesson4_gmapping.cpp and oracle/ref_lesson4_hector.cpp (two translation units: see the latter),
+built by oracle/recipes.py from a checkout of the original project; where it is absent the tests replay its
 recorded answers (tests/reference_record.py).  Only tests/ and __graft_entry__ may import this module.
 """
 from __future__ import annotations
 
 import ctypes as C
-import os
-import subprocess
 
 import numpy as np
 
-_HERE = os.path.dirname(os.path.abspath(__file__))
-_PATH = os.path.join(_HERE, "_ref", "liblesson4_ref.so")
-# the flags of oracle/Makefile's reference builds: x86-64 baseline, no -march, no FMA contraction
-CXXFLAGS = ["-std=c++17", "-O2", "-fPIC", "-w", "-ffp-contract=off"]
-_DRIVERS = ["ref_lesson4_gmapping.cpp", "ref_lesson4_hector.cpp"]
-_SHIM = ["ros/ros.h", "sensor_msgs/LaserScan.h", "nav_msgs/OccupancyGrid.h", "nav_msgs/MapMetaData.h",
-         "geometry_msgs/messages.h", "Eigen/mini_eigen.h"]
+from oracle import recipes
+
+_NAME = "_ref/liblesson4_ref.so"
 SENTINEL = 0x55  # ref_lesson4_gmapping.cpp: a byte behind the map the node did not write
 _lib = None
 
 
-def build(ref: str) -> str:
-    l4 = os.path.join(os.path.abspath(ref), "lesson4")
-    srcs = [os.path.join(l4, "src", "gmapping", "gmapping.cc"), os.path.join(l4, "src", "hector_mapping", "hector_mapping.cc")]
-    deps = srcs + [os.path.join(_HERE, d) for d in _DRIVERS] + [os.path.join(_HERE, "shim", h) for h in _SHIM]
-    if not os.path.exists(_PATH) or any(os.path.getmtime(d) > os.path.getmtime(_PATH) for d in deps):
-        os.makedirs(os.path.dirname(_PATH), exist_ok=True)
-        tmp = _PATH + f".{os.getpid()}.tmp"
-        inc = ["-I" + os.path.join(_HERE, "shim"), "-I" + os.path.abspath(ref),
-               "-I" + os.path.join(l4, "include"), "-I" + os.path.join(l4, "include", "lesson4", "hector_mapping")]
-        objs = []
-        for d in _DRIVERS:
-            obj = f"{tmp}.{d}.o"
-            subprocess.check_call([os.environ.get("CXX", "g++")] + CXXFLAGS + inc + ["-c", os.path.join(_HERE, d), "-o", obj])
-            objs.append(obj)
-        subprocess.check_call([os.environ.get("CXX", "g++"), "-shared"] + objs + ["-o", tmp, "-lm"])
-        for o in objs:
-            os.remove(o)
-        os.replace(tmp, _PATH)
-    return _PATH
-
-
 def available() -> bool:
-    return os.path.exists(_PATH)
+    return recipes.available(_NAME)
 
 
 def lib():
     global _lib
     if _lib is None:
-        L = C.CDLL(_PATH)
+        L = C.CDLL(recipes.path(_NAME))
         vp = C.c_void_p
         L.ref_l4_clear_params.argtypes = []
         L.ref_l4_clear_params.restype = None

@@ -1,7 +1,7 @@
 /*
  * ref_lesson4_gmapping.cpp — TEST INFRASTRUCTURE, NOT PRODUCT CODE.
  * extern "C" driver around the UNMODIFIED lesson4 GMapping make-map node, reference/lesson4/src/gmapping/gmapping.cc,
- * #included where it lies (oracle/ref_lesson4.py builds it into _ref/liblesson4_ref.so).  ROS is absent; the stand-ins
+ * #included where it lies (oracle/recipes.py builds it into _ref/liblesson4_ref.so).  ROS is absent; the stand-ins
  * under oracle/shim/ (the ROS core, LaserScan, OccupancyGrid, MapMetaData with a float32 resolution) provide the message types, the private node handle and its parameters.  The
  * node's main() is renamed so the library has none; every line of ScanCallback that runs here is the reference's.
  *

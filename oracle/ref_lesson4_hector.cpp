@@ -1,7 +1,7 @@
 /*
  * ref_lesson4_hector.cpp — TEST INFRASTRUCTURE, NOT PRODUCT CODE.
  * extern "C" driver around the UNMODIFIED lesson4 Hector make-map node, reference/lesson4/src/hector_mapping/
- * hector_mapping.cc, #included where it lies (oracle/ref_lesson4.py builds it into _ref/liblesson4_ref.so).  ROS and
+ * hector_mapping.cc, #included where it lies (oracle/recipes.py builds it into _ref/liblesson4_ref.so).  ROS and
  * Eigen are absent; the stand-ins under oracle/shim/ (the ROS core, LaserScan, OccupancyGrid, MapMetaData, the Eigen
  * stand-in) provide the message types, the private node handle and its
  * parameters and the fixed-size Eigen types.  The node's main() is renamed so the library has none; every line of

@@ -1,7 +1,7 @@
 /*
  * ref_lesson4_slam.cpp — TEST INFRASTRUCTURE, NOT PRODUCT CODE.
  * extern "C" driver around lesson4's UNMODIFIED Hector SLAM node, reference/lesson4/src/hector_mapping/hector_slam.cc,
- * #included where it lies (oracle/ref_lesson4_slam.py builds _ref/liblesson4_slam_ref.so).  ROS, tf, laser_geometry and
+ * #included where it lies (oracle/recipes.py builds _ref/liblesson4_slam_ref.so).  ROS, tf, laser_geometry and
  * Boost are absent.  The stand-ins are, first on the include path, oracle/shim_lesson4_slam/ (laser_geometry's
  * projection, PoseStamped / PoseWithCovarianceStamped, tf's poseMsgToTF, lookupTransform and a broadcaster hook,
  * boost::lexical_cast and mutex), then oracle/shim_lesson6/ (tf's listener and types, Boost's bind / mutex / thread) and

@@ -1,57 +1,29 @@
 """TEST INFRASTRUCTURE — ctypes binding of oracle/_ref/liblesson4_slam_ref.so: lesson4's UNMODIFIED Hector SLAM node,
 reference/lesson4/src/hector_mapping/hector_slam.cc, compiled where it lies against the stand-ins under
 oracle/shim_lesson4_slam/, oracle/shim_lesson6/ and oracle/shim/ by oracle/ref_lesson4_slam.cpp (its own translation
-unit).  `build(ref)` makes the library from a checkout of the original project; where it is absent the tests replay its
+unit), built by oracle/recipes.py from a checkout of the original project; where it is absent the tests replay its
 recorded answers (tests/reference_record.py).  Only tests/ and __graft_entry__ may import this module.
 """
 from __future__ import annotations
 
 import ctypes as C
-import os
-import subprocess
 
 import numpy as np
 
-_HERE = os.path.dirname(os.path.abspath(__file__))
-_PATH = os.path.join(_HERE, "_ref", "liblesson4_slam_ref.so")
-# the flags of oracle/Makefile's reference builds: x86-64 baseline, no -march, no FMA contraction
-CXXFLAGS = ["-std=c++17", "-O2", "-fPIC", "-w", "-ffp-contract=off"]
-_SHIM_DIRS = ("shim_lesson4_slam", "shim_lesson6", "shim")
+from oracle import recipes
+
+_NAME = "_ref/liblesson4_slam_ref.so"
 _lib = None
 
 
-def _shim_files():
-    out = []
-    for d in _SHIM_DIRS:
-        for root, _, files in os.walk(os.path.join(_HERE, d)):
-            out += [os.path.join(root, f) for f in files]
-    return out
-
-
-def build(ref: str) -> str:
-    ref = os.path.abspath(ref)
-    l4 = os.path.join(ref, "lesson4")
-    src = os.path.join(l4, "src", "hector_mapping", "hector_slam.cc")
-    drv = os.path.join(_HERE, "ref_lesson4_slam.cpp")
-    deps = [src, drv] + _shim_files()
-    if not os.path.exists(_PATH) or any(os.path.getmtime(d) > os.path.getmtime(_PATH) for d in deps):
-        os.makedirs(os.path.dirname(_PATH), exist_ok=True)
-        tmp = _PATH + f".{os.getpid()}.tmp"
-        inc = ["-I" + os.path.join(_HERE, d) for d in _SHIM_DIRS] + \
-              ["-I" + ref, "-I" + os.path.join(l4, "include"), "-I" + os.path.join(l4, "include", "lesson4", "hector_mapping")]
-        subprocess.check_call([os.environ.get("CXX", "g++")] + CXXFLAGS + inc + ["-shared", drv, "-o", tmp, "-lm"])
-        os.replace(tmp, _PATH)
-    return _PATH
-
-
 def available() -> bool:
-    return os.path.exists(_PATH)
+    return recipes.available(_NAME)
 
 
 def lib():
     global _lib
     if _lib is None:
-        L = C.CDLL(_PATH)
+        L = C.CDLL(recipes.path(_NAME))
         vp = C.c_void_p
         L.ref_l4s_clear_params.argtypes = []
         L.ref_l4s_clear_params.restype = None

@@ -1,7 +1,7 @@
 /*
  * ref_lesson5.cpp — TEST INFRASTRUCTURE, NOT PRODUCT CODE.
  * extern "C" driver around the UNMODIFIED lesson5 node, reference/lesson5/src/lidar_undistortion.cc, #included where it
- * lies (oracle/ref_lesson5.py builds _ref/liblesson5_ref.so).  ROS, tf, PCL and Eigen are absent; the stand-ins under
+ * lies (oracle/recipes.py builds _ref/liblesson5_ref.so).  ROS, tf, PCL and Eigen are absent; the stand-ins under
  * oracle/shim/ provide the message types, the node handle, tf's getRPY, pcl::getTransformation and Eigen's Affine3f.
  * The node's main() is renamed so the library has none; every line of the node's callbacks that runs here is the
  * reference's.  Messages go in through the public callbacks (ImuCallback, OdomCallback, ScanCallback); the published

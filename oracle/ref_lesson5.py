@@ -1,53 +1,30 @@
 """TEST INFRASTRUCTURE — ctypes binding of oracle/_ref/liblesson5_ref.so: the UNMODIFIED lesson5 node,
 reference/lesson5/src/lidar_undistortion.cc, compiled where it lies against the ROS, tf, PCL and Eigen stand-ins under
-oracle/shim/ by oracle/ref_lesson5.cpp.  `build(ref)` makes the library from a checkout of the original project; where it
+oracle/shim/ by oracle/ref_lesson5.cpp, built by oracle/recipes.py from a checkout of the original project; where it
 is absent the tests replay its recorded answers (tests/reference_record.py).  Only tests/ and __graft_entry__ may import
 this module.
 """
 from __future__ import annotations
 
 import ctypes as C
-import os
-import subprocess
 
 import numpy as np
 
-_HERE = os.path.dirname(os.path.abspath(__file__))
-_PATH = os.path.join(_HERE, "_ref", "liblesson5_ref.so")
-# the flags of oracle/Makefile's reference builds: x86-64 baseline, no -march, no FMA contraction
-CXXFLAGS = ["-std=c++17", "-O2", "-fPIC", "-w", "-ffp-contract=off"]
+from oracle import recipes
+
+_NAME = "_ref/liblesson5_ref.so"
 QUEUE_LENGTH = 2000  # the node's imu table length (lidar_undistortion.cc:20)
-_SHIM = ["ros/ros.h", "sensor_msgs/LaserScan.h", "sensor_msgs/Imu.h", "sensor_msgs/PointCloud2.h", "nav_msgs/Odometry.h",
-         "geometry_msgs/messages.h", "tf2/LinearMath/Transform.h", "tf/LinearMath/Quaternion.h", "tf/LinearMath/Matrix3x3.h",
-         "tf/transform_datatypes.h",
-         "pcl/point_types.h", "pcl/point_cloud.h", "pcl/common/common.h", "pcl/common/transforms.h",
-         "pcl_ros/point_cloud.h", "pcl_conversions/pcl_conversions.h", "Eigen/mini_eigen.h"]
 _lib = None
 
 
-def build(ref: str) -> str:
-    srcs = [os.path.join(ref, "lesson5", "src", "lidar_undistortion.cc"),
-            os.path.join(ref, "lesson5", "include", "lesson5", "lidar_undistortion.h")]
-    drv = os.path.join(_HERE, "ref_lesson5.cpp")
-    shim = [os.path.join(_HERE, "shim", h) for h in _SHIM]
-    if not os.path.exists(_PATH) or any(os.path.getmtime(d) > os.path.getmtime(_PATH) for d in srcs + [drv] + shim):
-        os.makedirs(os.path.dirname(_PATH), exist_ok=True)
-        tmp = _PATH + f".{os.getpid()}.tmp"
-        subprocess.check_call([os.environ.get("CXX", "g++")] + CXXFLAGS +
-                              ["-shared", "-I" + os.path.join(_HERE, "shim"), "-I" + os.path.abspath(ref),
-                               "-I" + os.path.join(os.path.abspath(ref), "lesson5", "include"), drv, "-o", tmp])
-        os.replace(tmp, _PATH)
-    return _PATH
-
-
 def available() -> bool:
-    return os.path.exists(_PATH)
+    return recipes.available(_NAME)
 
 
 def lib():
     global _lib
     if _lib is None:
-        L = C.CDLL(_PATH)
+        L = C.CDLL(recipes.path(_NAME))
         u32, dp, fp = C.c_uint32, C.POINTER(C.c_double), C.POINTER(C.c_float)
         L.ref_deskew_new.argtypes = [C.c_int, C.c_int]
         L.ref_deskew_new.restype = None

@@ -1,7 +1,7 @@
 /*
  * ref_lesson6.cpp — TEST INFRASTRUCTURE, NOT PRODUCT CODE.
  * extern "C" driver around the UNMODIFIED lesson6 node, reference/lesson6/src/karto_slam.cc, #included where it lies,
- * linked with the unmodified open_karto Karto.cpp / Mapper.cpp (oracle/ref_lesson6.py builds _ref/liblesson6_ref.so).
+ * linked with the unmodified open_karto Karto.cpp / Mapper.cpp (oracle/recipes.py builds _ref/liblesson6_ref.so).
  * ROS, tf and Boost threads are absent; the stand-ins under oracle/shim_lesson6/ (first on the include path: Boost,
  * message_filters, tf's listener and Stamped, the message types only this node uses) and oracle/shim/ provide the node handle and its parameters, ros::Time / Duration, the publishers (a hook per message
  * type), tf's LinearMath, a listener answering from the mount and the odometry the driver sets, and Boost's bind,

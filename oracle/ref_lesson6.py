@@ -1,7 +1,7 @@
 """TEST INFRASTRUCTURE — ctypes binding of oracle/_ref/liblesson6_ref.so: the UNMODIFIED lesson6 Karto SLAM node,
 reference/lesson6/src/karto_slam.cc, compiled where it lies with the unmodified open_karto Karto.cpp / Mapper.cpp against
-the ROS, tf and Boost stand-ins under oracle/shim_lesson6/ and oracle/shim/ by oracle/ref_lesson6.cpp.  `build(ref)` makes
-the library from a checkout of the original project; where it is absent the tests replay its recorded answers
+the ROS, tf and Boost stand-ins under oracle/shim_lesson6/ and oracle/shim/ by oracle/ref_lesson6.cpp, built by
+oracle/recipes.py from a checkout of the original project; where it is absent the tests replay its recorded answers
 (tests/reference_record.py).  Only tests/ and __graft_entry__ may import this module.
 """
 from __future__ import annotations
@@ -9,55 +9,27 @@ from __future__ import annotations
 import ctypes as C
 import importlib
 import os
-import subprocess
 import sys
 
 import numpy as np
 
+from oracle import recipes
+
 _HERE = os.path.dirname(os.path.abspath(__file__))
 _ROOT = os.path.dirname(_HERE)
-_PATH = os.path.join(_HERE, "_ref", "liblesson6_ref.so")
-# the flags of the other reference builds: x86-64 baseline, no -march, no FMA contraction
-CXXFLAGS = ["-std=c++17", "-O2", "-fPIC", "-w", "-ffp-contract=off"]
-_SHIM6 = ["boost/thread.hpp", "message_filters/subscriber.h", "tf/tf_core.h",
-          "tf/transform_listener.h", "tf/transform_broadcaster.h", "tf/message_filter.h", "visualization_msgs/MarkerArray.h",
-          "nav_msgs/GetMap.h"]
-_SHIM = ["ros/ros.h", "ros/console.h", "boost/thread.hpp", "tf2/LinearMath/Transform.h", "tf/LinearMath/Quaternion.h",
-         "tf/LinearMath/Matrix3x3.h", "sensor_msgs/LaserScan.h", "nav_msgs/OccupancyGrid.h",
-         "nav_msgs/MapMetaData.h", "geometry_msgs/messages.h"]
+_NAME = "_ref/liblesson6_ref.so"
 MAP_FN = C.CFUNCTYPE(None, C.c_void_p, C.c_int32, C.c_int32, C.c_float, C.c_double, C.c_double, C.POINTER(C.c_int8))
 _lib = None
 
 
-def build(ref: str) -> str:
-    ref = os.path.abspath(ref)
-    karto = os.path.join(ref, "lesson6", "lib", "open_karto")
-    srcs = [os.path.join(ref, "lesson6", "src", "karto_slam.cc"), os.path.join(ref, "lesson6", "include", "lesson6", "karto_slam.h"),
-            os.path.join(karto, "src", "Karto.cpp"), os.path.join(karto, "src", "Mapper.cpp")]
-    drv = os.path.join(_HERE, "ref_lesson6.cpp")
-    deps = srcs + [drv, os.path.join(_ROOT, "include", "b200slam.h")] + \
-        [os.path.join(_HERE, "shim_lesson6", h) for h in _SHIM6] + [os.path.join(_HERE, "shim", h) for h in _SHIM]
-    if not os.path.exists(_PATH) or any(os.path.getmtime(d) > os.path.getmtime(_PATH) for d in deps):
-        os.makedirs(os.path.dirname(_PATH), exist_ok=True)
-        tmp = _PATH + f".{os.getpid()}.tmp"
-        # the compiler oracle/Makefile builds open_karto with (its `CXX := g++` overrides the environment): the library is
-        # loaded next to numpy's C++ runtime, and a newer compiler's libstdc++ inlines do not mix with it
-        subprocess.check_call(["g++"] + CXXFLAGS +
-                              ["-shared", "-I" + os.path.join(_HERE, "shim_lesson6"), "-I" + os.path.join(_HERE, "shim"),
-                               "-I" + ref, "-I" + os.path.join(ref, "lesson6", "include"),
-                               "-I" + os.path.join(karto, "include"), drv, srcs[2], srcs[3], "-o", tmp, "-lm"])
-        os.replace(tmp, _PATH)
-    return _PATH
-
-
 def available() -> bool:
-    return os.path.exists(_PATH)
+    return recipes.available(_NAME)
 
 
 def lib():
     global _lib
     if _lib is None:
-        L = C.CDLL(_PATH)
+        L = C.CDLL(recipes.path(_NAME))
         dp, fp, ip = C.POINTER(C.c_double), C.POINTER(C.c_float), C.POINTER(C.c_int32)
         sys.path.insert(0, _ROOT) if _ROOT not in sys.path else None
         ScanSolver = importlib.import_module("creating-2d-laser-slam-from-scratch_b200.mapper").ScanSolver

@@ -1,6 +1,6 @@
 """Generate tests/golden/*.npz from the UNMODIFIED reference (oracle/_ref/libkarto_ref.so, asserts enabled).
 
-Needs the reference build (`make -C oracle ref REF=<checkout of the original project>`):
+Needs the reference build (`python -m oracle.recipes --ref <checkout of the original project>`):
     python tests/golden/make_golden.py
 The answers the *_live tests record (tests/golden/reference/) are rewritten by running those tests with
 SLAM_RECORD_GOLDEN=1 where the reference build is present.
@@ -231,7 +231,7 @@ def fleet_case():
 
 
 if __name__ == "__main__":
-    assert ref.available(), "run `make -C oracle ref` first"
+    assert ref.available(), "run `python -m oracle.recipes --ref <checkout>` first"
     if sys.argv[1:] == ["mapper"]:
         mapper_case()
         print("karto_mapper.npz", os.path.getsize(os.path.join(HERE, "karto_mapper.npz")))

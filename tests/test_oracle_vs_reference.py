@@ -1,6 +1,6 @@
 """The C restatement against the reference build (oracle/_ref/libkarto_ref.so = the unmodified open_karto sources,
-compiled by `make -C oracle ref`) on fresh seeded inputs.  Where that build is absent, the reference's answers come from
-its recording (tests/reference_record.py).  CPU only."""
+compiled by `python -m oracle.recipes --ref <checkout>`) on fresh seeded inputs.  Where that build is absent, the
+reference's answers come from its recording (tests/reference_record.py).  CPU only."""
 import numpy as np
 import pytest
 
