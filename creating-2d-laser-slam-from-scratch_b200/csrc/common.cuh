@@ -146,14 +146,12 @@ constexpr double MAX_VARIANCE = 500.0;             // Mapper.cpp:36
 constexpr double DISTANCE_PENALTY_GAIN = 0.2;      // Mapper.cpp:37
 constexpr double ANGLE_PENALTY_GAIN = 0.2;         // Mapper.cpp:38
 
-// math::Round (Math.h:87-90): half away from zero
+// math::Round (Math.h:87-90): half away from zero, v >= 0 ? floor(v + 0.5) : ceil(v - 0.5).  The same bits with one
+// rounding op instead of two: ceil(v - 0.5) == -floor(-v + 0.5) for v < 0 (negation is exact), and -0.0 takes the
+// v >= 0 side to +0.0 (tests/device_math_check.cu compares both builds with the reference's form).
 __host__ __device__ __forceinline__ double kround(double v) {
-#ifdef __CUDA_ARCH__
-  // identical values: ceil(v - 0.5) == -floor(-v + 0.5) for v < 0 (negation is exact); one rounding op instead of two
-  return copysign(floor(fabs(v) + 0.5), v);
-#else
-  return v >= 0.0 ? floor(v + 0.5) : ceil(v - 0.5);
-#endif
+  const double r = floor(fabs(v) + 0.5);
+  return v < 0.0 ? -r : r;
 }
 
 // static_cast<kt_int32s>(double) as the reference's x86-64 build performs it (cvttsd2si: out-of-range and NaN

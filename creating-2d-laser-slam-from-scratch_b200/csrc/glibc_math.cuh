@@ -126,6 +126,21 @@ B2S_HD float glibc_cosf(float y, bool use_fma) {
   return cosf(y);
 }
 
+// The reference's unqualified sin / cos of a float (OccGridMapUtil.h:87-88): the C library's DOUBLE functions, rounded to
+// float.  The device takes its own double sincos (within 2 double ulps of the exact value), so the two floats could only
+// differ where the exact value lies within a few double ulps of a float rounding boundary; tests/device_math_check.cu
+// compares every float with |a| <= 16 against the C library and finds none that differ.
+B2S_HD void libm_sincos_to_float(float a, float *s, float *c) {
+#if defined(__CUDA_ARCH__)
+  double ds, dc;
+  sincos((double)a, &ds, &dc);
+#else
+  const double ds = sin((double)a), dc = cos((double)a);
+#endif
+  *s = (float)ds;
+  *c = (float)dc;
+}
+
 // (host function)
 // Which build of s_sincosf does THIS host's libm run?  1 = FMA, 0 = separate multiply / add, -1 = neither restatement
 // reproduces it on the probe inputs (an unknown libm: callers fall back to 1 and report it).  The two builds differ on

@@ -164,6 +164,14 @@ inline float prob_to_log_odds_logf(float prob) {
   return logf(odds);
 }
 
+// GridMapLogOddsFunctions::getGridProbability (:136-140) as the processor computes it: the unqualified exp() is the C
+// library's double exp, rounded to float (the device's double exp; tests/device_math_check.cu compares every float in
+// [-128, 64] against the C library).
+__host__ __device__ __forceinline__ float log_odds_prob(float lo) {
+  const float odds = (float)exp((double)lo);
+  return odds / (odds + 1.0f);
+}
+
 // HectorMappingRos::publishMap (lesson4/src/hector_mapping/hector_slam.cc:254-317): free -> 0, occupied -> 100, else -1.
 __device__ __forceinline__ int8_t hector_ros_cell(float v) { return v < 0.0f ? 0 : (v > 0.0f ? 100 : -1); }
 

@@ -129,7 +129,7 @@ __global__ void __launch_bounds__(256)
 // ---- K3: Gauss-Newton scan-to-map alignment (one grid level), whole iteration loop in one launch ----
 
 // getGridProbability (GridMapLogOdds.h:136-140) with the device's float expf, where the reference rounds the C library's
-// double exp to float (as the processor's hs_prob_of does): the values can differ in the last bits, which is why
+// double exp to float (as the processor's log_odds_prob does): the values can differ in the last bits, which is why
 // b2s_hector_map_match_data is held to 1e-4 of the reference rather than bit for bit.
 __device__ __forceinline__ float hc_prob(const float *__restrict__ lo, int index) {
   const float odds = expf(lo[index]);

@@ -26,8 +26,8 @@
 // reference bit for bit: the nine sums of getCompleteHessianDerivs are accumulated sequentially in point order (one lane
 // per sum), Rotation2Df's std::cos / std::sin(float) are glibc's sincosf restated (glibc_math.cuh), the unqualified
 // sin / cos / exp of the reference (C library DOUBLE functions rounded to float) are the device's double functions
-// rounded to float (both are within 2 ulp of the exact double, so the float agrees unless the exact value lies within
-// ~1e-16 relative of a float rounding boundary: ~5e-9 per evaluation).  FAST mode differs in ONE thing: the nine sums are
+// rounded to float (libm_sincos_to_float, log_odds_prob).  Those floats equal glibc's for EVERY float angle with
+// |a| <= 16 and every float log-odds value in [-128, 64]: tests/test_gpu_device_math.py compares all of them.  FAST mode differs in ONE thing: the nine sums are
 // tree-reduced (warp shuffles) instead of accumulated in point order, so its Hessians / poses differ in the last float bits
 // (~1e-6 m per scan, inside the 1e-4 contract) and a cell can move when a pose lands an ulp away.
 //
@@ -231,10 +231,7 @@ __device__ __noinline__ HsTrig hs_trig(float angle, bool exact, bool use_fma) {
   HsTrig t;
   if (exact) {
     glibc_sincosf(angle, use_fma, &t.s, &t.c);
-    double ds, dc;
-    sincos((double)angle, &ds, &dc);
-    t.sin_rot = (float)ds;
-    t.cos_rot = (float)dc;
+    libm_sincos_to_float(angle, &t.sin_rot, &t.cos_rot);
   } else {
     // fast mode: the glibc-exact float sine / cosine also stand in for sinRot / cosRot (they differ from the rounded
     // double ones on ~1 % of angles, by one ulp).  The device's own sincosf was tried here and broke the 1e-4 contract on
@@ -690,11 +687,6 @@ __device__ __forceinline__ HsUpd hs_load_upd(const HsState *st, int lv) {
   return u;
 }
 
-__device__ __forceinline__ float hs_prob_of(float lo) {  // getGridProbability (GridMapLogOdds.h:136-140)
-  const float odds = (float)exp((double)lo);  // unqualified exp(): the C library's double exp, rounded to float
-  return odds / (odds + 1.0f);
-}
-
 // MapRepMultiMap::updateByScan (:174-191) for processor b, PASS 1 (mark): work item = (level, beam), flattened over
 // the levels, one warp each; lanes over Bresenham steps in closed form.  Every traversed cell records the LOWEST beam
 // index that frees it / ends on it (32-bit atomicMax of epoch | ~beam).  Returns this warp's cell visits.
@@ -793,12 +785,12 @@ __device__ void hs_apply_pass(const HsBatch &P, int b, int w, int nw, int lane) 
         }
         if (v < 50.0f) v = __fadd_rn(v, P.lo_occ);
         lo[off] = v;
-        hs_publish_prob(quad, m.sx, xb + 32 * q, y, hs_prob_of(v));
+        hs_publish_prob(quad, m.sx, xb + 32 * q, y, log_odds_prob(v));
         ui[off] = mark_occ;
       } else if (f[q] != 0 && (f[q] >> 12) == ep) {  // bresenhamCellFree (:302-312)
         const float v = __fadd_rn(__ldcg(lo + off), P.lo_free);
         lo[off] = v;
-        hs_publish_prob(quad, m.sx, xb + 32 * q, y, hs_prob_of(v));
+        hs_publish_prob(quad, m.sx, xb + 32 * q, y, log_odds_prob(v));
         ui[off] = mark_free;
       }
     }

@@ -1,18 +1,18 @@
 // TEST HELPER (host only): the three definitions of tf / tf2 LinearMath and roscpp Time / Duration — the library's
 // csrc/ros_math.cuh, the C restatements' oracle/linear_math.h and the node stand-ins' classes (oracle/shim/tf2,
-// oracle/shim/tf, oracle/shim_lesson6/tf/tf_core.h, oracle/shim/ros/ros.h) — on one seeded sweep of inputs, compared
-// bit for bit (a NaN matches any NaN).  Prints one JSON line: checks, mismatches, the first mismatch, and how often each
+// oracle/shim/tf, oracle/shim_lesson6/tf/tf_core.h, oracle/shim/ros/ros.h) — on the seeded sweep of inputs of
+// ros_math_sweep.h, compared bit for bit (a NaN matches any NaN).  Prints one JSON line: checks, mismatches, the first mismatch, and how often each
 // branch of the restated code was taken.  Build with -ffp-contract=off, as the library's host code and the stand-ins.
 #include <cmath>
 #include <cstdint>
 #include <cstdio>
 #include <cstring>
 #include <map>
-#include <random>
 #include <string>
 
 #include "../creating-2d-laser-slam-from-scratch_b200/csrc/ros_math.cuh"
 #include "../oracle/linear_math.h"
+#include "ros_math_sweep.h"
 #include "ros/ros.h"
 #include "tf/LinearMath/Matrix3x3.h"
 #include "tf/tf_core.h"
@@ -153,65 +153,15 @@ void check_compare(const b2s::RosDuration &a, const b2s::RosDuration &b) {
   expect2("Duration>", 0, b2s::ros_duration_gt(a, b), ros::Duration(a.sec, a.nsec) > ros::Duration(b.sec, b.nsec));
 }
 
-}  // namespace
-
-int main() {
-  std::mt19937_64 rng(20261016);
-  std::uniform_real_distribution<double> u(-1.0, 1.0), scale(0.05, 20.0), big(-1e6, 1e6);
-  std::uniform_int_distribution<uint32_t> any32;
-  const double pi = 3.14159265358979323846;
-
-  // quaternions: random unit and non-unit, zero, and each getRotation branch (w, then x, y or z largest), with ties
-  const double crafted[][4] = {{0, 0, 0, 1},    {0, 0, 0, -1},  {0, 0, 0, 0},      {1, 0.1, 0.1, 0.05}, {0.1, 1, 0.1, 0.05},
-                               {0.1, 0.1, 1, 0.05}, {1, 1, 0, 0}, {0, 1, 1, 0},     {1, 0, 1, 0},        {1, 1, 1, 0},
-                               {1, 0, 0, 0},    {0, 1, 0, 0},   {0, 0, 1, 0},      {0, 1, 0, 1},        {0, 1, 0, -1},
-                               {1, 1, -1, 1},   {1, 1, 1, -1},  {1e-300, 0, 0, 0}, {3, 4, 0, 0},        {-2, 0, 0, 1e-9}};
-  for (const auto &q : crafted) check_quaternion(q);
-  for (int n = 0; n < 20000; n++) {
-    double q[4] = {u(rng), u(rng), u(rng), u(rng)};
-    const double len = std::sqrt(q[0] * q[0] + q[1] * q[1] + q[2] * q[2] + q[3] * q[3]);
-    const double f = n % 2 ? scale(rng) : 1.0;
-    for (double &x : q) x = x / len * f;
-    if (n % 5 == 0) q[3] *= 1e-3;  // a small w: trace <= 0
-    check_quaternion(q);
-  }
-
-  // roll / pitch / yaw, with pitch exactly +-90 degrees and just inside
-  for (int n = 0; n < 5000; n++) check_rpy(pi * u(rng), 0.5 * pi * u(rng), pi * u(rng));
-  for (double p : {pi / 2, -pi / 2}) {
-    for (int k = 0; k < 40; k++) {
-      const double inside = p - (p > 0 ? 1 : -1) * k * 1e-9;
-      check_rpy(pi * u(rng), inside, pi * u(rng));
-      check_rpy(0, inside, 0);
-    }
-  }
-  // tf2::getYaw's sarg on both sides of +-0.99999: a pure pitch a has sarg = sin(a)
-  const double edge = std::asin(0.99999);
-  for (int k = -200; k <= 200; k++)
-    for (double sg : {1.0, -1.0}) {
-      const double a = sg * (edge + k * 1e-12), yaw = 0.3 * k;
-      check_rpy(0, a, 0);
-      check_rpy(0.1, a, yaw);
-    }
-
-  // matrices entered directly: m[2][0] at, beyond and just inside +-1, and random entries for every getRotation branch
-  for (int n = 0; n < 4000; n++) {
-    double m[3][3], o[3] = {u(rng), u(rng), u(rng)};
-    for (auto &r : m)
-      for (double &x : r) x = u(rng);
-    const double m20[] = {1.0, -1.0, std::nextafter(1.0, 0.0), std::nextafter(-1.0, 0.0), std::nextafter(1.0, 2.0),
-                          std::nextafter(-1.0, -2.0)};
-    if (n < 600) m[2][0] = m20[n % 6];
-    check_rotation(from_entries(m, o));
-  }
-
-  // chains of products and inverses, and Transform::operator()(v)
-  for (int chain = 0; chain < 300; chain++) {
-    double q[4] = {u(rng), u(rng), u(rng), u(rng)}, o[3] = {big(rng) * 1e-4, big(rng) * 1e-4, big(rng) * 1e-4};
+// the sweep's sink: every input through all three definitions
+struct Checks {
+  void quaternion(const double q[4]) { check_quaternion(q); }
+  void rpy(double r, double p, double y) { check_rpy(r, p, y); }
+  void entries(const double m[3][3], const double o[3]) { check_rotation(from_entries(m, o)); }
+  void chain(const double q[4], const double o[3], const double q2[][4], const double o2[][3], const double v[][3]) {
     Three acc = from_quaternion(q, o);
-    for (int step = 0; step < 12; step++) {
-      double q2[4] = {u(rng), u(rng), u(rng), u(rng)}, o2[3] = {u(rng) * 10, u(rng) * 10, u(rng) * 10};
-      const Three b = from_quaternion(q2, o2);
+    for (int step = 0; step < ROS_MATH_CHAIN_STEPS; step++) {
+      const Three b = from_quaternion(q2[step], o2[step]);
       Three next;
       if (step % 3 == 0) {  // acc * b^-1
         const b2s::TfTransform il = b2s::tf_inverse(b.lib);
@@ -232,10 +182,9 @@ int main() {
       }
       acc = next;
       compare("product / inverse", acc);
-      const double v[3] = {u(rng) * 5, u(rng) * 5, u(rng) * 5};
       double vl[3];
-      b2s::tf_apply(acc.lib, v, vl);
-      const tf2::Vector3 vs = acc.shim(tf2::Vector3(v[0], v[1], v[2]));
+      b2s::tf_apply(acc.lib, v[step], vl);
+      const tf2::Vector3 vs = acc.shim(tf2::Vector3(v[step][0], v[step][1], v[step][2]));
       for (int i = 0; i < 3; i++) expect2("Transform(v)", i, vl[i], vs[i]);
       check_rotation(acc);
     }
@@ -245,29 +194,21 @@ int main() {
     id.shim = tf2::Transform();
     compare("identity", id);
   }
-
-  // stamps: negative and overflowing nanoseconds, seconds across the int32 wrap.  A nanosecond field is below 2^31:
-  // roscpp subtracts the fields as int32, which overflows beyond that.
-  const uint32_t secs[] = {0, 1, 2, 1000, 0x7ffffffeu, 0x7fffffffu, 0x80000000u, 0x80000001u, 0xfffffffeu, 0xffffffffu};
-  const uint32_t nsecs[] = {0, 1, 999999999u, 1000000000u, 1000000001u, 1999999999u, 2000000000u, 0x7fffffffu, 500000000u};
-  for (uint32_t s1 : secs)
-    for (uint32_t s0 : secs)
-      for (uint32_t n1 : nsecs)
-        for (uint32_t n0 : nsecs) check_stamps(s1, n1, s0, n0);
-  for (int n = 0; n < 20000; n++) check_stamps(any32(rng), any32(rng) >> 1, any32(rng), any32(rng) >> 1);
-
-  // Duration::fromSec: x.9999999995 (rolls a second over), negative values, random values, and the comparison
-  const double secs_d[] = {0.0, -0.0, 0.9999999995, 1.9999999995, 41.9999999995, -0.0000000005, -1e-10, -0.5,
-                           -1.0, -2.5, -3.9999999995, -1.0000000005, 0.0000000005, 1e-10, 2147483647.0, -2147483648.0,
-                           0.99999999949999, 0.9999999994999999, 1.25, 3.0000000004999};
-  for (double d : secs_d) check_from_sec(d);
-  for (int n = 0; n < 20000; n++) {
-    const double d = n % 2 ? big(rng) : std::floor(big(rng)) + (n % 4 == 1 ? 0.9999999995 : -0.0000000005);
+  void stamps(uint32_t s1, uint32_t n1, uint32_t s0, uint32_t n0) { check_stamps(s1, n1, s0, n0); }
+  void from_sec(double d) { check_from_sec(d); }
+  void from_sec_pair(double d, double d2) {
     check_from_sec(d);
-    const b2s::RosDuration a = b2s::ros_duration_from_sec(d), b = b2s::ros_duration_from_sec(n % 3 ? big(rng) : d);
+    const b2s::RosDuration a = b2s::ros_duration_from_sec(d), b = b2s::ros_duration_from_sec(d2);
     check_compare(a, b);
     check_compare(b, a);
   }
+};
+
+}  // namespace
+
+int main() {
+  Checks checks_sink;
+  ros_math_sweep(checks_sink);
 
   std::printf("{\"checks\": %ld, \"mismatches\": %ld, \"first\": \"%s\", \"branches\": {", checks, mismatches, first.c_str());
   const char *sep = "";
