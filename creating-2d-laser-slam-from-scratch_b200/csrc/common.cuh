@@ -315,6 +315,11 @@ __device__ __forceinline__ bool mbar_try_wait(uint64_t *bar, uint32_t parity) {
 
 inline int ceil_div(long long a, long long b) { return (int)((a + b - 1) / b); }
 
+// gridDim.y's limit.  Kernels that put a batch on grid y loop `for (b = blockIdx.y; b < count; b += gridDim.y)` and are
+// launched with grid_rows(count) rows, so a batch of any size runs; up to this many items each row serves one.
+constexpr int GRID_Y_MAX = 65535;
+inline unsigned grid_rows(long long count) { return (unsigned)std::min<long long>(std::max<long long>(count, 1), GRID_Y_MAX); }
+
 // SMs of `device` (132 on an H100 SXM): grid-stride kernels size their grids as a multiple of it.
 inline int sm_count(int device) {
   int sms = 0;

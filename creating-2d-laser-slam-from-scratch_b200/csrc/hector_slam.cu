@@ -805,17 +805,20 @@ __global__ void __launch_bounds__(HS_THREADS, 1) k_hs_match(HsBatch P, HsCall C)
   extern __shared__ __align__(16) unsigned char hs_smem[];
   hs_match_cta<EXACT, false>(P, C, blockIdx.x, hs_smem);
 }
+// processors b = blockIdx.y, + gridDim.y, ... (grid_rows(batch) rows)
 __global__ void __launch_bounds__(256) k_hs_mark(HsBatch P) {
-  const int b = blockIdx.y;
-  if (!P.state[b].do_update) return;
-  const int lane = threadIdx.x & 31;
-  const unsigned long long v = hs_mark_pass(P, b, (blockIdx.x * blockDim.x + threadIdx.x) >> 5, (gridDim.x * blockDim.x) >> 5, lane);
-  if (lane == 0 && v) atomicAdd(&P.state[b].visits, v);  // lane 0 carries the warp's count
+  for (int b = blockIdx.y; b < P.batch; b += gridDim.y) {
+    if (!P.state[b].do_update) continue;
+    const int lane = threadIdx.x & 31;
+    const unsigned long long v = hs_mark_pass(P, b, (blockIdx.x * blockDim.x + threadIdx.x) >> 5, (gridDim.x * blockDim.x) >> 5, lane);
+    if (lane == 0 && v) atomicAdd(&P.state[b].visits, v);  // lane 0 carries the warp's count
+  }
 }
 __global__ void __launch_bounds__(256) k_hs_apply(HsBatch P) {
-  const int b = blockIdx.y;
-  if (!P.state[b].do_update) return;
-  hs_apply_pass(P, b, (blockIdx.x * blockDim.x + threadIdx.x) >> 5, (gridDim.x * blockDim.x) >> 5, threadIdx.x & 31);
+  for (int b = blockIdx.y; b < P.batch; b += gridDim.y) {
+    if (!P.state[b].do_update) continue;
+    hs_apply_pass(P, b, (blockIdx.x * blockDim.x + threadIdx.x) >> 5, (gridDim.x * blockDim.x) >> 5, threadIdx.x & 31);
+  }
 }
 
 // ---- single-processor path: ONE cooperative launch walks n_scans scans (n_scans = 1 for b2s_hector_slam_update) ----
@@ -1366,7 +1369,7 @@ static b2s_status hs_launch_step(b2s_hector_slam *p, const float *d_points, cons
   else k_hs_match<false><<<B, HS_THREADS, hs_smem_bytes(p->cap), p->stream>>>(p->P, C);
   // data containers of the coarse levels may hold more points than this step's scans (map_without_matching): size the
   // update grid by the capacity bound
-  const dim3 grid(std::max(1, std::min(ceil_div(std::max(max_n, 1) * p->levels, 8), sm_count(p->device) * 8 / std::max(1, std::min(B, 8)))), B);
+  const dim3 grid(std::max(1, std::min(ceil_div(std::max(max_n, 1) * p->levels, 8), sm_count(p->device) * 8 / std::max(1, std::min(B, 8)))), grid_rows(B));
   k_hs_mark<<<grid, 256, 0, p->stream>>>(p->P);
   k_hs_apply<<<grid, 256, 0, p->stream>>>(p->P);
   B2S_CUDA_CHECK(cudaGetLastError());

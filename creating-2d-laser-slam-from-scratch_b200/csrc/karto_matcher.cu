@@ -427,53 +427,55 @@ __global__ void __launch_bounds__(256) k_sweep_generic(const uint8_t *__restrict
                                                        const double *__restrict__ local,
                                                        const double *__restrict__ grid_off,
                                                        const double *__restrict__ centers, double angle_offset,
-                                                       double angle_res, int width_step, double scale, int k_first) {
-  const int b = blockIdx.y;
-  const int f = flags[b];
-  if (f & 2) return;
-  if (mode == 1 && (f & 1)) return;
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const uint8_t *grid = grids + (size_t)b * grid_pitch;
-  for (int c = blockIdx.x * (blockDim.x >> 5) + warp; c < ncell; c += gridDim.x * (blockDim.x >> 5)) {
-  const int32_t base = bases[(size_t)b * ncell + c];
-  for (int k = 0; k < na; k++) {
-    const int32_t *offs = lut ? lut + ((size_t)b * na + k) * n : nullptr;
-    double cosine = 0, sine = 0, gox = 0, goy = 0;
-    if (!lut) {  // no materialised table (window mode fall-through): GridIndexLookup values on the fly
-      const double angle = (centers[(size_t)b * 3 + 2] - angle_offset) + (double)(uint32_t)(k_first + k) * angle_res;
-      cosine = cos(angle); sine = sin(angle);
-      gox = grid_off[2 * b]; goy = grid_off[2 * b + 1];
-    }
-    int32_t sum = 0;
-    if (lut) {
-      // 8 independent (offset, cell) load chains in flight per lane: the gather is latency bound
-      constexpr int U = 8;
-      for (int i0 = lane; i0 < n; i0 += 32 * U) {
-        int32_t o[U];
+                                                       double angle_res, int width_step, double scale, int k_first,
+                                                       int batch) {
+  for (int b = blockIdx.y; b < batch; b += gridDim.y) {
+    const int f = flags[b];
+    if (f & 2) continue;
+    if (mode == 1 && (f & 1)) continue;
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const uint8_t *grid = grids + (size_t)b * grid_pitch;
+    for (int c = blockIdx.x * (blockDim.x >> 5) + warp; c < ncell; c += gridDim.x * (blockDim.x >> 5)) {
+      const int32_t base = bases[(size_t)b * ncell + c];
+      for (int k = 0; k < na; k++) {
+        const int32_t *offs = lut ? lut + ((size_t)b * na + k) * n : nullptr;
+        double cosine = 0, sine = 0, gox = 0, goy = 0;
+        if (!lut) {  // no materialised table (window mode fall-through): GridIndexLookup values on the fly
+          const double angle = (centers[(size_t)b * 3 + 2] - angle_offset) + (double)(uint32_t)(k_first + k) * angle_res;
+          cosine = cos(angle); sine = sin(angle);
+          gox = grid_off[2 * b]; goy = grid_off[2 * b + 1];
+        }
+        int32_t sum = 0;
+        if (lut) {
+          // 8 independent (offset, cell) load chains in flight per lane: the gather is latency bound
+          constexpr int U = 8;
+          for (int i0 = lane; i0 < n; i0 += 32 * U) {
+            int32_t o[U];
 #pragma unroll
-        for (int u = 0; u < U; u++) o[u] = (i0 + 32 * u < n) ? __ldg(offs + i0 + 32 * u) : INVALID_SCAN;
-        uint32_t v[U];
+            for (int u = 0; u < U; u++) o[u] = (i0 + 32 * u < n) ? __ldg(offs + i0 + 32 * u) : INVALID_SCAN;
+            uint32_t v[U];
 #pragma unroll
-        for (int u = 0; u < U; u++) {
-          const int32_t idx = (int32_t)((uint32_t)base + (uint32_t)o[u]);
-          v[u] = (o[u] != INVALID_SCAN && idx >= 0 && idx < data_size) ? (uint32_t)__ldg(grid + idx) : 0u;
+            for (int u = 0; u < U; u++) {
+              const int32_t idx = (int32_t)((uint32_t)base + (uint32_t)o[u]);
+              v[u] = (o[u] != INVALID_SCAN && idx >= 0 && idx < data_size) ? (uint32_t)__ldg(grid + idx) : 0u;
+            }
+#pragma unroll
+            for (int u = 0; u < U; u++) sum += (int32_t)v[u];
+          }
+        } else {
+          for (int i = lane; i < n; i += 32) {
+            const int32_t o = lut_value(ranges[(size_t)b * n + i], local[((size_t)b * n + i) * 2],
+                                        local[((size_t)b * n + i) * 2 + 1], cosine, sine, gox, goy, scale, width_step);
+            if (o == INVALID_SCAN) continue;
+            const int32_t idx = (int32_t)((uint32_t)base + (uint32_t)o);
+            if (idx >= 0 && idx < data_size) sum += __ldg(grid + idx);
+          }
         }
 #pragma unroll
-        for (int u = 0; u < U; u++) sum += (int32_t)v[u];
-      }
-    } else {
-      for (int i = lane; i < n; i += 32) {
-        const int32_t o = lut_value(ranges[(size_t)b * n + i], local[((size_t)b * n + i) * 2],
-                                    local[((size_t)b * n + i) * 2 + 1], cosine, sine, gox, goy, scale, width_step);
-        if (o == INVALID_SCAN) continue;
-        const int32_t idx = (int32_t)((uint32_t)base + (uint32_t)o);
-        if (idx >= 0 && idx < data_size) sum += __ldg(grid + idx);
+        for (int d = 16; d > 0; d >>= 1) sum += __shfl_xor_sync(0xffffffffu, sum, d);
+        if (lane == 0) sums[((size_t)b * na + k) * ncell + c] = sum;
       }
     }
-#pragma unroll
-    for (int d = 16; d > 0; d >>= 1) sum += __shfl_xor_sync(0xffffffffu, sum, d);
-    if (lane == 0) sums[((size_t)b * na + k) * ncell + c] = sum;
-  }
   }
 }
 
@@ -554,24 +556,25 @@ __global__ void __launch_bounds__(256)
 // ----------------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(256)
     k_grid_pool(const uint8_t *__restrict__ grids, size_t grid_pitch, int data_size, int width_step,
-                int lead, uint8_t *__restrict__ pools, size_t pitch) {
-  const int b = blockIdx.y;
+                int lead, uint8_t *__restrict__ pools, size_t pitch, int batch) {
   const int j4 = blockIdx.x * blockDim.x + threadIdx.x;
   if ((size_t)j4 * 4 >= pitch) return;
-  const uint8_t *grid = grids + (size_t)b * grid_pitch;
-  const int f = 4 * j4 - lead;  // a multiple of 4, as are width_step and data_size
-  auto word = [&](int r) { return (r >= 0 && r < data_size) ? __ldg(reinterpret_cast<const uint32_t *>(grid + r)) : 0u; };
-  uint32_t m = 0;
+  for (int b = blockIdx.y; b < batch; b += gridDim.y) {
+    const uint8_t *grid = grids + (size_t)b * grid_pitch;
+    const int f = 4 * j4 - lead;  // a multiple of 4, as are width_step and data_size
+    auto word = [&](int r) { return (r >= 0 && r < data_size) ? __ldg(reinterpret_cast<const uint32_t *>(grid + r)) : 0u; };
+    uint32_t m = 0;
 #pragma unroll
-  for (int dy = 0; dy < 4; dy++) {
-    const int r = f + dy * width_step;
-    const uint32_t w0 = word(r), w1 = word(r + 4);
-    // byte t of the result = max of bytes t..t+3 of the 8 bytes w1:w0
-    const uint32_t a = __vmaxu4(w0, __funnelshift_r(w0, w1, 8));
-    const uint32_t c = __vmaxu4(__funnelshift_r(w0, w1, 16), __funnelshift_r(w0, w1, 24));
-    m = __vmaxu4(m, __vmaxu4(a, c));
+    for (int dy = 0; dy < 4; dy++) {
+      const int r = f + dy * width_step;
+      const uint32_t w0 = word(r), w1 = word(r + 4);
+      // byte t of the result = max of bytes t..t+3 of the 8 bytes w1:w0
+      const uint32_t a = __vmaxu4(w0, __funnelshift_r(w0, w1, 8));
+      const uint32_t c = __vmaxu4(__funnelshift_r(w0, w1, 16), __funnelshift_r(w0, w1, 24));
+      m = __vmaxu4(m, __vmaxu4(a, c));
+    }
+    reinterpret_cast<uint32_t *>(pools + (size_t)b * pitch)[j4] = m;
   }
-  reinterpret_cast<uint32_t *>(pools + (size_t)b * pitch)[j4] = m;
 }
 
 // ----------------------------------------------------------------------------------------------
@@ -1883,8 +1886,9 @@ static b2s_status build_sat(b2s_matcher *m) {
 static b2s_status build_pool(b2s_matcher *m) {
   if (!pool_fits(m->g, m->smem_optin, m->win_static_smem)) return B2S_OK;
   const size_t pitch = pool_pitch(m->g);
-  k_grid_pool<<<dim3((unsigned)ceil_div((int)(pitch / 4), 256), (unsigned)m->batch), 256, 0, m->stream>>>(
-      m->d_grids, m->grid_pitch, m->g.data_size, m->g.width_step, pool_lead(m->g.width_step), m->d_pools, pitch);
+  k_grid_pool<<<dim3((unsigned)ceil_div((int)(pitch / 4), 256), grid_rows(m->batch)), 256, 0, m->stream>>>(
+      m->d_grids, m->grid_pitch, m->g.data_size, m->g.width_step, pool_lead(m->g.width_step), m->d_pools, pitch,
+      m->batch);
   B2S_CUDA_CHECK(cudaGetLastError());
   return B2S_OK;
 }
@@ -2623,16 +2627,16 @@ static b2s_status run_correlate(b2s_matcher *m, const b2s_search *s, int k_first
     // matches whose lattice is not the regular raster (a centre exactly on a rounding tie) fall through;
     // they compute their lookup values on the fly (no table was materialised for them)
     // (a few CTAs per match that exit at once unless the lattice is irregular: the kernel loops over the cells)
-    k_sweep_generic<<<dim3(4, (unsigned)B), 256, 0, m->stream>>>(m->d_grids, m->grid_pitch, m->g.data_size, nullptr, m->d_bases,
+    k_sweep_generic<<<dim3(4, grid_rows(B)), 256, 0, m->stream>>>(m->d_grids, m->grid_pitch, m->g.data_size, nullptr, m->d_bases,
                                                   m->d_flags, 1, n, na, ncell, m->d_sums, m->d_ranges, m->d_local,
                                                   m->d_grid_off, m->d_centers, s->angle_offset, s->angle_res,
-                                                  m->g.width_step, scale, k_first);
+                                                  m->g.width_step, scale, k_first, B);
     m->last_path = 2;
   } else {
-    k_sweep_generic<<<dim3((unsigned)ceil_div(ncell, 8), (unsigned)B), 256, 0, m->stream>>>(
+    k_sweep_generic<<<dim3((unsigned)ceil_div(ncell, 8), grid_rows(B)), 256, 0, m->stream>>>(
         m->d_grids, m->grid_pitch, m->g.data_size, m->d_lut, m->d_bases, m->d_flags, 0, n, na, ncell, m->d_sums,
         m->d_ranges, m->d_local, m->d_grid_off, m->d_centers, s->angle_offset, s->angle_res, m->g.width_step, scale,
-        k_first);
+        k_first, B);
     m->last_path = 1;
   }
   B2S_CUDA_CHECK(cudaGetLastError());

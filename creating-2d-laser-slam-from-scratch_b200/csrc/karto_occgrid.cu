@@ -262,15 +262,18 @@ __global__ void __launch_bounds__(256)
   }
 }
 
-// thresholds and ROS payload of every grid: blockIdx.y = grid, x-blocks stride over its w x h cells
+// thresholds and ROS payload of every grid: grids blockIdx.y, + gridDim.y, ... (grid_rows(n_grids) rows), x-blocks
+// stride over each one's w x h cells
 __global__ void k_occ_ros_grids(const uint32_t *__restrict__ pass, const uint32_t *__restrict__ hit,
-                                const OccGridDev *__restrict__ grids, int8_t *__restrict__ out) {
-  const OccGridDev G = grids[blockIdx.y];
-  const long long cells = (long long)G.w * G.h;
-  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < cells; i += (long long)gridDim.x * blockDim.x) {
-    const int x = (int)(i % G.w), y = (int)(i / G.w);
-    const size_t c = (size_t)G.counters + x + (size_t)y * G.step;
-    out[G.payload + i] = occ_ros_value(occ_cell_value(pass[c], hit[c]));
+                                const OccGridDev *__restrict__ grids, int n_grids, int8_t *__restrict__ out) {
+  for (int g = blockIdx.y; g < n_grids; g += gridDim.y) {
+    const OccGridDev G = grids[g];
+    const long long cells = (long long)G.w * G.h;
+    for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < cells; i += (long long)gridDim.x * blockDim.x) {
+      const int x = (int)(i % G.w), y = (int)(i / G.w);
+      const size_t c = (size_t)G.counters + x + (size_t)y * G.step;
+      out[G.payload + i] = occ_ros_value(occ_cell_value(pass[c], hit[c]));
+    }
   }
 }
 
@@ -681,7 +684,7 @@ b2s_status occ_batch_build(OccBatch *b, int G, const int32_t *n_scans, const int
     long long most = 0;
     for (const OccGridDev &D : b->grids) most = std::max(most, (long long)D.w * D.h);
     const unsigned xb = (unsigned)std::min<long long>(ceil_div(most, 256), 1024);
-    k_occ_ros_grids<<<dim3(xb, (unsigned)L), 256, 0, st>>>(b->d_pass, b->d_hit, b->d_grids, b->d_payload);
+    k_occ_ros_grids<<<dim3(xb, grid_rows(L)), 256, 0, st>>>(b->d_pass, b->d_hit, b->d_grids, L, b->d_payload);
   }
   B2S_CUDA_CHECK(cudaGetLastError());
   if (bytes) B2S_CUDA_CHECK(cudaMemcpyAsync(b->h_payload, b->d_payload, (size_t)bytes, cudaMemcpyDeviceToHost, st));

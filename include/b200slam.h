@@ -116,7 +116,8 @@ int b2s_device_count(void);                    /* 0 when no usable CUDA device *
  * until the next call that waits for the stream (correlate_scan, match_scan, _end, sync). */
 
 /* ScanMatcher::Create (Mapper.cpp:126-172).  `max_batch` matches share one handle, each with up to
- * `max_base_scans` base scans; buffers that depend on the search volume grow on demand.  `cuda_stream` may be NULL
+ * `max_base_scans` base scans; `max_batch` may be any count >= 1 whose buffers fit in device memory (65 535 is not a
+ * limit).  Buffers that depend on the search volume grow on demand.  `cuda_stream` may be NULL
  * (the handle then creates its own non-blocking stream) or a cudaStream_t owned by the caller. */
 b2s_status b2s_matcher_create(const b2s_matcher_params *params, const b2s_laser *laser, int device,
                               int max_batch, int max_base_scans, void *cuda_stream, b2s_matcher **out);
@@ -353,8 +354,9 @@ b2s_status b2s_occ_grid_create_from_scans(const b2s_laser *laser, int n_scans, c
  * to size the grids, one counter arena, one ray trace over every beam of every grid, one threshold + payload pass) and
  * the payloads come back in one copy.  on_grid(user, g, info, payload [height][width] int8 as b2s_occ_grid_copy_ros)
  * is called in ascending g for every grid with scans; a grid without scans has no map (CreateFromScans returns NULL)
- * and is skipped.  Pointers are valid only during the callback.  B2S_ERR_BAD_PARAMS for NULL arrays, negative counts
- * or a zero resolution of a grid with scans. */
+ * and is skipped.  Pointers are valid only during the callback.  n_grids may be any count whose maps fit in device
+ * memory (65 535 is not a limit).  B2S_ERR_BAD_PARAMS for NULL arrays, negative counts or a zero resolution of a grid
+ * with scans. */
 typedef void (*b2s_occ_grid_batch_fn)(void *user, int32_t grid, const b2s_occ_grid_info *info, const int8_t *payload);
 b2s_status b2s_occ_grid_create_from_scans_batch(const b2s_laser *laser, int n_grids, const int32_t *n_scans,
                                                 const float *ranges, const double *poses, const double *resolution,
@@ -485,7 +487,8 @@ b2s_status b2s_hector_slam_process_stream(b2s_hector_slam *p, int n_scans, const
                                           int map_without_matching, float *out_poses, int32_t *out_map_updated,
                                           float *out_last_cov);
 /* B independent HectorSlamProcessors (robots / maps) behind one handle (SURVEY.md §8(e): Hector maps shard over
- * independent maps, not within one).  max_points = capacity of one scan (<= 4096). */
+ * independent maps, not within one).  batch may be any count >= 1 whose maps fit in device memory (65 535 is not a
+ * limit).  max_points = capacity of one scan (<= 4096). */
 b2s_status b2s_hector_slam_create_batch(int batch, int max_points, float map_resolution, int map_size_x, int map_size_y,
                                         float start_x, float start_y, int levels, int device, void *cuda_stream,
                                         b2s_hector_slam **out);
