@@ -1,7 +1,7 @@
 // lesson4's HectorMappingRos node (lesson4/src/hector_mapping/hector_slam.cc) over whole recordings, B nodes per handle:
-// host C++ around the device batched HectorSlamProcessor (hector_slam.cu), one processor per node, whose ingest kernel
-// k_hs_stream_batch<true, true> converts (hector_scan.cuh, with each node's own filter) and matches every node's scans,
-// one CTA per node.  The publish schedule and the launch parts are hector_node_plan.cuh's; the single-node entry points
+// host C++ around the device fleet of HectorSlamProcessors (hector_slam.cu), one processor per node with its own map
+// settings, whose ingest kernel k_hs_stream_batch<true, true> converts (hector_scan.cuh, with each node's own laser and
+// filter) and matches every node's scans, one CTA per node.  The publish schedule and the launch parts are hector_node_plan.cuh's; the single-node entry points
 // are the batched ones with B = 1.
 //   HectorMappingRos::InitParams / constructor       hector_slam.cc:26-105, 119-162
 //   HectorMappingRos::setMapInfo                     :165-180
@@ -14,8 +14,10 @@
 #include <cstring>
 #include <functional>
 #include <memory>
+#include <map>
 #include <new>
 #include <string>
+#include <tuple>
 #include <vector>
 
 #include "common.cuh"
@@ -25,11 +27,13 @@
 
 namespace b2s {
 // hector_slam.cu
-void hs_node_map_info(const b2s_hector_slam *p, float &origin_x, float &origin_y, float &cell_length, int &w, int &h);
-float hs_scale_to_map(const b2s_hector_slam *p);
-b2s_status hs_node_run(b2s_hector_slam *p, HsNodeIo &io, const b2s_laser_scan_msg &geometry, const double *units,
-                       double range_cutoff, const HectorBeamFilter *filters, const HectorNodePlan &plan,
-                       const int32_t *n_scans, const float *ranges, float *out_rows,
+void hs_node_map_info(const b2s_hector_slam *p, int b, float &origin_x, float &origin_y, float &cell_length, int &w, int &h);
+float hs_scale_to_map(const b2s_hector_slam *p, int b);
+const char *hs_spec_error(const b2s_hector_map_spec &s);
+b2s_hector_map_spec hs_default_spec(float map_resolution, int map_size_x, int map_size_y, float start_x, float start_y,
+                                    int levels);
+b2s_status hs_node_run(b2s_hector_slam *p, HsNodeIo &io, const HsLaser *lasers, const double *units, size_t n_units,
+                       const HectorNodePlan &plan, const int32_t *n_scans, const float *ranges, float *out_rows,
                        const std::function<b2s_status(int, int, const int8_t *, const float *, long long)> &on_map);
 }  // namespace b2s
 
@@ -45,18 +49,16 @@ constexpr int64_t NS = 1000000000LL;
 // B nodes, one per processor of a batched HectorSlamProcessor; per-node state is indexed by node
 struct b2s_hector_node {
   int batch = 1;
-  b2s_laser_scan_msg geom{};
   int device = 0;
   b2s_hector_slam *proc = nullptr;
-  std::vector<HectorBeamFilter> filters;
-  double cutoff = 30.0;  // projector_.projectLaser(scan, laser_point_cloud_, 30.0)
-  std::vector<double> units;
+  std::vector<HsLaser> lasers;  // node b's laser and filter (base: set per call)
+  std::vector<double> units;    // the unit vectors of every distinct geometry ([n][2] each; HsLaser::unit0)
   std::vector<int64_t> period_ns;       // Duration::fromSec(map_pub_period)
   std::vector<HectorNodeClock> clock;   // the publish schedule (started, next tick)
   std::vector<int64_t> scans;           // scans handed in so far
   std::vector<int64_t> updates;         // map updates so far: level 0's getUpdateIndex() = updates - 1
   std::vector<int64_t> last_get_map_update_index;  // lastGetMapUpdateIndex
-  b2s_hector_node_map_info info{};
+  std::vector<b2s_hector_node_map_info> info;  // node b's setMapInfo
   HsNodeIo io;
   std::vector<float> rows;
   std::vector<int8_t> payload;      // b2s_hector_node_publish_map_of's
@@ -73,7 +75,7 @@ int32_t map_gate(b2s_hector_node *n, int b, int64_t updates) {
   return rebuilt ? 1 : 0;
 }
 
-// the fields the batched processor holds once (HsBatch): equal in every node's parameters
+// the processor's fields (b2s_hector_node_create_batch requires them equal in every node's parameters)
 bool same_processor(const b2s_hector_node_params &a, const b2s_hector_node_params &b) {
   return a.map_resolution == b.map_resolution && a.map_size == b.map_size &&
          a.map_multi_res_levels == b.map_multi_res_levels && a.map_start_x == b.map_start_x &&
@@ -94,63 +96,63 @@ void single_map(void *user, int32_t, int32_t scan_index, const uint32_t stamp[2]
   if (s->fn) s->fn(s->user, scan_index, stamp, info, payload, rebuilt);
 }
 
-}  // namespace
+// Node b's processor: HectorSlamProcessor(static_cast<float>(resolution), size, size, Vector2f(start), levels) + the
+// setters of the constructor
+b2s_hector_map_spec node_spec(const b2s_hector_node_params &p) {
+  b2s_hector_map_spec s = hs_default_spec(static_cast<float>(p.map_resolution), p.map_size, p.map_size,
+                                          static_cast<float>(p.map_start_x), static_cast<float>(p.map_start_y),
+                                          p.map_multi_res_levels);
+  s.update_free = static_cast<float>(p.update_factor_free);
+  s.update_occupied = static_cast<float>(p.update_factor_occupied);
+  s.min_dist = static_cast<float>(p.map_update_distance_thresh);
+  s.min_angle = static_cast<float>(p.map_update_angle_thresh);
+  return s;
+}
 
-extern "C" {
-
-b2s_status b2s_hector_node_create_batch(int batch, const b2s_hector_node_params *params,
-                                        const b2s_laser_scan_msg *geometry, const double *laser_mounts, int device,
-                                        b2s_hector_node **out) {
-  if (!out) B2S_FAIL(B2S_ERR_BAD_PARAMS, "b2s_hector_node_create: null argument");
+// The fleet behind every create entry point: node b's geometry is geometries[b * geometry_stride] (stride 0: one
+// geometry for all).  `api` names the entry point in refusals, with the node when there are several.
+b2s_status node_create(int batch, const b2s_hector_node_params *params, const b2s_laser_scan_msg *geometries,
+                       int geometry_stride, const double *laser_mounts, int device, b2s_hector_node **out,
+                       const char *api) {
+  if (!out) B2S_FAIL(B2S_ERR_BAD_PARAMS, std::string(api) + ": null argument");
   *out = nullptr;
-  if (!params || !geometry || !laser_mounts) B2S_FAIL(B2S_ERR_BAD_PARAMS, "b2s_hector_node_create: null argument");
-  if (batch < 1) B2S_FAIL(B2S_ERR_BAD_PARAMS, "b2s_hector_node_create_batch: batch must be positive");
-  if (batch > NODE_MAX_BATCH) B2S_FAIL(B2S_ERR_TOO_LARGE, "b2s_hector_node_create_batch: at most 65535 nodes");
+  if (!params || !geometries || !laser_mounts) B2S_FAIL(B2S_ERR_BAD_PARAMS, std::string(api) + ": null argument");
+  if (batch < 1) B2S_FAIL(B2S_ERR_BAD_PARAMS, std::string(api) + ": batch must be positive");
+  if (batch > NODE_MAX_BATCH) B2S_FAIL(B2S_ERR_TOO_LARGE, std::string(api) + ": at most 65535 nodes");
+  auto who = [&](int b) {
+    return batch > 1 ? std::string(api) + ": node " + std::to_string(b) + ": " : std::string(api) + ": ";
+  };
   std::vector<int64_t> period_ns((size_t)batch);
+  std::vector<b2s_hector_map_spec> specs((size_t)batch);
+  int most_ranges = 1;
   for (int b = 0; b < batch; b++) {
     const b2s_hector_node_params &pb = params[b];
+    const b2s_laser_scan_msg &g = geometries[(size_t)b * geometry_stride];
     const double *mount = laser_mounts + 7 * (size_t)b;
-    const std::string who = batch > 1 ? "b2s_hector_node_create_batch: node " + std::to_string(b) + ": "
-                                      : std::string("b2s_hector_node_create: ");
-    if (!same_processor(pb, params[0]))
-      B2S_FAIL(B2S_ERR_BAD_PARAMS, who + "the processor's fields (map size, resolution, levels, start, update factors, "
-                                         "update thresholds) differ from node 0's");
     const float res = static_cast<float>(pb.map_resolution);
-    if (!(res > 0.0f) || !std::isfinite(res)) B2S_FAIL(B2S_ERR_BAD_PARAMS, who + "map_resolution must be positive");
-    if (pb.map_size <= 0) B2S_FAIL(B2S_ERR_BAD_PARAMS, who + "map_size must be positive");
+    if (!(res > 0.0f) || !std::isfinite(res)) B2S_FAIL(B2S_ERR_BAD_PARAMS, who(b) + "map_resolution must be positive");
+    if (pb.map_size <= 0) B2S_FAIL(B2S_ERR_BAD_PARAMS, who(b) + "map_size must be positive");
+    specs[(size_t)b] = node_spec(pb);
+    if (const char *e = hs_spec_error(specs[(size_t)b])) B2S_FAIL(B2S_ERR_BAD_PARAMS, who(b) + e);
     const double period = pb.map_pub_period;
     if (!(period > 0.0) || !std::isfinite(period) || std::floor(period) > 2147483647.0)
-      B2S_FAIL(B2S_ERR_BAD_PARAMS, who + "map_pub_period must be positive, finite and inside ros::Duration's range");
+      B2S_FAIL(B2S_ERR_BAD_PARAMS, who(b) + "map_pub_period must be positive, finite and inside ros::Duration's range");
     const RosDuration d = ros_duration_from_sec(period);
     period_ns[(size_t)b] = (int64_t)d.sec * NS + (int64_t)d.nsec;
-    if (period_ns[(size_t)b] <= 0) B2S_FAIL(B2S_ERR_BAD_PARAMS, who + "map_pub_period rounds to a zero ros::Duration");
+    if (period_ns[(size_t)b] <= 0) B2S_FAIL(B2S_ERR_BAD_PARAMS, who(b) + "map_pub_period rounds to a zero ros::Duration");
     double qn = 0.0;
     for (int k = 0; k < 7; k++)
-      if (!std::isfinite(mount[k])) B2S_FAIL(B2S_ERR_BAD_PARAMS, who + "non-finite laser mount");
+      if (!std::isfinite(mount[k])) B2S_FAIL(B2S_ERR_BAD_PARAMS, who(b) + "non-finite laser mount");
     for (int k = 3; k < 7; k++) qn += mount[k] * mount[k];
-    if (!(qn > 0.0)) B2S_FAIL(B2S_ERR_BAD_PARAMS, who + "zero mount quaternion");
+    if (!(qn > 0.0)) B2S_FAIL(B2S_ERR_BAD_PARAMS, who(b) + "zero mount quaternion");
+    if (g.angle_increment == 0.0f || g.n_ranges < 0)
+      B2S_FAIL(B2S_ERR_BAD_PARAMS, who(b) + "zero angle_increment or negative n_ranges");
+    if (g.n_ranges > NODE_MAX_RANGES) B2S_FAIL(B2S_ERR_TOO_LARGE, who(b) + "at most 4096 ranges per scan");
+    most_ranges = std::max(most_ranges, (int)g.n_ranges);
   }
-  if (geometry->angle_increment == 0.0f || geometry->n_ranges < 0)
-    B2S_FAIL(B2S_ERR_BAD_PARAMS, "b2s_hector_node_create: zero angle_increment or negative n_ranges");
-  if (geometry->n_ranges > NODE_MAX_RANGES) B2S_FAIL(B2S_ERR_TOO_LARGE, "b2s_hector_node_create: at most 4096 ranges per scan");
 
-  // the constructor: HectorSlamProcessor(static_cast<float>(resolution), size, size, Vector2f(start), levels) + setters
-  const b2s_hector_node_params &p0 = params[0];
   b2s_hector_slam *proc = nullptr;
-  if (b2s_status st = b2s_hector_slam_create_batch(batch, std::max(geometry->n_ranges, 1),
-                                                   static_cast<float>(p0.map_resolution), p0.map_size, p0.map_size,
-                                                   static_cast<float>(p0.map_start_x), static_cast<float>(p0.map_start_y),
-                                                   p0.map_multi_res_levels, device, nullptr, &proc))
-    return st;
-  b2s_status st = b2s_hector_slam_set_update_factors(proc, static_cast<float>(p0.update_factor_free),
-                                                      static_cast<float>(p0.update_factor_occupied));
-  if (!st)
-    st = b2s_hector_slam_set_map_update_min_diff(proc, static_cast<float>(p0.map_update_distance_thresh),
-                                                 static_cast<float>(p0.map_update_angle_thresh));
-  if (st) {
-    b2s_hector_slam_destroy(proc);
-    return st;
-  }
+  if (b2s_status st = b2s_hector_slam_create_fleet(batch, most_ranges, specs.data(), device, nullptr, &proc)) return st;
   b2s_hector_node *n = new (std::nothrow) b2s_hector_node();
   if (!n) {
     b2s_hector_slam_destroy(proc);
@@ -158,8 +160,6 @@ b2s_status b2s_hector_node_create_batch(int batch, const b2s_hector_node_params 
   }
   std::unique_ptr<b2s_hector_node, decltype(&b2s_hector_node_destroy)> guard(n, b2s_hector_node_destroy);
   n->batch = batch;
-  n->geom = *geometry;
-  n->geom.ranges = nullptr;
   n->device = device;
   n->proc = proc;
   n->period_ns = period_ns;
@@ -167,12 +167,18 @@ b2s_status b2s_hector_node_create_batch(int batch, const b2s_hector_node_params 
   n->scans.assign((size_t)batch, 0);
   n->updates.assign((size_t)batch, 0);
   n->last_get_map_update_index.assign((size_t)batch, -100);
-  // rosPointCloudToDataContainer's settings: the thresholds as InitParams stores them, the mount's tf::Transform
-  n->filters.resize((size_t)batch);
+  n->lasers.resize((size_t)batch);
+  n->info.resize((size_t)batch);
+  // every distinct geometry's unit vectors once: (angle_min, angle_increment, n_ranges) bits -> unit0
+  std::map<std::tuple<uint32_t, uint32_t, int>, int> unit0;
   for (int b = 0; b < batch; b++) {
     const b2s_hector_node_params &pb = params[b];
+    const b2s_laser_scan_msg &g = geometries[(size_t)b * geometry_stride];
     const double *mount = laser_mounts + 7 * (size_t)b;
-    HectorBeamFilter &f = n->filters[(size_t)b];
+    HsLaser &l = n->lasers[(size_t)b];
+    std::memset(&l, 0, sizeof(l));
+    // rosPointCloudToDataContainer's settings: the thresholds as InitParams stores them, the mount's tf::Transform
+    HectorBeamFilter &f = l.filter;
     f.sqr_min = static_cast<float>(pb.laser_min_dist * pb.laser_min_dist);
     f.sqr_max = static_cast<float>(pb.laser_max_dist * pb.laser_max_dist);
     f.use_max_scan_range = pb.use_max_scan_range;
@@ -180,16 +186,29 @@ b2s_status b2s_hector_node_create_batch(int batch, const b2s_hector_node_params 
     f.mount.o[0] = mount[0]; f.mount.o[1] = mount[1]; f.mount.o[2] = mount[2];
     f.z_min = pb.laser_z_min_value;
     f.z_max = pb.laser_z_max_value;
-    f.scale_to_map = hs_scale_to_map(proc);
+    f.scale_to_map = hs_scale_to_map(proc, b);
+    l.n_ranges = g.n_ranges;
+    l.range_min = g.range_min;
+    l.range_cutoff = 30.0;  // projector_.projectLaser(scan, laser_point_cloud_, 30.0)
+    uint32_t am, ai;
+    std::memcpy(&am, &g.angle_min, 4);
+    std::memcpy(&ai, &g.angle_increment, 4);
+    const auto key = std::make_tuple(am, ai, (int)g.n_ranges);
+    auto it = unit0.find(key);
+    if (it == unit0.end()) {
+      it = unit0.emplace(key, (int)(n->units.size() / 2)).first;
+      n->units.resize(n->units.size() + 2 * (size_t)g.n_ranges);
+      hector_unit_vectors(g.angle_min, g.angle_increment, g.n_ranges, n->units.data() + 2 * (size_t)it->second);
+    }
+    l.unit0 = it->second;
+    float ox, oy, cl;
+    int w, h;
+    hs_node_map_info(proc, b, ox, oy, cl, w, h);
+    b2s_hector_node_map_info &info = n->info[(size_t)b];
+    info.origin_x = ox; info.origin_y = oy;
+    info.resolution = cl;
+    info.width = w; info.height = h;
   }
-  n->units.resize(2 * (size_t)std::max(geometry->n_ranges, 1));
-  hector_unit_vectors(geometry->angle_min, geometry->angle_increment, geometry->n_ranges, n->units.data());
-  float ox, oy, cl;
-  int w, h;
-  hs_node_map_info(proc, ox, oy, cl, w, h);
-  n->info.origin_x = ox; n->info.origin_y = oy;
-  n->info.resolution = cl;
-  n->info.width = w; n->info.height = h;
   B2S_CUDA_CHECK(cudaSetDevice(device));
   B2S_CUDA_CHECK(n->io.copy.init(nullptr));
   for (int k = 0; k < 2; k++) {
@@ -198,6 +217,32 @@ b2s_status b2s_hector_node_create_batch(int batch, const b2s_hector_node_params 
   }
   *out = guard.release();
   return B2S_OK;
+}
+
+}  // namespace
+
+extern "C" {
+
+b2s_status b2s_hector_node_create_fleet(int batch, const b2s_hector_node_params *params,
+                                        const b2s_laser_scan_msg *geometries, const double *laser_mounts, int device,
+                                        b2s_hector_node **out) {
+  return node_create(batch, params, geometries, 1, laser_mounts, device, out, "b2s_hector_node_create_fleet");
+}
+
+// the fleet with one geometry repeated, and the processor fields required equal
+b2s_status b2s_hector_node_create_batch(int batch, const b2s_hector_node_params *params,
+                                        const b2s_laser_scan_msg *geometry, const double *laser_mounts, int device,
+                                        b2s_hector_node **out) {
+  const char *api = batch == 1 ? "b2s_hector_node_create" : "b2s_hector_node_create_batch";
+  if (out && params && batch > 1 && batch <= NODE_MAX_BATCH)
+    for (int b = 1; b < batch; b++)
+      if (!same_processor(params[b], params[0])) {
+        *out = nullptr;
+        B2S_FAIL(B2S_ERR_BAD_PARAMS, std::string(api) + ": node " + std::to_string(b) +
+                                         ": the processor's fields (map size, resolution, levels, start, update "
+                                         "factors, update thresholds) differ from node 0's");
+      }
+  return node_create(batch, params, geometry, 0, laser_mounts, device, out, api);
 }
 
 b2s_status b2s_hector_node_create(const b2s_hector_node_params *params, const b2s_laser_scan_msg *geometry,
@@ -224,14 +269,15 @@ b2s_status b2s_hector_node_process_batch(b2s_hector_node *n, const int32_t *n_sc
   B2S_NVTX("HectorMappingRos::scanCallback");
   if (!n || !n_scans) B2S_FAIL(B2S_ERR_BAD_PARAMS, "b2s_hector_node_process: null argument");
   const int B = n->batch;
-  size_t T = 0;
+  size_t T = 0, floats = 0;
   bool too_many = false;
   for (int b = 0; b < B; b++) {
     if (n_scans[b] < 0) B2S_FAIL(B2S_ERR_BAD_PARAMS, "b2s_hector_node_process: negative scan count");
     T += (size_t)n_scans[b];
+    floats += (size_t)n_scans[b] * (size_t)n->lasers[(size_t)b].n_ranges;
     too_many = too_many || n_scans[b] >= NODE_MAX_SCANS;
   }
-  if (T > 0 && (!stamps || (!ranges && n->geom.n_ranges > 0)))
+  if (T > 0 && (!stamps || (!ranges && floats > 0)))
     B2S_FAIL(B2S_ERR_BAD_PARAMS, "b2s_hector_node_process: null argument");
   if (n->failed) B2S_FAIL(B2S_ERR_BAD_STATE, "b2s_hector_node_process: an earlier call failed partway; destroy the handle");
   if (too_many) B2S_FAIL(B2S_ERR_TOO_LARGE, "b2s_hector_node_process: too many scans of one node in one call (split it)");
@@ -244,11 +290,11 @@ b2s_status b2s_hector_node_process_batch(b2s_hector_node *n, const int32_t *n_sc
     const int32_t rebuilt = map_gate(n, b, updates[(size_t)b]);
     const int64_t tick = plan.ticks[(size_t)b][(size_t)k - 1];
     const uint32_t stamp[2] = {(uint32_t)(tick / NS), (uint32_t)(tick % NS)};
-    if (on_map) on_map(user, b, (int32_t)(n->scans[(size_t)b] + plan.cuts[(size_t)b][(size_t)k - 1]), stamp, &n->info,
-                       payload, rebuilt);
+    if (on_map) on_map(user, b, (int32_t)(n->scans[(size_t)b] + plan.cuts[(size_t)b][(size_t)k - 1]), stamp,
+                       &n->info[(size_t)b], payload, rebuilt);
     return B2S_OK;
   };
-  b2s_status st = hs_node_run(n->proc, n->io, n->geom, n->units.data(), n->cutoff, n->filters.data(), plan, n_scans,
+  b2s_status st = hs_node_run(n->proc, n->io, n->lasers.data(), n->units.data(), n->units.size() / 2, plan, n_scans,
                               ranges, n->rows.data(), publish);
   if (st) {
     // the processors, the maps handed out and the publish gates have moved, the schedules and the counters have not
@@ -302,10 +348,11 @@ b2s_status b2s_hector_node_publish_map_of(b2s_hector_node *n, int b, const uint3
   if (!n || !stamp) B2S_FAIL(B2S_ERR_BAD_PARAMS, "b2s_hector_node_publish_map: null argument");
   if (b < 0 || b >= n->batch) B2S_FAIL(B2S_ERR_BAD_PARAMS, "b2s_hector_node_publish_map_of: node index out of range");
   if (n->failed) B2S_FAIL(B2S_ERR_BAD_STATE, "b2s_hector_node_publish_map: an earlier call failed partway; destroy the handle");
-  n->payload.resize((size_t)n->info.width * (size_t)n->info.height);
+  const b2s_hector_node_map_info &info = n->info[(size_t)b];
+  n->payload.resize((size_t)info.width * (size_t)info.height);
   if (b2s_status st = b2s_hector_slam_copy_level_ros_of(n->proc, b, 0, n->payload.data())) return st;
   const int32_t rebuilt = map_gate(n, b, n->updates[(size_t)b]);
-  if (on_map) on_map(user, b, (int32_t)n->scans[(size_t)b], stamp, &n->info, n->payload.data(), rebuilt);
+  if (on_map) on_map(user, b, (int32_t)n->scans[(size_t)b], stamp, &info, n->payload.data(), rebuilt);
   return B2S_OK;
 }
 

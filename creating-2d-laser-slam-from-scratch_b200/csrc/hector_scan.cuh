@@ -63,13 +63,25 @@ inline HectorBeamFilter hector_scan_filter(const float laser_in_base[4], float s
   return f;
 }
 
+// One processor's laser in the batched stream kernel's ingest (hector_slam.cu: HsIngest::lasers).  Scan i (a call-wide
+// scan index) is the n_ranges floats at ranges + base + i * n_ranges.  Ranges are processor-major and ragged, so base
+// is the processor's first float minus its first scan index times n_ranges: it may be negative, the sum is not.
+struct HsLaser {
+  HectorBeamFilter filter;
+  long long base;
+  int unit0;            // the first of its n_ranges unit vectors ([n][2] double) in the call's table
+  int n_ranges;
+  float range_min;
+  double range_cutoff;  // projectLaser's cutoff (a negative one already replaced by range_max)
+};
+
 // The node handle's staging for its map publishes (hector_node.cu owns it, hs_node_run in hector_slam.cu fills it): a
 // copy stream, two slots of level-0 payloads (one per node publishing before a part) on the device and page-locked on
 // the host, and the per-scan record rows
 struct HsNodeIo {
   Stream copy;
   Buf<int8_t> d_map[2];
-  HostBuf<int8_t> h_map[2];
+  HostBuf<int8_t> h_map[2];  // a slot holds the payloads published before one part, back to back
   Event converted[2], copied[2];
   HostBuf<float> h_rows;  // [scans of the call][16], part-major: a part's rows are here once the next part's `copied` fired
 };

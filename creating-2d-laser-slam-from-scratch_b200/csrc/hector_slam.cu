@@ -17,7 +17,8 @@
 // no host round trip between scans (b2s_hector_slam_process_stream: ONE cooperative kernel walks the whole stream;
 // b2s_hector_slam_update: one launch per scan, the pose comes back through a host-mapped mailbox as soon as the match
 // is done while the map update still runs).  A handle holds B independent processors (independent robots / maps,
-// SURVEY.md §8(e): "shard over independent maps"); B = 1 is the reference's single processor.  They step together one
+// SURVEY.md §8(e): "shard over independent maps"), each with its own map layout and settings (one HsProc row of a
+// device table; b2s_hector_slam_create_fleet); B = 1 is the reference's single processor.  They step together one
 // scan each (b2s_hector_slam_update_batch: three launches per step), or each walks its own recording in ONE launch, one
 // CTA per processor (b2s_hector_slam_process_stream_batch; b2s_hector_slam_process_scans_batch takes the raw LaserScan
 // ranges and converts each scan inside that launch).
@@ -63,7 +64,7 @@ constexpr int HS_EPOCH_BITS = 20;
 constexpr unsigned HS_EPOCH_MAX = (1u << HS_EPOCH_BITS) - 1;
 constexpr int HS_STREAM_CTAS = 48;       // cooperative grid of the stream kernel (one CTA per SM, all co-resident)
 
-struct HsLevel {  // one MapRepMultiMap level, all B processors ([b][cells] planes)
+struct HsLevel {  // one MapRepMultiMap level of ONE processor: its planes, already offset into the level's pools
   float4 *quad;   // per cell (x, y): getGridProbability of the four cells (x, y), (x+1, y), (x, y+1), (x+1, y+1) — what one
                   // bilinear look-up of the matcher reads — refreshed whenever a cell's log-odds changes (the device-side
                   // form of the reference's per-scan GridMapCacheArray).  ONE 16-byte load per scan point instead of four
@@ -71,10 +72,18 @@ struct HsLevel {  // one MapRepMultiMap level, all B processors ([b][cells] plan
   float *lo;
   int32_t *ui;
   uint32_t *free_st, *occ_st;  // per-scan stamps: (epoch << 12) | (4095 - beam)
-  float *pts;                  // [b][cap][2] data container of this level (level 0: the current scan)
+  float *pts;                  // [cap][2] data container of this level (level 0: the current scan)
   int sx, sy;
   MapTransform tf;
   int iterations;  // 1 + maxIterations of MapRepMultiMap::matchData (:144-166): 1+5 on level 0, 1+3 above
+};
+
+// One processor's map layout and settings: a row of the handle's device table (HsBatch::procs).  Every kernel copies
+// its processor's row into shared memory first (hs_load_proc); levels at or above `levels` have no planes.
+struct HsProc {
+  HsLevel l[HS_L];
+  int levels;
+  float lo_free, lo_occ, min_dist, min_angle;
 };
 
 struct HsState {  // device-resident state of ONE processor
@@ -95,12 +104,20 @@ struct HsState {  // device-resident state of ONE processor
 };
 
 struct HsBatch {  // kernel parameter
-  HsLevel l[HS_L];
-  int levels, batch, cap;
-  float lo_free, lo_occ, min_dist, min_angle;
+  const HsProc *procs;  // [batch] device
+  int batch, cap;
   int exact, use_fma;
   HsState *state;  // [batch]
 };
+
+// processor b's row of the table -> `dst` (shared memory), by the whole CTA; ends with a __syncthreads
+__device__ __forceinline__ void hs_load_proc(const HsBatch &P, int b, HsProc *dst) {
+  static_assert(sizeof(HsProc) % sizeof(int) == 0, "copied as words");
+  const int *s = reinterpret_cast<const int *>(P.procs + b);
+  int *d = reinterpret_cast<int *>(dst);
+  for (int i = threadIdx.x; i < (int)(sizeof(HsProc) / sizeof(int)); i += blockDim.x) d[i] = s[i];
+  __syncthreads();
+}
 
 struct HsCall {  // one scan per processor
   const float *pts0;    // [b][pts_stride][2] level-0 points (device, or host-mapped for the per-scan call)
@@ -288,11 +305,11 @@ __host__ __device__ inline size_t hs_smem_bytes(int cap) { return hs_terms_offse
 
 // MapRepMultiMap::matchData (:144-166) on every level, coarsest first, + the gate and the update parameters of
 // HectorSlamProcessor::update (:81-108), by ONE CTA for processor b.
-// Returns the gate's verdict (map update or not).
+// Q = processor b's row of the table (shared memory).  Returns the gate's verdict (map update or not).
 // INGEST (k_hs_stream_batch<_, true>): the container's origo is the processor's own, which the host wrote into
 // st->origo[0] before the launch (hs_ingest_upload), not C's.
 template <bool EXACT, bool CLUSTER, bool INGEST = false>
-__device__ bool hs_match_cta(const HsBatch &P, const HsCall &C, int b, unsigned char *smem, HsXchg *xc = nullptr,
+__device__ bool hs_match_cta(const HsBatch &P, const HsProc &Q, const HsCall &C, int b, unsigned char *smem, HsXchg *xc = nullptr,
                              uint32_t *xc_parity = nullptr) {
   static_assert(!(EXACT && CLUSTER), "the bit-exact sums are one sequential chain: nothing to split");
   HsState *st = P.state + b;
@@ -343,7 +360,7 @@ __device__ bool hs_match_cta(const HsBatch &P, const HsCall &C, int b, unsigned 
   for (int i = tid; i < n; i += HS_THREADS) {
     const float2 p = gp[i];
     spts[i] = p;
-    reinterpret_cast<float2 *>(P.l[0].pts)[(size_t)b * P.cap + i] = p;  // level-0 container for the update passes
+    reinterpret_cast<float2 *>(Q.l[0].pts)[i] = p;  // level-0 container for the update passes
   }
   if (tid == 0) {
     const float *h = C.hints ? C.hints + 3 * row : st->last_match_pose;
@@ -354,13 +371,13 @@ __device__ bool hs_match_cta(const HsBatch &P, const HsCall &C, int b, unsigned 
   bool any = false;
   if (!C.map_without_matching && n > 0) {
     float factor = 1.0f;
-    for (int l = 1; l < P.levels; l++) factor *= 0.5f;  // static_cast<float>(1.0 / pow(2.0, l)) is exactly 2^-l
-    for (int lv = P.levels - 1; lv >= 0; lv--, factor *= 2.0f) {
-      const HsLevel &m = P.l[lv];
-      const float4 *prob = m.quad + (size_t)b * m.sx * m.sy;
+    for (int l = 1; l < Q.levels; l++) factor *= 0.5f;  // static_cast<float>(1.0 / pow(2.0, l)) is exactly 2^-l
+    for (int lv = Q.levels - 1; lv >= 0; lv--, factor *= 2.0f) {
+      const HsLevel &m = Q.l[lv];
+      const float4 *prob = m.quad;
       if (lv > 0)  // dataContainers[lv-1].setFrom(dataContainer, 2^-lv) (DataPointContainer.h:46-59): exact scaling
         for (int i = tid; i < n; i += HS_THREADS)
-          reinterpret_cast<float2 *>(m.pts)[(size_t)b * P.cap + i] = make_float2(__fmul_rn(spts[i].x, factor), __fmul_rn(spts[i].y, factor));
+          reinterpret_cast<float2 *>(m.pts)[i] = make_float2(__fmul_rn(spts[i].x, factor), __fmul_rn(spts[i].y, factor));
       if (tid == 0) {
         float e0, e1;
         get_map_coords(m.tf, world0, world1, e0, e1);
@@ -517,27 +534,27 @@ __device__ bool hs_match_cta(const HsBatch &P, const HsCall &C, int b, unsigned 
       st->n_matched = n_matched0 + 1;
       if (n > 0) {
         float factor = 1.0f;
-        for (int l = 1; l < P.levels; l++) {
+        for (int l = 1; l < Q.levels; l++) {
           factor *= 0.5f;
           st->n_pts[l] = n;
           st->origo[l][0] = origo_x * factor; st->origo[l][1] = origo_y * factor;
         }
       } else {
-        for (int l = 1; l < P.levels; l++) st->n_pts[l] = 0;  // setFrom of an empty container
+        for (int l = 1; l < Q.levels; l++) st->n_pts[l] = 0;  // setFrom of an empty container
       }
     }
     st->n_pts[0] = n;
     st->origo[0][0] = origo_x; st->origo[0][1] = origo_y;
     st->last_match_pose[0] = est[0]; st->last_match_pose[1] = est[1]; st->last_match_pose[2] = est[2];
     if (C.carry) { C.carry[0] = est[0]; C.carry[1] = est[1]; C.carry[2] = est[2]; }
-    const bool do_update = hs_pose_difference_larger_than(est, lup, P.min_dist, P.min_angle) ||
+    const bool do_update = hs_pose_difference_larger_than(est, lup, Q.min_dist, Q.min_angle) ||
                            C.map_without_matching;
     st->do_update = do_update ? 1 : 0;
     if (do_update) {
       float uc, us;  // Rotation2Df of the update transform: glibc cosf / sinf -> the same cells as the CPU
       glibc_sincosf(est[2], use_fma, &us, &uc);
-      for (int l = 0; l < P.levels; l++) {
-        const HsLevel &m = P.l[l];
+      for (int l = 0; l < Q.levels; l++) {
+        const HsLevel &m = Q.l[l];
         float mx, my;
         get_map_coords(m.tf, est[0], est[1], mx, my);
         st->uc[l] = uc; st->us[l] = us; st->umx[l] = mx; st->umy[l] = my;
@@ -571,12 +588,12 @@ __device__ bool hs_match_cta(const HsBatch &P, const HsCall &C, int b, unsigned 
     // cells the rays of this update can touch, per level: the apply pass sweeps this box instead of re-walking the rays
     if (tid < HS_L * 4) s_bb[tid >> 2][tid & 3] = (tid & 2) ? -2147483647 : 2147483647;  // {min x, min y, max x, max y}
     __syncthreads();
-    for (int lv = 0; lv < P.levels; lv++) {
-      const HsLevel &m = P.l[lv];
+    for (int lv = 0; lv < Q.levels; lv++) {
+      const HsLevel &m = Q.l[lv];
       const int nl = st->n_pts[lv];
       const float c = st->uc[lv], s = st->us[lv], mx = st->umx[lv], my = st->umy[lv];
       const int bx = st->bx[lv], by = st->by[lv];
-      const float2 *pp = reinterpret_cast<const float2 *>(m.pts) + (size_t)b * P.cap;
+      const float2 *pp = reinterpret_cast<const float2 *>(m.pts);
       int lo_x = 2147483647, lo_y = 2147483647, hi_x = -2147483647, hi_y = -2147483647;
       for (int i = tid; i < nl; i += HS_THREADS) {
         const float2 pt = pp[i];
@@ -596,7 +613,7 @@ __device__ bool hs_match_cta(const HsBatch &P, const HsCall &C, int b, unsigned 
       }
     }
     __syncthreads();
-    if (tid < P.levels) {
+    if (tid < Q.levels) {
       st->bb_x0[tid] = s_bb[tid][0]; st->bb_y0[tid] = s_bb[tid][1];
       st->bb_x1[tid] = s_bb[tid][2]; st->bb_y1[tid] = s_bb[tid][3];  // no ray: max < min -> an empty box
     }
@@ -631,7 +648,7 @@ __device__ __forceinline__ bool hs_wait_decision(const float *row, unsigned int 
 
 // A helper CTA of cluster 0 (rank >= 1): the same level / iteration loops as hs_match_cta, but only the per-point phase of
 // its share of the scan; the pose comes from the master, the nine partial sums go back to it.
-__device__ void hs_match_helper(const HsBatch &P, const HsCall &C, unsigned char *smem, HsXchg *xc, uint32_t rank,
+__device__ void hs_match_helper(const HsBatch &P, const HsProc &Q, const HsCall &C, unsigned char *smem, HsXchg *xc, uint32_t rank,
                                 uint32_t csize, uint32_t &pose_parity) {
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const int n = C.n0_uniform;
@@ -647,9 +664,9 @@ __device__ void hs_match_helper(const HsBatch &P, const HsCall &C, unsigned char
   const int pitch = hs_pitch(P.cap);
   const uint32_t r_part = hs_mapa(smem_u32(&xc->part[rank][0]), 0), r_bar = hs_mapa(smem_u32(&xc->bar_part), 0);
   float factor = 1.0f;
-  for (int l = 1; l < P.levels; l++) factor *= 0.5f;
-  for (int lv = P.levels - 1; lv >= 0; lv--, factor *= 2.0f) {
-    const HsLevel &m = P.l[lv];
+  for (int l = 1; l < Q.levels; l++) factor *= 0.5f;
+  for (int lv = Q.levels - 1; lv >= 0; lv--, factor *= 2.0f) {
+    const HsLevel &m = Q.l[lv];
     const float4 *prob = m.quad;
     for (int it = 0; it < m.iterations; it++) {
       if (tid == 0) mbar_expect_tx(&xc->bar_pose, 4u * HS_POSE_WORDS);
@@ -690,24 +707,23 @@ __device__ __forceinline__ HsUpd hs_load_upd(const HsState *st, int lv) {
 // MapRepMultiMap::updateByScan (:174-191) for processor b, PASS 1 (mark): work item = (level, beam), flattened over
 // the levels, one warp each; lanes over Bresenham steps in closed form.  Every traversed cell records the LOWEST beam
 // index that frees it / ends on it (32-bit atomicMax of epoch | ~beam).  Returns this warp's cell visits.
-__device__ unsigned long long hs_mark_pass(const HsBatch &P, int b, int w, int nw, int lane) {
+__device__ unsigned long long hs_mark_pass(const HsBatch &P, const HsProc &Q, int b, int w, int nw, int lane) {
   const HsState *st = P.state + b;
   unsigned long long my_visits = 0;
   int first[HS_L + 1];
   first[0] = 0;
-  for (int lv = 0; lv < P.levels; lv++) first[lv + 1] = first[lv] + st->n_pts[lv];
+  for (int lv = 0; lv < Q.levels; lv++) first[lv + 1] = first[lv] + st->n_pts[lv];
   int lv = 0;
   HsUpd u = hs_load_upd(st, 0);
-  for (int j = w; j < first[P.levels]; j += nw) {
+  for (int j = w; j < first[Q.levels]; j += nw) {
     if (j >= first[lv + 1]) {
       while (j >= first[lv + 1]) lv++;
       u = hs_load_upd(st, lv);
     }
     const int i = j - first[lv];
-    const HsLevel &m = P.l[lv];
-    const size_t cells = (size_t)m.sx * m.sy;
-    uint32_t *fs = m.free_st + (size_t)b * cells, *os = m.occ_st + (size_t)b * cells;
-    const float2 pt = __ldcg(reinterpret_cast<const float2 *>(m.pts) + (size_t)b * P.cap + i);
+    const HsLevel &m = Q.l[lv];
+    uint32_t *fs = m.free_st, *os = m.occ_st;
+    const float2 pt = __ldcg(reinterpret_cast<const float2 *>(m.pts) + i);
     const BresenhamLine ln = bresenham_line(u.bx, u.by, end_cell(u.c, u.s, u.mx, u.my, pt.x, pt.y), m.sx, m.sy);
     if (!ln.ok) continue;
     const uint32_t stamp = u.ehi | (uint32_t)(4095 - i);
@@ -738,11 +754,11 @@ __device__ __forceinline__ void hs_publish_prob(float4 *__restrict__ quad, int s
 // bresenhamCellOcc — with the "(v + f) - f" un-free rounding iff a LOWER beam index had freed the cell first (its
 // free stamp, same epoch, is larger) — then += logOddsOccupied if v < 50; cells only freed take bresenhamCellFree.
 // The floats are those of the sequential loop (OccGridMapBase.h:302-330), whatever the execution order.
-__device__ void hs_apply_pass(const HsBatch &P, int b, int w, int nw, int lane) {
+__device__ void hs_apply_pass(const HsBatch &P, const HsProc &Q, int b, int w, int nw, int lane) {
   const HsState *st = P.state + b;
   int first[HS_L + 1], x0[HS_L], y0[HS_L], x1[HS_L], chunks[HS_L];
   first[0] = 0;
-  for (int lv = 0; lv < P.levels; lv++) {
+  for (int lv = 0; lv < Q.levels; lv++) {
     x0[lv] = st->bb_x0[lv]; y0[lv] = st->bb_y0[lv];
     x1[lv] = st->bb_x1[lv];
     const int y1 = st->bb_y1[lv];
@@ -751,14 +767,13 @@ __device__ void hs_apply_pass(const HsBatch &P, int b, int w, int nw, int lane) 
     first[lv + 1] = first[lv] + (any ? (y1 - y0[lv] + 1) * chunks[lv] : 0);
   }
   int lv = 0;
-  for (int j = w; j < first[P.levels]; j += nw) {
+  for (int j = w; j < first[Q.levels]; j += nw) {
     while (j >= first[lv + 1]) lv++;
-    const HsLevel &m = P.l[lv];
-    const size_t cells = (size_t)m.sx * m.sy;
-    const uint32_t *fs = m.free_st + (size_t)b * cells, *os = m.occ_st + (size_t)b * cells;
-    float *lo = m.lo + (size_t)b * cells;
-    float4 *quad = m.quad + (size_t)b * cells;
-    int32_t *ui = m.ui + (size_t)b * cells;
+    const HsLevel &m = Q.l[lv];
+    const uint32_t *fs = m.free_st, *os = m.occ_st;
+    float *lo = m.lo;
+    float4 *quad = m.quad;
+    int32_t *ui = m.ui;
     const uint32_t ep = st->epoch_hi[lv] >> 12;
     const int mark_free = st->mark_free[lv], mark_occ = st->mark_occ[lv];
     const int r = j - first[lv];
@@ -780,15 +795,15 @@ __device__ void hs_apply_pass(const HsBatch &P, int b, int w, int nw, int lane) 
       if (o[q] != 0 && (o[q] >> 12) == ep) {  // bresenhamCellOcc (:315-330)
         float v = __ldcg(lo + off);
         if ((f[q] >> 12) == ep && f[q] > o[q]) {  // a lower beam index freed it first: set free, then unset
-          v = __fadd_rn(v, P.lo_free);
-          v = __fsub_rn(v, P.lo_free);
+          v = __fadd_rn(v, Q.lo_free);
+          v = __fsub_rn(v, Q.lo_free);
         }
-        if (v < 50.0f) v = __fadd_rn(v, P.lo_occ);
+        if (v < 50.0f) v = __fadd_rn(v, Q.lo_occ);
         lo[off] = v;
         hs_publish_prob(quad, m.sx, xb + 32 * q, y, log_odds_prob(v));
         ui[off] = mark_occ;
       } else if (f[q] != 0 && (f[q] >> 12) == ep) {  // bresenhamCellFree (:302-312)
-        const float v = __fadd_rn(__ldcg(lo + off), P.lo_free);
+        const float v = __fadd_rn(__ldcg(lo + off), Q.lo_free);
         lo[off] = v;
         hs_publish_prob(quad, m.sx, xb + 32 * q, y, log_odds_prob(v));
         ui[off] = mark_free;
@@ -803,21 +818,29 @@ __device__ void hs_apply_pass(const HsBatch &P, int b, int w, int nw, int lane) 
 template <bool EXACT>
 __global__ void __launch_bounds__(HS_THREADS, 1) k_hs_match(HsBatch P, HsCall C) {
   extern __shared__ __align__(16) unsigned char hs_smem[];
-  hs_match_cta<EXACT, false>(P, C, blockIdx.x, hs_smem);
+  __shared__ HsProc s_proc;
+  hs_load_proc(P, blockIdx.x, &s_proc);
+  hs_match_cta<EXACT, false>(P, s_proc, C, blockIdx.x, hs_smem);
 }
 // processors b = blockIdx.y, + gridDim.y, ... (grid_rows(batch) rows)
 __global__ void __launch_bounds__(256) k_hs_mark(HsBatch P) {
+  __shared__ HsProc s_proc;
   for (int b = blockIdx.y; b < P.batch; b += gridDim.y) {
     if (!P.state[b].do_update) continue;
+    hs_load_proc(P, b, &s_proc);
     const int lane = threadIdx.x & 31;
-    const unsigned long long v = hs_mark_pass(P, b, (blockIdx.x * blockDim.x + threadIdx.x) >> 5, (gridDim.x * blockDim.x) >> 5, lane);
+    const unsigned long long v = hs_mark_pass(P, s_proc, b, (blockIdx.x * blockDim.x + threadIdx.x) >> 5, (gridDim.x * blockDim.x) >> 5, lane);
     if (lane == 0 && v) atomicAdd(&P.state[b].visits, v);  // lane 0 carries the warp's count
+    __syncthreads();  // s_proc is rewritten for the next processor
   }
 }
 __global__ void __launch_bounds__(256) k_hs_apply(HsBatch P) {
+  __shared__ HsProc s_proc;
   for (int b = blockIdx.y; b < P.batch; b += gridDim.y) {
     if (!P.state[b].do_update) continue;
-    hs_apply_pass(P, b, (blockIdx.x * blockDim.x + threadIdx.x) >> 5, (gridDim.x * blockDim.x) >> 5, threadIdx.x & 31);
+    hs_load_proc(P, b, &s_proc);
+    hs_apply_pass(P, s_proc, b, (blockIdx.x * blockDim.x + threadIdx.x) >> 5, (gridDim.x * blockDim.x) >> 5, threadIdx.x & 31);
+    __syncthreads();
   }
 }
 
@@ -862,6 +885,8 @@ __global__ void __launch_bounds__(HS_THREADS, 1) k_hs_stream(HsBatch P, HsStream
   extern __shared__ __align__(16) unsigned char hs_smem[];
   __shared__ HsXchg xc;  // same offset in every CTA of the kernel: mapa() of a local address names the peer's copy
   __shared__ int s_flag;
+  __shared__ HsProc s_proc;
+  hs_load_proc(P, 0, &s_proc);
   uint32_t crank = 0, csize = 1, pose_parity = 0, part_parity = 0;
   if (CLUSTER) {
     crank = hs_cluster_rank();
@@ -904,17 +929,17 @@ __global__ void __launch_bounds__(HS_THREADS, 1) k_hs_stream(HsBatch P, HsStream
     // goes on to the next scan; the other CTAs follow the verdicts and meet it at the update's barriers.  (A grid barrier
     // per scan cost the matching CTA ~1 us: two fences and an L2 round trip.)
     if (blockIdx.x == 0) {
-      update = hs_match_cta<EXACT, CLUSTER>(P, C, 0, hs_smem, &xc, &part_parity);
+      update = hs_match_cta<EXACT, CLUSTER>(P, s_proc, C, 0, hs_smem, &xc, &part_parity);
     } else {
-      if (helper) hs_match_helper(P, C, hs_smem, &xc, crank, csize, pose_parity);
+      if (helper) hs_match_helper(P, s_proc, C, hs_smem, &xc, crank, csize, pose_parity);
       update = hs_wait_decision(C.out, S.tag, &s_flag);
     }
     if (update) {
       const unsigned long long t0 = hs_now_ns();
-      const unsigned long long v = hs_mark_pass(P, 0, w, nw, lane);
+      const unsigned long long v = hs_mark_pass(P, s_proc, 0, w, nw, lane);
       if (lane == 0 && v) atomicAdd(&st->visits, v);
       hs_grid_barrier(S.barrier, generation);
-      hs_apply_pass(P, 0, w, nw, lane);
+      hs_apply_pass(P, s_proc, 0, w, nw, lane);
       hs_grid_barrier(S.barrier, generation);  // the next match reads the refreshed probability planes
       if (blockIdx.x == 0 && threadIdx.x == 0) st->t_update_ns = hs_now_ns() - t0;
     }
@@ -939,12 +964,9 @@ struct HsFleet {
 // Scans as raw LaserScan ranges (k_hs_stream_batch<_, true>): F.pts / offsets / counts are unused.  In device memory
 // behind one pointer: a larger kernel parameter block costs the point-stream instantiations registers.
 struct HsIngest {
-  const float *ranges;       // [total scans][n_ranges] float32
-  const double2 *units;      // [n_ranges] the beams' unit vectors (host C library cos / sin)
-  int n_ranges;
-  float range_min;
-  double range_cutoff;       // projectLaser's cutoff (a negative one already replaced by range_max)
-  const HectorBeamFilter *filters;  // [B] processor b's conversion
+  const float *ranges;       // every scan's ranges, float32 (HsLaser::base)
+  const double2 *units;      // the beams' unit vectors (host C library cos / sin), per laser (HsLaser::unit0)
+  const HsLaser *lasers;     // [B]
 };
 
 // The loop of processor b = blockIdx.x over its scans: match (hs_match_cta), then, if the gate opens, the mark and
@@ -967,6 +989,8 @@ __global__ void __launch_bounds__(HS_THREADS, 1) k_hs_stream_batch(HsBatch P, Hs
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   constexpr int NW = HS_THREADS / 32;
   HsState *st = P.state + b;
+  __shared__ HsProc s_proc;
+  hs_load_proc(P, b, &s_proc);
   const long long s0 = F.first[2 * b], s1 = F.first[2 * b + 1];
   unsigned long long visits = 0;
   for (long long i = s0; i < s1; i++) {
@@ -974,17 +998,19 @@ __global__ void __launch_bounds__(HS_THREADS, 1) k_hs_stream_batch(HsBatch P, Hs
     if constexpr (INGEST) {
       __shared__ int s_warp_kept[NW];
       const HsIngest &I = *F.ingest;
-      float2 *row = reinterpret_cast<float2 *>(P.l[0].pts) + (size_t)b * P.cap;
-      const int nr = I.n_ranges;
-      const float *r = I.ranges + (size_t)i * nr;
+      const HsLaser &las = I.lasers[b];
+      float2 *row = reinterpret_cast<float2 *>(s_proc.l[0].pts);
+      const int nr = las.n_ranges;
+      const float *r = I.ranges + (las.base + i * nr);
+      const double2 *units = I.units + las.unit0;
       int base = 0;
       for (int c0 = 0; c0 < nr; c0 += HS_THREADS) {
         const int j = c0 + (int)threadIdx.x;
         float2 q = make_float2(0.0f, 0.0f);
         bool keep = false;
         if (j < nr) {
-          const double2 u = I.units[j];
-          keep = hector_node_beam(I.filters[b], r[j], u.x, u.y, I.range_cutoff, I.range_min, q.x, q.y);
+          const double2 u = units[j];
+          keep = hector_node_beam(las.filter, r[j], u.x, u.y, las.range_cutoff, las.range_min, q.x, q.y);
         }
         const unsigned m = __ballot_sync(0xffffffffu, keep);
         if (lane == 0) s_warp_kept[warp] = __popc(m);
@@ -1001,7 +1027,7 @@ __global__ void __launch_bounds__(HS_THREADS, 1) k_hs_stream_batch(HsBatch P, Hs
         __syncthreads();  // s_warp_kept is rewritten by the next round; the row is read by the match
       }
       if (threadIdx.x == 0) F.out[16 * i + 15] = __int_as_float(base);  // the scan's kept-beam count for the host
-      C.pts0 = P.l[0].pts + 2 * (size_t)b * P.cap;
+      C.pts0 = s_proc.l[0].pts;
       C.n0 = nullptr;
       C.n0_uniform = base;
     } else {
@@ -1019,11 +1045,11 @@ __global__ void __launch_bounds__(HS_THREADS, 1) k_hs_stream_batch(HsBatch P, Hs
     C.tag = 0;
     C.carry = s_last;
     C.own_row = 1;
-    if (hs_match_cta<EXACT, false, INGEST>(P, C, b, hs_smem)) {
+    if (hs_match_cta<EXACT, false, INGEST>(P, s_proc, C, b, hs_smem)) {
       const unsigned long long t0 = hs_now_ns();
-      visits += hs_mark_pass(P, b, warp, NW, lane);  // (lane 0 carries the warp's count)
+      visits += hs_mark_pass(P, s_proc, b, warp, NW, lane);  // (lane 0 carries the warp's count)
       __syncthreads();
-      hs_apply_pass(P, b, warp, NW, lane);
+      hs_apply_pass(P, s_proc, b, warp, NW, lane);
       __syncthreads();  // the next match reads the refreshed quads; the next gate rewrites the update parameters
       if (threadIdx.x == 0) st->t_update_ns = hs_now_ns() - t0;
     }
@@ -1064,15 +1090,18 @@ __global__ void k_hs_epoch_reset(HsState *st, int batch) {
 struct b2s_hector_slam {
   Stream stream;
   int device = 0;
-  int levels = 0, batch = 1, cap = 0;
-  int sx[HS_L] = {}, sy[HS_L] = {};
-  float cell_length[HS_L] = {};
-  HsBatch P;  // its level pointers view level_mem
-  struct {
+  int levels = 0;  // the most levels of any processor
+  int batch = 1, cap = 0;
+  std::vector<b2s_hector_map_spec> specs;  // [batch]
+  std::vector<HsProc> procs;               // [batch] the host copy of the device table P.procs
+  Buf<HsProc> d_procs;
+  HsBatch P;
+  struct {  // level l's pools: the planes of every processor with more than l levels, back to back
     Buf<float4> quad;
     Buf<float> lo, pts;
     Buf<int32_t> ui;
     Buf<uint32_t> free_st, occ_st;
+    size_t cells = 0;
   } level_mem[HS_L];
   Buf<HsState> d_state;
   Buf<float> d_out;                // [batch][16] (per-scan / batch calls)
@@ -1095,13 +1124,13 @@ extern "C" void b2s_hector_slam_destroy(b2s_hector_slam *p);
 
 static b2s_status hs_clear_maps(b2s_hector_slam *p) {  // GridMapBase::reset -> clear(): resetGridCell on every cell (:93-113)
   for (int l = 0; l < p->levels; l++) {
-    const HsLevel &m = p->P.l[l];
-    const size_t cells = (size_t)m.sx * m.sy * p->batch;
+    const auto &m = p->level_mem[l];
+    const size_t cells = m.cells;
     B2S_CUDA_CHECK(cudaMemsetAsync(m.lo, 0, cells * 4, p->stream));       // logOdds 0
     B2S_CUDA_CHECK(cudaMemsetAsync(m.ui, 0xff, cells * 4, p->stream));    // updateIndex -1
     B2S_CUDA_CHECK(cudaMemsetAsync(m.free_st, 0, cells * 4, p->stream));
     B2S_CUDA_CHECK(cudaMemsetAsync(m.occ_st, 0, cells * 4, p->stream));
-    k_hs_fill<<<ceil_div((long long)cells * 4, 256), 256, 0, p->stream>>>(reinterpret_cast<float *>(m.quad), cells * 4, 0.5f);  // e^0 / (e^0 + 1)
+    k_hs_fill<<<ceil_div((long long)cells * 4, 256), 256, 0, p->stream>>>(reinterpret_cast<float *>(m.quad.p), cells * 4, 0.5f);  // e^0 / (e^0 + 1)
   }
   B2S_CUDA_CHECK(cudaGetLastError());
   return B2S_OK;
@@ -1116,10 +1145,9 @@ static b2s_status hs_reserve_epochs(b2s_hector_slam *p, unsigned long long n_upd
   }
   if (n_updates >= HS_EPOCH_MAX) B2S_FAIL(B2S_ERR_TOO_LARGE, "too many scans in one call (stamp epochs are 20 bits)");
   for (int l = 0; l < p->levels; l++) {
-    const HsLevel &m = p->P.l[l];
-    const size_t cells = (size_t)m.sx * m.sy * p->batch;
-    B2S_CUDA_CHECK(cudaMemsetAsync(m.free_st, 0, cells * 4, p->stream));
-    B2S_CUDA_CHECK(cudaMemsetAsync(m.occ_st, 0, cells * 4, p->stream));
+    const auto &m = p->level_mem[l];
+    B2S_CUDA_CHECK(cudaMemsetAsync(m.free_st, 0, m.cells * 4, p->stream));
+    B2S_CUDA_CHECK(cudaMemsetAsync(m.occ_st, 0, m.cells * 4, p->stream));
   }
   k_hs_epoch_reset<<<ceil_div(p->batch, 128), 128, 0, p->stream>>>(p->d_state, p->batch);
   B2S_CUDA_CHECK(cudaGetLastError());
@@ -1127,52 +1155,121 @@ static b2s_status hs_reserve_epochs(b2s_hector_slam *p, unsigned long long n_upd
   return B2S_OK;
 }
 
-static b2s_status hs_create(float map_resolution, int map_size_x, int map_size_y, float start_x, float start_y, int levels,
-                            int batch, int max_points, int device, void *cuda_stream, b2s_hector_slam **out) {
-  if (!out || levels < 1 || levels > B2S_HECTOR_MAX_LEVELS || !(map_resolution > 0.0f) || (map_size_x >> (levels - 1)) <= 2 ||
-      (map_size_y >> (levels - 1)) <= 2 || batch < 1 || max_points < 1)
-    B2S_FAIL(B2S_ERR_BAD_PARAMS, "b2s_hector_slam_create: bad levels / size / resolution / batch");
+// the handle's table (p->procs) -> the device, in stream order: the next launch on the stream reads it
+static b2s_status hs_upload_procs(b2s_hector_slam *p) {
+  B2S_CUDA_CHECK(cudaSetDevice(p->device));
+  B2S_CUDA_CHECK(cudaMemcpyAsync(p->d_procs, p->procs.data(), sizeof(HsProc) * p->procs.size(), cudaMemcpyHostToDevice,
+                                 p->stream));  // (pageable source: staged before the call returns)
+  return B2S_OK;
+}
+
+namespace b2s {
+
+// why HectorSlamProcessor's constructor arguments in `s` are refused, or NULL (the checks of b2s_hector_slam_create):
+// levels 1 ... 8, a positive resolution, and more than 2 cells each way on the coarsest level
+const char *hs_spec_error(const b2s_hector_map_spec &s) {
+  if (s.levels < 1 || s.levels > B2S_HECTOR_MAX_LEVELS) return "levels must be 1 ... 8";
+  if (!(s.map_resolution > 0.0f)) return "map_resolution must be positive";
+  if ((s.map_size_x >> (s.levels - 1)) <= 2 || (s.map_size_y >> (s.levels - 1)) <= 2)
+    return "the map size leaves 2 cells or fewer on the coarsest level";
+  return nullptr;
+}
+
+// b2s_hector_slam_create's processor with the constructor's update factors and map-update gate
+b2s_hector_map_spec hs_default_spec(float map_resolution, int map_size_x, int map_size_y, float start_x, float start_y,
+                                    int levels) {
+  b2s_hector_map_spec s;
+  std::memset(&s, 0, sizeof(s));
+  s.map_resolution = map_resolution;
+  s.map_size_x = map_size_x; s.map_size_y = map_size_y;
+  s.start_x = start_x; s.start_y = start_y;
+  s.levels = levels;
+  s.update_free = 0.4f; s.update_occupied = 0.6f;  // GridMapLogOdds.h:98-102
+  s.min_dist = 0.4f; s.min_angle = 0.13f;          // HectorSlamProcessor.h:63-64
+  return s;
+}
+
+}  // namespace b2s
+
+// cell length of a processor's level: the resolution doubled per level (MapRepMultiMap.h:56-89)
+static float hs_cell_length(const b2s_hector_map_spec &s, int level) {
+  float res = s.map_resolution;
+  for (int l = 0; l < level; l++) res *= 2.0f;
+  return res;
+}
+
+// Every spec is checked before the device is touched; `who` names the entry point in refusals.
+static b2s_status hs_create(int batch, int max_points, const b2s_hector_map_spec *specs, int device, void *cuda_stream,
+                            b2s_hector_slam **out, const char *who) {
+  if (!out || !specs || batch < 1 || max_points < 1)
+    B2S_FAIL(B2S_ERR_BAD_PARAMS, std::string(who) + ": null argument or bad batch / max_points");
   *out = nullptr;
+  for (int b = 0; b < batch; b++)
+    if (const char *e = hs_spec_error(specs[b]))
+      B2S_FAIL(B2S_ERR_BAD_PARAMS, std::string(who) + ": processor " + std::to_string(b) + ": " + e);
   if (max_points > HS_MAX_PTS) B2S_FAIL(B2S_ERR_TOO_LARGE, "at most 4096 points per scan");
   if (b2s_status st = open_device(device)) return st;
   std::unique_ptr<b2s_hector_slam, decltype(&b2s_hector_slam_destroy)> p(new (std::nothrow) b2s_hector_slam(), b2s_hector_slam_destroy);
   if (!p) B2S_FAIL(B2S_ERR_CUDA, "out of host memory");
   p->device = device;
-  p->levels = levels;
   p->batch = batch;
   p->cap = max_points;
+  p->specs.assign(specs, specs + batch);
+  for (int b = 0; b < batch; b++) p->levels = std::max(p->levels, (int)specs[b].levels);
   B2S_CUDA_CHECK(p->stream.init(cuda_stream));
   std::memset(&p->P, 0, sizeof(p->P));
-  p->P.levels = levels; p->P.batch = batch; p->P.cap = max_points;
-  p->P.lo_free = prob_to_log_odds(0.4f);  // GridMapLogOdds.h:98-102
-  p->P.lo_occ = prob_to_log_odds(0.6f);
-  p->P.min_dist = 0.4f; p->P.min_angle = 0.13f;  // HectorSlamProcessor.h:63-64
+  p->P.batch = batch; p->P.cap = max_points;
   p->P.exact = 1;
   const int variant = glibc_sincosf_variant_of_host();
   p->P.use_fma = variant == 0 ? 0 : 1;
-  // MapRepMultiMap ctor (MapRepMultiMap.h:56-89): one offset for every level, dims halve, cell length doubles
-  const float total_x = map_resolution * static_cast<float>(map_size_x), total_y = map_resolution * static_cast<float>(map_size_y);
-  const float off_x = total_x * start_x, off_y = total_y * start_y;
-  int sx = map_size_x, sy = map_size_y;
-  float res = map_resolution;
-  for (int l = 0; l < levels; l++) {
-    HsLevel &m = p->P.l[l];
-    m.sx = sx; m.sy = sy;
-    p->sx[l] = sx; p->sy[l] = sy; p->cell_length[l] = res;
-    m.tf = map_transform(res, off_x, off_y);
-    m.iterations = 1 + (l == 0 ? 5 : 3);
-    const size_t cells = (size_t)sx * sy * batch;
+  // the pools: level l holds processor b's planes (b ascending) when b has more than l levels
+  std::vector<size_t> at((size_t)batch * HS_L, 0);  // [b][l] processor b's first cell in level l's pool
+  for (int l = 0; l < p->levels; l++) {
+    size_t cells = 0, rows = 0;
+    for (int b = 0; b < batch; b++) {
+      if (specs[b].levels <= l) continue;
+      at[(size_t)b * HS_L + l] = cells;
+      cells += (size_t)(specs[b].map_size_x >> l) * (size_t)(specs[b].map_size_y >> l);
+      rows++;
+    }
     auto &mem = p->level_mem[l];
+    mem.cells = cells;
     B2S_CUDA_CHECK(mem.lo.reserve(cells));
     B2S_CUDA_CHECK(mem.ui.reserve(cells));
     B2S_CUDA_CHECK(mem.free_st.reserve(cells));
     B2S_CUDA_CHECK(mem.occ_st.reserve(cells));
     B2S_CUDA_CHECK(mem.quad.reserve(cells));
-    B2S_CUDA_CHECK(mem.pts.reserve(2 * (size_t)max_points * batch));
-    m.lo = mem.lo; m.ui = mem.ui; m.free_st = mem.free_st; m.occ_st = mem.occ_st; m.quad = mem.quad; m.pts = mem.pts;
-    sx /= 2; sy /= 2;
-    res *= 2.0f;
+    B2S_CUDA_CHECK(mem.pts.reserve(2 * (size_t)max_points * rows));
   }
+  p->procs.resize((size_t)batch);
+  size_t rows[HS_L] = {};  // container rows handed out so far, per level
+  for (int b = 0; b < batch; b++) {
+    const b2s_hector_map_spec &s = specs[b];
+    HsProc &q = p->procs[(size_t)b];
+    std::memset(&q, 0, sizeof(q));
+    q.levels = s.levels;
+    q.lo_free = prob_to_log_odds(s.update_free);
+    q.lo_occ = prob_to_log_odds(s.update_occupied);
+    q.min_dist = s.min_dist; q.min_angle = s.min_angle;
+    // MapRepMultiMap ctor (MapRepMultiMap.h:56-89): one offset for every level, dims halve, cell length doubles
+    const float total_x = s.map_resolution * static_cast<float>(s.map_size_x), total_y = s.map_resolution * static_cast<float>(s.map_size_y);
+    const float off_x = total_x * s.start_x, off_y = total_y * s.start_y;
+    for (int l = 0; l < s.levels; l++) {
+      const size_t row = rows[l]++;
+      HsLevel &m = q.l[l];
+      m.sx = s.map_size_x >> l; m.sy = s.map_size_y >> l;
+      m.tf = map_transform(hs_cell_length(s, l), off_x, off_y);
+      m.iterations = 1 + (l == 0 ? 5 : 3);
+      const auto &mem = p->level_mem[l];
+      const size_t c0 = at[(size_t)b * HS_L + l];
+      m.lo = mem.lo.p + c0; m.ui = mem.ui.p + c0; m.free_st = mem.free_st.p + c0; m.occ_st = mem.occ_st.p + c0;
+      m.quad = mem.quad.p + c0;
+      m.pts = mem.pts.p + 2 * (size_t)max_points * row;
+    }
+  }
+  B2S_CUDA_CHECK(p->d_procs.reserve((size_t)batch));
+  p->P.procs = p->d_procs;
+  if (b2s_status st = hs_upload_procs(p.get())) return st;
   B2S_CUDA_CHECK(p->d_state.reserve(batch));
   p->P.state = p->d_state;
   B2S_CUDA_CHECK(p->d_out.reserve(16 * (size_t)batch));
@@ -1377,7 +1474,7 @@ static b2s_status hs_launch_step(b2s_hector_slam *p, const float *d_points, cons
 }
 
 // k_hs_stream_batch<_, true>'s input in device memory, freed in stream order with the caller: the ranges, the unit
-// vectors, and one block holding the HsIngest (`ingest`), then the B filters, then the B level-0 origos
+// vectors, and one block holding the HsIngest (`ingest`), then the B lasers, then the B level-0 origos
 struct HsIngestUpload {
   AsyncBuf<float> ranges;
   AsyncBuf<double> units;
@@ -1386,45 +1483,40 @@ struct HsIngestUpload {
   explicit HsIngestUpload(cudaStream_t s) : ranges(s), units(s), block(s) {}
 };
 
-// Uploads the call's n_scans x nr ranges, the beams' unit vectors ([nr][2]) and processor b's filter filters[b], and
+// Uploads the call's n_floats ranges, n_units unit vectors ([n_units][2]) and processor b's laser lasers[b], and
 // writes each processor's level-0 origo: dataContainer.setOrigo (hector_slam.cc:329) of its mount, the same on every
 // scan, which the ingest kernel's match reads there (hs_match_cta<_, _, true>) instead of a per-CTA value held through
 // the scan loop.  The origo of a processor without scans in the call is not read before it is written again: every
 // other match writes origo[0] before reading it, and every ingest launch follows this call's write.
-// The descriptor, the filters and the origos travel in ONE copy from pageable memory (each such copy is staged by the
+// The descriptor, the lasers and the origos travel in ONE copy from pageable memory (each such copy is staged by the
 // host before it returns, several microseconds that a call per scan pays every scan); the origos then reach the
 // processors' states by a copy on the device.
-static b2s_status hs_ingest_upload(b2s_hector_slam *p, HsIngestUpload &d, size_t n_scans, int nr, const float *ranges,
-                                   const double *units, float range_min, double range_cutoff,
-                                   const HectorBeamFilter *filters) {
-  static_assert(sizeof(HsIngest) % alignof(HectorBeamFilter) == 0 && sizeof(HectorBeamFilter) % alignof(float2) == 0,
+static b2s_status hs_ingest_upload(b2s_hector_slam *p, HsIngestUpload &d, size_t n_floats, const float *ranges,
+                                   size_t n_units, const double *units, const HsLaser *lasers) {
+  static_assert(sizeof(HsIngest) % alignof(HsLaser) == 0 && sizeof(HsLaser) % alignof(float2) == 0,
                 "the block's parts stay aligned");
   const int B = p->batch;
-  const size_t n_r = n_scans * (size_t)nr;
-  const size_t at_filters = sizeof(HsIngest), at_origo = at_filters + sizeof(HectorBeamFilter) * (size_t)B;
+  const size_t at_lasers = sizeof(HsIngest), at_origo = at_lasers + sizeof(HsLaser) * (size_t)B;
   const size_t bytes = at_origo + sizeof(float2) * (size_t)B;
-  B2S_CUDA_CHECK(d.ranges.alloc(std::max<size_t>(n_r, 1)));
-  B2S_CUDA_CHECK(d.units.alloc(2 * (size_t)std::max(nr, 1)));
+  B2S_CUDA_CHECK(d.ranges.alloc(std::max<size_t>(n_floats, 1)));
+  B2S_CUDA_CHECK(d.units.alloc(2 * std::max<size_t>(n_units, 1)));
   B2S_CUDA_CHECK(d.block.alloc(bytes));
   std::vector<unsigned char> h(bytes);
   HsIngest I;
   std::memset(&I, 0, sizeof(I));
   I.ranges = d.ranges;
   I.units = reinterpret_cast<const double2 *>(static_cast<double *>(d.units));
-  I.n_ranges = nr;
-  I.range_min = range_min;
-  I.range_cutoff = range_cutoff;
-  I.filters = reinterpret_cast<const HectorBeamFilter *>(d.block.p + at_filters);
+  I.lasers = reinterpret_cast<const HsLaser *>(d.block.p + at_lasers);
   std::memcpy(h.data(), &I, sizeof(I));
-  std::memcpy(h.data() + at_filters, filters, sizeof(HectorBeamFilter) * (size_t)B);
+  std::memcpy(h.data() + at_lasers, lasers, sizeof(HsLaser) * (size_t)B);
   for (int b = 0; b < B; b++) {
-    const float2 o = make_float2((float)filters[b].mount.o[0] * filters[b].scale_to_map,
-                                 (float)filters[b].mount.o[1] * filters[b].scale_to_map);
+    const HectorBeamFilter &f = lasers[b].filter;
+    const float2 o = make_float2((float)f.mount.o[0] * f.scale_to_map, (float)f.mount.o[1] * f.scale_to_map);
     std::memcpy(h.data() + at_origo + sizeof(float2) * (size_t)b, &o, sizeof(o));
   }
   // (pageable sources: staged before the calls return)
-  if (n_r > 0) B2S_CUDA_CHECK(cudaMemcpyAsync(d.ranges, ranges, sizeof(float) * n_r, cudaMemcpyHostToDevice, p->stream));
-  if (nr > 0) B2S_CUDA_CHECK(cudaMemcpyAsync(d.units, units, sizeof(double) * 2 * (size_t)nr, cudaMemcpyHostToDevice, p->stream));
+  if (n_floats > 0) B2S_CUDA_CHECK(cudaMemcpyAsync(d.ranges, ranges, sizeof(float) * n_floats, cudaMemcpyHostToDevice, p->stream));
+  if (n_units > 0) B2S_CUDA_CHECK(cudaMemcpyAsync(d.units, units, sizeof(double) * 2 * n_units, cudaMemcpyHostToDevice, p->stream));
   B2S_CUDA_CHECK(cudaMemcpyAsync(d.block, h.data(), bytes, cudaMemcpyHostToDevice, p->stream));
   B2S_CUDA_CHECK(cudaMemcpy2DAsync(&p->d_state.p[0].origo[0][0], sizeof(HsState), d.block.p + at_origo, sizeof(float2),
                                    sizeof(float2), (size_t)B, cudaMemcpyDeviceToDevice, p->stream));
@@ -1434,44 +1526,51 @@ static b2s_status hs_ingest_upload(b2s_hector_slam *p, HsIngestUpload &d, size_t
 
 namespace b2s {
 
-// HectorMappingRos::setMapInfo (hector_slam.cc:165-180) of level 0: getWorldCoords(0, 0) - cell length * 0.5f
-void hs_node_map_info(const b2s_hector_slam *p, float &origin_x, float &origin_y, float &cell_length, int &w, int &h) {
+// HectorMappingRos::setMapInfo (hector_slam.cc:165-180) of processor b's level 0: getWorldCoords(0, 0) - cell length * 0.5f
+void hs_node_map_info(const b2s_hector_slam *p, int b, float &origin_x, float &origin_y, float &cell_length, int &w, int &h) {
+  const HsLevel &m = p->procs[(size_t)b].l[0];
   float wx, wy;
-  get_world_coords(p->P.l[0].tf, 0.0f, 0.0f, wx, wy);
-  cell_length = p->cell_length[0];
+  get_world_coords(m.tf, 0.0f, 0.0f, wx, wy);
+  cell_length = p->specs[(size_t)b].map_resolution;
   origin_x = wx - cell_length * 0.5f;
   origin_y = wy - cell_length * 0.5f;
-  w = p->sx[0];
-  h = p->sy[0];
+  w = m.sx;
+  h = m.sy;
 }
 
-float hs_scale_to_map(const b2s_hector_slam *p) { return p->P.l[0].tf.tw_lin; }  // GridMapBase::getScaleToMap of level 0
+// GridMapBase::getScaleToMap of processor b's level 0
+float hs_scale_to_map(const b2s_hector_slam *p, int b) { return p->procs[(size_t)b].l[0].tf.tw_lin; }
 
 // ---- lesson4's HectorMappingRos (hector_node.cu): one node per processor, over one call ----
-// level 0 of the processors nodes[0 .. gridDim.y) -> their ROS payloads, back to back in `out`
-static __global__ void k_hector_ros_nodes(const float *__restrict__ lo, int cells, const int *__restrict__ nodes,
-                                          int8_t *__restrict__ out) {
+struct HsRosJob {  // one node's level-0 plane -> its ROS payload at `out` in a slot
+  const float *lo;
+  long long out;
+  int cells;
+};
+// the publishes before one part: job blockIdx.y converts its node's cells (nodes of any map size, back to back)
+static __global__ void k_hector_ros_nodes(const HsRosJob *__restrict__ jobs, int8_t *__restrict__ out) {
+  const HsRosJob J = jobs[blockIdx.y];
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= cells) return;
-  out[(size_t)blockIdx.y * cells + i] = hector_ros_cell(lo[(size_t)nodes[blockIdx.y] * cells + i]);
+  if (i >= J.cells) return;
+  out[J.out + i] = hector_ros_cell(J.lo[i]);
 }
 
 // The call runs as the plan's parts (hector_node_plan.cuh), one k_hs_stream_batch<true, true> launch of B CTAs per
 // part that has scans, CTA b on node b's scans of the part.  Before part k >= 1, one k_hector_ros_nodes launch on the
-// processor's stream converts level 0 of every node publishing there into one slot of payloads; a second stream copies
-// the slot, with those nodes' record rows of part k - 1, into page-locked memory while part k's launch runs.  Two
-// slots: a slot is handed to on_map (part by part, nodes ascending inside a part) before it is converted into again.
-// on_map(b, k, payload, rows, n) also gets node b's n record rows since its previous publish.  Rows are node-major
-// throughout.
-b2s_status hs_node_run(b2s_hector_slam *p, HsNodeIo &io, const b2s_laser_scan_msg &geometry, const double *units,
-                       double range_cutoff, const HectorBeamFilter *filters, const HectorNodePlan &plan,
-                       const int32_t *n_scans, const float *ranges, float *out_rows,
+// processor's stream converts level 0 of every node publishing there into one slot of payloads, back to back; a second
+// stream copies the slot, with those nodes' record rows of part k - 1, into page-locked memory while part k's launch
+// runs.  Two slots, each as large as the most cells published before one part: a slot is handed to on_map (part by
+// part, nodes ascending inside a part) before it is converted into again.  on_map(b, k, payload, rows, n) also gets
+// node b's n record rows since its previous publish.  Node b's scans are n_scans[b] rows of lasers[b].n_ranges floats
+// (lasers[b].base is set here), node-major; units holds every laser's unit vectors.  Rows are node-major throughout.
+b2s_status hs_node_run(b2s_hector_slam *p, HsNodeIo &io, const HsLaser *lasers, const double *units, size_t n_units,
+                       const HectorNodePlan &plan, const int32_t *n_scans, const float *ranges, float *out_rows,
                        const std::function<b2s_status(int, int, const int8_t *, const float *, long long)> &on_map) {
-  const int nr = geometry.n_ranges, B = plan.batch, K = plan.n_parts;
-  const size_t cells = (size_t)p->sx[0] * p->sy[0];
+  const int B = plan.batch, K = plan.n_parts;
   // parts [K][B] = node b's scans [first, end) of part k, node-major over the call
   std::vector<long long> parts(2 * (size_t)K * B);
-  long long first = 0;
+  std::vector<HsLaser> las(lasers, lasers + B);
+  long long first = 0, floats = 0;
   int longest = 0;
   for (int b = 0; b < B; b++) {
     for (int k = 0; k < K; k++) {
@@ -1479,40 +1578,53 @@ b2s_status hs_node_run(b2s_hector_slam *p, HsNodeIo &io, const b2s_laser_scan_ms
       parts[2 * e] = first + plan.begin[e];
       parts[2 * e + 1] = first + plan.end[e];
     }
+    las[(size_t)b].base = floats - first * las[(size_t)b].n_ranges;
     first += n_scans[b];
+    floats += (long long)n_scans[b] * las[(size_t)b].n_ranges;
     longest = std::max(longest, (int)n_scans[b]);
   }
   const size_t T = (size_t)first;
-  // the nodes publishing before part k: pub[pub0[k] .. pub0[k + 1]), those with k publishes or more, ascending
+  // the nodes publishing before part k: jobs[pub0[k] .. pub0[k + 1]) (nodes pub[...]), those with k publishes or more,
+  // ascending, each at its offset in the part's slot
   std::vector<int> pub;
+  std::vector<HsRosJob> jobs;
   std::vector<size_t> pub0((size_t)K + 1, 0);
-  size_t most = 0;
+  std::vector<int> widest((size_t)K, 0);  // the most cells of one node publishing before part k
+  long long most = 0;
   for (int k = 0; k < K; k++) {
+    long long at = 0;
     for (int b = 0; k > 0 && b < B; b++)
-      if ((int)plan.cuts[(size_t)b].size() >= k) pub.push_back(b);
+      if ((int)plan.cuts[(size_t)b].size() >= k) {
+        const HsLevel &m = p->procs[(size_t)b].l[0];
+        const int cells = m.sx * m.sy;
+        pub.push_back(b);
+        jobs.push_back(HsRosJob{m.lo, at, cells});
+        at += cells;
+        widest[(size_t)k] = std::max(widest[(size_t)k], cells);
+      }
     pub0[(size_t)k + 1] = pub.size();
-    most = std::max(most, pub0[(size_t)k + 1] - pub0[(size_t)k]);
+    most = std::max(most, at);
   }
   B2S_CUDA_CHECK(cudaSetDevice(p->device));
   b2s_status st = hs_wait_launch(p);
   if (st) return st;
   if ((st = hs_reserve_epochs(p, (unsigned long long)longest))) return st;  // per processor: its own scans
   B2S_CUDA_CHECK(io.h_rows.reserve(16 * T));
-  if (most > 0)  // the first call that publishes allocates the slots; later calls reuse them
+  if (most > 0)  // the first call that publishes allocates the slots; later calls reuse them (or grow them)
     for (int s = 0; s < 2; s++) {
-      B2S_CUDA_CHECK(io.d_map[s].reserve(most * cells));
-      B2S_CUDA_CHECK(io.h_map[s].reserve(most * cells));
+      B2S_CUDA_CHECK(io.d_map[s].reserve((size_t)most));
+      B2S_CUDA_CHECK(io.h_map[s].reserve((size_t)most));
     }
   HsIngestUpload d_in(p->stream);
   AsyncBuf<float> d_out(p->stream);
   AsyncBuf<long long> d_parts(p->stream);
-  AsyncBuf<int> d_pub(p->stream);
+  AsyncBuf<HsRosJob> d_jobs(p->stream);
   B2S_CUDA_CHECK(d_parts.alloc(parts.size()));
-  B2S_CUDA_CHECK(d_pub.alloc(std::max<size_t>(pub.size(), 1)));
+  B2S_CUDA_CHECK(d_jobs.alloc(std::max<size_t>(jobs.size(), 1)));
   B2S_CUDA_CHECK(d_out.alloc(16 * std::max<size_t>(T, 1)));
-  if ((st = hs_ingest_upload(p, d_in, T, nr, ranges, units, geometry.range_min, range_cutoff, filters))) return st;
+  if ((st = hs_ingest_upload(p, d_in, (size_t)floats, ranges, n_units, units, las.data()))) return st;
   B2S_CUDA_CHECK(cudaMemcpyAsync(d_parts, parts.data(), sizeof(long long) * parts.size(), cudaMemcpyHostToDevice, p->stream));
-  if (!pub.empty()) B2S_CUDA_CHECK(cudaMemcpyAsync(d_pub, pub.data(), sizeof(int) * pub.size(), cudaMemcpyHostToDevice, p->stream));
+  if (!jobs.empty()) B2S_CUDA_CHECK(cudaMemcpyAsync(d_jobs, jobs.data(), sizeof(HsRosJob) * jobs.size(), cudaMemcpyHostToDevice, p->stream));
   // the copy stream reads d_out: on every way out it is drained before the stream-ordered frees above
   struct DrainCopies {
     cudaStream_t s;
@@ -1532,8 +1644,7 @@ b2s_status hs_node_run(b2s_hector_slam *p, HsNodeIo &io, const b2s_laser_scan_ms
     B2S_CUDA_CHECK(cudaEventSynchronize(io.copied[q.slot]));
     for (size_t j = pub0[(size_t)q.k]; j < pub0[(size_t)q.k + 1]; j++) {
       const long long *prev = parts.data() + 2 * ((size_t)(q.k - 1) * B + pub[j]);  // the rows before this publish
-      if (b2s_status s = on_map(pub[j], q.k, io.h_map[q.slot] + (j - pub0[(size_t)q.k]) * cells, io.h_rows + 16 * prev[0],
-                                prev[1] - prev[0]))
+      if (b2s_status s = on_map(pub[j], q.k, io.h_map[q.slot] + jobs[j].out, io.h_rows + 16 * prev[0], prev[1] - prev[0]))
         return s;
     }
     return B2S_OK;
@@ -1544,12 +1655,14 @@ b2s_status hs_node_run(b2s_hector_slam *p, HsNodeIo &io, const b2s_laser_scan_ms
       if (pending.size() == 2) {
         if ((st = drain_one())) return st;
       }
-      k_hector_ros_nodes<<<dim3((unsigned)ceil_div((long long)cells, 256), (unsigned)np), 256, 0, p->stream>>>(
-          p->P.l[0].lo, (int)cells, d_pub + pub0[(size_t)k], io.d_map[slot]);
+      const HsRosJob &last = jobs[pub0[(size_t)k + 1] - 1];
+      k_hector_ros_nodes<<<dim3((unsigned)ceil_div((long long)widest[(size_t)k], 256), (unsigned)np), 256, 0, p->stream>>>(
+          d_jobs + pub0[(size_t)k], io.d_map[slot]);
       B2S_CUDA_CHECK(cudaGetLastError());
       B2S_CUDA_CHECK(cudaEventRecord(io.converted[slot], p->stream));
       B2S_CUDA_CHECK(cudaStreamWaitEvent(io.copy, io.converted[slot], 0));
-      B2S_CUDA_CHECK(cudaMemcpyAsync(io.h_map[slot], io.d_map[slot], np * cells, cudaMemcpyDeviceToHost, io.copy));
+      B2S_CUDA_CHECK(cudaMemcpyAsync(io.h_map[slot], io.d_map[slot], (size_t)(last.out + last.cells), cudaMemcpyDeviceToHost,
+                                     io.copy));
       for (size_t j = pub0[(size_t)k]; j < pub0[(size_t)k + 1]; j++) {
         const long long *prev = parts.data() + 2 * ((size_t)(k - 1) * B + pub[j]);
         if (prev[1] > prev[0])
@@ -1582,13 +1695,22 @@ extern "C" {
 
 b2s_status b2s_hector_slam_create(float map_resolution, int map_size_x, int map_size_y, float start_x, float start_y,
                                   int levels, int device, void *cuda_stream, b2s_hector_slam **out) {
-  return hs_create(map_resolution, map_size_x, map_size_y, start_x, start_y, levels, 1, 2048, device, cuda_stream, out);
+  const b2s_hector_map_spec s = hs_default_spec(map_resolution, map_size_x, map_size_y, start_x, start_y, levels);
+  return hs_create(1, 2048, &s, device, cuda_stream, out, "b2s_hector_slam_create");
 }
 
 b2s_status b2s_hector_slam_create_batch(int batch, int max_points, float map_resolution, int map_size_x, int map_size_y,
                                         float start_x, float start_y, int levels, int device, void *cuda_stream,
                                         b2s_hector_slam **out) {
-  return hs_create(map_resolution, map_size_x, map_size_y, start_x, start_y, levels, batch, max_points, device, cuda_stream, out);
+  if (batch < 1) return hs_create(batch, max_points, nullptr, device, cuda_stream, out, "b2s_hector_slam_create_batch");
+  const std::vector<b2s_hector_map_spec> specs(
+      (size_t)batch, hs_default_spec(map_resolution, map_size_x, map_size_y, start_x, start_y, levels));
+  return hs_create(batch, max_points, specs.data(), device, cuda_stream, out, "b2s_hector_slam_create_batch");
+}
+
+b2s_status b2s_hector_slam_create_fleet(int batch, int max_points, const b2s_hector_map_spec *maps, int device,
+                                        void *cuda_stream, b2s_hector_slam **out) {
+  return hs_create(batch, max_points, maps, device, cuda_stream, out, "b2s_hector_slam_create_fleet");
 }
 
 void b2s_hector_slam_destroy(b2s_hector_slam *p) {
@@ -1600,16 +1722,20 @@ void b2s_hector_slam_destroy(b2s_hector_slam *p) {
 
 b2s_status b2s_hector_slam_set_update_factors(b2s_hector_slam *p, float update_free, float update_occupied) {
   if (!p) B2S_FAIL(B2S_ERR_BAD_PARAMS, "null handle");
-  p->P.lo_free = prob_to_log_odds(update_free);
-  p->P.lo_occ = prob_to_log_odds(update_occupied);
-  return B2S_OK;
+  for (HsProc &q : p->procs) {
+    q.lo_free = prob_to_log_odds(update_free);
+    q.lo_occ = prob_to_log_odds(update_occupied);
+  }
+  return hs_upload_procs(p);
 }
 
 b2s_status b2s_hector_slam_set_map_update_min_diff(b2s_hector_slam *p, float min_dist, float min_angle) {
   if (!p) B2S_FAIL(B2S_ERR_BAD_PARAMS, "null handle");
-  p->P.min_dist = min_dist;
-  p->P.min_angle = min_angle;
-  return B2S_OK;
+  for (HsProc &q : p->procs) {
+    q.min_dist = min_dist;
+    q.min_angle = min_angle;
+  }
+  return hs_upload_procs(p);
 }
 
 b2s_status b2s_hector_slam_set_exact(b2s_hector_slam *p, int exact) {
@@ -1795,6 +1921,7 @@ b2s_status b2s_hector_slam_process_scans_batch(b2s_hector_slam *p, const b2s_las
   if (map_without_matching && !pose_hints) B2S_FAIL(B2S_ERR_BAD_PARAMS, "map_without_matching needs a pose per scan (pose_hints)");
   const int n = geometry->n_ranges;
   if (n > p->cap) B2S_FAIL(B2S_ERR_TOO_LARGE, "more ranges per scan than the handle's capacity");
+  const int B = p->batch;
   std::vector<long long> first;
   int longest = 0;
   b2s_status st = hs_fleet_counts(p, n_scans, first, longest);
@@ -1802,17 +1929,24 @@ b2s_status b2s_hector_slam_process_scans_batch(b2s_hector_slam *p, const b2s_las
   const long long total = first.back();
   if (total > 0 && n > 0 && !ranges) B2S_FAIL(B2S_ERR_BAD_PARAMS, "null argument");
   if ((unsigned)longest >= HS_EPOCH_MAX) B2S_FAIL(B2S_ERR_TOO_LARGE, "too many scans of one processor in one call (stamp epochs are 20 bits)");
-  const float scale_to_map = p->P.l[0].tf.tw_lin;  // GridMapBase::getScaleToMap of level 0: 1 / cell length
+  // one laser for every processor (base 0: scan i's ranges are row i), each scaled to its own level 0
   const b2s_hector_scan_filter &q = *filter;
-  const HectorBeamFilter f = hector_scan_filter(q.laser_in_base, scale_to_map, q.min_dist, q.max_dist, q.use_max_scan_range,
-                                                q.z_min, q.z_max);
-  const std::vector<HectorBeamFilter> filters((size_t)p->batch, f);  // one laser: every processor converts alike
+  std::vector<HsLaser> lasers((size_t)B);
+  for (int b = 0; b < B; b++) {
+    HsLaser &l = lasers[(size_t)b];
+    l.filter = hector_scan_filter(q.laser_in_base, hs_scale_to_map(p, b), q.min_dist, q.max_dist, q.use_max_scan_range,
+                                  q.z_min, q.z_max);
+    l.base = 0;
+    l.unit0 = 0;
+    l.n_ranges = n;
+    l.range_min = geometry->range_min;
+    l.range_cutoff = hector_range_cutoff(q.range_cutoff, geometry->range_max);
+  }
   std::vector<double> unit(2 * (size_t)n);
   hector_unit_vectors(geometry->angle_min, geometry->angle_increment, n, unit.data());
   HsIngestUpload d_in(p->stream);
   auto upload = [&](HsFleet &F) -> b2s_status {
-    if (b2s_status s = hs_ingest_upload(p, d_in, (size_t)total, n, ranges, unit.data(), geometry->range_min,
-                                        hector_range_cutoff(q.range_cutoff, geometry->range_max), filters.data()))
+    if (b2s_status s = hs_ingest_upload(p, d_in, (size_t)total * (size_t)n, ranges, (size_t)n, unit.data(), lasers.data()))
       return s;
     F.ingest = d_in.ingest;
     return B2S_OK;
@@ -1879,21 +2013,27 @@ b2s_status b2s_hector_slam_sync(b2s_hector_slam *p) {
   return B2S_OK;
 }
 
-b2s_status b2s_hector_slam_level_dims(b2s_hector_slam *p, int level, int dims[2], float *cell_length) {
-  if (!p || !dims || level < 0 || level >= p->levels) B2S_FAIL(B2S_ERR_BAD_PARAMS, "bad level");
-  dims[0] = p->sx[level];
-  dims[1] = p->sy[level];
-  if (cell_length) *cell_length = p->cell_length[level];
+b2s_status b2s_hector_slam_level_dims_of(b2s_hector_slam *p, int b, int level, int dims[2], float *cell_length) {
+  if (!p || !dims || b < 0 || b >= p->batch || level < 0 || level >= p->procs[(size_t)b].levels)
+    B2S_FAIL(B2S_ERR_BAD_PARAMS, "bad level / processor");
+  dims[0] = p->procs[(size_t)b].l[level].sx;
+  dims[1] = p->procs[(size_t)b].l[level].sy;
+  if (cell_length) *cell_length = hs_cell_length(p->specs[(size_t)b], level);
   return B2S_OK;
 }
 
+b2s_status b2s_hector_slam_level_dims(b2s_hector_slam *p, int level, int dims[2], float *cell_length) {
+  return b2s_hector_slam_level_dims_of(p, 0, level, dims, cell_length);
+}
+
 b2s_status b2s_hector_slam_copy_level_of(b2s_hector_slam *p, int b, int level, float *log_odds, int32_t *update_index) {
-  if (!p || level < 0 || level >= p->levels || b < 0 || b >= p->batch) B2S_FAIL(B2S_ERR_BAD_PARAMS, "bad level / processor");
+  if (!p || b < 0 || b >= p->batch || level < 0 || level >= p->procs[(size_t)b].levels)
+    B2S_FAIL(B2S_ERR_BAD_PARAMS, "bad level / processor");
   B2S_CUDA_CHECK(cudaSetDevice(p->device));
-  const HsLevel &m = p->P.l[level];
+  const HsLevel &m = p->procs[(size_t)b].l[level];
   const size_t cells = (size_t)m.sx * m.sy;
-  if (log_odds) B2S_CUDA_CHECK(cudaMemcpyAsync(log_odds, m.lo + (size_t)b * cells, cells * 4, cudaMemcpyDeviceToHost, p->stream));
-  if (update_index) B2S_CUDA_CHECK(cudaMemcpyAsync(update_index, m.ui + (size_t)b * cells, cells * 4, cudaMemcpyDeviceToHost, p->stream));
+  if (log_odds) B2S_CUDA_CHECK(cudaMemcpyAsync(log_odds, m.lo, cells * 4, cudaMemcpyDeviceToHost, p->stream));
+  if (update_index) B2S_CUDA_CHECK(cudaMemcpyAsync(update_index, m.ui, cells * 4, cudaMemcpyDeviceToHost, p->stream));
   B2S_CUDA_CHECK(cudaStreamSynchronize(p->stream));
   p->launch_pending = false;
   return B2S_OK;
@@ -1904,13 +2044,14 @@ b2s_status b2s_hector_slam_copy_level(b2s_hector_slam *p, int level, float *log_
 }
 
 b2s_status b2s_hector_slam_copy_level_ros_of(b2s_hector_slam *p, int b, int level, int8_t *out) {
-  if (!p || !out || level < 0 || level >= p->levels || b < 0 || b >= p->batch) B2S_FAIL(B2S_ERR_BAD_PARAMS, "bad level / processor");
+  if (!p || !out || b < 0 || b >= p->batch || level < 0 || level >= p->procs[(size_t)b].levels)
+    B2S_FAIL(B2S_ERR_BAD_PARAMS, "bad level / processor");
   B2S_CUDA_CHECK(cudaSetDevice(p->device));
-  const HsLevel &m = p->P.l[level];
+  const HsLevel &m = p->procs[(size_t)b].l[level];
   const int n = m.sx * m.sy;
   AsyncBuf<int8_t> d(p->stream);
   B2S_CUDA_CHECK(d.alloc((size_t)n));
-  k_hector_ros<<<ceil_div(n, 256), 256, 0, p->stream>>>(m.lo + (size_t)b * n, n, d);
+  k_hector_ros<<<ceil_div(n, 256), 256, 0, p->stream>>>(m.lo, n, d);
   B2S_CUDA_CHECK(cudaGetLastError());
   B2S_CUDA_CHECK(cudaMemcpyAsync(out, d, (size_t)n, cudaMemcpyDeviceToHost, p->stream));
   B2S_CUDA_CHECK(cudaStreamSynchronize(p->stream));

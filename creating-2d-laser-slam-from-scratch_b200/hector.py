@@ -10,6 +10,21 @@ from .matcher import check, lib
 _bound = False
 
 
+class HectorMapSpec(C.Structure):
+    """b2s_hector_map_spec: one processor of a fleet handle (HectorSlamProcessor's constructor + setters)."""
+    _fields_ = [("map_resolution", C.c_float), ("map_size_x", C.c_int32), ("map_size_y", C.c_int32),
+                ("start_x", C.c_float), ("start_y", C.c_float), ("levels", C.c_int32), ("update_free", C.c_float),
+                ("update_occupied", C.c_float), ("min_dist", C.c_float), ("min_angle", C.c_float),
+                ("reserved", C.c_int32 * 6)]
+
+
+def map_spec(resolution=0.05, size_x=1024, size_y=1024, start=(0.5, 0.5), levels=3, update_free=0.4,
+             update_occupied=0.6, min_dist=0.4, min_angle=0.13) -> HectorMapSpec:
+    """A fleet processor's spec; the defaults are b2s_hector_slam_create's."""
+    return HectorMapSpec(resolution, size_x, size_y, start[0], start[1], levels, update_free, update_occupied,
+                         min_dist, min_angle)
+
+
 def _bind():
     global _bound
     L = lib()
@@ -51,6 +66,8 @@ def _bind():
     L.b2s_hector_slam_last_poses.argtypes = [vp, C.c_int, fp, fp]
     L.b2s_hector_slam_debug_set_epoch.argtypes = [vp, C.c_uint]
     L.b2s_hector_slam_match_cluster_size.argtypes = [vp]
+    L.b2s_hector_slam_create_fleet.argtypes = [C.c_int, C.c_int, C.POINTER(HectorMapSpec), C.c_int, vp, C.POINTER(vp)]
+    L.b2s_hector_slam_level_dims_of.argtypes = [vp, C.c_int, C.c_int, C.POINTER(C.c_int), fp]
     _bound = True
     return L
 
@@ -144,6 +161,23 @@ class HectorSlam:
         if not exact:
             check(self.L.b2s_hector_slam_set_exact(self.h, 0))
         self.map_updated = False
+
+    @classmethod
+    def fleet(cls, specs, max_points=2048, exact=True, device=0, stream=None):
+        """B processors, each with its own map_spec (size, resolution, levels, start, update factors, gate), behind one
+        handle (b2s_hector_slam_create_fleet).  self.levels is then the list of every processor's levels."""
+        self = cls.__new__(cls)
+        self.L = _bind()
+        self.batch, self.cap = len(specs), max_points
+        self.levels = [int(s.levels) for s in specs]
+        self.h = C.c_void_p()
+        arr = (HectorMapSpec * len(specs))(*specs)
+        check(self.L.b2s_hector_slam_create_fleet(len(specs), max_points, arr, device,
+                                                  C.c_void_p(stream) if stream else None, C.byref(self.h)))
+        if not exact:
+            check(self.L.b2s_hector_slam_set_exact(self.h, 0))
+        self.map_updated = False
+        return self
 
     def set_exact(self, exact):
         check(self.L.b2s_hector_slam_set_exact(self.h, int(bool(exact))))
@@ -254,7 +288,7 @@ class HectorSlam:
         check(self.L.b2s_hector_slam_sync(self.h))
 
     def level_of(self, b, i):
-        sx, sy, _ = self.level_dims(i)
+        sx, sy, _ = self.level_dims(i, b)
         lo, ui = np.zeros(sx * sy, np.float32), np.zeros(sx * sy, np.int32)
         check(self.L.b2s_hector_slam_copy_level_of(self.h, b, i, _f(lo), ui.ctypes.data_as(C.POINTER(C.c_int32))))
         return lo.reshape(sy, sx), ui.reshape(sy, sx)
@@ -278,9 +312,10 @@ class HectorSlam:
     def reset(self):
         check(self.L.b2s_hector_slam_reset(self.h))
 
-    def level_dims(self, i):
+    def level_dims(self, i, b=0):
+        """(width, height, cell length) of processor b's level i"""
         dims, cl = (C.c_int * 2)(), C.c_float(0)
-        check(self.L.b2s_hector_slam_level_dims(self.h, i, dims, C.byref(cl)))
+        check(self.L.b2s_hector_slam_level_dims_of(self.h, b, i, dims, C.byref(cl)))
         return dims[0], dims[1], cl.value
 
     def level(self, i):
@@ -297,7 +332,7 @@ class HectorSlam:
 
     def ros_map_of(self, b, level=0):
         """nav_msgs/OccupancyGrid payload of processor b's level."""
-        sx, sy, _ = self.level_dims(level)
+        sx, sy, _ = self.level_dims(level, b)
         out = np.zeros((sy, sx), np.int8)
         check(self.L.b2s_hector_slam_copy_level_ros_of(self.h, b, level, out.ctypes.data_as(C.POINTER(C.c_int8))))
         return out

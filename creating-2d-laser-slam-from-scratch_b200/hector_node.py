@@ -97,6 +97,8 @@ def _bind():
                                                C.POINTER(vp)]
     L.b2s_hector_node_process_batch.argtypes = [vp, ip, fp, C.POINTER(C.c_uint32), fp, dp, dp, ip, ip, BATCH_MAP_FN, vp]
     L.b2s_hector_node_publish_map_of.argtypes = [vp, C.c_int, C.POINTER(C.c_uint32), BATCH_MAP_FN, vp]
+    L.b2s_hector_node_create_fleet.argtypes = [C.c_int, C.POINTER(HectorNodeParams), C.POINTER(LaserScanMsg), dp, C.c_int,
+                                               C.POINTER(vp)]
     _bound = True
     return L
 
@@ -191,13 +193,14 @@ class HectorNode:
 
 class HectorNodeBatch:
     """B HectorMappingRos nodes in one handle, one per recording or per setting (b2s_hector_node_create_batch): the
-    processor fields of every params set must be equal; mounts, range limits, z windows and periods may differ."""
+    processor fields of every params set must be equal; mounts, range limits, z windows and periods may differ.
+    HectorNodeBatch.fleet takes nodes with nothing in common."""
 
     def __init__(self, params_list, geometry: LaserScanMsg, mounts, device=0):
         self.L = _bind()
         self.h = C.c_void_p()
-        self.n_ranges = geometry.n_ranges
         self.batch = len(params_list)
+        self.n_ranges = [geometry.n_ranges] * self.batch
         params = (HectorNodeParams * self.batch)(*params_list)
         m = np.ascontiguousarray(mounts, np.float64)
         assert m.shape == (self.batch, 7)
@@ -205,18 +208,38 @@ class HectorNodeBatch:
                                                   m.ctypes.data_as(C.POINTER(C.c_double)), device, C.byref(self.h)))
         self.processor = C.c_void_p(self.L.b2s_hector_node_processor(self.h))
 
+    @classmethod
+    def fleet(cls, params_list, geometries, mounts, device=0):
+        """Nodes of different robots in one handle (b2s_hector_node_create_fleet): per node its own params (map size,
+        resolution, levels, ... included), its own LaserScanMsg geometry and its own mount."""
+        self = cls.__new__(cls)
+        self.L = _bind()
+        self.h = C.c_void_p()
+        self.batch = len(params_list)
+        assert len(geometries) == self.batch
+        self.n_ranges = [g.n_ranges for g in geometries]
+        params = (HectorNodeParams * self.batch)(*params_list)
+        geoms = (LaserScanMsg * self.batch)(*geometries)
+        m = np.ascontiguousarray(mounts, np.float64)
+        assert m.shape == (self.batch, 7)
+        check(self.L.b2s_hector_node_create_fleet(self.batch, params, geoms, m.ctypes.data_as(C.POINTER(C.c_double)),
+                                                  device, C.byref(self.h)))
+        self.processor = C.c_void_p(self.L.b2s_hector_node_processor(self.h))
+        return self
+
     def process(self, ranges_list, stamps_list, on_map=None):
-        """ranges_list[b] [S_b][n] float32, stamps_list[b] [S_b][2] -> one dict per node, shaped as
-        HectorNode.process's.  Maps go to on_map(node, dict) in the call's order when given."""
+        """ranges_list[b] [S_b][n_b] float32 (n_b = node b's n_ranges), stamps_list[b] [S_b][2] -> one dict per node,
+        shaped as HectorNode.process's.  Maps go to on_map(node, dict) in the call's order when given."""
         counts = np.array([len(s) for s in stamps_list], np.int32)
         assert len(counts) == self.batch and len(ranges_list) == self.batch
         S = int(counts.sum())
-        r = np.zeros((S, self.n_ranges), np.float32)
+        r = np.concatenate([np.ascontiguousarray(ranges_list[b], np.float32).reshape(-1) if counts[b] else
+                            np.zeros(0, np.float32) for b in range(self.batch)] + [np.zeros(0, np.float32)])
+        assert len(r) == int((counts * np.array(self.n_ranges, np.int64)).sum())
         s = np.zeros((S, 2), np.uint32)
         at = np.concatenate([[0], np.cumsum(counts)])
         for b in range(self.batch):
             if counts[b]:
-                r[at[b]:at[b + 1]] = np.asarray(ranges_list[b], np.float32).reshape(counts[b], self.n_ranges)
                 s[at[b]:at[b + 1]] = np.asarray(stamps_list[b], np.uint32).reshape(counts[b], 2)
         pose, msg, cov = np.zeros((S, 3), np.float32), np.zeros((S, 7)), np.zeros((S, 36))
         upd, kept = np.zeros(S, np.int32), np.zeros(S, np.int32)
@@ -241,7 +264,7 @@ class HectorNodeBatch:
     def level_ros(self, b, level=0):
         """Node b's processor level as a ROS payload (b2s_hector_slam_copy_level_ros_of)."""
         dims, cl = (C.c_int * 2)(), C.c_float(0)
-        check(self.L.b2s_hector_slam_level_dims(self.processor, level, dims, C.byref(cl)))
+        check(self.L.b2s_hector_slam_level_dims_of(self.processor, b, level, dims, C.byref(cl)))
         out = np.zeros((dims[1], dims[0]), np.int8)
         check(self.L.b2s_hector_slam_copy_level_ros_of(self.processor, b, level, out.ctypes.data_as(C.POINTER(C.c_int8))))
         return out

@@ -525,6 +525,33 @@ b2s_status b2s_hector_slam_process_stream_batch(b2s_hector_slam *p, const int32_
                                                 const float *first_pose_hints, const float *pose_hints,
                                                 int map_without_matching, float *out_poses, int32_t *out_map_updated,
                                                 float *out_last_covs);
+/* One processor of a fleet handle: HectorSlamProcessor's constructor arguments (as for b2s_hector_slam_create) and
+ * the values of its setters (b2s_hector_slam_set_update_factors, _set_map_update_min_diff).  The defaults of
+ * b2s_hector_slam_create are update_free 0.4, update_occupied 0.6, min_dist 0.4 m, min_angle 0.13 rad.  reserved:
+ * zero; it keeps the struct at 64 bytes. */
+typedef struct b2s_hector_map_spec {
+  float map_resolution;
+  int32_t map_size_x, map_size_y;
+  float start_x, start_y;
+  int32_t levels;
+  float update_free, update_occupied;
+  float min_dist, min_angle;
+  int32_t reserved[6];
+} b2s_hector_map_spec;
+/* B independent processors, each with its own map size, resolution, levels, start, update factors and map-update
+ * gate (maps [batch]), behind one handle: b2s_hector_slam_create_batch with nothing required equal.  Every processor
+ * gets its own planes (a processor with fewer levels has none above its last).  Each spec is checked as
+ * b2s_hector_slam_create checks its arguments, before the device is touched, and the refusal names the processor:
+ * B2S_ERR_BAD_PARAMS for levels outside 1 ... 8, a resolution that is not positive or a map whose coarsest level is
+ * 2 cells or fewer across; B2S_ERR_TOO_LARGE for max_points above 4096.  process_stream_batch, process_scans_batch
+ * (each processor scales the shared laser's points by its own level-0 cell length), update_batch and the _of getters
+ * serve it; set_update_factors and set_map_update_min_diff set every processor's values.  b2s_hector_slam_create and
+ * _create_batch are this with equal specs. */
+b2s_status b2s_hector_slam_create_fleet(int batch, int max_points, const b2s_hector_map_spec *maps, int device,
+                                        void *cuda_stream, b2s_hector_slam **out);
+/* getGridMap(level) of one processor; B2S_ERR_BAD_PARAMS for a level at or above that processor's levels.
+ * b2s_hector_slam_level_dims is processor 0's. */
+b2s_status b2s_hector_slam_level_dims_of(b2s_hector_slam *p, int processor, int level, int dims[2], float *cell_length);
 /* getLastScanMatchPose / getLastMapUpdatePose (HectorSlamProcessor.h:118-119) of one processor; either may be NULL */
 b2s_status b2s_hector_slam_last_poses(b2s_hector_slam *p, int processor, float last_scan_match_pose[3],
                                       float last_map_update_pose[3]);
@@ -812,6 +839,16 @@ typedef void (*b2s_hector_node_batch_map_fn)(void *user, int32_t node, int32_t s
 b2s_status b2s_hector_node_create_batch(int batch, const b2s_hector_node_params *params,
                                         const b2s_laser_scan_msg *geometry, const double *laser_mounts, int device,
                                         b2s_hector_node **out);
+/* Nodes of different robots in one handle: params [batch], geometries [batch] (each node's own LaserScan fields) and
+ * laser_mounts [batch][7], nothing required equal.  Each node gets its own processor (map size, resolution, levels,
+ * start, update factors, map-update gate) and its own laser, and is validated as b2s_hector_node_create validates its
+ * own, before the device is touched; the refusal names the node (B2S_ERR_TOO_LARGE for n_ranges above 4096 or more
+ * than 65535 nodes).  b2s_hector_node_create_batch is this with one geometry repeated.  process_batch reads node b's
+ * n_scans[b] scans as rows of its own n_ranges floats, node-major; each map carries its node's map info and payload
+ * size. */
+b2s_status b2s_hector_node_create_fleet(int batch, const b2s_hector_node_params *params,
+                                        const b2s_laser_scan_msg *geometries, const double *laser_mounts, int device,
+                                        b2s_hector_node **out);
 /* b2s_hector_node_process on every node at once: n_scans [batch] (0 leaves a node untouched, its schedule does not
  * start), ranges / stamps / outputs node-major (node 0's scans first), as b2s_hector_slam_process_scans_batch.  Each
  * node's maps reach on_map in its own publish order.  Across nodes the call runs in parts: part 0 holds every node's
@@ -820,8 +857,8 @@ b2s_status b2s_hector_node_create_batch(int batch, const b2s_hector_node_params 
  * one call.  B2S_ERR_BAD_PARAMS (nothing written, nothing changed) for a NULL n_scans, a negative count, or NULL
  * arrays with scans; B2S_ERR_TOO_LARGE for a node with 2^20 - 1 or more scans.  A failure after the call started marks
  * the handle failed, as for b2s_hector_node_process.  The maps due before a part are converted on the device into one
- * page-locked buffer per part, two parts in flight: 2 x (nodes publishing) x width x height bytes on each side,
- * allocated by the first call that publishes and kept. */
+ * page-locked buffer per part, two parts in flight: 2 x (the most cells published before one part) bytes on each
+ * side, allocated by the first call that publishes and kept (grown by a later call that publishes more). */
 b2s_status b2s_hector_node_process_batch(b2s_hector_node *node, const int32_t *n_scans, const float *ranges,
                                          const uint32_t *stamps, float *out_pose, double *out_pose_msg, double *out_cov,
                                          int32_t *out_map_updated, int32_t *out_n_points,
