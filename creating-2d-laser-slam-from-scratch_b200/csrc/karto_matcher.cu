@@ -549,31 +549,45 @@ __global__ void __launch_bounds__(256)
 }
 
 // ----------------------------------------------------------------------------------------------
-// k_grid_pool: per match, the 4x4 max-pooled grid of k_sweep_bound (layout: pool_lead / pool_pitch in
-// karto_sweep_plan.cuh).  The pooling is in FLAT index space, rows wrapping exactly as a candidate's `base + offset`
-// does, so the pooled byte at a block's corner is at least every byte a candidate of that block reads.  One thread
-// per 4 output bytes; grid bytes outside [0, data_size) count as 0.  grid(ceil(pool_pitch / 1024), B), 256 threads.
+// k_grid_pool: per match, the 4x4 max-pooled grid of k_sweep_bound in its four residue planes (layout: pool_lead /
+// pool_plane / pool_index in karto_sweep_plan.cuh).  The pooling is in FLAT index space, rows wrapping exactly as a
+// candidate's `base + offset` does, so the pooled byte at a block's corner is at least every byte a candidate of that
+// block reads.  Thread q pools P[f] for the 16 indices j = f + lead in [16q, 16q + 16) and writes word q of each
+// plane; grid bytes outside [0, data_size) count as 0, so the planes' padding comes out 0.
+// grid(ceil(pool_plane / 1024), B), 256 threads.
 // ----------------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(256)
     k_grid_pool(const uint8_t *__restrict__ grids, size_t grid_pitch, int data_size, int width_step,
-                int lead, uint8_t *__restrict__ pools, size_t pitch, int batch) {
-  const int j4 = blockIdx.x * blockDim.x + threadIdx.x;
-  if ((size_t)j4 * 4 >= pitch) return;
+                int lead, int plane, uint8_t *__restrict__ pools, size_t pitch, int batch) {
+  const int q = blockIdx.x * blockDim.x + threadIdx.x;
+  if (q * 4 >= plane) return;
   for (int b = blockIdx.y; b < batch; b += gridDim.y) {
     const uint8_t *grid = grids + (size_t)b * grid_pitch;
-    const int f = 4 * j4 - lead;  // a multiple of 4, as are width_step and data_size
+    const int f = 16 * q - lead;  // a multiple of 4, as are width_step and data_size
     auto word = [&](int r) { return (r >= 0 && r < data_size) ? __ldg(reinterpret_cast<const uint32_t *>(grid + r)) : 0u; };
-    uint32_t m = 0;
+    uint32_t m[4] = {0, 0, 0, 0};  // byte r of m[t] = P[f + 4t + r]
 #pragma unroll
     for (int dy = 0; dy < 4; dy++) {
       const int r = f + dy * width_step;
-      const uint32_t w0 = word(r), w1 = word(r + 4);
-      // byte t of the result = max of bytes t..t+3 of the 8 bytes w1:w0
-      const uint32_t a = __vmaxu4(w0, __funnelshift_r(w0, w1, 8));
-      const uint32_t c = __vmaxu4(__funnelshift_r(w0, w1, 16), __funnelshift_r(w0, w1, 24));
-      m = __vmaxu4(m, __vmaxu4(a, c));
+      uint32_t w[5];
+#pragma unroll
+      for (int t = 0; t < 5; t++) w[t] = word(r + 4 * t);
+#pragma unroll
+      for (int t = 0; t < 4; t++) {
+        // byte i of the row maximum = max of bytes i..i+3 of the 8 bytes w[t + 1]:w[t]
+        const uint32_t a = __vmaxu4(w[t], __funnelshift_r(w[t], w[t + 1], 8));
+        const uint32_t c = __vmaxu4(__funnelshift_r(w[t], w[t + 1], 16), __funnelshift_r(w[t], w[t + 1], 24));
+        m[t] = __vmaxu4(m[t], __vmaxu4(a, c));
+      }
     }
-    reinterpret_cast<uint32_t *>(pools + (size_t)b * pitch)[j4] = m;
+    // 4 x 4 byte transpose: plane r word q = byte r of m[0..3]
+    const uint32_t lo01 = __byte_perm(m[0], m[1], 0x5140), hi01 = __byte_perm(m[0], m[1], 0x7362);
+    const uint32_t lo23 = __byte_perm(m[2], m[3], 0x5140), hi23 = __byte_perm(m[2], m[3], 0x7362);
+    uint8_t *out = pools + (size_t)b * pitch + 4 * q;
+    *reinterpret_cast<uint32_t *>(out) = __byte_perm(lo01, lo23, 0x5410);
+    *reinterpret_cast<uint32_t *>(out + plane) = __byte_perm(lo01, lo23, 0x7632);
+    *reinterpret_cast<uint32_t *>(out + 2 * plane) = __byte_perm(hi01, hi23, 0x5410);
+    *reinterpret_cast<uint32_t *>(out + 3 * plane) = __byte_perm(hi01, hi23, 0x7632);
   }
 }
 
@@ -1169,41 +1183,48 @@ __device__ __forceinline__ float red_fscore(int32_t isum, float apf_k, float dpf
 //                   response is not penalised, Mapper.cpp:399) every angle is swept.
 // k_reduce reads 0 for the angles never swept; the response volume is completed on request (get_response_sums).
 // ----------------------------------------------------------------------------------------------
-// the window origins s_off[j0, j1) of this warp's staging row (j0, j1 multiples of 4), summed at the lane's two block
-// corners
-template <bool CHECK>
-__device__ __forceinline__ void bound_beams(const uint8_t *__restrict__ sp, const int32_t *__restrict__ s_off, int j0,
-                                            int j1, int off_a, int off_b, uint32_t lead, uint32_t limit, uint32_t &ua,
-                                            uint32_t &ub) {
-  for (int j = j0; j < j1; j += 4) {
-    const int4 a4 = *reinterpret_cast<const int4 *>(s_off + j);  // one broadcast load: four window origins
-    const int32_t as[4] = {a4.x, a4.y, a4.z, a4.w};
-#pragma unroll
-    for (int q = 0; q < 4; q++) {
-      if (CHECK) {  // flat index a + corner, modulo 2^32 like the reference's base + offset; P is 0 outside
-        const uint32_t fa = (uint32_t)as[q] + (uint32_t)off_a, fb = (uint32_t)as[q] + (uint32_t)off_b;
-        ua += (fa + lead < limit) ? sp[(int32_t)fa] : 0u;
-        ub += (fb + lead < limit) ? sp[(int32_t)fb] : 0u;
-      } else {
-        ua += sp[as[q] + off_a];
-        ub += sp[as[q] + off_b];
-      }
-    }
-  }
+// bytes c .. c + 3 of the 8 bytes hi:lo, c = sel % 4 (prmt's forward-4-extract mode reads only sel's two low bits)
+__device__ __forceinline__ uint32_t extract4(uint32_t lo, uint32_t hi, uint32_t sel) {
+  uint32_t d;
+  asm("prmt.b32.f4e %0, %1, %2, %3;" : "=r"(d) : "r"(lo), "r"(hi), "r"(sel));
+  return d;
 }
 
-// One persistent CTA per match at a time (like k_sweep_window): the pooled image is staged by TMA, warps take angles,
-// lane L owns blocks (L / 8, L % 8) and (L / 8 + 4, L % 8).  ubr[b][k] = UBr(k) (-1 for a match the window kernel
-// does not sweep).  The bound reads no window lists: for each angle a warp places 32 beams at a time, one per lane,
-// with win_origin_class (the definition k_offsets_sorted lists them by), drops the ones the lists would drop, and
-// compacts the interior and the edge ones into its staging row.  Which beams add is the same set as in the lists and
-// integer sums commute, so UBr is the one the lists would give.  It also counts the empty windows of every (beam,
-// angle) pair into stats[0], as the lists of a sweep that is not pruned do.
+// the 8 pooled bytes of block row `rw / width_step` of an interior beam whose block (0, 0) corner is at byte `addr` of
+// the staged image: P at block columns 0..3 (lo) and 4..7 (hi) in byte order.  rw % 8 == 0, so every row of the beam
+// has the alignment of addr.
+__device__ __forceinline__ void bound_row(const uint8_t *__restrict__ pb, int addr, int rw, uint32_t &lo,
+                                          uint32_t &hi) {
+  const uint32_t *w = reinterpret_cast<const uint32_t *>(pb + ((addr + rw) & ~3));
+  const uint32_t w0 = w[0], w1 = w[1], w2 = w[2];
+  lo = extract4(w0, w1, (uint32_t)addr);
+  hi = extract4(w1, w2, (uint32_t)addr);
+}
+
+constexpr int BOUND_FLUSH = 64 * 32;  // beams placed between flushes of k_sweep_bound's packed corner sums
+
+// One persistent CTA per match at a time (like k_sweep_window): the pooled image (its four residue planes, see
+// pool_index) is staged by TMA, warps take angles.  ubr[b][k] = UBr(k) (-1 for a match the window kernel does not
+// sweep).  The bound reads no window lists: for each angle a warp places 32 beams at a time, one per lane, with
+// win_origin_class (the definition k_offsets_sorted lists them by), drops the ones the lists would drop, and compacts
+// the interior and the edge ones into its staging row.  Which beams add is the same set as in the lists and integer
+// sums commute, so UBr is the one the lists would give.  It also counts the empty windows of every (beam, angle) pair
+// into stats[0], as the lists of a sweep that is not pruned do.
+//
+// Interior beams, four at a time: lane L = slot * 8 + row takes beam `slot` of the four and adds its 8 block corners
+// of block row `row` (8 contiguous plane bytes) as two words, one byte per block column.  Two beams' words add
+// bytewise without carry (the window kernel runs only on grids of bytes <= 127, so P <= 127), and each pair goes into
+// a plain u32 sum and, through one byte permute, a sum of bytes 1 and 3 in u16 lanes; the plain sum less the latter
+// shifted by 8 leaves bytes 0 and 2 in u16 lanes.  A slot takes at most 8 beams per 32 placed, 8 x 127 per u16 lane,
+// so the sums are flushed into the per-column u32 totals every BOUND_FLUSH beams placed (64 x 1016 < 65536) and at
+// the end of the angle.  The totals of the four slots are then summed by shuffles so that lane L ends with blocks
+// (L % 8, 2 (L / 8)) and (L % 8, 2 (L / 8) + 1).  Edge beams and the last 0..3 interior ones read P byte by byte
+// with the range test, at the lane's own two blocks (the value of an interior one is the same either way).
 // STAGE (SweepPlan::bound_stage): the scan-local points and the summed-area table sit in shared memory after the
 // pooled image; otherwise they are read from global memory through L1.
 template <bool STAGE>
 __global__ void __launch_bounds__(WIN_THREADS, 1)
-    k_sweep_bound(const uint8_t *__restrict__ pools, size_t pool_pitch_, int pool_bytes_, int lead,
+    k_sweep_bound(const uint8_t *__restrict__ pools, size_t pool_pitch_, int pool_bytes_, int plane, int lead,
                   const double *__restrict__ local, const double *__restrict__ grid_off,
                   const int32_t *__restrict__ bases, const uint16_t *__restrict__ sat_all, int sbx, int sby,
                   int height, int rows_total, int cols_total, double scale, const int32_t *__restrict__ flags,
@@ -1236,16 +1257,19 @@ __global__ void __launch_bounds__(WIN_THREADS, 1)
       }
     return mx;
   };
-  const double dpen_a = block_dpen(lane >> 3, lane & 7), dpen_b = block_dpen((lane >> 3) + 4, lane & 7);
+  const int slot = lane >> 3, row = lane & 7;
+  const double dpen_a = block_dpen(row, 2 * slot), dpen_b = block_dpen(row, 2 * slot + 1);
   for (int i = threadIdx.x; i < WIN_GUARD / 4; i += blockDim.x) reinterpret_cast<uint32_t *>(smem)[i] = 0;
   if (threadIdx.x == 0) {
     mbar_init(&bar, 1);
     fence_mbar_init();
   }
   __syncthreads();
-  const int off_a = 4 * (lane >> 3) * width_step + 4 * (lane & 7), off_b = off_a + 16 * width_step;
+  const int off_a = 4 * row * width_step + 8 * slot, off_b = off_a + 4;  // the lane's two block corners
+  const int rw = row * width_step;  // its block row in a plane
   const double D = (double)((uint32_t)n * (uint32_t)GRID_OCCUPIED);
-  const uint8_t *sp = smem + WIN_GUARD + lead;  // grid flat index 0
+  const uint8_t *pb = smem + WIN_GUARD;  // the staged pooled image
+  const uint32_t limit = (uint32_t)(lead + data_size);
   uint32_t parity = 0;
   while (true) {
     if (threadIdx.x == 0) s_unit = atomicAdd(work_counter, 1);
@@ -1286,7 +1310,9 @@ __global__ void __launch_bounds__(WIN_THREADS, 1)
     for (int k = warp; k < na; k += WIN_THREADS / 32) {
       const double angle = win_angle(ch, s.angle_offset, s.angle_res, k);
       const double cosine = cos(angle), sine = sin(angle);
-      uint32_t ua = 0, ub = 0;
+      uint32_t ua = 0, ub = 0;               // the lane's two blocks, beams read with the range test
+      uint32_t s0 = 0, s1 = 0, o0 = 0, o1 = 0;  // interior pairs: plain sums and byte 1 / 3 sums of columns 0..3, 4..7
+      uint32_t t[8] = {0, 0, 0, 0, 0, 0, 0, 0};  // interior totals of the lane's slot and row, per block column
       for (int i0 = 0; i0 < n; i0 += 32) {
         const int i = i0 + lane;
         int cls = 255;
@@ -1297,18 +1323,72 @@ __global__ void __launch_bounds__(WIN_THREADS, 1)
           cls = win_origin_class(plx, ply, cosine, sine, G, sat_all != nullptr, STAGE ? s_sat : g_sat, SW, a, empty);
         }
         empties += empty;
-        // interior beams first, then the edge ones, padded to a multiple of 4 with an origin far outside the grid.
         // Interior windows lie within WIN_GUARD - 16 bytes of the grid, so every corner they read is inside the staged
-        // image; the checked loop takes the last 0..3 of them with the edge beams (the value it reads is the same).
+        // planes or their zero padding.  The staging row holds the first n4 of them (a multiple of 4) as image
+        // addresses: beam q < n8 at 8 (q / 8) + 2 (q % 4) + (q / 4) % 2, so that one load gives a lane its slot's two
+        // beams of a group of 8, and a last group of 4 at q.  From n4 on it holds the origins of the other 0..3 and of
+        // the edge ones, padded to a multiple of 4 with an origin far outside the grid.
         const unsigned m_int = __ballot_sync(0xffffffffu, cls < 4), m_edge = __ballot_sync(0xffffffffu, cls >= 4 && cls < 8);
-        const int n_int = __popc(m_int), n_all = n_int + __popc(m_edge);
+        const int n_int = __popc(m_int), n8 = n_int & ~7, n4 = n_int & ~3, n_chk = n_int + __popc(m_edge) - n4;
         __syncwarp();
-        if (cls < 4) s_off[__popc(m_int & lanes_below)] = a;
-        else if (cls < 8) s_off[n_int + __popc(m_edge & lanes_below)] = a;
-        if (lane >= n_all && lane < ((n_all + 3) & ~3)) s_off[lane] = WIN_SKIP;  // slots no beam was compacted into
+        if (cls < 4) {
+          const int q = __popc(m_int & lanes_below);
+          s_off[q < n8 ? (q & ~7) + 2 * (q & 3) + ((q >> 2) & 1) : q] = q < n4 ? pool_index(a, lead, plane) : a;
+        } else if (cls < 8) {
+          s_off[n_int + __popc(m_edge & lanes_below)] = a;
+        }
+        const int n_end = n4 + ((n_chk + 3) & ~3);
+        if (lane >= n4 + n_chk && lane < n_end) s_off[lane] = WIN_SKIP;  // slots no beam was compacted into
         __syncwarp();
-        bound_beams<false>(sp, s_off, 0, n_int & ~3, off_a, off_b, lead, lead + data_size, ua, ub);
-        bound_beams<true>(sp, s_off, n_int & ~3, (n_all + 3) & ~3, off_a, off_b, lead, lead + data_size, ua, ub);
+        for (int g = 0; g < (n8 >> 3); g++) {
+          const int2 e = *reinterpret_cast<const int2 *>(s_off + 8 * g + 2 * slot);
+          uint32_t xl, xh, yl, yh;
+          bound_row(pb, e.x, rw, xl, xh);
+          bound_row(pb, e.y, rw, yl, yh);
+          xl += yl;
+          xh += yh;
+          s0 += xl;
+          o0 += __byte_perm(xl, 0, 0x4341);
+          s1 += xh;
+          o1 += __byte_perm(xh, 0, 0x4341);
+        }
+        if (n4 & 4) {
+          uint32_t xl, xh;
+          bound_row(pb, s_off[n8 + slot], rw, xl, xh);
+          s0 += xl;
+          o0 += __byte_perm(xl, 0, 0x4341);
+          s1 += xh;
+          o1 += __byte_perm(xh, 0, 0x4341);
+        }
+        if (((i0 + 32) & (BOUND_FLUSH - 1)) == 0 || i0 + 32 >= n) {
+          const uint32_t e0 = s0 - (o0 << 8), e1 = s1 - (o1 << 8);  // bytes 0 and 2 in u16 lanes
+          t[0] += e0 & 0xffffu; t[1] += o0 & 0xffffu; t[2] += e0 >> 16; t[3] += o0 >> 16;
+          t[4] += e1 & 0xffffu; t[5] += o1 & 0xffffu; t[6] += e1 >> 16; t[7] += o1 >> 16;
+          s0 = s1 = o0 = o1 = 0;
+        }
+        for (int j = n4; j < n_end; j += 4) {
+          const int4 a4 = *reinterpret_cast<const int4 *>(s_off + j);  // one broadcast load: four window origins
+          const int32_t as[4] = {a4.x, a4.y, a4.z, a4.w};
+#pragma unroll
+          for (int q = 0; q < 4; q++) {  // flat index a + corner, modulo 2^32 like the reference's base + offset; P is 0 outside
+            const uint32_t fa = (uint32_t)as[q] + (uint32_t)off_a, fb = (uint32_t)as[q] + (uint32_t)off_b;
+            ua += (fa + (uint32_t)lead < limit) ? pb[pool_index((int32_t)fa, lead, plane)] : 0u;
+            ub += (fb + (uint32_t)lead < limit) ? pb[pool_index((int32_t)fb, lead, plane)] : 0u;
+          }
+        }
+      }
+      // the four slots' totals summed: lane L keeps block columns 2 (L / 8) and 2 (L / 8) + 1 of row L % 8
+      {
+        const bool hi16 = lane & 16, hi8 = lane & 8;
+        uint32_t k4[4];
+#pragma unroll
+        for (int c = 0; c < 4; c++)
+          k4[c] = (hi16 ? t[c + 4] : t[c]) + __shfl_xor_sync(0xffffffffu, hi16 ? t[c] : t[c + 4], 16);
+#pragma unroll
+        for (int c = 0; c < 2; c++) {
+          const uint32_t v = (hi8 ? k4[c + 2] : k4[c]) + __shfl_xor_sync(0xffffffffu, hi8 ? k4[c] : k4[c + 2], 8);
+          if (c == 0) ua += v; else ub += v;
+        }
       }
       // candidate_response's operations, with the block's largest sum and largest distance penalty
       double apen = 1.0;
@@ -1885,10 +1965,10 @@ static b2s_status build_sat(b2s_matcher *m) {
 // (re)build the per-match pooled grids of the angle-pruning bound after the grids changed (when they fit, see pool_fits)
 static b2s_status build_pool(b2s_matcher *m) {
   if (!pool_fits(m->g, m->smem_optin, m->win_static_smem)) return B2S_OK;
-  const size_t pitch = pool_pitch(m->g);
-  k_grid_pool<<<dim3((unsigned)ceil_div((int)(pitch / 4), 256), grid_rows(m->batch)), 256, 0, m->stream>>>(
-      m->d_grids, m->grid_pitch, m->g.data_size, m->g.width_step, pool_lead(m->g.width_step), m->d_pools, pitch,
-      m->batch);
+  const int plane = pool_plane(m->g);
+  k_grid_pool<<<dim3((unsigned)ceil_div(plane / 4, 256), grid_rows(m->batch)), 256, 0, m->stream>>>(
+      m->d_grids, m->grid_pitch, m->g.data_size, m->g.width_step, pool_lead(m->g.width_step), plane, m->d_pools,
+      pool_pitch(m->g), m->batch);
   B2S_CUDA_CHECK(cudaGetLastError());
   return B2S_OK;
 }
@@ -2603,8 +2683,8 @@ static b2s_status run_correlate(b2s_matcher *m, const b2s_search *s, int k_first
       auto bound = [&](auto kern) -> b2s_status {
         B2S_CUDA_CHECK(raise_dyn_smem(kern, pl.bound_smem));
         kern<<<pl.ctas, WIN_THREADS, pl.bound_smem, m->stream>>>(
-            m->d_pools, pool_pitch(m->g), pool_bytes(m->g), pool_lead(m->g.width_step), m->d_local, m->d_grid_off,
-            m->d_bases, pl.skip_empty ? m->d_sat.p : nullptr, m->sbx, m->sby, m->g.height, pl.rows_total,
+            m->d_pools, pool_pitch(m->g), pool_bytes(m->g), pool_plane(m->g), pool_lead(m->g.width_step), m->d_local,
+            m->d_grid_off, m->d_bases, pl.skip_empty ? m->d_sat.p : nullptr, m->sbx, m->sby, m->g.height, pl.rows_total,
             pl.tiles_x * 32, scale, m->d_flags, m->d_centers, m->p, *s, B, n, na, nx, ny, m->g.width_step,
             m->g.data_size, m->d_ubr, m->d_work, m->d_stats.p);
         return B2S_OK;

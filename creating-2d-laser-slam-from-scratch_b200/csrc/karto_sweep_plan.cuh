@@ -25,12 +25,25 @@ constexpr int PRUNE_PROBE = 16;         // angles swept exactly to find the prun
 
 // u16 entries per match of the block summed-area tables (k_grid_sat), padded to 16 bytes
 inline size_t sat_stride(int sbx, int sby) { return (size_t)((((sbx + 1) * (sby + 1)) + 7) & ~7); }
-// The 4x4 max-pooled grid (k_grid_pool) of one match: byte j holds P[j - pool_lead], P[f] = max over dy, dx in [0, 4)
-// of grid[f + dy * width_step + dx] (0 outside the grid).  It starts pool_lead bytes before grid byte 0 because a block
-// whose corner lies above the grid still reaches it; pool_bytes is what the bound pass stages, pool_pitch the stride.
+// The 4x4 max-pooled grid (k_grid_pool) of one match: P[f] = max over dy, dx in [0, 4) of grid[f + dy * width_step + dx]
+// (0 outside the grid), for f from -pool_lead (a block whose corner lies above the grid still reaches it).  It is
+// stored as four planes split by the residue of j = f + pool_lead modulo 4: plane j & 3 byte j >> 2 holds P[f]
+// (pool_index), each plane pool_plane bytes long.  A beam's 8 block corners of one block row are 4 apart in f, so
+// they are 8 contiguous bytes of one plane, and the rows are width_step bytes apart in it (width_step % 8 == 0: one
+// word alignment for all 8 rows).  Each plane ends with POOL_PAD or more zero bytes (P of indices past the grid):
+// the corners of an interior window lie within WIN_GUARD - 16 flat bytes (28 plane bytes) of the grid, and the
+// three-word read that fetches 8 of them reaches at most 4 bytes past the last one, so an interior beam reads zeros
+// there and never enters the next plane.  pool_bytes is what the bound pass stages, pool_pitch the stride.
+constexpr int POOL_PAD = 32;
 inline int pool_lead(int width_step) { return 4 * width_step; }
-inline int pool_bytes(const b2s_grid_info &g) { return (pool_lead(g.width_step) + g.data_size + 15) & ~15; }
+inline int pool_plane(const b2s_grid_info &g) { return ((pool_lead(g.width_step) + g.data_size) / 4 + POOL_PAD + 15) & ~15; }
+inline int pool_bytes(const b2s_grid_info &g) { return 4 * pool_plane(g); }
 inline size_t pool_pitch(const b2s_grid_info &g) { return ((size_t)pool_bytes(g) + 127) & ~(size_t)127; }
+// the byte of the staged pooled image that holds P[f]
+__host__ __device__ __forceinline__ int pool_index(int f, int lead, int plane) {
+  const int j = f + lead;
+  return (j & 3) * plane + (j >> 2);
+}
 // the pooled image and its guards fit in k_sweep_bound's shared memory (k_sweep_bound's static shared memory is below
 // k_sweep_window's, so the window kernel's budget covers it)
 inline bool pool_fits(const b2s_grid_info &g, int smem_optin, size_t win_static) {
