@@ -20,7 +20,7 @@
 //   k_add_scans_seq    the same, sequential, when an off-centre smear value reaches 100 (order-dependent) or a base
 //                      scan does not fit in k_add_scan's shared memory
 //   k_grid_sat         per-match summed-area table of the grid's non-empty 4x4 blocks
-//   k_grid_pool        per-match 4x4 max-pooled grid of the angle-pruning bound
+//   k_grid_pool        per-match 4x4 and 7x7 max-pooled grids of the angle-pruning bound
 //   k_bases            candidate lattice -> flat base indices; flags irregular and out-of-grid lattices
 //   k_offsets          per-angle lookup tables                                         (fp64 -> i32)
 //   k_offsets_sorted   window kernel's lists: window origins grouped by row band, byte alignment and interior /
@@ -30,7 +30,7 @@
 //                      one warp per (angle, 32x32 candidate tile), one lane per candidate row; each 32-bit
 //                      shared-memory word feeds 4 adjacent-x candidates (byte-permute into packed u16
 //                      accumulators)                                                    (int, issue bound)
-//   k_sweep_bound, k_prune_probe, k_prune_select
+//   k_sweep_bound (groups, probe, select), k_prune_select, k_count_empty
 //                      angle pruning: an upper bound of every angle's responses from the pooled grid, an exact probe
 //                      of the most promising angles, then k_sweep_window on only the angles that can matter
 //   k_sweep_generic    any lattice / any grid size: one warp per (x,y) candidate, lanes over beams,
@@ -149,7 +149,12 @@ struct b2s_matcher {
   Buf<unsigned long long> d_stats;      // [0] beam-angle pairs dropped as empty windows, [1] angles pruned, last sweep
   HostBuf<unsigned long long> h_stats;  // pinned copy, read back with the results
   Buf<uint8_t> d_pools;                 // [B][pool_pitch] 4x4 max-pooled grids (k_grid_pool), when they fit (pool_fits)
-  Buf<double> d_ubr;                    // [B][nA] angle bounds of a pruned sweep
+  Buf<uint8_t> d_pools7;                // [B][pool7_pitch] 7x7 max-pooled grids of the group pass (pool7_fits)
+  Buf<double> d_ubr;                    // [B][nA] angle bounds of a pruned sweep (NaN: not bounded one by one)
+  Buf<double> d_gub;                    // [B][ceil(nA / BOUND_GROUP)] group bounds of a pruned sweep
+  Buf<int32_t> d_n_eval;                // [B] angles k_prune_select left for k_sweep_bound<BOUND_SELECT>
+  Buf<double> d_cuts;                   // [B] the pruning cut L - 0.1 - 1e-9 of each match
+  Buf<int32_t> d_bscratch;              // [B][nA + groups] k_sweep_bound's angle lists and group order
   Buf<int32_t> d_angles, d_n_angles;    // [B][nA], [B]: the angle lists of a pruned sweep's two exact passes
   Buf<uint8_t> d_keep;                  // [B][nA] angles a pruned sweep swept
   SweepPlan last_plan;                  // of the last sweep
@@ -158,6 +163,7 @@ struct b2s_matcher {
   bool pending = false;                   // a correlate_scan_begin awaits its _end
   int pending_batch = 0;                  // batch size that _begin enqueued
   double last_empty_frac = 0.0;
+  bool empty_pending = false;  // the last sweep was pruned: its empty windows are counted when last_stats asks
   bool grid_high_bytes = false;  // set_grids saw a byte > 127: the packed-byte window kernel is not applicable
   Buf<int32_t> d_sums;
   Buf<int32_t> d_bases;  // [B][ny*nx] candidate base indices
@@ -549,16 +555,20 @@ __global__ void __launch_bounds__(256)
 }
 
 // ----------------------------------------------------------------------------------------------
-// k_grid_pool: per match, the 4x4 max-pooled grid of k_sweep_bound in its four residue planes (layout: pool_lead /
-// pool_plane / pool_index in karto_sweep_plan.cuh).  The pooling is in FLAT index space, rows wrapping exactly as a
-// candidate's `base + offset` does, so the pooled byte at a block's corner is at least every byte a candidate of that
-// block reads.  Thread q pools P[f] for the 16 indices j = f + lead in [16q, 16q + 16) and writes word q of each
-// plane; grid bytes outside [0, data_size) count as 0, so the planes' padding comes out 0.
-// grid(ceil(pool_plane / 1024), B), 256 threads.
+// k_grid_pool<K>: per match, the K x K max-pooled grid (K = 4: P of k_sweep_bound; K = 7: P7 of k_sweep_bound_group)
+// in its four residue planes (layout: pool_lead / pool7_lead, pool_plane / pool7_plane, pool_index in
+// karto_sweep_plan.cuh).  The pooling is in FLAT index space, rows wrapping exactly as a candidate's `base + offset`
+// does, so the pooled byte at a block's corner is at least every byte a candidate of that block reads.  Thread q pools
+// P[f] for the 16 indices j = f + lead in [16q, 16q + 16) and writes word q of each plane; grid bytes outside
+// [0, data_size) count as 0, so the planes' padding comes out 0.
+// grid(ceil(plane / 1024), B), 256 threads.
 // ----------------------------------------------------------------------------------------------
+template <int K>
 __global__ void __launch_bounds__(256)
     k_grid_pool(const uint8_t *__restrict__ grids, size_t grid_pitch, int data_size, int width_step,
                 int lead, int plane, uint8_t *__restrict__ pools, size_t pitch, int batch) {
+  static_assert(K == 4 || K == 7, "4x4 or 7x7 pooling");
+  constexpr int NW = K == 4 ? 5 : 6;  // words per row: the 16 positions and the K - 1 bytes after them
   const int q = blockIdx.x * blockDim.x + threadIdx.x;
   if (q * 4 >= plane) return;
   for (int b = blockIdx.y; b < batch; b += gridDim.y) {
@@ -567,18 +577,21 @@ __global__ void __launch_bounds__(256)
     auto word = [&](int r) { return (r >= 0 && r < data_size) ? __ldg(reinterpret_cast<const uint32_t *>(grid + r)) : 0u; };
     uint32_t m[4] = {0, 0, 0, 0};  // byte r of m[t] = P[f + 4t + r]
 #pragma unroll
-    for (int dy = 0; dy < 4; dy++) {
+    for (int dy = 0; dy < K; dy++) {
       const int r = f + dy * width_step;
-      uint32_t w[5];
+      uint32_t w[NW];
 #pragma unroll
-      for (int t = 0; t < 5; t++) w[t] = word(r + 4 * t);
+      for (int t = 0; t < NW; t++) w[t] = word(r + 4 * t);
+      uint32_t m4[NW - 1];  // byte i of m4[t] = max of row bytes 4t + i .. 4t + i + 3
 #pragma unroll
-      for (int t = 0; t < 4; t++) {
-        // byte i of the row maximum = max of bytes i..i+3 of the 8 bytes w[t + 1]:w[t]
+      for (int t = 0; t < NW - 1; t++) {
         const uint32_t a = __vmaxu4(w[t], __funnelshift_r(w[t], w[t + 1], 8));
         const uint32_t c = __vmaxu4(__funnelshift_r(w[t], w[t + 1], 16), __funnelshift_r(w[t], w[t + 1], 24));
-        m[t] = __vmaxu4(m[t], __vmaxu4(a, c));
+        m4[t] = __vmaxu4(a, c);
       }
+#pragma unroll
+      for (int t = 0; t < 4; t++)  // K = 7: bytes i .. i + 6 = bytes i .. i + 3 and i + 3 .. i + 6
+        m[t] = __vmaxu4(m[t], K == 4 ? m4[t] : __vmaxu4(m4[t], __funnelshift_r(m4[t], m4[t + (K == 4 ? 0 : 1)], 24)));
     }
     // 4 x 4 byte transpose: plane r word q = byte r of m[0..3]
     const uint32_t lo01 = __byte_perm(m[0], m[1], 0x5140), hi01 = __byte_perm(m[0], m[1], 0x7362);
@@ -1177,7 +1190,10 @@ __device__ __forceinline__ float red_fscore(int32_t isum, float apf_k, float dpf
 //                   by the bound itself (beams dropped as empty windows add 0 everywhere).  Same fp64 operations as
 //                   candidate_response, so UBr(k) >= every response of angle k.  No window lists exist yet:
 //                   k_offsets_sorted lists only the angles of the two exact passes below.
-//   k_prune_probe   the PRUNE_PROBE angles with the largest UBr are swept exactly (k_sweep_window on an angle list);
+//                   UBr is computed only where it can matter: a group pass bounds BOUND_GROUP consecutive angles at
+//                   once from a 7x7 pooled image, and the rounds below bound single angles only in groups whose bound
+//                   reaches what they are compared with (see k_sweep_bound's modes).
+//   probe           the PRUNE_PROBE angles with the largest UBr are swept exactly (k_sweep_window on an angle list);
 //   k_prune_select  L = the largest exact response among them (a real candidate, so L <= best); every other angle is
 //                   swept iff UBr(k) >= L - 0.1 - 1e-9.  When L - 0.1 is near 0 (within the 1e-6 band in which a
 //                   response is not penalised, Mapper.cpp:399) every angle is swept.
@@ -1203,48 +1219,74 @@ __device__ __forceinline__ void bound_row(const uint8_t *__restrict__ pb, int ad
 
 constexpr int BOUND_FLUSH = 64 * 32;  // beams placed between flushes of k_sweep_bound's packed corner sums
 
+// What one launch of k_sweep_bound computes (see the angle-pruning comment above):
+//   BOUND_GROUPS  gub[b][g] = a bound of UBr over the BOUND_GROUP consecutive angles of group g, from the 7x7 image P7
+//   BOUND_PROBE   UBr for the top groups by gub (at least PRUNE_PROBE angles), f16 = the PRUNE_PROBE-th largest of
+//                 them, UBr for every other group whose gub reaches f16, then the probe list: the PRUNE_PROBE largest
+//                 UBr of all evaluated angles (ties: lower index).  Every angle not evaluated has UBr <= gub < f16,
+//                 so this is the top PRUNE_PROBE of every angle's UBr.
+//   BOUND_SELECT  UBr for the angles k_prune_select listed (groups not yet evaluated whose gub reaches the cut), and
+//                 of those, the ones whose UBr reaches the cut join the kept list
+enum { BOUND_GROUPS = 0, BOUND_PROBE = 1, BOUND_SELECT = 2 };
+
 // One persistent CTA per match at a time (like k_sweep_window): the pooled image (its four residue planes, see
-// pool_index) is staged by TMA, warps take angles.  ubr[b][k] = UBr(k) (-1 for a match the window kernel does not
-// sweep).  The bound reads no window lists: for each angle a warp places 32 beams at a time, one per lane, with
-// win_origin_class (the definition k_offsets_sorted lists them by), drops the ones the lists would drop, and compacts
-// the interior and the edge ones into its staging row.  Which beams add is the same set as in the lists and integer
-// sums commute, so UBr is the one the lists would give.  It also counts the empty windows of every (beam, angle) pair
-// into stats[0], as the lists of a sweep that is not pruned do.
+// pool_index) is staged by TMA, warps take units (an angle, or a group of BOUND_GROUP angles).  The bound reads no
+// window lists: for each unit a warp places 32 beams at a time, one per lane, and compacts the interior and the edge
+// ones into its staging row.
+//   One angle: the beam's window origin and class by win_origin_class (the definition k_offsets_sorted lists them
+//   by), dropping the ones the lists would drop.  Which beams add is the same set as in the lists and integer sums
+//   commute, so UBr is the one the lists would give.
+//   A group: the beam's origins at the group's angles are bracketed per axis in fp32 with a margin far above fp32's
+//   error (a beam's lookup value is a few hundred cells at most), rounded outwards the way kround can round.  When
+//   both brackets span at most BOUND_SPREAD cells, the beam adds P7 at the bracket's low corner: P7 there covers P at
+//   every member's origin, flat index and row wrap included.  Otherwise (long ranges, coarse angle steps, far or
+//   non-finite points) the beam adds the largest P7 over the members' exact origins.  Beams whose windows are empty
+//   are kept (they only loosen the bound), and the range test decides edge beams as before.
 //
 // Interior beams, four at a time: lane L = slot * 8 + row takes beam `slot` of the four and adds its 8 block corners
 // of block row `row` (8 contiguous plane bytes) as two words, one byte per block column.  Two beams' words add
-// bytewise without carry (the window kernel runs only on grids of bytes <= 127, so P <= 127), and each pair goes into
-// a plain u32 sum and, through one byte permute, a sum of bytes 1 and 3 in u16 lanes; the plain sum less the latter
-// shifted by 8 leaves bytes 0 and 2 in u16 lanes.  A slot takes at most 8 beams per 32 placed, 8 x 127 per u16 lane,
-// so the sums are flushed into the per-column u32 totals every BOUND_FLUSH beams placed (64 x 1016 < 65536) and at
-// the end of the angle.  The totals of the four slots are then summed by shuffles so that lane L ends with blocks
-// (L % 8, 2 (L / 8)) and (L % 8, 2 (L / 8) + 1).  Edge beams and the last 0..3 interior ones read P byte by byte
-// with the range test, at the lane's own two blocks (the value of an interior one is the same either way).
-// STAGE (SweepPlan::bound_stage): the scan-local points and the summed-area table sit in shared memory after the
-// pooled image; otherwise they are read from global memory through L1.
-template <bool STAGE>
+// bytewise without carry (the window kernel runs only on grids of bytes <= 127, so P, P7 <= 127), and each pair goes
+// into a plain u32 sum and, through one byte permute, a sum of bytes 1 and 3 in u16 lanes; the plain sum less the
+// latter shifted by 8 leaves bytes 0 and 2 in u16 lanes.  A slot takes at most 8 beams per 32 placed, 8 x 127 per u16
+// lane, so the sums are flushed into the per-column u32 totals every BOUND_FLUSH beams placed (64 x 1016 < 65536)
+// and at the end of the unit.  The totals of the four slots are then summed by shuffles so that lane L ends with
+// blocks (L % 8, 2 (L / 8)) and (L % 8, 2 (L / 8) + 1).  Edge beams and the last 0..3 interior ones read P byte by
+// byte with the range test, at the lane's own two blocks (the value of an interior one is the same either way).
+// The value of a unit is candidate_response's fp64 operations on the block's sum, the block's largest distance
+// penalty and the unit's largest angle penalty, so it is at least every response of every angle of the unit.
+// STAGE (SweepPlan::bound_stage / group_stage): the scan-local points (and for single angles the summed-area table)
+// sit in shared memory after the pooled image; otherwise they are read from global memory through L1.
+template <bool STAGE, int MODE>
 __global__ void __launch_bounds__(WIN_THREADS, 1)
     k_sweep_bound(const uint8_t *__restrict__ pools, size_t pool_pitch_, int pool_bytes_, int plane, int lead,
                   const double *__restrict__ local, const double *__restrict__ grid_off,
                   const int32_t *__restrict__ bases, const uint16_t *__restrict__ sat_all, int sbx, int sby,
                   int height, int rows_total, int cols_total, double scale, const int32_t *__restrict__ flags,
                   const double *__restrict__ centers, b2s_matcher_params p, b2s_search s, int batch, int n, int na,
-                  int nx, int ny, int width_step, int data_size, double *__restrict__ ubr, int *__restrict__ work_counter,
-                  unsigned long long *__restrict__ stats) {
+                  int nx, int ny, int width_step, int data_size, double *__restrict__ ubr, double *__restrict__ gub,
+                  int32_t *__restrict__ angles, int32_t *__restrict__ n_angles, uint8_t *__restrict__ keep,
+                  const int32_t *__restrict__ n_eval, const double *__restrict__ cuts,
+                  unsigned long long *__restrict__ pruned_total, int32_t *__restrict__ scratch,
+                  int *__restrict__ work_counter) {
+  constexpr bool GRP = MODE == BOUND_GROUPS;
+  constexpr int NJ = GRP ? BOUND_GROUP : 1;  // angles per unit
   // [WIN_GUARD zeros][pooled image][WIN_GUARD zeros] (+ STAGE: [n] x, [n] y of the scan-local points, the SAT)
   extern __shared__ __align__(128) unsigned char smem[];
   __shared__ uint64_t bar;
-  __shared__ int s_unit;
+  __shared__ int s_unit, s_cnt, s_top;
+  __shared__ double s_f16;
   __shared__ __align__(16) int32_t s_offsets[WIN_THREADS / 32][32];
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   int32_t *s_off = s_offsets[warp];
   const bool pen = s.do_penalize != 0;
   const int SW = sbx + 1;
   const int sat_len = ((sby + 1) * SW + 7) & ~7;  // entries per match, padded to 16 bytes
+  const int ng = (na + BOUND_GROUP - 1) / BOUND_GROUP;
+  // the match's list of angles to bound and (BOUND_PROBE) its groups by bound, largest first, in global memory
+  // (scratch[b][na + ng]): shared memory beside the pooled image is budgeted for k_sweep_window's static arrays only
   double *s_lx = reinterpret_cast<double *>(smem + WIN_GUARD + pool_bytes_ + WIN_GUARD), *s_ly = s_lx + n;
   uint16_t *s_sat = reinterpret_cast<uint16_t *>(s_ly + n);
   const unsigned lanes_below = (1u << lane) - 1u;
-  unsigned long long empties = 0;
   // the largest distance penalty of the candidates of block (by, bx), as k_reduce computes sq and candidate_response
   // the penalty (-1: the block holds no candidate)
   auto block_dpen = [&](int by, int bx) {
@@ -1270,6 +1312,12 @@ __global__ void __launch_bounds__(WIN_THREADS, 1)
   const double D = (double)((uint32_t)n * (uint32_t)GRID_OCCUPIED);
   const uint8_t *pb = smem + WIN_GUARD;  // the staged pooled image
   const uint32_t limit = (uint32_t)(lead + data_size);
+  const float scf = (float)scale;
+  // P (P7) at flat index a + corner, modulo 2^32 like the reference's base + offset; 0 outside the grid
+  auto pool_at = [&](int32_t a, int off) -> uint32_t {
+    const uint32_t fa = (uint32_t)a + (uint32_t)off;
+    return (fa + (uint32_t)lead < limit) ? pb[pool_index((int32_t)fa, lead, plane)] : 0u;
+  };
   uint32_t parity = 0;
   while (true) {
     if (threadIdx.x == 0) s_unit = atomicAdd(work_counter, 1);
@@ -1277,8 +1325,18 @@ __global__ void __launch_bounds__(WIN_THREADS, 1)
     const int b = s_unit;
     if (b >= batch) break;
     const int f = flags[b];
-    if ((f & 2) || !(f & 1)) {
-      for (int k = threadIdx.x; k < na; k += blockDim.x) ubr[(size_t)b * na + k] = -1.0;
+    if ((f & 2) || !(f & 1)) {  // not swept by the window kernel: no list, every angle kept (the generic kernel)
+      if (MODE == BOUND_PROBE) {
+        for (int k = threadIdx.x; k < na; k += blockDim.x) keep[(size_t)b * na + k] = 1;
+        if (threadIdx.x == 0) n_angles[b] = 0;
+      }
+      __syncthreads();
+      continue;
+    }
+    const int nev = MODE == BOUND_SELECT ? n_eval[b] : 0;
+    int32_t *s_list = scratch + (size_t)b * (na + ng), *s_order = s_list + na;
+    const double *s_gub = gub + (size_t)b * ng;
+    if (MODE == BOUND_SELECT && nev == 0) {  // nothing to bound: the kept list is final
       __syncthreads();
       continue;
     }
@@ -1301,15 +1359,56 @@ __global__ void __launch_bounds__(WIN_THREADS, 1)
         for (int i = threadIdx.x; i < sat_len / 8; i += blockDim.x)
           reinterpret_cast<uint4 *>(s_sat)[i] = reinterpret_cast<const uint4 *>(g_sat)[i];
     }
+    if (MODE == BOUND_PROBE) {  // round (a): the top groups by bound, until they hold PRUNE_PROBE angles
+      for (int k = threadIdx.x; k < na; k += blockDim.x) ubr[(size_t)b * na + k] = __longlong_as_double(0x7ff8000000000000ll);
+      __syncthreads();
+      for (int g = threadIdx.x; g < ng; g += blockDim.x) {
+        const double u = s_gub[g];
+        int rank = 0;
+        for (int h = 0; h < ng; h++) rank += (s_gub[h] > u) || (s_gub[h] == u && h < g);
+        s_order[rank] = g;
+      }
+      __syncthreads();
+      if (threadIdx.x == 0) {
+        int cnt = 0, r = 0;
+        while (cnt < min(PRUNE_PROBE, na)) {
+          const int g = s_order[r++];
+          for (int k = g * BOUND_GROUP; k < min(g * BOUND_GROUP + BOUND_GROUP, na); k++) s_list[cnt++] = k;
+        }
+        s_top = r;
+        s_cnt = cnt;
+      }
+    } else if (MODE == BOUND_SELECT) {  // the list k_prune_select left at the end of the match's angle list
+      for (int j = threadIdx.x; j < nev; j += blockDim.x) s_list[j] = angles[(size_t)b * na + na - nev + j];
+    }
     const WinGeom G = win_geom(grid_off[2 * b], grid_off[2 * b + 1], scale, bases[(size_t)b * nx * ny], 1, rows_total,
                                cols_total, width_step, data_size, height, nx, ny, 1, 1, 0);
+    // fp32 margin of a group's origin brackets, in cells: fp32's error of the rotation and of the products (far below
+    // 1e-5 of |x| + |y| in cells) and the (o + gridOffset) - gridOffset double rounding of the exact lookup value
+    const float mg_match = 4e-3f + (float)(1e-15 * (fabs(G.gox) + fabs(G.goy)) * scale);
     mbar_wait(&bar, parity);
     parity ^= 1;
     __syncthreads();
     const double ch = centers[3 * b + 2];
-    for (int k = warp; k < na; k += WIN_THREADS / 32) {
-      const double angle = win_angle(ch, s.angle_offset, s.angle_res, k);
-      const double cosine = cos(angle), sine = sin(angle);
+
+    // the bound of angles k0 .. k0 + cnt - 1 (cnt = 1 unless GRP), in every lane
+    auto bound_unit = [&](int k0, int cnt) -> double {
+      double cd[NJ], sd[NJ];
+      float cf[NJ], sf[NJ];
+      double apen = GRP ? -1.0 : 1.0;
+#pragma unroll
+      for (int j = 0; j < NJ; j++) {
+        const double angle = win_angle(ch, s.angle_offset, s.angle_res, k0 + min(j, cnt - 1));
+        cd[j] = cos(angle);
+        sd[j] = sin(angle);
+        cf[j] = (float)cd[j];
+        sf[j] = (float)sd[j];
+        if (pen) {
+          const double sq_a = (angle - ch) * (angle - ch);
+          const double ap = dmax(1.0 - (ANGLE_PENALTY_GAIN * sq_a / p.angle_variance_penalty), p.minimum_angle_penalty);
+          apen = GRP ? dmax(apen, ap) : ap;
+        }
+      }
       uint32_t ua = 0, ub = 0;               // the lane's two blocks, beams read with the range test
       uint32_t s0 = 0, s1 = 0, o0 = 0, o1 = 0;  // interior pairs: plain sums and byte 1 / 3 sums of columns 0..3, 4..7
       uint32_t t[8] = {0, 0, 0, 0, 0, 0, 0, 0};  // interior totals of the lane's slot and row, per block column
@@ -1317,17 +1416,55 @@ __global__ void __launch_bounds__(WIN_THREADS, 1)
         const int i = i0 + lane;
         int cls = 255;
         int32_t a = 0;
-        bool empty = false;
+        bool fb = false;           // GRP: the beam adds the largest P7 over its members' exact origins ...
+        int32_t fa[NJ];            // ... these (WIN_SKIP: the member's window is wholly outside the grid)
         if (i < n) {
           const double plx = STAGE ? s_lx[i] : __ldg(g_pts + 2 * i), ply = STAGE ? s_ly[i] : __ldg(g_pts + 2 * i + 1);
-          cls = win_origin_class(plx, ply, cosine, sine, G, sat_all != nullptr, STAGE ? s_sat : g_sat, SW, a, empty);
+          if (!GRP) {
+            bool empty;
+            cls = win_origin_class(plx, ply, cd[0], sd[0], G, sat_all != nullptr, STAGE ? s_sat : g_sat, SW, a, empty);
+          } else {
+            const float px = (float)plx, py = (float)ply;
+            float xl = INFINITY, xh = -INFINITY, yl = INFINITY, yh = -INFINITY;
+#pragma unroll
+            for (int j = 0; j < NJ; j++) {
+              const float x = cf[j] * px - sf[j] * py, y = sf[j] * px + cf[j] * py;
+              xl = fminf(xl, x); xh = fmaxf(xh, x); yl = fminf(yl, y); yh = fmaxf(yh, y);
+            }
+            const float mg = mg_match + 1e-5f * (fabsf(px) + fabsf(py)) * scf;
+            xl = xl * scf - mg; xh = xh * scf + mg; yl = yl * scf - mg; yh = yh * scf + mg;
+            // kround(v) lies in [ceil(v - 0.5), floor(v + 0.5)], both monotone in v
+            if (fabsf(xl) < 8192.f && fabsf(xh) < 8192.f && fabsf(yl) < 8192.f && fabsf(yh) < 8192.f) {
+              const int mx = (int)ceilf(xl - 0.5f), Mx = (int)floorf(xh + 0.5f);
+              const int my = (int)ceilf(yl - 0.5f), My = (int)floorf(yh + 0.5f);
+              if (Mx - mx <= BOUND_SPREAD && My - my <= BOUND_SPREAD) {
+                a = (int32_t)((uint32_t)G.base00 + (uint32_t)mx + (uint32_t)my * (uint32_t)width_step);
+                const long long last = (long long)a + 28ll * width_step + 28;  // the last corner
+                if (last < -lead || a >= data_size) cls = 255;                  // every corner reads 0
+                else if (a >= -lead && last <= (long long)data_size + 4 * (POOL_PAD - 8)) cls = 0;  // in the planes
+                else cls = 4;
+              } else {
+                fb = true;
+              }
+            } else {
+              fb = true;
+            }
+            if (fb) {
+#pragma unroll
+              for (int j = 0; j < NJ; j++) {
+                int32_t aj;
+                bool empty;
+                const int c = j < cnt ? win_origin_class(plx, ply, cd[j], sd[j], G, false, nullptr, SW, aj, empty) : 255;
+                fa[j] = c < 255 ? aj : WIN_SKIP;
+              }
+            }
+          }
         }
-        empties += empty;
-        // Interior windows lie within WIN_GUARD - 16 bytes of the grid, so every corner they read is inside the staged
-        // planes or their zero padding.  The staging row holds the first n4 of them (a multiple of 4) as image
-        // addresses: beam q < n8 at 8 (q / 8) + 2 (q % 4) + (q / 4) % 2, so that one load gives a lane its slot's two
-        // beams of a group of 8, and a last group of 4 at q.  From n4 on it holds the origins of the other 0..3 and of
-        // the edge ones, padded to a multiple of 4 with an origin far outside the grid.
+        // Interior windows lie within WIN_GUARD - 16 bytes of the grid (a group's low corner: within the planes), so
+        // every corner they read is inside the staged planes or their zero padding.  The staging row holds the first
+        // n4 of them (a multiple of 4) as image addresses: beam q < n8 at 8 (q / 8) + 2 (q % 4) + (q / 4) % 2, so that
+        // one load gives a lane its slot's two beams of a group of 8, and a last group of 4 at q.  From n4 on it holds
+        // the origins of the other 0..3 and of the edge ones, padded to a multiple of 4 with an origin far outside.
         const unsigned m_int = __ballot_sync(0xffffffffu, cls < 4), m_edge = __ballot_sync(0xffffffffu, cls >= 4 && cls < 8);
         const int n_int = __popc(m_int), n8 = n_int & ~7, n4 = n_int & ~3, n_chk = n_int + __popc(m_edge) - n4;
         __syncwarp();
@@ -1370,10 +1507,23 @@ __global__ void __launch_bounds__(WIN_THREADS, 1)
           const int4 a4 = *reinterpret_cast<const int4 *>(s_off + j);  // one broadcast load: four window origins
           const int32_t as[4] = {a4.x, a4.y, a4.z, a4.w};
 #pragma unroll
-          for (int q = 0; q < 4; q++) {  // flat index a + corner, modulo 2^32 like the reference's base + offset; P is 0 outside
-            const uint32_t fa = (uint32_t)as[q] + (uint32_t)off_a, fb = (uint32_t)as[q] + (uint32_t)off_b;
-            ua += (fa + (uint32_t)lead < limit) ? pb[pool_index((int32_t)fa, lead, plane)] : 0u;
-            ub += (fb + (uint32_t)lead < limit) ? pb[pool_index((int32_t)fb, lead, plane)] : 0u;
+          for (int q = 0; q < 4; q++) {
+            ua += pool_at(as[q], off_a);
+            ub += pool_at(as[q], off_b);
+          }
+        }
+        if (GRP) {
+          for (unsigned m_fb = __ballot_sync(0xffffffffu, fb); m_fb; m_fb &= m_fb - 1) {
+            const int src = __ffs(m_fb) - 1;
+            uint32_t va = 0, vb = 0;
+#pragma unroll
+            for (int j = 0; j < NJ; j++) {
+              const int32_t aj = __shfl_sync(0xffffffffu, fa[j], src);
+              va = max(va, pool_at(aj, off_a));
+              vb = max(vb, pool_at(aj, off_b));
+            }
+            ua += va;
+            ub += vb;
           }
         }
       }
@@ -1391,64 +1541,120 @@ __global__ void __launch_bounds__(WIN_THREADS, 1)
         }
       }
       // candidate_response's operations, with the block's largest sum and largest distance penalty
-      double apen = 1.0;
-      if (pen) {
-        const double sq_a = (angle - ch) * (angle - ch);
-        apen = dmax(1.0 - (ANGLE_PENALTY_GAIN * sq_a / p.angle_variance_penalty), p.minimum_angle_penalty);
-      }
       double r = -1.0;
       if (dpen_a >= 0.0) r = dmax(r, pen ? ((double)ua / D) * (dpen_a * apen) : (double)ua / D);
       if (dpen_b >= 0.0) r = dmax(r, pen ? ((double)ub / D) * (dpen_b * apen) : (double)ub / D);
 #pragma unroll
       for (int d = 16; d > 0; d >>= 1) r = dmax(r, __shfl_xor_sync(0xffffffffu, r, d));
-      if (lane == 0) ubr[(size_t)b * na + k] = r;
+      return r;
+    };
+    // the angles at list positions [j0, j1), one per warp
+    auto bound_list = [&](int j0, int j1) {
+      for (int j = j0 + warp; j < j1; j += WIN_THREADS / 32) {
+        const int k = s_list[j];
+        const double r = bound_unit(k, 1);
+        if (lane == 0) ubr[(size_t)b * na + k] = r;
+      }
+    };
+
+    if (GRP) {
+      for (int g = warp; g < ng; g += WIN_THREADS / 32) {
+        const double r = bound_unit(g * BOUND_GROUP, min(BOUND_GROUP, na - g * BOUND_GROUP));
+        if (lane == 0) gub[(size_t)b * ng + g] = r;
+      }
+    } else if (MODE == BOUND_PROBE) {
+      const int T = min(PRUNE_PROBE, na);
+      const int n_a = s_cnt;
+      bound_list(0, n_a);
+      __syncthreads();
+      // f16: the T-th largest bound of round (a)
+      for (int j = threadIdx.x; j < n_a; j += blockDim.x) {
+        const double u = ubr[(size_t)b * na + s_list[j]];
+        int rank = 0;
+        for (int h = 0; h < n_a; h++) {
+          const double v = ubr[(size_t)b * na + s_list[h]];
+          rank += (v > u) || (v == u && h < j);
+        }
+        if (rank == T - 1) s_f16 = u;
+      }
+      __syncthreads();
+      // round (b): every other group whose bound reaches f16
+      const double f16 = s_f16;
+      for (int r = s_top + threadIdx.x; r < ng; r += blockDim.x) {
+        const int g = s_order[r];
+        if (s_gub[g] >= f16) {
+          const int k1 = min(g * BOUND_GROUP + BOUND_GROUP, na);
+          const int pos = atomicAdd(&s_cnt, k1 - g * BOUND_GROUP);
+          for (int k = g * BOUND_GROUP; k < k1; k++) s_list[pos + k - g * BOUND_GROUP] = k;
+        }
+      }
+      __syncthreads();
+      const int n_ab = s_cnt;
+      bound_list(n_a, n_ab);
+      for (int k = threadIdx.x; k < na; k += blockDim.x) keep[(size_t)b * na + k] = 0;
+      __syncthreads();
+      // the probe: the T largest bounds of all evaluated angles, ties to the lower index
+      for (int j = threadIdx.x; j < n_ab; j += blockDim.x) {
+        const int k = s_list[j];
+        const double u = ubr[(size_t)b * na + k];
+        int rank = 0;
+        for (int h = 0; h < n_ab; h++) {
+          const int kh = s_list[h];
+          const double v = ubr[(size_t)b * na + kh];
+          rank += (v > u) || (v == u && kh < k);
+        }
+        if (rank < T) {
+          angles[(size_t)b * na + rank] = k;
+          keep[(size_t)b * na + k] = 1;
+        }
+      }
+      if (threadIdx.x == 0) n_angles[b] = T;
+    } else {  // BOUND_SELECT
+      bound_list(0, nev);
+      if (threadIdx.x == 0) s_cnt = n_angles[b];
+      __syncthreads();
+      const double cut = cuts[b];
+      int pruned = 0;
+      for (int j = threadIdx.x; j < nev; j += blockDim.x) {
+        const int k = s_list[j];
+        if (ubr[(size_t)b * na + k] >= cut) {
+          angles[(size_t)b * na + atomicAdd(&s_cnt, 1)] = k;
+          keep[(size_t)b * na + k] = 1;
+        } else {
+          pruned++;
+        }
+      }
+      if (pruned) atomicAdd(pruned_total, (unsigned long long)pruned);
+      __syncthreads();
+      if (threadIdx.x == 0) n_angles[b] = s_cnt;
     }
     __syncthreads();  // everyone is done with the image before the next match's copy is issued
   }
-#pragma unroll
-  for (int d = 16; d > 0; d >>= 1) empties += __shfl_xor_sync(0xffffffffu, empties, d);
-  if (lane == 0 && empties) atomicAdd(stats, empties);
-}
-
-// The PRUNE_PROBE angles with the largest bounds (ties: lower index first) become match b's first angle list; keep[b][k]
-// marks the angles that will have been swept.  A match the window kernel does not sweep gets an empty list and an
-// all-ones mask (the generic kernel fills its whole volume).  One CTA per match.
-__global__ void __launch_bounds__(256)
-    k_prune_probe(const double *__restrict__ ubr, const int32_t *__restrict__ flags, int na,
-                  int32_t *__restrict__ angles, int32_t *__restrict__ n_angles, uint8_t *__restrict__ keep) {
-  const int b = blockIdx.x;
-  __shared__ double s_u[PRUNE_MAX_ANGLES];
-  const int f = flags[b];
-  const bool swept = !(f & 2) && (f & 1);
-  for (int k = threadIdx.x; k < na; k += blockDim.x) s_u[k] = ubr[(size_t)b * na + k];
-  __syncthreads();
-  const int T = min(PRUNE_PROBE, na);
-  for (int k = threadIdx.x; k < na; k += blockDim.x) {
-    const double u = s_u[k];
-    int rank = 0;
-    for (int j = 0; j < na; j++) rank += (s_u[j] > u) || (s_u[j] == u && j < k);
-    if (swept && rank < T) angles[(size_t)b * na + rank] = k;
-    keep[(size_t)b * na + k] = !swept || rank < T;
-  }
-  if (threadIdx.x == 0) n_angles[b] = swept ? T : 0;
 }
 
 // L from the probe's exact sums, then match b's second angle list: the angles not probed whose bound reaches
-// L - 0.1 - 1e-9.  pruned_total += the angles left out.  One CTA per match.
+// L - 0.1 - 1e-9.  An angle the probe round did not bound (ubr NaN) has UBr <= the bound of its group: when that is
+// below the cut the angle is pruned, otherwise it is listed at the end of the match's angle list (n_eval[b] of them)
+// for k_sweep_bound<BOUND_SELECT>, which bounds it and keeps it by the same rule.  pruned_total += the angles left
+// out here.  One CTA per match.
 __global__ void __launch_bounds__(256)
-    k_prune_select(const int32_t *__restrict__ sums, const double *__restrict__ ubr, const double *__restrict__ centers,
-                   const int32_t *__restrict__ flags, b2s_matcher_params p, b2s_search s, int n, int nx, int ny, int na,
-                   int32_t *__restrict__ angles, int32_t *__restrict__ n_angles, uint8_t *__restrict__ keep,
-                   unsigned long long *__restrict__ pruned_total) {
+    k_prune_select(const int32_t *__restrict__ sums, const double *__restrict__ ubr, const double *__restrict__ gub,
+                   const double *__restrict__ centers, const int32_t *__restrict__ flags, b2s_matcher_params p,
+                   b2s_search s, int n, int nx, int ny, int na, int32_t *__restrict__ angles,
+                   int32_t *__restrict__ n_angles, uint8_t *__restrict__ keep, int32_t *__restrict__ n_eval,
+                   double *__restrict__ cuts, unsigned long long *__restrict__ pruned_total) {
   const int b = blockIdx.x;
   const int f = flags[b];
-  if ((f & 2) || !(f & 1)) return;  // n_angles[b] is still 0, keep[b] all ones
+  if ((f & 2) || !(f & 1)) {  // n_angles[b] is still 0, keep[b] all ones
+    if (threadIdx.x == 0) n_eval[b] = 0;
+    return;
+  }
   __shared__ int32_t s_probe[PRUNE_PROBE];
   __shared__ double s_red[256];
-  __shared__ int s_cnt;
-  const int T = n_angles[b], ncell = nx * ny;
+  __shared__ int s_cnt, s_ev;
+  const int T = n_angles[b], ncell = nx * ny, ng = (na + BOUND_GROUP - 1) / BOUND_GROUP;
   if (threadIdx.x < T) s_probe[threadIdx.x] = angles[(size_t)b * na + threadIdx.x];
-  if (threadIdx.x == 0) s_cnt = 0;
+  if (threadIdx.x == 0) s_cnt = s_ev = 0;
   __syncthreads();
   const bool pen = s.do_penalize != 0;
   const double ch = centers[3 * b + 2];
@@ -1473,16 +1679,59 @@ __global__ void __launch_bounds__(256)
   int pruned = 0;
   for (int k = threadIdx.x; k < na; k += blockDim.x) {
     if (keep[(size_t)b * na + k]) continue;  // probed
-    if (all || ubr[(size_t)b * na + k] >= cut) {
+    const double u = ubr[(size_t)b * na + k];
+    if (all || u >= cut) {
       angles[(size_t)b * na + atomicAdd(&s_cnt, 1)] = k;
       keep[(size_t)b * na + k] = 1;
+    } else if (isnan(u) && gub[(size_t)b * ng + k / BOUND_GROUP] >= cut) {
+      angles[(size_t)b * na + na - 1 - atomicAdd(&s_ev, 1)] = k;
     } else {
       pruned++;
     }
   }
   if (pruned) atomicAdd(pruned_total, (unsigned long long)pruned);
   __syncthreads();
-  if (threadIdx.x == 0) n_angles[b] = s_cnt;
+  if (threadIdx.x == 0) {
+    n_angles[b] = s_cnt;
+    n_eval[b] = s_ev;
+    cuts[b] = cut;
+  }
+}
+
+// The empty windows of the last pruned sweep, counted when they are asked for (b2s_matcher_last_stats): every
+// (beam, angle) pair of every match the window kernel swept, placed by win_origin_class as the lists would place it.
+// The pruned sweep itself places only the beams of the angles it bounds one by one.  One block per (match, chunk of
+// OFF_CHUNK angles).
+__global__ void __launch_bounds__(256)
+    k_count_empty(const double *__restrict__ local, const double *__restrict__ grid_off,
+                  const double *__restrict__ centers, const int32_t *__restrict__ bases,
+                  const int32_t *__restrict__ flags, const uint16_t *__restrict__ sat_all, int sbx, int sby,
+                  double angle_offset, double angle_res, int na, int n, int ncell, int width_step, int data_size,
+                  double scale, int rows_total, int cols_total, int height, int nx, int ny,
+                  unsigned long long *__restrict__ stats) {
+  const int chunks = (na + OFF_CHUNK - 1) / OFF_CHUNK;
+  const int b = blockIdx.x / chunks, k0 = (blockIdx.x % chunks) * OFF_CHUNK;
+  const int f = flags[b];
+  if ((f & 2) || !(f & 1)) return;
+  const int SW = sbx + 1;
+  const uint16_t *sat = sat_all + (size_t)b * (((sby + 1) * SW + 7) & ~7);
+  const WinGeom G = win_geom(grid_off[2 * b], grid_off[2 * b + 1], scale, bases[(size_t)b * ncell], 1, rows_total,
+                             cols_total, width_step, data_size, height, nx, ny, 1, 1, 0);
+  const double center = centers[(size_t)b * 3 + 2];
+  unsigned long long cnt = 0;
+  for (int k = k0; k < min(k0 + OFF_CHUNK, na); k++) {
+    const double ang = win_angle(center, angle_offset, angle_res, k);
+    const double c = cos(ang), sn = sin(ang);
+    for (int i = threadIdx.x; i < n; i += blockDim.x) {
+      int32_t a;
+      bool empty;
+      win_origin_class(local[((size_t)b * n + i) * 2], local[((size_t)b * n + i) * 2 + 1], c, sn, G, true, sat, SW, a, empty);
+      cnt += empty;
+    }
+  }
+#pragma unroll
+  for (int d = 16; d > 0; d >>= 1) cnt += __shfl_xor_sync(0xffffffffu, cnt, d);
+  if ((threadIdx.x & 31) == 0 && cnt) atomicAdd(stats, cnt);
 }
 
 __global__ void __launch_bounds__(RED_THREADS, 2) k_reduce(ReduceArgs A) {
@@ -1947,6 +2196,7 @@ static void read_sweep_ms(b2s_matcher *m) {
 static b2s_status run_correlate(b2s_matcher *m, const b2s_search *s, int k_first = 0, int na_override = -1,
                                 ReducePhase phase = REDUCE_WHOLE);
 static b2s_status launch_window(b2s_matcher *m, const SweepPlan &pl, const int32_t *angles);
+static b2s_status count_empty(b2s_matcher *m);
 static b2s_status launch_lists(b2s_matcher *m, const SweepPlan &pl, const b2s_search &s, int k_first, int listed_chunks,
                                bool count_empty);
 
@@ -1966,9 +2216,15 @@ static b2s_status build_sat(b2s_matcher *m) {
 static b2s_status build_pool(b2s_matcher *m) {
   if (!pool_fits(m->g, m->smem_optin, m->win_static_smem)) return B2S_OK;
   const int plane = pool_plane(m->g);
-  k_grid_pool<<<dim3((unsigned)ceil_div(plane / 4, 256), grid_rows(m->batch)), 256, 0, m->stream>>>(
+  k_grid_pool<4><<<dim3((unsigned)ceil_div(plane / 4, 256), grid_rows(m->batch)), 256, 0, m->stream>>>(
       m->d_grids, m->grid_pitch, m->g.data_size, m->g.width_step, pool_lead(m->g.width_step), plane, m->d_pools,
       pool_pitch(m->g), m->batch);
+  if (pool7_fits(m->g, m->smem_optin, m->win_static_smem)) {
+    const int plane7 = pool7_plane(m->g);
+    k_grid_pool<7><<<dim3((unsigned)ceil_div(plane7 / 4, 256), grid_rows(m->batch)), 256, 0, m->stream>>>(
+        m->d_grids, m->grid_pitch, m->g.data_size, m->g.width_step, pool7_lead(m->g.width_step), plane7, m->d_pools7,
+        pool7_pitch(m->g), m->batch);
+  }
   B2S_CUDA_CHECK(cudaGetLastError());
   return B2S_OK;
 }
@@ -2031,6 +2287,7 @@ static b2s_status matcher_create_impl(const b2s_matcher_params *params, const b2
   B2S_CUDA_CHECK(m->d_sat.reserve(B * sat_stride(m->sbx, m->sby)));
   B2S_CUDA_CHECK(m->d_stats.reserve(2));
   if (pool_fits(g, m->smem_optin, m->win_static_smem)) B2S_CUDA_CHECK(m->d_pools.reserve(B * pool_pitch(g)));
+  if (pool7_fits(g, m->smem_optin, m->win_static_smem)) B2S_CUDA_CHECK(m->d_pools7.reserve(B * pool7_pitch(g)));
   B2S_CUDA_CHECK(m->d_part_best.reserve(B));
   B2S_CUDA_CHECK(m->d_glob_best.reserve(B));
   B2S_CUDA_CHECK(m->d_tie.reserve(B * 5));
@@ -2289,6 +2546,7 @@ b2s_status b2s_matcher_correlate_scan_end(b2s_matcher *m, b2s_match_result *resu
   std::memcpy(results, m->h_results, sizeof(b2s_match_result) * B);
   if (m->last_path == 2 && m->last.na > 0 && m->n > 0) m->last_empty_frac = (double)*m->h_stats / ((double)B * m->last.na * m->n);
   else m->last_empty_frac = 0.0;
+  m->empty_pending = m->last_pruned && m->last_plan.skip_empty && m->n > 0;  // counted by last_stats
   m->last_pruned_frac = m->last_pruned ? (double)m->h_stats[1] / ((double)B * m->last.na) : 0.0;
   read_sweep_ms(m);
   return B2S_OK;
@@ -2562,6 +2820,16 @@ b2s_status b2s_matcher_get_response_sums(b2s_matcher *m, int b, int32_t *out, in
 
 b2s_status b2s_matcher_last_stats(b2s_matcher *m, double out[4]) {
   if (!m || !out) B2S_FAIL(B2S_ERR_BAD_PARAMS, "null argument");
+  if (m->empty_pending && !m->pending) {
+    // a pruned sweep does not place every (beam, angle) pair: count its empty windows now, from its inputs when they
+    // are still resident (NaN once set_scans / add_scans / set_grids replaced them)
+    m->empty_pending = false;
+    m->last_empty_frac = NAN;
+    if (m->have_sweep) {
+      B2S_CUDA_CHECK(cudaSetDevice(m->device));
+      if (b2s_status st = count_empty(m)) return st;
+    }
+  }
   out[0] = m->last_empty_frac;
   out[1] = (double)m->last_path;
   out[2] = (double)m->last.na * m->last.nx * m->last.ny;
@@ -2630,6 +2898,23 @@ static b2s_status launch_lists(b2s_matcher *m, const SweepPlan &pl, const b2s_se
   return launch(k_offsets_sorted<false>, ceil_div(na, OFF_CHUNK));
 }
 
+// last_empty_frac of the last (pruned) sweep from its resident inputs: k_count_empty over every (beam, angle) pair
+static b2s_status count_empty(b2s_matcher *m) {
+  const SweepPlan &pl = m->last_plan;
+  const b2s_search &s = m->last_search;
+  const int B = m->batch, na = pl.na;
+  B2S_CUDA_CHECK(cudaMemsetAsync(m->d_stats, 0, sizeof(unsigned long long), m->stream));
+  k_count_empty<<<B * ceil_div(na, OFF_CHUNK), 256, 0, m->stream>>>(
+      m->d_local, m->d_grid_off, m->d_centers, m->d_bases, m->d_flags, m->d_sat, m->sbx, m->sby, s.angle_offset,
+      s.angle_res, na, m->n, pl.nx * pl.ny, m->g.width_step, m->g.data_size, 1.0 / m->p.resolution, pl.rows_total,
+      pl.tiles_x * 32, m->g.height, pl.nx, pl.ny, m->d_stats);
+  B2S_CUDA_CHECK(cudaGetLastError());
+  B2S_CUDA_CHECK(cudaMemcpyAsync(m->h_stats, m->d_stats, sizeof(unsigned long long), cudaMemcpyDeviceToHost, m->stream));
+  B2S_CUDA_CHECK(cudaStreamSynchronize(m->stream));
+  m->last_empty_frac = (double)*m->h_stats / ((double)B * na * m->n);
+  return B2S_OK;
+}
+
 // One CorrelateScan over the batch with centres already in d_centers.  Results stay in d_results.
 static b2s_status run_correlate(b2s_matcher *m, const b2s_search *s, int k_first, int na_override, ReducePhase phase) {
   B2S_NVTX("K1 correlate (lists + sweep + tail)");
@@ -2647,8 +2932,13 @@ static b2s_status run_correlate(b2s_matcher *m, const b2s_search *s, int k_first
     B2S_CUDA_CHECK(m->d_counts.reserve((size_t)B * na * 8 * pl.nbands));
     B2S_CUDA_CHECK(m->d_starts.reserve((size_t)B * na * 8 * pl.nbands));
   }
+  m->empty_pending = false;
   if (pl.prune) {
     B2S_CUDA_CHECK(m->d_ubr.reserve((size_t)B * na));
+    B2S_CUDA_CHECK(m->d_gub.reserve((size_t)B * ceil_div(na, BOUND_GROUP)));
+    B2S_CUDA_CHECK(m->d_n_eval.reserve((size_t)B));
+    B2S_CUDA_CHECK(m->d_cuts.reserve((size_t)B));
+    B2S_CUDA_CHECK(m->d_bscratch.reserve((size_t)B * (na + ceil_div(na, BOUND_GROUP))));
     B2S_CUDA_CHECK(m->d_angles.reserve((size_t)B * na));
     B2S_CUDA_CHECK(m->d_n_angles.reserve((size_t)B));
     B2S_CUDA_CHECK(m->d_keep.reserve((size_t)B * na));
@@ -2663,7 +2953,7 @@ static b2s_status run_correlate(b2s_matcher *m, const b2s_search *s, int k_first
                                              s->angle_offset, s->angle_res, na, n, m->g.width_step, scale, m->d_lut, k_first);
   if (lists) {
     B2S_CUDA_CHECK(cudaMemsetAsync(m->d_stats, 0, 2 * sizeof(unsigned long long), m->stream));
-    // a pruned sweep lists only the angles it sweeps, inside the sweep stage; k_sweep_bound counts the empty windows
+    // a pruned sweep lists only the angles it sweeps, inside the sweep stage; its empty windows are counted on request
     if (!pl.prune)
       if (b2s_status st = launch_lists(m, pl, *s, k_first, 0, true)) return st;
   }
@@ -2678,25 +2968,43 @@ static b2s_status run_correlate(b2s_matcher *m, const b2s_search *s, int k_first
     // L2, no k_reduce pass — was built, parity-tested and measured SLOWER on cfg 2 (not re-measured on the H100): the
     // sweep kernel owns its SM, so the tail's serial stretches are no longer hidden by a second resident CTA as they are
     // in the stand-alone k_reduce.  Removed again; DESIGN.md §4.)
-    if (pl.prune) {  // bound, probe, select, sweep the selected angles (see k_sweep_bound); lists only for those
-      B2S_CUDA_CHECK(cudaMemsetAsync(m->d_work, 0, sizeof(int), m->stream));
-      auto bound = [&](auto kern) -> b2s_status {
-        B2S_CUDA_CHECK(raise_dyn_smem(kern, pl.bound_smem));
-        kern<<<pl.ctas, WIN_THREADS, pl.bound_smem, m->stream>>>(
-            m->d_pools, pool_pitch(m->g), pool_bytes(m->g), pool_plane(m->g), pool_lead(m->g.width_step), m->d_local,
-            m->d_grid_off, m->d_bases, pl.skip_empty ? m->d_sat.p : nullptr, m->sbx, m->sby, m->g.height, pl.rows_total,
-            pl.tiles_x * 32, scale, m->d_flags, m->d_centers, m->p, *s, B, n, na, nx, ny, m->g.width_step,
-            m->g.data_size, m->d_ubr, m->d_work, m->d_stats.p);
+    if (pl.prune) {  // group bounds, then bounds, probe, select, sweep the selected angles (see k_sweep_bound)
+      auto bound = [&](auto kern, const uint8_t *pools, size_t pitch, int bytes, int plane, int lead, bool sat,
+                       size_t smem) -> b2s_status {
+        B2S_CUDA_CHECK(cudaMemsetAsync(m->d_work, 0, sizeof(int), m->stream));
+        B2S_CUDA_CHECK(raise_dyn_smem(kern, smem));
+        kern<<<pl.ctas, WIN_THREADS, smem, m->stream>>>(
+            pools, pitch, bytes, plane, lead, m->d_local, m->d_grid_off, m->d_bases, sat ? m->d_sat.p : nullptr,
+            m->sbx, m->sby, m->g.height, pl.rows_total, pl.tiles_x * 32, scale, m->d_flags, m->d_centers, m->p, *s, B, n,
+            na, nx, ny, m->g.width_step, m->g.data_size, m->d_ubr, m->d_gub, m->d_angles, m->d_n_angles, m->d_keep,
+            m->d_n_eval, m->d_cuts, m->d_stats.p + 1, m->d_bscratch, m->d_work);
+        B2S_CUDA_CHECK(cudaGetLastError());
         return B2S_OK;
       };
-      if (b2s_status st = pl.bound_stage ? bound(k_sweep_bound<true>) : bound(k_sweep_bound<false>)) return st;
-      k_prune_probe<<<B, 256, 0, m->stream>>>(m->d_ubr, m->d_flags, na, m->d_angles, m->d_n_angles, m->d_keep);
-      B2S_CUDA_CHECK(cudaGetLastError());
+      const int pbytes = pool_bytes(m->g), pplane = pool_plane(m->g), plead = pool_lead(m->g.width_step);
+      auto single = [&](auto kern) {
+        return bound(kern, m->d_pools, pool_pitch(m->g), pbytes, pplane, plead, pl.skip_empty, pl.bound_smem);
+      };
+      if (pl.group) {
+        auto group = [&](auto kern) {
+          return bound(kern, m->d_pools7, pool7_pitch(m->g), pool7_bytes(m->g), pool7_plane(m->g),
+                       pool7_lead(m->g.width_step), false, pl.group_smem);
+        };
+        if (b2s_status st = pl.group_stage ? group(k_sweep_bound<true, BOUND_GROUPS>)
+                                           : group(k_sweep_bound<false, BOUND_GROUPS>)) return st;
+      } else {  // every group unbounded (0x7f7f... is a double near 1.4e306): every angle is bounded one by one
+        B2S_CUDA_CHECK(cudaMemsetAsync(m->d_gub, 0x7f, sizeof(double) * (size_t)B * ceil_div(na, BOUND_GROUP), m->stream));
+      }
+      if (b2s_status st = pl.bound_stage ? single(k_sweep_bound<true, BOUND_PROBE>)
+                                         : single(k_sweep_bound<false, BOUND_PROBE>)) return st;
       if (b2s_status st = launch_lists(m, pl, *s, k_first, ceil_div(PRUNE_PROBE, OFF_CHUNK), false)) return st;
       if (b2s_status st = launch_window(m, pl, m->d_angles)) return st;
-      k_prune_select<<<B, 256, 0, m->stream>>>(m->d_sums, m->d_ubr, m->d_centers, m->d_flags, m->p, *s, n, nx, ny, na,
-                                               m->d_angles, m->d_n_angles, m->d_keep, m->d_stats.p + 1);
+      k_prune_select<<<B, 256, 0, m->stream>>>(m->d_sums, m->d_ubr, m->d_gub, m->d_centers, m->d_flags, m->p, *s, n,
+                                               nx, ny, na, m->d_angles, m->d_n_angles, m->d_keep, m->d_n_eval,
+                                               m->d_cuts, m->d_stats.p + 1);
       B2S_CUDA_CHECK(cudaGetLastError());
+      if (b2s_status st = pl.bound_stage ? single(k_sweep_bound<true, BOUND_SELECT>)
+                                         : single(k_sweep_bound<false, BOUND_SELECT>)) return st;
       if (b2s_status st = launch_lists(m, pl, *s, k_first, ceil_div(na, OFF_CHUNK), false)) return st;
       if (b2s_status st = launch_window(m, pl, m->d_angles)) return st;
     } else {

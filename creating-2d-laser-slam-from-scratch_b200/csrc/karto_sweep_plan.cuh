@@ -22,6 +22,11 @@ constexpr size_t LIST_SMEM_MAX = 200 * 1024;  // dynamic shared memory of the li
 constexpr int PRUNE_MIN_ANGLES = 32;    // fewer angles: the bound pass and the probe cost more than they save
 constexpr int PRUNE_MAX_ANGLES = 1024;  // the select kernels and k_reduce's angle mask hold one entry per angle
 constexpr int PRUNE_PROBE = 16;         // angles swept exactly to find the pruning threshold (one per sweep warp)
+// consecutive angles the group pass of the bound takes at once: at cfg 2 a beam's window origin moves at most 2.42
+// cells per axis over 3 angle steps, so the four origins lie in a 4 x 4 cell square and a 7 x 7 pooled image read at
+// the square's low corner bounds all four (k_sweep_bound_group)
+constexpr int BOUND_GROUP = 4;
+constexpr int BOUND_SPREAD = 3;  // the origin spread per axis the 7 x 7 image covers: 7 = 4 + BOUND_SPREAD
 
 // u16 entries per match of the block summed-area tables (k_grid_sat), padded to 16 bytes
 inline size_t sat_stride(int sbx, int sby) { return (size_t)((((sbx + 1) * (sby + 1)) + 7) & ~7); }
@@ -39,6 +44,13 @@ inline int pool_lead(int width_step) { return 4 * width_step; }
 inline int pool_plane(const b2s_grid_info &g) { return ((pool_lead(g.width_step) + g.data_size) / 4 + POOL_PAD + 15) & ~15; }
 inline int pool_bytes(const b2s_grid_info &g) { return 4 * pool_plane(g); }
 inline size_t pool_pitch(const b2s_grid_info &g) { return ((size_t)pool_bytes(g) + 127) & ~(size_t)127; }
+// The 7x7 max-pooled grid of the group pass, P7[f] = max over dy, dx in [0, 7) of grid[f + dy * width_step + dx], in
+// the same four-plane layout (pool_index with pool7_lead / pool7_plane), from f = -pool7_lead on: the low corner of a
+// group's origins lies up to BOUND_SPREAD rows and columns before any member's origin.
+inline int pool7_lead(int width_step) { return 8 * width_step; }
+inline int pool7_plane(const b2s_grid_info &g) { return ((pool7_lead(g.width_step) + g.data_size) / 4 + POOL_PAD + 15) & ~15; }
+inline int pool7_bytes(const b2s_grid_info &g) { return 4 * pool7_plane(g); }
+inline size_t pool7_pitch(const b2s_grid_info &g) { return ((size_t)pool7_bytes(g) + 127) & ~(size_t)127; }
 // the byte of the staged pooled image that holds P[f]
 __host__ __device__ __forceinline__ int pool_index(int f, int lead, int plane) {
   const int j = f + lead;
@@ -48,6 +60,10 @@ __host__ __device__ __forceinline__ int pool_index(int f, int lead, int plane) {
 // k_sweep_window's, so the window kernel's budget covers it)
 inline bool pool_fits(const b2s_grid_info &g, int smem_optin, size_t win_static) {
   return (long long)pool_bytes(g) + 2 * WIN_GUARD <= (long long)smem_optin - (long long)win_static - 512;
+}
+// the same for the 7x7 image of the group pass (whose static shared memory is k_sweep_bound's)
+inline bool pool7_fits(const b2s_grid_info &g, int smem_optin, size_t win_static) {
+  return (long long)pool7_bytes(g) + 2 * WIN_GUARD <= (long long)smem_optin - (long long)win_static - 512;
 }
 // doubles per match of the per-cell maxima plane (m_pSearchSpaceProbs), rows padded to 8
 inline size_t probs_len(int search_side) { return (size_t)((search_side + 7) & ~7) * search_side; }
@@ -95,6 +111,11 @@ struct SweepPlan {
   // table) in shared memory after the pooled image when they fit there, and reads them through L1 otherwise
   bool bound_stage = false;
   size_t bound_smem = 0;  // dynamic shared memory of k_sweep_bound: pooled image + guards (+ points + SAT when staged)
+  // the group pass (k_sweep_bound_group over the 7x7 image) runs first, and k_sweep_bound bounds single angles only
+  // where a group's bound can matter; without it every group counts as unbounded and k_sweep_bound bounds every angle
+  bool group = false;
+  bool group_stage = false;  // the group pass stages the scan-local points after its image
+  size_t group_smem = 0;     // its dynamic shared memory: 7x7 image + guards (+ points when staged)
 };
 
 // shared memory k_sweep_bound stages after its pooled image (bound_stage): n scan-local points and the SAT when used
@@ -183,6 +204,12 @@ inline SweepPlan plan_sweep(const b2s_matcher_params &p, const b2s_grid_info &g,
   const size_t staged = bound_stage_bytes(n, pl.skip_empty, sbx, sby);
   pl.bound_stage = pl.prune && (long long)(pl.bound_smem + staged) <= smem_limit;
   if (pl.bound_stage) pl.bound_smem += staged;
+  pl.group = pl.prune && pool7_fits(g, smem_optin, win_static);
+  pl.group_smem = (size_t)pool7_bytes(g) + 2 * WIN_GUARD;
+  const size_t staged7 = bound_stage_bytes(n, false, sbx, sby);
+  pl.group_stage = pl.group && (long long)(pl.group_smem + staged7) <= smem_limit;
+  if (pl.group_stage) pl.group_smem += staged7;
+  if (!pl.group) pl.group_smem = 0;
   return pl;
 }
 
