@@ -48,6 +48,7 @@
 #include <cstring>
 #include <mutex>
 #include <new>
+#include <type_traits>
 #include <vector>
 
 #include <math_constants.h>
@@ -997,7 +998,7 @@ struct ReduceArgs {
   const double *glob_best;
   double *tie_out;
   const double *tie_in;
-  const uint8_t *keep;  // [B][na] angles swept by a pruned sweep (nullptr: every angle); the others read as 0
+  const uint8_t *keep;  // [B][na] angles swept by a pruned sweep (nullptr: every angle); k_reduce walks only those
 };
 
 
@@ -1168,7 +1169,28 @@ __device__ __forceinline__ double candidate_response(int32_t isum, int n, bool d
   return response;
 }
 
-// float score of a candidate (see k_reduce): relative error < 3e-7 vs candidate_response
+// The float pre-filter of k_reduce and k_prune_select.  apf[k] = anglePenalty(k) / (N * 100) for the angles
+// [0, na) of the launch (k_first + k of the search), the cell factor is red_dist_factor, and red_fscore is a candidate's
+// float score: relative error < 3e-7 vs candidate_response.  A candidate whose score is below red_margin(largest
+// score) cannot have the largest exact response; ambiguous ones (unpenalised response near the 1e-6 DoubleEqual
+// threshold of the penalty test, Mapper.cpp:399) must always be evaluated exactly.
+__device__ __forceinline__ void red_angle_factors(float *apf, int na, int k_first, double start_a, double center_h,
+                                                  double D, bool do_penalize, const b2s_search &s,
+                                                  const b2s_matcher_params &p) {
+  for (int k = threadIdx.x; k < na; k += blockDim.x) {
+    double apen = 1.0;
+    if (do_penalize) {
+      const double angle = start_a + (double)(uint32_t)(k_first + k) * s.angle_res;
+      apen = dmax(1.0 - (ANGLE_PENALTY_GAIN * ((angle - center_h) * (angle - center_h)) / p.angle_variance_penalty), p.minimum_angle_penalty);
+    }
+    apf[k] = (float)(apen / D);
+  }
+}
+
+__device__ __forceinline__ float red_dist_factor(double sq_xy, const b2s_matcher_params &p) {
+  return (float)dmax(1.0 - (DISTANCE_PENALTY_GAIN * sq_xy / p.distance_variance_penalty), p.minimum_distance_penalty);
+}
+
 __device__ __forceinline__ float red_fscore(int32_t isum, float apf_k, float dpf, float inv_d, bool do_penalize,
                                             bool &ambiguous) {
   const float u = (float)isum * inv_d;  // unpenalised response
@@ -1176,6 +1198,8 @@ __device__ __forceinline__ float red_fscore(int32_t isum, float apf_k, float dpf
   if (!do_penalize || u <= 1.0e-6f) return u;
   return (float)isum * apf_k * dpf;
 }
+
+__device__ __forceinline__ float red_margin(float fmax) { return fmax * (1.0f - 2.0e-6f) - 1.0e-30f; }
 
 // ----------------------------------------------------------------------------------------------
 // Angle pruning (SweepPlan::prune: one 32 x 32 stride-1 tile, the whole grid in shared memory, a whole search).
@@ -1194,10 +1218,12 @@ __device__ __forceinline__ float red_fscore(int32_t isum, float apf_k, float dpf
 //                   once from a 7x7 pooled image, and the rounds below bound single angles only in groups whose bound
 //                   reaches what they are compared with (see k_sweep_bound's modes).
 //   probe           the PRUNE_PROBE angles with the largest UBr are swept exactly (k_sweep_window on an angle list);
-//   k_prune_select  L = the largest exact response among them (a real candidate, so L <= best); every other angle is
+//   k_prune_select  L = the largest exact response among them (a real candidate, so L <= best; only the candidates
+//                   k_reduce's float pre-filter leaves are evaluated exactly); every other angle is
 //                   swept iff UBr(k) >= L - 0.1 - 1e-9.  When L - 0.1 is near 0 (within the 1e-6 band in which a
 //                   response is not penalised, Mapper.cpp:399) every angle is swept.
-// k_reduce reads 0 for the angles never swept; the response volume is completed on request (get_response_sums).
+// k_reduce walks only the swept angles (the others would read 0); the response volume is completed on request
+// (get_response_sums).
 // ----------------------------------------------------------------------------------------------
 // bytes c .. c + 3 of the 8 bytes hi:lo, c = sel % 4 (prmt's forward-4-extract mode reads only sel's two low bits)
 __device__ __forceinline__ uint32_t extract4(uint32_t lo, uint32_t hi, uint32_t sel) {
@@ -1651,21 +1677,58 @@ __global__ void __launch_bounds__(256)
   }
   __shared__ int32_t s_probe[PRUNE_PROBE];
   __shared__ double s_red[256];
+  __shared__ float s_apf[PRUNE_MAX_ANGLES];
+  __shared__ float s_fmax[256 / 32];
   __shared__ int s_cnt, s_ev;
   const int T = n_angles[b], ncell = nx * ny, ng = (na + BOUND_GROUP - 1) / BOUND_GROUP;
   if (threadIdx.x < T) s_probe[threadIdx.x] = angles[(size_t)b * na + threadIdx.x];
   if (threadIdx.x == 0) s_cnt = s_ev = 0;
-  __syncthreads();
   const bool pen = s.do_penalize != 0;
   const double ch = centers[3 * b + 2];
   const double start_a = ch - s.angle_offset;
-  double L = -1.0;
-  for (int t = threadIdx.x; t < T * ncell; t += blockDim.x) {
-    const int k = s_probe[t / ncell], c = t % ncell;
+  const double D = (double)((uint32_t)n * (uint32_t)GRID_OCCUPIED);
+  const float inv_d = (float)(1.0 / D);
+  red_angle_factors(s_apf, na, 0, start_a, ch, D, pen, s, p);
+  __syncthreads();
+  // The largest float score, then the exact response of the candidates the pre-filter cannot rule out: their maximum
+  // is the maximum over every probed candidate.  A thread holds at most 4 cells (ncell <= 32 x 32, SweepPlan::prune);
+  // only threads with such a candidate evaluate any.
+  const int32_t *bs = sums + (size_t)b * na * ncell;
+  float fmax_own = -1.0f;
+  bool amb_own = false;
+  for (int c = threadIdx.x; c < ncell; c += blockDim.x) {
     const int iy = c / nx, ix = c % nx;
     const double y = -s.offset_y + (double)(uint32_t)iy * s.res_y, x = -s.offset_x + (double)(uint32_t)ix * s.res_x;
-    const double angle = start_a + (double)(uint32_t)k * s.angle_res;
-    L = dmax(L, candidate_response(sums[((size_t)b * na + k) * ncell + c], n, pen, x * x + y * y, angle, ch, p));
+    const float dpf = red_dist_factor(x * x + y * y, p);
+    for (int t = 0; t < T; t++) {
+      const int k = s_probe[t];
+      bool amb;
+      fmax_own = fmaxf(fmax_own, red_fscore(__ldcg(bs + (size_t)k * ncell + c), s_apf[k], dpf, inv_d, pen, amb));
+      amb_own |= amb;
+    }
+  }
+  float fmax = fmax_own;
+#pragma unroll
+  for (int d = 16; d > 0; d >>= 1) fmax = fmaxf(fmax, __shfl_xor_sync(0xffffffffu, fmax, d));
+  if ((threadIdx.x & 31) == 0) s_fmax[threadIdx.x >> 5] = fmax;
+  __syncthreads();
+#pragma unroll
+  for (int w = 0; w < 256 / 32; w++) fmax = fmaxf(fmax, s_fmax[w]);
+  const float thr = red_margin(fmax);
+  double L = -1.0;
+  for (int c = threadIdx.x; c < ncell && (fmax_own >= thr || amb_own); c += blockDim.x) {
+    const int iy = c / nx, ix = c % nx;
+    const double y = -s.offset_y + (double)(uint32_t)iy * s.res_y, x = -s.offset_x + (double)(uint32_t)ix * s.res_x;
+    const double sq = x * x + y * y;
+    const float dpf = red_dist_factor(sq, p);
+    for (int t = 0; t < T; t++) {
+      const int k = s_probe[t];
+      const int32_t isum = __ldcg(bs + (size_t)k * ncell + c);
+      bool amb;
+      if (red_fscore(isum, s_apf[k], dpf, inv_d, pen, amb) < thr && !amb) continue;
+      const double angle = start_a + (double)(uint32_t)k * s.angle_res;
+      L = dmax(L, candidate_response(isum, n, pen, sq, angle, ch, p));
+    }
   }
   s_red[threadIdx.x] = L;
   __syncthreads();
@@ -1776,12 +1839,13 @@ __global__ void __launch_bounds__(RED_THREADS, 2) k_reduce(ReduceArgs A) {
   __shared__ double s_best;
   __shared__ double s_mean[3];
   __shared__ uint8_t s_keep[PRUNE_MAX_ANGLES];
-  const bool masked = A.keep != nullptr;  // only with na <= PRUNE_MAX_ANGLES
+  __shared__ uint16_t s_list[PRUNE_MAX_ANGLES];
+  __shared__ int s_nk;
+  // A pruned sweep (keep != nullptr, na <= PRUNE_MAX_ANGLES) swept only the angles of keep; the others read 0, so
+  // none of their candidates is a cell maximum above 0 or a tie (k_prune_select skips angles only when best > 0.1),
+  // and the passes below walk only the swept angles, ascending: s_list[0, nk).  Otherwise they walk 0 .. na-1.
+  const bool masked = A.keep != nullptr;
   for (int k = tid; k < na && masked; k += RED_THREADS) s_keep[k] = A.keep[(size_t)b * na + k];
-  // the sum of candidate c at angle k; an angle a pruned sweep skipped holds no candidate that can matter: 0
-  auto load_sum = [&](int k, int c) -> int32_t {
-    return (k < na && (!masked || s_keep[k])) ? __ldcg(bs + (size_t)k * ncell + c) : 0;
-  };
   if (tid == 0) { s_err = 0; s_count = 0; }
   if (!s.fine && phase <= REDUCE_SPLIT_BEST)
     for (int i = tid; i < pstep * g.search_side; i += RED_THREADS) probs[i] = 0.0;  // Clear (Mapper.cpp:329)
@@ -1794,15 +1858,41 @@ __global__ void __launch_bounds__(RED_THREADS, 2) k_reduce(ReduceArgs A) {
   const bool tab = na <= 1024;
   const double D = (double)((uint32_t)n * (uint32_t)GRID_OCCUPIED);
   const float inv_d = (float)(1.0 / D);
-  for (int k = tid; k < na && tab; k += RED_THREADS) {
-    double apen = 1.0;
-    if (pen) {
-      const double angle = start_a + (double)(uint32_t)(k_first + k) * s.angle_res;
-      apen = dmax(1.0 - (ANGLE_PENALTY_GAIN * ((angle - ch) * (angle - ch)) / p.angle_variance_penalty), p.minimum_angle_penalty);
+  if (tab) red_angle_factors(s_apf, na, k_first, start_a, ch, D, pen, s, p);
+  __syncthreads();
+  if (masked && tid < 32) {
+    int cnt = 0;
+    for (int k0 = 0; k0 < na; k0 += 32) {
+      const bool kept = k0 + tid < na && s_keep[k0 + tid];
+      const unsigned m = __ballot_sync(0xffffffffu, kept);
+      if (kept) s_list[cnt + __popc(m & ((1u << tid) - 1u))] = (uint16_t)(k0 + tid);
+      cnt += __popc(m);
     }
-    s_apf[k] = (float)(apen / D);
+    if (tid == 0) s_nk = cnt;
   }
   __syncthreads();
+  const int nk = masked ? s_nk : na;
+  // visit(k, sum) for the candidates of cell c in the walk's angle order, RED_UNROLL loads in flight; instantiated
+  // with and without the list, so that an unpruned walk carries no list lookup
+  auto walk = [&](auto listed, int c, auto &&visit) {
+    for (int j0 = 0; j0 < nk; j0 += RED_UNROLL) {
+      int k[RED_UNROLL];
+      int32_t v[RED_UNROLL];
+#pragma unroll
+      for (int u = 0; u < RED_UNROLL; u++) {
+        if constexpr (decltype(listed)::value) k[u] = j0 + u < nk ? (int)s_list[j0 + u] : 0;
+        else k[u] = j0 + u;
+        v[u] = j0 + u < nk ? __ldcg(bs + (size_t)k[u] * ncell + c) : 0;
+      }
+#pragma unroll
+      for (int u = 0; u < RED_UNROLL; u++)
+        if (j0 + u < nk) visit(k[u], v[u]);
+    }
+  };
+  auto walk_cell = [&](int c, auto &&visit) {
+    if (masked) walk(std::true_type{}, c, visit);
+    else walk(std::false_type{}, c, visit);
+  };
 
   // ---- pass 1: best response + per-cell maxima (Mapper.cpp:430-451); one thread per (x,y) cell ----
   // One read of the cell's nA sums: the running float maximum remembers its angle and whether any OTHER candidate
@@ -1818,29 +1908,22 @@ __global__ void __launch_bounds__(RED_THREADS, 2) k_reduce(ReduceArgs A) {
     const double sq = x * x + y * y;
     double cell_best = -1.0;
     if (tab) {
-      const float dpf = (float)dmax(1.0 - (DISTANCE_PENALTY_GAIN * sq / p.distance_variance_penalty), p.minimum_distance_penalty);
+      const float dpf = red_dist_factor(sq, p);
       float fmax = -1.0f;
       int kmax = 0;
       int32_t vmax = 0;
       bool near = false, any_amb = false;
-      for (int k0 = 0; k0 < na; k0 += RED_UNROLL) {
-        int32_t v[RED_UNROLL];
-#pragma unroll
-        for (int u = 0; u < RED_UNROLL; u++) v[u] = load_sum(k0 + u, c);
-#pragma unroll
-        for (int u = 0; u < RED_UNROLL; u++) {
-          if (k0 + u >= na) continue;
-          bool amb;
-          const float f = red_fscore(v[u], s_apf[k0 + u], dpf, inv_d, pen, amb);
-          any_amb |= amb;
-          if (f > fmax) {
-            near = fmax >= f * (1.0f - 2.0e-6f) - 1.0e-30f;  // the old maximum (and only it or its own near ones) may still be near
-            fmax = f; kmax = k0 + u; vmax = v[u];
-          } else if (f >= fmax * (1.0f - 2.0e-6f) - 1.0e-30f) {
-            near = true;
-          }
+      walk_cell(c, [&](int k, int32_t v) {
+        bool amb;
+        const float f = red_fscore(v, s_apf[k], dpf, inv_d, pen, amb);
+        any_amb |= amb;
+        if (f > fmax) {
+          near = fmax >= red_margin(f);  // the old maximum (and only it or its own near ones) may still be near
+          fmax = f; kmax = k; vmax = v;
+        } else if (f >= red_margin(fmax)) {
+          near = true;
         }
-      }
+      });
       if (c == tid) { fmax0 = fmax; known0 = !any_amb; }
       else if (c == tid + RED_THREADS) { fmax1 = fmax; known1 = !any_amb; }
       if (!near && !any_amb) {
@@ -1849,27 +1932,20 @@ __global__ void __launch_bounds__(RED_THREADS, 2) k_reduce(ReduceArgs A) {
       } else if (fmax == 0.0f && !any_amb) {
         cell_best = 0.0;  // every sum is 0: response 0 / D, never penalised (Mapper.cpp:399)
       } else {
-        const float thr = fmax * (1.0f - 2.0e-6f) - 1.0e-30f;
-        for (int k0 = 0; k0 < na; k0 += RED_UNROLL) {
-          int32_t v[RED_UNROLL];
-#pragma unroll
-          for (int u = 0; u < RED_UNROLL; u++) v[u] = load_sum(k0 + u, c);
-#pragma unroll
-          for (int u = 0; u < RED_UNROLL; u++) {
-            if (k0 + u >= na) continue;
-            bool amb;
-            const float f = red_fscore(v[u], s_apf[k0 + u], dpf, inv_d, pen, amb);
-            if (f >= thr || amb) {
-              const double angle = start_a + (double)(uint32_t)(k_first + k0 + u) * s.angle_res;
-              cell_best = dmax(cell_best, candidate_response(v[u], n, pen, sq, angle, ch, p));
-            }
+        const float thr = red_margin(fmax);
+        walk_cell(c, [&](int k, int32_t v) {
+          bool amb;
+          const float f = red_fscore(v, s_apf[k], dpf, inv_d, pen, amb);
+          if (f >= thr || amb) {
+            const double angle = start_a + (double)(uint32_t)(k_first + k) * s.angle_res;
+            cell_best = dmax(cell_best, candidate_response(v, n, pen, sq, angle, ch, p));
           }
-        }
+        });
       }
     } else {
-      for (int k = 0; k < na; k++) {
+      for (int k = 0; k < na; k++) {  // not pruned (masked needs tab)
         const double angle = start_a + (double)(uint32_t)(k_first + k) * s.angle_res;
-        cell_best = dmax(cell_best, candidate_response(load_sum(k, c), n, pen, sq, angle, ch, p));
+        cell_best = dmax(cell_best, candidate_response(__ldcg(bs + (size_t)k * ncell + c), n, pen, sq, angle, ch, p));
       }
     }
     best = dmax(best, cell_best);
@@ -1911,30 +1987,22 @@ __global__ void __launch_bounds__(RED_THREADS, 2) k_reduce(ReduceArgs A) {
     const int iy = c / nx, ix = c % nx;
     const double y = start_y + (double)(uint32_t)iy * s.res_y, x = start_x + (double)(uint32_t)ix * s.res_x;
     const double sq = x * x + y * y;
-    const float dpf = (float)dmax(1.0 - (DISTANCE_PENALTY_GAIN * sq / p.distance_variance_penalty), p.minimum_distance_penalty);
-    for (int k0 = 0; k0 < na; k0 += RED_UNROLL) {
-      int32_t v[RED_UNROLL];
-#pragma unroll
-      for (int u = 0; u < RED_UNROLL; u++) v[u] = load_sum(k0 + u, c);
-#pragma unroll
-      for (int u = 0; u < RED_UNROLL; u++) {
-        const int k = k0 + u;
-        if (k >= na) continue;
-        if (tab) {
-          bool amb;
-          const float f = red_fscore(v[u], s_apf[k], dpf, inv_d, pen, amb);
-          if (f < tie_thr && !amb) continue;
-        }
-        const double angle = start_a + (double)(uint32_t)(k_first + k) * s.angle_res;
-        const double r = candidate_response(v[u], n, pen, sq, angle, ch, p);
-        if (double_equal(r, best)) {
-          const double h = normalize_angle(angle);
-          ax += cx + x; ay += cy + y; tx += cos(h); ty += sin(h);
-          int slot = atomicAdd(&s_count, 1);
-          if (slot < RED_MAX_TIES) tie_idx[slot] = c * na + k;
-        }
+    const float dpf = red_dist_factor(sq, p);
+    walk_cell(c, [&](int k, int32_t v) {
+      if (tab) {
+        bool amb;
+        const float f = red_fscore(v, s_apf[k], dpf, inv_d, pen, amb);
+        if (f < tie_thr && !amb) return;
       }
-    }
+      const double angle = start_a + (double)(uint32_t)(k_first + k) * s.angle_res;
+      const double r = candidate_response(v, n, pen, sq, angle, ch, p);
+      if (double_equal(r, best)) {
+        const double h = normalize_angle(angle);
+        ax += cx + x; ay += cy + y; tx += cos(h); ty += sin(h);
+        int slot = atomicAdd(&s_count, 1);
+        if (slot < RED_MAX_TIES) tie_idx[slot] = c * na + k;
+      }
+    });
   }
   __syncthreads();
   if (phase == REDUCE_SPLIT_FINISH && tid == 0) s_count = (int)tie_in[5 * b + 4];
