@@ -1002,15 +1002,19 @@ struct ReduceArgs {
 };
 
 
-template <int STRIDE, bool GEN>
+template <int STRIDE, bool GEN, bool LISTED>
 __global__ void __launch_bounds__(WIN_THREADS, 1)
     k_sweep_window(const uint8_t *__restrict__ grids, size_t grid_pitch, int data_size, int copy_bytes,
                    const int32_t *__restrict__ lists, const int32_t *__restrict__ counts,
                    const int32_t *__restrict__ starts, const int32_t *__restrict__ flags, int batch, int n, int na,
                    int nx, int ny, int width_step, int32_t *__restrict__ sums, int *__restrict__ work_counter,
                    int band_rows, int nbands, int band_bytes, int neg_bands, const int32_t *__restrict__ angles,
-                   const int32_t *__restrict__ n_angles) {
-  // angles != nullptr (a pruned sweep, nbands == 1): match b sweeps only the n_angles[b] angles angles[b * na + ...].
+                   const int32_t *__restrict__ n_angles, int acc_slots) {
+  // LISTED (a pruned sweep: one stride-1 32 x 32 tile, nbands == 1, SweepPlan::prune): match b sweeps only the
+  // n_angles[b] angles angles[b * na + ...], each split into listed_chunks beam ranges (karto_sweep_plan.cuh).  With
+  // more than one range, the CTA zeroes one ny x nx plane of int32 per listed angle after the image (while its copy is
+  // in flight), every item adds its rows there with shared-memory atomics (integer sums commute: the volume is the
+  // same), and the planes are written out once the match's items are done.
   // Grids larger than shared memory are swept in `nbands` row bands: a work unit is (match, band, 32-row candidate
   // tile); the image holds the rows that tile of a window whose ORIGIN lies in the band can touch (band_rows +
   // STRIDE * 31 + 2), k_offsets_sorted grouped the beams by the band of their origin (bands [0, neg_bands) hold origins
@@ -1057,12 +1061,15 @@ __global__ void __launch_bounds__(WIN_THREADS, 1)
     if (unit >= batch * nbands * unit_tiles_y) break;
     const int b = unit / (nbands * unit_tiles_y), band = (unit / unit_tiles_y) % nbands, unit_ty = unit % unit_tiles_y;
     const int f = flags[b];
-    const int na_b = angles ? n_angles[b] : na;
+    const int na_b = LISTED ? n_angles[b] : na;
     if ((f & 2) || !(f & 1) || na_b == 0) {  // out-of-range lattice (error), irregular lattice (generic kernel takes it)
       __syncthreads();
       continue;
     }
-    const int items = na_b * tiles_x * (nbands > 1 ? 1 : tiles_y);
+    const int chunks = LISTED ? listed_chunks(na_b, n, WIN_THREADS / 32, acc_slots) : 1;
+    const int items = LISTED ? na_b * chunks : na_b * tiles_x * (nbands > 1 ? 1 : tiles_y);
+    int32_t *s_acc = reinterpret_cast<int32_t *>(smem + 2 * WIN_GUARD + copy_bytes);  // LISTED: [na_b][ny][nx]
+    const int plane = nx * ny;
     // first / one-past-last grid row of this unit's image (the whole grid when nbands == 1)
     const int row0 = (band - neg_bands) * band_rows + STRIDE * unit_ty * 32;
     const int lo_row = max(row0, 0);
@@ -1086,6 +1093,8 @@ __global__ void __launch_bounds__(WIN_THREADS, 1)
       }
     }
     if (threadIdx.x < WIN_GUARD / 4) reinterpret_cast<uint32_t *>(sgrid + WIN_GUARD + bytes)[threadIdx.x] = 0;  // trailing guard
+    if (LISTED && chunks > 1)
+      for (int i = threadIdx.x; i < na_b * plane; i += blockDim.x) s_acc[i] = 0;
     mbar_wait(&bar, parity);
     parity ^= 1;
     __syncthreads();
@@ -1097,12 +1106,14 @@ __global__ void __launch_bounds__(WIN_THREADS, 1)
       if (lane == 0) item = atomicAdd(&s_item, 1);
       item = __shfl_sync(0xffffffffu, item, 0);
       if (item >= items) break;
-      int k, ty, tx;
-      if (nbands > 1) {
+      int k, ty, tx, j = 0, c = 0;
+      if (LISTED) {
+        j = item / chunks; c = item - j * chunks;
+        k = angles[(size_t)b * na + j]; ty = 0; tx = 0;
+      } else if (nbands > 1) {
         k = item / tiles_x; tx = item % tiles_x; ty = unit_ty;
       } else {
         k = item / (tiles_x * tiles_y);
-        if (angles) k = angles[(size_t)b * na + k];
         const int t = item % (tiles_x * tiles_y);
         ty = t / tiles_x; tx = t % tiles_x;
       }
@@ -1119,16 +1130,31 @@ __global__ void __launch_bounds__(WIN_THREADS, 1)
       for (int j = 0; j < 9; j++) { lo[j] = 0; hi[j] = 0; }
       // groups of this band: I0 I1 I2 I3 E0 E1 E2 E3 (interior / edge beams of each alignment class)
       const int cols = min(CPT, nx - tx * CPT);
-      win_class_pair<0, STRIDE, GEN>(sgrid, list + sg[0], cn[0], list + sg[4], cn[4], cols, lane, hi_half, loff, row_delta, bias, data_size, s_off, lo, hi, acc);
-      win_class_pair<1, STRIDE, GEN>(sgrid, list + sg[1], cn[1], list + sg[5], cn[5], cols, lane, hi_half, loff, row_delta, bias, data_size, s_off, lo, hi, acc);
-      win_class_pair<2, STRIDE, GEN>(sgrid, list + sg[2], cn[2], list + sg[6], cn[6], cols, lane, hi_half, loff, row_delta, bias, data_size, s_off, lo, hi, acc);
-      win_class_pair<3, STRIDE, GEN>(sgrid, list + sg[3], cn[3], list + sg[7], cn[7], cols, lane, hi_half, loff, row_delta, bias, data_size, s_off, lo, hi, acc);
+      if (LISTED) {  // this item's range of the concatenated groups
+        int r0, r1, off[8], len[8];
+        chunk_range(cn[0] + cn[1] + cn[2] + cn[3] + cn[4] + cn[5] + cn[6] + cn[7], c, chunks, r0, r1);
+        chunk_groups(cn, r0, r1, off, len);
+        win_class_pair<0, STRIDE, GEN>(sgrid, list + sg[0] + off[0], len[0], list + sg[4] + off[4], len[4], cols, lane, hi_half, loff, row_delta, bias, data_size, s_off, lo, hi, acc);
+        win_class_pair<1, STRIDE, GEN>(sgrid, list + sg[1] + off[1], len[1], list + sg[5] + off[5], len[5], cols, lane, hi_half, loff, row_delta, bias, data_size, s_off, lo, hi, acc);
+        win_class_pair<2, STRIDE, GEN>(sgrid, list + sg[2] + off[2], len[2], list + sg[6] + off[6], len[6], cols, lane, hi_half, loff, row_delta, bias, data_size, s_off, lo, hi, acc);
+        win_class_pair<3, STRIDE, GEN>(sgrid, list + sg[3] + off[3], len[3], list + sg[7] + off[7], len[7], cols, lane, hi_half, loff, row_delta, bias, data_size, s_off, lo, hi, acc);
+      } else {
+        win_class_pair<0, STRIDE, GEN>(sgrid, list + sg[0], cn[0], list + sg[4], cn[4], cols, lane, hi_half, loff, row_delta, bias, data_size, s_off, lo, hi, acc);
+        win_class_pair<1, STRIDE, GEN>(sgrid, list + sg[1], cn[1], list + sg[5], cn[5], cols, lane, hi_half, loff, row_delta, bias, data_size, s_off, lo, hi, acc);
+        win_class_pair<2, STRIDE, GEN>(sgrid, list + sg[2], cn[2], list + sg[6], cn[6], cols, lane, hi_half, loff, row_delta, bias, data_size, s_off, lo, hi, acc);
+        win_class_pair<3, STRIDE, GEN>(sgrid, list + sg[3], cn[3], list + sg[7], cn[7], cols, lane, hi_half, loff, row_delta, bias, data_size, s_off, lo, hi, acc);
+      }
 
       // ---- write / accumulate this lane's row ----
       const int iy = ty * 32 + lane;
       if (iy < ny) {
         int32_t *dst = bsums + ((size_t)k * ny + iy) * nx + tx * CPT;
-        if (nbands == 1) {
+        if (LISTED && chunks > 1) {
+          int32_t *sdst = s_acc + (j * ny + iy) * nx;  // lane r's row: banks (r * nx + x) mod 32
+#pragma unroll
+          for (int x = 0; x < CPT; x++)
+            if (x < nx && acc[x]) atomicAdd(sdst + x, (int32_t)acc[x]);
+        } else if (nbands == 1) {
 #pragma unroll
           for (int x = 0; x < CPT; x++)
             if (tx * CPT + x < nx) dst[x] = (int32_t)acc[x];
@@ -1140,6 +1166,11 @@ __global__ void __launch_bounds__(WIN_THREADS, 1)
       }
     }
     __syncthreads();  // everyone is done with sgrid before the next unit's copy is issued
+    if (LISTED && chunks > 1)  // (the next unit zeroes the planes only after its own __syncthreads)
+      for (int i = threadIdx.x; i < na_b * plane; i += blockDim.x) {
+        const int jj = i / plane;
+        bsums[(size_t)angles[(size_t)b * na + jj] * plane + (i - jj * plane)] = s_acc[i];
+      }
   }
 }
 
@@ -2314,7 +2345,7 @@ static b2s_status matcher_create_impl(const b2s_matcher_params *params, const b2
   m->num_sms = prop.multiProcessorCount;
   m->smem_optin = (int)prop.sharedMemPerBlockOptin;
   cudaFuncAttributes fa;
-  B2S_CUDA_CHECK(cudaFuncGetAttributes(&fa, k_sweep_window<1, false>));
+  B2S_CUDA_CHECK(cudaFuncGetAttributes(&fa, k_sweep_window<1, false, false>));
   m->win_static_smem = fa.sharedSizeBytes;
   B2S_CUDA_CHECK(cudaFuncGetAttributes(&fa, k_add_scan));
   m->add_static_smem = fa.sharedSizeBytes;
@@ -2930,18 +2961,21 @@ namespace b2s {
 // d_angles / d_n_angles (a pruned sweep)
 static b2s_status launch_window(b2s_matcher *m, const SweepPlan &pl, const int32_t *angles) {
   B2S_CUDA_CHECK(cudaMemsetAsync(m->d_work, 0, sizeof(int), m->stream));
+  const size_t smem = angles ? pl.listed_smem : pl.win_smem;
   auto launch = [&](auto kern) -> b2s_status {
-    B2S_CUDA_CHECK(raise_dyn_smem(kern, pl.win_smem));
-    kern<<<pl.ctas, WIN_THREADS, pl.win_smem, m->stream>>>(m->d_grids, m->grid_pitch, m->g.data_size, pl.copy_bytes,
-                                                           m->d_lists, m->d_counts, m->d_starts, m->d_flags, m->batch,
-                                                           m->n, pl.na, pl.nx, pl.ny, m->g.width_step, m->d_sums,
-                                                           m->d_work, pl.band_rows, pl.nbands, pl.band_bytes,
-                                                           pl.neg_bands, angles, angles ? m->d_n_angles.p : nullptr);
+    B2S_CUDA_CHECK(raise_dyn_smem(kern, smem));
+    kern<<<pl.ctas, WIN_THREADS, smem, m->stream>>>(m->d_grids, m->grid_pitch, m->g.data_size, pl.copy_bytes,
+                                                    m->d_lists, m->d_counts, m->d_starts, m->d_flags, m->batch, m->n,
+                                                    pl.na, pl.nx, pl.ny, m->g.width_step, m->d_sums, m->d_work,
+                                                    pl.band_rows, pl.nbands, pl.band_bytes, pl.neg_bands, angles,
+                                                    angles ? m->d_n_angles.p : nullptr, pl.acc_slots);
     B2S_CUDA_CHECK(cudaGetLastError());
     return B2S_OK;
   };
-  if (pl.stride == 2) return pl.gen ? launch(k_sweep_window<2, true>) : launch(k_sweep_window<2, false>);
-  return pl.gen ? launch(k_sweep_window<1, true>) : launch(k_sweep_window<1, false>);
+  if (angles)  // a pruned sweep: stride 1, one tile (SweepPlan::prune)
+    return pl.gen ? launch(k_sweep_window<1, true, true>) : launch(k_sweep_window<1, false, true>);
+  if (pl.stride == 2) return pl.gen ? launch(k_sweep_window<2, true, false>) : launch(k_sweep_window<2, false, false>);
+  return pl.gen ? launch(k_sweep_window<1, true, false>) : launch(k_sweep_window<1, false, false>);
 }
 
 // The window lists of plan pl for search s: every angle (listed_chunks == 0), or only the angles of the per-match

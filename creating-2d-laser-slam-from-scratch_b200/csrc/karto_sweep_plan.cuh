@@ -28,6 +28,36 @@ constexpr int PRUNE_PROBE = 16;         // angles swept exactly to find the prun
 constexpr int BOUND_GROUP = 4;
 constexpr int BOUND_SPREAD = 3;  // the origin spread per axis the 7 x 7 image covers: 7 = 4 + BOUND_SPREAD
 
+// Work items of a pruned (listed) window sweep, k_sweep_window<LISTED>.  A match that lists few angles splits each
+// angle's beams into `chunks` ranges so that every warp of its CTA gets about two items: the concatenation
+// I0 I1 I2 I3 E0 E1 E2 E3 of the angle's groups (each a multiple of 4 long) is cut on multiples of 4 beams, and the
+// ranges' partial sums meet in shared-memory accumulators beside the grid image, one ny x nx plane per listed angle,
+// of which `slots` fit.  A match that lists more angles than that is swept one item per angle, written directly.
+constexpr int WIN_CHUNK_MIN_BEAMS = 32;  // beams per range on average at least: an item costs ~250 instructions besides its beams
+__host__ __device__ inline int listed_chunks(int listed, int n, int warps, int slots) {
+  if (listed <= 0 || listed > slots) return 1;
+  const int want = (2 * warps + listed - 1) / listed;
+  const int most = n / WIN_CHUNK_MIN_BEAMS;
+  return most < 2 ? 1 : (want < most ? want : most);
+}
+// the range [lo, hi) of chunk c of `chunks` in the concatenated groups of an angle that lists `total` beams (% 4 == 0)
+__host__ __device__ inline void chunk_range(int total, int c, int chunks, int &lo, int &hi) {
+  const long long q = total >> 2;
+  lo = 4 * (int)(q * c / chunks);
+  hi = 4 * (int)(q * (c + 1) / chunks);
+}
+// the part of each group g (count[g] beams) that lies in [lo, hi): beams off[g] .. off[g] + len[g] of the group
+__host__ __device__ inline void chunk_groups(const int32_t *count, int lo, int hi, int (&off)[8], int (&len)[8]) {
+  int p = 0;
+#pragma unroll
+  for (int g = 0; g < 8; g++) {
+    const int s = lo > p ? lo - p : 0, e = hi - p < count[g] ? hi - p : count[g];
+    off[g] = s;
+    len[g] = e > s ? e - s : 0;
+    p += count[g];
+  }
+}
+
 // u16 entries per match of the block summed-area tables (k_grid_sat), padded to 16 bytes
 inline size_t sat_stride(int sbx, int sby) { return (size_t)((((sbx + 1) * (sby + 1)) + 7) & ~7); }
 // The 4x4 max-pooled grid (k_grid_pool) of one match: P[f] = max over dy, dx in [0, 4) of grid[f + dy * width_step + dx]
@@ -116,6 +146,10 @@ struct SweepPlan {
   bool group = false;
   bool group_stage = false;  // the group pass stages the scan-local points after its image
   size_t group_smem = 0;     // its dynamic shared memory: 7x7 image + guards (+ points when staged)
+  // the listed sweeps of a pruned search: ny x nx accumulator planes after the grid image (listed_chunks), up to
+  // 2 * warps - 1 of them (a match that lists more angles is not split)
+  int acc_slots = 0;
+  size_t listed_smem = 0;  // win_smem + the planes
 };
 
 // shared memory k_sweep_bound stages after its pooled image (bound_stage): n scan-local points and the SAT when used
@@ -210,6 +244,11 @@ inline SweepPlan plan_sweep(const b2s_matcher_params &p, const b2s_grid_info &g,
   pl.group_stage = pl.group && (long long)(pl.group_smem + staged7) <= smem_limit;
   if (pl.group_stage) pl.group_smem += staged7;
   if (!pl.group) pl.group_smem = 0;
+  if (pl.prune) {
+    const long long plane = 4LL * pl.nx * pl.ny, room = smem_limit - (long long)pl.win_smem;
+    pl.acc_slots = (int)std::min<long long>(2 * (WIN_THREADS / 32) - 1, std::max(room, 0LL) / plane);
+    pl.listed_smem = pl.win_smem + (size_t)(pl.acc_slots * plane);
+  }
   return pl;
 }
 
