@@ -1287,9 +1287,12 @@ constexpr int BOUND_FLUSH = 64 * 32;  // beams placed between flushes of k_sweep
 enum { BOUND_GROUPS = 0, BOUND_PROBE = 1, BOUND_SELECT = 2 };
 
 // One persistent CTA per match at a time (like k_sweep_window): the pooled image (its four residue planes, see
-// pool_index) is staged by TMA, warps take units (an angle, or a group of BOUND_GROUP angles).  The bound reads no
-// window lists: for each unit a warp places 32 beams at a time, one per lane, and compacts the interior and the edge
-// ones into its staging row.
+// pool_index) is staged by TMA, warps take items of units (an angle, or a group of BOUND_GROUP angles).  A round of
+// few units cuts each unit's beams into ranges (bound_chunks / bound_range in karto_sweep_plan.cuh), and each item
+// adds its 64 block sums into the unit's u32 row in shared memory; after a __syncthreads one warp per unit scores the
+// row.  Integer sums commute, so the value is the one a single pass over the beams gives.  The bound reads no window
+// lists: for each item a warp places 32 beams at a time, one per lane, and compacts the interior and the edge ones
+// into its staging row.
 //   One angle: the beam's window origin and class by win_origin_class (the definition k_offsets_sorted lists them
 //   by), dropping the ones the lists would drop.  Which beams add is the same set as in the lists and integer sums
 //   commute, so UBr is the one the lists would give.
@@ -1306,13 +1309,14 @@ enum { BOUND_GROUPS = 0, BOUND_PROBE = 1, BOUND_SELECT = 2 };
 // into a plain u32 sum and, through one byte permute, a sum of bytes 1 and 3 in u16 lanes; the plain sum less the
 // latter shifted by 8 leaves bytes 0 and 2 in u16 lanes.  A slot takes at most 8 beams per 32 placed, 8 x 127 per u16
 // lane, so the sums are flushed into the per-column u32 totals every BOUND_FLUSH beams placed (64 x 1016 < 65536)
-// and at the end of the unit.  The totals of the four slots are then summed by shuffles so that lane L ends with
+// and at the end of the item's range.  The totals of the four slots are then summed by shuffles so that lane L ends with
 // blocks (L % 8, 2 (L / 8)) and (L % 8, 2 (L / 8) + 1).  Edge beams and the last 0..3 interior ones read P byte by
 // byte with the range test, at the lane's own two blocks (the value of an interior one is the same either way).
 // The value of a unit is candidate_response's fp64 operations on the block's sum, the block's largest distance
 // penalty and the unit's largest angle penalty, so it is at least every response of every angle of the unit.
 // STAGE (SweepPlan::bound_stage / group_stage): the scan-local points (and for single angles the summed-area table)
-// sit in shared memory after the pooled image; otherwise they are read from global memory through L1.
+// sit in shared memory after the pooled image; otherwise they are read from global memory through L1.  The `rows`
+// unit rows follow (SweepPlan::bound_rows / group_rows).
 template <bool STAGE, int MODE>
 __global__ void __launch_bounds__(WIN_THREADS, 1)
     k_sweep_bound(const uint8_t *__restrict__ pools, size_t pool_pitch_, int pool_bytes_, int plane, int lead,
@@ -1323,7 +1327,7 @@ __global__ void __launch_bounds__(WIN_THREADS, 1)
                   int nx, int ny, int width_step, int data_size, double *__restrict__ ubr, double *__restrict__ gub,
                   int32_t *__restrict__ angles, int32_t *__restrict__ n_angles, uint8_t *__restrict__ keep,
                   const int32_t *__restrict__ n_eval, const double *__restrict__ cuts,
-                  unsigned long long *__restrict__ pruned_total, int32_t *__restrict__ scratch,
+                  unsigned long long *__restrict__ pruned_total, int32_t *__restrict__ scratch, int rows,
                   int *__restrict__ work_counter) {
   constexpr bool GRP = MODE == BOUND_GROUPS;
   constexpr int NJ = GRP ? BOUND_GROUP : 1;  // angles per unit
@@ -1343,6 +1347,7 @@ __global__ void __launch_bounds__(WIN_THREADS, 1)
   // (scratch[b][na + ng]): shared memory beside the pooled image is budgeted for k_sweep_window's static arrays only
   double *s_lx = reinterpret_cast<double *>(smem + WIN_GUARD + pool_bytes_ + WIN_GUARD), *s_ly = s_lx + n;
   uint16_t *s_sat = reinterpret_cast<uint16_t *>(s_ly + n);
+  uint32_t *s_rows = STAGE ? reinterpret_cast<uint32_t *>(s_sat + (sat_all ? sat_len : 0)) : reinterpret_cast<uint32_t *>(s_lx);
   const unsigned lanes_below = (1u << lane) - 1u;
   // the largest distance penalty of the candidates of block (by, bx), as k_reduce computes sq and candidate_response
   // the penalty (-1: the block holds no candidate)
@@ -1448,11 +1453,34 @@ __global__ void __launch_bounds__(WIN_THREADS, 1)
     __syncthreads();
     const double ch = centers[3 * b + 2];
 
-    // the bound of angles k0 .. k0 + cnt - 1 (cnt = 1 unless GRP), in every lane
-    auto bound_unit = [&](int k0, int cnt) -> double {
+    // the largest angle penalty of angles k0 .. k0 + cnt - 1 (cnt = 1 unless GRP)
+    auto unit_apen = [&](int k0, int cnt) -> double {
+      double apen = GRP ? -1.0 : 1.0;
+      if (pen)
+#pragma unroll
+        for (int j = 0; j < NJ; j++) {
+          const double angle = win_angle(ch, s.angle_offset, s.angle_res, k0 + min(j, cnt - 1));
+          const double sq_a = (angle - ch) * (angle - ch);
+          const double ap = dmax(1.0 - (ANGLE_PENALTY_GAIN * sq_a / p.angle_variance_penalty), p.minimum_angle_penalty);
+          apen = GRP ? dmax(apen, ap) : ap;
+        }
+      return apen;
+    };
+    // candidate_response's operations, with the block's largest sum and largest distance penalty: the bound of a unit
+    // whose block sums are ua, ub in every lane (see bound_sums), in every lane
+    auto bound_value = [&](uint32_t ua, uint32_t ub, double apen) -> double {
+      double r = -1.0;
+      if (dpen_a >= 0.0) r = dmax(r, pen ? ((double)ua / D) * (dpen_a * apen) : (double)ua / D);
+      if (dpen_b >= 0.0) r = dmax(r, pen ? ((double)ub / D) * (dpen_b * apen) : (double)ub / D);
+#pragma unroll
+      for (int d = 16; d > 0; d >>= 1) r = dmax(r, __shfl_xor_sync(0xffffffffu, r, d));
+      return r;
+    };
+    // the sums of beams [i_lo, i_hi) (i_lo % 32 == 0) of angles k0 .. k0 + cnt - 1 at the lane's blocks
+    // (L % 8, 2 (L / 8)) -> ua and (L % 8, 2 (L / 8) + 1) -> ub
+    auto bound_sums = [&](int k0, int cnt, int i_lo, int i_hi, uint32_t &ua, uint32_t &ub) {
       double cd[NJ], sd[NJ];
       float cf[NJ], sf[NJ];
-      double apen = GRP ? -1.0 : 1.0;
 #pragma unroll
       for (int j = 0; j < NJ; j++) {
         const double angle = win_angle(ch, s.angle_offset, s.angle_res, k0 + min(j, cnt - 1));
@@ -1460,22 +1488,18 @@ __global__ void __launch_bounds__(WIN_THREADS, 1)
         sd[j] = sin(angle);
         cf[j] = (float)cd[j];
         sf[j] = (float)sd[j];
-        if (pen) {
-          const double sq_a = (angle - ch) * (angle - ch);
-          const double ap = dmax(1.0 - (ANGLE_PENALTY_GAIN * sq_a / p.angle_variance_penalty), p.minimum_angle_penalty);
-          apen = GRP ? dmax(apen, ap) : ap;
-        }
       }
-      uint32_t ua = 0, ub = 0;               // the lane's two blocks, beams read with the range test
+      ua = 0;                                   // the lane's two blocks, beams read with the range test
+      ub = 0;
       uint32_t s0 = 0, s1 = 0, o0 = 0, o1 = 0;  // interior pairs: plain sums and byte 1 / 3 sums of columns 0..3, 4..7
       uint32_t t[8] = {0, 0, 0, 0, 0, 0, 0, 0};  // interior totals of the lane's slot and row, per block column
-      for (int i0 = 0; i0 < n; i0 += 32) {
+      for (int i0 = i_lo; i0 < i_hi; i0 += 32) {
         const int i = i0 + lane;
         int cls = 255;
         int32_t a = 0;
         bool fb = false;           // GRP: the beam adds the largest P7 over its members' exact origins ...
         int32_t fa[NJ];            // ... these (WIN_SKIP: the member's window is wholly outside the grid)
-        if (i < n) {
+        if (i < i_hi) {
           const double plx = STAGE ? s_lx[i] : __ldg(g_pts + 2 * i), ply = STAGE ? s_ly[i] : __ldg(g_pts + 2 * i + 1);
           if (!GRP) {
             bool empty;
@@ -1554,7 +1578,7 @@ __global__ void __launch_bounds__(WIN_THREADS, 1)
           s1 += xh;
           o1 += __byte_perm(xh, 0, 0x4341);
         }
-        if (((i0 + 32) & (BOUND_FLUSH - 1)) == 0 || i0 + 32 >= n) {
+        if (((i0 + 32) & (BOUND_FLUSH - 1)) == 0 || i0 + 32 >= i_hi) {
           const uint32_t e0 = s0 - (o0 << 8), e1 = s1 - (o1 << 8);  // bytes 0 and 2 in u16 lanes
           t[0] += e0 & 0xffffu; t[1] += o0 & 0xffffu; t[2] += e0 >> 16; t[3] += o0 >> 16;
           t[4] += e1 & 0xffffu; t[5] += o1 & 0xffffu; t[6] += e1 >> 16; t[7] += o1 >> 16;
@@ -1597,28 +1621,52 @@ __global__ void __launch_bounds__(WIN_THREADS, 1)
           if (c == 0) ua += v; else ub += v;
         }
       }
-      // candidate_response's operations, with the block's largest sum and largest distance penalty
-      double r = -1.0;
-      if (dpen_a >= 0.0) r = dmax(r, pen ? ((double)ua / D) * (dpen_a * apen) : (double)ua / D);
-      if (dpen_b >= 0.0) r = dmax(r, pen ? ((double)ub / D) * (dpen_b * apen) : (double)ub / D);
-#pragma unroll
-      for (int d = 16; d > 0; d >>= 1) r = dmax(r, __shfl_xor_sync(0xffffffffu, r, d));
-      return r;
     };
-    // the angles at list positions [j0, j1), one per warp
-    auto bound_list = [&](int j0, int j1) {
-      for (int j = j0 + warp; j < j1; j += WIN_THREADS / 32) {
-        const int k = s_list[j];
-        const double r = bound_unit(k, 1);
-        if (lane == 0) ubr[(size_t)b * na + k] = r;
+    // one round: the bounds of `units` units, unit u being angles k0 .. k0 + cnt - 1 (unit_of(u, k0, cnt)), handed to
+    // put(u, bound) in lane 0 of one warp.  Split into ranges, the round ends with a __syncthreads.
+    auto bound_round = [&](int units, auto unit_of, auto put) {
+      constexpr int W = WIN_THREADS / 32;
+      const int C = bound_chunks(units, n, W, rows);
+      int k0, cnt;
+      uint32_t ua, ub;
+      if (C == 1) {
+        for (int u = warp; u < units; u += W) {
+          unit_of(u, k0, cnt);
+          bound_sums(k0, cnt, 0, n, ua, ub);
+          const double r = bound_value(ua, ub, unit_apen(k0, cnt));
+          if (lane == 0) put(u, r);
+        }
+        return;
       }
+      for (int i = threadIdx.x; i < units * 64; i += blockDim.x) s_rows[i] = 0;
+      __syncthreads();
+      for (int it = warp; it < units * C; it += W) {
+        const int u = it / C;
+        int lo, hi;
+        bound_range(n, it - u * C, C, lo, hi);
+        unit_of(u, k0, cnt);
+        bound_sums(k0, cnt, lo, hi, ua, ub);
+        atomicAdd(s_rows + 64 * u + 2 * lane, ua);
+        atomicAdd(s_rows + 64 * u + 2 * lane + 1, ub);
+      }
+      __syncthreads();
+      for (int u = warp; u < units; u += W) {
+        unit_of(u, k0, cnt);
+        const double r = bound_value(s_rows[64 * u + 2 * lane], s_rows[64 * u + 2 * lane + 1], unit_apen(k0, cnt));
+        if (lane == 0) put(u, r);
+      }
+    };
+    // the angles at list positions [j0, j1)
+    auto bound_list = [&](int j0, int j1) {
+      bound_round(
+          j1 - j0, [&](int u, int &k0, int &cnt) { k0 = s_list[j0 + u]; cnt = 1; },
+          [&](int u, double r) { ubr[(size_t)b * na + s_list[j0 + u]] = r; });
     };
 
     if (GRP) {
-      for (int g = warp; g < ng; g += WIN_THREADS / 32) {
-        const double r = bound_unit(g * BOUND_GROUP, min(BOUND_GROUP, na - g * BOUND_GROUP));
-        if (lane == 0) gub[(size_t)b * ng + g] = r;
-      }
+      bound_round(
+          ng, [&](int g, int &k0, int &cnt) { k0 = g * BOUND_GROUP; cnt = min(BOUND_GROUP, na - g * BOUND_GROUP); },
+          [&](int g, double r) { gub[(size_t)b * ng + g] = r; });
     } else if (MODE == BOUND_PROBE) {
       const int T = min(PRUNE_PROBE, na);
       const int n_a = s_cnt;
@@ -3072,25 +3120,27 @@ static b2s_status run_correlate(b2s_matcher *m, const b2s_search *s, int k_first
     // in the stand-alone k_reduce.  Removed again; DESIGN.md §4.)
     if (pl.prune) {  // group bounds, then bounds, probe, select, sweep the selected angles (see k_sweep_bound)
       auto bound = [&](auto kern, const uint8_t *pools, size_t pitch, int bytes, int plane, int lead, bool sat,
-                       size_t smem) -> b2s_status {
+                       size_t smem, int rows) -> b2s_status {
         B2S_CUDA_CHECK(cudaMemsetAsync(m->d_work, 0, sizeof(int), m->stream));
+        smem += (size_t)rows * BOUND_ROW_BYTES;
         B2S_CUDA_CHECK(raise_dyn_smem(kern, smem));
         kern<<<pl.ctas, WIN_THREADS, smem, m->stream>>>(
             pools, pitch, bytes, plane, lead, m->d_local, m->d_grid_off, m->d_bases, sat ? m->d_sat.p : nullptr,
             m->sbx, m->sby, m->g.height, pl.rows_total, pl.tiles_x * 32, scale, m->d_flags, m->d_centers, m->p, *s, B, n,
             na, nx, ny, m->g.width_step, m->g.data_size, m->d_ubr, m->d_gub, m->d_angles, m->d_n_angles, m->d_keep,
-            m->d_n_eval, m->d_cuts, m->d_stats.p + 1, m->d_bscratch, m->d_work);
+            m->d_n_eval, m->d_cuts, m->d_stats.p + 1, m->d_bscratch, rows, m->d_work);
         B2S_CUDA_CHECK(cudaGetLastError());
         return B2S_OK;
       };
       const int pbytes = pool_bytes(m->g), pplane = pool_plane(m->g), plead = pool_lead(m->g.width_step);
       auto single = [&](auto kern) {
-        return bound(kern, m->d_pools, pool_pitch(m->g), pbytes, pplane, plead, pl.skip_empty, pl.bound_smem);
+        return bound(kern, m->d_pools, pool_pitch(m->g), pbytes, pplane, plead, pl.skip_empty, pl.bound_smem,
+                     pl.bound_rows);
       };
       if (pl.group) {
         auto group = [&](auto kern) {
           return bound(kern, m->d_pools7, pool7_pitch(m->g), pool7_bytes(m->g), pool7_plane(m->g),
-                       pool7_lead(m->g.width_step), false, pl.group_smem);
+                       pool7_lead(m->g.width_step), false, pl.group_smem, pl.group_rows);
         };
         if (b2s_status st = pl.group_stage ? group(k_sweep_bound<true, BOUND_GROUPS>)
                                            : group(k_sweep_bound<false, BOUND_GROUPS>)) return st;

@@ -58,6 +58,27 @@ __host__ __device__ inline void chunk_groups(const int32_t *count, int lo, int h
   }
 }
 
+// Work items of the angle bound, k_sweep_bound.  A round bounds `units` units (an angle, or a group of BOUND_GROUP
+// angles).  When it has few, each unit's beams are cut into `chunks` ranges on multiples of 32 (one placement pass of
+// a warp), so that every warp of the CTA gets about two items.  The ranges' 64 block sums meet in one u32 row per unit
+// in shared memory after the bound's staged data, of which `rows` fit (SweepPlan::bound_rows / group_rows).  A round
+// of more units than that is bounded one item per unit, each summed and scored by one warp.
+constexpr int BOUND_CHUNK_MIN_BEAMS = 128;  // an item costs the unit's sincos, shuffles and row adds besides its beams
+constexpr int BOUND_ROW_BYTES = 64 * 4;     // one u32 per 4 x 4 block of the 32 x 32 candidate tile
+__host__ __device__ inline int bound_chunks(int units, int n, int warps, int rows) {
+  if (units <= 0 || units > rows) return 1;
+  const int want = (2 * warps + units - 1) / units;
+  const int most = n / BOUND_CHUNK_MIN_BEAMS;
+  return most < 2 ? 1 : (want < most ? want : most);
+}
+// the beams [lo, hi) of range c of `chunks` of a unit of n beams
+__host__ __device__ inline void bound_range(int n, int c, int chunks, int &lo, int &hi) {
+  const long long q = (n + 31) >> 5;
+  lo = 32 * (int)(q * c / chunks);
+  hi = 32 * (int)(q * (c + 1) / chunks);
+  if (hi > n) hi = n;
+}
+
 // u16 entries per match of the block summed-area tables (k_grid_sat), padded to 16 bytes
 inline size_t sat_stride(int sbx, int sby) { return (size_t)((((sbx + 1) * (sby + 1)) + 7) & ~7); }
 // The 4x4 max-pooled grid (k_grid_pool) of one match: P[f] = max over dy, dx in [0, 4) of grid[f + dy * width_step + dx]
@@ -146,6 +167,9 @@ struct SweepPlan {
   bool group = false;
   bool group_stage = false;  // the group pass stages the scan-local points after its image
   size_t group_smem = 0;     // its dynamic shared memory: 7x7 image + guards (+ points when staged)
+  // the bound's per-unit rows of block sums (bound_chunks), BOUND_ROW_BYTES each after bound_smem / group_smem, up to
+  // 2 * warps - 1 of them (a round of more units is not split); 0: every unit is one item
+  int bound_rows = 0, group_rows = 0;
   // the listed sweeps of a pruned search: ny x nx accumulator planes after the grid image (listed_chunks), up to
   // 2 * warps - 1 of them (a match that lists more angles is not split)
   int acc_slots = 0;
@@ -244,6 +268,12 @@ inline SweepPlan plan_sweep(const b2s_matcher_params &p, const b2s_grid_info &g,
   pl.group_stage = pl.group && (long long)(pl.group_smem + staged7) <= smem_limit;
   if (pl.group_stage) pl.group_smem += staged7;
   if (!pl.group) pl.group_smem = 0;
+  auto rows_fit = [&](size_t used) {
+    const long long room = std::max(smem_limit - (long long)used, 0LL);
+    return (int)std::min<long long>(2 * (WIN_THREADS / 32) - 1, room / BOUND_ROW_BYTES);
+  };
+  if (pl.prune) pl.bound_rows = rows_fit(pl.bound_smem);
+  if (pl.group) pl.group_rows = rows_fit(pl.group_smem);
   if (pl.prune) {
     const long long plane = 4LL * pl.nx * pl.ny, room = smem_limit - (long long)pl.win_smem;
     pl.acc_slots = (int)std::min<long long>(2 * (WIN_THREADS / 32) - 1, std::max(room, 0LL) / plane);
