@@ -107,6 +107,12 @@ def plicp_odom_params(icp=None, base_to_laser=(0, 0, 0, 0, 0, 0, 1), **kw) -> Pl
     return p
 
 
+class PlicpOdomLaser(C.Structure):
+    """b2s_plicp_odom_laser: one recording's LaserScan fields (float32 angles, as the message carries them)."""
+    _fields_ = [("n_beams", C.c_int32), ("angle_min", C.c_float), ("angle_increment", C.c_float),
+                ("reserved", C.c_int32)]
+
+
 class PlicpOdomStep(C.Structure):
     """b2s_plicp_odom_step."""
     _fields_ = [("position", C.c_double * 3), ("orientation", C.c_double * 4), ("linear", C.c_double * 3),

@@ -27,6 +27,11 @@ def _bind():
         L.b2s_plicp_odom_process.argtypes = [C.c_void_p, C.POINTER(C.c_int32), C.POINTER(C.c_float),
                                              C.POINTER(C.c_uint32), C.POINTER(abi.PlicpOdomStep)]
         L.b2s_plicp_odom_reset.argtypes = [C.c_void_p, C.c_int]
+        L.b2s_plicp_odom_create_fleet.argtypes = [C.c_int, C.POINTER(abi.PlicpOdomParams), C.POINTER(abi.PlicpOdomLaser),
+                                                  C.c_int, C.c_void_p, C.POINTER(C.c_void_p)]
+        L.b2s_plicp_odom_process_fleet.argtypes = [C.c_void_p, C.POINTER(C.c_int32), C.POINTER(C.c_float),
+                                                   C.POINTER(C.c_float), C.POINTER(C.c_uint32),
+                                                   C.POINTER(abi.PlicpOdomStep)]
         ip, fp = C.POINTER(C.c_int32), C.POINTER(C.c_float)
         L.b2s_plicp_scan_match_create.argtypes = [C.POINTER(abi.IcpParams), C.c_int, ip, fp, fp, C.c_int, C.c_void_p,
                                                   C.POINTER(C.c_void_p)]
@@ -63,32 +68,77 @@ STEP_DTYPE = np.dtype([("position", "<f8", 3), ("orientation", "<f8", 4), ("line
 
 
 class Odometry:
-    """B ScanMatchPLICP nodes of one laser on the device (b2s_plicp_odom_*).  angle_min, angle_increment, range_min and
-    range_max are the LaserScan's float32 fields."""
+    """B ScanMatchPLICP nodes on the device (b2s_plicp_odom_*).  The constructor makes B nodes of one laser, one
+    parameter set and fixed range fields (b2s_plicp_odom_create); Odometry.fleet gives every recording its own
+    parameters and laser, the range fields coming with every scan.  Angles and range fields are the LaserScan's
+    float32 fields."""
 
     def __init__(self, params: abi.PlicpOdomParams, batch, n_beams, angle_min, angle_increment, range_min, range_max,
                  device=0, stream=None):
         L = _bind()
         self._h = C.c_void_p()
         self.batch, self.n = int(batch), int(n_beams)
-        check(L.b2s_plicp_odom_create(C.byref(params), self.batch, self.n, angle_min, angle_increment, range_min,
+        self.n_beams = np.full(max(self.batch, 0), self.n, np.int32)
+        self.has_fields = True
+        check(L.b2s_plicp_odom_create(C.byref(params), self.batch, int(n_beams), angle_min, angle_increment, range_min,
                                       range_max, device, C.c_void_p(stream) if stream else None, C.byref(self._h)))
 
-    def process(self, recordings, stamps):
-        """recordings: B arrays [S_b][n] float32 ranges (S_b = 0 leaves recording b untouched); stamps: B arrays
-        [S_b][2] (sec, nsec).  -> list of B structured arrays of STEP_DTYPE, one row per scan."""
-        counts = np.array([len(r) for r in recordings], np.int32)
-        if len(counts) != self.batch or len(stamps) != self.batch or any(len(s) != c for s, c in zip(stamps, counts)):
-            raise ValueError("one recording and one stamp per scan for every recording of the handle")
+    @classmethod
+    def fleet(cls, params_list, n_beams, angle_min, angle_increment, device=0, stream=None):
+        """One node per recording: params_list [B] of abi.PlicpOdomParams, n_beams / angle_min / angle_increment [B]
+        (b2s_plicp_odom_create_fleet).  process() then needs each scan's range fields."""
+        L = _bind()
+        self = cls.__new__(cls)
+        self._h = C.c_void_p()
+        self.n = self.n_beams = np.ascontiguousarray(n_beams, np.int32).reshape(-1)
+        self.batch = len(self.n_beams)
+        self.has_fields = False
+        amin = np.asarray(angle_min, np.float32).reshape(-1)
+        ainc = np.asarray(angle_increment, np.float32).reshape(-1)
+        params_list = list(params_list)
+        if len(params_list) != self.batch or len(amin) != self.batch or len(ainc) != self.batch:
+            raise ValueError("one parameter set, beam count, angle_min and angle_increment per recording")
+        P = (abi.PlicpOdomParams * max(self.batch, 1))(*params_list)
+        lasers = (abi.PlicpOdomLaser * max(self.batch, 1))(
+            *[abi.PlicpOdomLaser(int(n), float(a), float(i), 0) for n, a, i in zip(self.n, amin, ainc)])
+        check(L.b2s_plicp_odom_create_fleet(self.batch, P, lasers, device, C.c_void_p(stream) if stream else None,
+                                            C.byref(self._h)))
+        return self
+
+    def process(self, recordings, stamps, range_limits=None):
+        """recordings: B arrays [S_b][n_beams[b]] float32 ranges (S_b = 0 leaves recording b untouched); stamps: B
+        arrays [S_b][2] (sec, nsec); range_limits: B arrays [S_b][2] float32 (range_min, range_max of each scan),
+        required on a fleet handle, else the create-time fields.  -> list of B structured arrays of STEP_DTYPE, one row
+        per scan."""
+        if len(recordings) != self.batch or len(stamps) != self.batch or \
+                (range_limits is not None and len(range_limits) != self.batch):
+            raise ValueError("one recording, stamp array and range-limit array per recording of the handle")
+        if range_limits is None and not self.has_fields:
+            raise ValueError("a fleet handle needs each scan's (range_min, range_max)")
+        rec = [np.asarray(r, np.float32) for r in recordings]
+        if not self.has_fields and any(r.size and (r.ndim != 2 or r.shape[1] != self.n_beams[b])
+                                       for b, r in enumerate(rec)):
+            raise ValueError("recording b is [S_b][n_beams[b]]")
+        rec = [r.reshape(-1, self.n_beams[b]) for b, r in enumerate(rec)]
+        counts = np.array([len(r) for r in rec], np.int32)
+        stm = [np.asarray(s, np.uint32).reshape(-1, 2) for s in stamps]
+        if any(len(s) != c for s, c in zip(stm, counts)):
+            raise ValueError("one stamp per scan")
         total = int(counts.sum())
-        rng = np.ascontiguousarray(np.concatenate([np.asarray(r, np.float32).reshape(-1, self.n) for r in recordings])
-                                   if total else np.zeros((0, self.n), np.float32))
-        stm = np.ascontiguousarray(np.concatenate([np.asarray(s, np.uint32).reshape(-1, 2) for s in stamps])
-                                   if total else np.zeros((0, 2), np.uint32))
+        rng = np.ascontiguousarray(np.concatenate([r.reshape(-1) for r in rec]) if total else np.zeros(1, np.float32))
+        st = np.ascontiguousarray(np.concatenate(stm) if total else np.zeros((1, 2), np.uint32))
         out = (abi.PlicpOdomStep * max(total, 1))()
-        check(_bind().b2s_plicp_odom_process(self._h, counts.ctypes.data_as(C.POINTER(C.c_int32)),
-                                             rng.ctypes.data_as(C.POINTER(C.c_float)),
-                                             stm.ctypes.data_as(C.POINTER(C.c_uint32)), out))
+        ip, fp, up = C.POINTER(C.c_int32), C.POINTER(C.c_float), C.POINTER(C.c_uint32)
+        if range_limits is None:
+            check(_bind().b2s_plicp_odom_process(self._h, counts.ctypes.data_as(ip), rng.ctypes.data_as(fp),
+                                                 st.ctypes.data_as(up), out))
+        else:
+            lim = [np.asarray(l, np.float32).reshape(-1, 2) for l in range_limits]
+            if any(len(l) != c for l, c in zip(lim, counts)):
+                raise ValueError("one (range_min, range_max) per scan")
+            lm = np.ascontiguousarray(np.concatenate(lim) if total else np.zeros((1, 2), np.float32))
+            check(_bind().b2s_plicp_odom_process_fleet(self._h, counts.ctypes.data_as(ip), rng.ctypes.data_as(fp),
+                                                       lm.ctypes.data_as(fp), st.ctypes.data_as(up), out))
         raw = np.frombuffer(out, dtype=STEP_DTYPE, count=total).copy()
         return np.split(raw, np.cumsum(counts)[:-1])
 

@@ -924,7 +924,7 @@ b2s_status b2s_plicp_match(const b2s_icp_params *params, int batch, int n, const
                            const double *first_guess, int device, void *cuda_stream, b2s_icp_result *results);
 
 /* ScanMatchPLICP (lesson3/src/plicp_odometry.cc:191-517), the node around sm_icp, for B independent recordings (robots)
- * of one laser: key frame, constant-velocity prediction (GetPrediction, :442-456: only linear.x >= 1e-6 predicts; there
+ * (each of its own laser, mount and parameters with b2s_plicp_odom_create_fleet): key frame, constant-velocity prediction (GetPrediction, :442-456: only linear.x >= 1e-6 predicts; there
  * is never an angular prediction), the prediction moved into the laser frame through the base-to-laser transform,
  * sm_icp against the key frame (the matcher of b2s_plicp_match), the correction composed into base_in_odom_ and the
  * key-frame rule (NewKeyframeNeeded, :498-517: |yaw| > kf_dist_angular, then ++count == kf_scan_count, which alone
@@ -932,7 +932,8 @@ b2s_status b2s_plicp_match(const b2s_icp_params *params, int batch, int n, const
  * in double) for base_in_odom_ and base_in_odom_keyframe_, latest_velocity_, last_icp_time_, the scan count and the key
  * frame's float32 ranges.  dt = (stamp - last stamp) as ros::Time arithmetic; equal stamps give dt = 0 and an inf / NaN
  * velocity, kept as IEEE arithmetic gives it.  last_icp_time_ always advances; velocity and pose change only on a valid
- * match.  One rule the node leaves undefined: after a failed match (icp.valid = 0) the node tests the key-frame rule on
+ * match.  Each LaserScan is converted with its own message's range fields (LaserScanToLDP, :285-322); the key frame
+ * keeps the valid flags its own message gave it (prev_ldp_scan_), so the handle keeps its fields with its ranges.  One rule the node leaves undefined: after a failed match (icp.valid = 0) the node tests the key-frame rule on
  * a default-constructed, uninitialised tf2::Transform; here it is the identity, so only the scan-count rule can
  * promote such a scan (DESIGN.md §7).  Pinned to the unmodified node except sm_icp and tf2's LinearMath, whose
  * published code is restated (PARITY UNPINNED for sm_icp; the device's sin / cos / atan2 may differ from glibc's in the
@@ -959,19 +960,43 @@ typedef struct b2s_plicp_odom_step { /* one LaserScan's outcome */
 
 typedef struct b2s_plicp_odom b2s_plicp_odom; /* opaque: B ScanMatchPLICP nodes */
 
-/* One laser geometry for every recording: the LaserScan's float32 angle_min, angle_increment (beam angle angle_min +
- * i * angle_increment summed in float, :308), range_min, range_max (valid iff range_min < r < range_max, :295).
- * B2S_ERR_BAD_PARAMS for NULL pointers, batch < 1, n_beams < 3, icp.max_iterations < 1 or a zero / non-finite mount
- * quaternion; B2S_ERR_NO_DEVICE without a device; B2S_ERR_TOO_LARGE above the pair kernel's beam limit (2408 on an
- * H100, 82 bytes of shared memory per beam). */
+/* The LaserScan fields the node reads per recording (LaserScanToLDP, :285-322), fixed for a recording at create. */
+typedef struct b2s_plicp_odom_laser { /* 16 bytes */
+  int32_t n_beams;                    /* scan_msg->ranges.size() */
+  float angle_min, angle_increment;   /* float32 message fields; beam i at angle_min + i * angle_increment summed in
+                                         float (:308), then widened */
+  int32_t reserved;                   /* 0 */
+} b2s_plicp_odom_laser;
+
+/* B ScanMatchPLICP nodes, one per recording: recording b has its own params[b] (sm_params subset, key-frame thresholds,
+ * base_to_laser mount, :64-185 and GetBaseToLaserTf :257-280) and its own lasers[b].  Range fields are per scan
+ * (b2s_plicp_odom_process_fleet).  Pinned to the unmodified node except sm_icp and tf2's LinearMath (PARITY UNPINNED for
+ * sm_icp, see above).  Everything is checked before the device is touched: B2S_ERR_BAD_PARAMS for NULL pointers,
+ * batch < 1, n_beams < 3, icp.max_iterations < 1, a zero / non-finite mount quaternion or a non-zero laser reserved,
+ * the refusal naming the recording in b2s_last_error(); B2S_ERR_NO_DEVICE without a device; B2S_ERR_TOO_LARGE when a
+ * recording is above the pair kernel's beam limit (2408 on an H100, 82 bytes of shared memory per beam). */
+b2s_status b2s_plicp_odom_create_fleet(int batch, const b2s_plicp_odom_params *params /* [batch] */,
+                                       const b2s_plicp_odom_laser *lasers /* [batch] */, int device, void *cuda_stream,
+                                       b2s_plicp_odom **out);
+/* One laser geometry, one parameter set and fixed range fields for every recording: the fleet of `batch` equal rows
+ * whose scans all carry range_min, range_max (valid iff range_min < r < range_max, :295).  Refusals as
+ * b2s_plicp_odom_create_fleet's. */
 b2s_status b2s_plicp_odom_create(const b2s_plicp_odom_params *params, int batch, int n_beams, float angle_min,
                                  float angle_increment, float range_min, float range_max, int device, void *cuda_stream,
                                  b2s_plicp_odom **out);
 void b2s_plicp_odom_destroy(b2s_plicp_odom *h);
 /* ScanCallback on every recording's next n_scans[b] LaserScans (0: recording b is untouched), in ONE launch (one CTA per
- * recording, no host round trip between scans).  Recordings are processor-major: ranges [sum n_scans][n_beams] float32,
- * stamps [sum n_scans][2] (header.stamp sec, nsec), out [sum n_scans].  Two calls over consecutive parts of every
- * recording equal one call.  B2S_ERR_BAD_PARAMS (nothing enqueued) for NULL arrays or a negative count. */
+ * recording, no host round trip between scans).  Recordings are processor-major and ragged: ranges holds n_scans[0]
+ * scans of n_beams[0] floats, then n_scans[1] scans of n_beams[1] floats, ...; range_limits [sum n_scans][2] = each
+ * scan's float32 (range_min, range_max); stamps [sum n_scans][2] (header.stamp sec, nsec); out [sum n_scans].  Works on
+ * handles of both create functions.  Two calls over consecutive parts of every recording, cut anywhere per recording,
+ * equal one call.  Refused before anything is enqueued or written, every recording's state unchanged:
+ * B2S_ERR_BAD_PARAMS for a NULL n_scans, a negative count or NULL arrays when the call has scans; B2S_ERR_TOO_LARGE for
+ * more than 2^31 - 1 scans. */
+b2s_status b2s_plicp_odom_process_fleet(b2s_plicp_odom *h, const int32_t *n_scans, const float *ranges,
+                                        const float *range_limits, const uint32_t *stamps, b2s_plicp_odom_step *out);
+/* b2s_plicp_odom_process_fleet with the create-time range fields for every scan: ranges [sum n_scans][n_beams].
+ * B2S_ERR_BAD_PARAMS on a handle from b2s_plicp_odom_create_fleet (it has no create-time fields). */
 b2s_status b2s_plicp_odom_process(b2s_plicp_odom *h, const int32_t *n_scans, const float *ranges, const uint32_t *stamps,
                                   b2s_plicp_odom_step *out);
 /* a fresh node for one recording, or for all with recording = -1: its next scan initialises it */
