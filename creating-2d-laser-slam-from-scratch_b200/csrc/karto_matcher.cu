@@ -149,8 +149,8 @@ struct b2s_matcher {
   bool sat_valid = false;
   Buf<unsigned long long> d_stats;      // [0] beam-angle pairs dropped as empty windows, [1] angles pruned, last sweep
   HostBuf<unsigned long long> h_stats;  // pinned copy, read back with the results
-  Buf<uint8_t> d_pools;                 // [B][pool_pitch] 4x4 max-pooled grids (k_grid_pool), when they fit (pool_fits)
-  Buf<uint8_t> d_pools7;                // [B][pool7_pitch] 7x7 max-pooled grids of the group pass (pool7_fits)
+  PoolLayout pool[2];                   // the 4x4 and 7x7 max-pooled grids' layouts (pool_layout), fixed at create
+  Buf<uint8_t> d_pools[2];              // [B][pool[i].pitch] the pooled grids (k_grid_pool), when they fit
   Buf<double> d_ubr;                    // [B][nA] angle bounds of a pruned sweep (NaN: not bounded one by one)
   Buf<double> d_gub;                    // [B][ceil(nA / BOUND_GROUP)] group bounds of a pruned sweep
   Buf<int32_t> d_n_eval;                // [B] angles k_prune_select left for k_sweep_bound<BOUND_SELECT>
@@ -557,7 +557,7 @@ __global__ void __launch_bounds__(256)
 
 // ----------------------------------------------------------------------------------------------
 // k_grid_pool<K>: per match, the K x K max-pooled grid (K = 4: P of k_sweep_bound; K = 7: P7 of k_sweep_bound_group)
-// in its four residue planes (layout: pool_lead / pool7_lead, pool_plane / pool7_plane, pool_index in
+// in its four residue planes (layout: pool_layout and pool_index in
 // karto_sweep_plan.cuh).  The pooling is in FLAT index space, rows wrapping exactly as a candidate's `base + offset`
 // does, so the pooled byte at a block's corner is at least every byte a candidate of that block reads.  Thread q pools
 // P[f] for the 16 indices j = f + lead in [16q, 16q + 16) and writes word q of each plane; grid bytes outside
@@ -2359,18 +2359,14 @@ static b2s_status build_sat(b2s_matcher *m) {
   return B2S_OK;
 }
 
-// (re)build the per-match pooled grids of the angle-pruning bound after the grids changed (when they fit, see pool_fits)
+// (re)build the per-match pooled grids of the angle-pruning bound after the grids changed (the ones that fit)
 static b2s_status build_pool(b2s_matcher *m) {
-  if (!pool_fits(m->g, m->smem_optin, m->win_static_smem)) return B2S_OK;
-  const int plane = pool_plane(m->g);
-  k_grid_pool<4><<<dim3((unsigned)ceil_div(plane / 4, 256), grid_rows(m->batch)), 256, 0, m->stream>>>(
-      m->d_grids, m->grid_pitch, m->g.data_size, m->g.width_step, pool_lead(m->g.width_step), plane, m->d_pools,
-      pool_pitch(m->g), m->batch);
-  if (pool7_fits(m->g, m->smem_optin, m->win_static_smem)) {
-    const int plane7 = pool7_plane(m->g);
-    k_grid_pool<7><<<dim3((unsigned)ceil_div(plane7 / 4, 256), grid_rows(m->batch)), 256, 0, m->stream>>>(
-        m->d_grids, m->grid_pitch, m->g.data_size, m->g.width_step, pool7_lead(m->g.width_step), plane7, m->d_pools7,
-        pool7_pitch(m->g), m->batch);
+  for (int i = 0; i < 2; i++) {
+    const PoolLayout &l = m->pool[i];
+    if (!l.fits) continue;
+    auto kern = i ? k_grid_pool<7> : k_grid_pool<4>;
+    kern<<<dim3((unsigned)ceil_div(l.plane / 4, 256), grid_rows(m->batch)), 256, 0, m->stream>>>(
+        m->d_grids, m->grid_pitch, m->g.data_size, m->g.width_step, l.lead, l.plane, m->d_pools[i], l.pitch, m->batch);
   }
   B2S_CUDA_CHECK(cudaGetLastError());
   return B2S_OK;
@@ -2433,8 +2429,10 @@ static b2s_status matcher_create_impl(const b2s_matcher_params *params, const b2
   m->sby = (g.height + 3) / 4;
   B2S_CUDA_CHECK(m->d_sat.reserve(B * sat_stride(m->sbx, m->sby)));
   B2S_CUDA_CHECK(m->d_stats.reserve(2));
-  if (pool_fits(g, m->smem_optin, m->win_static_smem)) B2S_CUDA_CHECK(m->d_pools.reserve(B * pool_pitch(g)));
-  if (pool7_fits(g, m->smem_optin, m->win_static_smem)) B2S_CUDA_CHECK(m->d_pools7.reserve(B * pool7_pitch(g)));
+  for (int i = 0; i < 2; i++) {
+    m->pool[i] = pool_layout(g, i ? 7 : 4, m->smem_optin, m->win_static_smem);
+    if (m->pool[i].fits) B2S_CUDA_CHECK(m->d_pools[i].reserve(B * m->pool[i].pitch));
+  }
   B2S_CUDA_CHECK(m->d_part_best.reserve(B));
   B2S_CUDA_CHECK(m->d_glob_best.reserve(B));
   B2S_CUDA_CHECK(m->d_tie.reserve(B * 5));
@@ -3065,6 +3063,46 @@ static b2s_status count_empty(b2s_matcher *m) {
   return B2S_OK;
 }
 
+// k_sweep_bound in mode MODE: the group pass over the 7x7 image, or single angles over the 4x4 image and the SAT
+template <int MODE>
+static b2s_status launch_bound(b2s_matcher *m, const SweepPlan &pl, const b2s_search &s) {
+  constexpr bool GRP = MODE == BOUND_GROUPS;
+  const PoolLayout &l = m->pool[GRP];
+  const int rows = GRP ? pl.group_rows : pl.bound_rows;
+  const size_t smem = (GRP ? pl.group_smem : pl.bound_smem) + (size_t)rows * BOUND_ROW_BYTES;
+  auto kern = (GRP ? pl.group_stage : pl.bound_stage) ? k_sweep_bound<true, MODE> : k_sweep_bound<false, MODE>;
+  B2S_CUDA_CHECK(cudaMemsetAsync(m->d_work, 0, sizeof(int), m->stream));
+  B2S_CUDA_CHECK(raise_dyn_smem(kern, smem));
+  kern<<<pl.ctas, WIN_THREADS, smem, m->stream>>>(
+      m->d_pools[GRP], l.pitch, l.bytes, l.plane, l.lead, m->d_local, m->d_grid_off, m->d_bases,
+      !GRP && pl.skip_empty ? m->d_sat.p : nullptr, m->sbx, m->sby, m->g.height, pl.rows_total, pl.tiles_x * 32,
+      1.0 / m->p.resolution, m->d_flags, m->d_centers, m->p, s, m->batch, m->n, pl.na, pl.nx, pl.ny, m->g.width_step,
+      m->g.data_size, m->d_ubr, m->d_gub, m->d_angles, m->d_n_angles, m->d_keep, m->d_n_eval, m->d_cuts,
+      m->d_stats.p + 1, m->d_bscratch, rows, m->d_work);
+  B2S_CUDA_CHECK(cudaGetLastError());
+  return B2S_OK;
+}
+
+// the response sweep of a pruned search: group bounds, then bounds, probe, select, sweep the selected angles
+static b2s_status run_pruned(b2s_matcher *m, const SweepPlan &pl, const b2s_search &s, int k_first) {
+  const int B = m->batch, na = pl.na;
+  if (pl.group) {
+    if (b2s_status st = launch_bound<BOUND_GROUPS>(m, pl, s)) return st;
+  } else {  // every group unbounded (0x7f7f... is a double near 1.4e306): every angle is bounded one by one
+    B2S_CUDA_CHECK(cudaMemsetAsync(m->d_gub, 0x7f, sizeof(double) * (size_t)B * ceil_div(na, BOUND_GROUP), m->stream));
+  }
+  if (b2s_status st = launch_bound<BOUND_PROBE>(m, pl, s)) return st;
+  if (b2s_status st = launch_lists(m, pl, s, k_first, ceil_div(PRUNE_PROBE, OFF_CHUNK), false)) return st;
+  if (b2s_status st = launch_window(m, pl, m->d_angles)) return st;
+  k_prune_select<<<B, 256, 0, m->stream>>>(m->d_sums, m->d_ubr, m->d_gub, m->d_centers, m->d_flags, m->p, s, m->n,
+                                           pl.nx, pl.ny, na, m->d_angles, m->d_n_angles, m->d_keep, m->d_n_eval,
+                                           m->d_cuts, m->d_stats.p + 1);
+  B2S_CUDA_CHECK(cudaGetLastError());
+  if (b2s_status st = launch_bound<BOUND_SELECT>(m, pl, s)) return st;
+  if (b2s_status st = launch_lists(m, pl, s, k_first, ceil_div(na, OFF_CHUNK), false)) return st;
+  return launch_window(m, pl, m->d_angles);
+}
+
 // One CorrelateScan over the batch with centres already in d_centers.  Results stay in d_results.
 static b2s_status run_correlate(b2s_matcher *m, const b2s_search *s, int k_first, int na_override, ReducePhase phase) {
   B2S_NVTX("K1 correlate (lists + sweep + tail)");
@@ -3118,47 +3156,8 @@ static b2s_status run_correlate(b2s_matcher *m, const b2s_search *s, int k_first
     // L2, no k_reduce pass — was built, parity-tested and measured SLOWER on cfg 2 (not re-measured on the H100): the
     // sweep kernel owns its SM, so the tail's serial stretches are no longer hidden by a second resident CTA as they are
     // in the stand-alone k_reduce.  Removed again; DESIGN.md §4.)
-    if (pl.prune) {  // group bounds, then bounds, probe, select, sweep the selected angles (see k_sweep_bound)
-      auto bound = [&](auto kern, const uint8_t *pools, size_t pitch, int bytes, int plane, int lead, bool sat,
-                       size_t smem, int rows) -> b2s_status {
-        B2S_CUDA_CHECK(cudaMemsetAsync(m->d_work, 0, sizeof(int), m->stream));
-        smem += (size_t)rows * BOUND_ROW_BYTES;
-        B2S_CUDA_CHECK(raise_dyn_smem(kern, smem));
-        kern<<<pl.ctas, WIN_THREADS, smem, m->stream>>>(
-            pools, pitch, bytes, plane, lead, m->d_local, m->d_grid_off, m->d_bases, sat ? m->d_sat.p : nullptr,
-            m->sbx, m->sby, m->g.height, pl.rows_total, pl.tiles_x * 32, scale, m->d_flags, m->d_centers, m->p, *s, B, n,
-            na, nx, ny, m->g.width_step, m->g.data_size, m->d_ubr, m->d_gub, m->d_angles, m->d_n_angles, m->d_keep,
-            m->d_n_eval, m->d_cuts, m->d_stats.p + 1, m->d_bscratch, rows, m->d_work);
-        B2S_CUDA_CHECK(cudaGetLastError());
-        return B2S_OK;
-      };
-      const int pbytes = pool_bytes(m->g), pplane = pool_plane(m->g), plead = pool_lead(m->g.width_step);
-      auto single = [&](auto kern) {
-        return bound(kern, m->d_pools, pool_pitch(m->g), pbytes, pplane, plead, pl.skip_empty, pl.bound_smem,
-                     pl.bound_rows);
-      };
-      if (pl.group) {
-        auto group = [&](auto kern) {
-          return bound(kern, m->d_pools7, pool7_pitch(m->g), pool7_bytes(m->g), pool7_plane(m->g),
-                       pool7_lead(m->g.width_step), false, pl.group_smem, pl.group_rows);
-        };
-        if (b2s_status st = pl.group_stage ? group(k_sweep_bound<true, BOUND_GROUPS>)
-                                           : group(k_sweep_bound<false, BOUND_GROUPS>)) return st;
-      } else {  // every group unbounded (0x7f7f... is a double near 1.4e306): every angle is bounded one by one
-        B2S_CUDA_CHECK(cudaMemsetAsync(m->d_gub, 0x7f, sizeof(double) * (size_t)B * ceil_div(na, BOUND_GROUP), m->stream));
-      }
-      if (b2s_status st = pl.bound_stage ? single(k_sweep_bound<true, BOUND_PROBE>)
-                                         : single(k_sweep_bound<false, BOUND_PROBE>)) return st;
-      if (b2s_status st = launch_lists(m, pl, *s, k_first, ceil_div(PRUNE_PROBE, OFF_CHUNK), false)) return st;
-      if (b2s_status st = launch_window(m, pl, m->d_angles)) return st;
-      k_prune_select<<<B, 256, 0, m->stream>>>(m->d_sums, m->d_ubr, m->d_gub, m->d_centers, m->d_flags, m->p, *s, n,
-                                               nx, ny, na, m->d_angles, m->d_n_angles, m->d_keep, m->d_n_eval,
-                                               m->d_cuts, m->d_stats.p + 1);
-      B2S_CUDA_CHECK(cudaGetLastError());
-      if (b2s_status st = pl.bound_stage ? single(k_sweep_bound<true, BOUND_SELECT>)
-                                         : single(k_sweep_bound<false, BOUND_SELECT>)) return st;
-      if (b2s_status st = launch_lists(m, pl, *s, k_first, ceil_div(na, OFF_CHUNK), false)) return st;
-      if (b2s_status st = launch_window(m, pl, m->d_angles)) return st;
+    if (pl.prune) {
+      if (b2s_status st = run_pruned(m, pl, *s, k_first)) return st;
     } else {
       if (pl.nbands > 1)  // bands accumulate with RED.ADD
         B2S_CUDA_CHECK(cudaMemsetAsync(m->d_sums, 0, sizeof(int32_t) * (size_t)B * na * ncell, m->stream));

@@ -28,24 +28,40 @@ constexpr int PRUNE_PROBE = 16;         // angles swept exactly to find the prun
 constexpr int BOUND_GROUP = 4;
 constexpr int BOUND_SPREAD = 3;  // the origin spread per axis the 7 x 7 image covers: 7 = 4 + BOUND_SPREAD
 
-// Work items of a pruned (listed) window sweep, k_sweep_window<LISTED>.  A match that lists few angles splits each
-// angle's beams into `chunks` ranges so that every warp of its CTA gets about two items: the concatenation
-// I0 I1 I2 I3 E0 E1 E2 E3 of the angle's groups (each a multiple of 4 long) is cut on multiples of 4 beams, and the
-// ranges' partial sums meet in shared-memory accumulators beside the grid image, one ny x nx plane per listed angle,
-// of which `slots` fit.  A match that lists more angles than that is swept one item per angle, written directly.
-constexpr int WIN_CHUNK_MIN_BEAMS = 32;  // beams per range on average at least: an item costs ~250 instructions besides its beams
-__host__ __device__ inline int listed_chunks(int listed, int n, int warps, int slots) {
-  if (listed <= 0 || listed > slots) return 1;
-  const int want = (2 * warps + listed - 1) / listed;
-  const int most = n / WIN_CHUNK_MIN_BEAMS;
+// Work items of a pruned search's rounds.  A round of few units (at most `cap`, the shared-memory accumulators that
+// fit) cuts each unit's `total` beams into `chunks` ranges on multiples of QUANTUM, so that every warp of the CTA gets
+// about two items with at least MIN_BEAMS beams per range on average; the ranges' partial sums meet in the unit's
+// accumulator.  A round of more units is one item per unit.  Two instances, below: k_sweep_window<LISTED>'s (a unit is
+// a listed angle, its accumulator an ny x nx plane, acc_slots) and k_sweep_bound's (a unit is an angle or a group of
+// BOUND_GROUP angles, its accumulator a u32 row of block sums, bound_rows / group_rows; 32: a warp's placement pass).
+constexpr int WIN_CHUNK_MIN_BEAMS = 32;     // a window item costs ~250 instructions besides its beams
+constexpr int BOUND_CHUNK_MIN_BEAMS = 128;  // a bound item costs the unit's sincos, shuffles and row adds besides its beams
+constexpr int BOUND_ROW_BYTES = 64 * 4;     // one u32 per 4 x 4 block of the 32 x 32 candidate tile
+template <int QUANTUM, int MIN_BEAMS>
+__host__ __device__ inline int split_chunks(int units, int n, int warps, int cap) {
+  static_assert(MIN_BEAMS % QUANTUM == 0, "a range of MIN_BEAMS beams is whole quanta");
+  if (units <= 0 || units > cap) return 1;
+  const int want = (2 * warps + units - 1) / units;
+  const int most = n / MIN_BEAMS;
   return most < 2 ? 1 : (want < most ? want : most);
 }
-// the range [lo, hi) of chunk c of `chunks` in the concatenated groups of an angle that lists `total` beams (% 4 == 0)
-__host__ __device__ inline void chunk_range(int total, int c, int chunks, int &lo, int &hi) {
-  const long long q = total >> 2;
-  lo = 4 * (int)(q * c / chunks);
-  hi = 4 * (int)(q * (c + 1) / chunks);
+__host__ __device__ constexpr int log2_of(int v) { return v > 1 ? 1 + log2_of(v >> 1) : 0; }
+// the beams [lo, hi) of range c of `chunks` of a unit of `total` beams
+template <int QUANTUM>
+__host__ __device__ inline void split_range(int total, int c, int chunks, int &lo, int &hi) {
+  static_assert((QUANTUM & (QUANTUM - 1)) == 0, "a power of two: the quanta are a shift");
+  const long long q = (total + QUANTUM - 1) >> log2_of(QUANTUM);
+  lo = QUANTUM * (int)(q * c / chunks);
+  hi = QUANTUM * (int)(q * (c + 1) / chunks);
+  if ((total & (QUANTUM - 1)) && hi > total) hi = total;  // only a total of part quanta ends inside the last one
 }
+// the window's: an angle's beams are its groups I0 I1 I2 I3 E0 E1 E2 E3, each a multiple of 4 long; the mask tells the
+// compiler so, and split_range's round-up and clamp vanish
+__host__ __device__ inline int listed_chunks(int listed, int n, int warps, int slots) { return split_chunks<4, WIN_CHUNK_MIN_BEAMS>(listed, n, warps, slots); }
+__host__ __device__ inline void chunk_range(int total, int c, int chunks, int &lo, int &hi) { split_range<4>(total & ~3, c, chunks, lo, hi); }
+// the bound's
+__host__ __device__ inline int bound_chunks(int units, int n, int warps, int rows) { return split_chunks<32, BOUND_CHUNK_MIN_BEAMS>(units, n, warps, rows); }
+__host__ __device__ inline void bound_range(int n, int c, int chunks, int &lo, int &hi) { split_range<32>(n, c, chunks, lo, hi); }
 // the part of each group g (count[g] beams) that lies in [lo, hi): beams off[g] .. off[g] + len[g] of the group
 __host__ __device__ inline void chunk_groups(const int32_t *count, int lo, int hi, int (&off)[8], int (&len)[8]) {
   int p = 0;
@@ -58,63 +74,40 @@ __host__ __device__ inline void chunk_groups(const int32_t *count, int lo, int h
   }
 }
 
-// Work items of the angle bound, k_sweep_bound.  A round bounds `units` units (an angle, or a group of BOUND_GROUP
-// angles).  When it has few, each unit's beams are cut into `chunks` ranges on multiples of 32 (one placement pass of
-// a warp), so that every warp of the CTA gets about two items.  The ranges' 64 block sums meet in one u32 row per unit
-// in shared memory after the bound's staged data, of which `rows` fit (SweepPlan::bound_rows / group_rows).  A round
-// of more units than that is bounded one item per unit, each summed and scored by one warp.
-constexpr int BOUND_CHUNK_MIN_BEAMS = 128;  // an item costs the unit's sincos, shuffles and row adds besides its beams
-constexpr int BOUND_ROW_BYTES = 64 * 4;     // one u32 per 4 x 4 block of the 32 x 32 candidate tile
-__host__ __device__ inline int bound_chunks(int units, int n, int warps, int rows) {
-  if (units <= 0 || units > rows) return 1;
-  const int want = (2 * warps + units - 1) / units;
-  const int most = n / BOUND_CHUNK_MIN_BEAMS;
-  return most < 2 ? 1 : (want < most ? want : most);
-}
-// the beams [lo, hi) of range c of `chunks` of a unit of n beams
-__host__ __device__ inline void bound_range(int n, int c, int chunks, int &lo, int &hi) {
-  const long long q = (n + 31) >> 5;
-  lo = 32 * (int)(q * c / chunks);
-  hi = 32 * (int)(q * (c + 1) / chunks);
-  if (hi > n) hi = n;
-}
-
 // u16 entries per match of the block summed-area tables (k_grid_sat), padded to 16 bytes
 inline size_t sat_stride(int sbx, int sby) { return (size_t)((((sbx + 1) * (sby + 1)) + 7) & ~7); }
-// The 4x4 max-pooled grid (k_grid_pool) of one match: P[f] = max over dy, dx in [0, 4) of grid[f + dy * width_step + dx]
-// (0 outside the grid), for f from -pool_lead (a block whose corner lies above the grid still reaches it).  It is
-// stored as four planes split by the residue of j = f + pool_lead modulo 4: plane j & 3 byte j >> 2 holds P[f]
-// (pool_index), each plane pool_plane bytes long.  A beam's 8 block corners of one block row are 4 apart in f, so
-// they are 8 contiguous bytes of one plane, and the rows are width_step bytes apart in it (width_step % 8 == 0: one
-// word alignment for all 8 rows).  Each plane ends with POOL_PAD or more zero bytes (P of indices past the grid):
-// the corners of an interior window lie within WIN_GUARD - 16 flat bytes (28 plane bytes) of the grid, and the
-// three-word read that fetches 8 of them reaches at most 4 bytes past the last one, so an interior beam reads zeros
-// there and never enters the next plane.  pool_bytes is what the bound pass stages, pool_pitch the stride.
+// The K x K max-pooled grid (k_grid_pool) of one match, K = 4 for k_sweep_bound's single angles, K = 7 for its group
+// pass: P[f] = max over dy, dx in [0, K) of grid[f + dy * width_step + dx] (0 outside the grid), for f from -lead on:
+// 4 rows (a block whose corner lies above the grid still reaches it), 8 for K = 7 (a group's low corner lies up to
+// BOUND_SPREAD rows and columns before any member's origin).  It is stored as four planes split by the residue of
+// j = f + lead modulo 4: plane j & 3 byte j >> 2 holds P[f] (pool_index), each plane `plane` bytes long.  A beam's 8
+// block corners of one block row are 4 apart in f, so they are 8 contiguous bytes of one plane, and the rows are
+// width_step bytes apart in it (width_step % 8 == 0: one word alignment for all 8 rows).  Each plane ends with
+// POOL_PAD or more zero bytes (P of indices past the grid): the corners of an interior window lie within WIN_GUARD - 16
+// flat bytes (28 plane bytes) of the grid, and the three-word read that fetches 8 of them reaches at most 4 bytes past
+// the last one, so an interior beam reads zeros there and never enters the next plane.  pool_bytes is what the bound
+// pass stages; pool_fits says whether the image and its guards fit k_sweep_bound's shared memory (its static shared
+// memory is below k_sweep_window's, so the window kernel's budget covers it).  Without the 4x4 image there is no
+// pruning, without the 7x7 one no group pass.
 constexpr int POOL_PAD = 32;
-inline int pool_lead(int width_step) { return 4 * width_step; }
-inline int pool_plane(const b2s_grid_info &g) { return ((pool_lead(g.width_step) + g.data_size) / 4 + POOL_PAD + 15) & ~15; }
-inline int pool_bytes(const b2s_grid_info &g) { return 4 * pool_plane(g); }
-inline size_t pool_pitch(const b2s_grid_info &g) { return ((size_t)pool_bytes(g) + 127) & ~(size_t)127; }
-// The 7x7 max-pooled grid of the group pass, P7[f] = max over dy, dx in [0, 7) of grid[f + dy * width_step + dx], in
-// the same four-plane layout (pool_index with pool7_lead / pool7_plane), from f = -pool7_lead on: the low corner of a
-// group's origins lies up to BOUND_SPREAD rows and columns before any member's origin.
-inline int pool7_lead(int width_step) { return 8 * width_step; }
-inline int pool7_plane(const b2s_grid_info &g) { return ((pool7_lead(g.width_step) + g.data_size) / 4 + POOL_PAD + 15) & ~15; }
-inline int pool7_bytes(const b2s_grid_info &g) { return 4 * pool7_plane(g); }
-inline size_t pool7_pitch(const b2s_grid_info &g) { return ((size_t)pool7_bytes(g) + 127) & ~(size_t)127; }
+inline int pool_lead(int width_step, int K = 4) { return (K == 4 ? 4 : 8) * width_step; }
+inline int pool_plane(const b2s_grid_info &g, int K = 4) { return ((pool_lead(g.width_step, K) + g.data_size) / 4 + POOL_PAD + 15) & ~15; }
+inline int pool_bytes(const b2s_grid_info &g, int K = 4) { return 4 * pool_plane(g, K); }
+inline int pool7_bytes(const b2s_grid_info &g) { return pool_bytes(g, 7); }
+inline bool pool_fits(const b2s_grid_info &g, int smem_optin, size_t win_static, int K = 4) {
+  return (long long)pool_bytes(g, K) + 2 * WIN_GUARD <= (long long)smem_optin - (long long)win_static - 512;
+}
+// the K x K image's layout, as the handle keeps it from create on (pitch: the per-match stride of its buffer)
+struct PoolLayout { int lead, plane, bytes; size_t pitch; bool fits; };
+inline PoolLayout pool_layout(const b2s_grid_info &g, int K, int smem_optin, size_t win_static) {
+  const int bytes = pool_bytes(g, K);
+  return {pool_lead(g.width_step, K), pool_plane(g, K), bytes, ((size_t)bytes + 127) & ~(size_t)127,
+          pool_fits(g, smem_optin, win_static, K)};
+}
 // the byte of the staged pooled image that holds P[f]
 __host__ __device__ __forceinline__ int pool_index(int f, int lead, int plane) {
   const int j = f + lead;
   return (j & 3) * plane + (j >> 2);
-}
-// the pooled image and its guards fit in k_sweep_bound's shared memory (k_sweep_bound's static shared memory is below
-// k_sweep_window's, so the window kernel's budget covers it)
-inline bool pool_fits(const b2s_grid_info &g, int smem_optin, size_t win_static) {
-  return (long long)pool_bytes(g) + 2 * WIN_GUARD <= (long long)smem_optin - (long long)win_static - 512;
-}
-// the same for the 7x7 image of the group pass (whose static shared memory is k_sweep_bound's)
-inline bool pool7_fits(const b2s_grid_info &g, int smem_optin, size_t win_static) {
-  return (long long)pool7_bytes(g) + 2 * WIN_GUARD <= (long long)smem_optin - (long long)win_static - 512;
 }
 // doubles per match of the per-cell maxima plane (m_pSearchSpaceProbs), rows padded to 8
 inline size_t probs_len(int search_side) { return (size_t)((search_side + 7) & ~7) * search_side; }
@@ -167,11 +160,10 @@ struct SweepPlan {
   bool group = false;
   bool group_stage = false;  // the group pass stages the scan-local points after its image
   size_t group_smem = 0;     // its dynamic shared memory: 7x7 image + guards (+ points when staged)
-  // the bound's per-unit rows of block sums (bound_chunks), BOUND_ROW_BYTES each after bound_smem / group_smem, up to
-  // 2 * warps - 1 of them (a round of more units is not split); 0: every unit is one item
+  // the accumulators of split_chunks, up to 2 * warps - 1 of them (a round of more units is not split): the bound's
+  // per-unit rows of block sums, BOUND_ROW_BYTES each after bound_smem / group_smem (0: every unit is one item), and
+  // the listed sweeps' ny x nx planes after the grid image
   int bound_rows = 0, group_rows = 0;
-  // the listed sweeps of a pruned search: ny x nx accumulator planes after the grid image (listed_chunks), up to
-  // 2 * warps - 1 of them (a match that lists more angles is not split)
   int acc_slots = 0;
   size_t listed_smem = 0;  // win_smem + the planes
 };
@@ -255,28 +247,31 @@ inline SweepPlan plan_sweep(const b2s_matcher_params &p, const b2s_grid_info &g,
   // Pruning needs the whole grid and the whole pooled image in shared memory, one 32 x 32 stride-1 candidate tile (the
   // bound's 8 x 8 blocks of 4 x 4 candidates), and the whole angle range of a search: an angle subset of a split sweep
   // cannot know the global best.  Selector 3 sweeps every beam and every angle.
-  pl.bound_smem = (size_t)pool_bytes(g) + 2 * WIN_GUARD;
+  const PoolLayout pool = pool_layout(g, 4, smem_optin, win_static), pool7 = pool_layout(g, 7, smem_optin, win_static);
+  pl.bound_smem = (size_t)pool.bytes + 2 * WIN_GUARD;
   pl.prune = pl.use_window && pl.nbands == 1 && pl.stride == 1 && pl.tiles_x == 1 && pl.tiles_y == 1 &&
-             na_override < 0 && force_kernel != 3 && pl.na >= PRUNE_MIN_ANGLES && pl.na <= PRUNE_MAX_ANGLES &&
-             pool_fits(g, smem_optin, win_static);
-  const size_t staged = bound_stage_bytes(n, pl.skip_empty, sbx, sby);
-  pl.bound_stage = pl.prune && (long long)(pl.bound_smem + staged) <= smem_limit;
-  if (pl.bound_stage) pl.bound_smem += staged;
-  pl.group = pl.prune && pool7_fits(g, smem_optin, win_static);
-  pl.group_smem = (size_t)pool7_bytes(g) + 2 * WIN_GUARD;
-  const size_t staged7 = bound_stage_bytes(n, false, sbx, sby);
-  pl.group_stage = pl.group && (long long)(pl.group_smem + staged7) <= smem_limit;
-  if (pl.group_stage) pl.group_smem += staged7;
-  if (!pl.group) pl.group_smem = 0;
-  auto rows_fit = [&](size_t used) {
-    const long long room = std::max(smem_limit - (long long)used, 0LL);
-    return (int)std::min<long long>(2 * (WIN_THREADS / 32) - 1, room / BOUND_ROW_BYTES);
+             na_override < 0 && force_kernel != 3 && pl.na >= PRUNE_MIN_ANGLES && pl.na <= PRUNE_MAX_ANGLES && pool.fits;
+  pl.group = pl.prune && pool7.fits;
+  pl.group_smem = (size_t)pool7.bytes + 2 * WIN_GUARD;
+  // a pass that runs stages `staged` bytes after its image of `smem` bytes when both fit
+  auto stage = [&](bool runs, size_t &smem, size_t staged) {
+    const bool fits = runs && (long long)(smem + staged) <= smem_limit;
+    if (fits) smem += staged;
+    return fits;
   };
-  if (pl.prune) pl.bound_rows = rows_fit(pl.bound_smem);
-  if (pl.group) pl.group_rows = rows_fit(pl.group_smem);
+  pl.bound_stage = stage(pl.prune, pl.bound_smem, bound_stage_bytes(n, pl.skip_empty, sbx, sby));
+  pl.group_stage = stage(pl.group, pl.group_smem, bound_stage_bytes(n, false, sbx, sby));
+  if (!pl.group) pl.group_smem = 0;
+  // the accumulators of `unit` bytes that fit after `used` bytes
+  auto accumulators = [&](size_t used, long long unit) {
+    const long long room = std::max(smem_limit - (long long)used, 0LL);
+    return (int)std::min<long long>(2 * (WIN_THREADS / 32) - 1, room / unit);
+  };
+  if (pl.prune) pl.bound_rows = accumulators(pl.bound_smem, BOUND_ROW_BYTES);
+  if (pl.group) pl.group_rows = accumulators(pl.group_smem, BOUND_ROW_BYTES);
   if (pl.prune) {
-    const long long plane = 4LL * pl.nx * pl.ny, room = smem_limit - (long long)pl.win_smem;
-    pl.acc_slots = (int)std::min<long long>(2 * (WIN_THREADS / 32) - 1, std::max(room, 0LL) / plane);
+    const long long plane = 4LL * pl.nx * pl.ny;
+    pl.acc_slots = accumulators(pl.win_smem, plane);
     pl.listed_smem = pl.win_smem + (size_t)(pl.acc_slots * plane);
   }
   return pl;

@@ -1,6 +1,6 @@
 """plan_sweep (csrc/karto_sweep_plan.cuh) decides on the host, before anything is enqueued, which sweep kernel a
 CorrelateScan runs, with which candidate stride, row bands and shared-memory sizes, or why the search is refused.
-tests/sweep_plan_check.cu runs it without a GPU.  Checked here: the geometries of the benchmark and of the GPU matcher
+tests/sweep_plan_check.cu runs it without a GPU, for this module and the other test_sweep_plan_* modules.  Checked here: the geometries of the benchmark and of the GPU matcher
 tests, every kernel selector, every refusal, and the invariants the kernels rely on over a seeded random sweep."""
 import importlib
 import json
@@ -25,7 +25,7 @@ WIN_MAX_BANDS = 32
 OK, BAD_PARAMS, TOO_LARGE = 0, 1, 7  # B2S_OK, B2S_ERR_BAD_PARAMS, B2S_ERR_TOO_LARGE
 
 
-@pytest.fixture(scope="module")
+@pytest.fixture(scope="session")
 def plan(tmp_path_factory):
     build = importlib.import_module("creating-2d-laser-slam-from-scratch_b200.build")
     exe = str(tmp_path_factory.mktemp("sweep_plan") / "sweep_plan_check")
@@ -43,10 +43,10 @@ def params(search, res, smear, rt):
     return f"{search!r} {res!r} {smear!r} {rt!r}"
 
 
-def plan_request(p, n, batch, search, k_first=0, na_override=-1, force=0, sat_valid=1, high_bytes=0):
+def plan_request(p, n, batch, search, k_first=0, na_override=-1, force=0, sat_valid=1, high_bytes=0, optin=OPTIN):
     ox, oy, rx, ry, ao, ar, fine = search
     return (f"plan {p} {n} {batch} {ox!r} {oy!r} {rx!r} {ry!r} {ao!r} {ar!r} {fine} {k_first} {na_override} {force} "
-            f"{sat_valid} {high_bytes} {SMS} {OPTIN} {WIN_STATIC}")
+            f"{sat_valid} {high_bytes} {SMS} {optin} {WIN_STATIC}")
 
 
 def window(side, res, mult=1, angle_offset=10 * D, angle_res=1 * D, fine=0):

@@ -1,87 +1,13 @@
-"""The work items of a pruned window sweep (csrc/karto_sweep_plan.cuh: listed_chunks, chunk_range, chunk_groups): a
-match that lists few angles splits each angle's groups I0..I3 E0..E3 into beam ranges cut on multiples of 4, which
-k_sweep_window<LISTED> sums in shared memory.  Checked on the host, without a GPU: every listed beam lies in exactly one
-range, every range boundary and every part of a group starts on a multiple of 4, empty groups included, and the
-split keeps about two items per warp within the accumulators that fit."""
-import importlib
-import json
-import subprocess
-
+"""The work items of a pruned window sweep (csrc/karto_sweep_plan.cuh: split_chunks<4, 32>, split_range<4>,
+chunk_groups): a match that lists few angles splits each angle's groups I0..I3 E0..E3 into beam ranges cut on multiples
+of 4, which k_sweep_window<LISTED> sums in shared memory.  Checked on the host, without a GPU (tests/sweep_plan_check.cu):
+every listed beam lies in exactly one range, every range boundary and every part of a group starts on a multiple of 4,
+empty groups included, and the split keeps about two items per warp within the accumulators that fit."""
 import numpy as np
-import pytest
+
+from test_sweep_plan import CFG2, CFG2_SEARCH, plan, plan_request  # noqa: F401 (plan: the driver fixture)
 
 WARPS = 16  # WIN_THREADS / 32
-
-DRIVER = r"""
-#include <cmath>
-#include <cstdio>
-#include <iostream>
-#include <sstream>
-#include "karto_sweep_plan.cuh"
-using namespace b2s;
-// request: plan                                           -> the benchmark search's accumulator planes
-//          chunks <listed> <n> <warps> <slots>            -> {"chunks": C}
-//          split <C> <count0> .. <count7>                  -> {"items": [[off0, len0, .., off7, len7], ...]}
-int main() {
-  std::string line;
-  while (std::getline(std::cin, line)) {
-    std::istringstream in(line);
-    std::string cmd;
-    in >> cmd;
-    if (cmd == "plan") {  // the benchmark's search: 1081 beams, 31 x 31 x 181 on a 0.05 m grid, the H100's budget
-      b2s_matcher_params p = {};
-      p.search_size = 1.5; p.resolution = 0.05; p.smear_deviation = 0.03; p.range_threshold = 9.25;
-      b2s_search s = {};
-      s.offset_x = s.offset_y = 0.75; s.res_x = s.res_y = 0.05; s.angle_offset = 22.5 * M_PI / 180; s.angle_res = 0.25 * M_PI / 180;
-      const b2s_grid_info g = grid_layout(p);
-      const SweepPlan pl = plan_sweep(p, g, s, 1081, 1024, 0, -1, 0, true, false, (g.width_step + 3) / 4,
-                                      (g.height + 3) / 4, 132, 232448, 3200);
-      printf("{\"prune\": %d, \"acc_slots\": %d, \"listed_smem\": %zu, \"win_smem\": %zu}\n", (int)pl.prune,
-             pl.acc_slots, pl.listed_smem, pl.win_smem);
-      continue;
-    }
-    if (cmd == "chunks") {
-      int listed, n, warps, slots;
-      in >> listed >> n >> warps >> slots;
-      printf("{\"chunks\": %d}\n", listed_chunks(listed, n, warps, slots));
-      continue;
-    }
-    int C;
-    int32_t cnt[8];
-    in >> C;
-    for (int g = 0; g < 8; g++) in >> cnt[g];
-    const int total = cnt[0] + cnt[1] + cnt[2] + cnt[3] + cnt[4] + cnt[5] + cnt[6] + cnt[7];
-    printf("{\"items\": [");
-    for (int c = 0; c < C; c++) {
-      int lo, hi, off[8], len[8];
-      chunk_range(total, c, C, lo, hi);
-      chunk_groups(cnt, lo, hi, off, len);
-      printf("%s[%d, %d", c ? ", " : "", lo, hi);
-      for (int g = 0; g < 8; g++) printf(", %d, %d", off[g], len[g]);
-      printf("]");
-    }
-    printf("]}\n");
-  }
-  return 0;
-}
-"""
-
-
-@pytest.fixture(scope="module")
-def run(tmp_path_factory):
-    build = importlib.import_module("creating-2d-laser-slam-from-scratch_b200.build")
-    d = tmp_path_factory.mktemp("chunks")
-    src, exe = d / "chunks.cu", str(d / "chunks")
-    src.write_text(DRIVER)
-    subprocess.check_call([build.nvcc(), "-std=c++17", "-O2", "-gencode", "arch=compute_90a,code=sm_90a",
-                           "-I", build.os.path.join(build.HERE, "csrc"), "-I", build.os.path.join(build.HERE, "..", "include"),
-                           str(src), "-o", exe])
-
-    def go(reqs):
-        out = subprocess.run([exe], input="".join(r + "\n" for r in reqs), capture_output=True, text=True, check=True)
-        return [json.loads(line) for line in out.stdout.splitlines()]
-
-    return go
 
 
 def check_split(C, counts, items):
@@ -116,30 +42,30 @@ def group_counts(rng, n):
     return [int(v) for v in c]
 
 
-def test_every_listed_beam_in_exactly_one_range(run):
+def test_every_listed_beam_in_exactly_one_range(plan):
     rng = np.random.default_rng(5)
     cases = []
     for n in (1, 3, 4, 5, 31, 33, 64, 1081, 4500, 9000):
         for listed in (1, 2, 3, 15, 16, 17, 31, 32, 181, 1024):
-            C = run([f"chunks {listed} {n} {WARPS} 16"])[0]["chunks"]
+            C = plan([f"chunks 4 {listed} {n} {WARPS} 16"])[0]["chunks"]
             for counts in ([0] * 8, [4 * ((n + 3) // 4)] + [0] * 7, [0] * 7 + [4 * ((n + 3) // 4)], group_counts(rng, n),
                            group_counts(rng, n)):
                 cases.append((C, counts))
     for C in (2, 3, 7, 16, 32, 33):  # more ranges than quads of beams: empty ranges
         cases.append((C, [4, 0, 0, 8, 0, 0, 4, 0]))
-    out = run([f"split {C} " + " ".join(map(str, counts)) for C, counts in cases])
+    out = plan([f"split {C} " + " ".join(map(str, counts)) for C, counts in cases])
     for (C, counts), r in zip(cases, out):
         check_split(C, counts, r["items"])
 
 
-def test_chunk_rule(run):
+def test_chunk_rule(plan):
     reqs, want = [], []
     for n in range(1, 9001, 97):
         for listed in list(range(1, 40)) + [181, 1024]:
             for slots in (0, 1, 15, 16, 31):
-                reqs.append(f"chunks {listed} {n} {WARPS} {slots}")
+                reqs.append(f"chunks 4 {listed} {n} {WARPS} {slots}")
                 want.append((listed, n, slots))
-    for (listed, n, slots), r in zip(want, run(reqs)):
+    for (listed, n, slots), r in zip(want, plan(reqs)):
         C = r["chunks"]
         assert C >= 1
         if listed > slots or n < 64:  # the planes do not fit, or too few beams for two ranges: one item per angle
@@ -150,10 +76,10 @@ def test_chunk_rule(run):
         assert n // C >= 32, (listed, n, slots, C)                            # at least 32 beams per range on average
 
 
-def test_cfg2_lists_fit_the_accumulators(run):
+def test_cfg2_lists_fit_the_accumulators(plan):
     """at the benchmark's shape (a 165 KB grid, 31 x 31 candidates) the 16 probe angles are split in two"""
-    (pl,) = run(["plan"])
+    (pl,) = plan([plan_request(CFG2, 1081, 1024, CFG2_SEARCH)])
     assert pl["prune"] and pl["acc_slots"] == 16, pl
     assert pl["listed_smem"] == pl["win_smem"] + 16 * 31 * 31 * 4 and pl["listed_smem"] + 3200 + 512 <= 232448, pl
-    out = run([f"chunks {listed} 1081 {WARPS} {pl['acc_slots']}" for listed in (16, 2, 1, 3, 17)])
+    out = plan([f"chunks 4 {listed} 1081 {WARPS} {pl['acc_slots']}" for listed in (16, 2, 1, 3, 17)])
     assert [r["chunks"] for r in out] == [2, 16, 32, 11, 1]
