@@ -12,7 +12,7 @@ CSRC = os.path.join(HERE, "csrc")
 OBJ = os.path.join(CSRC, "build")
 LIB = os.path.join(HERE, "libb200slam.so")
 SOURCES = ["library.cu", "karto_matcher.cu", "karto_occgrid.cu", "hector_map.cu", "hector_slam.cu", "gmapping_map.cu", "plicp.cu", "plicp_odometry.cu", "plicp_scan_match.cu","karto_mapper.cu", "pose_graph.cu", "ros_io.cu", "lidar_undistortion.cu", "pcl_icp.cu", "feature_detection.cu", "lesson4_node_maps.cu", "karto_node.cu", "hector_node.cu"]
-HEADERS = ["common.cuh", "scan_kernels.cuh", "glibc_math.cuh", "hector_grid.cuh", "karto_sweep_plan.cuh", "hector_node_plan.cuh", "introsort.cuh", "hector_scan.cuh", "plicp_pair.cuh", "gmapping_grid.cuh", "ros_math.cuh", os.path.join("..", "..", "include", "b200slam.h")]
+HEADERS = ["common.cuh", "scan_kernels.cuh", "glibc_math.cuh", "hector_grid.cuh", "karto_sweep_plan.cuh", "hector_node_plan.cuh", "introsort.cuh", "hector_scan.cuh", "plicp_pair.cuh", "gmapping_grid.cuh", "ros_math.cuh", "karto_internal.cuh", os.path.join("..", "..", "include", "b200slam.h")]
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-fmad=false", "-std=c++17",
               "-Xcompiler", "-fPIC"]
 

@@ -27,22 +27,7 @@
 #include <vector>
 
 #include "common.cuh"
-
-namespace b2s {
-// One batch of a Mapper's matches: base scans are named by their unique id in `mapper`, base_ids / base_poses
-// [batch][max_base] padded by repeating a match's last base scan.  karto_node.cu declares it too, identically.
-struct MatchRequest {
-  const b2s_mapper *mapper = nullptr;
-  int which = 0, batch = 0, max_base = 0, do_penalize = 0, do_refine = 0;
-  const double *ranges = nullptr, *poses = nullptr, *base_poses = nullptr;
-  const int32_t *base_ids = nullptr;
-  b2s_match_result *results = nullptr;
-};
-// A Mapper made by mapper_create_fleet hands each batch to `FleetMatchFn`, which runs it on a MatchPool: the Mapper's
-// own (b2s_mapper_create) or one shared by the nodes of a Karto node batch (karto_node.cu).
-typedef b2s_status (*FleetMatchFn)(void *user, const MatchRequest &r);
-struct MatchPool;
-}  // namespace b2s
+#include "karto_internal.cuh"
 
 using namespace b2s;
 

@@ -22,6 +22,7 @@
 #include <vector>
 
 #include "common.cuh"
+#include "karto_internal.cuh"
 #include "nccl_dl.cuh"
 #include "scan_kernels.cuh"
 
@@ -38,60 +39,20 @@ struct b2s_occ_grid {
 
 namespace b2s {
 
-// ---- per-beam / per-scan / per-cell device code, shared by the single-grid kernels and the batched build below
+// ---- the build: G grids, each CreateFromScans over its own scans, every stage one launch for all grids (the
+// single-grid handle is a build of one grid).  Scans are numbered over all grids (grid 0's first); scan s reads row
+// rows[s] of `ranges` (row s when rows is null) and belongs to grid scan_grid[s] (grid 0 when scan_grid is null).
 
-// per-scan bounding box over the sensor position and the FILTERED point readings
-// (InRange(reading, minRange, rangeThreshold), Karto.h:5382,5400,5418-5424).  One block of 256 threads per scan;
-// `ranges` and `pts` point at the scan's own row.
-template <class R>
-__device__ void scan_bbox_block(const R *__restrict__ ranges, const double *__restrict__ sensor,
-                                const double *__restrict__ pts, const b2s_laser &l, double *__restrict__ bbox) {
-  const int n = l.n_readings;
-  const double big = 999999999999999999.99999;  // Karto.h:2765
-  double mnx = big, mny = big, mxx = -big, mxy = -big;
-  if (threadIdx.x == 0) {
-    double x = sensor[0], y = sensor[1];
-    if (x < mnx) mnx = x;
-    if (y < mny) mny = y;
-    if (x > mxx) mxx = x;
-    if (y > mxy) mxy = y;
-  }
-  for (int i = threadIdx.x; i < n; i += blockDim.x) {
-    double r = (double)ranges[i];
-    if (!(r >= l.min_range && r <= l.range_threshold)) continue;
-    double x = pts[(size_t)i * 2], y = pts[(size_t)i * 2 + 1];
-    if (x < mnx) mnx = x;
-    if (y < mny) mny = y;
-    if (x > mxx) mxx = x;
-    if (y > mxy) mxy = y;
-  }
-  __shared__ double sh[4][256];
-  sh[0][threadIdx.x] = mnx; sh[1][threadIdx.x] = mny; sh[2][threadIdx.x] = mxx; sh[3][threadIdx.x] = mxy;
-  __syncthreads();
-  for (int d = blockDim.x / 2; d > 0; d >>= 1) {
-    if (threadIdx.x < d) {
-      sh[0][threadIdx.x] = fmin(sh[0][threadIdx.x], sh[0][threadIdx.x + d]);
-      sh[1][threadIdx.x] = fmin(sh[1][threadIdx.x], sh[1][threadIdx.x + d]);
-      sh[2][threadIdx.x] = fmax(sh[2][threadIdx.x], sh[2][threadIdx.x + d]);
-      sh[3][threadIdx.x] = fmax(sh[3][threadIdx.x], sh[3][threadIdx.x + d]);
-    }
-    __syncthreads();
-  }
-  if (threadIdx.x == 0) {
-    bbox[0] = sh[0][0]; bbox[1] = sh[1][0]; bbox[2] = sh[2][0]; bbox[3] = sh[3][0];
-  }
-}
+struct OccGridDev {       // one grid of a build, as its kernels read it
+  int w, h, step;
+  int first, scans;       // the grid's first scan and its scan count
+  double off_x, off_y, scale;
+  long long counters;     // first counter of the grid in the pass / hit arena
+  long long payload;      // first byte of its payload in the payload arena
+};
 
-// union of n_scans per-scan boxes (OccupancyGrid::ComputeDimensions, Karto.h:5810-5814); one block of 256 threads
-__device__ void bbox_union_block(const double *__restrict__ bbox, int n_scans, double *__restrict__ out) {
-  const double big = 999999999999999999.99999;
-  double mnx = big, mny = big, mxx = -big, mxy = -big;
-  for (int s = threadIdx.x; s < n_scans; s += blockDim.x) {
-    mnx = fmin(mnx, fmin(bbox[4 * s], bbox[4 * s + 2]));  // Add(min); Add(max) (Karto.h:2824-2828)
-    mny = fmin(mny, fmin(bbox[4 * s + 1], bbox[4 * s + 3]));
-    mxx = fmax(mxx, fmax(bbox[4 * s], bbox[4 * s + 2]));
-    mxy = fmax(mxy, fmax(bbox[4 * s + 1], bbox[4 * s + 3]));
-  }
+// block-wide {min x, min y, max x, max y} of the threads' boxes into out[0..3]; one block of 256 threads
+__device__ void bbox_reduce_block(double mnx, double mny, double mxx, double mxy, double *__restrict__ out) {
   __shared__ double sh[4][256];
   sh[0][threadIdx.x] = mnx; sh[1][threadIdx.x] = mny; sh[2][threadIdx.x] = mxx; sh[3][threadIdx.x] = mxy;
   __syncthreads();
@@ -105,6 +66,53 @@ __device__ void bbox_union_block(const double *__restrict__ bbox, int n_scans, d
     __syncthreads();
   }
   if (threadIdx.x == 0) { out[0] = sh[0][0]; out[1] = sh[1][0]; out[2] = sh[2][0]; out[3] = sh[3][0]; }
+}
+
+// per-scan bounding box over the sensor position and the FILTERED point readings
+// (InRange(reading, minRange, rangeThreshold), Karto.h:5382,5400,5418-5424).  One block of 256 threads per scan.
+template <class R>
+__global__ void k_scan_bbox(const R *__restrict__ ranges, const int32_t *__restrict__ rows,
+                            const double *__restrict__ sensor, const double *__restrict__ pts, b2s_laser l,
+                            double *__restrict__ bbox) {
+  const int s = blockIdx.x, n = l.n_readings;
+  const R *r = ranges + (rows ? (size_t)rows[s] : (size_t)s) * n;
+  const double *p = pts + (size_t)s * n * 2;
+  const double big = 999999999999999999.99999;  // Karto.h:2765
+  double mnx = big, mny = big, mxx = -big, mxy = -big;
+  if (threadIdx.x == 0) {
+    double x = sensor[3 * s], y = sensor[3 * s + 1];
+    if (x < mnx) mnx = x;
+    if (y < mny) mny = y;
+    if (x > mxx) mxx = x;
+    if (y > mxy) mxy = y;
+  }
+  for (int i = threadIdx.x; i < n; i += blockDim.x) {
+    double rr = (double)r[i];
+    if (!(rr >= l.min_range && rr <= l.range_threshold)) continue;
+    double x = p[(size_t)i * 2], y = p[(size_t)i * 2 + 1];
+    if (x < mnx) mnx = x;
+    if (y < mny) mny = y;
+    if (x > mxx) mxx = x;
+    if (y > mxy) mxy = y;
+  }
+  bbox_reduce_block(mnx, mny, mxx, mxy, bbox + 4 * s);
+}
+
+// union of each grid's scan boxes (OccupancyGrid::ComputeDimensions, Karto.h:5810-5814); one block of 256 threads per
+// grid
+__global__ void k_bbox_union(const double *__restrict__ bbox, const OccGridDev *__restrict__ grids,
+                             double *__restrict__ out) {
+  const int g = blockIdx.x, first = grids[g].first, scans = grids[g].scans;
+  const double big = 999999999999999999.99999;
+  double mnx = big, mny = big, mxx = -big, mxy = -big;
+  for (int k = threadIdx.x; k < scans; k += blockDim.x) {
+    const double *b = bbox + 4 * ((size_t)first + k);
+    mnx = fmin(mnx, fmin(b[0], b[2]));  // Add(min); Add(max) (Karto.h:2824-2828)
+    mny = fmin(mny, fmin(b[1], b[3]));
+    mxx = fmax(mxx, fmax(b[0], b[2]));
+    mxy = fmax(mxy, fmax(b[1], b[3]));
+  }
+  bbox_reduce_block(mnx, mny, mxx, mxy, out + 4 * g);
 }
 
 // OccupancyGrid::AddScan + RayTrace + Grid::TraceLine (Karto.h:5852-5945, 4680-4745) for ONE beam, by one warp: the
@@ -124,7 +132,13 @@ __device__ __forceinline__ unsigned long long trace_beam(double rr, double sx, d
   }
   int x0 = world_to_grid_1(sx, off_x, scale), y0 = world_to_grid_1(sy, off_y, scale);
   int x1 = world_to_grid_1(px, off_x, scale), y1 = world_to_grid_1(py, off_y, scale);
-  const int tx = x1, ty = y1;
+  // the end cell (Karto.h:5924-5942), counted before the walk so that its coordinates hold no register during it (the
+  // counters are sums: the order does not matter)
+  if (lane == 0 && end_valid && x1 >= 0 && x1 < w && y1 >= 0 && y1 < h) {
+    atomicAdd(pass + x1 + (size_t)y1 * step, 1u);
+    atomicAdd(hit + x1 + (size_t)y1 * step, 1u);
+    visits += 2;
+  }
   // TraceLine canonicalisation (Karto.h:4682-4692)
   const bool steep = abs(y1 - y0) > abs(x1 - x0);
   if (steep) { int t = x0; x0 = y0; y0 = t; t = x1; x1 = y1; y1 = t; }
@@ -141,13 +155,51 @@ __device__ __forceinline__ unsigned long long trace_beam(double rr, double sx, d
       visits++;
     }
   }
-  if (lane == 0 && end_valid && tx >= 0 && tx < w && ty >= 0 && ty < h) {  // Karto.h:5924-5942
-    atomicAdd(pass + tx + (size_t)ty * step, 1u);
-    atomicAdd(hit + tx + (size_t)ty * step, 1u);
-    visits += 2;
-  }
   return visits;
 }
+
+// the warp's visit counts added to *to by lane 0: one atomic per warp
+__device__ __forceinline__ void add_warp_visits(unsigned long long v, int lane, unsigned long long *__restrict__ to) {
+#pragma unroll
+  for (int d = 16; d > 0; d >>= 1) v += __shfl_xor_sync(0xffffffffu, v, d);
+  if (lane == 0 && v) atomicAdd(to, v);
+}
+
+// every beam of every scan of every grid, one warp per beam.  A lane sums its cell visits in a register; the warp adds
+// them to visits[g] when its next beam belongs to another grid, and once at the end, so a build of one grid costs one
+// atomic per warp.  48 registers, no spills (-Xptxas -v): 5 CTAs per SM.
+template <class R>
+__global__ void __launch_bounds__(256, 5)
+    k_raytrace(const R *__restrict__ ranges, const int32_t *__restrict__ rows, const int32_t *__restrict__ scan_grid,
+               const double *__restrict__ sensor, const double *__restrict__ pts, b2s_laser l, long long n_beams,
+               const OccGridDev *__restrict__ grids, uint32_t *__restrict__ pass, uint32_t *__restrict__ hit,
+               unsigned long long *__restrict__ visits) {
+  const int lane = threadIdx.x & 31;
+  const long long warp0 = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+  const int nwarps = (gridDim.x * blockDim.x) >> 5;
+  const int n = l.n_readings;
+  int g = -1;  // warp-uniform
+  OccGridDev G{};
+  unsigned long long my_visits = 0;
+  for (long long beam = warp0; beam < n_beams; beam += nwarps) {
+    const int s = (int)(beam / n), i = (int)(beam - (long long)s * n);
+    const int gs = scan_grid ? scan_grid[s] : 0;
+    if (gs != g) {
+      if (g >= 0) add_warp_visits(my_visits, lane, visits + g);
+      my_visits = 0;
+      g = gs;
+      G = grids[g];
+    }
+    if (G.w <= 0 || G.h <= 0) continue;
+    const size_t row = rows ? (size_t)rows[s] : (size_t)s;
+    my_visits += trace_beam((double)ranges[row * n + i], sensor[3 * s], sensor[3 * s + 1], pts[beam * 2],
+                            pts[beam * 2 + 1], l, G.w, G.h, G.step, G.off_x, G.off_y, G.scale, lane, pass + G.counters,
+                            hit + G.counters);
+  }
+  if (g >= 0) add_warp_visits(my_visits, lane, visits + g);
+}
+
+// ---- thresholds and ROS payloads
 
 // OccupancyGrid::UpdateCell (Karto.h:5970-5990): MinPassThrough = 2, OccupancyThreshold = 0.1
 __device__ __forceinline__ uint8_t occ_cell_value(uint32_t p, uint32_t h) {
@@ -161,40 +213,6 @@ __device__ __forceinline__ uint8_t occ_cell_value(uint32_t p, uint32_t h) {
 
 // SlamKarto::updateMap payload (karto_slam.cc:546-569): unknown -> -1, occupied -> 100, free -> 0
 __device__ __forceinline__ int8_t occ_ros_value(uint8_t v) { return v == 0 ? -1 : (v == GRID_OCCUPIED ? 100 : 0); }
-
-// ---- the single-grid kernels (b2s_occ_grid_*)
-
-// One block per scan.
-__global__ void k_scan_bbox(const double *__restrict__ ranges, const double *__restrict__ sensor,
-                            const double *__restrict__ pts, b2s_laser l, double *__restrict__ bbox) {
-  const int s = blockIdx.x, n = l.n_readings;
-  scan_bbox_block(ranges + (size_t)s * n, sensor + 3 * s, pts + (size_t)s * n * 2, l, bbox + 4 * s);
-}
-
-// single block
-__global__ void k_bbox_union(const double *__restrict__ bbox, int n_scans, double *__restrict__ out) {
-  bbox_union_block(bbox, n_scans, out);
-}
-
-// One warp per beam.
-__global__ void __launch_bounds__(256)
-    k_raytrace(const double *__restrict__ ranges, const double *__restrict__ sensor, const double *__restrict__ pts,
-               b2s_laser l, long long n_beams, int w, int h, int step, double off_x, double off_y, double scale,
-               uint32_t *__restrict__ pass, uint32_t *__restrict__ hit, unsigned long long *__restrict__ visits) {
-  const int lane = threadIdx.x & 31;
-  const long long warp0 = ((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
-  const long long nwarps = ((long long)gridDim.x * blockDim.x) >> 5;
-  const int n = l.n_readings;
-  unsigned long long my_visits = 0;
-  for (long long beam = warp0; beam < n_beams; beam += nwarps) {
-    const int s = (int)(beam / n);
-    my_visits += trace_beam(ranges[beam], sensor[3 * s], sensor[3 * s + 1], pts[beam * 2], pts[beam * 2 + 1], l, w, h,
-                            step, off_x, off_y, scale, lane, pass, hit);
-  }
-#pragma unroll
-  for (int d = 16; d > 0; d >>= 1) my_visits += __shfl_xor_sync(0xffffffffu, my_visits, d);
-  if (lane == 0 && my_visits) atomicAdd(visits, my_visits);
-}
 
 // OccupancyGrid::Update (Karto.h:5953-5968)
 __global__ void k_occ_threshold(const uint32_t *__restrict__ pass, const uint32_t *__restrict__ hit, int n,
@@ -210,56 +228,6 @@ __global__ void k_occ_ros(const uint8_t *__restrict__ cells, int w, int h, int s
   if (i >= w * h) return;
   const int x = i % w, y = i / w;
   out[i] = occ_ros_value(cells[x + (size_t)y * step]);
-}
-
-// ---- the batched build: G grids, each CreateFromScans over its own scans, every stage one launch for all grids.
-// Scans are numbered over all grids (grid 0's first); their readings are rows of a float32 pool.
-
-struct OccGridDev {     // one grid of a batched build, as its kernels read it
-  int w, h, step, scans;  // scans: the grid's scan count
-  double off_x, off_y, scale;
-  long long counters;   // first counter of the grid in the pass / hit arena
-  long long payload;    // first byte of its payload in the payload arena
-};
-
-// per-scan boxes; one block per scan, blockIdx.x = the scan's number over all grids
-__global__ void k_scan_bbox_rows(const float *__restrict__ pool, const int32_t *__restrict__ rows,
-                                 const double *__restrict__ sensor, const double *__restrict__ pts, b2s_laser l,
-                                 double *__restrict__ bbox) {
-  const int s = blockIdx.x, n = l.n_readings;
-  scan_bbox_block(pool + (size_t)rows[s] * n, sensor + 3 * s, pts + (size_t)s * n * 2, l, bbox + 4 * s);
-}
-
-// per-grid union; one block per grid, first[g] = the grid's first scan
-__global__ void k_bbox_union_grids(const double *__restrict__ bbox, const int32_t *__restrict__ first,
-                                   const int32_t *__restrict__ count, double *__restrict__ out) {
-  const int g = blockIdx.x;
-  bbox_union_block(bbox + 4 * (size_t)first[g], count[g], out + 4 * g);
-}
-
-// every beam of every scan of every grid, one warp per beam; scan_grid[s] = the grid scan s belongs to
-__global__ void __launch_bounds__(256)
-    k_raytrace_grids(const float *__restrict__ pool, const int32_t *__restrict__ rows,
-                     const int32_t *__restrict__ scan_grid, const double *__restrict__ sensor,
-                     const double *__restrict__ pts, b2s_laser l, long long n_beams,
-                     const OccGridDev *__restrict__ grids, uint32_t *__restrict__ pass, uint32_t *__restrict__ hit,
-                     unsigned long long *__restrict__ visits) {
-  const int lane = threadIdx.x & 31;
-  const long long warp0 = ((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
-  const long long nwarps = ((long long)gridDim.x * blockDim.x) >> 5;
-  const int n = l.n_readings;
-  for (long long beam = warp0; beam < n_beams; beam += nwarps) {
-    const int s = (int)(beam / n), i = (int)(beam - (long long)s * n);
-    const int g = scan_grid[s];
-    const OccGridDev G = grids[g];
-    if (G.w <= 0 || G.h <= 0) continue;
-    unsigned long long v = trace_beam((double)pool[(size_t)rows[s] * n + i], sensor[3 * s], sensor[3 * s + 1],
-                                      pts[beam * 2], pts[beam * 2 + 1], l, G.w, G.h, G.step, G.off_x, G.off_y,
-                                      G.scale, lane, pass + G.counters, hit + G.counters);
-#pragma unroll
-    for (int d = 16; d > 0; d >>= 1) v += __shfl_xor_sync(0xffffffffu, v, d);
-    if (lane == 0 && v) atomicAdd(visits + g, v);
-  }
 }
 
 // thresholds and ROS payload of every grid: grids blockIdx.y, + gridDim.y, ... (grid_rows(n_grids) rows), x-blocks
@@ -327,22 +295,28 @@ static b2s_status occ_create_impl(const b2s_laser *laser, int n_scans, const dou
   for (auto &e : ev) B2S_CUDA_CHECK(e.create());
   AsyncBuf<double> d_ranges(st), d_poses(st), d_sensor(st), d_pts(st), d_bbox(st);
   AsyncBuf<unsigned long long> d_visits(st);
+  AsyncBuf<OccGridDev> d_grid(st);
   B2S_CUDA_CHECK(d_ranges.alloc(std::max<size_t>(M * n, 1)));
   B2S_CUDA_CHECK(d_poses.alloc(std::max<size_t>(M * 3, 1)));
   B2S_CUDA_CHECK(d_sensor.alloc(std::max<size_t>(M * 3, 1)));
   B2S_CUDA_CHECK(d_pts.alloc(std::max<size_t>(M * n * 2, 1)));
   B2S_CUDA_CHECK(d_bbox.alloc((M + 1) * 4));
   B2S_CUDA_CHECK(d_visits.alloc(1));
+  B2S_CUDA_CHECK(d_grid.alloc(1));
   if (n && M) B2S_CUDA_CHECK(cudaMemcpyAsync(d_ranges, ranges, sizeof(double) * M * n, cudaMemcpyHostToDevice, st));
   if (M) B2S_CUDA_CHECK(cudaMemcpyAsync(d_poses, poses, sizeof(double) * M * 3, cudaMemcpyHostToDevice, st));
   B2S_CUDA_CHECK(cudaMemsetAsync(d_visits, 0, sizeof(unsigned long long), st));
+  // a build of one grid: scan s is row s of d_ranges, counters and payload start at 0
+  OccGridDev D{};
+  D.scans = n_scans;
   double bb[4];
   if (M) k_scan_points<<<(unsigned)M, 256, 0, st>>>(d_ranges, d_poses, *laser, d_sensor, d_pts, nullptr, nullptr);
   if (given_bbox) {
     for (int i = 0; i < 4; i++) bb[i] = given_bbox[i];
   } else {
-    k_scan_bbox<<<(unsigned)M, 256, 0, st>>>(d_ranges, d_sensor, d_pts, *laser, d_bbox);
-    k_bbox_union<<<1, 256, 0, st>>>(d_bbox, n_scans, d_bbox + 4 * M);
+    B2S_CUDA_CHECK(cudaMemcpyAsync(d_grid, &D, sizeof(D), cudaMemcpyHostToDevice, st));
+    k_scan_bbox<<<(unsigned)M, 256, 0, st>>>((const double *)d_ranges, nullptr, d_sensor, d_pts, *laser, d_bbox);
+    k_bbox_union<<<1, 256, 0, st>>>(d_bbox, d_grid, d_bbox + 4 * M);
     B2S_CUDA_CHECK(cudaGetLastError());
     B2S_CUDA_CHECK(cudaMemcpyAsync(bb, d_bbox + 4 * M, sizeof(bb), cudaMemcpyDeviceToHost, st));
     B2S_CUDA_CHECK(cudaStreamSynchronize(st));
@@ -351,9 +325,11 @@ static b2s_status occ_create_impl(const b2s_laser *laser, int n_scans, const dou
     for (int i = 0; i < 4; i++) bbox_out[i] = bb[i];
     return B2S_OK;
   }
-  const double scale = 1.0 / resolution;
   b2s_occ_grid_info &I = g->info;
   if (b2s_status s = occ_dims(bb, resolution, I)) return s;
+  D.w = I.width; D.h = I.height; D.step = I.width_step;
+  D.off_x = I.offset[0]; D.off_y = I.offset[1]; D.scale = 1.0 / resolution;
+  B2S_CUDA_CHECK(cudaMemcpyAsync(d_grid, &D, sizeof(D), cudaMemcpyHostToDevice, st));
   const size_t cells = (size_t)std::max(I.data_size, 1);
   B2S_CUDA_CHECK(g->d_pass.reserve(cells));
   B2S_CUDA_CHECK(g->d_hit.reserve(cells));
@@ -368,8 +344,8 @@ static b2s_status occ_create_impl(const b2s_laser *laser, int n_scans, const dou
     // to a band in closed form — was built and measured slower (not re-measured on the H100): shared-memory atomics
     // retire no faster than the L2 atomic units, and one 200 KB tile per SM leaves few warps to hide their latency.)
     const int blocks = (int)std::min<long long>((n_beams + 7) / 8, (long long)sms * 16);
-    k_raytrace<<<blocks, 256, 0, st>>>(d_ranges, d_sensor, d_pts, *laser, n_beams, I.width, I.height, I.width_step,
-                                       I.offset[0], I.offset[1], scale, g->d_pass, g->d_hit, d_visits);
+    k_raytrace<<<blocks, 256, 0, st>>>((const double *)d_ranges, nullptr, nullptr, d_sensor, d_pts, *laser, n_beams,
+                                       d_grid, g->d_pass, g->d_hit, d_visits);
   }
   B2S_CUDA_CHECK(cudaEventRecord(ev[1], st));
   if (I.data_size > 0) k_occ_threshold<<<ceil_div(I.data_size, 256), 256, 0, st>>>(g->d_pass, g->d_hit, I.data_size, g->d_cells);
@@ -511,13 +487,13 @@ struct OccBatch {
   Buf<float> d_pool;                 // [pool_rows][n_readings] readings, each uploaded once
   size_t pool_rows = 0;
   HostBuf<float> h_stage;            // page-locked staging of appended rows
-  Buf<int32_t> d_rows, d_first, d_count, d_scan_grid;
+  Buf<int32_t> d_rows, d_scan_grid;
   Buf<double> d_poses, d_sensor, d_pts, d_bbox, d_union;
   Buf<OccGridDev> d_grids;
   Buf<uint32_t> d_pass, d_hit;       // one arena of counters for every grid of a build
   Buf<unsigned long long> d_visits;
   Buf<int8_t> d_payload;
-  HostBuf<int32_t> h_i32;            // rows, first, count, scan_grid of a build
+  HostBuf<int32_t> h_i32;            // rows, scan_grid of a build
   HostBuf<double> h_f64;             // poses of a build; the unions read back
   HostBuf<OccGridDev> h_grids;
   HostBuf<unsigned long long> h_visits;
@@ -596,19 +572,26 @@ b2s_status occ_batch_build(OccBatch *b, int G, const int32_t *n_scans, const int
   for (int g = 0; g < G; g++)
     if (n_scans[g] > 0) live.push_back(g);
   const int L = (int)live.size();
-  B2S_CUDA_CHECK(b->h_i32.reserve(2 * M + 2 * (size_t)L));
+  B2S_CUDA_CHECK(b->h_i32.reserve(2 * M));
   B2S_CUDA_CHECK(b->h_f64.reserve(std::max<size_t>(3 * M, 4 * (size_t)L)));
-  int32_t *h_rows = b->h_i32, *h_grid = h_rows + M, *h_first = h_grid + M, *h_count = h_first + L;
+  B2S_CUDA_CHECK(b->d_grids.reserve((size_t)L));
+  B2S_CUDA_CHECK(b->h_grids.reserve((size_t)L));
+  int32_t *h_rows = b->h_i32, *h_grid = h_rows + M;
+  b->grids.assign((size_t)L, OccGridDev{});
   {
     size_t s = 0;
     for (int j = 0; j < L; j++) {
       const int g = live[(size_t)j];
-      h_first[j] = (int32_t)s;
-      h_count[j] = n_scans[g];
+      b->grids[(size_t)j].first = (int)s;
+      b->grids[(size_t)j].scans = n_scans[g];
       for (int k = 0; k < n_scans[g]; k++) h_grid[s + k] = j;
       s += (size_t)n_scans[g];
     }
   }
+  auto upload_grids = [&] {
+    std::memcpy(b->h_grids, b->grids.data(), sizeof(OccGridDev) * L);
+    return cudaMemcpyAsync(b->d_grids, b->h_grids, sizeof(OccGridDev) * L, cudaMemcpyHostToDevice, st);
+  };
   {
     size_t s = 0;
     for (int g = 0, src = 0; g < G; g++) {
@@ -625,8 +608,6 @@ b2s_status occ_batch_build(OccBatch *b, int G, const int32_t *n_scans, const int
     if (h_rows[s] < 0 || (size_t)h_rows[s] >= b->pool_rows) B2S_FAIL(B2S_ERR_OUT_OF_RANGE, "occupancy grid pool row out of range");
   B2S_CUDA_CHECK(b->d_rows.reserve(M));
   B2S_CUDA_CHECK(b->d_scan_grid.reserve(M));
-  B2S_CUDA_CHECK(b->d_first.reserve((size_t)L));
-  B2S_CUDA_CHECK(b->d_count.reserve((size_t)L));
   B2S_CUDA_CHECK(b->d_poses.reserve(3 * M));
   B2S_CUDA_CHECK(b->d_sensor.reserve(3 * M));
   B2S_CUDA_CHECK(b->d_pts.reserve(M * std::max<size_t>(n, 1) * 2));
@@ -634,25 +615,23 @@ b2s_status occ_batch_build(OccBatch *b, int G, const int32_t *n_scans, const int
   B2S_CUDA_CHECK(b->d_union.reserve(4 * (size_t)L));
   B2S_CUDA_CHECK(cudaMemcpyAsync(b->d_rows, h_rows, sizeof(int32_t) * M, cudaMemcpyHostToDevice, st));
   B2S_CUDA_CHECK(cudaMemcpyAsync(b->d_scan_grid, h_grid, sizeof(int32_t) * M, cudaMemcpyHostToDevice, st));
-  B2S_CUDA_CHECK(cudaMemcpyAsync(b->d_first, h_first, sizeof(int32_t) * L, cudaMemcpyHostToDevice, st));
-  B2S_CUDA_CHECK(cudaMemcpyAsync(b->d_count, h_count, sizeof(int32_t) * L, cudaMemcpyHostToDevice, st));
+  B2S_CUDA_CHECK(upload_grids());
   B2S_CUDA_CHECK(cudaMemcpyAsync(b->d_poses, b->h_f64, sizeof(double) * 3 * M, cudaMemcpyHostToDevice, st));
   // points, per-scan boxes, per-grid unions, then the unions back to size the grids on the host
   k_scan_points<<<(unsigned)M, 256, 0, st>>>((const float *)b->d_pool, (const double *)b->d_poses, l, b->d_sensor.p,
                                              b->d_pts.p, nullptr, (const int32_t *)b->d_rows);
-  k_scan_bbox_rows<<<(unsigned)M, 256, 0, st>>>(b->d_pool, b->d_rows, b->d_sensor, b->d_pts, l, b->d_bbox);
-  k_bbox_union_grids<<<(unsigned)L, 256, 0, st>>>(b->d_bbox, b->d_first, b->d_count, b->d_union);
+  k_scan_bbox<<<(unsigned)M, 256, 0, st>>>((const float *)b->d_pool, b->d_rows, b->d_sensor, b->d_pts, l, b->d_bbox);
+  k_bbox_union<<<(unsigned)L, 256, 0, st>>>(b->d_bbox, b->d_grids, b->d_union);
   B2S_CUDA_CHECK(cudaGetLastError());
   B2S_CUDA_CHECK(cudaMemcpyAsync(b->h_f64, b->d_union, sizeof(double) * 4 * L, cudaMemcpyDeviceToHost, st));
   B2S_CUDA_CHECK(cudaStreamSynchronize(st));
   b->bytes_d2h += sizeof(double) * 4.0 * L;
-  b->grids.resize((size_t)L);
   long long counters = 0, bytes = 0;
   for (int j = 0; j < L; j++) {
     const int g = live[(size_t)j];
     if (b2s_status s = occ_dims((const double *)b->h_f64 + 4 * j, resolution[g], info[g])) return s;
     OccGridDev &D = b->grids[(size_t)j];
-    D.w = info[g].width; D.h = info[g].height; D.step = info[g].width_step; D.scans = n_scans[g];
+    D.w = info[g].width; D.h = info[g].height; D.step = info[g].width_step;
     D.off_x = info[g].offset[0]; D.off_y = info[g].offset[1]; D.scale = 1.0 / resolution[g];
     D.counters = counters;
     D.payload = bytes;
@@ -662,13 +641,10 @@ b2s_status occ_batch_build(OccBatch *b, int G, const int32_t *n_scans, const int
   B2S_CUDA_CHECK(b->d_pass.reserve((size_t)counters));
   B2S_CUDA_CHECK(b->d_hit.reserve((size_t)counters));
   B2S_CUDA_CHECK(b->d_visits.reserve((size_t)L));
-  B2S_CUDA_CHECK(b->d_grids.reserve((size_t)L));
-  B2S_CUDA_CHECK(b->h_grids.reserve((size_t)L));
   B2S_CUDA_CHECK(b->d_payload.reserve((size_t)bytes));
   B2S_CUDA_CHECK(b->h_payload.reserve((size_t)bytes));
   B2S_CUDA_CHECK(b->h_visits.reserve((size_t)L));
-  std::memcpy(b->h_grids, b->grids.data(), sizeof(OccGridDev) * L);
-  B2S_CUDA_CHECK(cudaMemcpyAsync(b->d_grids, b->h_grids, sizeof(OccGridDev) * L, cudaMemcpyHostToDevice, st));
+  B2S_CUDA_CHECK(upload_grids());
   if (counters) {
     B2S_CUDA_CHECK(cudaMemsetAsync(b->d_pass, 0, sizeof(uint32_t) * counters, st));
     B2S_CUDA_CHECK(cudaMemsetAsync(b->d_hit, 0, sizeof(uint32_t) * counters, st));
@@ -677,8 +653,8 @@ b2s_status occ_batch_build(OccBatch *b, int G, const int32_t *n_scans, const int
   const long long n_beams = (long long)M * (long long)n;
   if (n_beams && counters) {
     const int blocks = (int)std::min<long long>((n_beams + 7) / 8, (long long)sm_count(b->device) * 16);
-    k_raytrace_grids<<<blocks, 256, 0, st>>>(b->d_pool, b->d_rows, b->d_scan_grid, b->d_sensor, b->d_pts, l, n_beams,
-                                             b->d_grids, b->d_pass, b->d_hit, b->d_visits);
+    k_raytrace<<<blocks, 256, 0, st>>>((const float *)b->d_pool, b->d_rows, b->d_scan_grid, b->d_sensor, b->d_pts, l,
+                                       n_beams, b->d_grids, b->d_pass, b->d_hit, b->d_visits);
   }
   if (bytes) {
     long long most = 0;

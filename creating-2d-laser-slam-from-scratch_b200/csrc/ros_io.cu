@@ -9,6 +9,7 @@
 
 #include "common.cuh"
 #include "hector_scan.cuh"
+#include "karto_internal.cuh"
 
 using namespace b2s;
 

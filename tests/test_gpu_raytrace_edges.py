@@ -5,6 +5,8 @@ and up to 4000 cells, rounding ties, every range-filter edge, grids smaller than
 widths, far offsets, crafted counters for the threshold, storage maps narrower, as wide as and one column wider than
 the published map, out-of-map beams and growing scan buffers.  The restatement (oracle/port.py) is compared too
 wherever it can express the case."""
+import dataclasses
+
 import numpy as np
 import pytest
 
@@ -52,6 +54,37 @@ def test_karto_grid_equals_brute_force(O, name):
     if c.bbox is None:
         karto_same(a, port.occupancy_grid(c.laser, c.ranges, c.poses, c.resolution))
     g.close()
+
+
+def test_karto_batched_build_equals_single_grid(O):
+    """the cases with CreateFromScans' own box through the batched build, which takes one laser per build and float32
+    readings: each case's readings rounded to float32 (its traced end points still off half cells), one build per laser
+    holding each of its cases twice, so that on the 16384-beam laser a warp's stride crosses from one grid to the next.
+    Every grid's info and payload equal the single-grid handle's and the brute force's on the same readings."""
+    groups = {}
+    for name, c in KARTO.items():
+        if c.bbox is None:
+            key = tuple(getattr(c.laser, f) for f, _ in c.laser._fields_ if f != "offset_pose") + tuple(c.laser.offset_pose)
+            groups.setdefault(key, []).append(dataclasses.replace(c, ranges=c.ranges.astype(np.float32).astype(np.float64)))
+    assert sum(map(len, groups.values())) == len([c for c in KARTO.values() if c.bbox is None]) and len(groups) > 1
+    for cases in groups.values():
+        for c in cases:
+            assert rc.karto_end_margins(c) >= rc.HALF_CELL_MARGIN
+        twice = cases + cases
+        out = O.create_from_scans_batch(cases[0].laser, [c.ranges for c in twice], [c.poses for c in twice],
+                                        [c.resolution for c in twice])
+        for k, c in enumerate(cases):
+            g = O.OccupancyGrid(c.laser, c.ranges, c.poses, c.resolution)
+            a = g.arrays()
+            b = rr.occupancy_grid(c.laser, c.ranges, c.poses, c.resolution)
+            karto_same(a, b)
+            want = rr.karto_ros_map(b["cells"], b["width"], b["height"])
+            assert np.array_equal(g.ros_map(), want)
+            for info, payload in (out[k], out[k + len(cases)]):
+                assert (info["width"], info["height"], info["width_step"]) == (a["width"], a["height"], a["width_step"])
+                assert np.array_equal(info["offset"], a["offset"]) and info["cell_visits"] == a["cell_visits"]
+                assert np.array_equal(payload, want)
+            g.close()
 
 
 def test_karto_threshold_on_crafted_counters(O):
