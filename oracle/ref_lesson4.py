@@ -90,6 +90,10 @@ def hector(params: dict, fields, ranges) -> np.ndarray:
         buf = np.zeros(1 << 24, np.int8) if out is None else out[s]
         rc = L.ref_l4_hector_scan(f.ctypes.data, r.shape[1], r[s].ctypes.data, info.ctypes.data, buf.ctypes.data,
                                   buf.size)
+        if rc == -3 and out is None:  # a map larger than the first buffer: its size is known now, and a scan's map is
+            buf = np.zeros(int(info[0]) * int(info[1]), np.int8)  # fresh, so the scan can run again
+            rc = L.ref_l4_hector_scan(f.ctypes.data, r.shape[1], r[s].ctypes.data, info.ctypes.data, buf.ctypes.data,
+                                      buf.size)
         assert rc == 0, f"the Hector node published nothing for scan {s} ({rc})"
         if out is None:
             out = np.zeros((len(r), info[1], info[0]), np.int8)
