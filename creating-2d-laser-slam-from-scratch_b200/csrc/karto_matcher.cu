@@ -160,6 +160,7 @@ struct b2s_matcher {
   Buf<uint8_t> d_keep;                  // [B][nA] angles a pruned sweep swept
   SweepPlan last_plan;                  // of the last sweep
   bool last_pruned = false;             // the last sweep skipped angles: get_response_sums sweeps them first
+  int last_batch = 0;                   // matches of the last sweep
   double last_pruned_frac = 0.0;
   bool pending = false;                   // a correlate_scan_begin awaits its _end
   int pending_batch = 0;                  // batch size that _begin enqueued
@@ -2988,6 +2989,36 @@ b2s_status b2s_matcher_last_pruned_frac(b2s_matcher *m, double *out) {
   return B2S_OK;
 }
 
+b2s_status b2s_matcher_last_prune_state(b2s_matcher *m, int32_t dims[2], double *ubr, double *gub, uint8_t *swept,
+                                        double *cut) {
+  if (!m || !dims) B2S_FAIL(B2S_ERR_BAD_PARAMS, "null argument");
+  if (b2s_status st = refuse_if_pending(m)) return st;
+  if (!m->have_sweep || !m->last_pruned)
+    B2S_FAIL(B2S_ERR_BAD_STATE, "the last sweep was not pruned, its angles were swept since, or its inputs were replaced");
+  const int B = m->last_batch, na = m->last.na, ng = ceil_div(na, BOUND_GROUP);
+  const bool arrays = ubr || gub || swept || cut;
+  const bool fits = dims[0] == B && dims[1] == na;
+  dims[0] = B;
+  dims[1] = na;
+  if (!arrays) return B2S_OK;
+  if (!fits) B2S_FAIL(B2S_ERR_BAD_PARAMS, "the arrays are not sized for the last sweep's matches and angles");
+  B2S_CUDA_CHECK(cudaSetDevice(m->device));
+  std::vector<int32_t> flags((size_t)B);
+  B2S_CUDA_CHECK(cudaMemcpyAsync(flags.data(), m->d_flags, sizeof(int32_t) * B, cudaMemcpyDeviceToHost, m->stream));
+  if (ubr) B2S_CUDA_CHECK(cudaMemcpyAsync(ubr, m->d_ubr, sizeof(double) * B * na, cudaMemcpyDeviceToHost, m->stream));
+  if (gub) B2S_CUDA_CHECK(cudaMemcpyAsync(gub, m->d_gub, sizeof(double) * B * ng, cudaMemcpyDeviceToHost, m->stream));
+  if (swept) B2S_CUDA_CHECK(cudaMemcpyAsync(swept, m->d_keep, (size_t)B * na, cudaMemcpyDeviceToHost, m->stream));
+  if (cut) B2S_CUDA_CHECK(cudaMemcpyAsync(cut, m->d_cuts, sizeof(double) * B, cudaMemcpyDeviceToHost, m->stream));
+  B2S_CUDA_CHECK(cudaStreamSynchronize(m->stream));
+  // a match the generic kernel swept was never bounded: its rows of d_ubr and d_cuts are an earlier call's
+  for (int b = 0; b < B; b++) {
+    if (!((flags[b] & 2) || !(flags[b] & 1))) continue;
+    if (ubr) std::fill(ubr + (size_t)b * na, ubr + (size_t)(b + 1) * na, (double)NAN);
+    if (cut) cut[b] = NAN;
+  }
+  return B2S_OK;
+}
+
 b2s_status b2s_matcher_last_timing(b2s_matcher *m, double out[4]) {
   if (!m || !out) B2S_FAIL(B2S_ERR_BAD_PARAMS, "null argument");
   if (m->have_sweep && !m->pending && cudaSetDevice(m->device) == cudaSuccess && cudaStreamSynchronize(m->stream) == cudaSuccess) {
@@ -3197,6 +3228,7 @@ static b2s_status run_correlate(b2s_matcher *m, const b2s_search *s, int k_first
   m->last.nx = nx; m->last.ny = ny; m->last.na = na;
   m->last_plan = pl;
   m->last_pruned = pl.prune && na > 0;
+  m->last_batch = B;
   m->last_search = *s;
   m->last_k_first = k_first;
   m->have_sweep = true;

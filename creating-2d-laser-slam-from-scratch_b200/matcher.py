@@ -61,6 +61,7 @@ def lib():
     L.b2s_matcher_last_timing.argtypes = [vp, dp]
     L.b2s_matcher_last_stats.argtypes = [vp, dp]
     L.b2s_matcher_last_pruned_frac.argtypes = [vp, dp]
+    L.b2s_matcher_last_prune_state.argtypes = [vp, ip, dp, dp, u8p, dp]
     L.b2s_matcher_sync.argtypes = [vp]
     L.b2s_matcher_set_kernel.argtypes = [vp, C.c_int]
     _lib = L
@@ -261,6 +262,20 @@ class ScanMatcher:
         out = np.zeros(1)
         check(self.L.b2s_matcher_last_pruned_frac(self.h, _d(out)))
         return float(out[0])
+
+    def last_prune_state(self):
+        """Angle-pruning state of the last sweep, which must have been pruned (b2s_matcher_last_prune_state):
+        dict(ubr [B, nA] (NaN: not bounded one by one), gub [B, ceil(nA / 4)], swept [B, nA] bool, cut [B]), sized
+        by the library."""
+        dims = np.zeros(2, dtype=np.int32)
+        i32 = C.POINTER(C.c_int32)
+        check(self.L.b2s_matcher_last_prune_state(self.h, dims.ctypes.data_as(i32), None, None, None, None))
+        B, na = int(dims[0]), int(dims[1])
+        ubr, gub = np.empty((B, na)), np.empty((B, (na + 3) // 4))
+        swept, cut = np.empty((B, na), dtype=np.uint8), np.empty(B)
+        check(self.L.b2s_matcher_last_prune_state(self.h, dims.ctypes.data_as(i32), _d(ubr), _d(gub),
+                                                  swept.ctypes.data_as(C.POINTER(C.c_uint8)), _d(cut)))
+        return dict(ubr=ubr, gub=gub, swept=swept.astype(bool), cut=cut)
 
     def sync(self):
         check(self.L.b2s_matcher_sync(self.h))

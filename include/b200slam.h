@@ -213,6 +213,20 @@ b2s_status b2s_matcher_last_stats(b2s_matcher *m, double out[4]);
 /* Fraction of the (match, angle) pairs of the LAST correlate_scan call that the window kernel never swept because an
  * upper bound of all their responses lies below best - 0.1 (results unchanged; 0 when the search was not pruned). */
 b2s_status b2s_matcher_last_pruned_frac(b2s_matcher *m, double *out);
+/* Angle-pruning state of the LAST sweep (tests): the last correlate_scan call, or the last stage of the last
+ * match_scan / match_scan_host / split call.  ubr [B][nA] (NaN where the angle was not bounded one by one),
+ * gub [B][ceil(nA / 4)], swept [B][nA] (1 = swept exactly), cut [B].  dims = {B, nA} the caller's arrays are sized
+ * for; on return it holds the last sweep's, and a call with every array null only reports them.  B2S_ERR_BAD_PARAMS
+ * (nothing written to the arrays) when they differ; B2S_ERR_BAD_STATE when that sweep was not pruned,
+ * b2s_matcher_get_response_sums has re-swept it since, or set_scans / add_scans / set_grids replaced its inputs.
+ * Null arrays are skipped.
+ * cut[b] = L - 0.1 - 1e-9, L the best exact response of the probed angles; when L - 0.1 <= 1e-6 every angle is swept
+ * and cut[b] still holds that value.  A match the generic kernel swept (an irregular candidate lattice, or no result)
+ * is not bounded: its ubr row and cut are NaN, its swept row all 1, and its gub row holds whatever the group pass
+ * left there (nothing it was compared with).  Without the group pass (SweepPlan::group) every gub is 0x7f7f... as
+ * a double (about 1.4e306): every group is bounded one angle at a time. */
+b2s_status b2s_matcher_last_prune_state(b2s_matcher *m, int32_t dims[2], double *ubr, double *gub, uint8_t *swept,
+                                        double *cut);
 b2s_status b2s_matcher_sync(b2s_matcher *m);
 /* 0 = automatic, 1 = force the generic global-memory gather kernel, 2 = force the shared-memory window kernel,
  * 3 = window kernel over every beam and every angle (no empty-window dropping, no angle pruning) */
