@@ -49,9 +49,51 @@ def stamps_at(t0_sec, t0_nsec, dt_ns, n, gaps=()):
     return np.array(out, np.uint32)
 
 
-def walk(seed, n, step_xy=0.05, step_th_deg=2.0):
-    _, _, ranges = synth.make_trajectory(seed, n, LASER, step_xy=step_xy, step_th_deg=step_th_deg)
+def walk(seed, n, step_xy=0.05, step_th_deg=2.0, laser=LASER, room=(8.0, 6.0)):
+    _, _, ranges = synth.make_trajectory(seed, n, laser, room[0], room[1], step_xy=step_xy, step_th_deg=step_th_deg)
     return ranges.astype(np.float32)
+
+
+def laser(beams, angle_min, angle_increment, range_min=0.1, range_max=30.0):
+    """A synth laser of `beams` beams from angle_min (radians, float32 message fields) and its LaserScan geometry."""
+    amin, inc = f32(angle_min), f32(angle_increment)
+    las = synth.Laser(n_readings=beams, min_angle=float(amin), max_angle=float(amin) + float(inc) * (beams - 1),
+                      angular_resolution=float(inc), min_range=range_min, max_range=range_max)
+    return las, (amin, inc, f32(range_min), f32(range_max))
+
+
+RING, RING_GEOMETRY = laser(360, -math.pi, 2 * math.pi / 360, 0.15, 12.0)
+DENSE, DENSE_GEOMETRY = laser(4096, -math.pi, 2 * math.pi / 4096, 0.1, 20.0)
+# the Hokuyo swept from +135 deg down: beam 0 on the left, a negative angle_increment
+CLOCKWISE, CLOCKWISE_GEOMETRY = laser(1081, -LASER.min_angle, -LASER.angular_resolution)
+BIG_ROOM = (14.0, 10.0)  # walls up to about 17 m from the walk
+FRONT = slice(520, 561)  # Hokuyo beams within 5 deg of straight ahead: x > 0, so the behind-the-robot rule keeps them
+
+
+def _band(seed, n, lo, hi, beams=FRONT, r=None, exact=()):
+    """A walk with the beams `beams` of every scan drawn from [lo, hi) (float32), and the values `exact` on the first
+    of them."""
+    r = walk(seed, n) if r is None else r
+    rng = np.random.default_rng(seed)
+    k = r[:, beams].shape[1]
+    r[:, beams] = rng.uniform(lo, hi, (len(r), k)).astype(np.float32)
+    np.clip(r[:, beams], f32(lo), np.nextafter(f32(hi), f32(0)), out=r[:, beams])
+    for j, v in enumerate(exact):
+        r[:, beams.start + j] = f32(v)
+    return r
+
+
+def _fields_lo(seed, n):
+    """range_min 0.05: readings in [0.05, 0.1) that the 0.1 of the other cases would drop, and [0.03, 0.05) below it."""
+    r = _band(seed, n, 0.05, 0.1, exact=(0.05, np.nextafter(f32(0.05), f32(0))))
+    return _band(seed + 1, n, 0.03, 0.05, beams=slice(561, 566), r=r)
+
+
+def _fields_40(seed, n):
+    """range_max 40: readings in [30, 40) (30 itself among them) that projectLaser's 30 m cutoff drops, and (20, 30)
+    that it keeps."""
+    r = _band(seed, n, 30.0, 40.0, exact=(30.0, np.nextafter(f32(30.0), f32(0))))
+    return _band(seed + 1, n, 20.0, 30.0, beams=slice(300, 330), r=r)
 
 
 def _bad(seed, n):
@@ -111,6 +153,55 @@ def cases():
                               stamps=stamps_at(10, 900_000_000, 25_000_000, 14, gaps=((4, 5_000_000_000),))),
         "short_period": dict(params=dict(SMALL, map_pub_period=0.01), mount=mount(), geometry=GEOMETRY,
                              ranges=walk(10, 8), stamps=stamps_at(1, 0, at40, 8)),
+        # ---- per-node map settings: each differs from every case above in the field it is named for ----
+        "start_asym": dict(params=dict(SMALL, map_start_x=0.3, map_start_y=0.7, map_pub_period=0.1,
+                                         map_update_distance_thresh=0.1, map_update_angle_thresh=0.1), mount=mount(),
+                           geometry=GEOMETRY, ranges=walk(12, 12, step_xy=0.3), stamps=stamps_at(4, 0, at40, 12)),
+        "start_asym_2": dict(params=dict(SMALL, map_start_x=0.65, map_start_y=0.35, map_pub_period=0.1,
+                                           map_update_distance_thresh=0.1, map_update_angle_thresh=0.1),
+                             mount=mount(0.08, 0.03, 0.2, yaw=-0.2), geometry=GEOMETRY,
+                             ranges=walk(30, 12, step_xy=0.3), stamps=stamps_at(4, 0, at40, 12)),
+        "res_0.1_levels_1": dict(params=dict(map_size=256, map_resolution=0.1, map_multi_res_levels=1,
+                                             map_pub_period=0.1), mount=mount(), geometry=GEOMETRY,
+                                 ranges=walk(14, 10), stamps=stamps_at(6, 0, at40, 10)),
+        "res_0.025_levels_4": dict(params=dict(map_size=512, map_resolution=0.025, map_multi_res_levels=4,
+                                               map_pub_period=0.1), mount=mount(), geometry=GEOMETRY,
+                                   ranges=walk(15, 10), stamps=stamps_at(6, 0, at40, 10)),
+        # 515 -> 257 -> 128 -> 64: the coarse levels drop a cell
+        "res_0.075_odd_size": dict(params=dict(map_size=515, map_resolution=0.075, map_multi_res_levels=4,
+                                               map_start_x=0.45, map_pub_period=0.1), mount=mount(),
+                                   geometry=GEOMETRY, ranges=walk(16, 10), stamps=stamps_at(6, 0, at40, 10)),
+        "factors": dict(params=dict(SMALL, update_factor_free=0.35, update_factor_occupied=0.7, map_pub_period=0.1),
+                        mount=mount(), geometry=GEOMETRY, ranges=walk(17, 10), stamps=stamps_at(6, 0, at40, 10)),
+        # ---- per-node lasers ----
+        "ring_360": dict(params=dict(SMALL, map_pub_period=0.1), mount=mount(), geometry=RING_GEOMETRY,
+                         ranges=walk(18, 10, laser=RING), stamps=stamps_at(8, 0, at40, 10)),
+        "clockwise": dict(params=dict(SMALL, map_pub_period=0.1), mount=mount(0.05, 0.0, 0.1, yaw=0.4),
+                          geometry=CLOCKWISE_GEOMETRY, ranges=walk(19, 10, laser=CLOCKWISE),
+                          stamps=stamps_at(8, 0, at40, 10)),
+        "dense_4096": dict(params=dict(SMALL, map_pub_period=0.1), mount=mount(), geometry=DENSE_GEOMETRY,
+                           ranges=walk(20, 6, laser=DENSE), stamps=stamps_at(8, 0, at40, 6)),
+        "fields_lo": dict(params=dict(SMALL, laser_min_dist=0.03, map_pub_period=0.1), mount=mount(),
+                          geometry=GEOMETRY[:2] + (f32(0.05), GEOMETRY[3]), ranges=_fields_lo(21, 10),
+                          stamps=stamps_at(8, 0, at40, 10)),
+        "min_dist_0.5": dict(params=dict(SMALL, laser_min_dist=0.5, map_pub_period=0.1), mount=mount(),
+                             geometry=GEOMETRY, ranges=_band(23, 10, 0.1, 0.5), stamps=stamps_at(8, 0, at40, 10)),
+        # range_max 10 in the message: projectLaser is asked for 30 m, so the walls past 10 m stay
+        "fields_hi": dict(params=dict(SMALL, use_max_scan_range=25.0, map_pub_period=0.1), mount=mount(),
+                          geometry=GEOMETRY[:3] + (f32(10.0),), ranges=walk(24, 10, laser=LASER, room=BIG_ROOM),
+                          stamps=stamps_at(8, 0, at40, 10)),
+        "fields_40": dict(params=dict(SMALL, use_max_scan_range=50.0, laser_max_dist=50.0, map_pub_period=0.1),
+                          mount=mount(), geometry=GEOMETRY[:3] + (f32(40.0),), ranges=_fields_40(25, 10),
+                          stamps=stamps_at(8, 0, at40, 10)),
+        "max_dist_8": dict(params=dict(SMALL, laser_max_dist=8.0, use_max_scan_range=12.0, map_pub_period=0.1),
+                           mount=mount(), geometry=GEOMETRY, ranges=walk(27, 10, room=BIG_ROOM),
+                           stamps=stamps_at(8, 0, at40, 10)),
+        "use_range_5": dict(params=dict(SMALL, use_max_scan_range=5.0, map_pub_period=0.1), mount=mount(),
+                            geometry=GEOMETRY, ranges=walk(28, 10), stamps=stamps_at(8, 0, at40, 10)),
+        # a new laser through the pitched mount's z window
+        "ring_pitched": dict(params=dict(SMALL, laser_z_min_value=-0.3, laser_z_max_value=0.3, map_pub_period=0.1),
+                             mount=mount(0.05, 0.0, 0.4, pitch=0.12, yaw=0.3), geometry=RING_GEOMETRY,
+                             ranges=walk(29, 10, laser=RING), stamps=stamps_at(8, 0, at40, 10)),
     }
 
 

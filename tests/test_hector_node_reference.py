@@ -37,7 +37,8 @@ def test_port_equals_node(request, name):
     c = CASES[name]
     live = ref_lesson4_slam.available()
     with recording(request, live) as rec:
-        want = rec.value("node", lambda: _node(c), inputs=(name, _params(c), c["mount"], c["ranges"], c["stamps"]))
+        want = rec.value("node", lambda: _node(c), inputs=(name, _params(c), c["geometry"], c["mount"], c["ranges"],
+                                                                   c["stamps"]))
     port = P.HectorNodePort(_params(c), c["geometry"], c["mount"])
     got = port.process(c["ranges"], c["stamps"])
     port.close()
